@@ -11,6 +11,7 @@
 #include <cmath>
 #include <mutex>
 #include <new>
+#include <type_traits>
 #include <vector>
 
 #include "isl_kernels.cuh"
@@ -18,6 +19,12 @@
 using namespace isl;
 
 static constexpr uint32_t kMaxStreamChunks = 4096;
+
+// What plan_pipeline decides for one k_pipeline launch: GPUs per stage (seg), stages, GPUs per sub-segment, speculative rounds.
+struct PipePlan {
+    uint32_t seg = 0, n_seg = 0, sub = 0;
+    bool spec = false;
+};
 
 struct isl_engine {
     isl_config cfg{};
@@ -94,8 +101,8 @@ struct isl_engine {
     // open stream (isl_stream_open / _submit / _wait / _close): one persistent k_pipeline, batches arrive while it runs
     struct Open {
         bool active = false, launched = false;
-        uint32_t max_batches = 0, submitted = 0, epoch = 0, seg = 0, n_seg = 0, sub = 0, q_stride = 0, free_stride = 0, tiles_per_batch = 0;
-        bool spec = false;
+        uint32_t max_batches = 0, submitted = 0, epoch = 0, q_stride = 0, free_stride = 0, tiles_per_batch = 0;
+        PipePlan plan;
         uint32_t* h_done = nullptr; uint32_t* d_done_host = nullptr; uint32_t cap_done = 0;   // mapped pinned: [batch] = epoch once its results are in host memory
         ChunkDesc* h_chunks = nullptr; TileDesc* h_tiles = nullptr; uint32_t cap_desc = 0;       // pinned staging of the per-batch descriptors
     } open;
@@ -155,6 +162,31 @@ int ensure_scratch(isl_engine* e, size_t bytes) {
     return ISL_OK;
 }
 
+// f(std::integral_constant<int, K>) with K = the candidate slots of the loaded tables (k_small<K>, k_chain<K>, k_pipeline<K, ..>)
+template <typename F>
+auto with_cand_slots(const isl_engine* e, F&& f) {
+    switch (e->n_cand_slots) {
+        case 1: return f(std::integral_constant<int, 1>{});
+        case 2: return f(std::integral_constant<int, 2>{});
+        default: return f(std::integral_constant<int, 4>{});
+    }
+}
+
+// The end of a path of one launch, or of k_prepare + one launch (with_prepare): under ISL_FLAG_TIMING ev[0] .. ev[1] are the frees and
+// ev[last - 1] .. ev[last] the commit; then the batch counters.
+void finish_batch(isl_engine* e, uint32_t n, bool with_prepare) {
+    if (e->cfg.flags & ISL_FLAG_TIMING) {
+        const uint32_t last = with_prepare ? 2 : 1;
+        cudaEventRecord(e->ev[last], e->stream);
+        cudaEventSynchronize(e->ev[last]);
+        float t;
+        if (with_prepare) { cudaEventElapsedTime(&t, e->ev[0], e->ev[1]); e->st.ms_free += t; }
+        cudaEventElapsedTime(&t, e->ev[last - 1], e->ev[last]); e->st.ms_commit += t;
+        cudaEventElapsedTime(&t, e->ev[0], e->ev[last]); e->st.ms_total += t;
+    }
+    ++e->st.batches; e->st.requests += n;
+}
+
 template <int K>
 int launch_chain(isl_engine* e, uint2* d_out_chunk, const uint32_t* d_heads_in, uint32_t* d_heads_out) {
     const size_t smem = (size_t)kQCap * sizeof(uint16_t);      // opted in per device by isl_create
@@ -176,22 +208,12 @@ int run_small(isl_engine* e, uint32_t n, const uint2* d_in, const SmallReqs* inl
     const SmallReqs& params = inl ? *inl : zero;
     const bool timing = e->cfg.flags & ISL_FLAG_TIMING;
     if (timing) cudaEventRecord(e->ev[0], e->stream);
-    switch (e->n_cand_slots) {
-        case 1: k_small<1><<<1, kSmallThreads, 0, e->stream>>>(e->tab, e->prof, n, d_in, params, d_out, e->d_occ, e->d_gtab, e->d_feas, e->G, e->lo, e->hi,
-                                                               e->cand_profiles, e->d_cand, e->d_cand_o16, e->d_ctrl); break;
-        case 2: k_small<2><<<1, kSmallThreads, 0, e->stream>>>(e->tab, e->prof, n, d_in, params, d_out, e->d_occ, e->d_gtab, e->d_feas, e->G, e->lo, e->hi,
-                                                               e->cand_profiles, e->d_cand, e->d_cand_o16, e->d_ctrl); break;
-        default: k_small<4><<<1, kSmallThreads, 0, e->stream>>>(e->tab, e->prof, n, d_in, params, d_out, e->d_occ, e->d_gtab, e->d_feas, e->G, e->lo, e->hi,
-                                                                e->cand_profiles, e->d_cand, e->d_cand_o16, e->d_ctrl); break;
-    }
+    with_cand_slots(e, [&](auto k) {
+        k_small<decltype(k)::value><<<1, kSmallThreads, 0, e->stream>>>(e->tab, e->prof, n, d_in, params, d_out, e->d_occ, e->d_gtab, e->d_feas, e->G, e->lo,
+                                                                         e->hi, e->cand_profiles, e->d_cand, e->d_cand_o16, e->d_ctrl);
+    });
     if (int rc = check_launch(e, "k_small")) return rc;
-    if (timing) {
-        cudaEventRecord(e->ev[1], e->stream);
-        cudaEventSynchronize(e->ev[1]);
-        float t;
-        cudaEventElapsedTime(&t, e->ev[0], e->ev[1]); e->st.ms_commit += t; e->st.ms_total += t;
-    }
-    ++e->st.batches; e->st.requests += n;
+    finish_batch(e, n, false);
     return ISL_OK;
 }
 
@@ -204,13 +226,7 @@ int run_few(isl_engine* e, uint32_t n, const SmallReqs& inl, uint2* d_out) {
     if (timing) cudaEventRecord(e->ev[0], e->stream);
     k_few<<<1, kFewThreads, 0, e->stream>>>(e->prof, n, inl, d_out, e->d_occ, e->d_gtab, e->d_lut, e->d_sizes, e->n_tables, e->G, e->lo, e->hi, e->d_ctrl);
     if (int rc = check_launch(e, "k_few")) return rc;
-    if (timing) {
-        cudaEventRecord(e->ev[1], e->stream);
-        cudaEventSynchronize(e->ev[1]);
-        float t;
-        cudaEventElapsedTime(&t, e->ev[0], e->ev[1]); e->st.ms_commit += t; e->st.ms_total += t;
-    }
-    ++e->st.batches; e->st.requests += n;
+    finish_batch(e, n, false);
     return ISL_OK;
 }
 
@@ -241,15 +257,7 @@ int run_bestfit(isl_engine* e, uint32_t n, const uint2* d_in, uint2* d_out) {
     if (e->n_tables == 1) k_bestfit<false><<<1, kBfThreads, smem, e->stream>>>(n, d_in, d_out, e->d_occ, e->lo, e->hi, e->d_lut, e->prof, e->d_bf_bitmaps, e->d_ctrl, e->d_score, e->d_gtab, e->d_sizes, 1);
     else k_bestfit<true><<<1, kBfThreads, 0, e->stream>>>(n, d_in, d_out, e->d_occ, e->lo, e->hi, e->d_lut, e->prof, e->d_bf_bitmaps, e->d_ctrl, e->d_score, e->d_gtab, e->d_sizes, e->n_tables);
     if (int rc = check_launch(e, "k_bestfit")) return rc;
-    if (timing) {
-        cudaEventRecord(e->ev[2], e->stream);
-        cudaEventSynchronize(e->ev[2]);
-        float t;
-        cudaEventElapsedTime(&t, e->ev[0], e->ev[1]); e->st.ms_free += t;
-        cudaEventElapsedTime(&t, e->ev[1], e->ev[2]); e->st.ms_commit += t;
-        cudaEventElapsedTime(&t, e->ev[0], e->ev[2]); e->st.ms_total += t;
-    }
-    ++e->st.batches; e->st.requests += n;
+    finish_batch(e, n, true);
     return ISL_OK;
 }
 
@@ -291,13 +299,7 @@ int run_batch(isl_engine* e, uint32_t n, const uint2* d_in, uint2* d_out, const 
             if (int rc = check_launch(e, "k_sweep_scatter")) return rc;
         }
         if (timing) cudaEventRecord(e->ev[4], e->stream);
-        int rc;
-        switch (e->n_cand_slots) {
-            case 1: rc = launch_chain<1>(e, d_out + c0, h_in, h_out); break;
-            case 2: rc = launch_chain<2>(e, d_out + c0, h_in, h_out); break;
-            default: rc = launch_chain<4>(e, d_out + c0, h_in, h_out); break;
-        }
-        if (rc) return rc;
+        if (int rc = with_cand_slots(e, [&](auto k) { return launch_chain<decltype(k)::value>(e, d_out + c0, h_in, h_out); })) return rc;
         if (timing) {
             cudaEventRecord(e->ev[5], e->stream);
             cudaEventSynchronize(e->ev[5]);
@@ -319,10 +321,14 @@ int run_batch(isl_engine* e, uint32_t n, const uint2* d_in, uint2* d_out, const 
 }
 
 
-template <int K, bool kP15>
+// One cooperative launch of k_pipeline<K, P15, Spec>.  P15: profile index 15 is in use, the pop test needs the slower, INF-safe form.
+template <int K>
 int launch_pipeline(isl_engine* e, PipeArgs& args) {
+    const bool p15 = e->prof.n == ISL_MAX_PROFILES;
+    void* kernel = p15 ? (args.spec ? (void*)k_pipeline<K, true, true> : (void*)k_pipeline<K, true, false>)
+                       : (args.spec ? (void*)k_pipeline<K, false, true> : (void*)k_pipeline<K, false, false>);
     void* params[] = {&e->tab, &args};
-    const cudaError_t err = cudaLaunchCooperativeKernel(args.spec ? (void*)k_pipeline<K, kP15, true> : (void*)k_pipeline<K, kP15, false>, dim3(args.n_seg + (args.copier ? 1u : 0u)), dim3(kPipeThreads), params, kPipeSmem, e->stream);
+    const cudaError_t err = cudaLaunchCooperativeKernel(kernel, dim3(args.n_seg + (args.copier ? 1u : 0u)), dim3(kPipeThreads), params, kPipeSmem, e->stream);
     if (err == cudaErrorCooperativeLaunchTooLarge || err == cudaErrorLaunchOutOfResources) {   // e.g. the GPU is shared: not all CTAs can be co-resident
         cudaGetLastError();
         return ISL_ESTATE;          // caller falls back to the chunk-by-chunk path
@@ -330,6 +336,11 @@ int launch_pipeline(isl_engine* e, PipeArgs& args) {
     if (err != cudaSuccess) { snprintf(e->cuda_err, sizeof(e->cuda_err), "cudaLaunchCooperativeKernel: %s", cudaGetErrorString(err)); return ISL_ECUDA; }
     ++e->st.kernel_launches;
     return ISL_OK;
+}
+
+// k_pipeline for the loaded tables
+int start_pipeline(isl_engine* e, PipeArgs& args) {
+    return with_cand_slots(e, [&](auto k) { return launch_pipeline<decltype(k)::value>(e, args); });
 }
 
 int query_coresident(isl_engine* e) {
@@ -353,14 +364,12 @@ int grow(isl_engine* e, T** buf, uint32_t* cap, size_t need, size_t elems_per_un
     return ISL_OK;
 }
 
-// Segment geometry of the pipeline for a stream of n_chunks chunks of ~avg_chunk requests.  ISL_ERANGE: the inventory does not fit the
-// co-resident CTAs (or the tables need too many candidates per segment) — the caller takes the chunk-by-chunk path.
-int plan_pipeline(isl_engine* e, uint32_t n_chunks, double avg_chunk, bool want_feed, uint32_t* seg_out, uint32_t* n_seg_out, uint32_t* sub_out, bool spec = false) {
+// Segment geometry of the pipeline for a stream of n_chunks chunks of ~avg_chunk requests; seg_cap: the largest segment whose queue
+// windows fit in shared memory.  ISL_ERANGE: the inventory does not fit the co-resident CTAs (or the tables need too many candidates per
+// segment).
+int segment_geometry(isl_engine* e, uint32_t n_chunks, double avg_chunk, bool want_feed, uint32_t seg_cap, bool spec, PipePlan* p) {
     if (int rc = query_coresident(e)) return rc;
     const uint32_t range = e->hi - e->lo;
-    uint32_t total_cand = 0;
-    for (uint32_t k = 0; k < 4; ++k) for (uint32_t l = 0; l < 32; ++l) total_cand += e->tab.desc[k][l] >> 31;
-    const uint32_t seg_cap = max_segment_for(total_cand);      // queue windows of a segment must fit in shared memory
     // Segments aimed for.  A batch's decisions form ONE sequential chain over the inventory, only different chunks overlap, so a
     // stream of B chunks over S stages takes about (S + B - 1) x (D x t_dec / S + t_fix), D = decisions of a chunk.  tools/chain_cost.py
     // on config 4, H100 SXM at 400 W: t_dec = 40.8 ns per decision, t_fix = 1.75 us per busy cell (token in -> loop start 1.58 us, loop
@@ -392,21 +401,48 @@ int plan_pipeline(isl_engine* e, uint32_t n_chunks, double avg_chunk, bool want_
     const uint32_t seg = sub * n_sub;
     const uint32_t n_seg = std::max(1u, ceil_div(range, seg));
     if (n_seg > (uint32_t)e->max_coresident) return ISL_ERANGE;
-    *seg_out = seg; *n_seg_out = n_seg; *sub_out = sub;
+    p->seg = seg; p->n_seg = n_seg; p->sub = sub;
     return ISL_OK;
+}
+
+// The pipeline of one call over n_chunks chunks of ~avg_chunk requests, with or without speculative rounds (isl_kernels.cuh,
+// DESIGN.md 4.5).  The mode is e->spec_mode, or ISL_SPEC=0|1 from the environment; auto_spec: what ISL_SPEC_AUTO means for the caller;
+// spec_allowed: the caller's own limits permit speculation; spec_feed_room: a speculative plan must also leave the copier CTA and the
+// feed reserve free.  Speculative rounds need one sub-segment per stage; a plan without them is the fallback.  ISL_ERANGE: see
+// segment_geometry — the caller takes the chunk-by-chunk path.
+int plan_pipeline(isl_engine* e, uint32_t n_chunks, double avg_chunk, bool want_feed, bool ring, bool auto_spec, bool spec_allowed,
+                  bool spec_feed_room, PipePlan* p) {
+    uint32_t total_cand = 0;
+    for (uint32_t k = 0; k < 4; ++k) for (uint32_t l = 0; l < 32; ++l) total_cand += e->tab.desc[k][l] >> 31;
+    const uint32_t seg_cap = max_segment_for(total_cand);      // queue windows of a segment must fit in shared memory
+    uint32_t mode = e->spec_mode;
+    if (const char* v = getenv("ISL_SPEC")) mode = atoi(v) ? ISL_SPEC_ON : ISL_SPEC_OFF;
+    *p = PipePlan{};
+    if (spec_allowed && !(ring && e->spec_world < 2) && kPipeThreads >= 208 && (mode == ISL_SPEC_ON || (mode == ISL_SPEC_AUTO && auto_spec))) {
+        const uint32_t range = e->hi - e->lo;
+        if (ring) {
+            // one sequence of stages over all ranks: a power-of-two stage size that every rank boundary is a multiple of (all ranks evaluate
+            // the same predicate over the same bounds, so they agree)
+            uint32_t sz = 64;
+            while (ceil_div(e->G, sz) > kSpecMaxStages) sz *= 2;
+            bool ok = sz <= kSegMax && e->spec_world == e->ring_world && n_chunks <= e->cap_spec && e->spec_bounds[e->spec_world] == e->G &&
+                      e->spec_bounds[e->spec_rank] == e->lo && e->spec_bounds[e->spec_rank + 1] == e->hi && query_coresident(e) == ISL_OK;
+            for (uint32_t r = 0; ok && r <= e->spec_world; ++r) ok = e->spec_bounds[r] % sz == 0 || e->spec_bounds[r] == e->G;
+            for (uint32_t r = 0; ok && r < e->spec_world; ++r) ok = e->spec_bounds[r] < e->spec_bounds[r + 1] && ceil_div(e->spec_bounds[r + 1] - e->spec_bounds[r], sz) <= (uint32_t)std::max(1, e->max_coresident);
+            if (ok && sz <= seg_cap) { p->seg = p->sub = sz; p->n_seg = ceil_div(range, sz); p->spec = true; return ISL_OK; }
+        } else {
+            const int rc = segment_geometry(e, n_chunks, avg_chunk, want_feed, seg_cap, true, p);
+            if (rc == ISL_ECUDA) return rc;
+            p->spec = rc == ISL_OK && p->seg == p->sub && p->n_seg <= kSpecMaxStages && p->n_seg >= 2 &&
+                      (!spec_feed_room || p->n_seg + 1 + kFeedReserve <= (uint32_t)e->max_coresident);
+            if (p->spec) return ISL_OK;
+        }
+    }
+    return segment_geometry(e, n_chunks, avg_chunk, want_feed, seg_cap, false, p);
 }
 
 constexpr unsigned long long kOpenWaitNs = 600000000000ull;     // open streams may idle between batches: 10 min
 
-// Speculative rounds (isl_kernels.cuh, DESIGN.md 4.5): wanted for this call?
-bool want_spec(isl_engine* e, uint32_t n_batches, uint32_t window, bool ring, bool legacy_token) {
-    if ((ring && e->spec_world < 2) || legacy_token || kPipeThreads < 208) return false;
-    uint32_t mode = e->spec_mode;
-    if (const char* v = getenv("ISL_SPEC")) mode = atoi(v) ? ISL_SPEC_ON : ISL_SPEC_OFF;
-    if (mode == ISL_SPEC_OFF) return false;
-    if (mode == ISL_SPEC_ON) return true;
-    return n_batches == 1 || (window >= 1 && window <= 3);
-}
 // record memory for n_chunks chunks; the words carry the call epoch (24 bits) — cleared when (re)allocated and when those bits wrap
 int prepare_spec(isl_engine* e, uint32_t n_chunks, uint32_t epoch, cudaStream_t st) {
     if (e->spec_shared) return n_chunks <= e->cap_spec ? ISL_OK : ISL_ERANGE;      // peers hold a mapping of it: fixed size, tags carry the stream id
@@ -418,6 +454,72 @@ int prepare_spec(isl_engine* e, uint32_t n_chunks, uint32_t epoch, cudaStream_t 
     return ISL_OK;
 }
 
+// A tool that serialises kernels is around: ncu and compute-sanitizer inject through the first variable, CUDA_LAUNCH_BLOCKING is the
+// second.  A pipeline that waits for kernels launched after it would starve.
+bool kernels_serialised() {
+    return getenv("CUDA_INJECTION64_PATH") || getenv("CUDA_LAUNCH_BLOCKING") || getenv("NV_COMPUTE_PROFILER_PERFWORKS_DIR");
+}
+
+int ensure_feed_stream(isl_engine* e) {
+    if (e->feed_stream) return ISL_OK;
+    ISL_CUDA(e, cudaStreamCreateWithFlags(&e->feed_stream, cudaStreamNonBlocking));
+    ISL_CUDA(e, cudaEventCreateWithFlags(&e->ev_feed, cudaEventDisableTiming));
+    ISL_CUDA(e, cudaEventCreateWithFlags(&e->ev_feed_done, cudaEventDisableTiming));
+    return ISL_OK;
+}
+
+// The epoch of a new pipeline launch.
+int next_epoch(isl_engine* e, uint32_t* epoch) {
+    *epoch = ++e->epoch;
+    if ((*epoch & 0x7FFFu) == 0) *epoch = ++e->epoch;      // the token words carry the low 15 bits as a tag; tag 0 is what a cleared buffer holds
+    if ((*epoch & 0x7FFFu) == 1 && *epoch != 1 && e->d_tokens)    // tag wrap-around: no stale word of 32 768 calls ago may look current
+        ISL_CUDA(e, cudaMemsetAsync(e->d_tokens, 0, (size_t)e->cap_tokens * kTokStride * sizeof(uint32_t), e->stream));
+    return ISL_OK;
+}
+
+// Device tables of a pipeline over n_chunks chunks (queues of q_stride entries, n_seg + 1 tokens each), n_tiles pre-pass tiles and the
+// free masks of n_batches batches; n_ready ready flags and n_done done counters (0: none needed).
+int grow_stream_buffers(isl_engine* e, uint32_t n_chunks, uint32_t q_stride, uint32_t n_tiles, uint32_t n_batches, uint32_t n_seg,
+                        uint32_t n_ready, uint32_t n_done) {
+    if (int rc = grow(e, &e->d_chunks, &e->cap_chunks, n_chunks, 1)) return rc;
+    if (int rc = grow(e, &e->d_cctl, &e->cap_cctl, n_chunks, 1)) return rc;
+    if (int rc = grow(e, &e->d_qall, &e->cap_qall, (size_t)n_chunks * q_stride, 1)) return rc;
+    if (int rc = grow(e, &e->d_tiles, &e->cap_tiles, n_tiles, 1)) return rc;
+    if (int rc = grow(e, &e->d_free_acc, &e->cap_free, (size_t)n_batches * (e->occ_bytes / 4), 1)) return rc;
+    {   // token flags carry the call epoch: a (re)allocated buffer must not hold stale flags of an earlier owner
+        const uint32_t before = e->cap_tokens;
+        if (int rc = grow(e, &e->d_tokens, &e->cap_tokens, (size_t)n_chunks * (n_seg + 1), kTokStride)) return rc;
+        if (e->cap_tokens != before) ISL_CUDA(e, cudaMemsetAsync(e->d_tokens, 0, (size_t)e->cap_tokens * kTokStride * sizeof(uint32_t), e->stream));
+    }
+    if (int rc = grow(e, &e->d_ready, &e->cap_ready, n_ready, 1)) return rc;
+    return grow(e, &e->d_done_cnt, &e->cap_done, n_done, 1);
+}
+
+// Descriptors of batch b, requests [off, off + n) of the stream: pipeline chunks of pc requests (the FREEs of a batch belong to its first
+// chunk) and tiles of kTile requests for the two pre-pass launches, stored at chunks[n_chunks] and tiles[n_tiles] on; both counts advance.
+void describe_batch(uint32_t b, uint32_t off, uint32_t n, uint32_t pc, ChunkDesc* chunks, uint32_t& n_chunks, TileDesc* tiles, uint32_t& n_tiles) {
+    const uint32_t batch_first_tile = n_tiles;
+    for (uint32_t c0 = 0; c0 < n; c0 += pc) {
+        const uint32_t cn = std::min(pc, n - c0), chunk = n_chunks++;
+        const uint32_t chunk_first_tile = n_tiles, chunk_tiles = ceil_div(cn, kTile);
+        chunks[chunk] = ChunkDesc{off + c0, cn, b, c0 == 0 ? 1u : 0u};
+        for (uint32_t t = 0; t < chunk_tiles; ++t)
+            tiles[n_tiles++] = TileDesc{off, n, b, batch_first_tile, chunk, chunk_first_tile, chunk_tiles, off + c0, cn, 0, 0, 0};
+    }
+}
+
+// The PipeArgs fields every k_pipeline launch shares; the callers add feeding, delivery, windows, rings and tracing.
+PipeArgs pipe_args(const isl_engine* e, const PipePlan& plan, uint32_t n_chunks, uint32_t epoch, uint32_t q_stride, uint2* out) {
+    PipeArgs args{};
+    args.n_chunks = n_chunks; args.n_seg = plan.n_seg; args.seg = plan.seg; args.sub = plan.sub; args.lo = e->lo; args.hi = e->hi; args.epoch = epoch;
+    args.flip = e->prof.flip; args.wait_ns = e->wait_ns;
+    args.chunks = e->d_chunks; args.cctl = e->d_cctl; args.q_all = e->d_qall; args.free_acc = reinterpret_cast<const uint8_t*>(e->d_free_acc);
+    args.q_stride = q_stride; args.free_stride = (uint32_t)e->occ_bytes; args.tokens = e->d_tokens; args.occ = e->d_occ; args.gtab = e->d_gtab;
+    args.out = out; args.feas = e->d_feas; args.stats = e->d_ctrl;
+    if (plan.spec) { args.spec = getenv("ISL_SPEC_NOREUSE") ? 3u : 1u; args.spec_mem = e->d_spec; args.spec_total = plan.n_seg; }
+    return args;
+}
+
 // Resolve a stream of batches (semantics: one batch after the other).  Enqueues only.
 // h_in / h_out (isl_place_stream): the caller's host buffers.  With the segment pipeline the batches are copied and pre-passed one
 // by one on a second stream while the pipeline already runs (it waits per batch on a device flag), and an extra CTA copies every
@@ -426,9 +528,12 @@ int run_stream(isl_engine* e, uint32_t n_batches, const uint32_t* sizes, const u
                const uint32_t* d_heads_in, uint32_t* d_heads_out, uint32_t xepoch = 0, const uint2* h_in = nullptr, uint2* h_out = nullptr,
                bool mixed_single_chunk = false) {
     e->delivered = false;
+    const uint32_t pc = e->pipe_chunk;
     uint64_t total = 0;
-    uint32_t n_chunks = 0;
-    for (uint32_t b = 0; b < n_batches; ++b) { total += sizes[b]; n_chunks += ceil_div(sizes[b], e->pipe_chunk); }
+    uint32_t n_chunks = 0, n_tiles_total = 0;
+    for (uint32_t b = 0; b < n_batches; ++b) {       // pipe_chunk is a whole number of tiles: a batch has as many tiles as its chunks
+        total += sizes[b]; n_chunks += ceil_div(sizes[b], pc); n_tiles_total += ceil_div(sizes[b], kTile);
+    }
     if (total == 0) return ISL_OK;
     if (total > e->cfg.max_batch) return ISL_ERANGE;
     const uint32_t range = e->hi - e->lo;
@@ -436,6 +541,15 @@ int run_stream(isl_engine* e, uint32_t n_batches, const uint32_t* sizes, const u
     if (ring && n_chunks > kMaxStreamChunks) return ISL_ERANGE;
     auto copy_in_whole = [&]() -> int {       // paths that do not feed batch by batch: one H2D copy up front
         if (h_in) ISL_CUDA(e, cudaMemcpyAsync(const_cast<uint2*>(d_in), h_in, (size_t)total * sizeof(uint2), cudaMemcpyHostToDevice, e->stream));
+        return ISL_OK;
+    };
+    auto batch_by_batch = [&]() -> int {      // one batch after the other through the single-chain path
+        uint64_t off = 0;
+        uint32_t hoff = 0;
+        for (uint32_t b = 0; b < n_batches; ++b) {
+            if (int rc = run_batch(e, sizes[b], d_in + off, d_out + off, d_heads_in ? d_heads_in + hoff : nullptr, d_heads_out ? d_heads_out + hoff : nullptr)) return rc;
+            off += sizes[b]; hoff += ceil_div(sizes[b], kChunk) * ISL_MAX_PROFILES;
+        }
         return ISL_OK;
     };
     if (n_batches == 1 && !d_heads_in && !d_heads_out && !xepoch && small_eligible(e, sizes[0])) {
@@ -448,102 +562,41 @@ int run_stream(isl_engine* e, uint32_t n_batches, const uint32_t* sizes, const u
     // the stream path keeps one free-mask byte per GPU and batch: very long streams over large inventories go batch by batch
     if (pipeline && (uint64_t)n_batches * e->occ_bytes > (256ull << 20)) { if (ring) return ISL_ERANGE; pipeline = false; }
     // feed mode (below): host buffers, more than one batch, no timing / tracing of the phases, no kernel-serialising tool around
-    // (ncu, compute-sanitizer, CUDA_LAUNCH_BLOCKING would starve a pipeline that waits for kernels launched after it: they inject
-    // through CUDA_INJECTION64_PATH; ISL_NO_FEED=1 switches feeding off by hand)
+    // (ISL_NO_FEED=1 switches feeding off by hand)
     const bool want_feed = h_in && h_out && n_batches >= 2 && !(e->cfg.flags & (ISL_FLAG_TIMING | ISL_FLAG_TRACE)) && !ring && !getenv("ISL_NO_FEED") &&
-                           !getenv("CUDA_INJECTION64_PATH") && !getenv("CUDA_LAUNCH_BLOCKING") && !getenv("NV_COMPUTE_PROFILER_PERFWORKS_DIR");
-    uint32_t seg = 0, n_seg = 0, sub = 0;
-    bool spec = false;
-    if (pipeline) {
-        const uint32_t win = (ring && e->ring_world == 0) ? 0u : e->window;
-        if (want_spec(e, n_batches, win, ring, legacy_token)) {      // speculative rounds need one sub-segment per stage
-            if (ring) {
-                // one sequence of stages over all ranks: a power-of-two stage size that every rank boundary is a multiple of (all ranks evaluate
-                // the same predicate over the same bounds, so they agree)
-                uint32_t sz = 64;
-                while (ceil_div(e->G, sz) > kSpecMaxStages) sz *= 2;
-                bool ok = sz <= kSegMax && e->spec_world == e->ring_world && n_chunks <= e->cap_spec && e->spec_bounds[e->spec_world] == e->G &&
-                          e->spec_bounds[e->spec_rank] == e->lo && e->spec_bounds[e->spec_rank + 1] == e->hi && query_coresident(e) == ISL_OK;
-                for (uint32_t r = 0; ok && r <= e->spec_world; ++r) ok = e->spec_bounds[r] % sz == 0 || e->spec_bounds[r] == e->G;
-                for (uint32_t r = 0; ok && r < e->spec_world; ++r) ok = e->spec_bounds[r] < e->spec_bounds[r + 1] && ceil_div(e->spec_bounds[r + 1] - e->spec_bounds[r], sz) <= (uint32_t)std::max(1, e->max_coresident);
-                uint32_t tc = 0; for (uint32_t k = 0; k < 4; ++k) for (uint32_t l = 0; l < 32; ++l) tc += e->tab.desc[k][l] >> 31;
-                ok = ok && sz <= max_segment_for(tc);
-                if (ok) { seg = sub = sz; n_seg = ceil_div(range, sz); spec = true; }
-            } else {
-                const int src = plan_pipeline(e, n_chunks, (double)total / n_chunks, want_feed, &seg, &n_seg, &sub, true);
-                if (src == ISL_ECUDA) return src;
-                spec = src == ISL_OK && seg == sub && n_seg <= kSpecMaxStages && n_seg >= 2;
-            }
-        }
-        if (!spec) {
-            const int prc = plan_pipeline(e, n_chunks, (double)total / n_chunks, want_feed, &seg, &n_seg, &sub);
-            if (prc == ISL_ECUDA) return prc;
-            if (prc != ISL_OK) { if (ring) return ISL_ERANGE; pipeline = false; }
-        }
+                           !kernels_serialised();
+    // causal window (device-side): chunk c waits for chunk c - window on every segment (of every rank: a ring counts ranks on the owner)
+    const uint32_t window = (ring && e->ring_world == 0) ? 0u : e->window;
+    PipePlan plan;
+    if (pipeline) {     // speculative rounds by default for a single batch or a window of 1..3
+        const int rc = plan_pipeline(e, n_chunks, (double)total / n_chunks, want_feed, ring, n_batches == 1 || (window >= 1 && window <= 3), true, false, &plan);
+        if (rc == ISL_ECUDA) return rc;
+        if (rc != ISL_OK) { if (ring) return ISL_ERANGE; pipeline = false; }
     }
-    if (!pipeline) {       // one batch after the other through the single-chain path
+    if (!pipeline) {
         if (int rc = copy_in_whole()) return rc;
-        uint64_t off = 0;
-        uint32_t hoff = 0;
-        for (uint32_t b = 0; b < n_batches; ++b) {
-            if (int rc = run_batch(e, sizes[b], d_in + off, d_out + off, d_heads_in ? d_heads_in + hoff : nullptr, d_heads_out ? d_heads_out + hoff : nullptr)) return rc;
-            off += sizes[b]; hoff += ceil_div(sizes[b], kChunk) * ISL_MAX_PROFILES;
-        }
-        return ISL_OK;
+        return batch_by_batch();
     }
     const bool timing = e->cfg.flags & ISL_FLAG_TIMING;
-    // Tables: every batch is cut into pipeline chunks of pipe_chunk requests (the FREEs of a batch belong to its first
-    // chunk) and into tiles of kTile requests for the two pre-pass launches.
-    const uint32_t pc = e->pipe_chunk;
-    e->h_chunks.clear(); e->h_tiles.clear();
-    uint32_t off = 0;
-    for (uint32_t b = 0; b < n_batches; ++b) {
-        const uint32_t batch_first_tile = (uint32_t)e->h_tiles.size();
-        for (uint32_t c0 = 0; c0 < sizes[b]; c0 += pc) {
-            const uint32_t cn = std::min(pc, sizes[b] - c0), chunk = (uint32_t)e->h_chunks.size();
-            const uint32_t chunk_first_tile = (uint32_t)e->h_tiles.size(), chunk_tiles = ceil_div(cn, kTile);
-            e->h_chunks.push_back(ChunkDesc{off + c0, cn, b, c0 == 0 ? 1u : 0u});
-            for (uint32_t t = 0; t < chunk_tiles; ++t)
-                e->h_tiles.push_back(TileDesc{off, sizes[b], b, batch_first_tile, chunk, chunk_first_tile, chunk_tiles, off + c0, cn, 0, 0, 0});
-        }
-        off += sizes[b];
+    e->h_chunks.resize(n_chunks); e->h_tiles.resize(n_tiles_total);
+    {
+        uint32_t off = 0, chunk = 0, tile = 0;
+        for (uint32_t b = 0; b < n_batches; ++b) { describe_batch(b, off, sizes[b], pc, e->h_chunks.data(), chunk, e->h_tiles.data(), tile); off += sizes[b]; }
     }
-    n_chunks = (uint32_t)e->h_chunks.size();
-    const uint32_t n_tiles_total = (uint32_t)e->h_tiles.size();
-    if (ring && n_chunks > kMaxStreamChunks) return ISL_ERANGE;
     const uint32_t q_stride = pc + kQPad * ISL_MAX_PROFILES;
     const uint32_t free_stride = (uint32_t)e->occ_bytes;           // bytes per batch
-    if (int rc = grow(e, &e->d_chunks, &e->cap_chunks, n_chunks, 1)) return rc;
-    if (int rc = grow(e, &e->d_cctl, &e->cap_cctl, n_chunks, 1)) return rc;
-    if (int rc = grow(e, &e->d_qall, &e->cap_qall, (size_t)n_chunks * q_stride, 1)) return rc;
-    if (int rc = grow(e, &e->d_tiles, &e->cap_tiles, n_tiles_total, 1)) return rc;
-    if (int rc = grow(e, &e->d_free_acc, &e->cap_free, (size_t)n_batches * (free_stride / 4), 1)) return rc;
-    {   // token flags carry the call epoch: a (re)allocated buffer must not hold stale flags of an earlier owner
-        const uint32_t before = e->cap_tokens;
-        if (int rc = grow(e, &e->d_tokens, &e->cap_tokens, (size_t)n_chunks * (n_seg + 1), kTokStride)) return rc;
-        if (e->cap_tokens != before) ISL_CUDA(e, cudaMemsetAsync(e->d_tokens, 0, (size_t)e->cap_tokens * kTokStride * sizeof(uint32_t), e->stream));
-    }
+    // feeding also needs room for the copier CTA plus the reserve: the pre-pass could starve behind a full house of pipeline CTAs
+    const bool feed = want_feed && plan.n_seg + 1 + kFeedReserve <= (uint32_t)e->max_coresident;
+    const bool need_done = feed || window;
+    if (int rc = grow_stream_buffers(e, n_chunks, q_stride, n_tiles_total, n_batches, plan.n_seg, feed ? n_batches + 1 : 0, need_done ? n_chunks : 0)) return rc;
     if (n_tiles_total > ceil_div(e->cfg.max_batch, kTile) + 4096) return ISL_ERANGE;
-    bool feed = want_feed;       // and room for the copier CTA plus the reserve
     uint2* h_out_dev = nullptr;
-    if (feed) {
-        if (n_seg + 1 + kFeedReserve > (uint32_t)e->max_coresident) feed = false;       // the pre-pass could starve behind a full house of pipeline CTAs
-    }
     if (feed) {
         cudaPointerAttributes pa{};
         if (cudaPointerGetAttributes(&pa, h_out) == cudaSuccess && pa.type == cudaMemoryTypeHost && pa.devicePointer) h_out_dev = static_cast<uint2*>(pa.devicePointer);
         cudaGetLastError();
-        if (!e->feed_stream) {
-            ISL_CUDA(e, cudaStreamCreateWithFlags(&e->feed_stream, cudaStreamNonBlocking));
-            ISL_CUDA(e, cudaEventCreateWithFlags(&e->ev_feed, cudaEventDisableTiming));
-            ISL_CUDA(e, cudaEventCreateWithFlags(&e->ev_feed_done, cudaEventDisableTiming));
-        }
-        if (int rc = grow(e, &e->d_ready, &e->cap_ready, n_batches + 1, 1)) return rc;
+        if (int rc = ensure_feed_stream(e)) return rc;
     }
-    // causal window (device-side): chunk c waits for chunk c - window on every segment (of every rank: a ring counts ranks on the owner)
-    const uint32_t window = (ring && e->ring_world == 0) ? 0u : e->window;
-    const bool need_done = feed || window;
-    if (need_done) if (int rc = grow(e, &e->d_done_cnt, &e->cap_done, n_chunks, 1)) return rc;
     const cudaStream_t pre = feed ? e->feed_stream : e->stream;     // the stream the tables and the pre-pass go to
     if (feed) {     // the feed stream starts behind whatever the engine's stream still holds (earlier calls, load_inventory)
         ISL_CUDA(e, cudaEventRecord(e->ev_feed, e->stream));
@@ -553,10 +606,8 @@ int run_stream(isl_engine* e, uint32_t n_batches, const uint32_t* sizes, const u
     ISL_CUDA(e, cudaMemcpyAsync(e->d_chunks, e->h_chunks.data(), n_chunks * sizeof(ChunkDesc), cudaMemcpyHostToDevice, pre));
     ISL_CUDA(e, cudaMemcpyAsync(e->d_tiles, e->h_tiles.data(), n_tiles_total * sizeof(TileDesc), cudaMemcpyHostToDevice, pre));
     ISL_CUDA(e, cudaMemsetAsync(e->d_free_acc, 0, (size_t)n_batches * free_stride, pre));
-    uint32_t epoch = ++e->epoch;
-    if ((epoch & 0x7FFFu) == 0) epoch = ++e->epoch;      // the token words carry the low 15 bits as a tag; tag 0 is what a cleared buffer holds
-    if ((epoch & 0x7FFFu) == 1 && epoch != 1 && e->d_tokens)    // tag wrap-around: no stale word of 32 768 calls ago may look current
-        ISL_CUDA(e, cudaMemsetAsync(e->d_tokens, 0, (size_t)e->cap_tokens * kTokStride * sizeof(uint32_t), e->stream));
+    uint32_t epoch;
+    if (int rc = next_epoch(e, &epoch)) return rc;
     // pre-pass of the tiles [t0, t1): defaults + free masks + histograms, then the stable partition into per-profile queues
     auto prepass = [&](uint32_t t0, uint32_t t1) -> int {
         k_prepare<<<t1 - t0, kTileThreads, 0, pre>>>(0, d_in, d_out, reinterpret_cast<uint32_t*>(e->d_occ), e->G, e->lo, e->hi, e->prof,
@@ -588,33 +639,31 @@ int run_stream(isl_engine* e, uint32_t n_batches, const uint32_t* sizes, const u
         ISL_CUDA(e, cudaStreamWaitEvent(e->stream, e->ev_feed, 0));
     } else if (int rc = prepass(0, n_tiles_total)) return rc;
     if (timing) cudaEventRecord(e->ev[2], e->stream);
-    PipeArgs args{};
-    args.n_chunks = n_chunks; args.n_seg = n_seg; args.seg = seg; args.sub = sub; args.lo = e->lo; args.hi = e->hi; args.epoch = epoch;
-    args.ready = feed ? e->d_ready : nullptr; args.done_cnt = (h_out_dev || window) ? e->d_done_cnt : nullptr; args.host_out = h_out_dev;
+    uint32_t* ring_done = nullptr;
     if (ring && window) {       // the owner's counters sit behind its result array; the other ranks reach them through the same peer mapping
         uint2* base = e->has_prev ? e->d_owner_out : e->d_res;
         if (!base) return ISL_ESTATE;
-        args.ring_done = reinterpret_cast<uint32_t*>(base + e->cfg.max_batch); args.world = e->ring_world;
-        if (!e->has_prev) ISL_CUDA(e, cudaMemsetAsync(args.ring_done, 0, (size_t)n_chunks * sizeof(uint32_t), e->stream));
+        ring_done = reinterpret_cast<uint32_t*>(base + e->cfg.max_batch);
+        if (!e->has_prev) ISL_CUDA(e, cudaMemsetAsync(ring_done, 0, (size_t)n_chunks * sizeof(uint32_t), e->stream));
     }
-    args.flip = e->prof.flip;
-    args.copier = h_out_dev ? 1u : 0u; args.window = window; args.wait_ns = e->wait_ns; args.owner_out = ring ? e->d_owner_out : nullptr;
-    args.chunks = e->d_chunks; args.cctl = e->d_cctl; args.q_all = e->d_qall; args.free_acc = reinterpret_cast<const uint8_t*>(e->d_free_acc);
-    args.q_stride = q_stride; args.free_stride = free_stride; args.tokens = e->d_tokens; args.occ = e->d_occ; args.gtab = e->d_gtab; args.out = d_out; args.feas = e->d_feas; args.stats = e->d_ctrl;
+    const bool trace = e->cfg.flags & ISL_FLAG_TRACE;
+    if (trace) {
+        if (int rc = grow(e, &e->d_trace, &e->cap_trace, (size_t)n_chunks * plan.n_seg, kTraceWords)) return rc;
+        ISL_CUDA(e, cudaMemsetAsync(e->d_trace, 0, (size_t)n_chunks * plan.n_seg * kTraceWords * sizeof(unsigned long long), e->stream));
+        e->trace_chunks = n_chunks; e->trace_seg = plan.n_seg;
+    }
+    if (plan.spec) if (int rc = prepare_spec(e, n_chunks, epoch, e->stream)) return rc;
+    PipeArgs args = pipe_args(e, plan, n_chunks, epoch, q_stride, d_out);
+    args.ready = feed ? e->d_ready : nullptr; args.done_cnt = (h_out_dev || window) ? e->d_done_cnt : nullptr; args.host_out = h_out_dev;
+    args.copier = h_out_dev ? 1u : 0u; args.window = window; args.owner_out = ring ? e->d_owner_out : nullptr;
+    if (ring_done) { args.ring_done = ring_done; args.world = e->ring_world; }
     args.heads_in = d_heads_in; args.heads_out = d_heads_out;
-    if (e->cfg.flags & ISL_FLAG_TRACE) {
-        if (int rc = grow(e, &e->d_trace, &e->cap_trace, (size_t)n_chunks * n_seg, kTraceWords)) return rc;
-        ISL_CUDA(e, cudaMemsetAsync(e->d_trace, 0, (size_t)n_chunks * n_seg * kTraceWords * sizeof(unsigned long long), e->stream));
-        e->trace_chunks = n_chunks; e->trace_seg = n_seg;
-    }
-    args.trace = (e->cfg.flags & ISL_FLAG_TRACE) ? e->d_trace : nullptr;
+    args.trace = trace ? e->d_trace : nullptr;
     args.inbox = ring && e->has_prev ? e->d_inbox : nullptr; args.outbox = ring ? e->d_outbox : nullptr; args.xepoch = xepoch;
-    if (spec) {
-        if (int rc2 = prepare_spec(e, n_chunks, epoch, e->stream)) return rc2;
-        args.spec = getenv("ISL_SPEC_NOREUSE") ? 3u : 1u; args.spec_mem = e->d_spec; args.spec_total = n_seg;
+    if (plan.spec) {
         if (ring) {         // no token ring: the records themselves cross the ranks
             args.inbox = nullptr; args.outbox = nullptr;
-            args.spec_world = e->spec_world; args.spec_rank = e->spec_rank; args.spec_base = e->lo / seg; args.spec_total = ceil_div(e->G, seg);
+            args.spec_world = e->spec_world; args.spec_rank = e->spec_rank; args.spec_base = e->lo / plan.seg; args.spec_total = ceil_div(e->G, plan.seg);
             for (uint32_t r = 0; r < e->spec_world; ++r) args.spec_peer[r] = e->spec_peer[r];
         }
         if (const char* v = getenv("ISL_SPEC_DBG")) {       // per-round stamps of one (chunk, stage) cell: tools/spec_trace.py
@@ -626,13 +675,7 @@ int run_stream(isl_engine* e, uint32_t n_batches, const uint32_t* sizes, const u
             }
         }
     }
-    int rc;
-    const bool p15 = e->prof.n == ISL_MAX_PROFILES;      // profile index 15 in use: the pop test needs the slower, INF-safe form
-    switch (e->n_cand_slots) {
-        case 1: rc = p15 ? launch_pipeline<1, true>(e, args) : launch_pipeline<1, false>(e, args); break;
-        case 2: rc = p15 ? launch_pipeline<2, true>(e, args) : launch_pipeline<2, false>(e, args); break;
-        default: rc = p15 ? launch_pipeline<4, true>(e, args) : launch_pipeline<4, false>(e, args); break;
-    }
+    const int rc = start_pipeline(e, args);
     if (rc == ISL_ESTATE && ring) return ISL_ERANGE;    // a partitioned run cannot leave the pipeline: the token ring lives inside it
     if (rc == ISL_ESTATE) {         // the pre-pass above did not touch the occupancy (frees went to the free masks): redo batch by batch
         e->max_coresident = -1;     // and do not try the pipeline again on this engine
@@ -641,12 +684,7 @@ int run_stream(isl_engine* e, uint32_t n_batches, const uint32_t* sizes, const u
             ISL_CUDA(e, cudaStreamWaitEvent(e->stream, e->ev_feed_done, 0));
             if (int rc2 = copy_in_whole()) return rc2;
         }
-        uint64_t boff = 0;
-        for (uint32_t b = 0; b < n_batches; ++b) {
-            if (int rc2 = run_batch(e, sizes[b], d_in + boff, d_out + boff, nullptr, nullptr)) return rc2;
-            boff += sizes[b];
-        }
-        return ISL_OK;
+        return batch_by_batch();
     }
     if (rc) return rc;
     if (feed) {     // the remaining batches, while the pipeline works on the first ones
@@ -700,6 +738,47 @@ void spec_disconnect(isl_engine* e) {
         e->spec_peer[r] = nullptr;
     }
     e->spec_world = 0;
+}
+
+// The checks of the stream entry points: 1..4096 batches that fit max_batch, buffers for a non-empty stream, an engine that is ready.
+int stream_entry(isl_engine* e, uint32_t n_batches, const uint32_t* sizes, bool have_buffers, uint64_t* total) {
+    if (!e || !sizes || n_batches == 0 || n_batches > 4096) return ISL_EINVAL;
+    *total = 0;
+    for (uint32_t b = 0; b < n_batches; ++b) *total += sizes[b];
+    if (*total && !have_buffers) return ISL_EINVAL;
+    if (*total > e->cfg.max_batch) return ISL_ERANGE;
+    return validate_ready(e, (uint32_t)*total);
+}
+
+// device copy of the live occupancy (isl_snapshot_occupancy, isl_what_if)
+int snapshot_occ(isl_engine* e) {
+    if (e->snap_bytes < e->occ_bytes) {
+        if (e->d_occ_snap) cudaFree(e->d_occ_snap);
+        e->d_occ_snap = nullptr; e->snap_bytes = 0;
+        ISL_CUDA(e, cudaMalloc(&e->d_occ_snap, e->occ_bytes));
+        e->snap_bytes = e->occ_bytes;
+    }
+    ISL_CUDA(e, cudaMemcpyAsync(e->d_occ_snap, e->d_occ, e->occ_bytes, cudaMemcpyDeviceToDevice, e->stream));
+    return ISL_OK;
+}
+
+// CUDA IPC: the 64-byte handle of device memory p, and the mapping of a peer's handle into this process
+int ipc_export(isl_engine* e, void* p, void* handle64) {
+    static_assert(sizeof(cudaIpcMemHandle_t) == 64, "IPC handle size");
+    cudaIpcMemHandle_t h;
+    ISL_CUDA(e, cudaIpcGetMemHandle(&h, p));
+    memcpy(handle64, &h, sizeof h);
+    return ISL_OK;
+}
+
+template <typename T>
+int ipc_open(isl_engine* e, const void* handle64, T** out) {
+    cudaIpcMemHandle_t h;
+    memcpy(&h, handle64, sizeof h);
+    void* p = nullptr;
+    ISL_CUDA(e, cudaIpcOpenMemHandle(&p, h, cudaIpcMemLazyEnablePeerAccess));
+    *out = static_cast<T*>(p);
+    return ISL_OK;
 }
 
 }  // namespace
@@ -757,21 +836,18 @@ int isl_create(const isl_config* cfg, isl_engine** out) {
         cudaFuncAttributes fa;
         const void* kernels[] = {(const void*)k_prepare, (const void*)k_partition, (const void*)k_set_flag, (const void*)k_few, (const void*)k_build_lut, (const void*)k_eval_starts,
                                  (const void*)k_free_spans, (const void*)k_capacity, (const void*)k_sweep_count, (const void*)k_sweep_scatter, (const void*)k_commit, (const void*)k_bestfit<false>, (const void*)k_bestfit<true>,
-                                 (const void*)k_chain<1>, (const void*)k_chain<2>, (const void*)k_chain<4>, (const void*)k_small<1>, (const void*)k_small<2>, (const void*)k_small<4>,
-                                 (const void*)k_pipeline<1, false, false>, (const void*)k_pipeline<1, true, false>, (const void*)k_pipeline<2, false, false>, (const void*)k_pipeline<2, true, false>,
-                                 (const void*)k_pipeline<4, false, false>, (const void*)k_pipeline<4, true, false>,
-                                 (const void*)k_pipeline<1, false, true>, (const void*)k_pipeline<1, true, true>, (const void*)k_pipeline<2, false, true>, (const void*)k_pipeline<2, true, true>,
-                                 (const void*)k_pipeline<4, false, true>, (const void*)k_pipeline<4, true, true>};
+                                 (const void*)k_chain<1>, (const void*)k_chain<2>, (const void*)k_chain<4>, (const void*)k_small<1>, (const void*)k_small<2>, (const void*)k_small<4>};
+        const void* pipes[] = {(const void*)k_pipeline<1, false, false>, (const void*)k_pipeline<1, true, false>, (const void*)k_pipeline<2, false, false>, (const void*)k_pipeline<2, true, false>,
+                               (const void*)k_pipeline<4, false, false>, (const void*)k_pipeline<4, true, false>,
+                               (const void*)k_pipeline<1, false, true>, (const void*)k_pipeline<1, true, true>, (const void*)k_pipeline<2, false, true>, (const void*)k_pipeline<2, true, true>,
+                               (const void*)k_pipeline<4, false, true>, (const void*)k_pipeline<4, true, true>};
         for (const void* k : kernels) ISL_TRY(cudaFuncGetAttributes(&fa, k));
+        for (const void* k : pipes) ISL_TRY(cudaFuncGetAttributes(&fa, k));
         // dynamic shared memory opt-in, once per engine on its own device (a process-wide cache keyed by a truncated ordinal would
         // skip devices 8.. and race between threads)
         const void* chains[] = {(const void*)k_chain<1>, (const void*)k_chain<2>, (const void*)k_chain<4>};
         for (const void* k : chains) ISL_TRY(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(kQCap * sizeof(uint16_t))));
         ISL_TRY(cudaFuncSetAttribute((const void*)k_bestfit<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(256 * (kBfSmemGpus / 32 + kBfSmemGpus / 1024) * sizeof(uint32_t))));
-        const void* pipes[] = {(const void*)k_pipeline<1, false, false>, (const void*)k_pipeline<1, true, false>, (const void*)k_pipeline<2, false, false>, (const void*)k_pipeline<2, true, false>,
-                               (const void*)k_pipeline<4, false, false>, (const void*)k_pipeline<4, true, false>,
-                               (const void*)k_pipeline<1, false, true>, (const void*)k_pipeline<1, true, true>, (const void*)k_pipeline<2, false, true>, (const void*)k_pipeline<2, true, true>,
-                               (const void*)k_pipeline<4, false, true>, (const void*)k_pipeline<4, true, true>};
         for (const void* k : pipes) ISL_TRY(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kPipeSmem));
     }
     e->occ_bytes = ((size_t)cfg->max_gpus + kSweepBlock - 1) / kSweepBlock * kSweepBlock;
@@ -1022,13 +1098,7 @@ int isl_snapshot_occupancy(isl_engine* e) {
     if (!e->have_inventory) return ISL_ESTATE;
     std::lock_guard<std::mutex> lk(e->mu);
     DeviceGuard guard(e->device);
-    if (e->snap_bytes < e->occ_bytes) {
-        if (e->d_occ_snap) cudaFree(e->d_occ_snap);
-        e->d_occ_snap = nullptr; e->snap_bytes = 0;
-        ISL_CUDA(e, cudaMalloc(&e->d_occ_snap, e->occ_bytes));
-        e->snap_bytes = e->occ_bytes;
-    }
-    ISL_CUDA(e, cudaMemcpyAsync(e->d_occ_snap, e->d_occ, e->occ_bytes, cudaMemcpyDeviceToDevice, e->stream));
+    if (int rc = snapshot_occ(e)) return rc;
     e->snap_G = e->G;
     return ISL_OK;
 }
@@ -1132,12 +1202,8 @@ static int place_batch_plain(isl_engine* e, uint32_t n, const isl_request* in, i
 }
 
 int isl_place_stream(isl_engine* e, uint32_t n_batches, const uint32_t* sizes, const isl_request* in, isl_result* out) {
-    if (!e || !sizes || n_batches == 0 || n_batches > 4096) return ISL_EINVAL;
-    uint64_t total = 0;
-    for (uint32_t b = 0; b < n_batches; ++b) total += sizes[b];
-    if (total && (!in || !out)) return ISL_EINVAL;
-    if (total > e->cfg.max_batch) return ISL_ERANGE;
-    if (int rc = validate_ready(e, (uint32_t)total)) return rc;
+    uint64_t total;
+    if (int rc = stream_entry(e, n_batches, sizes, in && out, &total)) return rc;
     if (total == 0) return ISL_OK;
     std::lock_guard<std::mutex> lk(e->mu);
     DeviceGuard guard(e->device);
@@ -1151,11 +1217,9 @@ int isl_place_stream(isl_engine* e, uint32_t n_batches, const uint32_t* sizes, c
 }
 
 int isl_place_stream_device(isl_engine* e, uint32_t n_batches, const uint32_t* sizes, const void* d_in, void* d_out) {
-    if (!e || !sizes || n_batches == 0 || n_batches > 4096 || !d_in || !d_out) return ISL_EINVAL;
-    uint64_t total = 0;
-    for (uint32_t b = 0; b < n_batches; ++b) total += sizes[b];
-    if (total > e->cfg.max_batch) return ISL_ERANGE;
-    if (int rc = validate_ready(e, (uint32_t)total)) return rc;
+    if (!d_in || !d_out) return ISL_EINVAL;
+    uint64_t total;
+    if (int rc = stream_entry(e, n_batches, sizes, true, &total)) return rc;
     std::lock_guard<std::mutex> lk(e->mu);
     DeviceGuard guard(e->device);
     return run_stream(e, n_batches, sizes, static_cast<const uint2*>(d_in), static_cast<uint2*>(d_out), nullptr, nullptr);
@@ -1169,11 +1233,7 @@ int isl_ipc_inbox_handle(isl_engine* e, void* handle64) {
         ISL_CUDA(e, cudaMalloc(&e->d_inbox, (size_t)kMaxStreamChunks * kTokStride * sizeof(uint32_t)));
         ISL_CUDA(e, cudaMemset(e->d_inbox, 0, (size_t)kMaxStreamChunks * kTokStride * sizeof(uint32_t)));
     }
-    static_assert(sizeof(cudaIpcMemHandle_t) == 64, "IPC handle size");
-    cudaIpcMemHandle_t h;
-    ISL_CUDA(e, cudaIpcGetMemHandle(&h, e->d_inbox));
-    memcpy(handle64, &h, sizeof h);
-    return ISL_OK;
+    return ipc_export(e, e->d_inbox, handle64);
 }
 
 int isl_ipc_connect(isl_engine* e, const void* next_handle64, int has_prev) {
@@ -1182,13 +1242,7 @@ int isl_ipc_connect(isl_engine* e, const void* next_handle64, int has_prev) {
     DeviceGuard guard(e->device);
     if (e->d_outbox && !e->outbox_local) cudaIpcCloseMemHandle(e->d_outbox);
     e->d_outbox = nullptr; e->outbox_local = false;
-    if (next_handle64) {
-        cudaIpcMemHandle_t h;
-        memcpy(&h, next_handle64, sizeof h);
-        void* p = nullptr;
-        ISL_CUDA(e, cudaIpcOpenMemHandle(&p, h, cudaIpcMemLazyEnablePeerAccess));
-        e->d_outbox = static_cast<uint32_t*>(p);
-    }
+    if (next_handle64) if (int rc = ipc_open(e, next_handle64, &e->d_outbox)) return rc;
     e->has_prev = has_prev != 0;
     if (e->has_prev && !e->d_inbox) return ISL_ESTATE;
     return ISL_OK;
@@ -1214,10 +1268,7 @@ int isl_ipc_spec_handle(isl_engine* e, void* handle64) {
     std::lock_guard<std::mutex> lk(e->mu);
     DeviceGuard guard(e->device);
     if (int rc = spec_shared_alloc(e)) return rc;
-    cudaIpcMemHandle_t h;
-    ISL_CUDA(e, cudaIpcGetMemHandle(&h, e->d_spec));
-    memcpy(handle64, &h, sizeof h);
-    return ISL_OK;
+    return ipc_export(e, e->d_spec, handle64);
 }
 
 // handles: world x 64 bytes (isl_ipc_spec_handle of every rank, own entry ignored); bounds: world + 1 canonical GPU indices, rank r owns
@@ -1233,11 +1284,7 @@ int isl_ipc_connect_spec(isl_engine* e, uint32_t world, uint32_t rank, const voi
     e->spec_peer_local = false;
     for (uint32_t r = 0; r < world; ++r) {
         if (r == rank) { e->spec_peer[r] = e->d_spec; continue; }
-        cudaIpcMemHandle_t h;
-        memcpy(&h, static_cast<const char*>(handles) + 64 * r, sizeof h);
-        void* p = nullptr;
-        ISL_CUDA(e, cudaIpcOpenMemHandle(&p, h, cudaIpcMemLazyEnablePeerAccess));
-        e->spec_peer[r] = static_cast<unsigned long long*>(p);
+        if (int rc = ipc_open(e, static_cast<const char*>(handles) + 64 * r, &e->spec_peer[r])) return rc;
     }
     for (uint32_t r = 0; r <= world; ++r) e->spec_bounds[r] = bounds[r];
     e->spec_world = world; e->spec_rank = rank;
@@ -1264,11 +1311,9 @@ int isl_connect_spec_local(isl_engine* e, uint32_t world, uint32_t rank, isl_eng
 }
 
 int isl_place_stream_partitioned(isl_engine* e, uint32_t n_batches, const uint32_t* sizes, const void* d_in, void* d_out, uint32_t stream_id) {
-    if (!e || !sizes || n_batches == 0 || n_batches > 4096 || !d_in || !d_out || stream_id == 0) return ISL_EINVAL;
-    uint64_t total = 0;
-    for (uint32_t b = 0; b < n_batches; ++b) total += sizes[b];
-    if (total > e->cfg.max_batch) return ISL_ERANGE;
-    if (int rc = validate_ready(e, (uint32_t)total)) return rc;
+    if (!d_in || !d_out || stream_id == 0) return ISL_EINVAL;
+    uint64_t total;
+    if (int rc = stream_entry(e, n_batches, sizes, true, &total)) return rc;
     std::lock_guard<std::mutex> lk(e->mu);
     DeviceGuard guard(e->device);
     return run_stream(e, n_batches, sizes, static_cast<const uint2*>(d_in), static_cast<uint2*>(d_out), nullptr, nullptr, stream_id);
@@ -1400,15 +1445,7 @@ int isl_what_if(isl_engine* e, uint32_t n, const isl_request* plan, isl_result* 
     if (int rc = validate_ready(e, n)) return rc;
     std::lock_guard<std::mutex> lk(e->mu);          // snapshot, plan, measurement and restore under ONE lock: nobody sees the hypothetical state
     DeviceGuard guard(e->device);
-    if (e->snap_bytes < e->occ_bytes) {
-        if (e->d_occ_snap) cudaFree(e->d_occ_snap);
-        e->d_occ_snap = nullptr; e->snap_bytes = 0;
-        ISL_CUDA(e, cudaMalloc(&e->d_occ_snap, e->occ_bytes));
-        e->snap_bytes = e->occ_bytes;
-    }
-    const uint32_t keep_snap_G = e->snap_G;         // a caller's own snapshot (isl_snapshot_occupancy) does not survive a what-if: say so
-    (void)keep_snap_G;
-    ISL_CUDA(e, cudaMemcpyAsync(e->d_occ_snap, e->d_occ, e->occ_bytes, cudaMemcpyDeviceToDevice, e->stream));
+    if (int rc = snapshot_occ(e)) return rc;
     int rc = ISL_OK;
     if (cap_before) rc = capacity_locked(e, cap_before);
     if (!rc && n) rc = place_batch_locked(e, n, plan, out);
@@ -1416,7 +1453,7 @@ int isl_what_if(isl_engine* e, uint32_t n, const isl_request* plan, isl_result* 
     // the live state comes back whatever happened above
     const cudaError_t err = cudaMemcpyAsync(e->d_occ, e->d_occ_snap, e->occ_bytes, cudaMemcpyDeviceToDevice, e->stream);
     const cudaError_t err2 = cudaStreamSynchronize(e->stream);
-    e->snap_G = 0;
+    e->snap_G = 0;                                  // a caller's own snapshot (isl_snapshot_occupancy) does not survive a what-if
     if (!rc && (err != cudaSuccess || err2 != cudaSuccess)) { snprintf(e->cuda_err, sizeof(e->cuda_err), "isl_what_if restore: %s", cudaGetErrorString(err != cudaSuccess ? err : err2)); rc = ISL_ECUDA; }
     return rc;
 }
@@ -1469,10 +1506,7 @@ int isl_ipc_results_handle(isl_engine* e, void* handle64) {
     if (!e || !handle64) return ISL_EINVAL;
     std::lock_guard<std::mutex> lk(e->mu);
     DeviceGuard guard(e->device);
-    cudaIpcMemHandle_t h;
-    ISL_CUDA(e, cudaIpcGetMemHandle(&h, e->d_res));
-    memcpy(handle64, &h, sizeof h);
-    return ISL_OK;
+    return ipc_export(e, e->d_res, handle64);
 }
 
 int isl_ipc_connect_owner(isl_engine* e, const void* owner_handle64) {
@@ -1481,13 +1515,7 @@ int isl_ipc_connect_owner(isl_engine* e, const void* owner_handle64) {
     DeviceGuard guard(e->device);
     if (e->d_owner_out && !e->owner_local) cudaIpcCloseMemHandle(e->d_owner_out);
     e->d_owner_out = nullptr; e->owner_local = false;
-    if (owner_handle64) {
-        cudaIpcMemHandle_t h;
-        memcpy(&h, owner_handle64, sizeof h);
-        void* p = nullptr;
-        ISL_CUDA(e, cudaIpcOpenMemHandle(&p, h, cudaIpcMemLazyEnablePeerAccess));
-        e->d_owner_out = static_cast<uint2*>(p);
-    }
+    if (owner_handle64) return ipc_open(e, owner_handle64, &e->d_owner_out);
     return ISL_OK;
 }
 
@@ -1507,9 +1535,9 @@ int isl_stream_open(isl_engine* e, uint32_t max_batches) {
     if (!e || max_batches == 0 || max_batches > kMaxStreamChunks) return ISL_EINVAL;
     if (!e->have_profiles || !e->have_inventory || e->open.active) return ISL_ESTATE;
     if (bestfit_family(e->cfg.policy)) return ISL_EINVAL;
-    // a tool that serialises kernels (ncu, compute-sanitizer, CUDA_LAUNCH_BLOCKING) would starve a resident kernel that waits for kernels
-    // launched after it: refuse instead of hanging until the device-side trap (callers fall back to isl_place_batch per batch)
-    if (getenv("ISL_NO_FEED") || getenv("CUDA_INJECTION64_PATH") || getenv("CUDA_LAUNCH_BLOCKING") || getenv("NV_COMPUTE_PROFILER_PERFWORKS_DIR")) {
+    // a tool that serialises kernels would starve a resident kernel that waits for kernels launched after it: refuse instead of hanging
+    // until the device-side trap (callers fall back to isl_place_batch per batch)
+    if (getenv("ISL_NO_FEED") || kernels_serialised()) {
         snprintf(e->cuda_err, sizeof(e->cuda_err), "isl_stream_open: kernel-serialising tool or ISL_NO_FEED set; open streams need concurrent kernels");
         return ISL_ESTATE;
     }
@@ -1518,35 +1546,15 @@ int isl_stream_open(isl_engine* e, uint32_t max_batches) {
     auto& o = e->open;
     const uint32_t pc = e->pipe_chunk;
     if ((uint64_t)max_batches * pc > e->cfg.max_batch) return ISL_ERANGE;       // every batch owns a slot of the staging buffers
-    uint32_t seg = 0, n_seg = 0, sub = 0;
-    // speculative rounds: the caller says (isl_set_causal_window) that it keeps at most 1..3 batches in flight, or asks for them outright
-    o.spec = false;
-    {
-        uint32_t mode = e->spec_mode;
-        if (const char* v = getenv("ISL_SPEC")) mode = atoi(v) ? ISL_SPEC_ON : ISL_SPEC_OFF;
-        if (kPipeThreads >= 208 && (mode == ISL_SPEC_ON || (mode == ISL_SPEC_AUTO && e->window >= 1 && e->window <= 3)) &&
-            (uint64_t)max_batches * kSpecWordsPerChunk * 8ull <= (1ull << 30)) {
-            const int src = plan_pipeline(e, std::max(2u, max_batches), (double)pc, true, &seg, &n_seg, &sub, true);
-            if (src == ISL_ECUDA) return src;
-            o.spec = src == ISL_OK && seg == sub && n_seg <= kSpecMaxStages && n_seg >= 2 && n_seg + 1 + kFeedReserve <= (uint32_t)e->max_coresident;
-        }
-    }
-    if (!o.spec) if (int rc = plan_pipeline(e, std::max(2u, max_batches), (double)pc, true, &seg, &n_seg, &sub)) return rc;
-    if (n_seg + 1 + kFeedReserve > (uint32_t)e->max_coresident) return ISL_ERANGE;  // the feed kernels need SMs next to the resident pipeline
-    o.seg = seg; o.n_seg = n_seg; o.sub = sub; o.max_batches = max_batches; o.submitted = 0; o.launched = false;
+    // speculative rounds: the caller says (isl_set_causal_window) that it keeps at most 1..3 batches in flight, or asks for them outright;
+    // their record memory stays within 1 GiB and their stages leave room for the copier CTA and the feed kernels
+    PipePlan plan;
+    if (int rc = plan_pipeline(e, std::max(2u, max_batches), (double)pc, true, false, e->window >= 1 && e->window <= 3,
+                               (uint64_t)max_batches * kSpecWordsPerChunk * 8ull <= (1ull << 30), true, &plan)) return rc;
+    if (plan.n_seg + 1 + kFeedReserve > (uint32_t)e->max_coresident) return ISL_ERANGE;  // the feed kernels need SMs next to the resident pipeline
+    o.plan = plan; o.max_batches = max_batches; o.submitted = 0; o.launched = false;
     o.q_stride = pc + kQPad * ISL_MAX_PROFILES; o.free_stride = (uint32_t)e->occ_bytes; o.tiles_per_batch = pc / kTile;
-    if (int rc = grow(e, &e->d_chunks, &e->cap_chunks, max_batches, 1)) return rc;
-    if (int rc = grow(e, &e->d_cctl, &e->cap_cctl, max_batches, 1)) return rc;
-    if (int rc = grow(e, &e->d_qall, &e->cap_qall, (size_t)max_batches * o.q_stride, 1)) return rc;
-    if (int rc = grow(e, &e->d_tiles, &e->cap_tiles, (size_t)max_batches * o.tiles_per_batch, 1)) return rc;
-    if (int rc = grow(e, &e->d_free_acc, &e->cap_free, (size_t)max_batches * (o.free_stride / 4), 1)) return rc;
-    {
-        const uint32_t before = e->cap_tokens;
-        if (int rc = grow(e, &e->d_tokens, &e->cap_tokens, (size_t)max_batches * (n_seg + 1), kTokStride)) return rc;
-        if (e->cap_tokens != before) ISL_CUDA(e, cudaMemsetAsync(e->d_tokens, 0, (size_t)e->cap_tokens * kTokStride * sizeof(uint32_t), e->stream));
-    }
-    if (int rc = grow(e, &e->d_ready, &e->cap_ready, max_batches + 1, 1)) return rc;
-    if (int rc = grow(e, &e->d_done_cnt, &e->cap_done, max_batches, 1)) return rc;
+    if (int rc = grow_stream_buffers(e, max_batches, o.q_stride, max_batches * o.tiles_per_batch, max_batches, plan.n_seg, max_batches + 1, max_batches)) return rc;
     if ((uint64_t)max_batches * o.tiles_per_batch > ceil_div(e->cfg.max_batch, kTile) + 4096) return ISL_ERANGE;
     if (o.cap_done < max_batches) {
         if (o.h_done) cudaFreeHost(o.h_done);
@@ -1564,17 +1572,9 @@ int isl_stream_open(isl_engine* e, uint32_t max_batches) {
         o.cap_desc = max_batches;
     }
     memset(o.h_done, 0, (size_t)max_batches * sizeof(uint32_t));
-    if (!e->feed_stream) {
-        ISL_CUDA(e, cudaStreamCreateWithFlags(&e->feed_stream, cudaStreamNonBlocking));
-        ISL_CUDA(e, cudaEventCreateWithFlags(&e->ev_feed, cudaEventDisableTiming));
-        ISL_CUDA(e, cudaEventCreateWithFlags(&e->ev_feed_done, cudaEventDisableTiming));
-    }
-    uint32_t epoch = ++e->epoch;
-    if ((epoch & 0x7FFFu) == 0) epoch = ++e->epoch;
-    if ((epoch & 0x7FFFu) == 1 && epoch != 1 && e->d_tokens)
-        ISL_CUDA(e, cudaMemsetAsync(e->d_tokens, 0, (size_t)e->cap_tokens * kTokStride * sizeof(uint32_t), e->stream));
-    o.epoch = epoch;
-    if (o.spec) if (int rc = prepare_spec(e, max_batches, epoch, e->stream)) return rc;
+    if (int rc = ensure_feed_stream(e)) return rc;
+    if (int rc = next_epoch(e, &o.epoch)) return rc;
+    if (plan.spec) if (int rc = prepare_spec(e, max_batches, o.epoch, e->stream)) return rc;
     // the feed stream starts behind whatever the engine's stream still holds
     ISL_CUDA(e, cudaEventRecord(e->ev_feed, e->stream));
     ISL_CUDA(e, cudaStreamWaitEvent(e->feed_stream, e->ev_feed, 0));
@@ -1598,8 +1598,9 @@ int isl_stream_submit(isl_engine* e, uint32_t n, const isl_request* in, isl_resu
     if (cudaPointerGetAttributes(&pa, out) != cudaSuccess || pa.type != cudaMemoryTypeHost || !pa.devicePointer) { cudaGetLastError(); return ISL_EINVAL; }
     const uint32_t b = o.submitted, pc = e->pipe_chunk, off = b * pc, tile0 = b * o.tiles_per_batch, n_tiles = ceil_div(n, kTile);
     const cudaStream_t pre = e->feed_stream;
-    o.h_chunks[b] = ChunkDesc{off, n, b, 1u, static_cast<uint2*>(pa.devicePointer), 0};
-    for (uint32_t t = 0; t < n_tiles; ++t) o.h_tiles[tile0 + t] = TileDesc{off, n, b, tile0, b, tile0, n_tiles, off, n, 0, 0, 0};
+    uint32_t chunk = b, tile = tile0;
+    describe_batch(b, off, n, pc, o.h_chunks, chunk, o.h_tiles, tile);        // n <= pipe_chunk: one chunk
+    o.h_chunks[b].host_out = static_cast<uint2*>(pa.devicePointer);
     ISL_CUDA(e, cudaMemcpyAsync(e->d_chunks + b, o.h_chunks + b, sizeof(ChunkDesc), cudaMemcpyHostToDevice, pre));
     ISL_CUDA(e, cudaMemcpyAsync(e->d_tiles + tile0, o.h_tiles + tile0, (size_t)n_tiles * sizeof(TileDesc), cudaMemcpyHostToDevice, pre));
     ISL_CUDA(e, cudaMemcpyAsync(e->d_req + off, in, (size_t)n * sizeof(isl_request), cudaMemcpyHostToDevice, pre));
@@ -1614,22 +1615,10 @@ int isl_stream_submit(isl_engine* e, uint32_t n, const isl_request* in, isl_resu
     if (!o.launched) {          // the persistent pipeline starts behind the first batch's tables
         ISL_CUDA(e, cudaEventRecord(e->ev_feed, pre));
         ISL_CUDA(e, cudaStreamWaitEvent(e->stream, e->ev_feed, 0));
-        PipeArgs args{};
-        args.n_chunks = o.max_batches; args.n_seg = o.n_seg; args.seg = o.seg; args.sub = o.sub; args.lo = e->lo; args.hi = e->hi; args.epoch = o.epoch;
-        args.ready = e->d_ready; args.done_cnt = e->d_done_cnt; args.host_out = nullptr; args.copier = 1; args.open = 1;
-        args.host_done = o.d_done_host; args.window = 0; args.wait_ns = std::max(kOpenWaitNs, e->wait_ns); args.flip = e->prof.flip;
-        args.chunks = e->d_chunks; args.cctl = e->d_cctl; args.q_all = e->d_qall; args.free_acc = reinterpret_cast<const uint8_t*>(e->d_free_acc);
-        args.q_stride = o.q_stride; args.free_stride = o.free_stride; args.tokens = e->d_tokens; args.occ = e->d_occ; args.gtab = e->d_gtab;
-        args.out = e->d_res; args.feas = e->d_feas; args.stats = e->d_ctrl;
-        if (o.spec) { args.spec = getenv("ISL_SPEC_NOREUSE") ? 3u : 1u; args.spec_mem = e->d_spec; args.spec_total = o.n_seg; }
-        int rc;
-        const bool p15 = e->prof.n == ISL_MAX_PROFILES;
-        switch (e->n_cand_slots) {
-            case 1: rc = p15 ? launch_pipeline<1, true>(e, args) : launch_pipeline<1, false>(e, args); break;
-            case 2: rc = p15 ? launch_pipeline<2, true>(e, args) : launch_pipeline<2, false>(e, args); break;
-            default: rc = p15 ? launch_pipeline<4, true>(e, args) : launch_pipeline<4, false>(e, args); break;
-        }
-        if (rc) return rc == ISL_ESTATE ? ISL_ERANGE : rc;
+        PipeArgs args = pipe_args(e, o.plan, o.max_batches, o.epoch, o.q_stride, e->d_res);
+        args.ready = e->d_ready; args.done_cnt = e->d_done_cnt; args.copier = 1; args.open = 1; args.host_done = o.d_done_host;
+        args.wait_ns = std::max(kOpenWaitNs, e->wait_ns);
+        if (int rc = start_pipeline(e, args)) return rc == ISL_ESTATE ? ISL_ERANGE : rc;
         o.launched = true;
     }
     if (ticket) *ticket = b;

@@ -56,15 +56,64 @@ class Stats(C.Structure):
         return {k: getattr(self, k) for k, _ in self._fields_}
 
 
-# every symbol include/islplace.h declares; tests check that the library exports all of them
-EXPORTED_SYMBOLS = [
-    "isl_create", "isl_destroy", "isl_set_stream", "isl_synchronize", "isl_load_profiles", "isl_load_profile_tables", "isl_set_node_tables", "isl_load_inventory", "isl_read_occupancy", "isl_write_occupancy",
-    "isl_snapshot_occupancy", "isl_restore_occupancy", "isl_num_gpus", "isl_gpu_to_node", "isl_place_batch", "isl_place_batch_device", "isl_place_stream", "isl_place_stream_device", "isl_free_batch",
-    "isl_eval_starts", "isl_set_partition", "isl_place_batch_partitioned", "isl_ipc_inbox_handle", "isl_ipc_connect", "isl_connect_local", "isl_place_stream_partitioned", "isl_device_occupancy", "isl_get_stats", "isl_read_trace",
-    "isl_reset_stats", "isl_strerror", "isl_last_cuda_error", "isl_abi_version",
-    "isl_place_batch_range", "isl_stream_open", "isl_stream_submit", "isl_stream_wait", "isl_stream_close", "isl_set_causal_window", "isl_set_speculation", "isl_ipc_spec_handle", "isl_ipc_connect_spec", "isl_connect_spec_local",
-    "isl_host_alloc", "isl_host_free", "isl_device_results", "isl_ipc_results_handle", "isl_ipc_connect_owner", "isl_connect_owner_local", "isl_set_ring_world", "isl_capacity", "isl_what_if",
-]
+# ctypes signature of every symbol include/islplace.h declares; tests check the header against these names and that the library
+# exports all of them
+_P = C.c_void_p
+SIGNATURES = {
+    "isl_create": (C.c_int, [C.POINTER(Config), C.POINTER(_P)]),
+    "isl_destroy": (C.c_int, [_P]),
+    "isl_set_stream": (C.c_int, [_P, _P]),
+    "isl_snapshot_occupancy": (C.c_int, [_P]),
+    "isl_restore_occupancy": (C.c_int, [_P]),
+    "isl_synchronize": (C.c_int, [_P]),
+    "isl_load_profiles": (C.c_int, [_P, C.c_uint32, _P]),
+    "isl_load_profile_tables": (C.c_int, [_P, C.c_uint32, C.c_uint32, _P]),
+    "isl_set_node_tables": (C.c_int, [_P, C.c_uint32, _P]),
+    "isl_load_inventory": (C.c_int, [_P, C.c_uint32, _P, _P]),
+    "isl_read_occupancy": (C.c_int, [_P, _P]),
+    "isl_write_occupancy": (C.c_int, [_P, C.c_uint32, C.c_uint32, _P]),
+    "isl_num_gpus": (C.c_uint32, [_P]),
+    "isl_gpu_to_node": (C.c_uint32, [_P, C.c_uint32]),
+    "isl_place_batch": (C.c_int, [_P, C.c_uint32, _P, _P]),
+    "isl_place_batch_device": (C.c_int, [_P, C.c_uint32, _P, _P]),
+    "isl_place_stream": (C.c_int, [_P, C.c_uint32, _P, _P, _P]),
+    "isl_place_stream_device": (C.c_int, [_P, C.c_uint32, _P, _P, _P]),
+    "isl_free_batch": (C.c_int, [_P, C.c_uint32, _P]),
+    "isl_eval_starts": (C.c_int, [_P, C.c_uint32, C.c_uint32, _P, _P]),
+    "isl_set_partition": (C.c_int, [_P, C.c_uint32, C.c_uint32]),
+    "isl_place_batch_partitioned": (C.c_int, [_P, C.c_uint32, _P, _P, _P, _P]),
+    "isl_ipc_inbox_handle": (C.c_int, [_P, _P]),
+    "isl_ipc_connect": (C.c_int, [_P, _P, C.c_int]),
+    "isl_connect_local": (C.c_int, [_P, _P, C.c_int]),
+    "isl_place_stream_partitioned": (C.c_int, [_P, C.c_uint32, _P, _P, _P, C.c_uint32]),
+    "isl_device_occupancy": (_P, [_P]),
+    "isl_get_stats": (C.c_int, [_P, C.POINTER(Stats)]),
+    "isl_read_trace": (C.c_int, [_P, _P, C.c_uint32, C.POINTER(C.c_uint32), C.POINTER(C.c_uint32)]),
+    "isl_reset_stats": (C.c_int, [_P]),
+    "isl_strerror": (C.c_char_p, [C.c_int]),
+    "isl_last_cuda_error": (C.c_char_p, [_P]),
+    "isl_abi_version": (C.c_uint32, []),
+    "isl_place_batch_range": (C.c_int, [_P, C.c_uint32, C.c_uint32, C.c_uint32, _P, _P]),
+    "isl_stream_open": (C.c_int, [_P, C.c_uint32]),
+    "isl_stream_submit": (C.c_int, [_P, C.c_uint32, _P, _P, C.POINTER(C.c_uint32)]),
+    "isl_stream_wait": (C.c_int, [_P, C.c_uint32]),
+    "isl_stream_close": (C.c_int, [_P]),
+    "isl_set_causal_window": (C.c_int, [_P, C.c_uint32]),
+    "isl_set_speculation": (C.c_int, [_P, C.c_uint32]),
+    "isl_ipc_spec_handle": (C.c_int, [_P, C.c_void_p]),
+    "isl_ipc_connect_spec": (C.c_int, [_P, C.c_uint32, C.c_uint32, C.c_void_p, C.c_void_p]),
+    "isl_connect_spec_local": (C.c_int, [_P, C.c_uint32, C.c_uint32, C.c_void_p, C.c_void_p]),
+    "isl_host_alloc": (_P, [C.c_size_t]),
+    "isl_host_free": (None, [_P]),
+    "isl_device_results": (_P, [_P]),
+    "isl_ipc_results_handle": (C.c_int, [_P, _P]),
+    "isl_ipc_connect_owner": (C.c_int, [_P, _P]),
+    "isl_connect_owner_local": (C.c_int, [_P, _P]),
+    "isl_set_ring_world": (C.c_int, [_P, C.c_uint32]),
+    "isl_capacity": (C.c_int, [_P, _P]),
+    "isl_what_if": (C.c_int, [_P, C.c_uint32, _P, _P, _P, _P]),
+}
+EXPORTED_SYMBOLS = list(SIGNATURES)
 
 _lib = None
 
@@ -77,62 +126,7 @@ def load_library(path: str = LIB_PATH):
     if not os.path.exists(path):
         raise ImportError(f"{path} not built: run __graft_entry__.build() (nvcc, sm_90a). There is no CPU fallback.")
     lib = C.CDLL(path)
-    p = C.c_void_p
-    sig = {
-        "isl_create": (C.c_int, [C.POINTER(Config), C.POINTER(p)]),
-        "isl_destroy": (C.c_int, [p]),
-        "isl_set_stream": (C.c_int, [p, p]),
-        "isl_snapshot_occupancy": (C.c_int, [p]),
-        "isl_restore_occupancy": (C.c_int, [p]),
-        "isl_synchronize": (C.c_int, [p]),
-        "isl_load_profiles": (C.c_int, [p, C.c_uint32, p]),
-        "isl_load_profile_tables": (C.c_int, [p, C.c_uint32, C.c_uint32, p]),
-        "isl_set_node_tables": (C.c_int, [p, C.c_uint32, p]),
-        "isl_load_inventory": (C.c_int, [p, C.c_uint32, p, p]),
-        "isl_read_occupancy": (C.c_int, [p, p]),
-        "isl_write_occupancy": (C.c_int, [p, C.c_uint32, C.c_uint32, p]),
-        "isl_num_gpus": (C.c_uint32, [p]),
-        "isl_gpu_to_node": (C.c_uint32, [p, C.c_uint32]),
-        "isl_place_batch": (C.c_int, [p, C.c_uint32, p, p]),
-        "isl_place_batch_device": (C.c_int, [p, C.c_uint32, p, p]),
-        "isl_place_stream": (C.c_int, [p, C.c_uint32, p, p, p]),
-        "isl_place_stream_device": (C.c_int, [p, C.c_uint32, p, p, p]),
-        "isl_free_batch": (C.c_int, [p, C.c_uint32, p]),
-        "isl_eval_starts": (C.c_int, [p, C.c_uint32, C.c_uint32, p, p]),
-        "isl_set_partition": (C.c_int, [p, C.c_uint32, C.c_uint32]),
-        "isl_place_batch_partitioned": (C.c_int, [p, C.c_uint32, p, p, p, p]),
-        "isl_ipc_inbox_handle": (C.c_int, [p, p]),
-        "isl_ipc_connect": (C.c_int, [p, p, C.c_int]),
-        "isl_connect_local": (C.c_int, [p, p, C.c_int]),
-        "isl_place_stream_partitioned": (C.c_int, [p, C.c_uint32, p, p, p, C.c_uint32]),
-        "isl_device_occupancy": (p, [p]),
-        "isl_get_stats": (C.c_int, [p, C.POINTER(Stats)]),
-        "isl_read_trace": (C.c_int, [p, p, C.c_uint32, C.POINTER(C.c_uint32), C.POINTER(C.c_uint32)]),
-        "isl_reset_stats": (C.c_int, [p]),
-        "isl_strerror": (C.c_char_p, [C.c_int]),
-        "isl_last_cuda_error": (C.c_char_p, [p]),
-        "isl_abi_version": (C.c_uint32, []),
-        "isl_place_batch_range": (C.c_int, [p, C.c_uint32, C.c_uint32, C.c_uint32, p, p]),
-        "isl_stream_open": (C.c_int, [p, C.c_uint32]),
-        "isl_stream_submit": (C.c_int, [p, C.c_uint32, p, p, C.POINTER(C.c_uint32)]),
-        "isl_stream_wait": (C.c_int, [p, C.c_uint32]),
-        "isl_stream_close": (C.c_int, [p]),
-        "isl_set_causal_window": (C.c_int, [p, C.c_uint32]),
-        "isl_set_speculation": (C.c_int, [p, C.c_uint32]),
-        "isl_ipc_spec_handle": (C.c_int, [p, C.c_void_p]),
-        "isl_ipc_connect_spec": (C.c_int, [p, C.c_uint32, C.c_uint32, C.c_void_p, C.c_void_p]),
-        "isl_connect_spec_local": (C.c_int, [p, C.c_uint32, C.c_uint32, C.c_void_p, C.c_void_p]),
-        "isl_host_alloc": (p, [C.c_size_t]),
-        "isl_host_free": (None, [p]),
-        "isl_device_results": (p, [p]),
-        "isl_ipc_results_handle": (C.c_int, [p, p]),
-        "isl_ipc_connect_owner": (C.c_int, [p, p]),
-        "isl_connect_owner_local": (C.c_int, [p, p]),
-        "isl_set_ring_world": (C.c_int, [p, C.c_uint32]),
-        "isl_capacity": (C.c_int, [p, p]),
-        "isl_what_if": (C.c_int, [p, C.c_uint32, p, p, p, p]),
-    }
-    for name, (res, args) in sig.items():
+    for name, (res, args) in SIGNATURES.items():
         try:
             fn = getattr(lib, name)
         except AttributeError:
