@@ -42,21 +42,10 @@ constexpr uint32_t kMaxTables = ISL_MAX_TABLES;   // per-node profile tables (he
 // The chain's occupancy word is 16 bits: the busy slices in the low byte and, in the high byte, every table bit set EXCEPT
 // the one of the table the GPU's node publishes.  A candidate of table t carries bit (8 + t) in its mask, so `(occ16 & mask) == 0`
 // holds only on GPUs of its own table — no extra instruction per decision.
-// A/B switches of the decision loop (tools/ab_build.sh builds the variants; the defaults are what measured fastest)
-#ifndef ISL_UNIFORM_WARP
-#define ISL_UNIFORM_WARP 1      // the chain warp is selected by a warp-UNIFORM predicate (redux of the warp index): ptxas then knows the warp
-#endif                          // is converged and drops the BRA.DIV / UMOV guard in front of every redux of the loop
-#ifndef ISL_DEFER_INF
-#define ISL_DEFER_INF 1         // the "nothing fits" test runs once per unrolled group instead of once per decision
-#endif
-// true for every lane of warp 0 and only there; with ISL_UNIFORM_WARP the predicate comes out of a redux (a uniform register)
-__device__ __forceinline__ bool is_chain_warp(uint32_t warp) {
-#if ISL_UNIFORM_WARP
-    return __reduce_or_sync(0xFFFFFFFFu, warp) == 0;
-#else
-    return warp == 0;
-#endif
-}
+// The decision loop's tuning choices (DESIGN.md 4.1) are plain constants; a variant is built by editing the constant.
+// true for every lane of warp 0 and only there.  The predicate comes out of a redux (a uniform register): ptxas then knows the warp is
+// converged and drops the BRA.DIV / UMOV guard in front of every redux of the loop.
+__device__ __forceinline__ bool is_chain_warp(uint32_t warp) { return __reduce_or_sync(0xFFFFFFFFu, warp) == 0; }
 
 __host__ __device__ inline uint32_t table_tag(uint32_t table) { return ((~(1u << table)) & 0xFFu) << 8; }
 
@@ -154,16 +143,26 @@ __global__ void k_eval_starts(const uint8_t* __restrict__ lut, uint32_t profile,
     for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) out[i] = s_lut[occ[i]];
 }
 
+// A release of `size` slices from `start` on canonical GPU `gpu`: false for a malformed span (BAD_SPAN).  Otherwise `gi` is where the
+// engine keeps that GPU and `span` the slot mask shifted into the GPU's byte of its packed occupancy word, or 0 when gi is outside [lo, hi).
+__device__ __forceinline__ bool free_span(uint32_t gpu, uint32_t start, uint32_t size, uint32_t G, uint32_t lo, uint32_t hi, uint32_t flip,
+                                          uint32_t& gi, uint32_t& span) {
+    span = 0;
+    if (gpu >= G || size == 0 || start + size > ISL_SLOTS) return false;
+    gi = flip_gpu(gpu, flip);
+    if (gi >= lo && gi < hi) span = (((1u << size) - 1u) << start) << ((gi & 3u) * 8u);
+    return true;
+}
+
 __global__ void k_free_spans(uint32_t n, const isl_span* __restrict__ spans, uint32_t* __restrict__ occ32,
                              uint32_t G, uint32_t lo, uint32_t hi, Ctrl* ctrl, uint32_t flip) {
     const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
-    isl_span s = spans[i];
-    if (s.gpu >= G || s.size == 0 || (uint32_t)s.start + s.size > ISL_SLOTS) { atomicAdd(&ctrl->bad, 1ull); return; }
-    s.gpu = flip_gpu(s.gpu, flip);
-    if (s.gpu < lo || s.gpu >= hi) return;
-    const uint32_t m = (((1u << s.size) - 1u) << s.start) << ((s.gpu & 3u) * 8u);
-    atomicAnd(&occ32[s.gpu >> 2], ~m);
+    const isl_span s = spans[i];
+    uint32_t gi, span;
+    if (!free_span(s.gpu, s.start, s.size, G, lo, hi, flip, gi, span)) { atomicAdd(&ctrl->bad, 1ull); return; }
+    if (!span) return;
+    atomicAnd(&occ32[gi >> 2], ~span);
     atomicAdd(&ctrl->freed, 1ull);
 }
 
@@ -175,6 +174,32 @@ __global__ void k_free_spans(uint32_t n, const isl_span* __restrict__ spans, uin
 // ---------------------------------------------------------------------------------------------
 __device__ __forceinline__ uint2 pack_result(uint32_t gpu, uint32_t start, uint32_t size, uint32_t status) {
     return make_uint2(gpu, start | (size << 8) | (status << 16));
+}
+
+// The per-request step every pre-pass shares (k_prepare, k_small phase A, k_few): decodes the request, writes its default record
+// (ALLOC: NO_CAPACITY or BAD_PROFILE; FREE: FREED or BAD_SPAN; anything else: NOOP) and returns its partition key (the profile of a valid
+// ALLOC, else kSkip).  For a valid FREE inside [lo, hi), `gi` and `span` (non-zero) say what to release; the caller applies it.
+__device__ __forceinline__ uint32_t prepare_request(uint2 rq, uint2& out, const DevProfiles& prof, uint32_t G, uint32_t lo, uint32_t hi,
+                                                    uint32_t& gi, uint32_t& span) {
+    const uint32_t handle = rq.x, profile = rq.y & 0xFFu, op = (rq.y >> 8) & 0xFFu, start = (rq.y >> 16) & 0xFFu, size = rq.y >> 24;
+    span = 0;
+    if (op == ISL_OP_ALLOC) {
+        if (profile < prof.n) { out = pack_result(ISL_GPU_NONE, ISL_START_NONE, prof.rows[profile].size, ISL_ST_NO_CAPACITY); return profile; }
+        out = pack_result(ISL_GPU_NONE, ISL_START_NONE, 0, ISL_ST_BAD_PROFILE);
+    } else if (op == ISL_OP_FREE) {
+        const bool ok = free_span(handle, start, size, G, lo, hi, prof.flip, gi, span);
+        out = pack_result(handle, start, size, ok ? ISL_ST_FREED : ISL_ST_BAD_SPAN);
+    } else out = pack_result(ISL_GPU_NONE, ISL_START_NONE, 0, ISL_ST_NOOP);
+    return kSkip;
+}
+
+// One logged decision of the chain (key, candidate index): the PLACED record of its request, and the slot mask ORed into the packed
+// occupancy word.  Distinct decisions on one GPU have disjoint masks (the chain only accepts free masks): the atomic only serialises
+// neighbours that share a word.  `cand` may have been written by the calling kernel, hence the L2 load.
+__device__ __forceinline__ void commit_decision(uint2 e, const uint32_t* cand, uint32_t* occ32, uint2* out, uint32_t flip) {
+    const uint32_t g = __ldcg(cand + e.y) >> 8, mask = e.x & 0xFFu, t = (e.x >> 15) & 0xFFFFu;
+    out[t] = pack_result(flip_gpu(g, flip), __ffs(mask) - 1, __popc(mask), ISL_ST_PLACED);
+    atomicOr(&occ32[g >> 2], mask << ((g & 3u) * 8u));
 }
 
 // One tile of 1024 requests of a stream: which batch / pipeline chunk it belongs to (host-built table, one launch
@@ -211,25 +236,13 @@ __global__ void __launch_bounds__(kTileThreads) k_prepare(uint32_t n, const uint
         const uint32_t i = tile * kTile + r * kTileThreads + threadIdx.x;
         uint32_t key = kSkip;
         if (i < n) {
-            const uint2 rq = in[i];
-            const uint32_t handle = rq.x, profile = rq.y & 0xFFu, op = (rq.y >> 8) & 0xFFu;
-            const uint32_t start = (rq.y >> 16) & 0xFFu, size = rq.y >> 24;
-            if (op == ISL_OP_ALLOC) {
-                if (profile < prof.n) { key = profile; out[i] = pack_result(ISL_GPU_NONE, ISL_START_NONE, prof.rows[profile].size, ISL_ST_NO_CAPACITY); }
-                else out[i] = pack_result(ISL_GPU_NONE, ISL_START_NONE, 0, ISL_ST_BAD_PROFILE);
-            } else if (op == ISL_OP_FREE) {
-                if (handle >= G || size == 0 || start + size > ISL_SLOTS) out[i] = pack_result(handle, start, size, ISL_ST_BAD_SPAN);
-                else {
-                    const uint32_t gi = flip_gpu(handle, prof.flip);       // where the engine keeps that GPU
-                    if (gi >= lo && gi < hi) {
-                        const uint32_t span = (((1u << size) - 1u) << start) << ((gi & 3u) * 8u);
-                        if (descs) atomicOr(&free_acc[gi >> 2], span);
-                        else atomicAnd(&occ32[gi >> 2], ~span);
-                        atomicAdd(&s_freed, 1u);
-                    }
-                    out[i] = pack_result(handle, start, size, ISL_ST_FREED);
-                }
-            } else out[i] = pack_result(ISL_GPU_NONE, ISL_START_NONE, 0, ISL_ST_NOOP);
+            uint32_t gi, span;
+            key = prepare_request(in[i], out[i], prof, G, lo, hi, gi, span);
+            if (span) {
+                if (descs) atomicOr(&free_acc[gi >> 2], span);
+                else atomicAnd(&occ32[gi >> 2], ~span);
+                atomicAdd(&s_freed, 1u);
+            }
         }
         const uint32_t peers = __match_any_sync(0xFFFFFFFFu, key);
         if (key != kSkip && lane == (uint32_t)(__ffs(peers) - 1)) atomicAdd(&s_cnt[key], (uint32_t)__popc(peers));
@@ -340,12 +353,18 @@ __device__ __forceinline__ uint4 ld_nc_v4(const uint4* p) {
     return r;
 }
 
+// byte j (0..15) of a 16-byte vector of occupancy or table bytes: the byte of the vector's j-th GPU
+__device__ __forceinline__ uint32_t byte16(const uint32_t (&w)[4], uint32_t j) { return (w[j >> 2] >> ((j & 3u) * 8u)) & 0xFFu; }
+__device__ __forceinline__ uint32_t byte16(const uint4 v, uint32_t j) {
+    const uint32_t w[4] = {v.x, v.y, v.z, v.w};
+    return byte16(w, j);
+}
+
 __device__ __forceinline__ uint32_t sweep_mask16(const uint4 v, const uint4 tv, const uint16_t* s_feas, uint32_t active, uint32_t g0, uint32_t lo, uint32_t hi) {
-    const uint32_t w[4] = {v.x, v.y, v.z, v.w}, tw[4] = {tv.x, tv.y, tv.z, tv.w};
     uint32_t mask = 0;
 #pragma unroll
     for (uint32_t j = 0; j < 16; ++j) {
-        const uint32_t o = (w[j >> 2] >> ((j & 3u) * 8u)) & 0xFFu, t = (tw[j >> 2] >> ((j & 3u) * 8u)) & (kMaxTables - 1);
+        const uint32_t o = byte16(v, j), t = byte16(tv, j) & (kMaxTables - 1);
         const uint32_t g = g0 + j;
         if ((s_feas[t * 256 + o] & active) && g >= lo && g < hi) mask |= 1u << j;
     }
@@ -356,15 +375,26 @@ __device__ __forceinline__ uint32_t sweep_mask16(const uint4 v, const uint4 tv, 
 // to interleave, GPU g simply takes the next capn[occ_g] requests of the queue.  The two sweep passes then compute the
 // device-wide exclusive scan of those capacities and commit results and occupancy directly — fully parallel, no chain.
 __device__ __forceinline__ uint32_t scan_capacity16(const uint4 v, const uint4 tv, const uint8_t* __restrict__ capn, uint32_t p, uint32_t g0, uint32_t lo, uint32_t hi) {
-    const uint32_t w[4] = {v.x, v.y, v.z, v.w}, tw[4] = {tv.x, tv.y, tv.z, tv.w};
     uint32_t c = 0;
 #pragma unroll
     for (uint32_t j = 0; j < 16; ++j) {
-        const uint32_t o = (w[j >> 2] >> ((j & 3u) * 8u)) & 0xFFu, t = (tw[j >> 2] >> ((j & 3u) * 8u)) & (kMaxTables - 1);
+        const uint32_t o = byte16(v, j), t = byte16(tv, j) & (kMaxTables - 1);
         const uint32_t g = g0 + j;
         if (g >= lo && g < hi) c += capn[(t * ISL_MAX_PROFILES + p) * 256 + o];
     }
     return c;
+}
+
+// Ordered compaction of the GPUs a 16-GPU sweep found feasible (`mask`), from position `off` on.  Returns the position after the last.
+__device__ __forceinline__ uint32_t emit_candidates(uint32_t mask, const uint4 v, const uint4 tv, uint32_t g0, uint32_t off,
+                                                    uint32_t* __restrict__ cand, uint16_t* __restrict__ cand_o16) {
+    while (mask) {
+        const uint32_t j = __ffs(mask) - 1; mask &= mask - 1;
+        const uint32_t o = byte16(v, j), t = byte16(tv, j) & (kMaxTables - 1);
+        cand_o16[off] = (uint16_t)(o | table_tag(t));          // what the chain needs: occupancy + table tag
+        cand[off++] = ((g0 + j) << 8) | o;                       // what the commit needs: the GPU
+    }
+    return off;
 }
 
 __global__ void __launch_bounds__(kSweepThreads) k_sweep_count(const uint4* __restrict__ occ16, const uint4* __restrict__ gtab16, const uint16_t* __restrict__ feas,
@@ -432,7 +462,6 @@ __global__ void __launch_bounds__(kSweepThreads) k_sweep_scatter(const uint4* __
     __syncthreads();
     uint32_t off = s_base + incl - c;
     for (uint32_t w = 0; w < warp; ++w) off += s_warp[w];
-    const uint32_t wv[4] = {v.x, v.y, v.z, v.w}, twv[4] = {tv.x, tv.y, tv.z, tv.w};
     if (scan_mode) {        // `off` is the exclusive scan of the capacities = queue position this thread's first GPU starts at
         const uint32_t h0 = heads_in ? heads_in[sp] : 0u, n_p = ctrl->qcnt[sp];
         const uint16_t* qp = q + ctrl->qoff[sp];
@@ -442,7 +471,7 @@ __global__ void __launch_bounds__(kSweepThreads) k_sweep_scatter(const uint4* __
             for (uint32_t j = 0; j < 16 && pos < n_p; ++j) {
                 const uint32_t g = g0 + j;
                 if (g < lo || g >= hi) continue;
-                const uint32_t o = (wv[j >> 2] >> ((j & 3u) * 8u)) & 0xFFu, t = (twv[j >> 2] >> ((j & 3u) * 8u)) & (kMaxTables - 1);
+                const uint32_t o = byte16(v, j), t = byte16(tv, j) & (kMaxTables - 1);
                 const uint32_t row = (t * ISL_MAX_PROFILES + sp) * 256 + o;
                 const uint32_t cg = capn[row], size = sizes[t * ISL_MAX_PROFILES + sp];
                 if (!cg) continue;
@@ -463,13 +492,7 @@ __global__ void __launch_bounds__(kSweepThreads) k_sweep_scatter(const uint4* __
         }
         return;
     }
-    uint32_t m = mask;
-    while (m) {
-        const uint32_t j = __ffs(m) - 1; m &= m - 1;
-        const uint32_t o = (wv[j >> 2] >> ((j & 3u) * 8u)) & 0xFFu, t = (twv[j >> 2] >> ((j & 3u) * 8u)) & (kMaxTables - 1);
-        cand_o16[off] = (uint16_t)(o | table_tag(t));          // what the chain needs: occupancy + table tag
-        cand[off++] = ((g0 + j) << 8) | o;                       // what the commit needs: the GPU
-    }
+    off = emit_candidates(mask, v, tv, g0, off, cand, cand_o16);
     if (blockIdx.x == gridDim.x - 1 && tid == kSweepThreads - 1) ctrl->n_cand = off;
 }
 
@@ -689,19 +712,9 @@ __global__ void __launch_bounds__(kSmallThreads, 1) k_small(CandTab tab, DevProf
     // ---- A: one request per thread
     uint32_t key = kSkip, rank = 0;
     if (tid < n) {
-        const uint2 rq = in ? in[tid] : inl.r[tid];
-        const uint32_t handle = rq.x, profile = rq.y & 0xFFu, op = (rq.y >> 8) & 0xFFu, start = (rq.y >> 16) & 0xFFu, size = rq.y >> 24;
-        if (op == ISL_OP_ALLOC) {
-            if (profile < prof.n) { key = profile; out[tid] = pack_result(ISL_GPU_NONE, ISL_START_NONE, prof.rows[profile].size, ISL_ST_NO_CAPACITY); }
-            else out[tid] = pack_result(ISL_GPU_NONE, ISL_START_NONE, 0, ISL_ST_BAD_PROFILE);
-        } else if (op == ISL_OP_FREE) {
-            if (handle >= G || size == 0 || start + size > ISL_SLOTS) out[tid] = pack_result(handle, start, size, ISL_ST_BAD_SPAN);
-            else {
-                const uint32_t gi = flip_gpu(handle, prof.flip);
-                if (gi >= lo && gi < hi) { atomicAnd(&occ32[gi >> 2], ~((((1u << size) - 1u) << start) << ((gi & 3u) * 8u))); atomicAdd(&s_freed, 1u); }
-                out[tid] = pack_result(handle, start, size, ISL_ST_FREED);
-            }
-        } else out[tid] = pack_result(ISL_GPU_NONE, ISL_START_NONE, 0, ISL_ST_NOOP);
+        uint32_t gi, span;
+        key = prepare_request(in ? in[tid] : inl.r[tid], out[tid], prof, G, lo, hi, gi, span);
+        if (span) { atomicAnd(&occ32[gi >> 2], ~span); atomicAdd(&s_freed, 1u); }
     }
     {
         const uint32_t peers = __match_any_sync(0xFFFFFFFFu, key);
@@ -756,15 +769,7 @@ __global__ void __launch_bounds__(kSmallThreads, 1) k_small(CandTab tab, DevProf
                 if (lane == 31) s_nlog = x;     // round total (s_nlog is reused as scratch here)
             }
             __syncthreads();
-            uint32_t off = s_base + s_scan[warp] + incl - c;
-            const uint32_t wv[4] = {v.x, v.y, v.z, v.w}, twv[4] = {tv.x, tv.y, tv.z, tv.w};
-            uint32_t m = mask;
-            while (m) {
-                const uint32_t j = __ffs(m) - 1; m &= m - 1;
-                const uint32_t o = (wv[j >> 2] >> ((j & 3u) * 8u)) & 0xFFu, t = (twv[j >> 2] >> ((j & 3u) * 8u)) & (kMaxTables - 1);
-                cand_o16[off] = (uint16_t)(o | table_tag(t));
-                cand[off++] = ((g0 + j) << 8) | o;
-            }
+            emit_candidates(mask, v, tv, g0, s_base + s_scan[warp] + incl - c, cand, cand_o16);
             __syncthreads();
             if (tid == 0) s_base += s_nlog;
             __syncthreads();
@@ -785,12 +790,7 @@ __global__ void __launch_bounds__(kSmallThreads, 1) k_small(CandTab tab, DevProf
     }
     __syncthreads();
     // ---- D: commit
-    for (uint32_t j = tid; j < s_nlog; j += kSmallThreads) {
-        const uint2 e = s_log[j];
-        const uint32_t g = __ldcg(cand + e.y) >> 8, mask = e.x & 0xFFu, t = (e.x >> 15) & 0xFFFFu;
-        out[t] = pack_result(flip_gpu(g, prof.flip), __ffs(mask) - 1, __popc(mask), ISL_ST_PLACED);
-        atomicOr(&occ32[g >> 2], mask << ((g & 3u) * 8u));
-    }
+    for (uint32_t j = tid; j < s_nlog; j += kSmallThreads) commit_decision(s_log[j], cand, occ32, out, prof.flip);
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -816,20 +816,10 @@ __global__ void __launch_bounds__(kFewThreads, 1) k_few(DevProfiles prof, uint32
     for (uint32_t i = tid; i < n_tables * ISL_MAX_PROFILES * 64; i += kFewThreads) reinterpret_cast<uint32_t*>(s_lut)[i] = reinterpret_cast<const uint32_t*>(lut)[i];
     if (tid < n_tables * ISL_MAX_PROFILES) s_sizes[tid] = sizes[tid];
     uint32_t freed = 0, allocs = 0;
-    if (tid < n) {          // defaults and FREEs, one request per thread (as k_prepare / k_small phase A)
-        const uint2 rq = inl.r[tid];
-        const uint32_t handle = rq.x, profile = rq.y & 0xFFu, op = (rq.y >> 8) & 0xFFu, start = (rq.y >> 16) & 0xFFu, size = rq.y >> 24;
-        if (op == ISL_OP_ALLOC) {
-            if (profile < prof.n) { out[tid] = pack_result(ISL_GPU_NONE, ISL_START_NONE, prof.rows[profile].size, ISL_ST_NO_CAPACITY); allocs = 1; }
-            else out[tid] = pack_result(ISL_GPU_NONE, ISL_START_NONE, 0, ISL_ST_BAD_PROFILE);
-        } else if (op == ISL_OP_FREE) {
-            if (handle >= G || size == 0 || start + size > ISL_SLOTS) out[tid] = pack_result(handle, start, size, ISL_ST_BAD_SPAN);
-            else {
-                const uint32_t gi = flip_gpu(handle, prof.flip);
-                if (gi >= lo && gi < hi) { atomicAnd(&occ32[gi >> 2], ~((((1u << size) - 1u) << start) << ((gi & 3u) * 8u))); freed = 1; }
-                out[tid] = pack_result(handle, start, size, ISL_ST_FREED);
-            }
-        } else out[tid] = pack_result(ISL_GPU_NONE, ISL_START_NONE, 0, ISL_ST_NOOP);
+    if (tid < n) {          // defaults and FREEs, one request per thread
+        uint32_t gi, span;
+        allocs = prepare_request(inl.r[tid], out[tid], prof, G, lo, hi, gi, span) != kSkip;
+        if (span) { atomicAnd(&occ32[gi >> 2], ~span); freed = 1; }
     }
     __threadfence();                        // the frees must be visible to the loads below
     __syncthreads();
@@ -845,7 +835,7 @@ __global__ void __launch_bounds__(kFewThreads, 1) k_few(DevProfiles prof, uint32
         uint32_t best = kInf;
 #pragma unroll
         for (int j = 15; j >= 0; --j) {     // descending, so the lowest feasible GPU of the thread is what remains
-            const uint32_t g = g0 + j, o = (wv[j >> 2] >> ((j & 3) * 8)) & 0xFFu, t = (twv[j >> 2] >> ((j & 3) * 8)) & (kMaxTables - 1);
+            const uint32_t g = g0 + j, o = byte16(wv, j), t = byte16(twv, j) & (kMaxTables - 1);
             if (g >= lo && g < hi && s_lut[(t * ISL_MAX_PROFILES + p) * 256 + o] != ISL_START_NONE) best = g;
         }
         const uint32_t wm = __reduce_min_sync(0xFFFFFFFFu, best);
@@ -855,7 +845,7 @@ __global__ void __launch_bounds__(kFewThreads, 1) k_few(DevProfiles prof, uint32
         __syncthreads();
         const uint32_t g = s_win;
         if (g != kInf && g >= g0 && g < g0 + 16u) {             // the owner commits
-            const uint32_t j = g - g0, sh = (j & 3u) * 8u, o = (wv[j >> 2] >> sh) & 0xFFu, t = (twv[j >> 2] >> sh) & (kMaxTables - 1);
+            const uint32_t j = g - g0, sh = (j & 3u) * 8u, o = byte16(wv, j), t = byte16(twv, j) & (kMaxTables - 1);
             const uint32_t st = s_lut[(t * ISL_MAX_PROFILES + p) * 256 + o], size = s_sizes[t * ISL_MAX_PROFILES + p];
             const uint32_t o2 = o | ((((1u << size) - 1u) << st) & 0xFFu);
             wv[j >> 2] = (wv[j >> 2] & ~(0xFFu << sh)) | (o2 << sh);
@@ -871,19 +861,13 @@ __global__ void __launch_bounds__(kFewThreads, 1) k_few(DevProfiles prof, uint32
 }
 
 // ---------------------------------------------------------------------------------------------
-// k_commit: one thread per logged decision.  Writes the result record of the request (the fields of
-// AllocationDetails the allocator decides) and ORs the slot mask into the packed occupancy word.
-// Distinct decisions on one GPU have disjoint masks (the chain only accepts free masks): no double
-// booking; the atomics only serialise neighbours that share a 32-bit word.
+// k_commit: one thread per logged decision: the result record of its request (the fields of
+// AllocationDetails the allocator decides) and the slot mask ORed into the packed occupancy word.
 // ---------------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(256) k_commit(const Ctrl* __restrict__ ctrl, const uint2* __restrict__ log, const uint32_t* __restrict__ cand,
                                                  uint32_t* __restrict__ occ32, uint2* __restrict__ out_chunk, uint32_t flip) {
     const uint32_t j = blockIdx.x * blockDim.x + threadIdx.x;
-    if (j >= ctrl->n_log) return;
-    const uint2 e = log[j];
-    const uint32_t g = cand[e.y] >> 8, mask = e.x & 0xFFu, t = (e.x >> 15) & 0xFFFFu;
-    out_chunk[t] = pack_result(flip_gpu(g, flip), __ffs(mask) - 1, __popc(mask), ISL_ST_PLACED);
-    atomicOr(&occ32[g >> 2], mask << ((g & 3u) * 8u));
+    if (j < ctrl->n_log) commit_decision(log[j], cand, occ32, out_chunk, flip);
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -910,10 +894,7 @@ __global__ void __launch_bounds__(256) k_commit(const Ctrl* __restrict__ ctrl, c
 // ---------------------------------------------------------------------------------------------
 constexpr uint32_t kSegMax = 512;                   // GPUs per (sub-)segment (2 per thread in the local sweep)
 constexpr uint32_t kSubMax = 8;                     // sub-segments one CTA walks per chunk: inventories beyond SMs x 512 GPUs stay on the pipeline
-#ifndef ISL_PIPE_THREADS
-#define ISL_PIPE_THREADS 256
-#endif
-constexpr uint32_t kPipeThreads = ISL_PIPE_THREADS;     // 1 or 2 GPUs per thread in the local sweep
+constexpr uint32_t kPipeThreads = 256;              // 1 or 2 GPUs per thread in the local sweep
 static_assert(kPipeThreads == kSegMax || 2 * kPipeThreads == kSegMax, "sweep layout");
 constexpr uint32_t kLogCap = 8 * kSegMax;           // a GPU accepts at most 8 placements
 constexpr uint32_t kTokStride = 32;                 // uint32 per token: 16 tagged head words inside a GPU; raw heads[16] + flag at [16] across GPUs
@@ -1027,10 +1008,7 @@ __host__ __device__ inline SpecMem spec_mem(unsigned long long* base, uint32_t c
 }
 
 constexpr uint32_t kTraceWords = 12;
-#ifndef ISL_UNROLL
-#define ISL_UNROLL 8
-#endif
-constexpr int kUnroll = ISL_UNROLL;          // decisions per trip of the decision loop
+constexpr int kUnroll = 8;                   // decisions per trip of the decision loop
 __device__ __forceinline__ unsigned long long globaltimer_ns() {
     unsigned long long t;
     asm volatile("mov.u64 %0, %globaltimer;" : "=l"(t));
@@ -1683,7 +1661,7 @@ __global__ void __launch_bounds__(kPipeThreads, 1) k_pipeline(CandTab tab, PipeA
             // instantiation records its cell at certification instead)
             if (!kSpec) stamp_if(tr && lane == 0, tr + 4);
             stamp_if(dbg && lane == 0, dbg + rnd * 8 + 2);
-            constexpr bool kDefer = ISL_DEFER_INF && !kP15;     // see the rare path below
+            constexpr bool kDefer = !kP15;      // the "nothing fits" test runs once per unrolled group, not per decision; see the rare path below
             const uint32_t la_cap = sa_log + 8u * s_cap;
             bool cut = false;
             while (true) {

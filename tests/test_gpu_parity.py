@@ -218,12 +218,23 @@ def test_edge_cases():
     req[3] = (0, 0, E.OP_FREE, 6, 4)         # span beyond slice 7
     req[4] = (0, 0, E.OP_FREE, 0, 0)         # empty span
     req[5] = (0, 5, E.OP_ALLOC, 0, 0)        # 7g.80gb: never places under REF_EXACT (Q1)
-    res = eng.place_batch(req)
-    assert res["status"].tolist() == [E.ST_BAD_PROFILE, E.ST_NOOP, E.ST_BAD_SPAN, E.ST_BAD_SPAN, E.ST_BAD_SPAN, E.ST_NO_CAPACITY]
-    assert (eng.read_occupancy() == 0).all()
     ref = oracle.Fast(node_off, rows)
     ref.load(np.zeros(6, dtype=np.uint8))
-    assert np.array_equal(res, ref.place(req))
+    want = ref.place(req)
+    # every request pre-pass: k_few (default), k_small, k_prepare on the chunk path and in stream mode (free mask)
+    for flags, no_few in ((0, ""), (0, "1"), (E.FLAG_NO_PIPELINE | E.FLAG_NO_SMALL, ""), (E.FLAG_FORCE_PIPELINE, "")):
+        os.environ.pop("ISL_NO_FEW", None)
+        if no_few:
+            os.environ["ISL_NO_FEW"] = "1"
+        try:
+            path = make_engine(node_off, np.zeros(6, dtype=np.uint8), rows, flags=flags)
+            res = path.place_batch(req)
+        finally:
+            os.environ.pop("ISL_NO_FEW", None)
+        assert res["status"].tolist() == [E.ST_BAD_PROFILE, E.ST_NOOP, E.ST_BAD_SPAN, E.ST_BAD_SPAN, E.ST_BAD_SPAN, E.ST_NO_CAPACITY], (flags, no_few)
+        assert (path.read_occupancy() == 0).all(), (flags, no_few)
+        assert np.array_equal(res, want), (flags, no_few)
+        path.close()
     # freeing a span and re-allocating it in the same batch: frees are applied first
     eng.place_batch(W.alloc_requests(np.array([4], dtype=np.uint8)))                    # 4g at gpu0:0-3
     req = np.zeros(2, dtype=E.REQUEST_DTYPE)
