@@ -1123,6 +1123,23 @@ __device__ __noinline__ uint32_t pipeline_skip(uint32_t sa_cand, const uint16_t*
     return kInf;
 }
 
+// A head word of a token is self-validating: a 15-bit tag above its 17 bits of payload (heads <= 65 536).  Inside a GPU the tag is the
+// call's epoch; across GPUs it is the stream id all ranks share, never 0, so that a cleared inbox slot is never valid.
+__device__ __forceinline__ uint32_t token_tag(const PipeArgs& a) { return a.epoch & 0x7FFFu; }
+__device__ __forceinline__ uint32_t xtoken_tag(const PipeArgs& a) { return a.xepoch % 32767u + 1u; }
+__device__ __forceinline__ uint32_t tag_word(uint32_t tag, uint32_t h) { return (tag << 17) | h; }
+
+// Lane p < 16: head h of profile p leaves stage seg for chunk c — the word the next stage polls and, behind the last stage, the heads
+// for the caller and the word in the next rank's inbox
+__device__ __forceinline__ void publish_token(const PipeArgs& a, uint32_t c, uint32_t seg, uint32_t lane, uint32_t h) {
+    const bool last = seg == a.n_seg - 1;
+    uint32_t* tok = a.tokens + ((size_t)c * (a.n_seg + 1) + seg) * kTokStride;
+    uint32_t* peer = last && a.outbox ? a.outbox + (size_t)c * kTokStride : nullptr;
+    st_relaxed_gpu(tok + lane, tag_word(token_tag(a), h));
+    if (last && a.heads_out) a.heads_out[(size_t)c * ISL_MAX_PROFILES + lane] = h;
+    if (peer) st_relaxed_sys(peer + lane, tag_word(xtoken_tag(a), h));
+}
+
 template <int K, bool kP15, bool kSpec>
 __global__ void __launch_bounds__(kPipeThreads, 1) k_pipeline(CandTab tab, PipeArgs a) {
     extern __shared__ __align__(16) uint8_t smem[];
@@ -1359,8 +1376,8 @@ __global__ void __launch_bounds__(kPipeThreads, 1) k_pipeline(CandTab tab, PipeA
         // 3. token of the previous segment
         unsigned long long* tr = a.trace ? a.trace + ((size_t)c * a.n_seg + seg) * kTraceWords : nullptr;
         const size_t tok_chunk = (size_t)c * (a.n_seg + 1);
-        constexpr bool spec = kSpec;        // host: only with one sub-segment per stage (a.spec); a separate instantiation, so that the plain pipeline's code is untouched by the rounds' machinery
-        const SpecMem sm = spec_mem(a.spec_mem, spec ? c : 0);
+        // kSpec (host: only with one sub-segment per stage) is a separate instantiation, so that the plain pipeline's code is untouched by the rounds' machinery
+        const SpecMem sm = spec_mem(a.spec_mem, kSpec ? c : 0);
         // a partitioned inventory tags with the stream id all ranks share
         const uint32_t tage = a.spec_world > 1 ? a.xepoch : a.epoch;
         const unsigned long long tagb = (unsigned long long)((tage & 0xFFFFFFu) << 8) << 32, tagF = tagb | (0xFFull << 32);
@@ -1378,7 +1395,7 @@ __global__ void __launch_bounds__(kPipeThreads, 1) k_pipeline(CandTab tab, PipeA
             if (remote) st_relaxed_sys_u64(a.spec_peer[prev ? a.spec_rank - 1 : a.spec_rank + 1] + (p - a.spec_mem), v);
             else st_relaxed_gpu_u64(p, v);
         };
-        if (spec) {     // round 0: what this stage's occupancy can take, per contention group -> predicted entry heads
+        if (kSpec) {     // round 0: what this stage's occupancy can take, per contention group -> predicted entry heads
             uint16_t* s_mj = reinterpret_cast<uint16_t*>(s_wkey);               // scratch (the windows are staged later): [3][kSpecStride] gathered masses of the stages in front
             if (tid < ISL_MAX_PROFILES) {
                 const bool on = ((active >> tid) & 1u) && s_maxacc[tid] != 0 && cc->qcnt[tid] != 0;
@@ -1460,11 +1477,11 @@ __global__ void __launch_bounds__(kPipeThreads, 1) k_pipeline(CandTab tab, PipeA
             __syncthreads();
         }
         uint32_t rnd = 1;
-        bool c_prev = spec ? gseg == 0 : seg == 0, need_sim = true, idle_break = false;
+        bool c_prev = kSpec ? gseg == 0 : seg == 0, need_sim = true, idle_break = false;
         bool known_exact = gseg == 0;       // everything in front of the stage right in front of me was consistent one round ago: my next entry may be the true one
         if (tid == 0) { s_capst[0] = 0; s_capst[1] = 0; s_capst[2] = 0; s_cap = kLogCap + 1; s_capped = 0; s_wvalid = 0; s_havepred = 0; }
         bool p_final = false; unsigned long long p_word = 0;      // pollers: a certified stage's final record is read once and kept
-        const unsigned long long t_cell = tr && spec ? globaltimer_ns() : 0ull, sims_cell = st_sims;   // spec trace: [0] sweep + prediction done, [2] certified, [7] simulations, [11] rounds
+        const unsigned long long t_cell = tr && kSpec ? globaltimer_ns() : 0ull, sims_cell = st_sims;   // spec trace: [0] sweep + prediction done, [2] certified, [7] simulations, [11] rounds
 #ifdef ISL_SPEC_DBG_STAMPS      // per-round stamps of one cell (tools/spec_trace.py): a debugging build — the extra live pointer around the decision loop slows it
         unsigned long long* dbg = a.spec_dbg && a.spec_dbg_cell == ((c << 16) | seg) ? a.spec_dbg : nullptr;
 #else
@@ -1473,17 +1490,16 @@ __global__ void __launch_bounds__(kPipeThreads, 1) k_pipeline(CandTab tab, PipeA
         while (true) {      // one pass unless the stage speculates
         stamp_if(dbg && tid == 0, dbg + rnd * 8 + 0);
         if (need_sim) {
-        // Inside a GPU a token is self-validating: every head word carries the call's 15-bit epoch tag above its 17 bits of payload
-        // (heads <= 65 536), so there is no separate flag, no fence on the producer side and no second round trip on this side —
-        // lanes 0..15 of warp 0 each poll their own word of the previous segment's token or of the chunk's 'done' record (whichever
-        // is valid first: when both are, they hold the same heads).  Across GPUs (inbox) the flag + system-scope release stays.
+        // Token words are self-validating (token_tag): no separate flag, no fence on the producer side and no second round trip on this
+        // side — lanes 0..15 of warp 0 each poll their own word of the previous segment's token or of the chunk's 'done' record (whichever
+        // is valid first: when both are, they hold the same heads).
         asm volatile("cp.async.wait_group 0;" ::: "memory");       // my share of the chunk's queues has landed (long ago, as a rule)
         if (tid < 32) {     // heads, window sizes and the compact window layout (exclusive scan over the 16 profiles)
             uint32_t h = 0, wn = 0, left = 0;
             bool from_done = false;
-            const uint32_t tag = a.epoch & 0x7FFFu;
+            const uint32_t tag = token_tag(a);
             stamp_if(tr && tid == 0, tr + 0);
-            if (spec) {                 // the predicted (or, at stage 0, the true) token
+            if (kSpec) {                 // the predicted (or, at stage 0, the true) token
                 if (tid < ISL_MAX_PROFILES) h = s_specH[tid];
             } else if (sb > 0) {        // behind the first sub-segment the heads are the ones its chain left
                 if (tid < ISL_MAX_PROFILES) h = s_heads[tid] + s_pop[tid];
@@ -1499,13 +1515,11 @@ __global__ void __launch_bounds__(kPipeThreads, 1) k_pipeline(CandTab tab, PipeA
                     }
                 }
             } else if (a.inbox) {       // first segment of a rank that has a predecessor: the token comes over NVLink
-                // Self-validating words across GPUs as well: every head word carries the low 15 bits of the stream id above its 17 bits of
-                // payload, written with ONE relaxed system-scope store each (4-byte stores are single-copy atomic) — no fence and no flag on
-                // the sender's side, one NVLink write latency per hop instead of fence + flag.  The consumer clears its slot after reading,
-                // so a tag can never be mistaken for one of 32 768 streams ago.  A dead or stuck predecessor must not hang this GPU for
-                // good: the wait traps like wait_ready does.
+                // Every word is written with ONE relaxed system-scope store (4-byte stores are single-copy atomic): no fence and no flag on the
+                // sender's side, one NVLink write latency per hop.  The consumer clears its slot after reading, so a tag can never be mistaken
+                // for one of 32 768 streams ago.  A dead or stuck predecessor must not hang this GPU for good: the wait traps like wait_ready does.
                 uint32_t* slot = const_cast<uint32_t*>(a.inbox) + (size_t)c * kTokStride + (tid & 15u);
-                const uint32_t xtag = a.xepoch % 32767u + 1u;      // never 0: a cleared slot is never valid
+                const uint32_t xtag = xtoken_tag(a);
                 bool ok = tid >= ISL_MAX_PROFILES;
                 const unsigned long long t0 = globaltimer_ns();
                 while (!__all_sync(0xFFFFFFFFu, ok)) {
@@ -1520,7 +1534,7 @@ __global__ void __launch_bounds__(kPipeThreads, 1) k_pipeline(CandTab tab, PipeA
             stamp_if(tr && tid == 0, tr + 1);
             const bool all_done = sb == 0 && __all_sync(0xFFFFFFFFu, from_done || tid >= ISL_MAX_PROFILES);
             if (tid < ISL_MAX_PROFILES) {
-                const uint32_t qc = spec ? s_qc[tid] : cc->qcnt[tid], qo = spec ? s_qo[tid] : cc->qoff[tid];     // re-simulations: no trip to L2
+                const uint32_t qc = kSpec ? s_qc[tid] : cc->qcnt[tid], qo = kSpec ? s_qo[tid] : cc->qoff[tid];     // re-simulations: no trip to L2
                 left = ((active >> tid) & 1u) && qc > h ? qc - h : 0u;
                 wn = min(left, min(s_ncand * s_maxacc[tid], s_nfree / s_minsize[tid]));   // no more pops than that are possible here
                 s_heads[tid] = h; s_pop[tid] = 0;
@@ -1555,7 +1569,7 @@ __global__ void __launch_bounds__(kPipeThreads, 1) k_pipeline(CandTab tab, PipeA
             }
             // nothing placeable is pending any more: tell every later segment at once instead of relaying hop by hop
             const bool idle = __ballot_sync(0xFFFFFFFFu, left != 0) == 0;
-            if (idle && !all_done && !spec && tid < ISL_MAX_PROFILES) st_relaxed_gpu(a.tokens + (tok_chunk + a.n_seg) * kTokStride + tid, (tag << 17) | h);
+            if (idle && !all_done && !kSpec && tid < ISL_MAX_PROFILES) st_relaxed_gpu(a.tokens + (tok_chunk + a.n_seg) * kTokStride + tid, tag_word(tag, h));
             if (tid == 0) {
                 s_idle = idle ? 1u : 0u;
                 if (kSpec) {        // an idle simulation stages nothing: a new layout that was never filled must not be kept by the next one
@@ -1566,7 +1580,7 @@ __global__ void __launch_bounds__(kPipeThreads, 1) k_pipeline(CandTab tab, PipeA
                 // stages in front are wrongly believed to have left over lands here) and would hold up the whole round.  Unless the entry is known
                 // to be the true one, the simulation is cut off at 1.3 x the largest complete one so far; a cut-off round publishes the exit
                 // extrapolated from the last complete simulation instead (what the stages behind would assume anyway).
-                s_cap = spec && s_capst[1] && !known_exact ? min(kLogCap + 1, ((s_capst[0] * 21u) >> 4) + 64u) : kLogCap + 1;
+                s_cap = kSpec && s_capst[1] && !known_exact ? min(kLogCap + 1, ((s_capst[0] * 21u) >> 4) + 64u) : kLogCap + 1;
                 s_capped = 0;
             }
             uint32_t incl = wn + kWinPad;                       // INF sentinels close every window
@@ -1577,18 +1591,10 @@ __global__ void __launch_bounds__(kPipeThreads, 1) k_pipeline(CandTab tab, PipeA
         __syncthreads();
         stamp_if(tr && tid == 0, tr + 8);
         stamp_if(dbg && tid == 0, dbg + rnd * 8 + 1);
-        if (s_idle && spec) { if (tid == 0) { s_nlog = 0; spec_steps = 0; spec_visited = 0; } }      // nothing pending at these heads: the exit equals the entry
+        if (s_idle && kSpec) { if (tid == 0) { s_nlog = 0; spec_steps = 0; spec_visited = 0; } }      // nothing pending at these heads: the exit equals the entry
         else if (s_idle) {  // pass-through: the token (unchanged heads) still reaches the next rank / the caller from the last segment
             if (warp == 0) {
-                const bool last = seg == a.n_seg - 1;
-                uint32_t* tok = a.tokens + (tok_chunk + seg) * kTokStride;
-                uint32_t* peer = last && a.outbox ? a.outbox + (size_t)c * kTokStride : nullptr;
-                if (lane < ISL_MAX_PROFILES) {
-                    const uint32_t h = s_heads[lane];
-                    st_relaxed_gpu(tok + lane, ((a.epoch & 0x7FFFu) << 17) | h);
-                    if (last && a.heads_out) a.heads_out[(size_t)c * ISL_MAX_PROFILES + lane] = h;
-                    if (peer) st_relaxed_sys(peer + lane, ((a.xepoch % 32767u + 1u) << 17) | h);
-                }
+                if (lane < ISL_MAX_PROFILES) publish_token(a, c, seg, lane, s_heads[lane]);
                 __syncwarp();
                 if (lane == 0) {
                     if (tr) { tr[2] = globaltimer_ns(); tr[3] = tr[2]; }
@@ -1752,21 +1758,13 @@ __global__ void __launch_bounds__(kPipeThreads, 1) k_pipeline(CandTab tab, PipeA
             store_if(tr && lane == 0, tr + 6, nlog);
             store_if(tr && lane == 0, tr + 7, (st_jumps - jumps0) | ((unsigned long long)(((ca - sa_cand) >> 2) - 2) << 32));
             }
-            if (!spec) { st_steps += nlog; st_visited += ((ca - sa_cand) >> 2) - 2; }
+            if (!kSpec) { st_steps += nlog; st_visited += ((ca - sa_cand) >> 2) - 2; }
             else { spec_steps = nlog; spec_visited = ((ca - sa_cand) >> 2) - 2; ++st_sims; }
 #pragma unroll
             for (int k = 0; k < K; ++k) if (reports[k]) s_pop[cprof[k]] = min((wa[k] - wa0[k] - 12) >> 2, s_wn[cprof[k]]);
             __syncwarp();
-            // 5. token for the next segment: heads first, then the flag (release) — behind the stage's last sub-segment
-            uint32_t* tok = a.tokens + (tok_chunk + seg) * kTokStride;
-            const bool last = seg == a.n_seg - 1;
-            uint32_t* peer = last && a.outbox ? a.outbox + (size_t)c * kTokStride : nullptr;
-            if (last_sub && lane < ISL_MAX_PROFILES && !spec) {
-                const uint32_t h = s_heads[lane] + s_pop[lane];
-                st_relaxed_gpu(tok + lane, ((a.epoch & 0x7FFFu) << 17) | h);       // the next segment starts
-                if (last && a.heads_out) a.heads_out[(size_t)c * ISL_MAX_PROFILES + lane] = h;
-                if (peer) st_relaxed_sys(peer + lane, ((a.xepoch % 32767u + 1u) << 17) | h);
-            }
+            // 5. token for the next segment (it starts), behind the stage's last sub-segment
+            if (last_sub && lane < ISL_MAX_PROFILES && !kSpec) publish_token(a, c, seg, lane, s_heads[lane] + s_pop[lane]);
             __syncwarp();
             if (lane == 0) {
                 s_nlog = nlog;
@@ -1774,7 +1772,7 @@ __global__ void __launch_bounds__(kPipeThreads, 1) k_pipeline(CandTab tab, PipeA
                 if (tr) tr[2] = globaltimer_ns();
             }
         }
-        else if (spec && tid == kPipeThreads - 32 && rnd >= 3 && gseg + 1 < gtot) {
+        else if (kSpec && tid == kPipeThreads - 32 && rnd >= 3 && gseg + 1 < gtot) {
             // in the shadow of the chain: the slot of round rnd - 2 is about to be overwritten — the successor must have read it (it has, as a rule)
             const unsigned long long t0 = globaltimer_ns();
             uint32_t spins = 0;
@@ -1787,7 +1785,7 @@ __global__ void __launch_bounds__(kPipeThreads, 1) k_pipeline(CandTab tab, PipeA
         }   // !s_idle
         __syncthreads();
         }   // need_sim
-        if (!spec) break;
+        if (!kSpec) break;
         {   // ---- the round's exchange: publish exit heads and consumed masses, read the predecessor's exit and every earlier stage's masses
             const unsigned long long tagr = tagb | ((unsigned long long)rnd << 32);
             if (tid < 32) {
