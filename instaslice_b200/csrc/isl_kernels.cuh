@@ -873,23 +873,20 @@ __global__ void __launch_bounds__(256) k_commit(const Ctrl* __restrict__ ctrl, c
 // ---------------------------------------------------------------------------------------------
 // k_pipeline<K>: the segment pipeline for STREAMS of batches (BASELINE config 4's shape).
 //
-// The commit chain of one chunk is sequential, but chunks of a stream pipeline exactly over
-// inventory segments: segment s may work on chunk c+1 while segment s+1 is still on chunk c, because
-//   * inside a segment everything happens in stream order: allocs of chunk c, then the frees of the
-//     next batch, then its allocs (occupancy of the segment lives in this CTA's shared memory), and
-//   * the only state that crosses a segment boundary is the per-profile queue-head token (16 counters).
+// The commit chain of one chunk is sequential, but chunks of a stream pipeline exactly over inventory segments: segment s may work on
+// chunk c+1 while segment s+1 is still on chunk c, because inside a segment everything happens in stream order (occupancy of the
+// segment lives in this CTA's shared memory), and the only state that crosses a segment boundary is the per-profile queue-head token.
 // One persistent CTA per segment (cooperative launch, all co-resident; one CTA fills an SM's shared memory).  Per chunk a CTA
-//   0. has the chunk's queues (uint16 request indices) copied into shared memory by cp.async, issued when the previous
-//      chunk's chain ended: they do not depend on the token
-//   1. applies the batch's frees that fall into its range                      (all threads)
-//   2. sweeps its occupancy bytes into an ordered candidate list               (all threads, before the token arrives)
-//   3. waits for the token of segment s-1 (self-validating words: epoch tag + head, polled by 16 lanes), converts the queue
-//      windows it may pop into ready-made 32-bit keys (shared -> shared)
-//   4. runs the decision chain on its candidates                               (warp 0; DESIGN.md 4.1)
-//   5. publishes the token for segment s+1 and only then
-//   6. commits the logged decisions: result records + occupancy bits           (all threads)
-// Host-buffer streams: the batches are fed by a second stream while this kernel runs (ready flags), an extra CTA delivers
-// finished chunks into the caller's pinned result array (done counters).
+//   0. has the chunk's queues copied into shared memory by cp.async when the previous chunk's chain ended      queue_load_async
+//   1. applies the batch's frees that fall into its range                                                       apply_frees
+//   2. sweeps its occupancy bytes into an ordered candidate list, before the token arrives                     sweep_subsegment
+//   3. takes its entry heads: the token of segment s-1 (self-validating words: epoch tag + head, polled by 16 lanes), or in the
+//      speculative rounds a prediction; converts the queue windows it may pop into ready-made keys     read_entry, stage_windows
+//   4. runs the decision chain on its candidates (warp 0; DESIGN.md 4.1) and                                     decide
+//   5. publishes the token for segment s+1 (speculative rounds: exchanges records until certified)       exchange_round
+//   6. commits the logged decisions: result records + occupancy bits                                            commit_log
+// resolve_plain and resolve_rounds run steps 3-5.  Host-buffer streams: the batches are fed by a second stream while this kernel runs
+// (wait_ready), an extra CTA delivers finished chunks into the caller's pinned result array (deliver_chunks).
 // Results are bit-identical to resolving the batches one after the other.
 // ---------------------------------------------------------------------------------------------
 constexpr uint32_t kSegMax = 512;                   // GPUs per (sub-)segment (2 per thread in the local sweep)
@@ -897,7 +894,7 @@ constexpr uint32_t kSubMax = 8;                     // sub-segments one CTA walk
 constexpr uint32_t kPipeThreads = 256;              // 1 or 2 GPUs per thread in the local sweep
 static_assert(kPipeThreads == kSegMax || 2 * kPipeThreads == kSegMax, "sweep layout");
 constexpr uint32_t kLogCap = 8 * kSegMax;           // a GPU accepts at most 8 placements
-constexpr uint32_t kTokStride = 32;                 // uint32 per token: 16 tagged head words inside a GPU; raw heads[16] + flag at [16] across GPUs
+constexpr uint32_t kTokStride = 32;                 // uint32 per token: 16 tagged head words (token_tag inside a GPU, xtoken_tag across GPUs)
 // shared memory: occupancy bytes | candidate records (+8 sentinels) | decision log (+1 pseudo-decision) | the chunk's queues (uint16) | queue-window keys
 constexpr uint32_t kPipeOffCand = kSegMax * kSubMax;      // occupancy bytes of the whole stage (all its sub-segments)
 constexpr uint32_t kCandPad = 16;                   // INF records behind a segment's candidates: a group of pseudo-decisions may walk that far
@@ -938,7 +935,7 @@ struct PipeArgs {
     Ctrl* stats;
     const uint32_t* heads_in;       // [chunk][16] token entering the first segment (nullptr = zeros)
     uint32_t* heads_out;            // [chunk][16] token leaving the last segment (may be nullptr)
-    // partitioned inventory: the token crosses GPUs through peer-mapped memory (NVLink), system-scope release/acquire
+    // partitioned inventory: the token crosses GPUs through peer-mapped memory (NVLink), one relaxed system-scope store per head word
     const uint32_t* inbox;          // local [chunk][kTokStride] of tagged head words, written by the previous rank's last segment (nullptr = first rank); cleared by the reader
     uint32_t* outbox;               // the next rank's inbox, peer-mapped (nullptr = last rank)
     uint32_t xepoch;                // stream id shared by all ranks
@@ -1140,93 +1137,180 @@ __device__ __forceinline__ void publish_token(const PipeArgs& a, uint32_t c, uin
     if (peer) st_relaxed_sys(peer + lane, tag_word(xtoken_tag(a), h));
 }
 
-template <int K, bool kP15, bool kSpec>
-__global__ void __launch_bounds__(kPipeThreads, 1) k_pipeline(CandTab tab, PipeArgs a) {
-    extern __shared__ __align__(16) uint8_t smem[];
-    uint32_t* s_occ32 = reinterpret_cast<uint32_t*>(smem);                       // kSegMax occupancy bytes
-    uint32_t* s_cand = reinterpret_cast<uint32_t*>(smem + kPipeOffCand);         // records (local gpu << 16 | table tag | occ) + sentinels
-    uint2* s_log = reinterpret_cast<uint2*>(smem + kPipeOffLog);                 // (key, candidate index) per decision
-    __shared__ uint16_t s_feas[kMaxTables * 256];
-    __shared__ uint8_t s_tab[kSegMax * kSubMax];                                 // table of every local GPU
-    __shared__ uint32_t s_heads[ISL_MAX_PROFILES], s_wn[ISL_MAX_PROFILES], s_wbase[ISL_MAX_PROFILES], s_qbeg[ISL_MAX_PROFILES], s_pop[ISL_MAX_PROFILES];
-    __shared__ uint32_t s_maxacc[ISL_MAX_PROFILES], s_minsize[ISL_MAX_PROFILES], s_usable[kMaxTables], s_plist[ISL_MAX_PROFILES], s_nplist;
-    __shared__ uint32_t s_warp[kPipeThreads / 32], s_ncand, s_nfree, s_nlog, s_idle, s_closed;
-    // speculative rounds: predicted entry heads, own / predecessor's exit heads, queue lengths, gathered sums, contention groups
-    __shared__ uint32_t s_specH[ISL_MAX_PROFILES], s_specX[ISL_MAX_PROFILES], s_specXp[ISL_MAX_PROFILES], s_qc[ISL_MAX_PROFILES];
-    __shared__ uint32_t s_acc[4], s_grp_big, s_grp_small, s_specflag, s_bigd[32], s_nbigd, s_dqr[2], s_us[kMaxTables], s_qo[ISL_MAX_PROFILES];
-    __shared__ uint8_t s_smallm[kMaxTables][ISL_MAX_PROFILES];
-    // speculative rounds, bounded simulations: entry / exit heads of the stage's last COMPLETE simulation; {decisions of the largest complete one,
-    // have one, the log in shared memory is a complete simulation of the current entry}; decisions this simulation may take; it was cut off
-    // speculative rounds: the staged key windows outlive a simulation — per profile the queue position of the first staged entry, the number
-    // of staged entries, where the current entry sits inside them; the windows are valid for this chunk; this simulation must stage anew
-    __shared__ uint32_t s_wlo[ISL_MAX_PROFILES], s_wlen[ISL_MAX_PROFILES], s_woff[ISL_MAX_PROFILES], s_wvalid, s_restage;
-    __shared__ uint32_t s_predc, s_predA[ISL_MAX_PROFILES], s_predB[ISL_MAX_PROFILES], s_havepred;
-    __shared__ uint32_t s_Hc[ISL_MAX_PROFILES], s_Xc[ISL_MAX_PROFILES], s_capst[3], s_cap, s_capped;
-    const uint32_t tid = threadIdx.x, lane = tid & 31u, warp = tid >> 5, seg = blockIdx.x;
-    if (seg == a.n_seg) {       // the extra CTA of a host-buffer stream: every chunk all segments have committed goes to the caller's
-                                // (mapped, pinned) result array right away, so the D2H of the results hides behind the rest of the stream
-        __shared__ uint32_t s_stop;
-        for (uint32_t c = 0; c < a.n_chunks; ++c) {
-            if (tid == 0) {
-                uint32_t stop = 0;
-                const unsigned long long t0 = globaltimer_ns();
-                while (ld_acquire_gpu(a.done_cnt + c) < a.n_seg) {
-                    // a closed (or aborted) stream never commits this chunk: ready[batch] holds ~epoch
-                    if (a.ready && ld_acquire_gpu(a.ready + (a.open ? c : a.chunks[c].batch)) == ~a.epoch) { stop = 1; break; }
-                    __nanosleep(256);
-                    if (globaltimer_ns() - t0 > a.wait_ns + 5000000000ull) __trap();
-                }
-                s_stop = stop;
-            }
-            __syncthreads();
-            if (s_stop) break;
-            const ChunkDesc cd = a.chunks[c];
-            const uint2* __restrict__ src = a.out + cd.req_off;
-            uint2* __restrict__ dst = cd.host_out ? cd.host_out : a.host_out + cd.req_off;
-            // 16-byte body between an 8-byte head / tail when source and destination are 16-byte aligned at the same records;
-            // otherwise (a destination that is only 8-byte aligned relative to the staging buffer) plain 8-byte stores
-            const bool same = ((reinterpret_cast<uintptr_t>(src) ^ reinterpret_cast<uintptr_t>(dst)) & 8u) == 0;
-            if (same) {
-                const uint32_t head = min(cd.n, (uint32_t)((reinterpret_cast<uintptr_t>(dst) >> 3) & 1u)), pairs = (cd.n - head) >> 1;
-                if (tid == 0 && head) dst[0] = __ldcg(src);
-                const uint4* __restrict__ s4 = reinterpret_cast<const uint4*>(src + head);
-                uint4* __restrict__ d4 = reinterpret_cast<uint4*>(dst + head);
-#pragma unroll 4
-                for (uint32_t i = tid; i < pairs; i += kPipeThreads) d4[i] = __ldcg(s4 + i);
-                if (tid == 0 && ((cd.n - head) & 1u)) dst[cd.n - 1] = __ldcg(src + cd.n - 1);
-            } else {
-#pragma unroll 4
-                for (uint32_t i = tid; i < cd.n; i += kPipeThreads) dst[i] = __ldcg(src + i);
-            }
-            if (a.host_done) {          // the host may read the chunk's results as soon as it sees this word
-                __threadfence_system();
-                __syncthreads();
-                if (tid == 0) st_release_sys(a.host_done + c, a.epoch);
-            }
-        }
-        __threadfence_system();
-        return;
+// The one bounded wait of the pipeline: polls until poll() holds, sleeping sleep_ns between polls (0: spin).  A wait that starves for
+// deadline_ns (from t0) traps instead of hanging the GPU; the clock is read every 256th poll only.  A __trap ends the whole grid, so every
+// chain of stages that wait on each other ends in such a wait: the in-GPU token poll (read_entry) has no deadline of its own.
+template <typename Poll>
+__device__ __forceinline__ void wait_until(Poll poll, unsigned long long deadline_ns, uint32_t sleep_ns, unsigned long long t0 = globaltimer_ns()) {
+    for (uint32_t n = 1; !poll(); ++n) {
+        if (sleep_ns) __nanosleep(sleep_ns);
+        if ((n & 255u) == 0 && globaltimer_ns() - t0 > deadline_ns) __trap();
     }
-    const uint32_t lo_s = min(a.hi, a.lo + seg * a.seg), hi_s = min(a.hi, lo_s + a.seg), n_g = hi_s - lo_s;
-    const uint32_t sa_cand = (uint32_t)__cvta_generic_to_shared(s_cand), sa_log = (uint32_t)__cvta_generic_to_shared(s_log);
-    const uint32_t sa_q = (uint32_t)__cvta_generic_to_shared(smem + kPipeOffQ);     // the chunk's queues: uint16 in-chunk request indices
-    uint32_t* s_wkey = reinterpret_cast<uint32_t*>(smem + kPipeOffWin);          // per-profile windows of ready-made keys t<<15 | p<<11
-    const uint32_t sa_wkey = (uint32_t)__cvta_generic_to_shared(s_wkey);
+}
 
-    for (uint32_t i = tid; i < kSegMax * kSubMax / 4; i += kPipeThreads) s_occ32[i] = 0xFFFFFFFFu;
-    for (uint32_t i = tid; i < kMaxTables * 256; i += kPipeThreads) s_feas[i] = a.feas[i];
-    for (uint32_t i = tid; i < kSegMax * kSubMax; i += kPipeThreads) s_tab[i] = i < n_g ? a.gtab[lo_s + i] & (kMaxTables - 1) : 0;
+// A stage's shared state beside the dynamic buffers (kPipeSmem).  The plain instantiations never touch SpecShared: it takes no shared
+// memory there.
+struct PipeShared {
+    uint16_t feas[kMaxTables * 256];
+    uint8_t tab[kSegMax * kSubMax];                 // table of every local GPU
+    uint32_t heads[ISL_MAX_PROFILES], wn[ISL_MAX_PROFILES], wbase[ISL_MAX_PROFILES], qbeg[ISL_MAX_PROFILES], pop[ISL_MAX_PROFILES];
+    uint32_t maxacc[ISL_MAX_PROFILES], minsize[ISL_MAX_PROFILES], usable[kMaxTables], plist[ISL_MAX_PROFILES], nplist;
+    uint32_t warp[kPipeThreads / 32], ncand, nfree, nlog, idle, closed, cap;
+};
+struct SpecShared {
+    // predicted entry heads, own / predecessor's exit heads, queue lengths and offsets, gathered sums, contention groups
+    uint32_t specH[ISL_MAX_PROFILES], specX[ISL_MAX_PROFILES], specXp[ISL_MAX_PROFILES], qc[ISL_MAX_PROFILES], qo[ISL_MAX_PROFILES];
+    uint32_t acc[4], grp_big, grp_small, specflag, bigd[32], nbigd, dqr[2], us[kMaxTables];
+    uint8_t smallm[kMaxTables][ISL_MAX_PROFILES];
+    // staged key windows outlive a simulation: per profile the first staged queue position, the staged entries, the entry's place among them
+    uint32_t wlo[ISL_MAX_PROFILES], wlen[ISL_MAX_PROFILES], woff[ISL_MAX_PROFILES], wvalid, restage;
+    // the c bit of the stage right in front; both correction rules' candidates of the previous round (Newton step, plain chaining)
+    uint32_t predc, predA[ISL_MAX_PROFILES], predB[ISL_MAX_PROFILES], havepred;
+    // bounded simulations: entry / exit heads of the last COMPLETE simulation; {decisions of the largest complete one, have one, the log
+    // in shared memory is a complete simulation of the current entry}; this simulation was cut off
+    uint32_t Hc[ISL_MAX_PROFILES], Xc[ISL_MAX_PROFILES], capst[3], capped;
+};
+
+struct Stage {                      // a pipeline stage (CTA): its GPUs and its dynamic shared buffers (kPipeSmem), with their shared addresses
+    uint32_t seg, lo, n_g, sa_cand, sa_log, sa_q, sa_wkey;
+    uint32_t *occ32, *cand, *wkey;  // occupancy bytes of all sub-segments; records (local gpu << 16 | table tag | occ) + sentinels; key windows
+    uint2* log;                     // (key, candidate index) per decision
+    const uint16_t* q;              // the chunk's queues: uint16 in-chunk request indices
+};
+struct PipeCounters { unsigned long long steps, jumps, visited, sims, rounds_sum, cells, spec_steps, spec_visited; };
+template <int K>
+struct ChainSlots {                 // chain-warp constants: one (profile, start) candidate per slot
+    uint32_t cmask[K], klow[K], cprof[K];
+    bool valid[K], reports[K];
+    __device__ __forceinline__ ChainSlots(const CandTab& tab, uint32_t lane) {
+#pragma unroll
+        for (int k = 0; k < K; ++k) {
+            const uint32_t d = tab.desc[k][lane];
+            valid[k] = d >> 31;
+            cprof[k] = d & 15u;
+            cmask[k] = valid[k] ? ((d >> 16) & 0xFFu) | (1u << (8 + ((d >> 24) & 7u))) : 0xFFFFu;   // slot mask + own-table bit
+            klow[k] = (((d >> 4) & 7u) << 8) | (cmask[k] & 0xFFu);            // order-in-row and slot mask; t and profile come from the window key
+            reports[k] = valid[k] && ((d >> 4) & 7u) == 0;
+        }
+    }
+};
+struct Rounds {                     // one speculative cell's way through the rounds
+    SpecMem sm;
+    unsigned long long tagb, tagF, p_word, t_cell, sims_cell;     // spec trace: [0] sweep + prediction done, [7] simulations
+    uint32_t tage, gseg, gtot, rnd;                               // gseg: my place in the sequence of all stages of all ranks
+    bool c_prev, need_sim, known_exact, p_final;                  // p_final: the pollers' certified stage's final record is kept in p_word
+};
+
+// Record words of the rounds: a partitioned inventory reads and writes them at system scope
+__device__ __forceinline__ unsigned long long spec_ld(const PipeArgs& a, const unsigned long long* p) { return a.spec_world > 1 ? ld_relaxed_sys_u64(p) : ld_relaxed_gpu_u64(p); }
+// a word every LATER stage reads: my copy and the copies of the ranks behind me
+__device__ __forceinline__ void spec_pub_down(const PipeArgs& a, unsigned long long* p, unsigned long long v) {
+    st_relaxed_gpu_u64(p, v);
+    if (a.spec_world > 1) for (uint32_t r = a.spec_rank + 1; r < a.spec_world; ++r) st_relaxed_sys_u64(a.spec_peer[r] + (p - a.spec_mem), v);
+}
+// a word only the next (prev = false) / the previous (prev = true) stage reads
+__device__ __forceinline__ void spec_pub_nb(const PipeArgs& a, uint32_t seg, unsigned long long* p, unsigned long long v, bool prev) {
+    const bool remote = a.spec_world > 1 && (prev ? (seg == 0 && a.spec_rank > 0) : (seg + 1 == a.n_seg && a.spec_rank + 1 < a.spec_world));
+    if (remote) st_relaxed_sys_u64(a.spec_peer[prev ? a.spec_rank - 1 : a.spec_rank + 1] + (p - a.spec_mem), v);
+    else st_relaxed_gpu_u64(p, v);
+}
+// Round rnd's record at p, or — once its stage is certified — that stage's final record at pf, which stands for every round from then on
+// and is read once
+__device__ __forceinline__ unsigned long long read_record(const PipeArgs& a, const unsigned long long* p, const unsigned long long* pf,
+                                                          unsigned long long tagr, Rounds& r) {
+    if (r.p_final) return r.p_word;
+    unsigned long long w;
+    uint32_t polls = 0;
+    wait_until([&] {
+        w = spec_ld(a, p);
+        if ((w >> 32) == (tagr >> 32)) return true;
+        if ((polls++ & 3u) != 0) return false;
+        w = spec_ld(a, pf);
+        r.p_final = (w >> 32) == (r.tagF >> 32) && ((w >> 24) & 0xFFu) <= r.rnd;
+        return r.p_final;
+    }, a.wait_ns, 0);
+    if (r.p_final) r.p_word = w;
+    return w;
+}
+// The X slot of round rnd - 2 is about to be overwritten: the successor must have read it (it has, as a rule)
+__device__ __forceinline__ void wait_ack(const PipeArgs& a, const Rounds& r) {
+    wait_until([&] { const unsigned long long w = spec_ld(a, r.sm.ack + r.gseg + 1); return (uint32_t)(w >> 32) == r.tage && (uint32_t)w + 2u >= r.rnd; }, a.wait_ns, 0);
+}
+// By warp 0, lane p < 16 for profile p: the masses of per-profile counts v (placements of the big group, slices of the small group),
+// and the heads h moved so that the masses change by dq / dr (spec_spread_warp)
+__device__ __forceinline__ void group_masses(uint32_t v, const PipeShared& s, const SpecShared& ss, uint32_t lane, uint32_t& q, uint32_t& r) {
+    q = __reduce_add_sync(0xFFFFFFFFu, lane < ISL_MAX_PROFILES && ((ss.grp_big >> lane) & 1u) ? v : 0u);
+    r = __reduce_add_sync(0xFFFFFFFFu, lane < ISL_MAX_PROFILES && ((ss.grp_small >> lane) & 1u) ? v * s.minsize[lane] : 0u);
+}
+__device__ __forceinline__ uint32_t shift_groups(uint32_t h, const PipeShared& s, const SpecShared& ss, int dq, int dr, uint32_t lane) {
+    const uint32_t qc = lane < ISL_MAX_PROFILES ? ss.qc[lane] : 0u, w = lane < ISL_MAX_PROFILES ? s.minsize[lane] : 1u;
+    h = spec_spread_warp(h, qc, w, ss.grp_big, dq, false, lane);
+    return spec_spread_warp(h, qc, w, ss.grp_small, dr, true, lane);
+}
+
+// The extra CTA of a host-buffer stream (index n_seg): every chunk all segments have committed goes to the caller's (mapped, pinned)
+// result array right away, so the D2H of the results hides behind the rest of the stream
+__device__ __forceinline__ void deliver_chunks(const PipeArgs& a) {
+    __shared__ uint32_t s_stop;
+    const uint32_t tid = threadIdx.x;
+    for (uint32_t c = 0; c < a.n_chunks; ++c) {
+        if (tid == 0) {
+            uint32_t stop = 0;
+            wait_until([&] {        // 5 s beyond the stages' deadline: a starved stage traps first
+                if (ld_acquire_gpu(a.done_cnt + c) >= a.n_seg) return true;
+                // a closed (or aborted) stream never commits this chunk: ready[batch] holds ~epoch
+                stop = a.ready && ld_acquire_gpu(a.ready + (a.open ? c : a.chunks[c].batch)) == ~a.epoch;
+                return stop != 0;
+            }, a.wait_ns + 5000000000ull, 256);
+            s_stop = stop;
+        }
+        __syncthreads();
+        if (s_stop) break;
+        const ChunkDesc cd = a.chunks[c];
+        const uint2* __restrict__ src = a.out + cd.req_off;
+        uint2* __restrict__ dst = cd.host_out ? cd.host_out : a.host_out + cd.req_off;
+        // 16-byte body between an 8-byte head / tail when source and destination are 16-byte aligned at the same records;
+        // otherwise (a destination that is only 8-byte aligned relative to the staging buffer) plain 8-byte stores
+        const bool same = ((reinterpret_cast<uintptr_t>(src) ^ reinterpret_cast<uintptr_t>(dst)) & 8u) == 0;
+        if (same) {
+            const uint32_t head = min(cd.n, (uint32_t)((reinterpret_cast<uintptr_t>(dst) >> 3) & 1u)), pairs = (cd.n - head) >> 1;
+            if (tid == 0 && head) dst[0] = __ldcg(src);
+            const uint4* __restrict__ s4 = reinterpret_cast<const uint4*>(src + head);
+            uint4* __restrict__ d4 = reinterpret_cast<uint4*>(dst + head);
+#pragma unroll 4
+            for (uint32_t i = tid; i < pairs; i += kPipeThreads) d4[i] = __ldcg(s4 + i);
+            if (tid == 0 && ((cd.n - head) & 1u)) dst[cd.n - 1] = __ldcg(src + cd.n - 1);
+        } else {
+#pragma unroll 4
+            for (uint32_t i = tid; i < cd.n; i += kPipeThreads) dst[i] = __ldcg(src + i);
+        }
+        if (a.host_done) {          // the host may read the chunk's results as soon as it sees this word
+            __threadfence_system();
+            __syncthreads();
+            if (tid == 0) st_release_sys(a.host_done + c, a.epoch);
+        }
+    }
+    __threadfence_system();
+}
+
+// Per-stage constants: feasibility table, table tags, occupancy, what each profile can take and, for the rounds, the contention groups' spans
+template <bool kSpec>
+__device__ __forceinline__ void stage_init(const CandTab& tab, const PipeArgs& a, const Stage& st, PipeShared& s, SpecShared& ss) {
+    const uint32_t tid = threadIdx.x;
+    for (uint32_t i = tid; i < kSegMax * kSubMax / 4; i += kPipeThreads) st.occ32[i] = 0xFFFFFFFFu;
+    for (uint32_t i = tid; i < kMaxTables * 256; i += kPipeThreads) s.feas[i] = a.feas[i];
+    for (uint32_t i = tid; i < kSegMax * kSubMax; i += kPipeThreads) s.tab[i] = i < st.n_g ? a.gtab[st.lo + i] & (kMaxTables - 1) : 0;
     if (tid < ISL_MAX_PROFILES) {
         uint32_t n = 0, sz = 8;
         for (uint32_t k = 0; k < 4; ++k) for (uint32_t l = 0; l < 32; ++l) {
             const uint32_t d = tab.desc[k][l];
             if ((d >> 31) && (d & 15u) == tid) { ++n; sz = min(sz, (uint32_t)__popc((d >> 16) & 0xFFu)); }
         }
-        s_maxacc[tid] = n;
-        s_minsize[tid] = max(sz, 1u);           // smallest span of the profile over all tables
+        s.maxacc[tid] = n;
+        s.minsize[tid] = max(sz, 1u);           // smallest span of the profile over all tables
         const uint32_t have = __ballot_sync(0xFFFFu, n != 0);      // profiles that own at least one candidate: only these get a window
-        if (n) s_plist[__popc(have & ((1u << tid) - 1u))] = tid;
-        if (tid == 0) s_nplist = __popc(have);
+        if (n) s.plist[__popc(have & ((1u << tid) - 1u))] = tid;
+        if (tid == 0) s.nplist = __popc(have);
     }
     if (tid >= 32 && tid < 32 + kMaxTables) {   // slices any candidate of the table can ever cover (REF_EXACT 80GB-class tables: 0x7F)
         uint32_t u = 0;
@@ -1234,7 +1318,7 @@ __global__ void __launch_bounds__(kPipeThreads, 1) k_pipeline(CandTab tab, PipeA
             const uint32_t d = tab.desc[k][l];
             if ((d >> 31) && ((d >> 24) & 7u) == tid - 32) u |= (d >> 16) & 0xFFu;
         }
-        s_usable[tid - 32] = u;
+        s.usable[tid - 32] = u;
     }
     if (kSpec && tid >= 64 && tid < 96) {      // speculative rounds: the (profile, start) candidates of >= 4 slices as a list; per (table, profile) the slices of its smaller spans
         const uint32_t l = tid - 64;
@@ -1243,10 +1327,10 @@ __global__ void __launch_bounds__(kPipeThreads, 1) k_pipeline(CandTab tab, PipeA
             const uint32_t d = tab.desc[k][l];
             const bool big = (d >> 31) && __popc((d >> 16) & 0xFFu) >= 4;
             const uint32_t b = __ballot_sync(0xFFFFFFFFu, big);
-            if (big) { const uint32_t at = n + __popc(b & ((1u << l) - 1u)); if (at < 32) s_bigd[at] = d; }
+            if (big) { const uint32_t at = n + __popc(b & ((1u << l) - 1u)); if (at < 32) ss.bigd[at] = d; }
             n += __popc(b);
         }
-        if (l == 0) s_nbigd = min(n, 32u);
+        if (l == 0) ss.nbigd = min(n, 32u);
         for (uint32_t i = l; i < kMaxTables * ISL_MAX_PROFILES; i += 32) {
             const uint32_t t = i / ISL_MAX_PROFILES, pp = i % ISL_MAX_PROFILES;
             uint32_t u = 0;
@@ -1254,711 +1338,685 @@ __global__ void __launch_bounds__(kPipeThreads, 1) k_pipeline(CandTab tab, PipeA
                 const uint32_t d = tab.desc[k][x];
                 if ((d >> 31) && ((d >> 24) & 7u) == t && (d & 15u) == pp && __popc((d >> 16) & 0xFFu) < 4) u |= (d >> 16) & 0xFFu;
             }
-            s_smallm[t][pp] = (uint8_t)u;
+            ss.smallm[t][pp] = (uint8_t)u;
         }
     }
     __syncthreads();
-    for (uint32_t i = tid; i < n_g; i += kPipeThreads) reinterpret_cast<uint8_t*>(s_occ32)[i] = a.occ[lo_s + i];
+    for (uint32_t i = tid; i < st.n_g; i += kPipeThreads) reinterpret_cast<uint8_t*>(st.occ32)[i] = a.occ[st.lo + i];
     __syncthreads();
+}
 
-    // chain-warp constants: one (profile, start) candidate per slot
-    uint32_t cmask[K], klow[K], cprof[K];
-    bool valid[K], reports[K];
+// The queues of a chunk (k_partition wrote them before this kernel started) are copied into shared memory with cp.async
+// while the segment still waits for the chunk's token: they do not depend on the heads, so nothing is staged on the
+// critical path between 'token in' and the first decision.  Offset -> thread mapping is the same for every chunk, so a
+// thread's own wait_group orders its copies of consecutive chunks.
+__device__ __forceinline__ void queue_load_async(const PipeArgs& a, const Stage& st, uint32_t chunk) {
+    const char* src = reinterpret_cast<const char*>(a.q_all + (size_t)chunk * a.q_stride);
+    const uint32_t bytes = (a.cctl[chunk].qoff[ISL_MAX_PROFILES] * 2u + 15u) & ~15u;
+    for (uint32_t off = threadIdx.x * 16u; off < bytes; off += kPipeThreads * 16u)
+        asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(st.sa_q + off), "l"(src + off) : "memory");
+    asm volatile("cp.async.commit_group;" ::: "memory");
+}
+// Fed streams: the requests of a batch may still be on their way (H2D + pre-pass on the feed stream) when the pipeline gets there.
+// Causal window: chunk c additionally waits until every segment has committed chunk c - window; one deadline covers both waits.
+// Returns true when the stream ends in front of this chunk (an open stream was closed, or the host aborted a feed).
+__device__ __forceinline__ bool wait_ready(const PipeArgs& a, PipeShared& s, uint32_t chunk) {
+    if (!a.ready && !a.window) return false;
+    const bool gate_ring = a.ring_done && !a.inbox;          // ranks behind the owner are gated by the token itself
+    if (threadIdx.x == 0) {
+        bool closed = false;
+        const unsigned long long t0 = globaltimer_ns();
+        if (a.ready) {
+            const uint32_t* f = a.ready + (a.open ? chunk : a.chunks[chunk].batch);
+            // the feed kernels are launched AFTER this one; a tool that serialises kernels would starve the wait (the host side switches
+            // feeding off when it detects one, ISL_NO_FEED=1 forces it) — fail loudly instead of hanging the GPU
+            uint32_t v;
+            wait_until([&] { v = ld_acquire_gpu(f); return v == a.epoch || v == ~a.epoch; }, a.wait_ns, 128, t0);
+            closed = v == ~a.epoch;
+        }
+        if (!closed && a.window && chunk >= a.window) {
+            if (gate_ring) wait_until([&] { return ld_acquire_sys(a.ring_done + chunk - a.window) >= a.world; }, a.wait_ns, 64, t0);
+            else if (!a.ring_done) wait_until([&] { return ld_acquire_gpu(a.done_cnt + chunk - a.window) >= a.n_seg; }, a.wait_ns, 64, t0);
+        }
+        s.closed = closed;
+    }
+    __syncthreads();
+    return s.closed != 0;
+}
+__device__ __forceinline__ void chunk_done(const PipeArgs& a, uint32_t chunk) {     // after the barrier that ends the chunk's commit
+    if (a.done_cnt && threadIdx.x == 0) {
+        if (a.ring_done) __threadfence_system(); else __threadfence();
+        const uint32_t before = atomicAdd(a.done_cnt + chunk, 1u);
+        if (a.ring_done && before + 1 == a.n_seg) atomicAdd_system(a.ring_done + chunk, 1u);     // this rank is through with the chunk
+    }
+}
+
+// 1. frees of this batch inside my range: one byte per GPU
+__device__ __forceinline__ void apply_frees(const PipeArgs& a, const Stage& st, const ChunkDesc& cd) {
+    const uint8_t* fa = a.free_acc + (size_t)cd.batch * a.free_stride + st.lo;
+    for (uint32_t i = threadIdx.x; i < st.n_g; i += kPipeThreads) {
+        const uint32_t f = fa[i];
+        if (f) atomicAnd(&st.occ32[i >> 2], ~(f << ((i & 3u) * 8u)));
+    }
+    __syncthreads();
+}
+
+// 2. local sweep: thread t owns kSegMax / kPipeThreads consecutive local GPUs; ordered compaction.  One scan carries both counts:
+// candidates (low half) and free usable slices on the candidates (high half) — the latter bounds what the segment can accept: a profile
+// of span z pops at most free / z requests here
+__device__ __forceinline__ void sweep_subsegment(const Stage& st, PipeShared& s, uint32_t sb_base, uint32_t n_sb, uint32_t active) {
+    constexpr uint32_t kGpt = kSegMax / kPipeThreads;
+    const uint32_t tid = threadIdx.x, lane = tid & 31u, warp = tid >> 5;
+    uint32_t og[kGpt], tg[kGpt];
+    bool fg[kGpt];
+    uint32_t cnt = 0;
+#pragma unroll
+    for (uint32_t x = 0; x < kGpt; ++x) {
+        const uint32_t g = kGpt * tid + x;
+        og[x] = reinterpret_cast<const uint8_t*>(st.occ32)[sb_base + g]; tg[x] = s.tab[sb_base + g];
+        fg[x] = g < n_sb && (s.feas[tg[x] * 256 + og[x]] & active);
+        if (fg[x]) cnt += 1u | ((uint32_t)__popc(~og[x] & s.usable[tg[x]]) << 16);
+    }
+    uint32_t incl = cnt;
+#pragma unroll
+    for (int d = 1; d < 32; d <<= 1) { const uint32_t t = __shfl_up_sync(0xFFFFFFFFu, incl, d); if ((int)lane >= d) incl += t; }
+    if (lane == 31) s.warp[warp] = incl;
+    __syncthreads();
+    uint32_t off = incl - cnt;
+    for (uint32_t x = 0; x < warp; ++x) off += s.warp[x];
+    const uint32_t nfree = (off + cnt) >> 16;
+    off &= 0xFFFFu;
+#pragma unroll
+    for (uint32_t x = 0; x < kGpt; ++x) if (fg[x]) st.cand[off++] = ((kGpt * tid + x) << 16) | table_tag(tg[x]) | og[x];
+    if (tid == kPipeThreads - 1) { s.ncand = off; s.nfree = nfree; for (uint32_t x = 0; x < kCandPad; ++x) st.cand[off + x] = kInf; }   // sentinels: nothing fits
+    __syncthreads();                    // s.ncand / s.nfree of the sweep are visible to warp 0
+}
+
+// Round 0 of the speculative rounds: what this stage's occupancy can take, per contention group -> predicted entry heads (ss.specH)
+__device__ __forceinline__ void predict_entry(const PipeArgs& a, const Stage& st, PipeShared& s, SpecShared& ss, const Rounds& r,
+                                              uint32_t c, uint32_t active, uint32_t sb_base, uint32_t n_sb) {
+    const uint32_t tid = threadIdx.x, lane = tid & 31u, gseg = r.gseg;
+    const Ctrl* cc = a.cctl + c;
+    uint16_t* s_mj = reinterpret_cast<uint16_t*>(st.wkey);             // scratch (the windows are staged later): [3][kSpecStride] gathered masses of the stages in front
+    if (tid < ISL_MAX_PROFILES) {
+        const bool on = ((active >> tid) & 1u) && s.maxacc[tid] != 0 && cc->qcnt[tid] != 0;
+        ss.qc[tid] = on ? cc->qcnt[tid] : 0u; ss.qo[tid] = cc->qoff[tid];
+        const uint32_t big = __ballot_sync(0xFFFFu, on && s.minsize[tid] >= 4), small = __ballot_sync(0xFFFFu, on && s.minsize[tid] < 4);
+        if (tid == 0) { ss.grp_big = big; ss.grp_small = small; ss.acc[0] = 0; ss.acc[1] = 0; ss.acc[2] = 0; }
+        if (tid < kMaxTables) { uint32_t us = 0; for (uint32_t m = small; m; m &= m - 1) us |= ss.smallm[tid][__ffs(m) - 1]; ss.us[tid] = us; }   // slices the small group can use, per table
+    }
+    __syncthreads();
+    {   // per GPU: the big group takes the widest span that still fits, twice at most (two quads); the small group fills the usable rest
+        constexpr uint32_t kGpt = kSegMax / kPipeThreads;
+        const uint32_t gb = ss.grp_big, nb = ss.nbigd;
+        uint32_t mq = 0, mw = 0, mo = 0;
+#pragma unroll
+        for (uint32_t x = 0; x < kGpt; ++x) {
+            const uint32_t g = kGpt * tid + x;
+            if (g < n_sb) {
+                const uint32_t t = s.tab[sb_base + g], o0 = reinterpret_cast<const uint8_t*>(st.occ32)[sb_base + g], us = ss.us[t];
+                uint32_t o = o0;
+                for (uint32_t it = 0; it < 2; ++it) {
+                    uint32_t best = 0;
+                    for (uint32_t y = 0; y < nb; ++y) {
+                        const uint32_t d = ss.bigd[y], mk = (d >> 16) & 0xFFu;
+                        if (((d >> 24) & 7u) == t && ((gb >> (d & 15u)) & 1u) && (o & mk) == 0 && __popc(mk) > __popc(best)) best = mk;
+                    }
+                    if (!best) break;
+                    o |= best; ++mq;
+                }
+                mw += __popc(~o & us); mo += __popc(~o0 & us);
+            }
+        }
+        mq = __reduce_add_sync(0xFFFFFFFFu, mq); mw = __reduce_add_sync(0xFFFFFFFFu, mw); mo = __reduce_add_sync(0xFFFFFFFFu, mo);
+        if (lane == 0) { atomicAdd(&ss.acc[0], mq); atomicAdd(&ss.acc[1], mw); atomicAdd(&ss.acc[2], mo); }
+    }
+    __syncthreads();
+    if (tid == 0) {
+        spec_pub_down(a, r.sm.m + gseg * 2, r.tagb | ss.acc[0]);
+        spec_pub_down(a, r.sm.m + gseg * 2 + 1, r.tagb | (min(ss.acc[1], 0xFFFFu) << 16) | min(ss.acc[2], 0xFFFFu));
+    }
+    if (tid < gseg) {       // masses of every stage in front of this one
+        unsigned long long w0, w1;
+        wait_until([&] {
+            w0 = spec_ld(a, r.sm.m + tid * 2); w1 = spec_ld(a, r.sm.m + tid * 2 + 1);
+            return (w0 >> 32) == (r.tagb >> 32) && (w1 >> 32) == (r.tagb >> 32);
+        }, a.wait_ns, 0);
+        s_mj[tid] = (uint16_t)w0; s_mj[kSpecStride + tid] = (uint16_t)(w1 >> 16); s_mj[2 * kSpecStride + tid] = (uint16_t)w1;
+    }
+    __syncthreads();
+    if (tid < 32) {         // the big group takes its placements until its queues run dry; the small group fills what is left
+        uint32_t totb = 0, tots = 0;
+        for (uint32_t m = ss.grp_big; m; m &= m - 1) totb += ss.qc[__ffs(m) - 1];
+        for (uint32_t m = ss.grp_small; m; m &= m - 1) { const uint32_t pp = __ffs(m) - 1; tots += ss.qc[pp] * s.minsize[pp]; }
+        constexpr uint32_t kPer = (kSpecStride + 31) / 32;
+        uint32_t ql = 0;
+        for (uint32_t x = 0; x < kPer; ++x) { const uint32_t j = lane * kPer + x; if (j < gseg) ql += s_mj[j]; }
+        uint32_t incl = ql;
+#pragma unroll
+        for (int d = 1; d < 32; d <<= 1) { const uint32_t t = __shfl_up_sync(0xFFFFFFFFu, incl, d); if ((int)lane >= d) incl += t; }
+        uint32_t run = incl - ql, rr = 0;
+        for (uint32_t x = 0; x < kPer; ++x) {
+            const uint32_t j = lane * kPer + x;
+            if (j < gseg) { rr += run < totb ? s_mj[kSpecStride + j] : s_mj[2 * kSpecStride + j]; run += s_mj[j]; }
+        }
+        rr = __reduce_add_sync(0xFFFFFFFFu, rr);
+        const uint32_t Q = min(__shfl_sync(0xFFFFFFFFu, incl, 31), totb), R = min(rr, tots);
+        uint32_t hg = lane < ISL_MAX_PROFILES && gseg == 0 && a.heads_in ? a.heads_in[(size_t)c * ISL_MAX_PROFILES + lane] : 0u;
+        if (gseg > 0) hg = shift_groups(hg, s, ss, (int)Q, (int)R, lane);
+        if (lane < ISL_MAX_PROFILES) ss.specH[lane] = hg;
+    }
+    __syncthreads();
+}
+
+// 3. entry heads (the token, the prediction or what the previous sub-segment left), window sizes and layout, the idle test and the
+// cut-off of a speculative simulation.  Returns true when nothing placeable is pending at these heads.
+template <bool kSpec>
+__device__ __forceinline__ bool read_entry(const PipeArgs& a, const Stage& st, PipeShared& s, SpecShared& ss, uint32_t c, uint32_t sb,
+                                           uint32_t active, bool known_exact, unsigned long long* tr, unsigned long long* dbg, uint32_t rnd) {
+    const uint32_t tid = threadIdx.x, lane = tid & 31u, seg = st.seg;
+    const size_t tok_chunk = (size_t)c * (a.n_seg + 1);
+    asm volatile("cp.async.wait_group 0;" ::: "memory");       // my share of the chunk's queues has landed (long ago, as a rule)
+    if (tid < 32) {
+        uint32_t h = 0, wn = 0, left = 0;
+        bool from_done = false;
+        const uint32_t tag = token_tag(a);
+        stamp_if(tr && tid == 0, tr + 0);
+        if (kSpec) {                 // the predicted (or, at stage 0, the true) token
+            if (tid < ISL_MAX_PROFILES) h = ss.specH[tid];
+        } else if (sb > 0) {        // behind the first sub-segment the heads are the ones its chain left
+            if (tid < ISL_MAX_PROFILES) h = s.heads[tid] + s.pop[tid];
+        } else if (seg > 0) {
+            // Token words are self-validating (token_tag): no separate flag, no fence on the producer side and no second round trip on this
+            // side — lanes 0..15 each poll their own word of the previous segment's token or of the chunk's 'done' record (whichever is
+            // valid first: when both are, they hold the same heads).  This poll is on every token hop and has no deadline: the stage in
+            // front is itself in a wait that traps, or working.
+            const uint32_t* pt = a.tokens + (tok_chunk + seg - 1) * kTokStride + (tid & 15u);
+            const uint32_t* pd = a.tokens + (tok_chunk + a.n_seg) * kTokStride + (tid & 15u);
+            bool ok = tid >= ISL_MAX_PROFILES;
+            while (!__all_sync(0xFFFFFFFFu, ok)) {
+                if (!ok) {
+                    uint32_t v = ld_relaxed_gpu(pt);
+                    if ((v >> 17) == tag) { h = v & 0x1FFFFu; ok = true; }
+                    else { v = ld_relaxed_gpu(pd); if ((v >> 17) == tag) { h = v & 0x1FFFFu; ok = true; from_done = true; } }
+                }
+            }
+        } else if (a.inbox) {       // first segment of a rank that has a predecessor: the token comes over NVLink
+            // Every word is written with ONE relaxed system-scope store (4-byte stores are single-copy atomic): no fence and no flag on the
+            // sender's side, one NVLink write latency per hop.  The consumer clears its slot after reading, so a tag can never be mistaken
+            // for one of 32 768 streams ago.  A dead or stuck predecessor must not hang this GPU for good: the wait traps.
+            uint32_t* slot = const_cast<uint32_t*>(a.inbox) + (size_t)c * kTokStride + (tid & 15u);
+            const uint32_t xtag = xtoken_tag(a);
+            bool ok = tid >= ISL_MAX_PROFILES;
+            wait_until([&] {
+                if (!ok) { const uint32_t v = ld_relaxed_sys(slot); if ((v >> 17) == xtag) { h = v & 0x1FFFFu; ok = true; } }
+                return __all_sync(0xFFFFFFFFu, ok);
+            }, a.wait_ns, 0);
+            if (tid < ISL_MAX_PROFILES) st_relaxed_sys(slot, 0u);
+        } else if (tid < ISL_MAX_PROFILES) h = a.heads_in ? a.heads_in[(size_t)c * ISL_MAX_PROFILES + tid] : 0u;
+        stamp_if(tr && tid == 0, tr + 1);
+        const bool all_done = sb == 0 && __all_sync(0xFFFFFFFFu, from_done || tid >= ISL_MAX_PROFILES);
+        if (tid < ISL_MAX_PROFILES) {
+            const Ctrl* cc = a.cctl + c;
+            const uint32_t qc = kSpec ? ss.qc[tid] : cc->qcnt[tid], qo = kSpec ? ss.qo[tid] : cc->qoff[tid];     // re-simulations: no trip to L2
+            left = ((active >> tid) & 1u) && qc > h ? qc - h : 0u;
+            wn = min(left, min(s.ncand * s.maxacc[tid], s.nfree / s.minsize[tid]));   // no more pops than that are possible here
+            s.heads[tid] = h; s.pop[tid] = 0;
+            if (!kSpec) {
+                s.wn[tid] = wn;
+                s.qbeg[tid] = qo + h;                                       // first pending entry in the shared copy of the queues
+            }
+        }
+        bool win_keep = true;
+        if (kSpec) {
+            // A corrected entry usually sits a few requests from the one simulated before: the windows are staged with kWinMargin entries on
+            // either side and stay for the next simulation when every profile's new window [h, h + wn + 2) lies inside what is staged (real
+            // keys behind the first wn entries are as good as the INF sentinels there: capacity, not the window, ends a profile's pops)
+            uint32_t lo = 0, len = 0, woff = 0;
+            bool ok = true;
+            const uint32_t qc = tid < ISL_MAX_PROFILES ? ss.qc[tid] : 0u;
+            if (tid < ISL_MAX_PROFILES) {
+                lo = ss.wlo[tid]; len = ss.wlen[tid];
+                if (left == 0) woff = len;                                  // nothing pending: straight onto the sentinels
+                else { ok = ss.wvalid && h >= lo && (h + wn + 2 <= lo + len || lo + len >= qc); woff = h - lo; }
+            }
+            win_keep = __all_sync(0xFFFFFFFFu, ok);
+            if (!win_keep && tid < ISL_MAX_PROFILES) {
+                if (left == 0) { lo = h; len = 0; woff = 0; }
+                else { lo = h - min(h, kWinMargin); len = min(qc - lo, (h - lo) + wn + kWinMargin + 2); woff = h - lo; }
+                ss.wlo[tid] = lo; ss.wlen[tid] = len;
+                s.qbeg[tid] = ss.qo[tid] + lo;
+            }
+            if (tid < ISL_MAX_PROFILES) { ss.woff[tid] = woff; s.wn[tid] = len - woff; }     // real entries from the entry to the staged end
+            wn = len;                                                       // the layout below counts the staged entries
+        }
+        // nothing placeable is pending any more: tell every later segment at once instead of relaying hop by hop
+        const bool idle = __ballot_sync(0xFFFFFFFFu, left != 0) == 0;
+        if (idle && !all_done && !kSpec && tid < ISL_MAX_PROFILES) st_relaxed_gpu(a.tokens + (tok_chunk + a.n_seg) * kTokStride + tid, tag_word(tag, h));
+        if (tid == 0) {
+            s.idle = idle ? 1u : 0u;
+            if (kSpec) {        // an idle simulation stages nothing: a new layout that was never filled must not be kept by the next one
+                ss.restage = win_keep ? 0u : 1u;
+                if (!win_keep) ss.wvalid = idle ? 0u : 1u;
+                // A speculative simulation from an entry that is far off can run several times longer than the segment's true work (everything
+                // the stages in front are wrongly believed to have left over lands here) and would hold up the whole round.  Unless the entry
+                // is known to be the true one, the simulation is cut off at 1.3 x the largest complete one so far; a cut-off round publishes
+                // the exit extrapolated from the last complete simulation instead (what the stages behind would assume anyway).
+                s.cap = ss.capst[1] && !known_exact ? min(kLogCap + 1, ((ss.capst[0] * 21u) >> 4) + 64u) : kLogCap + 1;
+                ss.capped = 0;
+            } else s.cap = kLogCap + 1;
+        }
+        uint32_t incl = wn + kWinPad;                       // INF sentinels close every window
+#pragma unroll
+        for (int d = 1; d < 16; d <<= 1) { const uint32_t t = __shfl_up_sync(0xFFFFFFFFu, incl, d); if ((int)lane >= d) incl += t; }
+        if (tid < ISL_MAX_PROFILES) s.wbase[tid] = incl - (wn + kWinPad);
+    }
+    __syncthreads();
+    stamp_if(tr && tid == 0, tr + 8);
+    stamp_if(dbg && tid == 0, dbg + rnd * 8 + 1);
+    return s.idle != 0;
+}
+
+// Windows of ready-made keys t << 15 | profile << 11, each closed by two INF sentinels — converted from the shared copy of the queues
+// (a shared-memory round trip per round instead of an L2 one), only for profiles that own candidates
+template <bool kSpec>
+__device__ __forceinline__ void stage_windows(const Stage& st, PipeShared& s, const SpecShared& ss, unsigned long long* tr) {
+    const uint32_t tid = threadIdx.x;
+    const uint32_t npl = kSpec && !ss.restage ? 0u : s.nplist;
+    for (uint32_t x = 0; x < npl; ++x) {
+        const uint32_t p = s.plist[x], wn = kSpec ? ss.wlen[p] : s.wn[p], pk = p << 11, qb = s.qbeg[p];
+        uint32_t* __restrict__ dst = st.wkey + s.wbase[p];
+        // plain, unconditional (clamped) accesses: the loads of a round overlap instead of queueing behind each other
+        for (uint32_t i = tid; i < wn + kWinPad; i += kPipeThreads) { const uint32_t v = st.q[qb + min(i, wn)]; dst[i] = i < wn ? (v << 15) | pk : kInf; }
+    }
+    stamp_if(tr && tid == 0, tr + 10);
+    store_if(tr && tid == 0, tr + 11, s.wn[s.plist[0]] | ((unsigned long long)s.nfree << 32));
+    __syncthreads();
+    stamp_if(tr && tid == 0, tr + 9);
+}
+
+// 4. the decision chain (see k_chain), tuned for the shortest loop-carried path, and 5. the token for the next segment behind the
+// stage's last sub-segment.  By the chain warp.
+template <int K, bool kP15, bool kSpec>
+__device__ __forceinline__ void decide(const PipeArgs& a, const Stage& st, PipeShared& s, SpecShared& ss, const ChainSlots<K>& cs, PipeCounters& n,
+                                       uint32_t c, bool last_sub, unsigned long long* tr, unsigned long long* dbg, uint32_t rnd) {
+    const uint32_t lane = threadIdx.x & 31u, sa_cand = st.sa_cand, sa_log = st.sa_log;
+    const uint32_t *cmask = cs.cmask, *klow = cs.klow, *cprof = cs.cprof, n_cand = s.ncand;
+    uint32_t tcur[K], tnext[K], tnn[K], wa[K], wa0[K];
+    const uint32_t* wnp[K];         // &s.wn of each slot's profile, formed once: computed next to s.wbase inside the loop it slowed the rounds
 #pragma unroll
     for (int k = 0; k < K; ++k) {
-        const uint32_t d = tab.desc[k][lane];
-        valid[k] = d >> 31;
-        cprof[k] = d & 15u;
-        cmask[k] = valid[k] ? ((d >> 16) & 0xFFu) | (1u << (8 + ((d >> 24) & 7u))) : 0xFFFFu;   // slot mask + own-table bit
-        klow[k] = (((d >> 4) & 7u) << 8) | (cmask[k] & 0xFFu);            // order-in-row and slot mask; t and profile come from the window key
-        reports[k] = valid[k] && ((d >> 4) & 7u) == 0;
+        wa0[k] = st.sa_wkey + 4 * (s.wbase[cprof[k]] + (kSpec ? ss.woff[cprof[k]] : 0u));
+        const bool has = cs.valid[k];
+        tcur[k] = has ? lds_u32(wa0[k]) | klow[k] : kInf;               // INF | anything = INF
+        tnext[k] = has ? lds_u32(wa0[k] + 4) | klow[k] : kInf;
+        wnp[k] = s.wn + cprof[k];
+        const bool two = has && *wnp[k] >= 1;                           // a third entry exists only behind >= 1 real one
+        tnn[k] = two ? lds_u32(wa0[k] + 8) : kInf;
+        wa[k] = wa0[k] + 12;                                            // next entry to load on a pop
     }
-    unsigned long long st_steps = 0, st_jumps = 0, st_visited = 0, st_sims = 0, st_rounds_sum = 0, st_cells = 0, spec_steps = 0, spec_visited = 0;
-
-    // The queues of a chunk (k_partition wrote them before this kernel started) are copied into shared memory with cp.async
-    // while the segment still waits for the chunk's token: they do not depend on the heads, so nothing is staged on the
-    // critical path between 'token in' and the first decision.  Offset -> thread mapping is the same for every chunk, so a
-    // thread's own wait_group orders its copies of consecutive chunks.
-    auto queue_load_async = [&](uint32_t chunk) {
-        const char* src = reinterpret_cast<const char*>(a.q_all + (size_t)chunk * a.q_stride);
-        const uint32_t bytes = (a.cctl[chunk].qoff[ISL_MAX_PROFILES] * 2u + 15u) & ~15u;
-        for (uint32_t off = tid * 16u; off < bytes; off += kPipeThreads * 16u)
-            asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(sa_q + off), "l"(src + off) : "memory");
-        asm volatile("cp.async.commit_group;" ::: "memory");
-    };
-    // fed streams: the requests of a batch may still be on their way (H2D + pre-pass on the feed stream) when the pipeline gets there.
-    // Returns true when the stream ends in front of this chunk (an open stream was closed, or the host aborted a feed).
-    // Causal window: chunk c additionally waits until every segment has committed chunk c - window.
-    auto wait_ready = [&](uint32_t chunk) -> bool {
-        if (!a.ready && !a.window) return false;
-        const bool gate_ring = a.ring_done && !a.inbox;          // ranks behind the owner are gated by the token itself
-        if (tid == 0) {
-            uint32_t closed = 0;
-            const unsigned long long t0 = globaltimer_ns();
-            if (a.ready) {
-                const uint32_t* f = a.ready + (a.open ? chunk : a.chunks[chunk].batch);
-                // the feed kernels are launched AFTER this one; a tool that serialises kernels would starve the wait (the host side switches
-                // feeding off when it detects one, ISL_NO_FEED=1 forces it) — fail loudly instead of hanging the GPU
-                while (true) {
-                    const uint32_t v = ld_acquire_gpu(f);
-                    if (v == a.epoch) break;
-                    if (v == ~a.epoch) { closed = 1; break; }
-                    __nanosleep(128);
-                    if (globaltimer_ns() - t0 > a.wait_ns) __trap();
-                }
-            }
-            if (!closed && a.window && chunk >= a.window) {
-                if (gate_ring) while (ld_acquire_sys(a.ring_done + chunk - a.window) < a.world) { __nanosleep(64); if (globaltimer_ns() - t0 > a.wait_ns) __trap(); }
-                else if (!a.ring_done) while (ld_acquire_gpu(a.done_cnt + chunk - a.window) < a.n_seg) { __nanosleep(64); if (globaltimer_ns() - t0 > a.wait_ns) __trap(); }
-            }
-            s_closed = closed;
-        }
-        __syncthreads();
-        return s_closed != 0;
-    };
-    auto chunk_done = [&](uint32_t chunk) {     // after the barrier that ends the chunk's commit
-        if (a.done_cnt && tid == 0) {
-            if (a.ring_done) __threadfence_system(); else __threadfence();
-            const uint32_t before = atomicAdd(a.done_cnt + chunk, 1u);
-            if (a.ring_done && before + 1 == a.n_seg) atomicAdd_system(a.ring_done + chunk, 1u);     // this rank is through with the chunk
+    uint32_t la = sa_log, ca = sa_cand + 8;                             // ca: shared address of candidate record (current + 2)
+    // Per slot the loop carries conflict words z = occupancy & candidate mask of the current / next / next-but-one candidate GPU
+    // and g = "fits on that GPU ? sel bit : nothing" as a ready OR mask; the key of the NEXT decision is formed at the end of the
+    // body.  Loop-carried path behind the redux: sign mask of `sel` -> bitwise mux of z -> fold the winner's slices in and test
+    // (one LOP3 with a predicate output) -> pick the key: four ALU levels (a freshly updated occupancy register tested through
+    // ISETP / SEL needs five, and ISETP + SEL behind the redux is the slower of the two: tools/microbench_pred.cu times both).
+    // The updates are issued unconditionally and the "nothing fits" test comes LAST: a branch is not speculated, so a test in
+    // front of the updates would put its resolution on the loop-carried path of every decision.  m == INF behaves like a decision
+    // that lands on the next GPU and pops only exhausted lanes (no real key has all-ones t / profile fields unless profile 15
+    // is in use, kP15); the rare path rewinds the cursors and reloads the conflict words after the jump.
+    uint32_t z0[K], z1[K], z2[K], g1[K], g2[K], cm8[K];
+    auto reload_z = [&]() {
+        const uint32_t a0 = lds_u16(ca - 8), a1 = lds_u16(ca - 4), a2 = lds_u16(ca);
+#pragma unroll
+        for (int k = 0; k < K; ++k) {
+            z0[k] = a0 & cmask[k]; z1[k] = a1 & cmask[k]; z2[k] = a2 & cmask[k];
+            g1[k] = z1[k] == 0 ? 0x80000000u : kInf; g2[k] = z2[k] == 0 ? 0x80000000u : kInf;
         }
     };
-    bool closed = wait_ready(0);
-    if (!closed) queue_load_async(0);
-
-    for (uint32_t c = 0; c < a.n_chunks && !closed; ++c) {
-        const ChunkDesc cd = a.chunks[c];
-        const Ctrl* cc = a.cctl + c;
-        if (cd.first_of_batch) {            // 1. frees of this batch inside my range: one byte per GPU
-            const uint8_t* fa = a.free_acc + (size_t)cd.batch * a.free_stride + lo_s;
-            for (uint32_t i = tid; i < n_g; i += kPipeThreads) {
-                const uint32_t f = fa[i];
-                if (f) atomicAnd(&s_occ32[i >> 2], ~(f << ((i & 3u) * 8u)));
-            }
-            __syncthreads();
-        }
-        const uint32_t active = cc->active;
-        // A stage is walked sub-segment by sub-segment (one for inventories up to SMs x 512 GPUs): sweep, heads, windows, chain, commit per
-        // sub-segment; the token is awaited in front of the first and published behind the last one (or as soon as nothing is pending).
-        const uint32_t n_sub = max(1u, (n_g + a.sub - 1) / a.sub);
-        bool prefetched = false;            // the next chunk's queues are on their way (they may only overwrite this chunk's after its last chain)
-        for (uint32_t sb = 0; sb < n_sub; ++sb) {
-        const uint32_t sb_base = sb * a.sub, n_sb = min(a.sub, n_g - min(n_g, sb_base));
-        const bool last_sub = sb + 1 == n_sub;
-        {   // 2. local sweep: thread t owns kSegMax / kPipeThreads consecutive local GPUs; ordered compaction
-            constexpr uint32_t kGpt = kSegMax / kPipeThreads;
-            uint32_t og[kGpt], tg[kGpt];
-            bool fg[kGpt];
-            // one scan carries both counts: candidates (low half) and free usable slices on the candidates (high half) — the latter
-            // bounds what the segment can accept: a profile of span z pops at most free / z requests here
-            uint32_t cnt = 0;
 #pragma unroll
-            for (uint32_t x = 0; x < kGpt; ++x) {
-                const uint32_t g = kGpt * tid + x;
-                og[x] = reinterpret_cast<const uint8_t*>(s_occ32)[sb_base + g]; tg[x] = s_tab[sb_base + g];
-                fg[x] = g < n_sb && (s_feas[tg[x] * 256 + og[x]] & active);
-                if (fg[x]) cnt += 1u | ((uint32_t)__popc(~og[x] & s_usable[tg[x]]) << 16);
-            }
-            uint32_t incl = cnt;
+    for (int k = 0; k < K; ++k) cm8[k] = cmask[k] & 0xFFu;
+    reload_z();
+    uint32_t key = kInf, a2 = lds_u16(ca);
+    auto first_key = [&]() {
+        key = kInf;
 #pragma unroll
-            for (int d = 1; d < 32; d <<= 1) { const uint32_t t = __shfl_up_sync(0xFFFFFFFFu, incl, d); if ((int)lane >= d) incl += t; }
-            if (lane == 31) s_warp[warp] = incl;
-            __syncthreads();
-            uint32_t off = incl - cnt;
-            for (uint32_t x = 0; x < warp; ++x) off += s_warp[x];
-            const uint32_t nfree = (off + cnt) >> 16;
-            off &= 0xFFFFu;
+        for (int k = 0; k < K; ++k) key = min(key, z0[k] == 0 ? tcur[k] : (tcur[k] | g1[k]));
+    };
+    first_key();
+    const unsigned long long jumps0 = n.jumps;
+    // (trace stamps next to the decision loop perturb its schedule in the instantiation with the rounds and slow every round; that
+    // instantiation records its cell at certification instead)
+    if (!kSpec) stamp_if(tr && lane == 0, tr + 4);
+    stamp_if(dbg && lane == 0, dbg + rnd * 8 + 2);
+    constexpr bool kDefer = !kP15;      // the "nothing fits" test runs once per unrolled group, not per decision; see the rare path below
+    const uint32_t la_cap = sa_log + 8u * s.cap;
+    bool cut = false;
+    while (true) {
+        if (!kDefer && la >= la_cap) { cut = true; break; }     // once per group of decisions, off the loop-carried path
+        bool none = false;
+        uint32_t m = 0, mmax = 0;
 #pragma unroll
-            for (uint32_t x = 0; x < kGpt; ++x) if (fg[x]) s_cand[off++] = ((kGpt * tid + x) << 16) | table_tag(tg[x]) | og[x];
-            if (tid == kPipeThreads - 1) { s_ncand = off; s_nfree = nfree; for (uint32_t x = 0; x < kCandPad; ++x) s_cand[off + x] = kInf; }   // sentinels: nothing fits
-        }
-        __syncthreads();                    // s_ncand / s_nfree of the sweep are visible to warp 0
-        // 3. token of the previous segment
-        unsigned long long* tr = a.trace ? a.trace + ((size_t)c * a.n_seg + seg) * kTraceWords : nullptr;
-        const size_t tok_chunk = (size_t)c * (a.n_seg + 1);
-        // kSpec (host: only with one sub-segment per stage) is a separate instantiation, so that the plain pipeline's code is untouched by the rounds' machinery
-        const SpecMem sm = spec_mem(a.spec_mem, kSpec ? c : 0);
-        // a partitioned inventory tags with the stream id all ranks share
-        const uint32_t tage = a.spec_world > 1 ? a.xepoch : a.epoch;
-        const unsigned long long tagb = (unsigned long long)((tage & 0xFFFFFFu) << 8) << 32, tagF = tagb | (0xFFull << 32);
-        const bool xr = a.spec_world > 1;                                  // records cross ranks
-        const uint32_t gseg = a.spec_base + seg, gtot = a.spec_total;      // my place in the sequence of all stages of all ranks
-        auto sld = [&](const unsigned long long* p) { return xr ? ld_relaxed_sys_u64(p) : ld_relaxed_gpu_u64(p); };
-        // a word every LATER stage reads: my copy and the copies of the ranks behind me
-        auto pub_down = [&](unsigned long long* p, unsigned long long v) {
-            st_relaxed_gpu_u64(p, v);
-            if (xr) for (uint32_t r = a.spec_rank + 1; r < a.spec_world; ++r) st_relaxed_sys_u64(a.spec_peer[r] + (p - a.spec_mem), v);
-        };
-        // a word only the next (prev = false) / the previous (prev = true) stage reads
-        auto pub_nb = [&](unsigned long long* p, unsigned long long v, bool prev) {
-            const bool remote = xr && (prev ? (seg == 0 && a.spec_rank > 0) : (seg + 1 == a.n_seg && a.spec_rank + 1 < a.spec_world));
-            if (remote) st_relaxed_sys_u64(a.spec_peer[prev ? a.spec_rank - 1 : a.spec_rank + 1] + (p - a.spec_mem), v);
-            else st_relaxed_gpu_u64(p, v);
-        };
-        if (kSpec) {     // round 0: what this stage's occupancy can take, per contention group -> predicted entry heads
-            uint16_t* s_mj = reinterpret_cast<uint16_t*>(s_wkey);               // scratch (the windows are staged later): [3][kSpecStride] gathered masses of the stages in front
-            if (tid < ISL_MAX_PROFILES) {
-                const bool on = ((active >> tid) & 1u) && s_maxacc[tid] != 0 && cc->qcnt[tid] != 0;
-                s_qc[tid] = on ? cc->qcnt[tid] : 0u; s_qo[tid] = cc->qoff[tid];
-                const uint32_t big = __ballot_sync(0xFFFFu, on && s_minsize[tid] >= 4), small = __ballot_sync(0xFFFFu, on && s_minsize[tid] < 4);
-                if (tid == 0) { s_grp_big = big; s_grp_small = small; s_acc[0] = 0; s_acc[1] = 0; s_acc[2] = 0; }
-                if (tid < kMaxTables) { uint32_t us = 0; for (uint32_t m = small; m; m &= m - 1) us |= s_smallm[tid][__ffs(m) - 1]; s_us[tid] = us; }   // slices the small group can use, per table
-            }
-            __syncthreads();
-            {   // per GPU: the big group takes the widest span that still fits, twice at most (two quads); the small group fills the usable rest
-                constexpr uint32_t kGpt = kSegMax / kPipeThreads;
-                const uint32_t gb = s_grp_big, nb = s_nbigd;
-                uint32_t mq = 0, mw = 0, mo = 0;
+        for (int u = 0; u < kUnroll; ++u) {     // unrolled: one taken branch per kUnroll decisions
+            m = redux_min_u32(key);
 #pragma unroll
-                for (uint32_t x = 0; x < kGpt; ++x) {
-                    const uint32_t g = kGpt * tid + x;
-                    if (g < n_sb) {
-                        const uint32_t t = s_tab[sb_base + g], o0 = reinterpret_cast<const uint8_t*>(s_occ32)[sb_base + g], us = s_us[t];
-                        uint32_t o = o0;
-                        for (uint32_t it = 0; it < 2; ++it) {
-                            uint32_t best = 0;
-                            for (uint32_t y = 0; y < nb; ++y) {
-                                const uint32_t d = s_bigd[y], mk = (d >> 16) & 0xFFu;
-                                if (((d >> 24) & 7u) == t && ((gb >> (d & 15u)) & 1u) && (o & mk) == 0 && __popc(mk) > __popc(best)) best = mk;
-                            }
-                            if (!best) break;
-                            o |= best; ++mq;
-                        }
-                        mw += __popc(~o & us); mo += __popc(~o0 & us);
-                    }
-                }
-                mq = __reduce_add_sync(0xFFFFFFFFu, mq); mw = __reduce_add_sync(0xFFFFFFFFu, mw); mo = __reduce_add_sync(0xFFFFFFFFu, mo);
-                if (lane == 0) { atomicAdd(&s_acc[0], mq); atomicAdd(&s_acc[1], mw); atomicAdd(&s_acc[2], mo); }
+            for (int k = 0; k < K; ++k) {       // in the shadow of the redux: the record fetched by the previous decision (the same one again if it did not advance)
+                z2[k] = a2 & cmask[k];
+                g2[k] = z2[k] == 0 ? 0x80000000u : kInf;
             }
-            __syncthreads();
-            if (tid == 0) {
-                pub_down(sm.m + gseg * 2, tagb | s_acc[0]);
-                pub_down(sm.m + gseg * 2 + 1, tagb | (min(s_acc[1], 0xFFFFu) << 16) | min(s_acc[2], 0xFFFFu));
+            if (kP15) { none = m == kInf; if (none) break; }
+            uint32_t ks;
+            asm("shr.s32 %0, %1, 31;" : "=r"(ks) : "r"(m));                                            // all ones: landed on the next GPU
+            asm("mad.lo.s32 %0, %1, -4, %0;" : "+r"(ca) : "r"(ks));                                     // ca += sel * 4
+            if (kDefer) {       // a pseudo-decision (m == INF: nothing fits here or on the next GPU, move on by one) leaves no log record
+                const bool real = m != kInf;
+                sts_v2_if(lane == 0 && real, la, m, ca);
+                la = add_if(real, la, 8u);
+                mmax = max(mmax, m);
+            } else {
+                sts_v2_if(lane == 0, la, m, ca);                // decision log: (key, address of the record two past the GPU it landed on)
+                la += 8;
             }
-            if (tid < gseg) {       // masses of every stage in front of this one
-                const unsigned long long t0 = globaltimer_ns();
-                unsigned long long w0, w1;
-                uint32_t spins = 0;
-                while (true) {
-                    w0 = sld(sm.m + tid * 2); w1 = sld(sm.m + tid * 2 + 1);
-                    if ((w0 >> 32) == (tagb >> 32) && (w1 >> 32) == (tagb >> 32)) break;
-                    if ((++spins & 255u) == 0 && globaltimer_ns() - t0 > a.wait_ns) __trap();
-                }
-                s_mj[tid] = (uint16_t)w0; s_mj[kSpecStride + tid] = (uint16_t)(w1 >> 16); s_mj[2 * kSpecStride + tid] = (uint16_t)w1;
-            }
-            __syncthreads();
-            if (tid < 32) {         // the big group takes its placements until its queues run dry; the small group fills what is left
-                uint32_t totb = 0, tots = 0;
-                for (uint32_t m = s_grp_big; m; m &= m - 1) totb += s_qc[__ffs(m) - 1];
-                for (uint32_t m = s_grp_small; m; m &= m - 1) { const uint32_t pp = __ffs(m) - 1; tots += s_qc[pp] * s_minsize[pp]; }
-                constexpr uint32_t kPer = (kSpecStride + 31) / 32;
-                uint32_t ql = 0;
-                for (uint32_t x = 0; x < kPer; ++x) { const uint32_t j = lane * kPer + x; if (j < gseg) ql += s_mj[j]; }
-                uint32_t incl = ql;
-#pragma unroll
-                for (int d = 1; d < 32; d <<= 1) { const uint32_t t = __shfl_up_sync(0xFFFFFFFFu, incl, d); if ((int)lane >= d) incl += t; }
-                uint32_t run = incl - ql, r = 0;
-                for (uint32_t x = 0; x < kPer; ++x) {
-                    const uint32_t j = lane * kPer + x;
-                    if (j < gseg) { r += run < totb ? s_mj[kSpecStride + j] : s_mj[2 * kSpecStride + j]; run += s_mj[j]; }
-                }
-                r = __reduce_add_sync(0xFFFFFFFFu, r);
-                const uint32_t Q = min(__shfl_sync(0xFFFFFFFFu, incl, 31), totb), R = min(r, tots);
-                {
-                    const uint32_t qcl = lane < ISL_MAX_PROFILES ? s_qc[lane] : 0u, wl = lane < ISL_MAX_PROFILES ? s_minsize[lane] : 1u;
-                    uint32_t hg = lane < ISL_MAX_PROFILES && gseg == 0 && a.heads_in ? a.heads_in[(size_t)c * ISL_MAX_PROFILES + lane] : 0u;
-                    if (gseg > 0) {
-                        hg = spec_spread_warp(hg, qcl, wl, s_grp_big, (int)Q, false, lane);
-                        hg = spec_spread_warp(hg, qcl, wl, s_grp_small, (int)R, true, lane);
-                    }
-                    if (lane < ISL_MAX_PROFILES) s_specH[lane] = hg;
-                }
-            }
-            __syncthreads();
-        }
-        uint32_t rnd = 1;
-        bool c_prev = kSpec ? gseg == 0 : seg == 0, need_sim = true, idle_break = false;
-        bool known_exact = gseg == 0;       // everything in front of the stage right in front of me was consistent one round ago: my next entry may be the true one
-        if (tid == 0) { s_capst[0] = 0; s_capst[1] = 0; s_capst[2] = 0; s_cap = kLogCap + 1; s_capped = 0; s_wvalid = 0; s_havepred = 0; }
-        bool p_final = false; unsigned long long p_word = 0;      // pollers: a certified stage's final record is read once and kept
-        const unsigned long long t_cell = tr && kSpec ? globaltimer_ns() : 0ull, sims_cell = st_sims;   // spec trace: [0] sweep + prediction done, [2] certified, [7] simulations, [11] rounds
-#ifdef ISL_SPEC_DBG_STAMPS      // per-round stamps of one cell (tools/spec_trace.py): a debugging build — the extra live pointer around the decision loop slows it
-        unsigned long long* dbg = a.spec_dbg && a.spec_dbg_cell == ((c << 16) | seg) ? a.spec_dbg : nullptr;
-#else
-        constexpr unsigned long long* dbg = nullptr;
-#endif
-        while (true) {      // one pass unless the stage speculates
-        stamp_if(dbg && tid == 0, dbg + rnd * 8 + 0);
-        if (need_sim) {
-        // Token words are self-validating (token_tag): no separate flag, no fence on the producer side and no second round trip on this
-        // side — lanes 0..15 of warp 0 each poll their own word of the previous segment's token or of the chunk's 'done' record (whichever
-        // is valid first: when both are, they hold the same heads).
-        asm volatile("cp.async.wait_group 0;" ::: "memory");       // my share of the chunk's queues has landed (long ago, as a rule)
-        if (tid < 32) {     // heads, window sizes and the compact window layout (exclusive scan over the 16 profiles)
-            uint32_t h = 0, wn = 0, left = 0;
-            bool from_done = false;
-            const uint32_t tag = token_tag(a);
-            stamp_if(tr && tid == 0, tr + 0);
-            if (kSpec) {                 // the predicted (or, at stage 0, the true) token
-                if (tid < ISL_MAX_PROFILES) h = s_specH[tid];
-            } else if (sb > 0) {        // behind the first sub-segment the heads are the ones its chain left
-                if (tid < ISL_MAX_PROFILES) h = s_heads[tid] + s_pop[tid];
-            } else if (seg > 0) {
-                const uint32_t* pt = a.tokens + (tok_chunk + seg - 1) * kTokStride + (tid & 15u);
-                const uint32_t* pd = a.tokens + (tok_chunk + a.n_seg) * kTokStride + (tid & 15u);
-                bool ok = tid >= ISL_MAX_PROFILES;
-                while (!__all_sync(0xFFFFFFFFu, ok)) {
-                    if (!ok) {
-                        uint32_t v = ld_relaxed_gpu(pt);
-                        if ((v >> 17) == tag) { h = v & 0x1FFFFu; ok = true; }
-                        else { v = ld_relaxed_gpu(pd); if ((v >> 17) == tag) { h = v & 0x1FFFFu; ok = true; from_done = true; } }
-                    }
-                }
-            } else if (a.inbox) {       // first segment of a rank that has a predecessor: the token comes over NVLink
-                // Every word is written with ONE relaxed system-scope store (4-byte stores are single-copy atomic): no fence and no flag on the
-                // sender's side, one NVLink write latency per hop.  The consumer clears its slot after reading, so a tag can never be mistaken
-                // for one of 32 768 streams ago.  A dead or stuck predecessor must not hang this GPU for good: the wait traps like wait_ready does.
-                uint32_t* slot = const_cast<uint32_t*>(a.inbox) + (size_t)c * kTokStride + (tid & 15u);
-                const uint32_t xtag = xtoken_tag(a);
-                bool ok = tid >= ISL_MAX_PROFILES;
-                const unsigned long long t0 = globaltimer_ns();
-                while (!__all_sync(0xFFFFFFFFu, ok)) {
-                    if (!ok) {
-                        const uint32_t v = ld_relaxed_sys(slot);
-                        if ((v >> 17) == xtag) { h = v & 0x1FFFFu; ok = true; }
-                        else if (globaltimer_ns() - t0 > a.wait_ns) __trap();
-                    }
-                }
-                if (tid < ISL_MAX_PROFILES) st_relaxed_sys(slot, 0u);
-            } else if (tid < ISL_MAX_PROFILES) h = a.heads_in ? a.heads_in[(size_t)c * ISL_MAX_PROFILES + tid] : 0u;
-            stamp_if(tr && tid == 0, tr + 1);
-            const bool all_done = sb == 0 && __all_sync(0xFFFFFFFFu, from_done || tid >= ISL_MAX_PROFILES);
-            if (tid < ISL_MAX_PROFILES) {
-                const uint32_t qc = kSpec ? s_qc[tid] : cc->qcnt[tid], qo = kSpec ? s_qo[tid] : cc->qoff[tid];     // re-simulations: no trip to L2
-                left = ((active >> tid) & 1u) && qc > h ? qc - h : 0u;
-                wn = min(left, min(s_ncand * s_maxacc[tid], s_nfree / s_minsize[tid]));   // no more pops than that are possible here
-                s_heads[tid] = h; s_pop[tid] = 0;
-                if (!kSpec) {
-                    s_wn[tid] = wn;
-                    s_qbeg[tid] = qo + h;                                       // first pending entry in the shared copy of the queues
-                }
-            }
-            bool win_keep = true;
-            if (kSpec) {
-                // A corrected entry usually sits a few requests from the one simulated before: the windows are staged with kWinMargin entries on
-                // either side and stay for the next simulation when every profile's new window [h, h + wn + 2) lies inside what is staged (real
-                // keys behind the first wn entries are as good as the INF sentinels there: capacity, not the window, ends a profile's pops)
-                uint32_t lo = 0, len = 0, woff = 0;
-                bool ok = true;
-                const uint32_t qc = tid < ISL_MAX_PROFILES ? s_qc[tid] : 0u;
-                if (tid < ISL_MAX_PROFILES) {
-                    lo = s_wlo[tid]; len = s_wlen[tid];
-                    if (left == 0) woff = len;                                  // nothing pending: straight onto the sentinels
-                    else { ok = s_wvalid && h >= lo && (h + wn + 2 <= lo + len || lo + len >= qc); woff = h - lo; }
-                }
-                const bool keep = __all_sync(0xFFFFFFFFu, ok) && !(a.spec & 2u);      // (bit 1 of PipeArgs.spec: stage anew every time — a debugging switch, ISL_SPEC_NOREUSE)
-                if (!keep && tid < ISL_MAX_PROFILES) {
-                    if (left == 0) { lo = h; len = 0; woff = 0; }
-                    else { lo = h - min(h, kWinMargin); len = min(qc - lo, (h - lo) + wn + kWinMargin + 2); woff = h - lo; }
-                    s_wlo[tid] = lo; s_wlen[tid] = len;
-                    s_qbeg[tid] = s_qo[tid] + lo;
-                }
-                if (tid < ISL_MAX_PROFILES) { s_woff[tid] = woff; s_wn[tid] = len - woff; }     // real entries from the entry to the staged end
-                win_keep = keep;
-                wn = len;                                                       // the layout below counts the staged entries
-            }
-            // nothing placeable is pending any more: tell every later segment at once instead of relaying hop by hop
-            const bool idle = __ballot_sync(0xFFFFFFFFu, left != 0) == 0;
-            if (idle && !all_done && !kSpec && tid < ISL_MAX_PROFILES) st_relaxed_gpu(a.tokens + (tok_chunk + a.n_seg) * kTokStride + tid, tag_word(tag, h));
-            if (tid == 0) {
-                s_idle = idle ? 1u : 0u;
-                if (kSpec) {        // an idle simulation stages nothing: a new layout that was never filled must not be kept by the next one
-                    s_restage = win_keep ? 0u : 1u;
-                    if (!win_keep) s_wvalid = idle ? 0u : 1u;
-                }
-                // A speculative simulation from an entry that is far off can run several times longer than the segment's true work (everything the
-                // stages in front are wrongly believed to have left over lands here) and would hold up the whole round.  Unless the entry is known
-                // to be the true one, the simulation is cut off at 1.3 x the largest complete one so far; a cut-off round publishes the exit
-                // extrapolated from the last complete simulation instead (what the stages behind would assume anyway).
-                s_cap = kSpec && s_capst[1] && !known_exact ? min(kLogCap + 1, ((s_capst[0] * 21u) >> 4) + 64u) : kLogCap + 1;
-                s_capped = 0;
-            }
-            uint32_t incl = wn + kWinPad;                       // INF sentinels close every window
-#pragma unroll
-            for (int d = 1; d < 16; d <<= 1) { const uint32_t t = __shfl_up_sync(0xFFFFFFFFu, incl, d); if ((int)lane >= d) incl += t; }
-            if (tid < ISL_MAX_PROFILES) s_wbase[tid] = incl - (wn + kWinPad);
-        }
-        __syncthreads();
-        stamp_if(tr && tid == 0, tr + 8);
-        stamp_if(dbg && tid == 0, dbg + rnd * 8 + 1);
-        if (s_idle && kSpec) { if (tid == 0) { s_nlog = 0; spec_steps = 0; spec_visited = 0; } }      // nothing pending at these heads: the exit equals the entry
-        else if (s_idle) {  // pass-through: the token (unchanged heads) still reaches the next rank / the caller from the last segment
-            if (warp == 0) {
-                if (lane < ISL_MAX_PROFILES) publish_token(a, c, seg, lane, s_heads[lane]);
-                __syncwarp();
-                if (lane == 0) {
-                    if (tr) { tr[2] = globaltimer_ns(); tr[3] = tr[2]; }
-                }
-            }
-            __syncthreads();
-            idle_break = true;
-            break;              // the remaining sub-segments have nothing to take either
-        }
-        if (!s_idle) {
-        {   // windows of ready-made keys t << 15 | profile << 11, each closed by two INF sentinels — converted from the shared copy of
-            // the queues (a shared-memory round trip per round instead of an L2 one), only for profiles that own candidates
-            const uint32_t npl = kSpec && !s_restage ? 0u : s_nplist;
-            const uint16_t* __restrict__ sq = reinterpret_cast<const uint16_t*>(smem + kPipeOffQ);
-            for (uint32_t x = 0; x < npl; ++x) {
-                const uint32_t p = s_plist[x], wn = kSpec ? s_wlen[p] : s_wn[p], pk = p << 11, qb = s_qbeg[p];
-                uint32_t* __restrict__ dst = s_wkey + s_wbase[p];
-                // plain, unconditional (clamped) accesses: the loads of a round overlap instead of queueing behind each other
-                for (uint32_t i = tid; i < wn + kWinPad; i += kPipeThreads) { const uint32_t v = sq[qb + min(i, wn)]; dst[i] = i < wn ? (v << 15) | pk : kInf; }
-            }
-            stamp_if(tr && tid == 0, tr + 10);
-            store_if(tr && tid == 0, tr + 11, s_wn[s_plist[0]] | ((unsigned long long)s_nfree << 32));
-        }
-        __syncthreads();
-        stamp_if(tr && tid == 0, tr + 9);
-        if (is_chain_warp(warp)) {          // 4. the decision chain (see k_chain), tuned for the shortest loop-carried path
-            const uint32_t n_cand = s_ncand;
-            uint32_t tcur[K], tnext[K], tnn[K], wa[K], wa0[K];
+            a2 = lds_u16(ca);
+            key = kInf;
 #pragma unroll
             for (int k = 0; k < K; ++k) {
-                wa0[k] = sa_wkey + 4 * (s_wbase[cprof[k]] + (kSpec ? s_woff[cprof[k]] : 0u));
-                const bool has = valid[k];
-                tcur[k] = has ? lds_u32(wa0[k]) | klow[k] : kInf;               // INF | anything = INF
-                tnext[k] = has ? lds_u32(wa0[k] + 4) | klow[k] : kInf;
-                const bool two = has && s_wn[cprof[k]] >= 1;                    // a third entry exists only behind >= 1 real one
-                tnn[k] = two ? lds_u32(wa0[k] + 8) : kInf;
-                wa[k] = wa0[k] + 12;                                            // next entry to load on a pop
+                const bool adv = kP15 ? (((m & 0x7FFFF800u) ^ tcur[k]) & 0xFFFFF800u) == 0 : ((m ^ tcur[k]) & 0x7FFFF800u) == 0;
+                const uint32_t tn = adv ? tnext[k] : tcur[k];
+                uint32_t zs, gn, kk;
+                asm("lop3.b32 %0, %1, %2, %3, 0xca;" : "=r"(zs) : "r"(ks), "r"(z1[k]), "r"(z0[k]));       // sel ? z1 : z0
+                asm("lop3.b32 %0, %1, %2, %3, 0xca;" : "=r"(gn) : "r"(ks), "r"(g2[k]), "r"(g1[k]));       // sel ? g2 : g1
+                asm("{ .reg .pred p; .reg .b32 t; lop3.b32 t, %1, %2, %3, 0xF8; setp.eq.u32 p, t, 0; selp.b32 %0, %4, %5, p; }"
+                    : "=r"(kk) : "r"(zs), "r"(m), "r"(cm8[k]), "r"(tn), "r"(tn | gn));
+                key = min(key, kk);
+                z0[k] = zs | (m & cm8[k]);
+                g1[k] = gn;
+                asm("lop3.b32 %0, %1, %2, %3, 0xca;" : "=r"(z1[k]) : "r"(ks), "r"(z2[k]), "r"(z1[k]));    // sel ? z2 : z1
+                tcur[k] = tn;
+                tnext[k] = adv ? (tnn[k] | klow[k]) : tnext[k];
+                tnn[k] = lds_u32_if(adv, wa[k], tnn[k]);        // consumed at the earliest one pop later
+                wa[k] = add_if(adv, wa[k], 4u);
             }
-            uint32_t la = sa_log, ca = sa_cand + 8;                             // ca: shared address of candidate record (current + 2)
-            // Per slot the loop carries conflict words z = occupancy & candidate mask of the current / next / next-but-one candidate GPU
-            // and g = "fits on that GPU ? sel bit : nothing" as a ready OR mask; the key of the NEXT decision is formed at the end of the
-            // body.  Loop-carried path behind the redux: sign mask of `sel` -> bitwise mux of z -> fold the winner's slices in and test
-            // (one LOP3 with a predicate output) -> pick the key: four ALU levels (a freshly updated occupancy register tested through
-            // ISETP / SEL needs five, and ISETP + SEL behind the redux is the slower of the two: tools/microbench_pred.cu times both).
-            // The updates are issued unconditionally and the "nothing fits" test comes LAST: a branch is not speculated, so a test in
-            // front of the updates would put its resolution on the loop-carried path of every decision.  m == INF behaves like a decision
-            // that lands on the next GPU and pops only exhausted lanes (no real key has all-ones t / profile fields unless profile 15
-            // is in use, kP15); the rare path rewinds the cursors and reloads the conflict words after the jump.
-            uint32_t z0[K], z1[K], z2[K], g1[K], g2[K], cm8[K];
-            auto reload_z = [&]() {
-                const uint32_t a0 = lds_u16(ca - 8), a1 = lds_u16(ca - 4), a2 = lds_u16(ca);
-#pragma unroll
-                for (int k = 0; k < K; ++k) {
-                    z0[k] = a0 & cmask[k]; z1[k] = a1 & cmask[k]; z2[k] = a2 & cmask[k];
-                    g1[k] = z1[k] == 0 ? 0x80000000u : kInf; g2[k] = z2[k] == 0 ? 0x80000000u : kInf;
-                }
-            };
-#pragma unroll
-            for (int k = 0; k < K; ++k) cm8[k] = cmask[k] & 0xFFu;
-            reload_z();
-            uint32_t key = kInf, a2 = lds_u16(ca);
-            auto first_key = [&]() {
-                key = kInf;
-#pragma unroll
-                for (int k = 0; k < K; ++k) key = min(key, z0[k] == 0 ? tcur[k] : (tcur[k] | g1[k]));
-            };
-            first_key();
-            const unsigned long long jumps0 = st_jumps;
-            // (trace stamps next to the decision loop perturb its schedule in the instantiation with the rounds and slow every round; that
-            // instantiation records its cell at certification instead)
-            if (!kSpec) stamp_if(tr && lane == 0, tr + 4);
-            stamp_if(dbg && lane == 0, dbg + rnd * 8 + 2);
-            constexpr bool kDefer = !kP15;      // the "nothing fits" test runs once per unrolled group, not per decision; see the rare path below
-            const uint32_t la_cap = sa_log + 8u * s_cap;
-            bool cut = false;
-            while (true) {
-                if (!kDefer && la >= la_cap) { cut = true; break; }     // once per group of decisions, off the loop-carried path
-                bool none = false;
-                uint32_t m = 0, mmax = 0;
-#pragma unroll
-                for (int u = 0; u < kUnroll; ++u) {     // unrolled: one taken branch per kUnroll decisions
-                    m = redux_min_u32(key);
-#pragma unroll
-                    for (int k = 0; k < K; ++k) {       // in the shadow of the redux: the record fetched by the previous decision (the same one again if it did not advance)
-                        z2[k] = a2 & cmask[k];
-                        g2[k] = z2[k] == 0 ? 0x80000000u : kInf;
-                    }
-                    if (kP15) { none = m == kInf; if (none) break; }
-                    uint32_t ks;
-                    asm("shr.s32 %0, %1, 31;" : "=r"(ks) : "r"(m));                                            // all ones: landed on the next GPU
-                    asm("mad.lo.s32 %0, %1, -4, %0;" : "+r"(ca) : "r"(ks));                                     // ca += sel * 4
-                    if (kDefer) {       // a pseudo-decision (m == INF: nothing fits here or on the next GPU, move on by one) leaves no log record
-                        const bool real = m != kInf;
-                        sts_v2_if(lane == 0 && real, la, m, ca);
-                        la = add_if(real, la, 8u);
-                        mmax = max(mmax, m);
-                    } else {
-                        sts_v2_if(lane == 0, la, m, ca);                // decision log: (key, address of the record two past the GPU it landed on)
-                        la += 8;
-                    }
-                    a2 = lds_u16(ca);
-                    key = kInf;
-#pragma unroll
-                    for (int k = 0; k < K; ++k) {
-                        const bool adv = kP15 ? (((m & 0x7FFFF800u) ^ tcur[k]) & 0xFFFFF800u) == 0 : ((m ^ tcur[k]) & 0x7FFFF800u) == 0;
-                        const uint32_t tn = adv ? tnext[k] : tcur[k];
-                        uint32_t zs, gn, kk;
-                        asm("lop3.b32 %0, %1, %2, %3, 0xca;" : "=r"(zs) : "r"(ks), "r"(z1[k]), "r"(z0[k]));       // sel ? z1 : z0
-                        asm("lop3.b32 %0, %1, %2, %3, 0xca;" : "=r"(gn) : "r"(ks), "r"(g2[k]), "r"(g1[k]));       // sel ? g2 : g1
-                        asm("{ .reg .pred p; .reg .b32 t; lop3.b32 t, %1, %2, %3, 0xF8; setp.eq.u32 p, t, 0; selp.b32 %0, %4, %5, p; }"
-                            : "=r"(kk) : "r"(zs), "r"(m), "r"(cm8[k]), "r"(tn), "r"(tn | gn));
-                        key = min(key, kk);
-                        z0[k] = zs | (m & cm8[k]);
-                        g1[k] = gn;
-                        asm("lop3.b32 %0, %1, %2, %3, 0xca;" : "=r"(z1[k]) : "r"(ks), "r"(z2[k]), "r"(z1[k]));    // sel ? z2 : z1
-                        tcur[k] = tn;
-                        tnext[k] = adv ? (tnn[k] | klow[k]) : tnext[k];
-                        tnn[k] = lds_u32_if(adv, wa[k], tnn[k]);        // consumed at the earliest one pop later
-                        wa[k] = add_if(adv, wa[k], 4u);
-                    }
-                    if (!kP15 && !kDefer) {
-                        none = m == kInf;
-                        if (__builtin_expect(none, 0)) {
-                            ca -= 4; la -= 8;                           // rewind the pseudo-decision
-#pragma unroll
-                            for (int k = 0; k < K; ++k)
-                                if (tcur[k] == kInf) { tnext[k] = kInf; wa[k] -= 4; }
-                            break;
-                        }
-                    }
-                }
-                uint32_t from = (ca - sa_cand) >> 2;        // record index of (current + 2)
-                if (kDefer) {
-                    // m == INF is a legitimate step of the recurrence ("neither this GPU nor the next takes anything: the next one becomes
-                    // current"; it pops only lanes whose window is exhausted, into their INF sentinels), so the loop body needs no exit
-                    // test per decision — one test per group: did ANY decision of the group find nothing?
-                    if (__builtin_expect(mmax != kInf && la < la_cap, 1)) continue;     // (the cut-off test rides on the group's one branch)
-                    if (la >= la_cap) { cut = true; break; }
-                    // exhausted lanes were popped past the end of their windows: back onto the sentinels (at most kUnroll pops since the last time)
+            if (!kP15 && !kDefer) {
+                none = m == kInf;
+                if (__builtin_expect(none, 0)) {
+                    ca -= 4; la -= 8;                           // rewind the pseudo-decision
 #pragma unroll
                     for (int k = 0; k < K; ++k)
-                        if (tcur[k] == kInf) { tnext[k] = kInf; tnn[k] = kInf; wa[k] = wa0[k] + 12 + 4 * s_wn[cprof[k]]; }
-                    if (m != kInf) continue;                // the group ended on a real decision: carry on
-                    from -= 1;                              // the pseudo-decision already moved on by one GPU: the new 'next' is still unexamined
-                } else if (__builtin_expect(!none, 1)) continue;
-                uint32_t alive = 0;
+                        if (tcur[k] == kInf) { tnext[k] = kInf; wa[k] -= 4; }
+                    break;
+                }
+            }
+        }
+        uint32_t from = (ca - sa_cand) >> 2;        // record index of (current + 2)
+        if (kDefer) {
+            // m == INF is a legitimate step of the recurrence ("neither this GPU nor the next takes anything: the next one becomes
+            // current"; it pops only lanes whose window is exhausted, into their INF sentinels), so the loop body needs no exit
+            // test per decision — one test per group: did ANY decision of the group find nothing?
+            if (__builtin_expect(mmax != kInf && la < la_cap, 1)) continue;     // (the cut-off test rides on the group's one branch)
+            if (la >= la_cap) { cut = true; break; }
+            // exhausted lanes were popped past the end of their windows: back onto the sentinels (at most kUnroll pops since the last time)
 #pragma unroll
-                for (int k = 0; k < K; ++k) alive |= tcur[k] != kInf ? 1u << cprof[k] : 0u;
-                const uint32_t j = pipeline_skip(sa_cand, s_feas, n_cand, from, alive, lane);
-                ++st_jumps;
-                if (j == kInf) break;
-                ca = sa_cand + 4 * (j + 2);
-                reload_z();
-                a2 = lds_u16(ca);
-                first_key();
-            }
-            const uint32_t nlog = (la - sa_log) >> 3;
-            if (!kSpec) {
-            stamp_if(tr && lane == 0, tr + 5);
-            stamp_if(dbg && lane == 0, dbg + rnd * 8 + 3);
-            store_if(tr && lane == 0, tr + 6, nlog);
-            store_if(tr && lane == 0, tr + 7, (st_jumps - jumps0) | ((unsigned long long)(((ca - sa_cand) >> 2) - 2) << 32));
-            }
-            if (!kSpec) { st_steps += nlog; st_visited += ((ca - sa_cand) >> 2) - 2; }
-            else { spec_steps = nlog; spec_visited = ((ca - sa_cand) >> 2) - 2; ++st_sims; }
+            for (int k = 0; k < K; ++k)
+                if (tcur[k] == kInf) { tnext[k] = kInf; tnn[k] = kInf; wa[k] = wa0[k] + 12 + 4 * *wnp[k]; }
+            if (m != kInf) continue;                // the group ended on a real decision: carry on
+            from -= 1;                              // the pseudo-decision already moved on by one GPU: the new 'next' is still unexamined
+        } else if (__builtin_expect(!none, 1)) continue;
+        uint32_t alive = 0;
 #pragma unroll
-            for (int k = 0; k < K; ++k) if (reports[k]) s_pop[cprof[k]] = min((wa[k] - wa0[k] - 12) >> 2, s_wn[cprof[k]]);
+        for (int k = 0; k < K; ++k) alive |= tcur[k] != kInf ? 1u << cprof[k] : 0u;
+        const uint32_t j = pipeline_skip(sa_cand, s.feas, n_cand, from, alive, lane);
+        ++n.jumps;
+        if (j == kInf) break;
+        ca = sa_cand + 4 * (j + 2);
+        reload_z();
+        a2 = lds_u16(ca);
+        first_key();
+    }
+    const uint32_t nlog = (la - sa_log) >> 3;
+    if (!kSpec) {
+        stamp_if(tr && lane == 0, tr + 5);
+        stamp_if(dbg && lane == 0, dbg + rnd * 8 + 3);
+        store_if(tr && lane == 0, tr + 6, nlog);
+        store_if(tr && lane == 0, tr + 7, (n.jumps - jumps0) | ((unsigned long long)(((ca - sa_cand) >> 2) - 2) << 32));
+        n.steps += nlog; n.visited += ((ca - sa_cand) >> 2) - 2;
+    } else {
+        n.spec_steps = nlog; n.spec_visited = ((ca - sa_cand) >> 2) - 2; ++n.sims;
+    }
+#pragma unroll
+    for (int k = 0; k < K; ++k) if (cs.reports[k]) s.pop[cprof[k]] = min((wa[k] - wa0[k] - 12) >> 2, *wnp[k]);
+    __syncwarp();
+    if (last_sub && lane < ISL_MAX_PROFILES && !kSpec) publish_token(a, c, st.seg, lane, s.heads[lane] + s.pop[lane]);    // the next segment starts
+    __syncwarp();
+    if (lane == 0) {
+        s.nlog = nlog;
+        if (kSpec) ss.capped = cut ? 1u : 0u;
+        if (tr) tr[2] = globaltimer_ns();
+    }
+}
+
+// The round's exchange: publish exit heads X and consumed masses D, read the predecessor's X and every earlier stage's D, then certify
+// (returns true: the log in shared memory is THE log) or correct the predicted entry for the next round
+__device__ __forceinline__ bool exchange_round(const PipeArgs& a, uint32_t seg, PipeShared& s, SpecShared& ss, Rounds& r, PipeCounters& n,
+                                               uint32_t c, unsigned long long* tr, unsigned long long* dbg) {
+    const uint32_t tid = threadIdx.x, lane = tid & 31u, rnd = r.rnd, gseg = r.gseg;
+    const unsigned long long tagr = r.tagb | ((unsigned long long)rnd << 32);
+    if (tid < 32) {
+        uint32_t X = 0, dq, dr, pop = 0;
+        const bool was_cut = ss.capped != 0;
+        if (tid < ISL_MAX_PROFILES) { pop = s.pop[tid]; X = s.heads[tid] + pop; }
+        if (was_cut) {      // exit of the last complete simulation, moved by what the entry has moved since (per group, shares as always)
+            uint32_t eq, er;
+            group_masses(tid < ISL_MAX_PROFILES ? s.heads[tid] - ss.Hc[tid] : 0u, s, ss, lane, eq, er);
+            const uint32_t xe = shift_groups(tid < ISL_MAX_PROFILES ? ss.Xc[tid] : 0u, s, ss, (int)eq, (int)er, lane);
+            if (tid < ISL_MAX_PROFILES) { X = max(xe, s.heads[tid]); pop = X - s.heads[tid]; }
+        }
+        if (tid < ISL_MAX_PROFILES) { ss.specX[tid] = X; if (!was_cut) { ss.Hc[tid] = s.heads[tid]; ss.Xc[tid] = X; } }
+        if (tid == 0) { if (was_cut) ss.capst[2] = 0; else { ss.capst[0] = max(ss.capst[0], s.nlog); ss.capst[1] = 1; ss.capst[2] = 1; } }
+        group_masses(pop, s, ss, lane, dq, dr);
+        if (rnd >= 3 && gseg + 1 < r.gtot && !(r.need_sim && !s.idle)) wait_ack(a, r);     // (checked behind the chain when one ran)
+        if (tid < ISL_MAX_PROFILES) spec_pub_nb(a, seg, r.sm.x + ((size_t)gseg * 2 + (rnd & 1u)) * 16 + tid, tagr | X, false);
+        if (tid == 16) spec_pub_down(a, r.sm.d + (size_t)rnd * kSpecStride + gseg, tagr | ((r.c_prev ? 1u : 0u) << 31) | (dq << 13) | dr);
+        if (tid == 0) { ss.dqr[0] = dq; ss.dqr[1] = dr; ss.acc[0] = 0; ss.acc[1] = 0; }
+        stamp_if(dbg && tid == 0, dbg + rnd * 8 + 4);
+    }
+    __syncthreads();
+    bool cbit = true;
+    if (tid < gseg) {       // D of every stage in front
+        const unsigned long long w = read_record(a, r.sm.d + (size_t)rnd * kSpecStride + tid, r.sm.df + tid, tagr, r);
+        cbit = r.p_final || ((w >> 31) & 1u);
+        atomicAdd(&ss.acc[0], (uint32_t)(w >> 13) & 0x7FFu);
+        atomicAdd(&ss.acc[1], (uint32_t)w & 0x1FFFu);
+    }
+    if (gseg > 0 && tid >= 192 && tid < 192 + ISL_MAX_PROFILES) {      // X of the stage in front
+        const uint32_t i = tid - 192;
+        ss.specXp[i] = (uint32_t)read_record(a, r.sm.x + ((size_t)(gseg - 1) * 2 + (rnd & 1u)) * 16 + i, r.sm.xf + (size_t)(gseg - 1) * 16 + i, tagr, r) & 0x1FFFFu;
+    }
+    if (tid + 1 == gseg) ss.predc = cbit ? 1u : 0u;         // the bit of the stage right in front of me
+    const int unset = __syncthreads_count(!cbit);
+    const bool allc = unset == 0;
+    // Knowledge lags a round: the stage whose entry becomes the true one NEXT round sits behind a consistent prefix whose last member's
+    // bit is not set yet (that member's own entry became the true one only this round).  So "everything in front but the stage right
+    // in front of me is consistent" already exempts the next simulation from the cut-off — otherwise the frontier itself could be cut
+    // off and every step of it would cost a second round (tests/spec_rounds_model.cpp).
+    const bool near = allc || (unset == 1 && !ss.predc);
+    const bool certified = allc && r.c_prev;
+    stamp_if(dbg && tid == 0, dbg + rnd * 8 + 5);
+    store_if(dbg && tid == 0, dbg + rnd * 8 + 7, s.nlog | ((unsigned long long)r.need_sim << 32));
+    if (gseg > 0 && tid == 192) spec_pub_nb(a, seg, r.sm.ack + gseg, ((unsigned long long)r.tage << 32) | (certified ? 0xFFFFu : rnd), true);
+    if (certified) {    // every entry up to mine was the true token one round ago and has not moved since
+        if (tid < ISL_MAX_PROFILES) {
+            spec_pub_nb(a, seg, r.sm.xf + (size_t)gseg * 16 + tid, r.tagF | (rnd << 24) | ss.specX[tid], false);
+            if (gseg == r.gtot - 1 && a.heads_out) a.heads_out[(size_t)c * ISL_MAX_PROFILES + tid] = ss.specX[tid];
+        }
+        if (tid == 16) spec_pub_down(a, r.sm.df + gseg, r.tagF | (rnd << 24) | (ss.dqr[0] << 13) | ss.dqr[1]);
+        if (tid == 0) {
+            n.steps += n.spec_steps; n.visited += n.spec_visited;
+            if (gseg == r.gtot - 1) { n.rounds_sum += rnd; ++n.cells; }
+            if (tr) { tr[0] = r.t_cell; tr[2] = globaltimer_ns(); tr[6] = s.nlog; tr[7] = n.sims - r.sims_cell; tr[11] = rnd; }
+        }
+        return true;
+    }
+    if (tid < 32) {     // c for the next round; the corrected prediction
+        const bool same = tid >= ISL_MAX_PROFILES || ss.specH[tid] == ss.specXp[tid];
+        const bool cnow = __all_sync(0xFFFFFFFFu, same);
+        const uint32_t hold = tid < ISL_MAX_PROFILES ? ss.specH[tid] : 0u;
+        uint32_t hn = tid < ISL_MAX_PROFILES ? ss.specXp[tid] : 0u, mq, mr;
+        group_masses(hn, s, ss, lane, mq, mr);
+        hn = shift_groups(hn, s, ss, (int)ss.acc[0] - (int)mq, (int)ss.acc[1] - (int)mr, lane);
+        {   // Two candidates for the next entry: the Newton step (hn) and plain chaining (the exit of the stage in front as it is).  Where a
+            // batch's contested front reaches far the Newton step over-corrects round after round; each stage uses the rule whose
+            // candidate of the PREVIOUS round came closer to what the stage in front has published now (study, section 8).
+            const uint32_t xp = tid < ISL_MAX_PROFILES ? ss.specXp[tid] : 0u;
+            uint32_t ea = 0, eb = 0;
+            if (tid < ISL_MAX_PROFILES && ss.havepred) { ea = (uint32_t)abs((int)ss.predA[tid] - (int)xp); eb = (uint32_t)abs((int)ss.predB[tid] - (int)xp); }
+            ea = __reduce_add_sync(0xFFFFFFFFu, ea); eb = __reduce_add_sync(0xFFFFFFFFu, eb);
             __syncwarp();
-            // 5. token for the next segment (it starts), behind the stage's last sub-segment
-            if (last_sub && lane < ISL_MAX_PROFILES && !kSpec) publish_token(a, c, seg, lane, s_heads[lane] + s_pop[lane]);
+            if (tid < ISL_MAX_PROFILES) { ss.predA[tid] = hn; ss.predB[tid] = xp; }
+            if (tid == 0) ss.havepred = 1;
+            if (eb < ea) hn = xp;
+        }
+        if (tid < ISL_MAX_PROFILES) ss.specH[tid] = hn;
+        const bool moved = tid < ISL_MAX_PROFILES && hn != hold;
+        const bool changed = __any_sync(0xFFFFFFFFu, moved);
+        // a cut-off simulation left no usable log: the entry is simulated again (in full once it is known to be the true one) and counts as
+        // inconsistent until then
+        if (tid == 0) ss.specflag = (cnow && ss.capst[2] ? 1u : 0u) | (changed || !ss.capst[2] ? 2u : 0u);
+        stamp_if(dbg && tid == 0, dbg + rnd * 8 + 6);
+    }
+    __syncthreads();
+    r.c_prev = ss.specflag & 1u; r.need_sim = ss.specflag & 2u; r.known_exact = near;
+    if (++r.rnd >= kSpecRounds - 1) __trap();      // cannot happen: every round certifies at least one more stage
+    return false;
+}
+
+// 6. commit: result records + occupancy bits of the logged decisions
+__device__ __forceinline__ void commit_log(const PipeArgs& a, const Stage& st, const PipeShared& s, const ChunkDesc& cd, uint32_t sb_base,
+                                           unsigned long long* tr) {
+    const uint32_t nlog = s.nlog;
+    for (uint32_t j = threadIdx.x; j < nlog; j += kPipeThreads) {
+        const uint2 e = st.log[j];
+        const uint32_t l = sb_base + (st.cand[((e.y - st.sa_cand) >> 2) - 2] >> 16), mask = e.x & 0xFFu, t = (e.x >> 15) & 0xFFFFu;
+        const uint2 rec = pack_result(flip_gpu(st.lo + l, a.flip), __ffs(mask) - 1, __popc(mask), ISL_ST_PLACED);
+        a.out[cd.req_off + t] = rec;
+        if (a.owner_out) a.owner_out[cd.req_off + t] = rec;         // partitioned inventory: straight into the owner rank's result array (peer store over NVLink)
+        atomicOr(&st.occ32[l >> 2], mask << ((l & 3u) * 8u));
+    }
+    __syncthreads();
+    if (tr && threadIdx.x == 0) tr[3] = globaltimer_ns();
+}
+
+// 3.-5. through the plain pipeline.  Returns false when nothing placeable is pending at the entry: the token went on unchanged, and the
+// stage's remaining sub-segments have nothing to take either.
+template <int K, bool kP15>
+__device__ __forceinline__ bool resolve_plain(const PipeArgs& a, const Stage& st, PipeShared& s, SpecShared& ss, const ChainSlots<K>& cs,
+                                              PipeCounters& n, uint32_t c, uint32_t sb, uint32_t active, bool last_sub, unsigned long long* tr) {
+    const uint32_t tid = threadIdx.x, lane = tid & 31u, warp = tid >> 5;
+    if (read_entry<false>(a, st, s, ss, c, sb, active, false, tr, nullptr, 1)) {
+        if (warp == 0) {    // pass-through: the token (unchanged heads) still reaches the next rank / the caller from the last segment
+            if (lane < ISL_MAX_PROFILES) publish_token(a, c, st.seg, lane, s.heads[lane]);
             __syncwarp();
-            if (lane == 0) {
-                s_nlog = nlog;
-                s_capped = cut ? 1u : 0u;
-                if (tr) tr[2] = globaltimer_ns();
-            }
-        }
-        else if (kSpec && tid == kPipeThreads - 32 && rnd >= 3 && gseg + 1 < gtot) {
-            // in the shadow of the chain: the slot of round rnd - 2 is about to be overwritten — the successor must have read it (it has, as a rule)
-            const unsigned long long t0 = globaltimer_ns();
-            uint32_t spins = 0;
-            while (true) {
-                const unsigned long long w = sld(sm.ack + gseg + 1);
-                if ((uint32_t)(w >> 32) == tage && (uint32_t)w + 2u >= rnd) break;
-                if ((++spins & 255u) == 0 && globaltimer_ns() - t0 > a.wait_ns) __trap();
-            }
-        }
-        }   // !s_idle
-        __syncthreads();
-        }   // need_sim
-        if (!kSpec) break;
-        {   // ---- the round's exchange: publish exit heads and consumed masses, read the predecessor's exit and every earlier stage's masses
-            const unsigned long long tagr = tagb | ((unsigned long long)rnd << 32);
-            if (tid < 32) {
-                uint32_t X = 0, dq = 0, dr = 0, pop = 0;
-                const bool was_cut = s_capped != 0;
-                if (tid < ISL_MAX_PROFILES) { pop = s_pop[tid]; X = s_heads[tid] + pop; }
-                if (was_cut) {      // exit of the last complete simulation, moved by what the entry has moved since (per group, shares as always)
-                    int eq = 0, er = 0;
-                    uint32_t xe = 0;
-                    const uint32_t qcl = tid < ISL_MAX_PROFILES ? s_qc[tid] : 0u, wl = tid < ISL_MAX_PROFILES ? s_minsize[tid] : 1u;
-                    if (tid < ISL_MAX_PROFILES) {
-                        const int d = (int)s_heads[tid] - (int)s_Hc[tid];
-                        if ((s_grp_big >> tid) & 1u) eq = d;
-                        if ((s_grp_small >> tid) & 1u) er = d * (int)s_minsize[tid];
-                        xe = s_Xc[tid];
-                    }
-                    eq = __reduce_add_sync(0xFFFFFFFFu, eq); er = __reduce_add_sync(0xFFFFFFFFu, er);
-                    xe = spec_spread_warp(xe, qcl, wl, s_grp_big, eq, false, lane);
-                    xe = spec_spread_warp(xe, qcl, wl, s_grp_small, er, true, lane);
-                    if (tid < ISL_MAX_PROFILES) { X = max(xe, s_heads[tid]); pop = X - s_heads[tid]; }
-                }
-                if (tid < ISL_MAX_PROFILES) {
-                    s_specX[tid] = X;
-                    if (!was_cut) { s_Hc[tid] = s_heads[tid]; s_Xc[tid] = X; }
-                    if ((s_grp_big >> tid) & 1u) dq = pop;
-                    if ((s_grp_small >> tid) & 1u) dr = pop * s_minsize[tid];
-                }
-                if (tid == 0) { if (was_cut) s_capst[2] = 0; else { s_capst[0] = max(s_capst[0], s_nlog); s_capst[1] = 1; s_capst[2] = 1; } }
-                dq = __reduce_add_sync(0xFFFFFFFFu, dq); dr = __reduce_add_sync(0xFFFFFFFFu, dr);
-                if (rnd >= 3 && gseg + 1 < gtot && !(need_sim && !s_idle)) {      // the slot of round rnd - 2 is overwritten: the successor must have read it (checked behind the chain when one ran)
-                    const unsigned long long t0 = globaltimer_ns();
-                    uint32_t spins = 0;
-                    while (true) {
-                        const unsigned long long w = sld(sm.ack + gseg + 1);
-                        if ((uint32_t)(w >> 32) == tage && (uint32_t)w + 2u >= rnd) break;
-                        if ((++spins & 255u) == 0 && globaltimer_ns() - t0 > a.wait_ns) __trap();
-                    }
-                }
-                if (tid < ISL_MAX_PROFILES) pub_nb(sm.x + ((size_t)gseg * 2 + (rnd & 1u)) * 16 + tid, tagr | X, false);
-                if (tid == 16) pub_down(sm.d + (size_t)rnd * kSpecStride + gseg, tagr | ((c_prev ? 1u : 0u) << 31) | (dq << 13) | dr);
-                if (tid == 0) { s_dqr[0] = dq; s_dqr[1] = dr; s_acc[0] = 0; s_acc[1] = 0; }
-                stamp_if(dbg && tid == 0, dbg + rnd * 8 + 4);
-            }
-            __syncthreads();
-            bool cbit = true;
-            if (tid < gseg) {
-                unsigned long long w = p_word;
-                if (!p_final) {
-                    const unsigned long long t0 = globaltimer_ns();
-                    uint32_t spins = 0;
-                    while (true) {
-                        w = sld(sm.d + (size_t)rnd * kSpecStride + tid);
-                        if ((w >> 32) == (tagr >> 32)) { cbit = (w >> 31) & 1u; break; }
-                        if ((spins++ & 3u) == 0) {      // a certified stage no longer publishes rounds: its final record stands for every round from then on
-                            w = sld(sm.df + tid);
-                            if ((w >> 32) == (tagF >> 32) && ((w >> 24) & 0xFFu) <= rnd) { p_final = true; p_word = w; break; }
-                        }
-                        if ((spins & 255u) == 0 && globaltimer_ns() - t0 > a.wait_ns) __trap();
-                    }
-                }
-                atomicAdd(&s_acc[0], (uint32_t)(w >> 13) & 0x7FFu);
-                atomicAdd(&s_acc[1], (uint32_t)w & 0x1FFFu);
-            }
-            if (gseg > 0 && tid >= 192 && tid < 192 + ISL_MAX_PROFILES) {
-                const uint32_t i = tid - 192;
-                unsigned long long w = p_word;
-                if (!p_final) {
-                    const unsigned long long t0 = globaltimer_ns();
-                    uint32_t spins = 0;
-                    while (true) {
-                        w = sld(sm.x + ((size_t)(gseg - 1) * 2 + (rnd & 1u)) * 16 + i);
-                        if ((w >> 32) == (tagr >> 32)) break;
-                        if ((spins++ & 3u) == 0) {
-                            w = sld(sm.xf + (size_t)(gseg - 1) * 16 + i);
-                            if ((w >> 32) == (tagF >> 32) && ((w >> 24) & 0xFFu) <= rnd) { p_final = true; p_word = w; break; }
-                        }
-                        if ((spins & 255u) == 0 && globaltimer_ns() - t0 > a.wait_ns) __trap();
-                    }
-                }
-                s_specXp[i] = (uint32_t)w & 0x1FFFFu;
-            }
-            if (tid + 1 == gseg) s_predc = cbit ? 1u : 0u;         // the bit of the stage right in front of me
-            const int unset = __syncthreads_count(!cbit);
-            const bool allc = unset == 0;
-            // Knowledge lags a round: the stage whose entry becomes the true one NEXT round sits behind a consistent prefix whose last member's
-            // bit is not set yet (that member's own entry became the true one only this round).  So "everything in front but the stage right
-            // in front of me is consistent" already exempts the next simulation from the cut-off — otherwise the frontier itself could be cut
-            // off and every step of it would cost a second round (tests/spec_rounds_model.cpp).
-            const bool near = allc || (unset == 1 && !s_predc);
-            const bool certified = allc && c_prev;
-            stamp_if(dbg && tid == 0, dbg + rnd * 8 + 5);
-            store_if(dbg && tid == 0, dbg + rnd * 8 + 7, s_nlog | ((unsigned long long)need_sim << 32));
-            if (gseg > 0 && tid == 192) pub_nb(sm.ack + gseg, ((unsigned long long)tage << 32) | (certified ? 0xFFFFu : rnd), true);
-            if (certified) {    // every entry up to mine was the true token one round ago and has not moved since: the log in shared memory is THE log
-                if (tid < ISL_MAX_PROFILES) {
-                    pub_nb(sm.xf + (size_t)gseg * 16 + tid, tagF | (rnd << 24) | s_specX[tid], false);
-                    if (gseg == gtot - 1 && a.heads_out) a.heads_out[(size_t)c * ISL_MAX_PROFILES + tid] = s_specX[tid];
-                }
-                if (tid == 16) pub_down(sm.df + gseg, tagF | (rnd << 24) | (s_dqr[0] << 13) | s_dqr[1]);
-                if (tid == 0) { st_steps += spec_steps; st_visited += spec_visited; if (gseg == gtot - 1) { st_rounds_sum += rnd; ++st_cells; } if (tr) { tr[0] = t_cell; tr[2] = globaltimer_ns(); tr[6] = s_nlog; tr[7] = st_sims - sims_cell; tr[11] = rnd; } }
-                break;
-            }
-            if (tid < 32) {     // c for the next round; the corrected prediction
-                const bool same = tid >= ISL_MAX_PROFILES || s_specH[tid] == s_specXp[tid];
-                const bool cnow = __all_sync(0xFFFFFFFFu, same);
-                uint32_t mq = 0, mr = 0, hold = 0, hn = 0;
-                const uint32_t qcl = tid < ISL_MAX_PROFILES ? s_qc[tid] : 0u, wl = tid < ISL_MAX_PROFILES ? s_minsize[tid] : 1u;
-                if (tid < ISL_MAX_PROFILES) {
-                    hold = s_specH[tid];
-                    hn = s_specXp[tid];
-                    if ((s_grp_big >> tid) & 1u) mq = hn;
-                    if ((s_grp_small >> tid) & 1u) mr = hn * s_minsize[tid];
-                }
-                mq = __reduce_add_sync(0xFFFFFFFFu, mq); mr = __reduce_add_sync(0xFFFFFFFFu, mr);
-                hn = spec_spread_warp(hn, qcl, wl, s_grp_big, (int)s_acc[0] - (int)mq, false, lane);
-                hn = spec_spread_warp(hn, qcl, wl, s_grp_small, (int)s_acc[1] - (int)mr, true, lane);
-                {   // Two candidates for the next entry: the Newton step (hn) and plain chaining (the exit of the stage in front as it is).  Where a
-                    // batch's contested front reaches far the Newton step over-corrects round after round; each stage uses the rule whose
-                    // candidate of the PREVIOUS round came closer to what the stage in front has published now (study, section 8).
-                    const uint32_t xp = tid < ISL_MAX_PROFILES ? s_specXp[tid] : 0u;
-                    uint32_t ea = 0, eb = 0;
-                    if (tid < ISL_MAX_PROFILES && s_havepred) { ea = (uint32_t)abs((int)s_predA[tid] - (int)xp); eb = (uint32_t)abs((int)s_predB[tid] - (int)xp); }
-                    ea = __reduce_add_sync(0xFFFFFFFFu, ea); eb = __reduce_add_sync(0xFFFFFFFFu, eb);
-                    __syncwarp();
-                    if (tid < ISL_MAX_PROFILES) { s_predA[tid] = hn; s_predB[tid] = xp; }
-                    if (tid == 0) s_havepred = 1;
-                    if (eb < ea) hn = xp;
-                }
-                if (tid < ISL_MAX_PROFILES) s_specH[tid] = hn;
-                const bool moved = tid < ISL_MAX_PROFILES && hn != hold;
-                const bool changed = __any_sync(0xFFFFFFFFu, moved);
-                // a cut-off simulation left no usable log: the entry is simulated again (in full once it is known to be the true one) and counts as
-                // inconsistent until then
-                if (tid == 0) s_specflag = (cnow && s_capst[2] ? 1u : 0u) | (changed || !s_capst[2] ? 2u : 0u);
-                stamp_if(dbg && tid == 0, dbg + rnd * 8 + 6);
-            }
-            __syncthreads();
-            c_prev = s_specflag & 1u; need_sim = s_specflag & 2u; known_exact = near;
-            if (++rnd >= kSpecRounds - 1) __trap();      // cannot happen: every round certifies at least one more stage
-        }
-        }   // rounds
-        if (idle_break) break;
-        if (last_sub && c + 1 < a.n_chunks && !a.ready && !a.window) { queue_load_async(c + 1); prefetched = true; }   // the chain is done with the queues: fetch the next chunk's behind the commit
-        {   // 6. commit
-            const uint32_t nlog = s_nlog;
-            for (uint32_t j = tid; j < nlog; j += kPipeThreads) {
-                const uint2 e = s_log[j];
-                const uint32_t l = sb_base + (s_cand[((e.y - sa_cand) >> 2) - 2] >> 16), mask = e.x & 0xFFu, t = (e.x >> 15) & 0xFFFFu;
-                const uint2 rec = pack_result(flip_gpu(lo_s + l, a.flip), __ffs(mask) - 1, __popc(mask), ISL_ST_PLACED);
-                a.out[cd.req_off + t] = rec;
-                if (a.owner_out) a.owner_out[cd.req_off + t] = rec;         // partitioned inventory: straight into the owner rank's result array (peer store over NVLink)
-                atomicOr(&s_occ32[l >> 2], mask << ((l & 3u) * 8u));
-            }
+            if (lane == 0 && tr) { tr[2] = globaltimer_ns(); tr[3] = tr[2]; }
         }
         __syncthreads();
-        if (tr && tid == 0) tr[3] = globaltimer_ns();
-        }   // sub-segments
-        chunk_done(c);
-        if (c + 1 < a.n_chunks && !prefetched) { closed = wait_ready(c + 1); if (!closed) queue_load_async(c + 1); }   // fed / windowed stream: the next batch may not be due yet
+        return false;
+    }
+    stage_windows<false>(st, s, ss, tr);
+    if (is_chain_warp(warp)) decide<K, kP15, false>(a, st, s, ss, cs, n, c, last_sub, tr, nullptr, 1);
+    __syncthreads();
+    return true;
+}
+
+// 3.-5. by speculative rounds (one sub-segment per stage): predict the entry, then simulate, exchange and correct round by round until
+// the stage is certified
+template <int K, bool kP15>
+__device__ __forceinline__ void resolve_rounds(const PipeArgs& a, const Stage& st, PipeShared& s, SpecShared& ss, const ChainSlots<K>& cs,
+                                               PipeCounters& n, uint32_t c, uint32_t active, uint32_t sb_base, uint32_t n_sb, unsigned long long* tr) {
+    const uint32_t tid = threadIdx.x;
+    Rounds r;
+    r.sm = spec_mem(a.spec_mem, c);
+    r.tage = a.spec_world > 1 ? a.xepoch : a.epoch;        // a partitioned inventory tags with the stream id all ranks share
+    r.tagb = (unsigned long long)((r.tage & 0xFFFFFFu) << 8) << 32; r.tagF = r.tagb | (0xFFull << 32);
+    r.gseg = a.spec_base + st.seg; r.gtot = a.spec_total;
+    predict_entry(a, st, s, ss, r, c, active, sb_base, n_sb);
+    // known_exact: everything in front of the stage right in front of me was consistent one round ago: my next entry may be the true one
+    r.rnd = 1; r.c_prev = r.gseg == 0; r.need_sim = true; r.known_exact = r.gseg == 0; r.p_final = false; r.p_word = 0;
+    if (tid == 0) { ss.capst[0] = 0; ss.capst[1] = 0; ss.capst[2] = 0; s.cap = kLogCap + 1; ss.capped = 0; ss.wvalid = 0; ss.havepred = 0; }
+    r.t_cell = tr ? globaltimer_ns() : 0ull; r.sims_cell = n.sims;
+#ifdef ISL_SPEC_DBG_STAMPS      // per-round stamps of one cell (tools/spec_trace.py): a debugging build — the extra live pointer around the decision loop slows it
+    unsigned long long* dbg = a.spec_dbg && a.spec_dbg_cell == ((c << 16) | st.seg) ? a.spec_dbg : nullptr;
+#else
+    constexpr unsigned long long* dbg = nullptr;
+#endif
+    do {
+        stamp_if(dbg && tid == 0, dbg + r.rnd * 8 + 0);
+        if (r.need_sim) {       // an unchanged entry is not simulated again
+            if (read_entry<true>(a, st, s, ss, c, 0, active, r.known_exact, tr, dbg, r.rnd)) {
+                if (tid == 0) { s.nlog = 0; n.spec_steps = 0; n.spec_visited = 0; }    // nothing pending at these heads: the exit equals the entry
+            } else {
+                stage_windows<true>(st, s, ss, tr);
+                if (is_chain_warp(tid >> 5)) decide<K, kP15, true>(a, st, s, ss, cs, n, c, true, tr, dbg, r.rnd);
+                else if (tid == kPipeThreads - 32 && r.rnd >= 3 && r.gseg + 1 < r.gtot) wait_ack(a, r);     // in the shadow of the chain
+            }
+            __syncthreads();
+        }
+    } while (!exchange_round(a, st.seg, s, ss, r, n, c, tr, dbg));
+}
+
+template <int K, bool kP15, bool kSpec>
+__global__ void __launch_bounds__(kPipeThreads, 1) k_pipeline(CandTab tab, PipeArgs a) {
+    extern __shared__ __align__(16) uint8_t smem[];
+    __shared__ PipeShared s;
+    __shared__ SpecShared ss;
+    const uint32_t tid = threadIdx.x, seg = blockIdx.x;
+    if (seg == a.n_seg) { deliver_chunks(a); return; }
+    Stage st;
+    st.seg = seg; st.lo = min(a.hi, a.lo + seg * a.seg); st.n_g = min(a.hi, st.lo + a.seg) - st.lo;
+    st.occ32 = reinterpret_cast<uint32_t*>(smem); st.cand = reinterpret_cast<uint32_t*>(smem + kPipeOffCand); st.log = reinterpret_cast<uint2*>(smem + kPipeOffLog);
+    st.q = reinterpret_cast<const uint16_t*>(smem + kPipeOffQ); st.wkey = reinterpret_cast<uint32_t*>(smem + kPipeOffWin);
+    st.sa_cand = (uint32_t)__cvta_generic_to_shared(st.cand); st.sa_log = (uint32_t)__cvta_generic_to_shared(st.log);
+    st.sa_q = (uint32_t)__cvta_generic_to_shared(st.q); st.sa_wkey = (uint32_t)__cvta_generic_to_shared(st.wkey);
+    stage_init<kSpec>(tab, a, st, s, ss);
+    const ChainSlots<K> cs(tab, tid & 31u);
+    PipeCounters n{};
+
+    bool closed = wait_ready(a, s, 0);
+    if (!closed) queue_load_async(a, st, 0);
+    for (uint32_t c = 0; c < a.n_chunks && !closed; ++c) {
+        const ChunkDesc cd = a.chunks[c];
+        if (cd.first_of_batch) apply_frees(a, st, cd);
+        const uint32_t active = a.cctl[c].active;
+        // A stage is walked sub-segment by sub-segment (one for inventories up to SMs x 512 GPUs): sweep, heads, windows, chain, commit per
+        // sub-segment; the token is awaited in front of the first and published behind the last one (or as soon as nothing is pending).
+        const uint32_t n_sub = max(1u, (st.n_g + a.sub - 1) / a.sub);
+        bool prefetched = false;            // the next chunk's queues are on their way (they may only overwrite this chunk's after its last chain)
+        for (uint32_t sb = 0; sb < n_sub; ++sb) {
+            const uint32_t sb_base = sb * a.sub, n_sb = min(a.sub, st.n_g - min(st.n_g, sb_base));
+            const bool last_sub = sb + 1 == n_sub;
+            unsigned long long* tr = a.trace ? a.trace + ((size_t)c * a.n_seg + seg) * kTraceWords : nullptr;
+            sweep_subsegment(st, s, sb_base, n_sb, active);
+            // kSpec (host: only with one sub-segment per stage) is a separate instantiation, so that the plain pipeline's code is untouched by the rounds' machinery
+            if (kSpec) resolve_rounds<K, kP15>(a, st, s, ss, cs, n, c, active, sb_base, n_sb, tr);
+            else if (!resolve_plain<K, kP15>(a, st, s, ss, cs, n, c, sb, active, last_sub, tr)) break;
+            if (last_sub && c + 1 < a.n_chunks && !a.ready && !a.window) { queue_load_async(a, st, c + 1); prefetched = true; }   // the chain is done with the queues: fetch the next chunk's behind the commit
+            commit_log(a, st, s, cd, sb_base, tr);
+        }
+        chunk_done(a, c);
+        if (c + 1 < a.n_chunks && !prefetched) { closed = wait_ready(a, s, c + 1); if (!closed) queue_load_async(a, st, c + 1); }   // fed / windowed stream: the next batch may not be due yet
     }
     asm volatile("cp.async.wait_group 0;" ::: "memory");
-    for (uint32_t i = tid; i < n_g; i += kPipeThreads) a.occ[lo_s + i] = reinterpret_cast<uint8_t*>(s_occ32)[i];
+    for (uint32_t i = tid; i < st.n_g; i += kPipeThreads) a.occ[st.lo + i] = reinterpret_cast<uint8_t*>(st.occ32)[i];
     if (a.owner_out) __threadfence_system();        // the peer stores of this CTA are performed before the grid is seen as complete
-    if (tid == 0 && st_steps + st_jumps) {
-        atomicAdd(&a.stats->placed, st_steps);
-        atomicAdd(&a.stats->steps, st_steps);
-        atomicAdd(&a.stats->visited, st_visited);
-        atomicAdd(&a.stats->jumps, st_jumps);
+    if (tid == 0 && n.steps + n.jumps) {
+        atomicAdd(&a.stats->placed, n.steps);
+        atomicAdd(&a.stats->steps, n.steps);
+        atomicAdd(&a.stats->visited, n.visited);
+        atomicAdd(&a.stats->jumps, n.jumps);
     }
     if (kSpec && tid == 0) {
-        atomicAdd(&a.stats->spec_sims, st_sims);
-        atomicAdd(&a.stats->spec_rounds, st_rounds_sum);
-        atomicAdd(&a.stats->spec_cells, (unsigned long long)st_cells);
+        atomicAdd(&a.stats->spec_sims, n.sims);
+        atomicAdd(&a.stats->spec_rounds, n.rounds_sum);
+        atomicAdd(&a.stats->spec_cells, (unsigned long long)n.cells);
     }
 }
 

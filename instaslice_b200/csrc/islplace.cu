@@ -516,7 +516,7 @@ PipeArgs pipe_args(const isl_engine* e, const PipePlan& plan, uint32_t n_chunks,
     args.chunks = e->d_chunks; args.cctl = e->d_cctl; args.q_all = e->d_qall; args.free_acc = reinterpret_cast<const uint8_t*>(e->d_free_acc);
     args.q_stride = q_stride; args.free_stride = (uint32_t)e->occ_bytes; args.tokens = e->d_tokens; args.occ = e->d_occ; args.gtab = e->d_gtab;
     args.out = out; args.feas = e->d_feas; args.stats = e->d_ctrl;
-    if (plan.spec) { args.spec = getenv("ISL_SPEC_NOREUSE") ? 3u : 1u; args.spec_mem = e->d_spec; args.spec_total = plan.n_seg; }
+    if (plan.spec) { args.spec = 1; args.spec_mem = e->d_spec; args.spec_total = plan.n_seg; }
     return args;
 }
 
