@@ -94,6 +94,7 @@ extern "C" {
 #define ISL_ST_FREED       3u
 #define ISL_ST_BAD_SPAN    4u   /* FREE outside the inventory or start+size > 8 (the reference would panic, Q7) */
 #define ISL_ST_NOOP        5u
+#define ISL_ST_GANG_ABORTED 6u  /* placeable as far as it was tried, but another member of its gang was not: nothing of the gang was committed */
 
 typedef struct isl_engine isl_engine;
 
@@ -248,6 +249,24 @@ int  isl_place_batch_device(isl_engine* e, uint32_t n, const void* d_in, void* d
  * loop (:190) calls it node after node.  Restriction, placement and restore happen under one engine lock (two reconcile workers
  * cannot interleave, nothing leaks when the call fails); the engine's own partition (isl_set_partition) is left untouched. */
 int  isl_place_batch_range(isl_engine* e, uint32_t lo, uint32_t hi, uint32_t n, const isl_request* in, isl_result* out);
+/* All-or-nothing pod groups (the replicas of a deployment, the workers of a job).  `in` / `out` hold n = gang_off[n_gangs] requests and
+ * records (host buffers, as isl_place_batch); gang i is in[gang_off[i] .. gang_off[i + 1]), gang_off[0] == 0, no gang is empty.
+ *   1. Every FREE of the call is applied first, wherever it is listed (FREED / BAD_SPAN); a FREE never aborts a gang.  NOOP members
+ *      report NOOP and do not count.
+ *   2. Gangs in array order; inside a gang the ALLOC members are resolved in order by the engine's policy, each one seeing every commit
+ *      before it, tentative ones of its own gang included.  A gang of one ALLOC is an ordinary request.
+ *   3. A gang whose ALLOC members are all placed commits: the usual PLACED records.
+ *   4. Otherwise the first member that cannot be placed gets its usual record (NO_CAPACITY, or BAD_PROFILE for an unknown profile), the
+ *      members after it are not tried, and every other ALLOC member of the gang reports ISL_ST_GANG_ABORTED with the unplaced default
+ *      record (gpu ISL_GPU_NONE, start 9, the profile's size or 0 for an unknown profile).
+ *   5. The occupancy after an aborted gang is exactly what it was before it: later gangs see no trace of it.
+ *   6. Every policy, both quirk sets and per-node tables; inside the engine's partition (isl_set_partition).  Stats count committed
+ *      placements only.
+ * A call whose gangs all have one member equals isl_place_batch on the same requests, records and occupancy.  The gangs are resolved
+ * request by request (the best-fit kernel's loop, DESIGN.md 4.6): first-fit gangs do not use the segment pipeline.
+ * ISL_EINVAL: malformed offsets, NULL buffers, an engine created with ISL_FLAG_ALL_NODES.  ISL_ERANGE: n > max_batch, or a partition
+ * that is empty or holds more than 2^20 GPUs.  ISL_ESTATE: no profiles or inventory, or an open stream. */
+int  isl_place_gangs(isl_engine* e, uint32_t n_gangs, const uint32_t* gang_off, const isl_request* in, isl_result* out);
 
 /* ---- open streams: the causal feed --------------------------------------- */
 /* A reconciler that composes batch b+1 from the results of batch b (a FREE names an allocation an earlier batch placed) cannot hand

@@ -249,6 +249,42 @@ class InstasliceReconciler:
                 out.append(self._commit_or_veto(pod, pod["profile"], policy, res))
         return out
 
+    def place_pending_gangs(self, gangs: list, policy=None):
+        """All-or-nothing pod groups (the replicas of one deployment, the workers of one job): ``gangs`` is a list of non-empty pod
+        lists shaped as ``place_pending_pods`` takes them, resolved in order with ONE engine call (isl_place_gangs).
+
+        Returns per gang ("placed", [AllocationDetails...]) | ("veto", None) | ("none", None).  A gang is placed only when every pod of
+        it gets a slice, and only then are its allocations written to the custom resources.  When the Prepared exact-match veto
+        (:198-203) fires on any pod, the spans of the whole gang are released again.  With realised slices whose allocation is gone
+        (the only state in which the veto can fire) the gangs are resolved one engine call each, as ``place_pending_pods`` does per pod.
+        """
+        policy = policy or FirstFitPolicy()
+        if any(not g for g in gangs):
+            raise ValueError("empty gang")
+        if self._has_orphans and len(gangs) > 1:
+            return [self.place_pending_gangs([g], policy)[0] for g in gangs]
+        if not gangs:
+            return []
+        off = np.cumsum([0] + [len(g) for g in gangs]).astype(np.uint32)
+        results = self._engine.place_gangs(self._requests([p["profile"] for g in gangs for p in g]), off)
+        out = []
+        for gang, a, b in zip(gangs, off[:-1], off[1:]):
+            res = results[a:b]
+            if (res["status"] != E.ST_PLACED).any():
+                out.append(("none", None))
+                continue
+            packed = [self._alloc_for(pod, pod["profile"], policy, r) for pod, r in zip(gang, res)]
+            if any(self._vetoed(instaslice, alloc) for instaslice, alloc in packed):
+                spans = np.zeros(len(res), dtype=E.SPAN_DTYPE)
+                spans["gpu"], spans["start"], spans["size"] = res["gpu"], res["start"], res["size"]
+                self._engine.free_batch(spans)
+                out.append(("veto", None))
+                continue
+            for pod, (instaslice, alloc) in zip(gang, packed):
+                instaslice["spec"].setdefault("allocations", {})[pod["uid"]] = alloc   # :215-219
+            out.append(("placed", [alloc for _, alloc in packed]))
+        return out
+
     def release(self, pod_uid: str):
         """The daemonset deleted ``Allocations[podUID]`` (instaslice_daemonset.go:261-263): free its span."""
         for n, it in enumerate(self.items):
@@ -262,14 +298,17 @@ class InstasliceReconciler:
         return False
 
     # -- internals --------------------------------------------------------------------------------
-    def _place(self, profile_names, lo, hi):
+    def _requests(self, profile_names):
         req = np.zeros(len(profile_names), dtype=E.REQUEST_DTYPE)
         req["handle"] = np.arange(len(profile_names), dtype=np.uint32)
         req["profile"] = [self.profile_names.get(n, E.PROFILE_UNKNOWN) for n in profile_names]
         req["op"] = E.OP_ALLOC
+        return req
+
+    def _place(self, profile_names, lo, hi):
         # ONE locked call restricts, places and restores (isl_place_batch_range): two reconcile workers cannot interleave and
         # nothing leaks when the call fails
-        return self._engine.place_batch_range(lo, hi, req)
+        return self._engine.place_batch_range(lo, hi, self._requests(profile_names))
 
     def _release(self, res):
         spans = np.zeros(1, dtype=E.SPAN_DTYPE)
@@ -282,13 +321,20 @@ class InstasliceReconciler:
                                            "creating", gi, ci, cieng, pod.get("namespace", "default"), pod["name"],
                                            self.gpu_uuid[int(res["gpu"])])
 
+    def _alloc_for(self, pod, profileName, policy, res):
+        """The owning Instaslice of a PLACED record and the AllocationDetails the policy packs for it."""
+        instaslice = self.items[self.node_of_uuid[self.gpu_uuid[int(res["gpu"])]]]
+        return instaslice, self._details(instaslice, profileName, policy, pod, res)
+
+    @staticmethod
+    def _vetoed(instaslice, alloc):
+        return any(item["parent"] == alloc["gpuUUID"] and item["size"] == alloc["size"] and item["start"] == alloc["start"]
+                   for item in instaslice["spec"].get("prepared", {}).values())          # :198-203
+
     def _commit_or_veto(self, pod, profileName, policy, res):
-        uuid = self.gpu_uuid[int(res["gpu"])]
-        instaslice = self.items[self.node_of_uuid[uuid]]
-        alloc = self._details(instaslice, profileName, policy, pod, res)
-        for item in instaslice["spec"].get("prepared", {}).values():          # :198-203
-            if item["parent"] == alloc["gpuUUID"] and item["size"] == alloc["size"] and item["start"] == alloc["start"]:
-                self._release(res)
-                return ("veto", None)
+        instaslice, alloc = self._alloc_for(pod, profileName, policy, res)
+        if self._vetoed(instaslice, alloc):
+            self._release(res)
+            return ("veto", None)
         instaslice["spec"].setdefault("allocations", {})[pod["uid"]] = alloc   # :215-219
         return ("placed", alloc)

@@ -2057,16 +2057,23 @@ __global__ void __launch_bounds__(256) k_capacity(const uint8_t* __restrict__ oc
 // State: GPUs grouped by occupancy byte (256 classes); per class a two-level bitmap (32 GPUs per word, 1024 per
 // summary bit) and its minimum member.  One warp: lane = a few classes, key = (8 - popcount) << 24 | class minimum,
 // redux.min picks the GPU; lane 0 moves it to its new class.  One CTA; all threads build the class structure.
+// kGang (isl_place_gangs): the requests come in gangs [gang_off[i], gang_off[i + 1]) that commit all or nothing.  With a zero score table
+// (ISL_POLICY_FIRST_FIT / _RIGHT_TO_LEFT) the key is the class minimum, i.e. exact first-fit.  The first ALLOC of a gang that cannot be
+// placed keeps its record, the gang's later members are not tried, and when the gang ends its placed members are moved back to their old
+// classes in reverse order (a PLACED record holds gpu, start and size: `occupancy & ~span` is the byte it came from) and, like every
+// other ALLOC of the gang, reported GANG_ABORTED.  The `dead` profile mask assumes occupancy only grows: it is restored as well, except
+// for a profile that died before any member of its gang was placed (it died in the committed state).
 // ---------------------------------------------------------------------------------------------
 constexpr uint32_t kBfThreads = 1024;
 constexpr uint32_t kBfMaxGpus = 1u << 20;           // class bitmaps: G / 32 words + G / 1024 summary words per (table, occupancy byte) class
 constexpr uint32_t kBfSmemGpus = 4096;              // up to here the class bitmaps live in shared memory (132 KiB)
 
-template <bool kMulti>
+template <bool kMulti, bool kGang = false>
 __global__ void __launch_bounds__(kBfThreads, 1) k_bestfit(uint32_t n, const uint2* __restrict__ in, uint2* __restrict__ out, uint8_t* __restrict__ occ,
                                                            uint32_t lo, uint32_t hi, const uint8_t* __restrict__ lut, DevProfiles prof,
                                                            uint32_t* __restrict__ g_bitmaps, Ctrl* ctrl, const uint8_t* __restrict__ score,
-                                                           const uint8_t* __restrict__ gtab, const uint8_t* __restrict__ sizes, uint32_t n_tables) {
+                                                           const uint8_t* __restrict__ gtab, const uint8_t* __restrict__ sizes, uint32_t n_tables,
+                                                           const uint32_t* __restrict__ gang_off = nullptr, uint32_t n_gangs = 0) {
     extern __shared__ __align__(16) uint32_t s_dyn[];
     // a class = (table of the GPU's node, occupancy byte): every GPU of a class behaves the same for every profile
     __shared__ uint32_t s_min[kMaxTables * 256];
@@ -2097,23 +2104,114 @@ __global__ void __launch_bounds__(kBfThreads, 1) k_bestfit(uint32_t n, const uin
     }
     __syncthreads();
     if (!is_chain_warp(tid >> 5)) return;
+    // lane 0: GPU g leaves the class whose bitmaps are c0 and joins the one of c1 (independent words, loads first)
+    auto move_bits = [&](uint32_t* c0, uint32_t* c1, uint32_t g) {
+        const uint32_t w0 = c0[g >> 5] & ~(1u << (g & 31u)), w1 = c1[g >> 5] | (1u << (g & 31u));
+        const uint32_t s1 = c1[W0 + (g >> 10)] | (1u << ((g >> 5) & 31u));
+        c0[g >> 5] = w0; c1[g >> 5] = w1; c1[W0 + (g >> 10)] = s1;
+        if (w0 == 0) c0[W0 + (g >> 10)] &= ~(1u << ((g >> 5) & 31u));
+    };
+    // new minimum of the class of c0 after its minimum g left it (nothing below g).  Usually it sits under the summary word that held g:
+    // every lane reads that word (one broadcast); only when it is empty do the lanes look at the further summary words, 32 at a time
+    auto min_after = [&](const uint32_t* c0, uint32_t g) -> uint32_t {
+        uint32_t mn = kInf;
+        const uint32_t k = g >> 10, sw = c0[W0 + k];
+        if (sw) { const uint32_t wi = k * 32 + __ffs(sw) - 1; mn = wi * 32 + __ffs(c0[wi]) - 1; }
+        else
+            for (uint32_t k0 = k + 1; k0 < W1; k0 += 32) {
+                const uint32_t s2 = k0 + lane < W1 ? c0[W0 + k0 + lane] : 0u;
+                const uint32_t b = __ballot_sync(0xFFFFFFFFu, s2 != 0);
+                if (b) {
+                    const uint32_t src = __ffs(b) - 1;
+                    const uint32_t wi = (k0 + src) * 32 + __ffs(__shfl_sync(0xFFFFFFFFu, s2, src)) - 1;
+                    mn = wi * 32 + __ffs(c0[wi]) - 1;
+                    break;
+                }
+            }
+        return mn;
+    };
     uint32_t placed = 0;
     uint32_t dead = 0;              // profiles that found no GPU: occupancy only grows inside a batch's ALLOC phase, so they never will again
+    // kGang: the open gang is requests [g_first, g_end); g_fail = its member that could not be placed (kInf: none yet); g_placed = its
+    // members placed so far; dead_at = `dead` when it began.  Lane l holds gang_off[g_win + 1 + l]: one load per 32 gangs
+    uint32_t gang = 0, g_first = 0, g_end = 0, g_fail = kInf, g_placed = 0, dead_at = 0, g_win = 0, g_offs = 0;
+    if (kGang) {
+        g_offs = lane < n_gangs ? __ldg(gang_off + 1 + lane) : n;
+        g_end = __shfl_sync(0xFFFFFFFFu, g_offs, 0);
+    }
+    // kGang, the open gang failed: its placed members (every ALLOC before g_fail) leave their classes again, last placed first, and
+    // report GANG_ABORTED (the members after g_fail already do)
+    auto abort_gang = [&]() {
+        for (uint32_t top = g_fail; g_placed;) {
+            const uint32_t cnt = min(32u, top - g_first), r = top - 1 - lane;       // lane order = descending request order
+            const uint2 q = lane < cnt ? in[r] : make_uint2(0, (uint32_t)ISL_OP_NOOP << 8);
+            const bool alloc = ((q.y >> 8) & 0xFFu) == ISL_OP_ALLOC;
+            const uint2 rec = alloc ? out[r] : make_uint2(0, 0);
+            uint32_t undo = __ballot_sync(0xFFFFFFFFu, alloc);
+            while (undo) {
+                const uint32_t src = __ffs(undo) - 1;
+                undo &= undo - 1;
+                const uint32_t rx = __shfl_sync(0xFFFFFFFFu, rec.x, src), ry = __shfl_sync(0xFFFFFFFFu, rec.y, src);
+                const uint32_t p = __shfl_sync(0xFFFFFFFFu, q.y, src) & 0xFFu;
+                const uint32_t g = flip_gpu(rx, prof.flip) - lo, span = (((1u << ((ry >> 8) & 0xFFu)) - 1u) << (ry & 0xFFu)) & 0xFFu;
+                const uint32_t t = kMulti ? (uint32_t)(gtab[lo + g] & (kMaxTables - 1)) : 0u;
+                const uint32_t o2 = occ[lo + g], cw2 = (t << 8) | o2, cw = (t << 8) | (o2 & ~span);
+                uint32_t* c2 = bm + cw2 * stride;
+                const bool was_min = s_min[cw2] == g;
+                __syncwarp();
+                if (lane == 0) {                                // back from class o2 to class o2 & ~span
+                    move_bits(c2, bm + cw * stride, g);
+                    occ[lo + g] = (uint8_t)(o2 & ~span);
+                    out[top - 1 - src] = pack_result(ISL_GPU_NONE, ISL_START_NONE, prof.rows[p].size, ISL_ST_GANG_ABORTED);
+                    if (g < s_min[cw]) s_min[cw] = g;
+                    --placed;
+                }
+                __syncwarp();
+                if (was_min) {
+                    const uint32_t mn = min_after(c2, g);
+                    if (lane == 0) s_min[cw2] = mn;
+                }
+                __syncwarp();
+                --g_placed;
+            }
+            top -= cnt;
+        }
+        dead = dead_at;
+    };
+    // kGang: end every gang that lies wholly before request `upto` (commit, or abort when a member failed)
+    auto close_gangs = [&](uint32_t upto) {
+        while (g_end <= upto && gang < n_gangs) {
+            if (g_fail != kInf) abort_gang();
+            g_fail = kInf; g_placed = 0; dead_at = dead; g_first = g_end;
+            if (++gang < n_gangs) {
+                if (gang - g_win == 32) { g_win = gang; g_offs = gang + lane < n_gangs ? __ldg(gang_off + gang + 1 + lane) : n; }
+                g_end = __shfl_sync(0xFFFFFFFFu, g_offs, gang - g_win);
+            }
+        }
+    };
     uint2 ahead = lane < n ? in[lane] : make_uint2(0, (uint32_t)ISL_OP_NOOP << 8);
     for (uint32_t base = 0; base < n; base += 32) {
         const uint2 mine = ahead;                               // the next block's requests are fetched while this one is resolved
         ahead = base + 32 + lane < n ? in[base + 32 + lane] : make_uint2(0, (uint32_t)ISL_OP_NOOP << 8);
-        // only the live ALLOCs of the block are looked at (frees, unknown or dead profiles: defaults were written by k_prepare)
+        // only the live ALLOCs of the block are looked at (frees, unknown or dead profiles: defaults were written by k_prepare); in a
+        // gang every ALLOC is looked at, since an unknown or dead profile fails its gang
         uint32_t live;
         {
             const uint32_t wp = mine.y & 0xFFu, wop = (mine.y >> 8) & 0xFFu;
-            live = __ballot_sync(0xFFFFFFFFu, wop == ISL_OP_ALLOC && wp < prof.n && !((dead >> wp) & 1u));
+            live = __ballot_sync(0xFFFFFFFFu, wop == ISL_OP_ALLOC && (kGang || (wp < prof.n && !((dead >> wp) & 1u))));
         }
         while (live) {
             const uint32_t j = __ffs(live) - 1;
             live &= live - 1;
             const uint32_t p = __shfl_sync(0xFFFFFFFFu, mine.y, j) & 0xFFu;
-            if ((dead >> p) & 1u) continue;                     // died inside this block
+            if (kGang) {
+                close_gangs(base + j);
+                if (g_fail != kInf) {                           // a member of this gang failed: the rest is not tried
+                    if (lane == 0) out[base + j] = pack_result(ISL_GPU_NONE, ISL_START_NONE, p < prof.n ? prof.rows[p].size : 0u, ISL_ST_GANG_ABORTED);
+                    continue;
+                }
+                if (p >= prof.n || ((dead >> p) & 1u)) { g_fail = base + j; continue; }
+            } else if ((dead >> p) & 1u) continue;              // died inside this block
             uint32_t key = kInf, kc = 0;
 #pragma unroll 8
             for (uint32_t c = lane; c < n_cls; c += 32) {       // lane l looks at classes l, l+32, ...
@@ -2125,7 +2223,14 @@ __global__ void __launch_bounds__(kBfThreads, 1) k_bestfit(uint32_t n, const uin
                 }
             }
             const uint32_t m = __reduce_min_sync(0xFFFFFFFFu, key);
-            if (m == kInf) { dead |= 1u << p; continue; }      // stays NO_CAPACITY, and so does every later request of the profile
+            if (m == kInf) {                                    // stays NO_CAPACITY, and so does every later request of the profile
+                dead |= 1u << p;
+                if (kGang) {
+                    g_fail = base + j;
+                    if (g_placed == 0) dead_at |= 1u << p;      // nothing of the gang placed yet: it died in the committed state
+                }
+                continue;
+            }
             const uint32_t g = m & 0xFFFFFFu;
             const uint32_t cw = __shfl_sync(0xFFFFFFFFu, kc, __ffs(__ballot_sync(0xFFFFFFFFu, key == m)) - 1);   // the class IS (table, occupancy byte)
             const uint32_t t = cw >> 8, o = cw & 255u;
@@ -2134,39 +2239,21 @@ __global__ void __launch_bounds__(kBfThreads, 1) k_bestfit(uint32_t n, const uin
             uint32_t* c0 = bm + cw * stride;
             uint32_t* c1 = bm + cw2 * stride;
             __syncwarp();                                       // all lanes have read the class minima before they are rewritten
-            if (lane == 0) {                                    // the GPU leaves class o and joins class o2: independent words, loads first
-                const uint32_t w0 = c0[g >> 5] & ~(1u << (g & 31u)), w1 = c1[g >> 5] | (1u << (g & 31u));
-                const uint32_t s1 = c1[W0 + (g >> 10)] | (1u << ((g >> 5) & 31u));
-                c0[g >> 5] = w0; c1[g >> 5] = w1; c1[W0 + (g >> 10)] = s1;
-                if (w0 == 0) c0[W0 + (g >> 10)] &= ~(1u << ((g >> 5) & 31u));
+            if (lane == 0) {                                    // the GPU leaves class o and joins class o2
+                move_bits(c0, c1, g);
                 occ[lo + g] = (uint8_t)o2;
                 out[base + j] = pack_result(flip_gpu(lo + g, prof.flip), start, size, ISL_ST_PLACED);
                 if (g < s_min[cw2]) s_min[cw2] = g;
                 ++placed;
             }
+            if (kGang) ++g_placed;
             __syncwarp();
-            // new minimum of the class (g was its minimum: nothing below it).  Usually it sits under the summary word that held g: every
-            // lane reads that word (one broadcast); only when it is empty do the lanes look at the further summary words, 32 at a time
-            uint32_t mn = kInf;
-            {
-                const uint32_t k = g >> 10, sw = c0[W0 + k];
-                if (sw) { const uint32_t wi = k * 32 + __ffs(sw) - 1; mn = wi * 32 + __ffs(c0[wi]) - 1; }
-                else
-                    for (uint32_t k0 = k + 1; k0 < W1; k0 += 32) {
-                        const uint32_t s2 = k0 + lane < W1 ? c0[W0 + k0 + lane] : 0u;
-                        const uint32_t b = __ballot_sync(0xFFFFFFFFu, s2 != 0);
-                        if (b) {
-                            const uint32_t src = __ffs(b) - 1;
-                            const uint32_t wi = (k0 + src) * 32 + __ffs(__shfl_sync(0xFFFFFFFFu, s2, src)) - 1;
-                            mn = wi * 32 + __ffs(c0[wi]) - 1;
-                            break;
-                        }
-                    }
-            }
+            const uint32_t mn = min_after(c0, g);               // g was the class minimum
             if (lane == 0) s_min[cw] = mn;
             __syncwarp();
         }
     }
+    if (kGang) close_gangs(n);
     if (lane == 0) { atomicAdd(&ctrl->placed, (unsigned long long)placed); atomicAdd(&ctrl->steps, (unsigned long long)placed); }
 }
 

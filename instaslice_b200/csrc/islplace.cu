@@ -230,14 +230,14 @@ int run_few(isl_engine* e, uint32_t n, const SmallReqs& inl, uint2* d_out) {
     return ISL_OK;
 }
 
-// ISL_POLICY_BEST_FIT: frees + defaults, then the request-major class-bitmap kernel (one CTA).
-int run_bestfit(isl_engine* e, uint32_t n, const uint2* d_in, uint2* d_out) {
-    if (n == 0) return ISL_OK;
+// What run_bestfit and run_gangs share in front of k_bestfit: the class bitmaps (shared memory up to kBfSmemGpus GPUs of one table, else
+// global memory zeroed here), then k_prepare (frees + default records).  *smem = the dynamic shared memory k_bestfit needs.
+int prepare_bestfit(isl_engine* e, uint32_t n, const uint2* d_in, uint2* d_out, size_t* smem) {
     const uint32_t Gr = e->hi - e->lo;
     if (Gr == 0 || Gr > kBfMaxGpus) return ISL_ERANGE;
     const uint32_t W0 = (Gr + 31) / 32, W1 = (W0 + 31) / 32, stride = W0 + W1;
     const bool in_smem = e->n_tables == 1 && Gr <= kBfSmemGpus;
-    const size_t smem = in_smem ? (size_t)256 * stride * sizeof(uint32_t) : 0;
+    *smem = in_smem ? (size_t)256 * stride * sizeof(uint32_t) : 0;
     if (!in_smem) {         // class bitmaps in global memory: one set of 256 per table, zeroed here (HBM speed) instead of by the lone CTA
         const size_t words = (size_t)256 * e->n_tables * stride;
         if (words > e->bf_words) {
@@ -254,9 +254,32 @@ int run_bestfit(isl_engine* e, uint32_t n, const uint2* d_in, uint2* d_out) {
                                                                   e->prof, e->d_tile_counts, e->d_ctrl, nullptr, nullptr, 0, 0);
     if (int rc = check_launch(e, "k_prepare")) return rc;
     if (timing) cudaEventRecord(e->ev[1], e->stream);
+    return ISL_OK;
+}
+
+// ISL_POLICY_BEST_FIT: frees + defaults, then the request-major class-bitmap kernel (one CTA).
+int run_bestfit(isl_engine* e, uint32_t n, const uint2* d_in, uint2* d_out) {
+    if (n == 0) return ISL_OK;
+    size_t smem;
+    if (int rc = prepare_bestfit(e, n, d_in, d_out, &smem)) return rc;
     if (e->n_tables == 1) k_bestfit<false><<<1, kBfThreads, smem, e->stream>>>(n, d_in, d_out, e->d_occ, e->lo, e->hi, e->d_lut, e->prof, e->d_bf_bitmaps, e->d_ctrl, e->d_score, e->d_gtab, e->d_sizes, 1);
     else k_bestfit<true><<<1, kBfThreads, 0, e->stream>>>(n, d_in, d_out, e->d_occ, e->lo, e->hi, e->d_lut, e->prof, e->d_bf_bitmaps, e->d_ctrl, e->d_score, e->d_gtab, e->d_sizes, e->n_tables);
     if (int rc = check_launch(e, "k_bestfit")) return rc;
+    finish_batch(e, n, true);
+    return ISL_OK;
+}
+
+// isl_place_gangs, every policy: frees + defaults, then k_bestfit's gang instantiation over the n_gangs + 1 offsets at d_gang_off.
+int run_gangs(isl_engine* e, uint32_t n_gangs, const uint32_t* d_gang_off, uint32_t n, const uint2* d_in, uint2* d_out) {
+    size_t smem;
+    if (int rc = prepare_bestfit(e, n, d_in, d_out, &smem)) return rc;
+    if (e->n_tables == 1)
+        k_bestfit<false, true><<<1, kBfThreads, smem, e->stream>>>(n, d_in, d_out, e->d_occ, e->lo, e->hi, e->d_lut, e->prof, e->d_bf_bitmaps, e->d_ctrl, e->d_score,
+                                                                   e->d_gtab, e->d_sizes, 1, d_gang_off, n_gangs);
+    else
+        k_bestfit<true, true><<<1, kBfThreads, 0, e->stream>>>(n, d_in, d_out, e->d_occ, e->lo, e->hi, e->d_lut, e->prof, e->d_bf_bitmaps, e->d_ctrl, e->d_score,
+                                                               e->d_gtab, e->d_sizes, e->n_tables, d_gang_off, n_gangs);
+    if (int rc = check_launch(e, "k_bestfit (gangs)")) return rc;
     finish_batch(e, n, true);
     return ISL_OK;
 }
@@ -836,6 +859,7 @@ int isl_create(const isl_config* cfg, isl_engine** out) {
         cudaFuncAttributes fa;
         const void* kernels[] = {(const void*)k_prepare, (const void*)k_partition, (const void*)k_set_flag, (const void*)k_few, (const void*)k_build_lut, (const void*)k_eval_starts,
                                  (const void*)k_free_spans, (const void*)k_capacity, (const void*)k_sweep_count, (const void*)k_sweep_scatter, (const void*)k_commit, (const void*)k_bestfit<false>, (const void*)k_bestfit<true>,
+                                 (const void*)k_bestfit<false, true>, (const void*)k_bestfit<true, true>,
                                  (const void*)k_chain<1>, (const void*)k_chain<2>, (const void*)k_chain<4>, (const void*)k_small<1>, (const void*)k_small<2>, (const void*)k_small<4>};
         const void* pipes[] = {(const void*)k_pipeline<1, false, false>, (const void*)k_pipeline<1, true, false>, (const void*)k_pipeline<2, false, false>, (const void*)k_pipeline<2, true, false>,
                                (const void*)k_pipeline<4, false, false>, (const void*)k_pipeline<4, true, false>,
@@ -847,7 +871,8 @@ int isl_create(const isl_config* cfg, isl_engine** out) {
         // skip devices 8.. and race between threads)
         const void* chains[] = {(const void*)k_chain<1>, (const void*)k_chain<2>, (const void*)k_chain<4>};
         for (const void* k : chains) ISL_TRY(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(kQCap * sizeof(uint16_t))));
-        ISL_TRY(cudaFuncSetAttribute((const void*)k_bestfit<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(256 * (kBfSmemGpus / 32 + kBfSmemGpus / 1024) * sizeof(uint32_t))));
+        for (const void* k : {(const void*)k_bestfit<false>, (const void*)k_bestfit<false, true>})
+            ISL_TRY(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(256 * (kBfSmemGpus / 32 + kBfSmemGpus / 1024) * sizeof(uint32_t))));
         for (const void* k : pipes) ISL_TRY(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kPipeSmem));
     }
     e->occ_bytes = ((size_t)cfg->max_gpus + kSweepBlock - 1) / kSweepBlock * kSweepBlock;
@@ -983,9 +1008,10 @@ static int load_tables(isl_engine* e, uint32_t n_tables, uint32_t n, const isl_p
         for (uint32_t t = 0; t < n_tables; ++t) for (uint32_t p = 0; p < n; ++p) sizes[t * ISL_MAX_PROFILES + p] = e->rows_all[t][p].size;
         ISL_CUDA(e, cudaMemcpyAsync(e->d_sizes, sizes, sizeof(sizes), cudaMemcpyHostToDevice, e->stream));
     }
-    {   // what a best-fit family policy minimises, per table
+    {   // what a best-fit family policy minimises, per table; zero for first-fit and right-to-left, whose gangs (isl_place_gangs) run
+        // through the same kernel: its key is then the class minimum alone
         std::vector<uint8_t> score((size_t)ISL_MAX_TABLES * ISL_MAX_PROFILES * 256);      // the copy below completes before this function returns (stream sync)
-        for (uint32_t t = 0; t < n_tables; ++t) {
+        for (uint32_t t = 0; t < n_tables && bestfit_family(e->cfg.policy); ++t) {
             std::vector<uint32_t> cand;                              // every (profile, start) mask of the table the search can return
             for (uint32_t p = 0; p < n; ++p)
                 for (uint32_t k = 0; k < e->rows_all[t][p].n_starts; ++k)
@@ -1143,6 +1169,29 @@ int isl_place_batch_range(isl_engine* e, uint32_t lo, uint32_t hi, uint32_t n, c
     const int rc = place_batch_locked(e, n, in, out);
     e->lo = lo0; e->hi = hi0;
     return rc;
+}
+
+int isl_place_gangs(isl_engine* e, uint32_t n_gangs, const uint32_t* gang_off, const isl_request* in, isl_result* out) {
+    if (!e || (n_gangs && !gang_off)) return ISL_EINVAL;
+    if (gang_off && gang_off[0] != 0) return ISL_EINVAL;
+    for (uint32_t i = 0; i < n_gangs; ++i) if (gang_off[i + 1] <= gang_off[i]) return ISL_EINVAL;      // no empty gang
+    const uint32_t n = n_gangs ? gang_off[n_gangs] : 0;
+    if (n && (!in || !out)) return ISL_EINVAL;
+    if (e->cfg.flags & ISL_FLAG_ALL_NODES) return ISL_EINVAL;      // one pod on every node with capacity: no all-or-nothing meaning
+    if (n > e->cfg.max_batch) return ISL_ERANGE;
+    if (int rc = validate_ready(e, n)) return rc;
+    if (n == 0) return ISL_OK;
+    std::lock_guard<std::mutex> lk(e->mu);
+    DeviceGuard guard(e->device);
+    if (e->hi - e->lo > kBfMaxGpus) return ISL_ERANGE;          // the class bitmaps of k_bestfit
+    if (int rc = ensure_scratch(e, ((size_t)n_gangs + 1) * sizeof(uint32_t))) return rc;
+    uint32_t* d_gang_off = reinterpret_cast<uint32_t*>(e->d_scratch);
+    ISL_CUDA(e, cudaMemcpyAsync(d_gang_off, gang_off, ((size_t)n_gangs + 1) * sizeof(uint32_t), cudaMemcpyHostToDevice, e->stream));
+    ISL_CUDA(e, cudaMemcpyAsync(e->d_req, in, (size_t)n * sizeof(isl_request), cudaMemcpyHostToDevice, e->stream));
+    if (int rc = run_gangs(e, n_gangs, d_gang_off, n, e->d_req, e->d_res)) return rc;
+    ISL_CUDA(e, cudaMemcpyAsync(out, e->d_res, (size_t)n * sizeof(isl_result), cudaMemcpyDeviceToHost, e->stream));
+    ISL_CUDA(e, cudaStreamSynchronize(e->stream));
+    return ISL_OK;
 }
 
 static int place_batch_plain(isl_engine* e, uint32_t n, const isl_request* in, isl_result* out);

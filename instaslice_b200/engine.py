@@ -26,7 +26,7 @@ POLICY_FIRST_FIT, POLICY_BEST_FIT, POLICY_RIGHT_TO_LEFT, POLICY_MIN_FRAG = 0, 1,
 QUIRK_STRICT_BOUND, QUIRK_POW2_ONLY = 1, 2
 QUIRKS_REF_EXACT, QUIRKS_FIXED = 3, 0
 OP_ALLOC, OP_FREE, OP_NOOP = 0, 1, 2
-ST_PLACED, ST_NO_CAPACITY, ST_BAD_PROFILE, ST_FREED, ST_BAD_SPAN, ST_NOOP = 0, 1, 2, 3, 4, 5
+ST_PLACED, ST_NO_CAPACITY, ST_BAD_PROFILE, ST_FREED, ST_BAD_SPAN, ST_NOOP, ST_GANG_ABORTED = 0, 1, 2, 3, 4, 5, 6
 FLAG_TIMING, FLAG_NO_PIPELINE, FLAG_FORCE_PIPELINE, FLAG_TRACE, FLAG_NO_SMALL, FLAG_ALL_NODES = 1, 2, 4, 8, 16, 32
 SPEC_AUTO, SPEC_OFF, SPEC_ON = 0, 1, 2
 
@@ -94,6 +94,7 @@ SIGNATURES = {
     "isl_last_cuda_error": (C.c_char_p, [_P]),
     "isl_abi_version": (C.c_uint32, []),
     "isl_place_batch_range": (C.c_int, [_P, C.c_uint32, C.c_uint32, C.c_uint32, _P, _P]),
+    "isl_place_gangs": (C.c_int, [_P, C.c_uint32, _P, _P, _P]),
     "isl_stream_open": (C.c_int, [_P, C.c_uint32]),
     "isl_stream_submit": (C.c_int, [_P, C.c_uint32, _P, _P, C.POINTER(C.c_uint32)]),
     "isl_stream_wait": (C.c_int, [_P, C.c_uint32]),
@@ -322,6 +323,18 @@ class Engine:
         if out is None:
             out = np.empty(len(requests), dtype=RESULT_DTYPE)
         self._check(self._lib.isl_place_batch_range(self._h, lo, hi, len(requests), _ptr(requests), _ptr(out)), "isl_place_batch_range")
+        return out
+
+    def place_gangs(self, requests: np.ndarray, gang_off) -> np.ndarray:
+        """All-or-nothing groups: gang i is ``requests[gang_off[i]:gang_off[i + 1]]`` (``gang_off[0] == 0``, no empty gang, the last
+        offset is ``len(requests)``).  A gang commits only when every ALLOC member is placed; otherwise the first member that did not fit
+        keeps its record and every other ALLOC member reports ``ST_GANG_ABORTED`` (include/islplace.h)."""
+        requests = np.ascontiguousarray(requests, dtype=REQUEST_DTYPE)
+        gang_off = np.ascontiguousarray(gang_off, dtype=np.uint32)
+        if len(gang_off) == 0 or int(gang_off[-1]) != len(requests):
+            raise ValueError("gang_off must have n_gangs + 1 entries ending at len(requests)")
+        out = np.empty(len(requests), dtype=RESULT_DTYPE)
+        self._check(self._lib.isl_place_gangs(self._h, len(gang_off) - 1, _ptr(gang_off), _ptr(requests), _ptr(out)), "isl_place_gangs")
         return out
 
     # -- open streams (the causal feed)

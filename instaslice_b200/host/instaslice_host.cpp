@@ -150,13 +150,18 @@ uint32_t InstasliceReconciler::getStartIndexFromPreparedState(const Instaslice& 
     return start;
 }
 
-std::vector<isl_result> InstasliceReconciler::place(const std::vector<std::string>& names, uint32_t lo, uint32_t hi) {
+std::vector<isl_request> InstasliceReconciler::requests(const std::vector<std::string>& names) const {
     std::vector<isl_request> req(names.size());
-    std::vector<isl_result> res(names.size());
     for (size_t i = 0; i < names.size(); ++i) {
         auto it = profiles_.find(names[i]);
         req[i] = isl_request{(uint32_t)i, it == profiles_.end() ? (uint8_t)ISL_PROFILE_UNKNOWN : it->second, (uint8_t)ISL_OP_ALLOC, 0, 0};
     }
+    return req;
+}
+
+std::vector<isl_result> InstasliceReconciler::place(const std::vector<std::string>& names, uint32_t lo, uint32_t hi) {
+    std::vector<isl_request> req = requests(names);
+    std::vector<isl_result> res(names.size());
     // restriction, placement and restore under ONE engine lock: nothing leaks when the call throws, two callers cannot interleave
     check(isl_place_batch_range(h_, lo, hi, (uint32_t)req.size(), req.data(), res.data()), h_, "isl_place_batch_range");
     return res;
@@ -180,24 +185,71 @@ bool InstasliceReconciler::findDeviceForASlice(const InstasliceList& list, size_
     return true;
 }
 
-Outcome InstasliceReconciler::commitOrVeto(InstasliceList& list, AllocationPolicy& policy, const PendingPod& p, const isl_result& r) {
-    Outcome o;
-    Instaslice& is = list.Items[gpuNode_[r.gpu]];
+AllocationDetails InstasliceReconciler::pack(const InstasliceList& list, AllocationPolicy& policy, const PendingPod& p, const isl_result& r) {
+    const Instaslice& is = list.Items[gpuNode_[r.gpu]];
     int size, gi, ci, cieng;
     extractGpuProfile(is, p.ProfileName, &size, &gi, &ci, &cieng);
-    o.alloc = policy.SetAllocationDetails(p.ProfileName, r.start, (uint32_t)size, p.pod.UID, is.Name, "creating", gi, ci, cieng, p.pod.Namespace,
-                                          p.pod.Name, gpuUUID_[r.gpu]);
-    for (const auto& kv : is.Spec.Prepared) {                      // :198-203 exact-match veto
+    return policy.SetAllocationDetails(p.ProfileName, r.start, (uint32_t)size, p.pod.UID, is.Name, "creating", gi, ci, cieng, p.pod.Namespace,
+                                       p.pod.Name, gpuUUID_[r.gpu]);
+}
+
+bool InstasliceReconciler::vetoed(const InstasliceList& list, const isl_result& r, const AllocationDetails& a) const {
+    for (const auto& kv : list.Items[gpuNode_[r.gpu]].Spec.Prepared) {     // :198-203 exact-match veto
         const PreparedDetails& item = kv.second;
-        if (item.Parent == o.alloc.GPUUUID && item.Size == o.alloc.Size && item.Start == o.alloc.Start) {
-            releaseSpan(r);
-            o.verdict = Verdict::Veto;
-            return o;
-        }
+        if (item.Parent == a.GPUUUID && item.Size == a.Size && item.Start == a.Start) return true;
     }
-    is.Spec.Allocations[p.pod.UID] = o.alloc;                      // :215-219 (r.Update)
+    return false;
+}
+
+Outcome InstasliceReconciler::commitOrVeto(InstasliceList& list, AllocationPolicy& policy, const PendingPod& p, const isl_result& r) {
+    Outcome o;
+    o.alloc = pack(list, policy, p, r);
+    if (vetoed(list, r, o.alloc)) {
+        releaseSpan(r);
+        o.verdict = Verdict::Veto;
+        return o;
+    }
+    list.Items[gpuNode_[r.gpu]].Spec.Allocations[p.pod.UID] = o.alloc;     // :215-219 (r.Update)
     o.verdict = Verdict::Placed;
     return o;
+}
+
+std::vector<GangOutcome> InstasliceReconciler::PlaceGangs(InstasliceList& list, AllocationPolicy& policy, const std::vector<std::vector<PendingPod>>& gangs) {
+    std::vector<GangOutcome> out(gangs.size());
+    if (gangs.empty()) return out;
+    if (orphans_ && gangs.size() > 1) {         // the veto must see one gang at a time: a vetoed gang leaves no trace before the next
+        for (size_t g = 0; g < gangs.size(); ++g) out[g] = PlaceGangs(list, policy, {gangs[g]})[0];
+        return out;
+    }
+    std::vector<std::string> names;
+    std::vector<uint32_t> off{0};
+    for (const auto& gang : gangs) {
+        if (gang.empty()) throw std::runtime_error("empty gang");
+        for (const PendingPod& p : gang) names.push_back(p.ProfileName);
+        off.push_back((uint32_t)names.size());
+    }
+    const std::vector<isl_request> req = requests(names);
+    std::vector<isl_result> res(names.size());
+    check(isl_place_gangs(h_, (uint32_t)gangs.size(), off.data(), req.data(), res.data()), h_, "isl_place_gangs");
+    for (size_t g = 0; g < gangs.size(); ++g) {
+        bool placed = true, veto = false;
+        for (uint32_t i = off[g]; i < off[g + 1]; ++i) placed = placed && res[i].status == ISL_ST_PLACED;
+        if (!placed) continue;                  // nothing of the gang was committed
+        GangOutcome& o = out[g];
+        for (uint32_t i = off[g]; i < off[g + 1]; ++i) {
+            o.allocs.push_back(pack(list, policy, gangs[g][i - off[g]], res[i]));
+            veto = veto || vetoed(list, res[i], o.allocs.back());
+        }
+        if (veto) {                             // one member vetoed: every span of the gang is released again
+            for (uint32_t i = off[g]; i < off[g + 1]; ++i) releaseSpan(res[i]);
+            o.allocs.clear();
+            o.verdict = Verdict::Veto;
+            continue;
+        }
+        for (uint32_t i = off[g]; i < off[g + 1]; ++i) list.Items[gpuNode_[res[i].gpu]].Spec.Allocations[gangs[g][i - off[g]].pod.UID] = o.allocs[i - off[g]];
+        o.verdict = Verdict::Placed;
+    }
+    return out;
 }
 
 std::vector<Outcome> InstasliceReconciler::PlacePending(InstasliceList& list, AllocationPolicy& policy, const std::vector<PendingPod>& pods) {

@@ -8,6 +8,7 @@
 //   InstasliceReconciler::extractGpuProfile              :283-300
 //   AllocationPolicy / FirstFitPolicy / LeftToRightPolicy / RightToLeftPolicy  :48-56, :436-469
 //   InstasliceReconciler::PlacePending                   node loop + Prepared veto of Reconcile :188-232, batched
+//   InstasliceReconciler::PlaceGangs                     the same for all-or-nothing pod groups (extension: isl_place_gangs)
 // Types follow api/v1alpha1/instaslice_types.go:23-72.  Nothing here decides a placement: every decision comes
 // back from libislplace.so.  The Go twin of this file is integration/go/placement_engine.go.
 #pragma once
@@ -70,6 +71,7 @@ struct RightToLeftPolicy : LeftToRightPolicy {}; // :464-469
 enum class Verdict { Placed, None, Veto };       // allocation written / "failed to find allocatable gpu" everywhere / :198-203 requeue
 struct PendingPod { Pod pod; std::string ProfileName; };
 struct Outcome { Verdict verdict = Verdict::None; AllocationDetails alloc; };
+struct GangOutcome { Verdict verdict = Verdict::None; std::vector<AllocationDetails> allocs; };   // allocs: one per pod when Placed
 
 extern const char* const kErrNoGpu;              // "failed to find allocatable gpu" (:261)
 
@@ -95,6 +97,10 @@ public:
                              AllocationDetails* out, std::string* err);
     // Reconcile's node loop for many gated pods in order, ONE engine call; allocations are written into `list`.
     std::vector<Outcome> PlacePending(InstasliceList& list, AllocationPolicy& policy, const std::vector<PendingPod>& pods);
+    // All-or-nothing pod groups in order, ONE engine call (isl_place_gangs): a gang is Placed only when every pod of it got a slice, and
+    // only then are its allocations written into `list`.  None: a pod found no GPU, nothing of the gang was committed.  Veto: the
+    // Prepared exact-match check (:198-203) fired on a pod, every span of the gang was released again.  Empty gangs throw.
+    std::vector<GangOutcome> PlaceGangs(InstasliceList& list, AllocationPolicy& policy, const std::vector<std::vector<PendingPod>>& gangs);
     // The daemonset removed Allocations[podUID] (instaslice_daemonset.go:261-263).
     bool Release(InstasliceList& list, const std::string& podUID);
 
@@ -108,8 +114,11 @@ private:
     std::map<std::string, uint8_t> profiles_;
     std::map<std::string, uint32_t> gpuIndex_;
     bool orphans_ = false;
+    std::vector<isl_request> requests(const std::vector<std::string>& names) const;
     std::vector<isl_result> place(const std::vector<std::string>& names, uint32_t lo, uint32_t hi);
     void releaseSpan(const isl_result& r);
+    AllocationDetails pack(const InstasliceList& list, AllocationPolicy& policy, const PendingPod& p, const isl_result& r);
+    bool vetoed(const InstasliceList& list, const isl_result& r, const AllocationDetails& a) const;
     Outcome commitOrVeto(InstasliceList& list, AllocationPolicy& policy, const PendingPod& p, const isl_result& r);
 };
 

@@ -337,6 +337,88 @@ func (r *InstasliceReconciler) PlacePending(e *PlacementEngine, list *inferencev
 	return out, nil
 }
 
+// PlaceGangs resolves all-or-nothing pod groups (the replicas of one deployment, the workers of one job) in order with ONE
+// engine call (isl_place_gangs).  result[g] holds one AllocationDetails per pod of gang g, or is nil when the gang was not placed:
+// a pod found no GPU (nothing of the gang was committed; requeue), or the Prepared exact-match veto (:198-203) fired on a pod, in
+// which case every node the gang touched is rebuilt from the CR, which holds none of its allocations.  As in PlacePending the
+// caller writes the returned allocations (r.Update).  Empty gangs are an error.
+func (r *InstasliceReconciler) PlaceGangs(e *PlacementEngine, list *inferencev1alpha1.InstasliceList, policy AllocationPolicy,
+	gangs [][]PendingPod) ([][]*inferencev1alpha1.AllocationDetails, error) {
+	out := make([][]*inferencev1alpha1.AllocationDetails, len(gangs))
+	if len(gangs) == 0 {
+		return out, nil
+	}
+	n := 0
+	for _, g := range gangs {
+		if len(g) == 0 {
+			return nil, fmt.Errorf("empty gang")
+		}
+		n += len(g)
+	}
+	if e.orphans && len(gangs) > 1 { // the exact-match veto (:198-203) must see one gang at a time
+		for g := range gangs {
+			one, err := r.PlaceGangs(e, list, policy, gangs[g:g+1])
+			if err != nil {
+				return nil, err
+			}
+			out[g] = one[0]
+		}
+		return out, nil
+	}
+	reqP, resP := C.malloc(C.size_t(n)*C.sizeof_isl_request), C.malloc(C.size_t(n)*C.sizeof_isl_result)
+	offP := C.malloc(C.size_t(len(gangs)+1) * 4)
+	if reqP == nil || resP == nil || offP == nil {
+		C.free(reqP)
+		C.free(resP)
+		C.free(offP)
+		return nil, fmt.Errorf("out of memory")
+	}
+	defer C.free(reqP)
+	defer C.free(resP)
+	defer C.free(offP)
+	req := (*[1 << 28]C.isl_request)(reqP)[:n:n]
+	res := (*[1 << 28]C.isl_result)(resP)[:n:n]
+	off := (*[1 << 28]C.uint32_t)(offP)[: len(gangs)+1 : len(gangs)+1]
+	off[0] = 0
+	for g, pods := range gangs {
+		e.fillRequests(req, pods, int(off[g]))
+		off[g+1] = off[g] + C.uint32_t(len(pods))
+	}
+	if rc := C.isl_place_gangs(e.h, C.uint32_t(len(gangs)), &off[0], &req[0], &res[0]); rc != C.ISL_OK {
+		return nil, fmt.Errorf("isl_place_gangs: %s (%s)", C.GoString(C.isl_strerror(rc)), C.GoString(C.isl_last_cuda_error(e.h)))
+	}
+	for g, pods := range gangs {
+		gres := res[off[g]:off[g+1]]
+		placed := true
+		for i := range gres {
+			placed = placed && gres[i].status == C.ISL_ST_PLACED
+		}
+		if !placed {
+			continue
+		}
+		allocs := make([]*inferencev1alpha1.AllocationDetails, len(pods))
+		vetoed := false
+		for i, p := range pods {
+			a, err := r.commitOrVeto(e, list, policy, p, gres[i])
+			if err != nil {
+				return nil, err
+			}
+			vetoed = vetoed || a == nil
+			allocs[i] = a
+		}
+		if vetoed { // the whole gang goes: rebuild every node it touched
+			for i := range gres {
+				if err := e.UpdateNode(list, e.gpuNode[int(gres[i].gpu)]); err != nil {
+					return nil, err
+				}
+			}
+			continue
+		}
+		out[g] = allocs
+	}
+	return out, nil
+}
+
 // Release: the daemonset removed Allocations[podUID] from list.Items[n] (instaslice_daemonset.go:261-263).  The node's occupancy
 // bytes are REBUILT from the CR (OR over every remaining Prepared / Allocations entry, :306-328) rather than cleared blindly: if
 // another entry still covers part of the span, those slices stay busy — exactly what the reference's next rebuild would say.
