@@ -82,7 +82,7 @@ extern "C" {
 #define ISL_QUIRKS_REF_EXACT   (ISL_QUIRK_STRICT_BOUND | ISL_QUIRK_POW2_ONLY)
 #define ISL_QUIRKS_FIXED       0u
 
-/* isl_request.op */
+/* isl_request.op; any other value is treated as ISL_OP_NOOP (record status ISL_ST_NOOP) */
 #define ISL_OP_ALLOC 0u
 #define ISL_OP_FREE  1u
 #define ISL_OP_NOOP  2u
@@ -247,7 +247,13 @@ int  isl_place_stream_device(isl_engine* e, uint32_t n_batches, const uint32_t* 
 int  isl_place_batch_device(isl_engine* e, uint32_t n, const void* d_in, void* d_out);
 /* isl_place_batch restricted to the canonical GPU range [lo, hi) — findDeviceForASlice looks at ONE node's GPUs (:240-262), the node
  * loop (:190) calls it node after node.  Restriction, placement and restore happen under one engine lock (two reconcile workers
- * cannot interleave, nothing leaks when the call fails); the engine's own partition (isl_set_partition) is left untouched. */
+ * cannot interleave, nothing leaks when the call fails); the engine's own partition (isl_set_partition) is left untouched.
+ * Inside a restricted range (this call, isl_set_partition, each node pass of ISL_FLAG_ALL_NODES):
+ *   - a well-formed FREE naming a GPU outside [lo, hi) is reported ISL_ST_FREED and NOT applied (the rank that owns the GPU applies it;
+ *     the element-wise MIN merge of partitioned results relies on every rank reporting the same FREED record); a malformed one is BAD_SPAN;
+ *   - an unplaced ALLOC reports the size of the whole inventory's default row (first node, canonical order, whose table has the name),
+ *     not that of the first node of the range;
+ *   - an empty range (lo == hi) places nothing: ALLOCs NO_CAPACITY, FREEs FREED and not applied, on every policy. */
 int  isl_place_batch_range(isl_engine* e, uint32_t lo, uint32_t hi, uint32_t n, const isl_request* in, isl_result* out);
 /* All-or-nothing pod groups (the replicas of a deployment, the workers of a job).  `in` / `out` hold n = gang_off[n_gangs] requests and
  * records (host buffers, as isl_place_batch); gang i is in[gang_off[i] .. gang_off[i + 1]), gang_off[0] == 0, no gang is empty.
@@ -311,7 +317,9 @@ int  isl_eval_starts(isl_engine* e, uint32_t profile, uint32_t n, const uint8_t*
 /* ---- partitioned inventory (BASELINE config 4; DESIGN.md "Multi-GPU") ---- */
 /* Restrict this engine to the canonical GPU range [lo, hi) of the loaded
  * inventory.  The batch is resolved by chaining ranks in range order: rank d
- * starts from the per-profile queue heads rank d-1 ended with. */
+ * starts from the per-profile queue heads rank d-1 ended with.  Every single-engine entry point (batch, stream, open stream,
+ * isl_capacity, isl_what_if, isl_free_batch, gangs, the best-fit family) then sees [lo, hi) only, with the FREE and default-size rules
+ * of isl_place_batch_range; isl_free_batch skips spans outside the partition. */
 int  isl_set_partition(isl_engine* e, uint32_t lo, uint32_t hi);
 /* d_heads_in / d_heads_out: ISL_MAX_PROFILES uint32 each in device memory
  * (NULL d_heads_in = first rank).  Results of requests this rank did not place

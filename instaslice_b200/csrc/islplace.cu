@@ -231,14 +231,15 @@ int run_few(isl_engine* e, uint32_t n, const SmallReqs& inl, uint2* d_out) {
 }
 
 // What run_bestfit and run_gangs share in front of k_bestfit: the class bitmaps (shared memory up to kBfSmemGpus GPUs of one table, else
-// global memory zeroed here), then k_prepare (frees + default records).  *smem = the dynamic shared memory k_bestfit needs.
+// global memory zeroed here), then k_prepare (frees + default records).  *smem = the dynamic shared memory k_bestfit needs.  An empty
+// range has no class bitmaps: k_prepare's default records are the whole answer.
 int prepare_bestfit(isl_engine* e, uint32_t n, const uint2* d_in, uint2* d_out, size_t* smem) {
     const uint32_t Gr = e->hi - e->lo;
-    if (Gr == 0 || Gr > kBfMaxGpus) return ISL_ERANGE;
+    if (Gr > kBfMaxGpus) return ISL_ERANGE;
     const uint32_t W0 = (Gr + 31) / 32, W1 = (W0 + 31) / 32, stride = W0 + W1;
     const bool in_smem = e->n_tables == 1 && Gr <= kBfSmemGpus;
     *smem = in_smem ? (size_t)256 * stride * sizeof(uint32_t) : 0;
-    if (!in_smem) {         // class bitmaps in global memory: one set of 256 per table, zeroed here (HBM speed) instead of by the lone CTA
+    if (!in_smem && Gr) {   // class bitmaps in global memory: one set of 256 per table, zeroed here (HBM speed) instead of by the lone CTA
         const size_t words = (size_t)256 * e->n_tables * stride;
         if (words > e->bf_words) {
             if (e->d_bf_bitmaps) cudaFree(e->d_bf_bitmaps);
@@ -262,6 +263,7 @@ int run_bestfit(isl_engine* e, uint32_t n, const uint2* d_in, uint2* d_out) {
     if (n == 0) return ISL_OK;
     size_t smem;
     if (int rc = prepare_bestfit(e, n, d_in, d_out, &smem)) return rc;
+    if (e->hi == e->lo) { finish_batch(e, n, true); return ISL_OK; }     // empty range: ALLOCs NO_CAPACITY, every FREE outside it
     if (e->n_tables == 1) k_bestfit<false><<<1, kBfThreads, smem, e->stream>>>(n, d_in, d_out, e->d_occ, e->lo, e->hi, e->d_lut, e->prof, e->d_bf_bitmaps, e->d_ctrl, e->d_score, e->d_gtab, e->d_sizes, 1);
     else k_bestfit<true><<<1, kBfThreads, 0, e->stream>>>(n, d_in, d_out, e->d_occ, e->lo, e->hi, e->d_lut, e->prof, e->d_bf_bitmaps, e->d_ctrl, e->d_score, e->d_gtab, e->d_sizes, e->n_tables);
     if (int rc = check_launch(e, "k_bestfit")) return rc;
@@ -1183,7 +1185,7 @@ int isl_place_gangs(isl_engine* e, uint32_t n_gangs, const uint32_t* gang_off, c
     if (n == 0) return ISL_OK;
     std::lock_guard<std::mutex> lk(e->mu);
     DeviceGuard guard(e->device);
-    if (e->hi - e->lo > kBfMaxGpus) return ISL_ERANGE;          // the class bitmaps of k_bestfit
+    if (e->hi == e->lo || e->hi - e->lo > kBfMaxGpus) return ISL_ERANGE;          // the class bitmaps of k_bestfit
     if (int rc = ensure_scratch(e, ((size_t)n_gangs + 1) * sizeof(uint32_t))) return rc;
     uint32_t* d_gang_off = reinterpret_cast<uint32_t*>(e->d_scratch);
     ISL_CUDA(e, cudaMemcpyAsync(d_gang_off, gang_off, ((size_t)n_gangs + 1) * sizeof(uint32_t), cudaMemcpyHostToDevice, e->stream));

@@ -242,8 +242,8 @@ int orc_f_place(orc_faithful* h, uint32_t n, const isl_request* in, isl_result* 
     const uint32_t G = (uint32_t)h->gpu_uuid.size();
     // canonical batch: FREEs first (an Allocations entry deleted by the daemonset, instaslice_daemonset.go:261-263)
     for (uint32_t i = 0; i < n; ++i) {
-        if (in[i].op == ISL_OP_NOOP) { out[i] = {ISL_GPU_NONE, (uint8_t)ISL_START_NONE, 0, (uint16_t)ISL_ST_NOOP}; continue; }
-        if (in[i].op != ISL_OP_FREE) continue;
+        if (in[i].op == ISL_OP_ALLOC) continue;
+        if (in[i].op != ISL_OP_FREE) { out[i] = {ISL_GPU_NONE, (uint8_t)ISL_START_NONE, 0, (uint16_t)ISL_ST_NOOP}; continue; }   // NOOP and any unknown op
         const uint32_t g = in[i].handle, st = in[i].start, sz = in[i].size;
         if (g >= G || sz == 0 || st + sz > ISL_SLOTS) { out[i] = {g, (uint8_t)st, (uint8_t)sz, (uint16_t)ISL_ST_BAD_SPAN}; continue; }
         const uint64_t key = orc_faithful::span_key(g, st, sz);

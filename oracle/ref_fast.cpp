@@ -93,8 +93,8 @@ void orc_fast_occupancy(orc_fast* h, uint8_t* out) { std::copy(h->occ.begin(), h
 
 int orc_fast_place(orc_fast* h, uint32_t n, const isl_request* in, isl_result* out) {
     for (uint32_t i = 0; i < n; ++i) {                              // canonical batch: FREEs first
-        if (in[i].op == ISL_OP_NOOP) { out[i] = {ISL_GPU_NONE, (uint8_t)ISL_START_NONE, 0, (uint16_t)ISL_ST_NOOP}; continue; }
-        if (in[i].op != ISL_OP_FREE) continue;
+        if (in[i].op == ISL_OP_ALLOC) continue;
+        if (in[i].op != ISL_OP_FREE) { out[i] = {ISL_GPU_NONE, (uint8_t)ISL_START_NONE, 0, (uint16_t)ISL_ST_NOOP}; continue; }   // NOOP and any unknown op
         const uint32_t g = in[i].handle, st = in[i].start, sz = in[i].size;
         if (g >= h->G || sz == 0 || st + sz > ISL_SLOTS) { out[i] = {g, (uint8_t)st, (uint8_t)sz, (uint16_t)ISL_ST_BAD_SPAN}; continue; }
         h->occ[g] &= (uint8_t)~(((1u << sz) - 1u) << st);
