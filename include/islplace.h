@@ -116,7 +116,8 @@ typedef struct isl_config {
 #define ISL_FLAG_FORCE_PIPELINE 4u  /* use the segment pipeline even for a single chunk (tests) */
 #define ISL_FLAG_ALL_NODES     32u  /* isl_place_batch reproduces the reference's missing `break` (:190-227, SURVEY Q5): a pod is allocated on EVERY
                                        node that has capacity (state effect); the record reports the first node.  One restricted pass per node —
-                                       a compatibility mode for parity studies, not a fast path */
+                                       a compatibility mode for parity studies, not a fast path.  isl_place_batch_range and isl_what_if
+                                       follow it; the stream calls and isl_place_batch_device place each pod once, isl_place_gangs is EINVAL */
 
 /* One Migplacement row (api/v1alpha1/instaslice_types.go:23-29).  `size` is
  * Placements[0].Size (:334); `starts` is [p.Start for p in Placements] in CRD
@@ -195,7 +196,8 @@ int  isl_synchronize(isl_engine* e);
 
 /* ---- tables and inventory --------------------------------------------- */
 /* Replaces reading instaslice.Spec.Migplacement (:332-340, :288-298). Builds the
- * per-(profile, occupancy byte) first-start table on the device. */
+ * per-(profile, occupancy byte) first-start table on the device.  Loading tables (this call or isl_load_profile_tables) resets every
+ * node to table 0: call isl_set_node_tables again after it.  The inventory, the partition and a snapshot are kept. */
 int  isl_load_profiles(isl_engine* e, uint32_t n, const isl_profile* rows);
 /* Heterogeneous cluster: every node publishes its OWN Migplacement (instaslice_daemonset.go:588-664), and the reference
  * looks a profile up in the table of the node it is scanning (:332-340).  rows[t * n_profiles + p] is the row of profile
@@ -206,7 +208,8 @@ int  isl_load_profile_tables(isl_engine* e, uint32_t n_tables, uint32_t n_profil
 int  isl_set_node_tables(isl_engine* e, uint32_t n_nodes, const uint8_t* table_of_node);
 /* Replaces the occupancy rebuild (:306-328) for every GPU of every node.
  * node_off has n_nodes+1 entries (node i owns GPUs [node_off[i], node_off[i+1]));
- * occ has node_off[n_nodes] bytes.  This is also "resume": the CR is the checkpoint. */
+ * occ has node_off[n_nodes] bytes.  This is also "resume": the CR is the checkpoint.
+ * It resets the partition to [0, G), every node to table 0 (isl_set_node_tables) and drops a snapshot (isl_snapshot_occupancy). */
 int  isl_load_inventory(isl_engine* e, uint32_t n_nodes, const uint32_t* node_off, const uint8_t* occ);
 int  isl_read_occupancy(isl_engine* e, uint8_t* out /* G bytes */);
 /* Incremental sync: overwrite the occupancy bytes of canonical GPUs [first_gpu, first_gpu + n) — what the shim does
@@ -215,7 +218,9 @@ int  isl_read_occupancy(isl_engine* e, uint8_t* out /* G bytes */);
 int  isl_write_occupancy(isl_engine* e, uint32_t first_gpu, uint32_t n, const uint8_t* occ);
 /* What-if queries (defragmentation planning, SURVEY 8f-4): isl_snapshot_occupancy keeps a device-side copy of the whole
  * occupancy, any number of isl_place_* / isl_free_batch calls then run against the live state, isl_restore_occupancy puts the
- * snapshot back (a 1-byte-per-GPU device copy, no host round trip).  ISL_ESTATE if there is no inventory / no snapshot. */
+ * snapshot back (a 1-byte-per-GPU device copy, no host round trip).  ISL_ESTATE if there is no inventory / no snapshot.
+ * A snapshot is the whole occupancy and outlives placement calls, open streams, isl_free_batch, isl_write_occupancy, isl_set_partition
+ * and table reloads; isl_load_inventory and isl_what_if drop it, and it can be restored any number of times. */
 int  isl_snapshot_occupancy(isl_engine* e);
 int  isl_restore_occupancy(isl_engine* e);
 /* cap[p] (ISL_MAX_PROFILES entries) = how many more pods of profile p ALONE the inventory (the engine's partition) could still take:
@@ -284,7 +289,10 @@ int  isl_place_gangs(isl_engine* e, uint32_t n_gangs, const uint32_t* gang_off, 
  *   isl_stream_wait(e, ticket)                 returns when that batch's results are in `out`
  *   isl_stream_close(e)                        end of stream: the kernel drains, the occupancy is written back
  * Results are exactly those of isl_place_batch per batch in submission order.  Batches submitted before earlier ones are waited for
- * overlap on the device (segment pipeline).  While a stream is open every other call on the engine returns ISL_ESTATE. */
+ * overlap on the device (segment pipeline).  While a stream is open (isl_stream_open until isl_stream_close, launched or not) every
+ * call on the engine returns ISL_ESTATE and changes nothing, except: isl_stream_submit, _wait and _close, isl_destroy (closes the stream
+ * first), and isl_num_gpus, isl_gpu_to_node, isl_device_occupancy, isl_device_results, isl_abi_version, isl_strerror,
+ * isl_last_cuda_error, isl_host_alloc and isl_host_free.  The test is made under the engine lock. */
 int  isl_stream_open(isl_engine* e, uint32_t max_batches);
 int  isl_stream_submit(isl_engine* e, uint32_t n, const isl_request* in, isl_result* out, uint32_t* ticket);
 int  isl_stream_wait(isl_engine* e, uint32_t ticket);

@@ -739,10 +739,40 @@ int run_stream(isl_engine* e, uint32_t n_batches, const uint32_t* sizes, const u
     return ISL_OK;
 }
 
+// The engine lock of every entry point except the stream calls and the pure getters, refused while an open stream owns the engine: its
+// resident kernel would keep any work enqueued behind it waiting until isl_stream_close, and the state it runs on must not change under
+// it.  The test runs under the lock, so no call can slip in after another thread's isl_stream_open.
+int lock_idle(isl_engine* e, std::unique_lock<std::mutex>& lk) {
+    lk = std::unique_lock<std::mutex>(e->mu);
+    return e->open.active ? ISL_ESTATE : ISL_OK;
+}
+
+// under lock_idle
 int validate_ready(isl_engine* e, uint32_t n) {
     if (!e->have_profiles || !e->have_inventory) return ISL_ESTATE;
-    if (e->open.active) return ISL_ESTATE;         // an open stream owns the engine until isl_stream_close
     if (n > e->cfg.max_batch) return ISL_ERANGE;
+    return ISL_OK;
+}
+
+// Default row of every name (its size is what an unplaced ALLOC reports): the row of the first node, in canonical order, whose table has
+// the name; without a node map (isl_set_node_tables) every node uses table 0.
+void derive_default_rows(isl_engine* e) {
+    for (uint32_t p = 0; p < e->prof.n; ++p) {
+        e->prof.rows[p] = isl_profile{};
+        if (e->node_table.empty()) {
+            if (e->rows_all[0][p].n_starts) e->prof.rows[p] = e->rows_all[0][p];
+            continue;
+        }
+        for (const uint8_t t : e->node_table)
+            if (e->rows_all[t][p].n_starts) { e->prof.rows[p] = e->rows_all[t][p]; break; }
+    }
+}
+
+// Every node back to table 0: no node map, the per-GPU table bytes zeroed, default rows from table 0 (isl_load_inventory, table reloads).
+int reset_node_tables(isl_engine* e) {
+    e->node_table.clear();
+    ISL_CUDA(e, cudaMemsetAsync(e->d_gtab, 0, e->occ_bytes, e->stream));
+    derive_default_rows(e);
     return ISL_OK;
 }
 
@@ -765,14 +795,15 @@ void spec_disconnect(isl_engine* e) {
     e->spec_world = 0;
 }
 
-// The checks of the stream entry points: 1..4096 batches that fit max_batch, buffers for a non-empty stream, an engine that is ready.
+// The argument checks of the stream entry points: 1..4096 batches that fit max_batch, buffers for a non-empty stream.  The engine's
+// readiness is checked under the lock (lock_idle, validate_ready).
 int stream_entry(isl_engine* e, uint32_t n_batches, const uint32_t* sizes, bool have_buffers, uint64_t* total) {
     if (!e || !sizes || n_batches == 0 || n_batches > 4096) return ISL_EINVAL;
     *total = 0;
     for (uint32_t b = 0; b < n_batches; ++b) *total += sizes[b];
     if (*total && !have_buffers) return ISL_EINVAL;
     if (*total > e->cfg.max_batch) return ISL_ERANGE;
-    return validate_ready(e, (uint32_t)*total);
+    return ISL_OK;
 }
 
 // device copy of the live occupancy (isl_snapshot_occupancy, isl_what_if)
@@ -940,7 +971,8 @@ int isl_destroy(isl_engine* e) {
 
 int isl_set_stream(isl_engine* e, void* cuda_stream) {
     if (!e) return ISL_EINVAL;
-    std::lock_guard<std::mutex> lk(e->mu);
+    std::unique_lock<std::mutex> lk;
+    if (int rc = lock_idle(e, lk)) return rc;
     DeviceGuard guard(e->device);
     if (e->stream) ISL_CUDA(e, cudaStreamSynchronize(e->stream));
     if (e->own_stream && e->stream) { cudaStreamDestroy(e->stream); e->own_stream = false; }
@@ -951,6 +983,8 @@ int isl_set_stream(isl_engine* e, void* cuda_stream) {
 
 int isl_synchronize(isl_engine* e) {
     if (!e) return ISL_EINVAL;
+    std::unique_lock<std::mutex> lk;
+    if (int rc = lock_idle(e, lk)) return rc;
     DeviceGuard guard(e->device);
     ISL_CUDA(e, cudaStreamSynchronize(e->stream));
     return ISL_OK;
@@ -971,16 +1005,17 @@ static int load_tables(isl_engine* e, uint32_t n_tables, uint32_t n, const isl_p
         }
     }
     if (total_cand > kMaxCand) return ISL_EINVAL;          // more (table, profile, start) candidates than the chain's 4 x 32 lane slots
-    std::lock_guard<std::mutex> lk(e->mu);
+    std::unique_lock<std::mutex> lk;
+    if (int rc = lock_idle(e, lk)) return rc;
     DeviceGuard guard(e->device);
     e->n_tables = n_tables;
     memset(e->rows_all, 0, sizeof(e->rows_all));
     for (uint32_t t = 0; t < n_tables; ++t) memcpy(e->rows_all[t], rows + (size_t)t * n, n * sizeof(isl_profile));
     e->prof.n = n; e->prof.quirks = e->cfg.quirks; e->prof.flip = reversed(e) ? e->G : 0u;
     memset(e->prof.rows, 0, sizeof(e->prof.rows));
-    // default row of a name (its size is what an unplaced result reports) = the row of the first NODE in canonical order
-    // that knows the name; until isl_set_node_tables every node uses table 0
-    for (uint32_t p = 0; p < n; ++p) e->prof.rows[p] = e->rows_all[0][p];
+    // new tables, new node map: every node uses table 0 until isl_set_node_tables names the tables again (a map kept from the old
+    // tables could name a table that no longer exists, or one whose rows changed)
+    if (int rc = reset_node_tables(e)) return rc;
     // chain candidates: every (table, profile, start) the search can ever return, in row order
     memset(&e->tab, 0, sizeof(e->tab));
     uint32_t c = 0; e->cand_profiles = 0;
@@ -1051,10 +1086,11 @@ int isl_load_profile_tables(isl_engine* e, uint32_t n_tables, uint32_t n_profile
 
 int isl_set_node_tables(isl_engine* e, uint32_t n_nodes, const uint8_t* table_of_node) {
     if (!e || !table_of_node) return ISL_EINVAL;
+    std::unique_lock<std::mutex> lk;
+    if (int rc = lock_idle(e, lk)) return rc;
     if (!e->have_inventory || !e->have_profiles) return ISL_ESTATE;
     if (n_nodes + 1 != e->node_off.size()) return ISL_EINVAL;
     for (uint32_t n = 0; n < n_nodes; ++n) if (table_of_node[n] >= e->n_tables) return ISL_EINVAL;
-    std::lock_guard<std::mutex> lk(e->mu);
     DeviceGuard guard(e->device);
     e->node_table.assign(table_of_node, table_of_node + n_nodes);
     std::vector<uint8_t> gtab(e->G);
@@ -1062,11 +1098,7 @@ int isl_set_node_tables(isl_engine* e, uint32_t n_nodes, const uint8_t* table_of
         for (uint32_t g = e->node_off[n]; g < e->node_off[n + 1]; ++g) gtab[flip_gpu(g, e->prof.flip)] = table_of_node[n];
     ISL_CUDA(e, cudaMemcpyAsync(e->d_gtab, gtab.data(), e->G, cudaMemcpyHostToDevice, e->stream));
     ISL_CUDA(e, cudaStreamSynchronize(e->stream));
-    for (uint32_t p = 0; p < e->prof.n; ++p) {              // size reported for an unplaced request: first node (canonical order) that knows the name
-        e->prof.rows[p] = isl_profile{};
-        for (uint32_t n = 0; n < n_nodes; ++n)
-            if (e->rows_all[table_of_node[n]][p].n_starts) { e->prof.rows[p] = e->rows_all[table_of_node[n]][p]; break; }
-    }
+    derive_default_rows(e);
     return ISL_OK;
 }
 
@@ -1077,17 +1109,15 @@ int isl_load_inventory(isl_engine* e, uint32_t n_nodes, const uint32_t* node_off
     const uint32_t G = node_off[n_nodes];
     if (G == 0 || !occ) return ISL_EINVAL;
     if (G > e->cfg.max_gpus) return ISL_ERANGE;
-    if (e->open.active) return ISL_ESTATE;
-    std::lock_guard<std::mutex> lk(e->mu);
+    std::unique_lock<std::mutex> lk;
+    if (int rc = lock_idle(e, lk)) return rc;
     DeviceGuard guard(e->device);
     e->node_off.assign(node_off, node_off + n_nodes + 1);
     e->G = G; e->lo = 0; e->hi = G;
     e->prof.flip = reversed(e) ? G : 0u;      // ISL_POLICY_RIGHT_TO_LEFT: the inventory is stored in reverse canonical order
     e->snap_G = 0;                  // a snapshot belongs to the inventory it was taken from
     ISL_CUDA(e, cudaMemsetAsync(e->d_occ, 0xFF, e->occ_bytes, e->stream));
-    ISL_CUDA(e, cudaMemsetAsync(e->d_gtab, 0, e->occ_bytes, e->stream));        // every node uses table 0 until isl_set_node_tables
-    e->node_table.clear();
-    for (uint32_t p = 0; p < e->prof.n; ++p) e->prof.rows[p] = e->rows_all[0][p];
+    if (int rc = reset_node_tables(e)) return rc;      // every node uses table 0 until isl_set_node_tables
     std::vector<uint8_t> rev;
     if (e->prof.flip) { rev.assign(occ, occ + G); std::reverse(rev.begin(), rev.end()); occ = rev.data(); }
     ISL_CUDA(e, cudaMemcpyAsync(e->d_occ, occ, G, cudaMemcpyHostToDevice, e->stream));
@@ -1098,8 +1128,9 @@ int isl_load_inventory(isl_engine* e, uint32_t n_nodes, const uint32_t* node_off
 
 int isl_read_occupancy(isl_engine* e, uint8_t* out) {
     if (!e || !out) return ISL_EINVAL;
-    if (!e->have_inventory || e->open.active) return ISL_ESTATE;
-    std::lock_guard<std::mutex> lk(e->mu);
+    std::unique_lock<std::mutex> lk;
+    if (int rc = lock_idle(e, lk)) return rc;
+    if (!e->have_inventory) return ISL_ESTATE;
     DeviceGuard guard(e->device);
     ISL_CUDA(e, cudaMemcpyAsync(out, e->d_occ, e->G, cudaMemcpyDeviceToHost, e->stream));
     ISL_CUDA(e, cudaStreamSynchronize(e->stream));
@@ -1109,10 +1140,11 @@ int isl_read_occupancy(isl_engine* e, uint8_t* out) {
 
 int isl_write_occupancy(isl_engine* e, uint32_t first_gpu, uint32_t n, const uint8_t* occ) {
     if (!e || (n && !occ)) return ISL_EINVAL;
-    if (!e->have_inventory || e->open.active) return ISL_ESTATE;
+    std::unique_lock<std::mutex> lk;
+    if (int rc = lock_idle(e, lk)) return rc;
+    if (!e->have_inventory) return ISL_ESTATE;
     if ((uint64_t)first_gpu + n > e->G) return ISL_ERANGE;
     if (n == 0) return ISL_OK;
-    std::lock_guard<std::mutex> lk(e->mu);
     DeviceGuard guard(e->device);
     std::vector<uint8_t> rev;
     if (e->prof.flip) { rev.assign(occ, occ + n); std::reverse(rev.begin(), rev.end()); occ = rev.data(); first_gpu = e->G - first_gpu - n; }
@@ -1123,8 +1155,9 @@ int isl_write_occupancy(isl_engine* e, uint32_t first_gpu, uint32_t n, const uin
 
 int isl_snapshot_occupancy(isl_engine* e) {
     if (!e) return ISL_EINVAL;
+    std::unique_lock<std::mutex> lk;
+    if (int rc = lock_idle(e, lk)) return rc;
     if (!e->have_inventory) return ISL_ESTATE;
-    std::lock_guard<std::mutex> lk(e->mu);
     DeviceGuard guard(e->device);
     if (int rc = snapshot_occ(e)) return rc;
     e->snap_G = e->G;
@@ -1133,8 +1166,9 @@ int isl_snapshot_occupancy(isl_engine* e) {
 
 int isl_restore_occupancy(isl_engine* e) {
     if (!e) return ISL_EINVAL;
+    std::unique_lock<std::mutex> lk;
+    if (int rc = lock_idle(e, lk)) return rc;
     if (!e->have_inventory || !e->d_occ_snap || e->snap_G != e->G) return ISL_ESTATE;     // a snapshot belongs to the inventory it was taken from
-    std::lock_guard<std::mutex> lk(e->mu);
     DeviceGuard guard(e->device);
     ISL_CUDA(e, cudaMemcpyAsync(e->d_occ, e->d_occ_snap, e->occ_bytes, cudaMemcpyDeviceToDevice, e->stream));
     return ISL_OK;
@@ -1152,19 +1186,21 @@ static int place_batch_locked(isl_engine* e, uint32_t n, const isl_request* in, 
 
 int isl_place_batch(isl_engine* e, uint32_t n, const isl_request* in, isl_result* out) {
     if (!e || (n && (!in || !out))) return ISL_EINVAL;
+    std::unique_lock<std::mutex> lk;
+    if (int rc = lock_idle(e, lk)) return rc;
     if (int rc = validate_ready(e, n)) return rc;
     if (n == 0) return ISL_OK;
-    std::lock_guard<std::mutex> lk(e->mu);
     DeviceGuard guard(e->device);
     return place_batch_locked(e, n, in, out);
 }
 
 int isl_place_batch_range(isl_engine* e, uint32_t lo, uint32_t hi, uint32_t n, const isl_request* in, isl_result* out) {
     if (!e || (n && (!in || !out))) return ISL_EINVAL;
+    std::unique_lock<std::mutex> lk;                // restriction, placement and restore under ONE lock: two callers cannot interleave
+    if (int rc = lock_idle(e, lk)) return rc;
     if (int rc = validate_ready(e, n)) return rc;
     if (lo > hi || hi > e->G) return ISL_EINVAL;
     if (n == 0) return ISL_OK;
-    std::lock_guard<std::mutex> lk(e->mu);          // restriction, placement and restore under ONE lock: two callers cannot interleave
     DeviceGuard guard(e->device);
     const uint32_t lo0 = e->lo, hi0 = e->hi;
     if (e->prof.flip) { e->lo = e->G - hi; e->hi = e->G - lo; } else { e->lo = lo; e->hi = hi; }
@@ -1181,9 +1217,10 @@ int isl_place_gangs(isl_engine* e, uint32_t n_gangs, const uint32_t* gang_off, c
     if (n && (!in || !out)) return ISL_EINVAL;
     if (e->cfg.flags & ISL_FLAG_ALL_NODES) return ISL_EINVAL;      // one pod on every node with capacity: no all-or-nothing meaning
     if (n > e->cfg.max_batch) return ISL_ERANGE;
+    std::unique_lock<std::mutex> lk;
+    if (int rc = lock_idle(e, lk)) return rc;
     if (int rc = validate_ready(e, n)) return rc;
     if (n == 0) return ISL_OK;
-    std::lock_guard<std::mutex> lk(e->mu);
     DeviceGuard guard(e->device);
     if (e->hi == e->lo || e->hi - e->lo > kBfMaxGpus) return ISL_ERANGE;          // the class bitmaps of k_bestfit
     if (int rc = ensure_scratch(e, ((size_t)n_gangs + 1) * sizeof(uint32_t))) return rc;
@@ -1255,8 +1292,10 @@ static int place_batch_plain(isl_engine* e, uint32_t n, const isl_request* in, i
 int isl_place_stream(isl_engine* e, uint32_t n_batches, const uint32_t* sizes, const isl_request* in, isl_result* out) {
     uint64_t total;
     if (int rc = stream_entry(e, n_batches, sizes, in && out, &total)) return rc;
+    std::unique_lock<std::mutex> lk;
+    if (int rc = lock_idle(e, lk)) return rc;
+    if (int rc = validate_ready(e, (uint32_t)total)) return rc;
     if (total == 0) return ISL_OK;
-    std::lock_guard<std::mutex> lk(e->mu);
     DeviceGuard guard(e->device);
     if (int rc = run_stream(e, n_batches, sizes, e->d_req, e->d_res, nullptr, nullptr, 0, reinterpret_cast<const uint2*>(in), reinterpret_cast<uint2*>(out))) {
         if (e->feed_stream) cudaStreamSynchronize(e->feed_stream);
@@ -1271,14 +1310,17 @@ int isl_place_stream_device(isl_engine* e, uint32_t n_batches, const uint32_t* s
     if (!d_in || !d_out) return ISL_EINVAL;
     uint64_t total;
     if (int rc = stream_entry(e, n_batches, sizes, true, &total)) return rc;
-    std::lock_guard<std::mutex> lk(e->mu);
+    std::unique_lock<std::mutex> lk;
+    if (int rc = lock_idle(e, lk)) return rc;
+    if (int rc = validate_ready(e, (uint32_t)total)) return rc;
     DeviceGuard guard(e->device);
     return run_stream(e, n_batches, sizes, static_cast<const uint2*>(d_in), static_cast<uint2*>(d_out), nullptr, nullptr);
 }
 
 int isl_ipc_inbox_handle(isl_engine* e, void* handle64) {
     if (!e || !handle64) return ISL_EINVAL;
-    std::lock_guard<std::mutex> lk(e->mu);
+    std::unique_lock<std::mutex> lk;
+    if (int rc = lock_idle(e, lk)) return rc;
     DeviceGuard guard(e->device);
     if (!e->d_inbox) {
         ISL_CUDA(e, cudaMalloc(&e->d_inbox, (size_t)kMaxStreamChunks * kTokStride * sizeof(uint32_t)));
@@ -1289,7 +1331,8 @@ int isl_ipc_inbox_handle(isl_engine* e, void* handle64) {
 
 int isl_ipc_connect(isl_engine* e, const void* next_handle64, int has_prev) {
     if (!e) return ISL_EINVAL;
-    std::lock_guard<std::mutex> lk(e->mu);
+    std::unique_lock<std::mutex> lk;
+    if (int rc = lock_idle(e, lk)) return rc;
     DeviceGuard guard(e->device);
     if (e->d_outbox && !e->outbox_local) cudaIpcCloseMemHandle(e->d_outbox);
     e->d_outbox = nullptr; e->outbox_local = false;
@@ -1301,7 +1344,8 @@ int isl_ipc_connect(isl_engine* e, const void* next_handle64, int has_prev) {
 
 int isl_connect_local(isl_engine* e, isl_engine* next, int has_prev) {
     if (!e) return ISL_EINVAL;
-    std::lock_guard<std::mutex> lk(e->mu);
+    std::unique_lock<std::mutex> lk;
+    if (int rc = lock_idle(e, lk)) return rc;
     if (e->d_outbox && !e->outbox_local) cudaIpcCloseMemHandle(e->d_outbox);
     e->d_outbox = nullptr; e->outbox_local = true;
     if (next) {
@@ -1316,7 +1360,8 @@ int isl_connect_local(isl_engine* e, isl_engine* next, int has_prev) {
 // ---- speculative rounds over a partitioned inventory: every rank's record memory mapped into every other rank ------------------------
 int isl_ipc_spec_handle(isl_engine* e, void* handle64) {
     if (!e || !handle64) return ISL_EINVAL;
-    std::lock_guard<std::mutex> lk(e->mu);
+    std::unique_lock<std::mutex> lk;
+    if (int rc = lock_idle(e, lk)) return rc;
     DeviceGuard guard(e->device);
     if (int rc = spec_shared_alloc(e)) return rc;
     return ipc_export(e, e->d_spec, handle64);
@@ -1326,7 +1371,8 @@ int isl_ipc_spec_handle(isl_engine* e, void* handle64) {
 // [bounds[r], bounds[r + 1]).  world = 0 disconnects.
 int isl_ipc_connect_spec(isl_engine* e, uint32_t world, uint32_t rank, const void* handles, const uint32_t* bounds) {
     if (!e) return ISL_EINVAL;
-    std::lock_guard<std::mutex> lk(e->mu);
+    std::unique_lock<std::mutex> lk;
+    if (int rc = lock_idle(e, lk)) return rc;
     DeviceGuard guard(e->device);
     spec_disconnect(e);
     if (world == 0) return ISL_OK;
@@ -1345,7 +1391,8 @@ int isl_ipc_connect_spec(isl_engine* e, uint32_t world, uint32_t rank, const voi
 // same-process engines (tests: several ranks on one GPU)
 int isl_connect_spec_local(isl_engine* e, uint32_t world, uint32_t rank, isl_engine* const* engines, const uint32_t* bounds) {
     if (!e) return ISL_EINVAL;
-    std::lock_guard<std::mutex> lk(e->mu);
+    std::unique_lock<std::mutex> lk;
+    if (int rc = lock_idle(e, lk)) return rc;
     DeviceGuard guard(e->device);
     spec_disconnect(e);
     if (world == 0) return ISL_OK;
@@ -1365,23 +1412,27 @@ int isl_place_stream_partitioned(isl_engine* e, uint32_t n_batches, const uint32
     if (!d_in || !d_out || stream_id == 0) return ISL_EINVAL;
     uint64_t total;
     if (int rc = stream_entry(e, n_batches, sizes, true, &total)) return rc;
-    std::lock_guard<std::mutex> lk(e->mu);
+    std::unique_lock<std::mutex> lk;
+    if (int rc = lock_idle(e, lk)) return rc;
+    if (int rc = validate_ready(e, (uint32_t)total)) return rc;
     DeviceGuard guard(e->device);
     return run_stream(e, n_batches, sizes, static_cast<const uint2*>(d_in), static_cast<uint2*>(d_out), nullptr, nullptr, stream_id);
 }
 
 int isl_place_batch_device(isl_engine* e, uint32_t n, const void* d_in, void* d_out) {
     if (!e || (n && (!d_in || !d_out))) return ISL_EINVAL;
+    std::unique_lock<std::mutex> lk;
+    if (int rc = lock_idle(e, lk)) return rc;
     if (int rc = validate_ready(e, n)) return rc;
-    std::lock_guard<std::mutex> lk(e->mu);
     DeviceGuard guard(e->device);
     return run_stream(e, 1, &n, static_cast<const uint2*>(d_in), static_cast<uint2*>(d_out), nullptr, nullptr);
 }
 
 int isl_place_batch_partitioned(isl_engine* e, uint32_t n, const void* d_in, void* d_out, const void* d_heads_in, void* d_heads_out) {
     if (!e || (n && (!d_in || !d_out)) || !d_heads_out) return ISL_EINVAL;
+    std::unique_lock<std::mutex> lk;
+    if (int rc = lock_idle(e, lk)) return rc;
     if (int rc = validate_ready(e, n)) return rc;
-    std::lock_guard<std::mutex> lk(e->mu);
     DeviceGuard guard(e->device);
     return run_stream(e, 1, &n, static_cast<const uint2*>(d_in), static_cast<uint2*>(d_out), static_cast<const uint32_t*>(d_heads_in),
                       static_cast<uint32_t*>(d_heads_out));
@@ -1389,9 +1440,10 @@ int isl_place_batch_partitioned(isl_engine* e, uint32_t n, const void* d_in, voi
 
 int isl_set_partition(isl_engine* e, uint32_t lo, uint32_t hi) {
     if (!e) return ISL_EINVAL;
+    std::unique_lock<std::mutex> lk;
+    if (int rc = lock_idle(e, lk)) return rc;
     if (!e->have_inventory) return ISL_ESTATE;
     if (lo > hi || hi > e->G) return ISL_EINVAL;
-    std::lock_guard<std::mutex> lk(e->mu);
     if (e->prof.flip) { e->lo = e->G - hi; e->hi = e->G - lo; } else { e->lo = lo; e->hi = hi; }
     return ISL_OK;
 }
@@ -1400,9 +1452,10 @@ void* isl_device_occupancy(isl_engine* e) { return e ? e->d_occ : nullptr; }
 
 int isl_free_batch(isl_engine* e, uint32_t n, const isl_span* spans) {
     if (!e || (n && !spans)) return ISL_EINVAL;
-    if (!e->have_inventory || e->open.active) return ISL_ESTATE;
+    std::unique_lock<std::mutex> lk;
+    if (int rc = lock_idle(e, lk)) return rc;
+    if (!e->have_inventory) return ISL_ESTATE;
     if (n == 0) return ISL_OK;
-    std::lock_guard<std::mutex> lk(e->mu);
     DeviceGuard guard(e->device);
     if (int rc = ensure_scratch(e, (size_t)n * sizeof(isl_span))) return rc;
     ISL_CUDA(e, cudaMemcpyAsync(e->d_scratch, spans, (size_t)n * sizeof(isl_span), cudaMemcpyHostToDevice, e->stream));
@@ -1415,12 +1468,13 @@ int isl_free_batch(isl_engine* e, uint32_t n, const isl_span* spans) {
 
 int isl_eval_starts(isl_engine* e, uint32_t profile, uint32_t n, const uint8_t* occ, uint8_t* out) {
     if (!e || (n && (!occ || !out))) return ISL_EINVAL;
+    std::unique_lock<std::mutex> lk;
+    if (int rc = lock_idle(e, lk)) return rc;
     if (!e->have_profiles) return ISL_ESTATE;
     const uint32_t table = profile >> 8;
     profile &= 0xFFu;
     if (profile >= e->prof.n || table >= e->n_tables) return ISL_EINVAL;
     if (n == 0) return ISL_OK;
-    std::lock_guard<std::mutex> lk(e->mu);
     DeviceGuard guard(e->device);
     if (int rc = ensure_scratch(e, (size_t)n * 2)) return rc;
     ISL_CUDA(e, cudaMemcpyAsync(e->d_scratch, occ, n, cudaMemcpyHostToDevice, e->stream));
@@ -1433,7 +1487,8 @@ int isl_eval_starts(isl_engine* e, uint32_t profile, uint32_t n, const uint8_t* 
 
 int isl_read_trace(isl_engine* e, uint64_t* out, uint32_t max_words, uint32_t* n_chunks, uint32_t* n_seg) {
     if (!e || !n_chunks || !n_seg) return ISL_EINVAL;
-    std::lock_guard<std::mutex> lk(e->mu);
+    std::unique_lock<std::mutex> lk;
+    if (int rc = lock_idle(e, lk)) return rc;
     DeviceGuard guard(e->device);
     *n_chunks = e->trace_chunks; *n_seg = e->trace_seg;
     const size_t words = (size_t)e->trace_chunks * e->trace_seg * kTraceWords;
@@ -1446,7 +1501,8 @@ int isl_read_trace(isl_engine* e, uint64_t* out, uint32_t max_words, uint32_t* n
 
 int isl_get_stats(isl_engine* e, isl_stats* out) {
     if (!e || !out) return ISL_EINVAL;
-    std::lock_guard<std::mutex> lk(e->mu);
+    std::unique_lock<std::mutex> lk;
+    if (int rc = lock_idle(e, lk)) return rc;
     DeviceGuard guard(e->device);
     Ctrl c;
     ISL_CUDA(e, cudaMemcpyAsync(&c, e->d_ctrl, sizeof(Ctrl), cudaMemcpyDeviceToHost, e->stream));
@@ -1459,7 +1515,8 @@ int isl_get_stats(isl_engine* e, isl_stats* out) {
 
 int isl_reset_stats(isl_engine* e) {
     if (!e) return ISL_EINVAL;
-    std::lock_guard<std::mutex> lk(e->mu);
+    std::unique_lock<std::mutex> lk;
+    if (int rc = lock_idle(e, lk)) return rc;
     DeviceGuard guard(e->device);
     const uint64_t launches = e->st.kernel_launches;
     e->st = isl_stats{};
@@ -1485,16 +1542,18 @@ static int capacity_locked(isl_engine* e, uint64_t* cap) {
 
 int isl_capacity(isl_engine* e, uint64_t* cap) {
     if (!e || !cap) return ISL_EINVAL;
+    std::unique_lock<std::mutex> lk;
+    if (int rc = lock_idle(e, lk)) return rc;
     if (int rc = validate_ready(e, 0)) return rc;
-    std::lock_guard<std::mutex> lk(e->mu);
     DeviceGuard guard(e->device);
     return capacity_locked(e, cap);
 }
 
 int isl_what_if(isl_engine* e, uint32_t n, const isl_request* plan, isl_result* out, uint64_t* cap_before, uint64_t* cap_after) {
     if (!e || (n && (!plan || !out))) return ISL_EINVAL;
+    std::unique_lock<std::mutex> lk;                // snapshot, plan, measurement and restore under ONE lock: nobody sees the hypothetical state
+    if (int rc = lock_idle(e, lk)) return rc;
     if (int rc = validate_ready(e, n)) return rc;
-    std::lock_guard<std::mutex> lk(e->mu);          // snapshot, plan, measurement and restore under ONE lock: nobody sees the hypothetical state
     DeviceGuard guard(e->device);
     if (int rc = snapshot_occ(e)) return rc;
     int rc = ISL_OK;
@@ -1512,8 +1571,8 @@ int isl_what_if(isl_engine* e, uint32_t n, const isl_request* plan, isl_result* 
 // ---- causal window / pinned buffers / owner-gathered results --------------------------------------------------------------
 int isl_set_causal_window(isl_engine* e, uint32_t window) {
     if (!e) return ISL_EINVAL;
-    if (e->open.active) return ISL_ESTATE;
-    std::lock_guard<std::mutex> lk(e->mu);
+    std::unique_lock<std::mutex> lk;
+    if (int rc = lock_idle(e, lk)) return rc;
     e->window = window;
     return ISL_OK;
 }
@@ -1521,7 +1580,8 @@ int isl_set_causal_window(isl_engine* e, uint32_t window) {
 // debugging aid (not part of the boundary): the per-round stamps recorded under ISL_SPEC_DBG=chunk,stage; out: kSpecRounds x 8 uint64
 int isl_debug_spec_rounds(isl_engine* e, uint64_t* out, uint32_t max_words) {
     if (!e || !out || !e->d_specdbg) return ISL_EINVAL;
-    std::lock_guard<std::mutex> lk(e->mu);
+    std::unique_lock<std::mutex> lk;
+    if (int rc = lock_idle(e, lk)) return rc;
     DeviceGuard guard(e->device);
     ISL_CUDA(e, cudaStreamSynchronize(e->stream));
     ISL_CUDA(e, cudaMemcpy(out, e->d_specdbg, std::min<size_t>(max_words, kSpecRounds * 8) * sizeof(uint64_t), cudaMemcpyDeviceToHost));
@@ -1530,15 +1590,16 @@ int isl_debug_spec_rounds(isl_engine* e, uint64_t* out, uint32_t max_words) {
 
 int isl_set_speculation(isl_engine* e, uint32_t mode) {
     if (!e || mode > ISL_SPEC_ON) return ISL_EINVAL;
-    if (e->open.active) return ISL_ESTATE;
-    std::lock_guard<std::mutex> lk(e->mu);
+    std::unique_lock<std::mutex> lk;
+    if (int rc = lock_idle(e, lk)) return rc;
     e->spec_mode = mode;
     return ISL_OK;
 }
 
 int isl_set_ring_world(isl_engine* e, uint32_t world) {
     if (!e) return ISL_EINVAL;
-    std::lock_guard<std::mutex> lk(e->mu);
+    std::unique_lock<std::mutex> lk;
+    if (int rc = lock_idle(e, lk)) return rc;
     e->ring_world = world;
     return ISL_OK;
 }
@@ -1555,14 +1616,16 @@ void* isl_device_results(isl_engine* e) { return e ? e->d_res : nullptr; }
 
 int isl_ipc_results_handle(isl_engine* e, void* handle64) {
     if (!e || !handle64) return ISL_EINVAL;
-    std::lock_guard<std::mutex> lk(e->mu);
+    std::unique_lock<std::mutex> lk;
+    if (int rc = lock_idle(e, lk)) return rc;
     DeviceGuard guard(e->device);
     return ipc_export(e, e->d_res, handle64);
 }
 
 int isl_ipc_connect_owner(isl_engine* e, const void* owner_handle64) {
     if (!e) return ISL_EINVAL;
-    std::lock_guard<std::mutex> lk(e->mu);
+    std::unique_lock<std::mutex> lk;
+    if (int rc = lock_idle(e, lk)) return rc;
     DeviceGuard guard(e->device);
     if (e->d_owner_out && !e->owner_local) cudaIpcCloseMemHandle(e->d_owner_out);
     e->d_owner_out = nullptr; e->owner_local = false;
@@ -1572,7 +1635,8 @@ int isl_ipc_connect_owner(isl_engine* e, const void* owner_handle64) {
 
 int isl_connect_owner_local(isl_engine* e, isl_engine* owner) {
     if (!e) return ISL_EINVAL;
-    std::lock_guard<std::mutex> lk(e->mu);
+    std::unique_lock<std::mutex> lk;
+    if (int rc = lock_idle(e, lk)) return rc;
     if (e->d_owner_out && !e->owner_local) cudaIpcCloseMemHandle(e->d_owner_out);
     e->d_owner_out = owner ? owner->d_res : nullptr; e->owner_local = true;
     return ISL_OK;
@@ -1584,7 +1648,9 @@ int isl_connect_owner_local(isl_engine* e, isl_engine* owner) {
 // isl_stream_wait returns as soon as that word is up — the caller composes batch b+1 (or b+k) from results it has already seen.
 int isl_stream_open(isl_engine* e, uint32_t max_batches) {
     if (!e || max_batches == 0 || max_batches > kMaxStreamChunks) return ISL_EINVAL;
-    if (!e->have_profiles || !e->have_inventory || e->open.active) return ISL_ESTATE;
+    std::unique_lock<std::mutex> lk;
+    if (int rc = lock_idle(e, lk)) return rc;
+    if (int rc = validate_ready(e, 0)) return rc;
     if (bestfit_family(e->cfg.policy)) return ISL_EINVAL;
     // a tool that serialises kernels would starve a resident kernel that waits for kernels launched after it: refuse instead of hanging
     // until the device-side trap (callers fall back to isl_place_batch per batch)
@@ -1592,7 +1658,6 @@ int isl_stream_open(isl_engine* e, uint32_t max_batches) {
         snprintf(e->cuda_err, sizeof(e->cuda_err), "isl_stream_open: kernel-serialising tool or ISL_NO_FEED set; open streams need concurrent kernels");
         return ISL_ESTATE;
     }
-    std::lock_guard<std::mutex> lk(e->mu);
     DeviceGuard guard(e->device);
     auto& o = e->open;
     const uint32_t pc = e->pipe_chunk;
@@ -1638,8 +1703,8 @@ int isl_stream_open(isl_engine* e, uint32_t max_batches) {
 
 int isl_stream_submit(isl_engine* e, uint32_t n, const isl_request* in, isl_result* out, uint32_t* ticket) {
     if (!e || n == 0 || !in || !out) return ISL_EINVAL;
-    if (!e->open.active) return ISL_ESTATE;
     std::lock_guard<std::mutex> lk(e->mu);
+    if (!e->open.active) return ISL_ESTATE;
     DeviceGuard guard(e->device);
     auto& o = e->open;
     if (o.submitted >= o.max_batches || n > e->pipe_chunk) return ISL_ERANGE;
@@ -1703,8 +1768,8 @@ int isl_stream_wait(isl_engine* e, uint32_t ticket) {
 
 int isl_stream_close(isl_engine* e) {
     if (!e) return ISL_EINVAL;
-    if (!e->open.active) return ISL_ESTATE;
     std::lock_guard<std::mutex> lk(e->mu);
+    if (!e->open.active) return ISL_ESTATE;
     DeviceGuard guard(e->device);
     auto& o = e->open;
     int rc = ISL_OK;

@@ -14,8 +14,12 @@
 ``place_range`` is one call; with ``all_nodes=True`` it is ISL_FLAG_ALL_NODES: one restricted call per node of the clipped range in policy
 order (right-to-left: last node first), each seeing the whole request array; a pod's record is that of the first pass that placed it, the
 FREE records those of the first pass.
+
+``capacity_by_hand`` is isl_capacity over a slice of the occupancy, repeating the start search byte by byte.
 """
 from __future__ import annotations
+
+import functools
 
 import numpy as np
 
@@ -131,6 +135,36 @@ def node_order(node_off, lo, hi, policy):
     spans = [(max(lo, int(a)), min(hi, int(b))) for a, b in zip(node_off[:-1], node_off[1:])]
     spans = [(a, b) for a, b in spans if a < b]
     return spans[::-1] if policy == E.POLICY_RIGHT_TO_LEFT else spans
+
+
+@functools.lru_cache(maxsize=None)
+def _in_a_row(row_bytes, quirks):
+    """[256]: for every occupancy byte, how many placements of the row the start search grants in a row."""
+    row = np.frombuffer(row_bytes, dtype=E.PROFILE_DTYPE)[0]
+    out = np.zeros(256, dtype=np.uint64)
+    for o in range(256):
+        b, k = o, 0
+        while (s := oracle.start_for(row, quirks, b)) != E.START_NONE:
+            b |= ((1 << int(row["size"])) - 1) << s
+            k += 1
+        out[o] = k
+    return out
+
+
+def capacity_by_hand(rows, quirks, occ, gpu_table=None):
+    """cap[p] (MAX_PROFILES entries) over the occupancy bytes ``occ``: the placements of p alone that the start search grants in a row,
+    summed over the GPUs.  ``rows``: [n_profiles], or [n_tables][n_profiles] with ``gpu_table`` the table of every GPU of ``occ``."""
+    rows = np.asarray(rows, dtype=E.PROFILE_DTYPE)
+    occ = np.asarray(occ, dtype=np.uint8)
+    if rows.ndim == 1:
+        rows, gpu_table = rows[None], np.zeros(len(occ), dtype=np.uint8)
+    gpu_table = np.asarray(gpu_table, dtype=np.uint8)
+    cap = np.zeros(E.MAX_PROFILES, dtype=np.uint64)
+    for t in range(rows.shape[0]):
+        counts = np.bincount(occ[gpu_table == t], minlength=256).astype(np.uint64)
+        for p in range(rows.shape[1]):
+            cap[p] += np.dot(_in_a_row(rows[t, p].tobytes(), quirks), counts)
+    return cap
 
 
 def place_range(node_off, rows, occ, lo, hi, requests, quirks=E.QUIRKS_REF_EXACT, policy=E.POLICY_FIRST_FIT, node_table=None,

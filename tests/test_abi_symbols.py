@@ -18,6 +18,28 @@ def test_header_and_binding_agree():
     assert declared_symbols() == sorted(E.EXPORTED_SYMBOLS)
 
 
+def test_every_symbol_has_a_contract_row():
+    """Every entry point is classified in tests/engine_contract.py: its code in every engine state, and whether an open stream allows it.
+    A symbol added to the ABI fails here until it has a row."""
+    import engine_contract as K
+    assert sorted(K.CODES) == sorted(E.SIGNATURES)
+    assert K.LEGAL_DURING_OPEN <= set(E.SIGNATURES) and K.NO_ENGINE <= set(E.SIGNATURES)
+    contexts = [K.Ctx(policy, flags, empty, snap) for policy in range(4) for flags in (0, E.FLAG_ALL_NODES)
+                for empty in (False, True) for snap in (False, True)]
+    for name, row in K.CODES.items():
+        assert set(row) == set(K.ALL_STATES), name
+        for ctx in contexts:
+            for state in K.ALL_STATES:
+                code = K.expected(name, state, ctx)
+                assert code in (K.VALUE, E.OK, E.EINVAL, E.ESTATE, E.ERANGE), (name, state, code)
+            if name in K.LEGAL_DURING_OPEN or name in K.NO_ENGINE:
+                continue
+            # refused in every sub-state of an open stream; only a config the call never accepts reports EINVAL first
+            never = {K.expected(name, s, ctx) for s in K.STATES} == {E.EINVAL}
+            for state in K.OPEN_STATES:
+                assert K.expected(name, state, ctx) == (E.EINVAL if never else E.ESTATE), (name, state, ctx)
+
+
 def test_library_exports_every_declared_symbol():
     lib = ctypes.CDLL(E.LIB_PATH)
     for name in declared_symbols():

@@ -8,6 +8,8 @@ import oracle
 from instaslice_b200 import engine as E
 from instaslice_b200 import tables, workloads as W
 
+from range_oracle import capacity_by_hand
+
 pytestmark = pytest.mark.gpu
 
 
@@ -110,24 +112,6 @@ def test_min_frag_policy_vs_oracle(G, table):
     eng.close()
 
 
-def _capacity_by_hand(rows, quirks, occ):
-    """How many pods of each profile alone a GPU with occupancy byte o takes in a row: repeat the reference's search (:343-383)."""
-    cap = np.zeros(E.MAX_PROFILES, dtype=np.uint64)
-    per_byte = np.zeros((len(rows), 256), dtype=np.uint64)
-    for p in range(len(rows)):
-        for o in range(256):
-            cur, c = o, 0
-            while True:
-                s = oracle.start_for(rows[p], quirks, cur)
-                if s == E.START_NONE:
-                    break
-                cur |= (((1 << int(rows[p]["size"])) - 1) << s) & 0xFF
-                c += 1
-            per_byte[p, o] = c
-        cap[p] = per_byte[p][occ].sum()
-    return cap
-
-
 def test_capacity_and_what_if_query():
     rows = E.make_profiles(tables.H100_80GB)
     rng = W.SplitMix64(99)
@@ -137,7 +121,7 @@ def test_capacity_and_what_if_query():
     eng = E.Engine(max_gpus=G, max_batch=1 << 16)
     eng.load_profiles(rows)
     eng.load_inventory(node_off, occ)
-    assert np.array_equal(eng.capacity(), _capacity_by_hand(rows, 3, occ))
+    assert np.array_equal(eng.capacity(), capacity_by_hand(rows, 3, occ))
     # plan: release 200 busy spans, then ask for 3000 mixed pods
     ref = oracle.Fast(node_off, rows)
     ref.load(occ)
@@ -148,8 +132,8 @@ def test_capacity_and_what_if_query():
     want = ref.place(plan)
     got, before, after = eng.what_if(plan)
     assert np.array_equal(got, want)
-    assert np.array_equal(before, _capacity_by_hand(rows, 3, occ))
-    assert np.array_equal(after, _capacity_by_hand(rows, 3, ref.occupancy()))
+    assert np.array_equal(before, capacity_by_hand(rows, 3, occ))
+    assert np.array_equal(after, capacity_by_hand(rows, 3, ref.occupancy()))
     assert np.array_equal(eng.read_occupancy(), occ)            # the live state is back
     # and the engine goes on from the LIVE state
     req = W.alloc_requests(W.mix_profiles(rng, 500))

@@ -19,7 +19,7 @@ from instaslice_b200 import tables
 from instaslice_b200 import workloads as W
 
 import gang_oracle as GO
-from range_oracle import RangeFast, mixed_requests, place_range
+from range_oracle import RangeFast, capacity_by_hand, mixed_requests, place_range
 
 pytestmark = pytest.mark.gpu
 MIX_NAMES = [tables.A100_40GB, tables.H100_80GB, tables.A30_24GB]
@@ -211,20 +211,6 @@ def test_best_fit_family_on_ranges(policy, n_tables):
 
 
 # ---- (b) isl_set_partition on one engine at unaligned bounds: every entry point ----------------------------------------------------------
-def capacity_by_hand(rows, quirks, occ):
-    """cap[p] over the given occupancy bytes: placements of p alone that the start search grants in a row on every GPU."""
-    cap = np.zeros(E.MAX_PROFILES, dtype=np.uint64)
-    counts = np.bincount(occ, minlength=256)
-    for p, row in enumerate(rows):
-        for o in np.flatnonzero(counts):
-            b, k = int(o), 0
-            while (s := oracle.start_for(row, quirks, b)) != E.START_NONE:
-                b |= ((1 << int(row["size"])) - 1) << s
-                k += 1
-            cap[p] += np.uint64(k * int(counts[o]))
-    return cap
-
-
 PARTITIONS = [(65536, 13, 65536 - 29), (100000, 4097, 70001)]
 
 

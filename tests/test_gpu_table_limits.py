@@ -16,6 +16,7 @@ import pytest
 import oracle
 from instaslice_b200 import engine as E
 from instaslice_b200 import workloads as W
+from range_oracle import capacity_by_hand
 from test_oracle_table_limits import (EDGE_N, candidates, churn_batches, default_sizes, edge65535, plus_one_candidate, ragged_nodes,
                                       t16mix, t16top, t16x8, t8tab, t8tab_node_tables)
 
@@ -327,26 +328,6 @@ def test_policies(policy, name, quirks):
 
 
 # ---- queries ------------------------------------------------------------------------------------------------------------------------
-def capacity_by_hand(rows2d, gpu_table, quirks, occ):
-    """Per profile: how many pods of it alone the GPUs take, each GPU under its node's table — repeating the search byte by byte."""
-    cap = np.zeros(E.MAX_PROFILES, dtype=np.uint64)
-    for t in range(rows2d.shape[0]):
-        on_t = occ[gpu_table == t]
-        for p in range(rows2d.shape[1]):
-            per_byte = np.zeros(256, dtype=np.uint64)
-            for o in range(256):
-                cur, c = o, 0
-                while True:
-                    s = oracle.start_for(rows2d[t, p], quirks, cur)
-                    if s == E.START_NONE:
-                        break
-                    cur |= (((1 << int(rows2d[t, p]["size"])) - 1) << s) & 0xFF
-                    c += 1
-                per_byte[o] = c
-            cap[p] += per_byte[on_t].sum()
-    return cap
-
-
 def test_capacity_and_what_if_t8tab():
     rows = t8tab()
     rng = W.SplitMix64(31337)
@@ -357,7 +338,7 @@ def test_capacity_and_what_if_t8tab():
     gpu_table = np.repeat(node_table, np.diff(node_off))
     occ = ((rng.next(G) & rng.next(G)) & np.uint64(0xFF)).astype(np.uint8)
     eng = make_engine(rows, node_off, occ, E.QUIRKS_FIXED, node_table)
-    assert np.array_equal(eng.capacity(), capacity_by_hand(rows, gpu_table, E.QUIRKS_FIXED, occ))
+    assert np.array_equal(eng.capacity(), capacity_by_hand(rows, E.QUIRKS_FIXED, occ, gpu_table))
     ref = make_oracle(rows, node_off, occ, E.QUIRKS_FIXED, node_table)
     plan = W.alloc_requests((rng.next(3000) % np.uint64(16)).astype(np.uint8))
     for i, g in enumerate(np.flatnonzero(occ & 1)[:200]):        # release 200 busy slices first
@@ -365,8 +346,8 @@ def test_capacity_and_what_if_t8tab():
     want = ref.place(plan)
     got, before, after = eng.what_if(plan)
     assert np.array_equal(got, want)
-    assert np.array_equal(before, capacity_by_hand(rows, gpu_table, E.QUIRKS_FIXED, occ))
-    assert np.array_equal(after, capacity_by_hand(rows, gpu_table, E.QUIRKS_FIXED, ref.occupancy()))
+    assert np.array_equal(before, capacity_by_hand(rows, E.QUIRKS_FIXED, occ, gpu_table))
+    assert np.array_equal(after, capacity_by_hand(rows, E.QUIRKS_FIXED, ref.occupancy(), gpu_table))
     assert np.array_equal(eng.read_occupancy(), occ)            # the live state is back
     # an unplaced request reports the size of the first node (canonical order) whose table knows the name: table 7 for profile 15
     full = np.full(G, 0xFF, dtype=np.uint8)
