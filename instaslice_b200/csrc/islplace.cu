@@ -12,6 +12,7 @@
 #include <mutex>
 #include <new>
 #include <type_traits>
+#include <utility>
 #include <vector>
 
 #include "isl_kernels.cuh"
@@ -26,11 +27,90 @@ struct PipePlan {
     bool spec = false;
 };
 
+// Owners of the engine's CUDA resources.  Each is move-only and releases its resource in its destructor, so deleting an isl_engine
+// (with its device current) frees everything it holds.  They convert to the raw pointer or handle for kernel arguments and CUDA calls.
+enum class Growth { exact, headroom };       // headroom: need + need / 4 + 1 units, so that a growing stream reallocates rarely
+
+// Device memory of cap() units of `unit` elements each.
+template <typename T>
+class DevMem {
+    T* p_ = nullptr; size_t cap_ = 0, unit_;
+  public:
+    explicit DevMem(size_t unit = 1) : unit_(unit) {}
+    DevMem(DevMem&& o) noexcept : p_(std::exchange(o.p_, nullptr)), cap_(std::exchange(o.cap_, 0)), unit_(o.unit_) {}
+    ~DevMem() { release(); }
+    operator T*() const { return p_; }
+    T* get() const { return p_; }
+    size_t cap() const { return cap_; }
+    size_t bytes() const { return cap_ * unit_ * sizeof(T); }
+    void release() { if (p_) cudaFree(p_); p_ = nullptr; cap_ = 0; }
+    // Room for `need` units.  A buffer that is too small is freed and allocated anew (*fresh: it was, its contents are undefined); a
+    // failed allocation leaves it empty.
+    cudaError_t reserve(size_t need, Growth g = Growth::exact, bool* fresh = nullptr) {
+        if (fresh) *fresh = false;
+        if (need <= cap_) return cudaSuccess;
+        release();
+        const size_t units = g == Growth::headroom ? need + need / 4 + 1 : need;
+        if (cudaError_t err = cudaMalloc(&p_, units * unit_ * sizeof(T))) { p_ = nullptr; return err; }
+        cap_ = units;
+        if (fresh) *fresh = true;
+        return cudaSuccess;
+    }
+    cudaError_t replace(size_t n) { release(); return reserve(n); }      // exactly n units, whatever the buffer held
+};
+
+// Pinned host memory of cap() elements; a mapped buffer (cudaHostAllocMapped) also holds its device alias dev().
+template <typename T>
+class HostMem {
+    T *p_ = nullptr, *dev_ = nullptr;
+    size_t cap_ = 0; unsigned flags_;
+  public:
+    explicit HostMem(unsigned flags) : flags_(flags) {}
+    HostMem(HostMem&& o) noexcept : p_(std::exchange(o.p_, nullptr)), dev_(std::exchange(o.dev_, nullptr)), cap_(std::exchange(o.cap_, 0)), flags_(o.flags_) {}
+    ~HostMem() { release(); }
+    operator T*() const { return p_; }
+    T* dev() const { return dev_; }
+    void release() { if (p_) cudaFreeHost(p_); p_ = dev_ = nullptr; cap_ = 0; }
+    // Room for n elements, exactly.  A buffer that is too small is freed first; a failed allocation leaves it empty.
+    cudaError_t reserve(size_t n) {
+        if (n <= cap_) return cudaSuccess;
+        release();
+        cudaError_t err = cudaHostAlloc(&p_, n * sizeof(T), flags_);
+        if (err != cudaSuccess) { p_ = nullptr; return err; }
+        if (flags_ & cudaHostAllocMapped) err = cudaHostGetDevicePointer(&dev_, p_, 0);
+        if (err == cudaSuccess) cap_ = n; else release();
+        return err;
+    }
+};
+
+// A stream, event or peer mapping, released (Release) only if this holder owns it: out() is where a create or open call writes a
+// handle the holder then owns; borrow() keeps one that belongs to someone else (a caller's stream, a same-process engine's memory,
+// the engine's own record memory).
+template <typename H, auto Release>
+class Handle {
+    H h_ = nullptr; bool own_ = false;
+  public:
+    Handle() = default;
+    Handle(Handle&& o) noexcept : h_(std::exchange(o.h_, nullptr)), own_(std::exchange(o.own_, false)) {}
+    ~Handle() { reset(); }
+    operator H() const { return h_; }
+    H get() const { return h_; }
+    void reset() { if (own_ && h_) Release(h_); h_ = nullptr; own_ = false; }
+    void borrow(H h) { reset(); h_ = h; }
+    H* out() { reset(); own_ = true; return &h_; }
+};
+using Stream = Handle<cudaStream_t, cudaStreamDestroy>;
+using Event = Handle<cudaEvent_t, cudaEventDestroy>;
+template <typename T> using PeerMap = Handle<T*, cudaIpcCloseMemHandle>;      // opened through CUDA IPC, or borrowed
+
 struct isl_engine {
+    // declared first, so destroyed last: the memory below is freed before the streams it was used on go away
+    Stream stream;
+    // host-buffer streams: batches are fed on their own stream while the pipeline runs; results leave chunk by chunk
+    Stream feed_stream; Event ev_feed, ev_feed_done;
+    Event ev[6];                     // ISL_FLAG_TIMING
     isl_config cfg{};
     int device = 0;
-    cudaStream_t stream = nullptr;
-    bool own_stream = false;
     std::mutex mu;
     char cuda_err[256] = {0};
 
@@ -46,73 +126,68 @@ struct isl_engine {
     uint32_t n_tables = 1;
     isl_profile rows_all[ISL_MAX_TABLES][ISL_MAX_PROFILES] = {};
     std::vector<uint8_t> node_table;     // table of every node (empty = all 0)
-    uint8_t* d_gtab = nullptr;           // table of every GPU's node, one byte per GPU
-    uint8_t* d_capn = nullptr;           // [table][profile][occ]: placements of the profile the GPU takes in a row
-    uint32_t* d_seq = nullptr;           // [table][profile][occ]: their starts, 4 bits each
-    uint8_t* d_sizes = nullptr;          // [table][profile]: slices per placement
-    uint8_t* d_score = nullptr;          // [profile][occ] of table 0: what a best-fit family policy minimises (k_bestfit)
-    unsigned long long* d_cap = nullptr; // isl_capacity: per-profile counters
-    uint16_t* d_cand_o16 = nullptr;      // single-chain path: occupancy + table tag of every candidate
+    DevMem<uint8_t> d_gtab;              // table of every GPU's node, one byte per GPU
+    DevMem<uint8_t> d_capn;              // [table][profile][occ]: placements of the profile the GPU takes in a row
+    DevMem<uint32_t> d_seq;              // [table][profile][occ]: their starts, 4 bits each
+    DevMem<uint8_t> d_sizes;             // [table][profile]: slices per placement
+    DevMem<uint8_t> d_score;             // [profile][occ] of table 0: what a best-fit family policy minimises (k_bestfit)
+    DevMem<unsigned long long> d_cap;    // isl_capacity: per-profile counters
+    DevMem<uint16_t> d_cand_o16;         // single-chain path: occupancy + table tag of every candidate
 
     // device buffers
-    uint8_t* d_occ = nullptr;        // one byte per GPU, padded to whole sweep blocks with 0xFF
+    DevMem<uint8_t> d_occ;           // one byte per GPU, padded to whole sweep blocks with 0xFF
     size_t occ_bytes = 0;
-    uint8_t* d_lut = nullptr;        // [16][256]
-    uint16_t* d_feas = nullptr;      // [256]
-    uint2* d_req = nullptr;          // staging for the host-buffer entry point
-    uint2* d_res = nullptr;
-    uint16_t* d_q = nullptr;         // per-chunk queues
-    uint32_t* d_tile_counts = nullptr;
-    uint32_t* d_cand = nullptr;
-    uint2* d_log = nullptr;          // decision log of one chunk (chain -> commit)
-    uint32_t* d_bf_bitmaps = nullptr; size_t bf_words = 0;   // best-fit class bitmaps for inventories beyond the shared-memory size / several tables
-    uint2* h_small_out = nullptr;     // mapped pinned results of tiny batches (k_small writes them over PCIe directly)
-    uint2* d_small_out = nullptr;     // device alias of h_small_out
-    uint32_t* d_sweep_counts = nullptr;
-    Ctrl* d_ctrl = nullptr;
-    uint8_t* d_scratch = nullptr;    // eval_starts / free_batch staging
+    DevMem<uint8_t> d_lut;           // [16][256]
+    DevMem<uint16_t> d_feas;         // [256]
+    DevMem<uint2> d_req;             // staging for the host-buffer entry point
+    DevMem<uint2> d_res;             // results, then kMaxStreamChunks 'ranks done' counters of a partitioned run (peer-mapped with them)
+    DevMem<uint16_t> d_q;            // per-chunk queues
+    DevMem<uint32_t> d_tile_counts;
+    DevMem<uint32_t> d_cand;
+    DevMem<uint2> d_log;             // decision log of one chunk (chain -> commit)
+    DevMem<uint32_t> d_bf_bitmaps;   // best-fit class bitmaps for inventories beyond the shared-memory size / several tables
+    HostMem<uint2> h_small_out{cudaHostAllocMapped};     // results of tiny batches (k_small writes them over PCIe directly)
+    DevMem<uint32_t> d_sweep_counts;
+    DevMem<Ctrl> d_ctrl;
+    DevMem<uint8_t> d_scratch;       // eval_starts / free_batch / gang offsets staging
     // stream / segment-pipeline state (grown on demand)
-    ChunkDesc* d_chunks = nullptr; Ctrl* d_cctl = nullptr; uint16_t* d_qall = nullptr; uint32_t* d_tokens = nullptr;
-    uint32_t* d_free_acc = nullptr; TileDesc* d_tiles = nullptr; std::vector<TileDesc> h_tiles;
-    uint32_t cap_chunks = 0, cap_cctl = 0, cap_qall = 0, cap_tokens = 0, cap_free = 0, cap_tiles = 0;
+    DevMem<ChunkDesc> d_chunks; DevMem<Ctrl> d_cctl; DevMem<uint16_t> d_qall; DevMem<uint32_t> d_tokens{kTokStride};
+    DevMem<uint32_t> d_free_acc; DevMem<TileDesc> d_tiles; std::vector<TileDesc> h_tiles;
     uint32_t pipe_chunk = 0;         // requests per pipeline chunk (multiple of kTile, <= kChunk)
     std::vector<ChunkDesc> h_chunks;
     uint32_t epoch = 0;
-    uint32_t* d_inbox = nullptr;      // [kMaxStreamChunks][kTokStride] tokens written by the previous rank (peer store)
-    uint32_t* d_outbox = nullptr;     // next rank's inbox, opened through CUDA IPC
-    bool has_prev = false, outbox_local = false;
-    unsigned long long* d_trace = nullptr; uint32_t cap_trace = 0, trace_chunks = 0, trace_seg = 0;
+    DevMem<uint32_t> d_inbox{kTokStride};   // [kMaxStreamChunks][kTokStride] tokens written by the previous rank (peer store)
+    PeerMap<uint32_t> d_outbox;      // next rank's inbox
+    bool has_prev = false;
+    DevMem<unsigned long long> d_trace{kTraceWords}; uint32_t trace_chunks = 0, trace_seg = 0;
     int max_coresident = 0;          // CTAs of k_pipeline that can be resident at once (0 = not queried)
-    // host-buffer streams: batches are fed on their own stream while the pipeline runs; results leave chunk by chunk
-    cudaStream_t feed_stream = nullptr; cudaEvent_t ev_feed = nullptr, ev_feed_done = nullptr;
-    uint32_t* d_ready = nullptr; uint32_t cap_ready = 0;      // [batch] epoch flag
-    uint32_t* d_done_cnt = nullptr; uint32_t cap_done = 0;    // [chunk] committed segments
-    uint8_t* d_occ_snap = nullptr; size_t snap_bytes = 0; uint32_t snap_G = 0;      // isl_snapshot_occupancy / isl_restore_occupancy
+    DevMem<uint32_t> d_ready;        // [batch] epoch flag
+    DevMem<uint32_t> d_done_cnt;     // [chunk] committed segments
+    DevMem<uint8_t> d_occ_snap; uint32_t snap_G = 0;      // isl_snapshot_occupancy / isl_restore_occupancy
     bool delivered = false;          // the last run_stream call already put the results into the caller's host buffer
-    size_t scratch_bytes = 0;
     unsigned long long wait_ns = 20000000000ull;   // a starved device-side wait traps after this long (ISL_WAIT_SECONDS overrides the 20 s)
     uint32_t window = 0;             // causal window of stream calls (isl_set_causal_window): chunk c starts after chunk c - window is committed
     uint32_t spec_mode = ISL_SPEC_AUTO;     // speculative rounds (isl_set_speculation); ISL_SPEC=0|1 in the environment overrides
-    unsigned long long* d_specdbg = nullptr;
+    DevMem<unsigned long long> d_specdbg{8};      // [kSpecRounds][8]
+    DevMem<unsigned long long> d_spec{kSpecWordsPerChunk}; uint32_t spec_hi = 0;    // record memory of the rounds, cap() chunks
     // partitioned inventory: every rank's record memory, peer-mapped (own entry = d_spec); bounds of all ranks; the shared memory never moves
-    unsigned long long* spec_peer[8] = {}; bool spec_peer_local = false, spec_shared = false;
+    PeerMap<unsigned long long> spec_peer[8]; bool spec_shared = false;
     uint32_t spec_world = 0, spec_rank = 0, spec_bounds[9] = {};
-    unsigned long long* d_spec = nullptr; uint32_t cap_spec = 0, spec_hi = 0;    // record memory of the rounds: kSpecWordsPerChunk words per chunk
     // open stream (isl_stream_open / _submit / _wait / _close): one persistent k_pipeline, batches arrive while it runs
     struct Open {
         bool active = false, launched = false;
         uint32_t max_batches = 0, submitted = 0, epoch = 0, q_stride = 0, free_stride = 0, tiles_per_batch = 0;
         PipePlan plan;
-        uint32_t* h_done = nullptr; uint32_t* d_done_host = nullptr; uint32_t cap_done = 0;   // mapped pinned: [batch] = epoch once its results are in host memory
-        ChunkDesc* h_chunks = nullptr; TileDesc* h_tiles = nullptr; uint32_t cap_desc = 0;       // pinned staging of the per-batch descriptors
+        HostMem<uint32_t> h_done{cudaHostAllocMapped};        // [batch] = epoch once its results are in host memory
+        HostMem<ChunkDesc> h_chunks{cudaHostAllocDefault};    // staging of the per-batch descriptors
+        HostMem<TileDesc> h_tiles{cudaHostAllocDefault};
     } open;
     // partitioned inventory with the results gathered on the owner rank (rank 0): peer-mapped d_res of the owner
-    uint2* d_owner_out = nullptr; bool owner_local = false;
+    PeerMap<uint2> d_owner_out;
     uint32_t ring_world = 0;         // ranks of the partitioned run (isl_set_ring_world); the causal window of a ring needs it
 
     // stats
     isl_stats st{};
-    cudaEvent_t ev[6] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};
 };
 
 namespace {
@@ -153,15 +228,6 @@ int check_launch(isl_engine* e, const char* what) {
     return ISL_OK;
 }
 
-int ensure_scratch(isl_engine* e, size_t bytes) {
-    if (bytes <= e->scratch_bytes) return ISL_OK;
-    if (e->d_scratch) cudaFree(e->d_scratch);
-    e->d_scratch = nullptr; e->scratch_bytes = 0;
-    ISL_CUDA(e, cudaMalloc(&e->d_scratch, bytes));
-    e->scratch_bytes = bytes;
-    return ISL_OK;
-}
-
 // f(std::integral_constant<int, K>) with K = the candidate slots of the loaded tables (k_small<K>, k_chain<K>, k_pipeline<K, ..>)
 template <typename F>
 auto with_cand_slots(const isl_engine* e, F&& f) {
@@ -192,7 +258,7 @@ int launch_chain(isl_engine* e, uint2* d_out_chunk, const uint32_t* d_heads_in, 
     const size_t smem = (size_t)kQCap * sizeof(uint16_t);      // opted in per device by isl_create
     k_chain<K><<<1, kChainThreads, smem, e->stream>>>(e->tab, e->d_ctrl, e->d_q, e->d_cand_o16, e->d_feas, e->d_log, d_heads_in, d_heads_out);
     if (int rc = check_launch(e, "k_chain")) return rc;
-    k_commit<<<kChunk / 256, 256, 0, e->stream>>>(e->d_ctrl, e->d_log, e->d_cand, reinterpret_cast<uint32_t*>(e->d_occ), d_out_chunk, e->prof.flip);
+    k_commit<<<kChunk / 256, 256, 0, e->stream>>>(e->d_ctrl, e->d_log, e->d_cand, reinterpret_cast<uint32_t*>(e->d_occ.get()), d_out_chunk, e->prof.flip);
     return check_launch(e, "k_commit");
 }
 
@@ -241,17 +307,12 @@ int prepare_bestfit(isl_engine* e, uint32_t n, const uint2* d_in, uint2* d_out, 
     *smem = in_smem ? (size_t)256 * stride * sizeof(uint32_t) : 0;
     if (!in_smem && Gr) {   // class bitmaps in global memory: one set of 256 per table, zeroed here (HBM speed) instead of by the lone CTA
         const size_t words = (size_t)256 * e->n_tables * stride;
-        if (words > e->bf_words) {
-            if (e->d_bf_bitmaps) cudaFree(e->d_bf_bitmaps);
-            e->d_bf_bitmaps = nullptr; e->bf_words = 0;
-            ISL_CUDA(e, cudaMalloc(&e->d_bf_bitmaps, words * sizeof(uint32_t)));
-            e->bf_words = words;
-        }
+        ISL_CUDA(e, e->d_bf_bitmaps.reserve(words));
         ISL_CUDA(e, cudaMemsetAsync(e->d_bf_bitmaps, 0, words * sizeof(uint32_t), e->stream));
     }
     const bool timing = e->cfg.flags & ISL_FLAG_TIMING;
     if (timing) cudaEventRecord(e->ev[0], e->stream);
-    k_prepare<<<ceil_div(n, kTile), kTileThreads, 0, e->stream>>>(n, d_in, d_out, reinterpret_cast<uint32_t*>(e->d_occ), e->G, e->lo, e->hi,
+    k_prepare<<<ceil_div(n, kTile), kTileThreads, 0, e->stream>>>(n, d_in, d_out, reinterpret_cast<uint32_t*>(e->d_occ.get()), e->G, e->lo, e->hi,
                                                                   e->prof, e->d_tile_counts, e->d_ctrl, nullptr, nullptr, 0, 0);
     if (int rc = check_launch(e, "k_prepare")) return rc;
     if (timing) cudaEventRecord(e->ev[1], e->stream);
@@ -292,7 +353,7 @@ int run_batch(isl_engine* e, uint32_t n, const uint2* d_in, uint2* d_out, const 
     const bool timing = e->cfg.flags & ISL_FLAG_TIMING;
     const uint32_t tiles = ceil_div(n, kTile);
     if (timing) cudaEventRecord(e->ev[0], e->stream);
-    k_prepare<<<tiles, kTileThreads, 0, e->stream>>>(n, d_in, d_out, reinterpret_cast<uint32_t*>(e->d_occ), e->G, e->lo, e->hi,
+    k_prepare<<<tiles, kTileThreads, 0, e->stream>>>(n, d_in, d_out, reinterpret_cast<uint32_t*>(e->d_occ.get()), e->G, e->lo, e->hi,
                                                      e->prof, e->d_tile_counts, e->d_ctrl, nullptr, nullptr, 0, 0);
     if (int rc = check_launch(e, "k_prepare")) return rc;
     if (timing) cudaEventRecord(e->ev[1], e->stream);
@@ -315,10 +376,10 @@ int run_batch(isl_engine* e, uint32_t n, const uint2* d_in, uint2* d_out, const 
             else ISL_CUDA(e, cudaMemsetAsync(h_out, 0, ISL_MAX_PROFILES * sizeof(uint32_t), e->stream));
         }
         if (sweep_blocks) {     // candidate compaction — or, for a single-profile chunk, the capacity scan that commits directly
-            k_sweep_count<<<sweep_blocks, kSweepThreads, 0, e->stream>>>(reinterpret_cast<const uint4*>(e->d_occ), reinterpret_cast<const uint4*>(e->d_gtab), e->d_feas, first_block, e->lo, e->hi,
+            k_sweep_count<<<sweep_blocks, kSweepThreads, 0, e->stream>>>(reinterpret_cast<const uint4*>(e->d_occ.get()), reinterpret_cast<const uint4*>(e->d_gtab.get()), e->d_feas, first_block, e->lo, e->hi,
                                                                          e->d_ctrl, e->d_sweep_counts, e->d_capn);
             if (int rc = check_launch(e, "k_sweep_count")) return rc;
-            k_sweep_scatter<<<sweep_blocks, kSweepThreads, 0, e->stream>>>(reinterpret_cast<const uint4*>(e->d_occ), reinterpret_cast<const uint4*>(e->d_gtab), e->d_feas, first_block, e->lo, e->hi,
+            k_sweep_scatter<<<sweep_blocks, kSweepThreads, 0, e->stream>>>(reinterpret_cast<const uint4*>(e->d_occ.get()), reinterpret_cast<const uint4*>(e->d_gtab.get()), e->d_feas, first_block, e->lo, e->hi,
                                                                            e->d_ctrl, e->d_sweep_counts, e->d_cand, e->d_cand_o16, e->d_capn, e->d_seq, e->d_q, e->d_occ,
                                                                            d_out + c0, h_in, h_out, e->d_sizes, e->prof.flip);
             if (int rc = check_launch(e, "k_sweep_scatter")) return rc;
@@ -375,17 +436,6 @@ int query_coresident(isl_engine* e) {
     ISL_CUDA(e, cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, e->device));
     ISL_CUDA(e, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_pipeline<4, true, true>, kPipeThreads, kPipeSmem));
     e->max_coresident = coop ? std::max(1, per_sm * sms) : -1;
-    return ISL_OK;
-}
-
-template <typename T>
-int grow(isl_engine* e, T** buf, uint32_t* cap, size_t need, size_t elems_per_unit) {
-    if (need <= *cap) return ISL_OK;
-    if (*buf) cudaFree(*buf);
-    *buf = nullptr; *cap = 0;
-    const size_t units = need + need / 4 + 1;
-    ISL_CUDA(e, cudaMalloc(buf, units * elems_per_unit * sizeof(T)));
-    *cap = (uint32_t)units;
     return ISL_OK;
 }
 
@@ -450,7 +500,7 @@ int plan_pipeline(isl_engine* e, uint32_t n_chunks, double avg_chunk, bool want_
             // the same predicate over the same bounds, so they agree)
             uint32_t sz = 64;
             while (ceil_div(e->G, sz) > kSpecMaxStages) sz *= 2;
-            bool ok = sz <= kSegMax && e->spec_world == e->ring_world && n_chunks <= e->cap_spec && e->spec_bounds[e->spec_world] == e->G &&
+            bool ok = sz <= kSegMax && e->spec_world == e->ring_world && n_chunks <= e->d_spec.cap() && e->spec_bounds[e->spec_world] == e->G &&
                       e->spec_bounds[e->spec_rank] == e->lo && e->spec_bounds[e->spec_rank + 1] == e->hi && query_coresident(e) == ISL_OK;
             for (uint32_t r = 0; ok && r <= e->spec_world; ++r) ok = e->spec_bounds[r] % sz == 0 || e->spec_bounds[r] == e->G;
             for (uint32_t r = 0; ok && r < e->spec_world; ++r) ok = e->spec_bounds[r] < e->spec_bounds[r + 1] && ceil_div(e->spec_bounds[r + 1] - e->spec_bounds[r], sz) <= (uint32_t)std::max(1, e->max_coresident);
@@ -470,11 +520,11 @@ constexpr unsigned long long kOpenWaitNs = 600000000000ull;     // open streams 
 
 // record memory for n_chunks chunks; the words carry the call epoch (24 bits) — cleared when (re)allocated and when those bits wrap
 int prepare_spec(isl_engine* e, uint32_t n_chunks, uint32_t epoch, cudaStream_t st) {
-    if (e->spec_shared) return n_chunks <= e->cap_spec ? ISL_OK : ISL_ERANGE;      // peers hold a mapping of it: fixed size, tags carry the stream id
-    const uint32_t before = e->cap_spec;
-    if (int rc = grow(e, &e->d_spec, &e->cap_spec, n_chunks, kSpecWordsPerChunk)) return rc;
-    const bool fresh = e->cap_spec != before, wrapped = (epoch >> 24) != e->spec_hi;
-    if (fresh || wrapped) ISL_CUDA(e, cudaMemsetAsync(e->d_spec, 0, (size_t)e->cap_spec * kSpecWordsPerChunk * sizeof(unsigned long long), st));
+    if (e->spec_shared) return n_chunks <= e->d_spec.cap() ? ISL_OK : ISL_ERANGE;      // peers hold a mapping of it: fixed size, tags carry the stream id
+    bool fresh;
+    ISL_CUDA(e, e->d_spec.reserve(n_chunks, Growth::headroom, &fresh));
+    const bool wrapped = (epoch >> 24) != e->spec_hi;
+    if (fresh || wrapped) ISL_CUDA(e, cudaMemsetAsync(e->d_spec, 0, e->d_spec.bytes(), st));
     e->spec_hi = epoch >> 24;
     return ISL_OK;
 }
@@ -487,9 +537,9 @@ bool kernels_serialised() {
 
 int ensure_feed_stream(isl_engine* e) {
     if (e->feed_stream) return ISL_OK;
-    ISL_CUDA(e, cudaStreamCreateWithFlags(&e->feed_stream, cudaStreamNonBlocking));
-    ISL_CUDA(e, cudaEventCreateWithFlags(&e->ev_feed, cudaEventDisableTiming));
-    ISL_CUDA(e, cudaEventCreateWithFlags(&e->ev_feed_done, cudaEventDisableTiming));
+    ISL_CUDA(e, cudaStreamCreateWithFlags(e->feed_stream.out(), cudaStreamNonBlocking));
+    ISL_CUDA(e, cudaEventCreateWithFlags(e->ev_feed.out(), cudaEventDisableTiming));
+    ISL_CUDA(e, cudaEventCreateWithFlags(e->ev_feed_done.out(), cudaEventDisableTiming));
     return ISL_OK;
 }
 
@@ -498,7 +548,7 @@ int next_epoch(isl_engine* e, uint32_t* epoch) {
     *epoch = ++e->epoch;
     if ((*epoch & 0x7FFFu) == 0) *epoch = ++e->epoch;      // the token words carry the low 15 bits as a tag; tag 0 is what a cleared buffer holds
     if ((*epoch & 0x7FFFu) == 1 && *epoch != 1 && e->d_tokens)    // tag wrap-around: no stale word of 32 768 calls ago may look current
-        ISL_CUDA(e, cudaMemsetAsync(e->d_tokens, 0, (size_t)e->cap_tokens * kTokStride * sizeof(uint32_t), e->stream));
+        ISL_CUDA(e, cudaMemsetAsync(e->d_tokens, 0, e->d_tokens.bytes(), e->stream));
     return ISL_OK;
 }
 
@@ -506,18 +556,17 @@ int next_epoch(isl_engine* e, uint32_t* epoch) {
 // free masks of n_batches batches; n_ready ready flags and n_done done counters (0: none needed).
 int grow_stream_buffers(isl_engine* e, uint32_t n_chunks, uint32_t q_stride, uint32_t n_tiles, uint32_t n_batches, uint32_t n_seg,
                         uint32_t n_ready, uint32_t n_done) {
-    if (int rc = grow(e, &e->d_chunks, &e->cap_chunks, n_chunks, 1)) return rc;
-    if (int rc = grow(e, &e->d_cctl, &e->cap_cctl, n_chunks, 1)) return rc;
-    if (int rc = grow(e, &e->d_qall, &e->cap_qall, (size_t)n_chunks * q_stride, 1)) return rc;
-    if (int rc = grow(e, &e->d_tiles, &e->cap_tiles, n_tiles, 1)) return rc;
-    if (int rc = grow(e, &e->d_free_acc, &e->cap_free, (size_t)n_batches * (e->occ_bytes / 4), 1)) return rc;
-    {   // token flags carry the call epoch: a (re)allocated buffer must not hold stale flags of an earlier owner
-        const uint32_t before = e->cap_tokens;
-        if (int rc = grow(e, &e->d_tokens, &e->cap_tokens, (size_t)n_chunks * (n_seg + 1), kTokStride)) return rc;
-        if (e->cap_tokens != before) ISL_CUDA(e, cudaMemsetAsync(e->d_tokens, 0, (size_t)e->cap_tokens * kTokStride * sizeof(uint32_t), e->stream));
-    }
-    if (int rc = grow(e, &e->d_ready, &e->cap_ready, n_ready, 1)) return rc;
-    return grow(e, &e->d_done_cnt, &e->cap_done, n_done, 1);
+    ISL_CUDA(e, e->d_chunks.reserve(n_chunks, Growth::headroom));
+    ISL_CUDA(e, e->d_cctl.reserve(n_chunks, Growth::headroom));
+    ISL_CUDA(e, e->d_qall.reserve((size_t)n_chunks * q_stride, Growth::headroom));
+    ISL_CUDA(e, e->d_tiles.reserve(n_tiles, Growth::headroom));
+    ISL_CUDA(e, e->d_free_acc.reserve((size_t)n_batches * (e->occ_bytes / 4), Growth::headroom));
+    bool fresh;     // token flags carry the call epoch: a (re)allocated buffer must not hold stale flags of an earlier owner
+    ISL_CUDA(e, e->d_tokens.reserve((size_t)n_chunks * (n_seg + 1), Growth::headroom, &fresh));
+    if (fresh) ISL_CUDA(e, cudaMemsetAsync(e->d_tokens, 0, e->d_tokens.bytes(), e->stream));
+    ISL_CUDA(e, e->d_ready.reserve(n_ready, Growth::headroom));
+    ISL_CUDA(e, e->d_done_cnt.reserve(n_done, Growth::headroom));
+    return ISL_OK;
 }
 
 // Descriptors of batch b, requests [off, off + n) of the stream: pipeline chunks of pc requests (the FREEs of a batch belong to its first
@@ -538,7 +587,7 @@ PipeArgs pipe_args(const isl_engine* e, const PipePlan& plan, uint32_t n_chunks,
     PipeArgs args{};
     args.n_chunks = n_chunks; args.n_seg = plan.n_seg; args.seg = plan.seg; args.sub = plan.sub; args.lo = e->lo; args.hi = e->hi; args.epoch = epoch;
     args.flip = e->prof.flip; args.wait_ns = e->wait_ns;
-    args.chunks = e->d_chunks; args.cctl = e->d_cctl; args.q_all = e->d_qall; args.free_acc = reinterpret_cast<const uint8_t*>(e->d_free_acc);
+    args.chunks = e->d_chunks; args.cctl = e->d_cctl; args.q_all = e->d_qall; args.free_acc = reinterpret_cast<const uint8_t*>(e->d_free_acc.get());
     args.q_stride = q_stride; args.free_stride = (uint32_t)e->occ_bytes; args.tokens = e->d_tokens; args.occ = e->d_occ; args.gtab = e->d_gtab;
     args.out = out; args.feas = e->d_feas; args.stats = e->d_ctrl;
     if (plan.spec) { args.spec = 1; args.spec_mem = e->d_spec; args.spec_total = plan.n_seg; }
@@ -635,7 +684,7 @@ int run_stream(isl_engine* e, uint32_t n_batches, const uint32_t* sizes, const u
     if (int rc = next_epoch(e, &epoch)) return rc;
     // pre-pass of the tiles [t0, t1): defaults + free masks + histograms, then the stable partition into per-profile queues
     auto prepass = [&](uint32_t t0, uint32_t t1) -> int {
-        k_prepare<<<t1 - t0, kTileThreads, 0, pre>>>(0, d_in, d_out, reinterpret_cast<uint32_t*>(e->d_occ), e->G, e->lo, e->hi, e->prof,
+        k_prepare<<<t1 - t0, kTileThreads, 0, pre>>>(0, d_in, d_out, reinterpret_cast<uint32_t*>(e->d_occ.get()), e->G, e->lo, e->hi, e->prof,
                                                      e->d_tile_counts, e->d_ctrl, e->d_tiles, e->d_free_acc, free_stride / 4, t0);
         if (int rc = check_launch(e, "k_prepare")) return rc;
         if (timing) cudaEventRecord(e->ev[1], e->stream);
@@ -666,25 +715,25 @@ int run_stream(isl_engine* e, uint32_t n_batches, const uint32_t* sizes, const u
     if (timing) cudaEventRecord(e->ev[2], e->stream);
     uint32_t* ring_done = nullptr;
     if (ring && window) {       // the owner's counters sit behind its result array; the other ranks reach them through the same peer mapping
-        uint2* base = e->has_prev ? e->d_owner_out : e->d_res;
+        uint2* base = e->has_prev ? e->d_owner_out.get() : e->d_res.get();
         if (!base) return ISL_ESTATE;
         ring_done = reinterpret_cast<uint32_t*>(base + e->cfg.max_batch);
         if (!e->has_prev) ISL_CUDA(e, cudaMemsetAsync(ring_done, 0, (size_t)n_chunks * sizeof(uint32_t), e->stream));
     }
     const bool trace = e->cfg.flags & ISL_FLAG_TRACE;
     if (trace) {
-        if (int rc = grow(e, &e->d_trace, &e->cap_trace, (size_t)n_chunks * plan.n_seg, kTraceWords)) return rc;
+        ISL_CUDA(e, e->d_trace.reserve((size_t)n_chunks * plan.n_seg, Growth::headroom));
         ISL_CUDA(e, cudaMemsetAsync(e->d_trace, 0, (size_t)n_chunks * plan.n_seg * kTraceWords * sizeof(unsigned long long), e->stream));
         e->trace_chunks = n_chunks; e->trace_seg = plan.n_seg;
     }
     if (plan.spec) if (int rc = prepare_spec(e, n_chunks, epoch, e->stream)) return rc;
     PipeArgs args = pipe_args(e, plan, n_chunks, epoch, q_stride, d_out);
-    args.ready = feed ? e->d_ready : nullptr; args.done_cnt = (h_out_dev || window) ? e->d_done_cnt : nullptr; args.host_out = h_out_dev;
-    args.copier = h_out_dev ? 1u : 0u; args.window = window; args.owner_out = ring ? e->d_owner_out : nullptr;
+    args.ready = feed ? e->d_ready.get() : nullptr; args.done_cnt = (h_out_dev || window) ? e->d_done_cnt.get() : nullptr; args.host_out = h_out_dev;
+    args.copier = h_out_dev ? 1u : 0u; args.window = window; args.owner_out = ring ? e->d_owner_out.get() : nullptr;
     if (ring_done) { args.ring_done = ring_done; args.world = e->ring_world; }
     args.heads_in = d_heads_in; args.heads_out = d_heads_out;
-    args.trace = trace ? e->d_trace : nullptr;
-    args.inbox = ring && e->has_prev ? e->d_inbox : nullptr; args.outbox = ring ? e->d_outbox : nullptr; args.xepoch = xepoch;
+    args.trace = trace ? e->d_trace.get() : nullptr;
+    args.inbox = ring && e->has_prev ? e->d_inbox.get() : nullptr; args.outbox = ring ? e->d_outbox.get() : nullptr; args.xepoch = xepoch;
     if (plan.spec) {
         if (ring) {         // no token ring: the records themselves cross the ranks
             args.inbox = nullptr; args.outbox = nullptr;
@@ -694,8 +743,8 @@ int run_stream(isl_engine* e, uint32_t n_batches, const uint32_t* sizes, const u
         if (const char* v = getenv("ISL_SPEC_DBG")) {       // per-round stamps of one (chunk, stage) cell: tools/spec_trace.py
             unsigned cchunk = 0, cstage = 0;
             if (sscanf(v, "%u,%u", &cchunk, &cstage) == 2) {
-                if (!e->d_specdbg) ISL_CUDA(e, cudaMalloc(&e->d_specdbg, kSpecRounds * 8 * sizeof(unsigned long long)));
-                ISL_CUDA(e, cudaMemsetAsync(e->d_specdbg, 0, kSpecRounds * 8 * sizeof(unsigned long long), e->stream));
+                ISL_CUDA(e, e->d_specdbg.reserve(kSpecRounds));
+                ISL_CUDA(e, cudaMemsetAsync(e->d_specdbg, 0, e->d_specdbg.bytes(), e->stream));
                 args.spec_dbg = e->d_specdbg; args.spec_dbg_cell = (cchunk << 16) | cstage;
             }
         }
@@ -780,18 +829,14 @@ constexpr uint32_t kSpecRingChunks = 64;         // chunks of one partitioned st
 
 int spec_shared_alloc(isl_engine* e) {
     if (e->spec_shared) return ISL_OK;
-    if (e->d_spec) { cudaFree(e->d_spec); e->d_spec = nullptr; e->cap_spec = 0; }
-    ISL_CUDA(e, cudaMalloc(&e->d_spec, (size_t)kSpecRingChunks * kSpecWordsPerChunk * sizeof(unsigned long long)));
-    ISL_CUDA(e, cudaMemset(e->d_spec, 0, (size_t)kSpecRingChunks * kSpecWordsPerChunk * sizeof(unsigned long long)));
-    e->cap_spec = kSpecRingChunks; e->spec_shared = true;
+    ISL_CUDA(e, e->d_spec.replace(kSpecRingChunks));
+    ISL_CUDA(e, cudaMemset(e->d_spec, 0, e->d_spec.bytes()));
+    e->spec_shared = true;
     return ISL_OK;
 }
 
 void spec_disconnect(isl_engine* e) {
-    for (uint32_t r = 0; r < 8; ++r) {
-        if (e->spec_peer[r] && e->spec_peer[r] != e->d_spec && !e->spec_peer_local) cudaIpcCloseMemHandle(e->spec_peer[r]);
-        e->spec_peer[r] = nullptr;
-    }
+    for (auto& peer : e->spec_peer) peer.reset();
     e->spec_world = 0;
 }
 
@@ -808,12 +853,7 @@ int stream_entry(isl_engine* e, uint32_t n_batches, const uint32_t* sizes, bool 
 
 // device copy of the live occupancy (isl_snapshot_occupancy, isl_what_if)
 int snapshot_occ(isl_engine* e) {
-    if (e->snap_bytes < e->occ_bytes) {
-        if (e->d_occ_snap) cudaFree(e->d_occ_snap);
-        e->d_occ_snap = nullptr; e->snap_bytes = 0;
-        ISL_CUDA(e, cudaMalloc(&e->d_occ_snap, e->occ_bytes));
-        e->snap_bytes = e->occ_bytes;
-    }
+    ISL_CUDA(e, e->d_occ_snap.reserve(e->occ_bytes));
     ISL_CUDA(e, cudaMemcpyAsync(e->d_occ_snap, e->d_occ, e->occ_bytes, cudaMemcpyDeviceToDevice, e->stream));
     return ISL_OK;
 }
@@ -881,10 +921,9 @@ int isl_create(const isl_config* cfg, isl_engine** out) {
     if (cudaGetDeviceCount(&ndev) != cudaSuccess || dev >= ndev) { delete e; return ISL_ECUDA; }
     e->device = dev;
     DeviceGuard guard(dev);
-    auto fail = [&](int rc) { isl_destroy(e); return rc; };
-#define ISL_TRY(call) do { if ((call) != cudaSuccess) { return fail(ISL_ECUDA); } } while (0)
-    ISL_TRY(cudaStreamCreateWithFlags(&e->stream, cudaStreamNonBlocking));
-    e->own_stream = true;
+    // a half-built engine is deleted under the guard: its members free what was allocated so far on its device
+#define ISL_TRY(call) do { if ((call) != cudaSuccess) { delete e; return ISL_ECUDA; } } while (0)
+    ISL_TRY(cudaStreamCreateWithFlags(e->stream.out(), cudaStreamNonBlocking));
     {   // Load every kernel NOW.  With CUDA's lazy module loading the first launch of a kernel loads it, and that load can wait for the
         // device to drain — a fed host stream launches k_prepare / k_partition / k_set_flag for batch b WHILE the pipeline kernel is
         // spinning on ready[b]: a first-ever launch at that moment deadlocks (seen as the 20 s trap of a process whose first call was a
@@ -910,31 +949,30 @@ int isl_create(const isl_config* cfg, isl_engine** out) {
     }
     e->occ_bytes = ((size_t)cfg->max_gpus + kSweepBlock - 1) / kSweepBlock * kSweepBlock;
     const uint32_t max_tiles = ceil_div(cfg->max_batch, kTile) + 4096;   // + one partial tile per batch of a stream
-    ISL_TRY(cudaMalloc(&e->d_occ, e->occ_bytes));
-    ISL_TRY(cudaMalloc(&e->d_lut, ISL_MAX_TABLES * ISL_MAX_PROFILES * 256));
-    ISL_TRY(cudaMalloc(&e->d_feas, ISL_MAX_TABLES * 256 * sizeof(uint16_t)));
-    ISL_TRY(cudaMemset(e->d_feas, 0, ISL_MAX_TABLES * 256 * sizeof(uint16_t)));
-    ISL_TRY(cudaMalloc(&e->d_capn, ISL_MAX_TABLES * ISL_MAX_PROFILES * 256));
-    ISL_TRY(cudaMalloc(&e->d_seq, ISL_MAX_TABLES * ISL_MAX_PROFILES * 256 * sizeof(uint32_t)));
-    ISL_TRY(cudaMalloc(&e->d_sizes, ISL_MAX_TABLES * ISL_MAX_PROFILES));
-    ISL_TRY(cudaMalloc(&e->d_score, ISL_MAX_TABLES * ISL_MAX_PROFILES * 256));
-    ISL_TRY(cudaMalloc(&e->d_cap, ISL_MAX_PROFILES * sizeof(unsigned long long)));
-    ISL_TRY(cudaMalloc(&e->d_gtab, e->occ_bytes));
+    ISL_TRY(e->d_occ.reserve(e->occ_bytes));
+    ISL_TRY(e->d_lut.reserve(ISL_MAX_TABLES * ISL_MAX_PROFILES * 256));
+    ISL_TRY(e->d_feas.reserve(ISL_MAX_TABLES * 256));
+    ISL_TRY(cudaMemset(e->d_feas, 0, e->d_feas.bytes()));
+    ISL_TRY(e->d_capn.reserve(ISL_MAX_TABLES * ISL_MAX_PROFILES * 256));
+    ISL_TRY(e->d_seq.reserve(ISL_MAX_TABLES * ISL_MAX_PROFILES * 256));
+    ISL_TRY(e->d_sizes.reserve(ISL_MAX_TABLES * ISL_MAX_PROFILES));
+    ISL_TRY(e->d_score.reserve(ISL_MAX_TABLES * ISL_MAX_PROFILES * 256));
+    ISL_TRY(e->d_cap.reserve(ISL_MAX_PROFILES));
+    ISL_TRY(e->d_gtab.reserve(e->occ_bytes));
     ISL_TRY(cudaMemset(e->d_gtab, 0, e->occ_bytes));
-    ISL_TRY(cudaMalloc(&e->d_cand_o16, e->occ_bytes * sizeof(uint16_t)));
-    ISL_TRY(cudaMalloc(&e->d_req, (size_t)cfg->max_batch * sizeof(uint2)));
-    ISL_TRY(cudaMalloc(&e->d_res, (size_t)cfg->max_batch * sizeof(uint2) + kMaxStreamChunks * sizeof(uint32_t)));   // + per-chunk 'ranks done' counters of a partitioned run (peer-mapped with the results)
-    ISL_TRY(cudaMalloc(&e->d_q, (size_t)kQCap * sizeof(uint16_t)));
-    ISL_TRY(cudaMalloc(&e->d_tile_counts, (size_t)max_tiles * ISL_MAX_PROFILES * sizeof(uint32_t)));
-    ISL_TRY(cudaMalloc(&e->d_cand, e->occ_bytes * sizeof(uint32_t)));
-    ISL_TRY(cudaMalloc(&e->d_log, (size_t)kChunk * sizeof(uint2)));
-    ISL_TRY(cudaMalloc(&e->d_sweep_counts, (e->occ_bytes / kSweepBlock) * sizeof(uint32_t)));
-    ISL_TRY(cudaMalloc(&e->d_ctrl, sizeof(Ctrl)));
+    ISL_TRY(e->d_cand_o16.reserve(e->occ_bytes));
+    ISL_TRY(e->d_req.reserve(cfg->max_batch));
+    ISL_TRY(e->d_res.reserve((size_t)cfg->max_batch + kMaxStreamChunks * sizeof(uint32_t) / sizeof(uint2)));
+    ISL_TRY(e->d_q.reserve(kQCap));
+    ISL_TRY(e->d_tile_counts.reserve((size_t)max_tiles * ISL_MAX_PROFILES));
+    ISL_TRY(e->d_cand.reserve(e->occ_bytes));
+    ISL_TRY(e->d_log.reserve(kChunk));
+    ISL_TRY(e->d_sweep_counts.reserve(e->occ_bytes / kSweepBlock));
+    ISL_TRY(e->d_ctrl.reserve(1));
     ISL_TRY(cudaMemset(e->d_ctrl, 0, sizeof(Ctrl)));
     ISL_TRY(cudaMemset(e->d_occ, 0xFF, e->occ_bytes));
-    for (auto& ev : e->ev) ISL_TRY(cudaEventCreate(&ev));
-    ISL_TRY(cudaHostAlloc(&e->h_small_out, kSmallInline * sizeof(uint2), cudaHostAllocMapped));
-    ISL_TRY(cudaHostGetDevicePointer(&e->d_small_out, e->h_small_out, 0));
+    for (auto& ev : e->ev) ISL_TRY(cudaEventCreate(ev.out()));
+    ISL_TRY(e->h_small_out.reserve(kSmallInline));
 #undef ISL_TRY
     *out = e;
     return ISL_OK;
@@ -943,28 +981,8 @@ int isl_create(const isl_config* cfg, isl_engine** out) {
 int isl_destroy(isl_engine* e) {
     if (!e) return ISL_EINVAL;
     if (e->open.active) isl_stream_close(e);        // a persistent pipeline would never let the stream synchronise
-    {
-        DeviceGuard guard(e->device);
-        if (e->stream) cudaStreamSynchronize(e->stream);
-        cudaFree(e->d_score); cudaFree(e->d_cap); cudaFree(e->d_gtab); cudaFree(e->d_cand_o16); cudaFree(e->d_capn); cudaFree(e->d_seq); cudaFree(e->d_sizes);
-        cudaFree(e->d_occ); cudaFree(e->d_lut); cudaFree(e->d_feas); cudaFree(e->d_req); cudaFree(e->d_res);
-        cudaFree(e->d_q); cudaFree(e->d_tile_counts); cudaFree(e->d_cand); cudaFree(e->d_log); cudaFree(e->d_sweep_counts);
-        cudaFree(e->d_ctrl); cudaFree(e->d_scratch);
-        cudaFree(e->d_chunks); cudaFree(e->d_cctl); cudaFree(e->d_qall); cudaFree(e->d_tokens); spec_disconnect(e); cudaFree(e->d_spec); cudaFree(e->d_specdbg);
-        cudaFree(e->d_free_acc); cudaFree(e->d_tiles);
-        if (e->d_outbox && !e->outbox_local) cudaIpcCloseMemHandle(e->d_outbox);
-        cudaFree(e->d_inbox); cudaFree(e->d_trace); cudaFree(e->d_bf_bitmaps); cudaFree(e->d_ready); cudaFree(e->d_done_cnt); cudaFree(e->d_occ_snap);
-        if (e->feed_stream) cudaStreamDestroy(e->feed_stream);
-        if (e->ev_feed) cudaEventDestroy(e->ev_feed);
-        if (e->ev_feed_done) cudaEventDestroy(e->ev_feed_done);
-        if (e->h_small_out) cudaFreeHost(e->h_small_out);
-        if (e->open.h_done) cudaFreeHost(e->open.h_done);
-        if (e->open.h_chunks) cudaFreeHost(e->open.h_chunks);
-        if (e->open.h_tiles) cudaFreeHost(e->open.h_tiles);
-        if (e->d_owner_out && !e->owner_local) cudaIpcCloseMemHandle(e->d_owner_out);
-        for (auto& ev : e->ev) if (ev) cudaEventDestroy(ev);
-        if (e->own_stream && e->stream) cudaStreamDestroy(e->stream);
-    }
+    DeviceGuard guard(e->device);                   // the members release everything on the engine's device
+    if (e->stream) cudaStreamSynchronize(e->stream);
     delete e;
     return ISL_OK;
 }
@@ -975,9 +993,8 @@ int isl_set_stream(isl_engine* e, void* cuda_stream) {
     if (int rc = lock_idle(e, lk)) return rc;
     DeviceGuard guard(e->device);
     if (e->stream) ISL_CUDA(e, cudaStreamSynchronize(e->stream));
-    if (e->own_stream && e->stream) { cudaStreamDestroy(e->stream); e->own_stream = false; }
-    if (cuda_stream) e->stream = static_cast<cudaStream_t>(cuda_stream);
-    else { ISL_CUDA(e, cudaStreamCreateWithFlags(&e->stream, cudaStreamNonBlocking)); e->own_stream = true; }
+    if (cuda_stream) e->stream.borrow(static_cast<cudaStream_t>(cuda_stream));
+    else ISL_CUDA(e, cudaStreamCreateWithFlags(e->stream.out(), cudaStreamNonBlocking));
     return ISL_OK;
 }
 
@@ -1223,8 +1240,8 @@ int isl_place_gangs(isl_engine* e, uint32_t n_gangs, const uint32_t* gang_off, c
     if (n == 0) return ISL_OK;
     DeviceGuard guard(e->device);
     if (e->hi == e->lo || e->hi - e->lo > kBfMaxGpus) return ISL_ERANGE;          // the class bitmaps of k_bestfit
-    if (int rc = ensure_scratch(e, ((size_t)n_gangs + 1) * sizeof(uint32_t))) return rc;
-    uint32_t* d_gang_off = reinterpret_cast<uint32_t*>(e->d_scratch);
+    ISL_CUDA(e, e->d_scratch.reserve(((size_t)n_gangs + 1) * sizeof(uint32_t)));
+    uint32_t* d_gang_off = reinterpret_cast<uint32_t*>(e->d_scratch.get());
     ISL_CUDA(e, cudaMemcpyAsync(d_gang_off, gang_off, ((size_t)n_gangs + 1) * sizeof(uint32_t), cudaMemcpyHostToDevice, e->stream));
     ISL_CUDA(e, cudaMemcpyAsync(e->d_req, in, (size_t)n * sizeof(isl_request), cudaMemcpyHostToDevice, e->stream));
     if (int rc = run_gangs(e, n_gangs, d_gang_off, n, e->d_req, e->d_res)) return rc;
@@ -1267,7 +1284,7 @@ static int place_batch_plain(isl_engine* e, uint32_t n, const isl_request* in, i
     if (n <= kSmallInline && small_eligible(e, n)) {        // requests as kernel parameters, results into mapped pinned memory: 1 launch + 1 sync
         SmallReqs inl{};
         memcpy(inl.r, in, (size_t)n * sizeof(isl_request));
-        if (int rc = few_eligible(e, n) ? run_few(e, n, inl, e->d_small_out) : run_small(e, n, nullptr, &inl, e->d_small_out)) return rc;
+        if (int rc = few_eligible(e, n) ? run_few(e, n, inl, e->h_small_out.dev()) : run_small(e, n, nullptr, &inl, e->h_small_out.dev())) return rc;
         ISL_CUDA(e, cudaStreamSynchronize(e->stream));
         memcpy(out, e->h_small_out, (size_t)n * sizeof(isl_result));
         return ISL_OK;
@@ -1322,10 +1339,9 @@ int isl_ipc_inbox_handle(isl_engine* e, void* handle64) {
     std::unique_lock<std::mutex> lk;
     if (int rc = lock_idle(e, lk)) return rc;
     DeviceGuard guard(e->device);
-    if (!e->d_inbox) {
-        ISL_CUDA(e, cudaMalloc(&e->d_inbox, (size_t)kMaxStreamChunks * kTokStride * sizeof(uint32_t)));
-        ISL_CUDA(e, cudaMemset(e->d_inbox, 0, (size_t)kMaxStreamChunks * kTokStride * sizeof(uint32_t)));
-    }
+    bool fresh;
+    ISL_CUDA(e, e->d_inbox.reserve(kMaxStreamChunks, Growth::exact, &fresh));
+    if (fresh) ISL_CUDA(e, cudaMemset(e->d_inbox, 0, e->d_inbox.bytes()));
     return ipc_export(e, e->d_inbox, handle64);
 }
 
@@ -1334,9 +1350,8 @@ int isl_ipc_connect(isl_engine* e, const void* next_handle64, int has_prev) {
     std::unique_lock<std::mutex> lk;
     if (int rc = lock_idle(e, lk)) return rc;
     DeviceGuard guard(e->device);
-    if (e->d_outbox && !e->outbox_local) cudaIpcCloseMemHandle(e->d_outbox);
-    e->d_outbox = nullptr; e->outbox_local = false;
-    if (next_handle64) if (int rc = ipc_open(e, next_handle64, &e->d_outbox)) return rc;
+    e->d_outbox.reset();
+    if (next_handle64) if (int rc = ipc_open(e, next_handle64, e->d_outbox.out())) return rc;
     e->has_prev = has_prev != 0;
     if (e->has_prev && !e->d_inbox) return ISL_ESTATE;
     return ISL_OK;
@@ -1346,11 +1361,10 @@ int isl_connect_local(isl_engine* e, isl_engine* next, int has_prev) {
     if (!e) return ISL_EINVAL;
     std::unique_lock<std::mutex> lk;
     if (int rc = lock_idle(e, lk)) return rc;
-    if (e->d_outbox && !e->outbox_local) cudaIpcCloseMemHandle(e->d_outbox);
-    e->d_outbox = nullptr; e->outbox_local = true;
+    e->d_outbox.reset();
     if (next) {
         if (!next->d_inbox) return ISL_ESTATE;
-        e->d_outbox = next->d_inbox;
+        e->d_outbox.borrow(next->d_inbox);
     }
     e->has_prev = has_prev != 0;
     if (e->has_prev && !e->d_inbox) return ISL_ESTATE;
@@ -1378,10 +1392,9 @@ int isl_ipc_connect_spec(isl_engine* e, uint32_t world, uint32_t rank, const voi
     if (world == 0) return ISL_OK;
     if (world < 2 || world > 8 || rank >= world || !handles || !bounds) return ISL_EINVAL;
     if (int rc = spec_shared_alloc(e)) return rc;
-    e->spec_peer_local = false;
     for (uint32_t r = 0; r < world; ++r) {
-        if (r == rank) { e->spec_peer[r] = e->d_spec; continue; }
-        if (int rc = ipc_open(e, static_cast<const char*>(handles) + 64 * r, &e->spec_peer[r])) return rc;
+        if (r == rank) e->spec_peer[r].borrow(e->d_spec);
+        else if (int rc = ipc_open(e, static_cast<const char*>(handles) + 64 * r, e->spec_peer[r].out())) return rc;
     }
     for (uint32_t r = 0; r <= world; ++r) e->spec_bounds[r] = bounds[r];
     e->spec_world = world; e->spec_rank = rank;
@@ -1398,10 +1411,9 @@ int isl_connect_spec_local(isl_engine* e, uint32_t world, uint32_t rank, isl_eng
     if (world == 0) return ISL_OK;
     if (world < 2 || world > 8 || rank >= world || !engines || !bounds) return ISL_EINVAL;
     if (int rc = spec_shared_alloc(e)) return rc;
-    e->spec_peer_local = true;
     for (uint32_t r = 0; r < world; ++r) {
         if (r != rank && (!engines[r] || !engines[r]->spec_shared)) return ISL_ESTATE;     // every engine allocates first (isl_ipc_spec_handle)
-        e->spec_peer[r] = r == rank ? e->d_spec : engines[r]->d_spec;
+        e->spec_peer[r].borrow(r == rank ? e->d_spec.get() : engines[r]->d_spec.get());
     }
     for (uint32_t r = 0; r <= world; ++r) e->spec_bounds[r] = bounds[r];
     e->spec_world = world; e->spec_rank = rank;
@@ -1448,7 +1460,7 @@ int isl_set_partition(isl_engine* e, uint32_t lo, uint32_t hi) {
     return ISL_OK;
 }
 
-void* isl_device_occupancy(isl_engine* e) { return e ? e->d_occ : nullptr; }
+void* isl_device_occupancy(isl_engine* e) { return e ? e->d_occ.get() : nullptr; }
 
 int isl_free_batch(isl_engine* e, uint32_t n, const isl_span* spans) {
     if (!e || (n && !spans)) return ISL_EINVAL;
@@ -1457,9 +1469,9 @@ int isl_free_batch(isl_engine* e, uint32_t n, const isl_span* spans) {
     if (!e->have_inventory) return ISL_ESTATE;
     if (n == 0) return ISL_OK;
     DeviceGuard guard(e->device);
-    if (int rc = ensure_scratch(e, (size_t)n * sizeof(isl_span))) return rc;
+    ISL_CUDA(e, e->d_scratch.reserve((size_t)n * sizeof(isl_span)));
     ISL_CUDA(e, cudaMemcpyAsync(e->d_scratch, spans, (size_t)n * sizeof(isl_span), cudaMemcpyHostToDevice, e->stream));
-    k_free_spans<<<ceil_div(n, 256), 256, 0, e->stream>>>(n, reinterpret_cast<const isl_span*>(e->d_scratch), reinterpret_cast<uint32_t*>(e->d_occ),
+    k_free_spans<<<ceil_div(n, 256), 256, 0, e->stream>>>(n, reinterpret_cast<const isl_span*>(e->d_scratch.get()), reinterpret_cast<uint32_t*>(e->d_occ.get()),
                                                           e->G, e->lo, e->hi, e->d_ctrl, e->prof.flip);
     if (int rc = check_launch(e, "k_free_spans")) return rc;
     ISL_CUDA(e, cudaStreamSynchronize(e->stream));
@@ -1476,7 +1488,7 @@ int isl_eval_starts(isl_engine* e, uint32_t profile, uint32_t n, const uint8_t* 
     if (profile >= e->prof.n || table >= e->n_tables) return ISL_EINVAL;
     if (n == 0) return ISL_OK;
     DeviceGuard guard(e->device);
-    if (int rc = ensure_scratch(e, (size_t)n * 2)) return rc;
+    ISL_CUDA(e, e->d_scratch.reserve((size_t)n * 2));
     ISL_CUDA(e, cudaMemcpyAsync(e->d_scratch, occ, n, cudaMemcpyHostToDevice, e->stream));
     k_eval_starts<<<std::min(ceil_div(n, 256), 1184u), 256, 0, e->stream>>>(e->d_lut + (size_t)table * ISL_MAX_PROFILES * 256, profile, n, e->d_scratch, e->d_scratch + n);
     if (int rc = check_launch(e, "k_eval_starts")) return rc;
@@ -1521,7 +1533,7 @@ int isl_reset_stats(isl_engine* e) {
     const uint64_t launches = e->st.kernel_launches;
     e->st = isl_stats{};
     e->st.kernel_launches = launches;      // launches are counted since creation
-    ISL_CUDA(e, cudaMemsetAsync(&e->d_ctrl->placed, 0, 8 * sizeof(unsigned long long), e->stream));
+    ISL_CUDA(e, cudaMemsetAsync(&e->d_ctrl.get()->placed, 0, 8 * sizeof(unsigned long long), e->stream));
     ISL_CUDA(e, cudaStreamSynchronize(e->stream));
     return ISL_OK;
 }
@@ -1612,7 +1624,7 @@ void* isl_host_alloc(size_t bytes) {
 
 void isl_host_free(void* p) { if (p) cudaFreeHost(p); }
 
-void* isl_device_results(isl_engine* e) { return e ? e->d_res : nullptr; }
+void* isl_device_results(isl_engine* e) { return e ? e->d_res.get() : nullptr; }
 
 int isl_ipc_results_handle(isl_engine* e, void* handle64) {
     if (!e || !handle64) return ISL_EINVAL;
@@ -1627,9 +1639,8 @@ int isl_ipc_connect_owner(isl_engine* e, const void* owner_handle64) {
     std::unique_lock<std::mutex> lk;
     if (int rc = lock_idle(e, lk)) return rc;
     DeviceGuard guard(e->device);
-    if (e->d_owner_out && !e->owner_local) cudaIpcCloseMemHandle(e->d_owner_out);
-    e->d_owner_out = nullptr; e->owner_local = false;
-    if (owner_handle64) return ipc_open(e, owner_handle64, &e->d_owner_out);
+    e->d_owner_out.reset();
+    if (owner_handle64) return ipc_open(e, owner_handle64, e->d_owner_out.out());
     return ISL_OK;
 }
 
@@ -1637,8 +1648,7 @@ int isl_connect_owner_local(isl_engine* e, isl_engine* owner) {
     if (!e) return ISL_EINVAL;
     std::unique_lock<std::mutex> lk;
     if (int rc = lock_idle(e, lk)) return rc;
-    if (e->d_owner_out && !e->owner_local) cudaIpcCloseMemHandle(e->d_owner_out);
-    e->d_owner_out = owner ? owner->d_res : nullptr; e->owner_local = true;
+    e->d_owner_out.borrow(owner ? owner->d_res.get() : nullptr);
     return ISL_OK;
 }
 
@@ -1672,21 +1682,9 @@ int isl_stream_open(isl_engine* e, uint32_t max_batches) {
     o.q_stride = pc + kQPad * ISL_MAX_PROFILES; o.free_stride = (uint32_t)e->occ_bytes; o.tiles_per_batch = pc / kTile;
     if (int rc = grow_stream_buffers(e, max_batches, o.q_stride, max_batches * o.tiles_per_batch, max_batches, plan.n_seg, max_batches + 1, max_batches)) return rc;
     if ((uint64_t)max_batches * o.tiles_per_batch > ceil_div(e->cfg.max_batch, kTile) + 4096) return ISL_ERANGE;
-    if (o.cap_done < max_batches) {
-        if (o.h_done) cudaFreeHost(o.h_done);
-        o.h_done = nullptr; o.cap_done = 0;
-        ISL_CUDA(e, cudaHostAlloc(&o.h_done, (size_t)max_batches * sizeof(uint32_t), cudaHostAllocMapped));
-        ISL_CUDA(e, cudaHostGetDevicePointer(&o.d_done_host, o.h_done, 0));
-        o.cap_done = max_batches;
-    }
-    if (o.cap_desc < max_batches) {
-        if (o.h_chunks) cudaFreeHost(o.h_chunks);
-        if (o.h_tiles) cudaFreeHost(o.h_tiles);
-        o.h_chunks = nullptr; o.h_tiles = nullptr; o.cap_desc = 0;
-        ISL_CUDA(e, cudaHostAlloc(&o.h_chunks, (size_t)max_batches * sizeof(ChunkDesc), cudaHostAllocDefault));
-        ISL_CUDA(e, cudaHostAlloc(&o.h_tiles, (size_t)max_batches * o.tiles_per_batch * sizeof(TileDesc), cudaHostAllocDefault));
-        o.cap_desc = max_batches;
-    }
+    ISL_CUDA(e, o.h_done.reserve(max_batches));
+    ISL_CUDA(e, o.h_chunks.reserve(max_batches));
+    ISL_CUDA(e, o.h_tiles.reserve((size_t)max_batches * o.tiles_per_batch));
     memset(o.h_done, 0, (size_t)max_batches * sizeof(uint32_t));
     if (int rc = ensure_feed_stream(e)) return rc;
     if (int rc = next_epoch(e, &o.epoch)) return rc;
@@ -1720,7 +1718,7 @@ int isl_stream_submit(isl_engine* e, uint32_t n, const isl_request* in, isl_resu
     ISL_CUDA(e, cudaMemcpyAsync(e->d_chunks + b, o.h_chunks + b, sizeof(ChunkDesc), cudaMemcpyHostToDevice, pre));
     ISL_CUDA(e, cudaMemcpyAsync(e->d_tiles + tile0, o.h_tiles + tile0, (size_t)n_tiles * sizeof(TileDesc), cudaMemcpyHostToDevice, pre));
     ISL_CUDA(e, cudaMemcpyAsync(e->d_req + off, in, (size_t)n * sizeof(isl_request), cudaMemcpyHostToDevice, pre));
-    k_prepare<<<n_tiles, kTileThreads, 0, pre>>>(0, e->d_req, e->d_res, reinterpret_cast<uint32_t*>(e->d_occ), e->G, e->lo, e->hi, e->prof,
+    k_prepare<<<n_tiles, kTileThreads, 0, pre>>>(0, e->d_req, e->d_res, reinterpret_cast<uint32_t*>(e->d_occ.get()), e->G, e->lo, e->hi, e->prof,
                                                  e->d_tile_counts, e->d_ctrl, e->d_tiles, e->d_free_acc, o.free_stride / 4, tile0);
     if (int rc = check_launch(e, "k_prepare")) return rc;
     k_partition<<<n_tiles, kTileThreads, 0, pre>>>(0, e->d_req, e->prof.n, e->d_tile_counts, 0, e->cand_profiles, e->d_qall, e->d_cctl,
@@ -1732,7 +1730,7 @@ int isl_stream_submit(isl_engine* e, uint32_t n, const isl_request* in, isl_resu
         ISL_CUDA(e, cudaEventRecord(e->ev_feed, pre));
         ISL_CUDA(e, cudaStreamWaitEvent(e->stream, e->ev_feed, 0));
         PipeArgs args = pipe_args(e, o.plan, o.max_batches, o.epoch, o.q_stride, e->d_res);
-        args.ready = e->d_ready; args.done_cnt = e->d_done_cnt; args.copier = 1; args.open = 1; args.host_done = o.d_done_host;
+        args.ready = e->d_ready; args.done_cnt = e->d_done_cnt; args.copier = 1; args.open = 1; args.host_done = o.h_done.dev();
         args.wait_ns = std::max(kOpenWaitNs, e->wait_ns);
         if (int rc = start_pipeline(e, args)) return rc == ISL_ESTATE ? ISL_ERANGE : rc;
         o.launched = true;
