@@ -9,11 +9,14 @@
 //   no-op         a consistent prefix is not moved by the correction (so "certified" implies "the log in shared memory is the log")
 //   bounded sims  cutting a simulation off and extrapolating its exit never certifies a cut-off log
 // It shares no code with the kernel: prediction, correction and certification are re-derived here from the design.
+// Random mode: spec_rounds_model [cases].  Given workload: spec_rounds_model --world FILE [--bounded] (tests/spec_workloads.py writes it)
+// prints the rounds until the last stage was certified and the stage count.
 #include <algorithm>
 #include <cmath>
 #include <cstdint>
 #include <cstdio>
 #include <cstdlib>
+#include <string>
 #include <vector>
 
 static uint64_t rng_state = 0x9E3779B97F4A7C15ull;
@@ -68,7 +71,8 @@ static void spread(const World& w, Heads& h, const std::vector<int>& grp, long d
     for (int p : grp) { long v = (long)h[p] + dp[p]; h[p] = (uint32_t)std::max(0l, std::min<long>(v, (long)w.q[p].size())); }
 }
 
-static int run_case(uint32_t G, uint32_t seg, uint32_t n_req, int table, bool bounded, uint32_t fill_mask) {
+// random inventory, request mix and table (the random mode below)
+static World random_world(uint32_t G, uint32_t n_req, int table, uint32_t fill_mask) {
     World w;
     // tables: (size, starts) under the reference's quirks (strict bound) or the repaired rule
     auto add = [&](int size, std::vector<int> starts, bool strict) {
@@ -84,6 +88,13 @@ static int run_case(uint32_t G, uint32_t seg, uint32_t n_req, int table, bool bo
     for (auto& o : w.occ) o = (uint8_t)(rnd() & rnd() & fill_mask);
     w.q.assign(np, {});
     for (uint32_t t = 0; t < n_req; ++t) { int p = (int)(rnd() % (np + 1)); if (p < np && !w.prof[p].masks.empty()) w.q[p].push_back(t); }
+    return w;
+}
+
+// The round loop over one world, GPUs [0, G) in stages of seg GPUs.  Returns 0 (and the rounds until the last stage was certified in
+// *rounds_out) or 1 after a FAIL: line.
+static int run_world(const World& w, uint32_t G, uint32_t seg, bool bounded, int* rounds_out) {
+    const int np = (int)w.prof.size();
     const uint32_t S = (G + seg - 1) / seg;
     // truth
     std::vector<Heads> truth(S + 1, Heads(np, 0));
@@ -110,7 +121,8 @@ static int run_case(uint32_t G, uint32_t seg, uint32_t n_req, int table, bool bo
     std::vector<long> Dq(S, 0), Dr(S, 0);
     cprev[0] = true; known[0] = true;
     uint32_t n_cert = 0;
-    for (int round = 1; n_cert < S; ++round) {
+    int round = 1;
+    for (; n_cert < S; ++round) {
         if (getenv("SPEC_MODEL_VERBOSE")) { uint32_t f = 0; while (f < S && certified[f]) ++f; uint32_t e = 0; while (e < S && H[e] == truth[e]) ++e; printf("round %d: certified prefix %u, exact entries prefix %u of %u\n", round, f, e, S); }
         if (round > (int)S + 2) { printf("FAIL: no termination (G %u seg %u)\n", G, seg); return 1; }
         // simulate
@@ -177,11 +189,56 @@ static int run_case(uint32_t G, uint32_t seg, uint32_t n_req, int table, bool bo
             H[s] = Hn[s];
         }
     }
+    if (rounds_out) *rounds_out = round - 1;
     return 0;
+}
+
+static int run_case(uint32_t G, uint32_t seg, uint32_t n_req, int table, bool bounded, uint32_t fill_mask) {
+    const World w = random_world(G, n_req, table, fill_mask);
+    return run_world(w, G, seg, bounded, nullptr);
+}
+
+// A given workload, as whitespace-separated numbers:
+//   G seg n_profiles
+//   per profile: size n_masks mask...            (the masks in the order the start search tries them)
+//   G occupancy bytes
+//   per profile: n_requests time...              (ascending request times)
+static bool read_world(const char* path, World& w, uint32_t& G, uint32_t& seg) {
+    FILE* f = fopen(path, "r");
+    if (!f) return false;
+    bool ok = true;
+    auto num = [&]() -> uint64_t { unsigned long long v = 0; if (fscanf(f, "%llu", &v) != 1) ok = false; return (uint64_t)v; };
+    G = (uint32_t)num(); seg = (uint32_t)num();
+    const uint32_t np = (uint32_t)num();
+    for (uint32_t p = 0; p < np && ok; ++p) {
+        Profile pr; pr.size = (int)num();
+        const uint32_t nm = (uint32_t)num();
+        for (uint32_t k = 0; k < nm && ok; ++k) pr.masks.push_back((uint32_t)num());
+        w.prof.push_back(pr);
+    }
+    w.occ.resize(G);
+    for (uint32_t g = 0; g < G && ok; ++g) w.occ[g] = (uint8_t)num();
+    w.q.assign(np, {});
+    for (uint32_t p = 0; p < np && ok; ++p) {
+        const uint32_t n = (uint32_t)num();
+        for (uint32_t i = 0; i < n && ok; ++i) w.q[p].push_back((uint32_t)num());
+        for (uint32_t i = 1; i < n && ok; ++i) ok = w.q[p][i - 1] < w.q[p][i];
+    }
+    fclose(f);
+    return ok && G > 0 && seg > 0;
 }
 
 #ifndef SPEC_MODEL_NO_MAIN
 int main(int argc, char** argv) {
+    if (argc > 2 && std::string(argv[1]) == "--world") {       // spec_rounds_model --world FILE [--bounded]
+        World w; uint32_t G = 0, seg = 0;
+        if (!read_world(argv[2], w, G, seg)) { printf("FAIL: cannot read world %s\n", argv[2]); return 2; }
+        const bool bounded = argc > 3 && std::string(argv[3]) == "--bounded";
+        int rounds = 0;
+        const int bad = run_world(w, G, seg, bounded, &rounds);
+        if (!bad) printf("rounds %d stages %u\n", rounds, (G + seg - 1) / seg);
+        return bad;
+    }
     const int cases = argc > 1 ? atoi(argv[1]) : 60;
     int bad = 0;
     for (int i = 0; i < cases && !bad; ++i) {
