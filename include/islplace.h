@@ -279,6 +279,50 @@ int  isl_place_batch_range(isl_engine* e, uint32_t lo, uint32_t hi, uint32_t n, 
  * that is empty or holds more than 2^20 GPUs.  ISL_ESTATE: no profiles or inventory, or an open stream. */
 int  isl_place_gangs(isl_engine* e, uint32_t n_gangs, const uint32_t* gang_off, const isl_request* in, isl_result* out);
 
+/* 8 bytes: one running allocation that MAY be evicted (isl_preempt). */
+typedef struct isl_victim {
+    uint32_t gpu;                  /* canonical GPU index */
+    uint8_t  start, size;          /* its span */
+    uint8_t  priority;             /* rank, higher = more important; 255 = never evicted */
+    uint8_t  pad;
+} isl_victim;
+
+/* Priority preemption (the kube-scheduler's PriorityClass preemption for pods the scheduler never sees): for each pending pod that
+ * does not fit, which GPU and start it should take and which lower-priority allocations must leave first.  `in`, `priority` (one byte
+ * per request, higher = more important), `out` and `evict` (n x 8 uint32) are host buffers of n entries; `victims` has n_victims.
+ *   1. A query.  The live occupancy, a snapshot (isl_snapshot_occupancy), the partition and the stats (except kernel_launches) are the
+ *      same after the call as before; everything runs under one engine lock.  The caller deletes the victim pods; once their
+ *      Allocations entries are gone, an ordinary placement call places the pod.
+ *   2. Each victims[k] names a span that is busy in the live occupancy.  Every busy slice not covered by a listed victim is pinned
+ *      (dangling Prepared slices, allocations the caller does not list, victims with priority 255).  A victim on a GPU outside the
+ *      engine's partition is ignored, as isl_free_batch ignores such spans.  ISL_EINVAL, nothing changed: a victim with size 0,
+ *      start + size > 8 or gpu >= G, or (inside the partition) one that covers a free slice or overlaps another victim.
+ *   3. The preemptors are in[i] at priority[i], in array order; preemptor i sees the state left by 0..i-1 of the same call: their
+ *      victims are gone (slices free, no longer listed), their own spans busy and pinned.  An ALLOC of an unknown profile gets the
+ *      BAD_PROFILE record of isl_place_batch; ISL_OP_FREE makes the call ISL_EINVAL (the victim list is how releases are expressed);
+ *      any other op gets an ISL_ST_NOOP record.
+ *   4. A candidate for an ALLOC of profile p at priority pi is a GPU g of the partition with a start v of p's row in the table of g's
+ *      node, legal under the engine's quirk set (candidate_mask, the rule of the start search), such that every busy slice of the
+ *      mask belongs to a listed victim with priority < pi.  V(g, v) is every victim that overlaps the mask; a victim leaves whole,
+ *      also where it extends beyond the mask.
+ *   5. The choice is the lexicographic minimum over all candidates of: the highest priority in V (an empty V below every priority),
+ *      the sum of V's priorities, |V|, the GPU's position in the engine's scan order (ascending canonical index; descending under
+ *      ISL_POLICY_RIGHT_TO_LEFT; ascending for the best-fit family), v's position in the row — the order of the kube-scheduler's
+ *      pickOneNodeForPreemption without its PodDisruptionBudget and start-time keys.  The record is PLACED (g, v, size) and
+ *      evict[8i .. 8i+8) holds the indices into `victims` of V in ascending order, padded with ISL_GPU_NONE.  With no candidate the
+ *      record is the usual unplaced one (NO_CAPACITY, gpu NONE, start 9, the default size); a record that is not PLACED has an
+ *      evict row of ISL_GPU_NONE only.  Consequences:
+ *      (a) v is what the start search (:343-383) returns on g's occupancy with V removed: an earlier start in the row would need a
+ *          subset of V, and so would have a smaller key.
+ *      (b) a pod that fits without eviction evicts nothing: a one-request call on a FIRST_FIT or RIGHT_TO_LEFT engine returns the
+ *          record isl_place_batch returns.
+ *   6. Every policy, both quirk sets, per-node tables, inside isl_set_partition.  n == 0 does nothing.
+ *      ISL_EINVAL: NULL buffers with n > 0 (or victims NULL with n_victims > 0), an engine created with ISL_FLAG_ALL_NODES.
+ *      ISL_ERANGE: n > max_batch, n_victims > 8 x max_gpus, a partition that is empty or holds more than 2^20 GPUs.
+ *      ISL_ESTATE: no profiles or inventory, or an open stream. */
+int  isl_preempt(isl_engine* e, uint32_t n, const isl_request* in, const uint8_t* priority,
+                 uint32_t n_victims, const isl_victim* victims, isl_result* out, uint32_t* evict);
+
 /* ---- open streams: the causal feed --------------------------------------- */
 /* A reconciler that composes batch b+1 from the results of batch b (a FREE names an allocation an earlier batch placed) cannot hand
  * all batches over up front.  An open stream keeps ONE persistent pipeline kernel resident:

@@ -285,6 +285,54 @@ class InstasliceReconciler:
             out.append(("placed", [alloc for _, alloc in packed]))
         return out
 
+    def preempt_pending_pods(self, pods: list, pod_priority: dict):
+        """Priority preemption for gated pods the kube-scheduler never sees as MIG-constrained (ONE engine call, isl_preempt).
+
+        ``pods`` are shaped as ``place_pending_pods`` takes them, each with a ``"priority"`` (the int32 value of its PriorityClass);
+        ``pod_priority`` maps the UID of each running pod to its value.  Values become dense order-preserving ranks over every value
+        seen (more than 255 distinct values is a ``ValueError``).  An ``Allocations`` entry may be evicted only when its pod's priority
+        is known, its status is not ``"deleted"`` (it is already leaving) and no other entry that marks slices busy (a dangling
+        Prepared slice or another allocation) overlaps its span, for otherwise releasing it would not free its slices; every other
+        busy slice is pinned.
+
+        Returns per pod ("fits", None, []) | ("preempt", {"nodename", "gpuUUID", "start", "size"}, [victim pod UIDs]) |
+        ("none", None, []).  Nothing is written to the custom resources: the caller deletes the victim pods, and once the daemonset
+        has removed their allocations a later ``place_pending_pods`` places the pod on the reported slices (first-fit engine).
+        """
+        values = sorted({int(p["priority"]) for p in pods} | {int(v) for v in pod_priority.values()})
+        if len(values) > 255:
+            raise ValueError("more than 255 distinct priority values")
+        rank = {v: r for r, v in enumerate(values)}
+        victims, uids = [], []
+        for n, it in enumerate(self.items):
+            spec = it["spec"]
+            for g in range(int(self.node_off[n]), int(self.node_off[n + 1])):
+                uuid = self.gpu_uuid[g]
+                entries = [(None, p) for p in spec.get("prepared", {}).values() if p["parent"] == uuid and p.get("podUUID", "") == ""]
+                entries += [(uid, a) for uid, a in spec.get("allocations", {}).items() if a["gpuUUID"] == uuid]
+                masks = [((1 << int(x["size"])) - 1) << int(x["start"]) for _, x in entries]
+                for j, (uid, a) in sorted(enumerate(entries), key=lambda e: int(e[1][1]["start"])):
+                    if uid is None or uid not in pod_priority or a.get("allocationStatus") == "deleted":
+                        continue
+                    if any(masks[j] & m for k, m in enumerate(masks) if k != j):
+                        continue
+                    victims.append((g, int(a["start"]), int(a["size"]), rank[int(pod_priority[uid])], 0))
+                    uids.append(uid)
+        res, evict = self._engine.preempt(self._requests([p["profile"] for p in pods]),
+                                          np.array([rank[int(p["priority"])] for p in pods], dtype=np.uint8),
+                                          np.array(victims, dtype=E.VICTIM_DTYPE))
+        out = []
+        for r, row in zip(res, evict):
+            if r["status"] != E.ST_PLACED:
+                out.append(("none", None, []))
+                continue
+            gone = [uids[int(k)] for k in row if k != E.GPU_NONE]
+            uuid = self.gpu_uuid[int(r["gpu"])]
+            where = {"nodename": self.items[self.node_of_uuid[uuid]]["metadata"]["name"], "gpuUUID": uuid,
+                     "start": int(r["start"]), "size": int(r["size"])}
+            out.append(("preempt", where, gone) if gone else ("fits", None, []))
+        return out
+
     def release(self, pod_uid: str):
         """The daemonset deleted ``Allocations[podUID]`` (instaslice_daemonset.go:261-263): free its span."""
         for n, it in enumerate(self.items):

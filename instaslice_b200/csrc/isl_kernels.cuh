@@ -17,6 +17,7 @@
 //                        (profile, start) candidate and a warp min-reduction per accepted placement
 #pragma once
 
+#include <cooperative_groups.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
 
@@ -2255,6 +2256,181 @@ __global__ void __launch_bounds__(kBfThreads, 1) k_bestfit(uint32_t n, const uin
     }
     if (kGang) close_gangs(n);
     if (lane == 0) { atomicAdd(&ctrl->placed, (unsigned long long)placed); atomicAdd(&ctrl->steps, (unsigned long long)placed); }
+}
+
+// ---------------------------------------------------------------------------------------------
+// Priority preemption (isl_preempt, DESIGN.md 4.7).
+//   k_victim_map  one thread per victim: validates its span and claims its slices in the per-slice victim-index map (partition-local
+//                 GPU x 8 words, kVictimNone where no listed victim covers the slice); any violation raises a bit of *err
+//   k_preempt     one cooperative launch for the whole call: each CTA keeps its contiguous share of the partition in shared memory,
+//                 every preemptor is one 64-bit min over all (GPU, legal start) candidates, reduced per CTA and then grid-wide
+// ---------------------------------------------------------------------------------------------
+constexpr uint32_t kVictimNone = 0xFFFFFFFFu;
+constexpr uint32_t kPreThreads = 512;
+constexpr uint32_t kPreMaxGpus = 1u << 20;              // the key's GPU field has 24 bits; the gang limit of the engine's other paths
+// Shared memory per GPU of a CTA's share: 8 priority bytes, the occupancy byte, the run-start byte, the table byte.  At kPreMaxGpus over
+// the 132 SMs of an H100 a CTA holds 7 944 GPUs = 87 KB, below the 227 KB a CTA may opt into on sm_90 (the host checks the device's limit).
+constexpr uint32_t kPreBytesPerGpu = 11;
+constexpr uint32_t kVmErrSpan = 1u, kVmErrFree = 2u, kVmErrOverlap = 4u;
+
+__global__ void k_victim_map(uint32_t n, const isl_victim* __restrict__ victims, const uint8_t* __restrict__ occ, uint32_t G, uint32_t lo,
+                             uint32_t hi, uint32_t flip, uint32_t* __restrict__ vmap, uint32_t* __restrict__ err) {
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const isl_victim v = victims[i];
+    if (v.gpu >= G || v.size == 0 || v.start + v.size > ISL_SLOTS) { atomicOr(err, kVmErrSpan); return; }
+    const uint32_t gi = flip_gpu(v.gpu, flip);
+    if (gi < lo || gi >= hi) return;                    // outside the partition: ignored, as isl_free_batch ignores such spans
+    const uint32_t span = ((1u << v.size) - 1u) << v.start;
+    if ((occ[gi] & span) != span) atomicOr(err, kVmErrFree);
+    uint32_t* w = vmap + (size_t)(gi - lo) * ISL_SLOTS;
+    for (uint32_t s = v.start; s < v.start + v.size; ++s)
+        if (atomicCAS(w + s, kVictimNone, i) != kVictimNone) atomicOr(err, kVmErrOverlap);
+}
+
+struct PreemptArgs {            // kernel parameter (by value)
+    const uint2* in;            // requests (isl_request)
+    const uint8_t* prio;        // priority of every request
+    const isl_victim* victims;
+    const uint32_t* vmap;       // k_victim_map's output
+    const uint8_t* occ;         // the live occupancy (storage order), read only
+    const uint8_t* gtab;        // table of every GPU's node (storage order)
+    const uint8_t* masks;       // [table][profile][position in the row]: candidate_mask of that start, 0 = none
+    uint2* out;
+    uint32_t* evict;            // n x 8 victim indices
+    unsigned long long* keys;   // [2][gridDim.x] per-CTA minima, double-buffered by preemptor parity
+    uint32_t n, lo, Gr, per_cta;
+};
+
+// Candidate key, lexicographic (isl_preempt rule 5):  [50:42] highest priority in V + 1, 0 for an empty V | [41:31] sum of V's
+// priorities (<= 8 x 254) | [30:27] |V| | [26:3] GPU in scan order (partition-local storage index) | [2:0] position of the start in the
+// row.  V of a legal (GPU, start) is every victim that overlaps the mask: one head slice per victim — the run starts inside the mask, plus
+// the mask's lowest slice when it is busy (a victim that begins below the mask).
+__device__ __forceinline__ unsigned long long preempt_key(uint32_t m, uint32_t o, uint32_t rs, unsigned long long pr, uint32_t g, uint32_t k) {
+    const uint32_t heads = (rs & m) | (o & m & (m & (0u - m)));
+    uint32_t mx = 0, sum = 0;
+    for (uint32_t h = heads; h; h &= h - 1) {
+        const uint32_t b = (uint32_t)(pr >> (8 * (__ffs(h) - 1))) & 0xFFu;
+        mx = max(mx, b + 1u); sum += b;
+    }
+    return ((unsigned long long)mx << 42) | ((unsigned long long)sum << 31) | ((unsigned long long)__popc(heads) << 27) |
+           ((unsigned long long)g << 3) | k;
+}
+
+__device__ __forceinline__ unsigned long long warp_min_u64(unsigned long long v) {
+    const uint32_t hi = redux_min_u32((uint32_t)(v >> 32));
+    const uint32_t lo = redux_min_u32((uint32_t)(v >> 32) == hi ? (uint32_t)v : kInf);
+    return ((unsigned long long)hi << 32) | lo;
+}
+
+__global__ void __launch_bounds__(kPreThreads, 1) k_preempt(PreemptArgs a, DevProfiles prof) {
+    extern __shared__ __align__(8) unsigned char pre_smem[];
+    __shared__ uint8_t s_masks[kMaxTables * ISL_MAX_PROFILES * ISL_MAX_STARTS];
+    __shared__ unsigned long long s_warp[kPreThreads / 32];
+    __shared__ unsigned long long s_win;
+    const uint32_t tid = threadIdx.x, lane = tid & 31u, warp = tid >> 5;
+    const uint32_t base = blockIdx.x * a.per_cta, cnt = base < a.Gr ? min(a.per_cta, a.Gr - base) : 0u;
+    unsigned long long* s_prio = reinterpret_cast<unsigned long long*>(pre_smem);      // byte s = priority of slice s, 255 = no victim
+    uint8_t* s_occ = pre_smem + (size_t)a.per_cta * 8;
+    uint8_t* s_rs = s_occ + a.per_cta;                  // bit s: a victim begins at slice s
+    uint8_t* s_tab = s_rs + a.per_cta;
+    for (uint32_t i = tid; i < sizeof(s_masks); i += kPreThreads) s_masks[i] = a.masks[i];
+    for (uint32_t g = tid; g < cnt; g += kPreThreads) {
+        const uint4* w4 = reinterpret_cast<const uint4*>(a.vmap + (size_t)(base + g) * ISL_SLOTS);
+        const uint4 w0 = w4[0], w1 = w4[1];
+        const uint32_t w[ISL_SLOTS] = {w0.x, w0.y, w0.z, w0.w, w1.x, w1.y, w1.z, w1.w};
+        unsigned long long pr = 0;
+        uint32_t rs = 0;
+#pragma unroll
+        for (uint32_t s = 0; s < ISL_SLOTS; ++s) {
+            const uint32_t p = w[s] == kVictimNone ? 0xFFu : a.victims[w[s]].priority;
+            pr |= (unsigned long long)p << (8 * s);
+            if (w[s] != kVictimNone && (s == 0 || w[s - 1] != w[s])) rs |= 1u << s;
+        }
+        s_prio[g] = pr; s_rs[g] = (uint8_t)rs;
+        s_occ[g] = a.occ[a.lo + base + g]; s_tab[g] = a.gtab[a.lo + base + g];
+    }
+    __syncthreads();
+    cooperative_groups::grid_group grid = cooperative_groups::this_grid();
+    uint32_t parity = 0;
+    for (uint32_t i = 0; i < a.n; ++i) {
+        const uint2 rq = a.in[i];
+        const uint32_t profile = rq.y & 0xFFu, op = (rq.y >> 8) & 0xFFu;
+        if (op != ISL_OP_ALLOC || profile >= prof.n) {      // the same for every CTA: no exchange
+            if (blockIdx.x == 0 && tid < ISL_SLOTS) {
+                if (tid == 0) a.out[i] = op == ISL_OP_ALLOC ? pack_result(ISL_GPU_NONE, ISL_START_NONE, 0, ISL_ST_BAD_PROFILE)
+                                                            : pack_result(ISL_GPU_NONE, ISL_START_NONE, 0, ISL_ST_NOOP);
+                a.evict[(size_t)i * ISL_SLOTS + tid] = kVictimNone;
+            }
+            continue;
+        }
+        const uint32_t pi = a.prio[i];
+        unsigned long long best = ~0ull;
+        for (uint32_t g = tid; g < cnt; g += kPreThreads) {
+            const unsigned long long pr = s_prio[g];
+            const uint32_t o = s_occ[g], rs = s_rs[g];
+            uint32_t ev = 0;                                // slices whose victim has a priority below the preemptor's
+#pragma unroll
+            for (uint32_t s = 0; s < ISL_SLOTS; ++s) ev |= (((uint32_t)(pr >> (8 * s)) & 0xFFu) < pi) << s;
+            const uint32_t blocked = o & ~ev;
+            const uint8_t* mk = s_masks + ((uint32_t)s_tab[g] * ISL_MAX_PROFILES + profile) * ISL_MAX_STARTS;
+#pragma unroll
+            for (uint32_t k = 0; k < ISL_MAX_STARTS; ++k) {
+                const uint32_t m = mk[k];
+                if (m && !(m & blocked)) best = min(best, preempt_key(m, o, rs, pr, base + g, k));
+            }
+        }
+        best = warp_min_u64(best);
+        if (lane == 0) s_warp[warp] = best;
+        __syncthreads();
+        if (warp == 0) {
+            best = warp_min_u64(lane < kPreThreads / 32 ? s_warp[lane] : ~0ull);
+            if (lane == 0) a.keys[parity * gridDim.x + blockIdx.x] = best;
+        }
+        grid.sync();                                        // every CTA's minimum of preemptor i is in keys[parity]
+        if (warp == 0) {
+            unsigned long long v = ~0ull;
+            for (uint32_t c = lane; c < gridDim.x; c += 32) v = min(v, __ldcg(a.keys + parity * gridDim.x + c));
+            v = warp_min_u64(v);
+            if (lane == 0) s_win = v;
+        }
+        __syncthreads();
+        const unsigned long long win = s_win;
+        parity ^= 1u;
+        if (win == ~0ull) {                                 // no candidate anywhere: the usual unplaced record
+            if (blockIdx.x == 0 && tid < ISL_SLOTS) {
+                if (tid == 0) a.out[i] = pack_result(ISL_GPU_NONE, ISL_START_NONE, prof.rows[profile].size, ISL_ST_NO_CAPACITY);
+                a.evict[(size_t)i * ISL_SLOTS + tid] = kVictimNone;
+            }
+            continue;
+        }
+        const uint32_t gw = (uint32_t)(win >> 3) & 0xFFFFFFu, k = (uint32_t)win & 7u;
+        if (gw - base < cnt && tid == 0) {                  // the CTA that owns the GPU applies the eviction to its own state
+            const uint32_t g = gw - base, o = s_occ[g], rs = s_rs[g];
+            const uint32_t m = s_masks[((uint32_t)s_tab[g] * ISL_MAX_PROFILES + profile) * ISL_MAX_STARTS + k];
+            const uint32_t heads = (rs & m) | (o & m & (m & (0u - m)));
+            const uint4* w4 = reinterpret_cast<const uint4*>(a.vmap + (size_t)gw * ISL_SLOTS);
+            const uint4 w0 = w4[0], w1 = w4[1];
+            const uint32_t w[ISL_SLOTS] = {w0.x, w0.y, w0.z, w0.w, w1.x, w1.y, w1.z, w1.w};
+            uint32_t idx[ISL_SLOTS], nv = 0, gone = 0;
+            for (uint32_t h = heads; h; h &= h - 1) {
+                const uint32_t v = w[__ffs(h) - 1];     // a victim leaves whole: every slice it covers is still its own
+                uint32_t j = nv++;
+                for (; j > 0 && idx[j - 1] > v; --j) idx[j] = idx[j - 1];
+                idx[j] = v;
+#pragma unroll
+                for (uint32_t s = 0; s < ISL_SLOTS; ++s) gone |= (w[s] == v) << s;
+            }
+            const uint32_t touched = gone | m;          // freed or taken: either way no victim any more
+            unsigned long long pr = s_prio[g];
+#pragma unroll
+            for (uint32_t s = 0; s < ISL_SLOTS; ++s) if ((touched >> s) & 1u) pr |= 0xFFull << (8 * s);
+            s_prio[g] = pr; s_rs[g] = (uint8_t)(rs & ~touched); s_occ[g] = (uint8_t)((o & ~gone) | m);
+            a.out[i] = pack_result(flip_gpu(a.lo + gw, prof.flip), __ffs(m) - 1, __popc(m), ISL_ST_PLACED);
+            for (uint32_t j = 0; j < ISL_SLOTS; ++j) a.evict[(size_t)i * ISL_SLOTS + j] = j < nv ? idx[j] : kVictimNone;
+        }
+        __syncthreads();                                    // the owner's state is updated before its threads score the next preemptor
+    }
 }
 
 }  // namespace isl

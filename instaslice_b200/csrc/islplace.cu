@@ -164,6 +164,14 @@ struct isl_engine {
     DevMem<uint32_t> d_ready;        // [batch] epoch flag
     DevMem<uint32_t> d_done_cnt;     // [chunk] committed segments
     DevMem<uint8_t> d_occ_snap; uint32_t snap_G = 0;      // isl_snapshot_occupancy / isl_restore_occupancy
+    // isl_preempt: the victim-index map (8 words per GPU of the partition), the victims, staging of [candidate masks | priorities], the
+    // evict rows, the per-CTA minima of k_preempt and k_victim_map's error word
+    struct Preempt {
+        DevMem<uint32_t> vmap, evict, err;
+        DevMem<isl_victim> victims;
+        DevMem<uint8_t> stage;
+        DevMem<unsigned long long> keys;
+    } pre;
     bool delivered = false;          // the last run_stream call already put the results into the caller's host buffer
     unsigned long long wait_ns = 20000000000ull;   // a starved device-side wait traps after this long (ISL_WAIT_SECONDS overrides the 20 s)
     uint32_t window = 0;             // causal window of stream calls (isl_set_causal_window): chunk c starts after chunk c - window is committed
@@ -931,7 +939,7 @@ int isl_create(const isl_config* cfg, isl_engine** out) {
         cudaFuncAttributes fa;
         const void* kernels[] = {(const void*)k_prepare, (const void*)k_partition, (const void*)k_set_flag, (const void*)k_few, (const void*)k_build_lut, (const void*)k_eval_starts,
                                  (const void*)k_free_spans, (const void*)k_capacity, (const void*)k_sweep_count, (const void*)k_sweep_scatter, (const void*)k_commit, (const void*)k_bestfit<false>, (const void*)k_bestfit<true>,
-                                 (const void*)k_bestfit<false, true>, (const void*)k_bestfit<true, true>,
+                                 (const void*)k_bestfit<false, true>, (const void*)k_bestfit<true, true>, (const void*)k_victim_map, (const void*)k_preempt,
                                  (const void*)k_chain<1>, (const void*)k_chain<2>, (const void*)k_chain<4>, (const void*)k_small<1>, (const void*)k_small<2>, (const void*)k_small<4>};
         const void* pipes[] = {(const void*)k_pipeline<1, false, false>, (const void*)k_pipeline<1, true, false>, (const void*)k_pipeline<2, false, false>, (const void*)k_pipeline<2, true, false>,
                                (const void*)k_pipeline<4, false, false>, (const void*)k_pipeline<4, true, false>,
@@ -946,6 +954,10 @@ int isl_create(const isl_config* cfg, isl_engine** out) {
         for (const void* k : {(const void*)k_bestfit<false>, (const void*)k_bestfit<false, true>})
             ISL_TRY(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(256 * (kBfSmemGpus / 32 + kBfSmemGpus / 1024) * sizeof(uint32_t))));
         for (const void* k : pipes) ISL_TRY(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kPipeSmem));
+        int optin = 0;          // k_preempt's share of the partition: up to what the device lets one CTA have
+        ISL_TRY(cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev));
+        ISL_TRY(cudaFuncGetAttributes(&fa, k_preempt));
+        ISL_TRY(cudaFuncSetAttribute((const void*)k_preempt, cudaFuncAttributeMaxDynamicSharedMemorySize, optin - (int)fa.sharedSizeBytes));
     }
     e->occ_bytes = ((size_t)cfg->max_gpus + kSweepBlock - 1) / kSweepBlock * kSweepBlock;
     const uint32_t max_tiles = ceil_div(cfg->max_batch, kTile) + 4096;   // + one partial tile per batch of a stream
@@ -1246,6 +1258,69 @@ int isl_place_gangs(isl_engine* e, uint32_t n_gangs, const uint32_t* gang_off, c
     ISL_CUDA(e, cudaMemcpyAsync(e->d_req, in, (size_t)n * sizeof(isl_request), cudaMemcpyHostToDevice, e->stream));
     if (int rc = run_gangs(e, n_gangs, d_gang_off, n, e->d_req, e->d_res)) return rc;
     ISL_CUDA(e, cudaMemcpyAsync(out, e->d_res, (size_t)n * sizeof(isl_result), cudaMemcpyDeviceToHost, e->stream));
+    ISL_CUDA(e, cudaStreamSynchronize(e->stream));
+    return ISL_OK;
+}
+
+int isl_preempt(isl_engine* e, uint32_t n, const isl_request* in, const uint8_t* priority,
+                uint32_t n_victims, const isl_victim* victims, isl_result* out, uint32_t* evict) {
+    if (!e || (n && (!in || !priority || !out || !evict)) || (n_victims && !victims)) return ISL_EINVAL;
+    if (e->cfg.flags & ISL_FLAG_ALL_NODES) return ISL_EINVAL;      // one pod on every node with capacity: no single GPU to evict on
+    for (uint32_t i = 0; i < n; ++i) if (in[i].op == ISL_OP_FREE) return ISL_EINVAL;      // releases are expressed by the victim list
+    if (n > e->cfg.max_batch || (uint64_t)n_victims > (uint64_t)ISL_SLOTS * e->cfg.max_gpus) return ISL_ERANGE;
+    std::unique_lock<std::mutex> lk;
+    if (int rc = lock_idle(e, lk)) return rc;
+    if (int rc = validate_ready(e, n)) return rc;
+    if (n == 0) return ISL_OK;
+    const uint32_t Gr = e->hi - e->lo;
+    if (Gr == 0 || Gr > kPreMaxGpus) return ISL_ERANGE;
+    DeviceGuard guard(e->device);
+    // one CTA per SM at most (the grid-wide exchange per preemptor is cheaper with fewer CTAs), at least one thread per GPU below that
+    int sms = 0, per_sm = 0;
+    ISL_CUDA(e, cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, e->device));
+    const uint32_t grid = std::max(1u, std::min((uint32_t)sms, ceil_div(Gr, kPreThreads))), per_cta = ceil_div(Gr, grid);
+    const size_t smem = (size_t)per_cta * kPreBytesPerGpu;
+    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_preempt, kPreThreads, smem) != cudaSuccess || per_sm < 1) {
+        cudaGetLastError();
+        return ISL_ERANGE;                                  // a share too large for one CTA's shared memory on this device
+    }
+    auto& p = e->pre;
+    constexpr size_t kMaskBytes = kMaxTables * ISL_MAX_PROFILES * ISL_MAX_STARTS;
+    ISL_CUDA(e, p.vmap.reserve((size_t)Gr * ISL_SLOTS));
+    ISL_CUDA(e, p.evict.reserve((size_t)n * ISL_SLOTS));
+    ISL_CUDA(e, p.err.reserve(1));
+    ISL_CUDA(e, p.victims.reserve(std::max(n_victims, 1u)));
+    ISL_CUDA(e, p.stage.reserve(kMaskBytes + n));
+    ISL_CUDA(e, p.keys.reserve((size_t)2 * grid));
+    uint8_t masks[kMaskBytes] = {0};                        // [table][profile][position in the row]: the start search's legal masks
+    for (uint32_t t = 0; t < e->n_tables; ++t)
+        for (uint32_t q = 0; q < e->prof.n; ++q)
+            for (uint32_t k = 0; k < e->rows_all[t][q].n_starts; ++k)
+                masks[(t * ISL_MAX_PROFILES + q) * ISL_MAX_STARTS + k] = (uint8_t)candidate_mask(e->rows_all[t][q].size, e->rows_all[t][q].starts[k], e->cfg.quirks);
+    ISL_CUDA(e, cudaMemcpyAsync(e->d_req, in, (size_t)n * sizeof(isl_request), cudaMemcpyHostToDevice, e->stream));
+    ISL_CUDA(e, cudaMemcpyAsync(p.stage, masks, kMaskBytes, cudaMemcpyHostToDevice, e->stream));
+    ISL_CUDA(e, cudaMemcpyAsync(p.stage + kMaskBytes, priority, n, cudaMemcpyHostToDevice, e->stream));
+    ISL_CUDA(e, cudaMemsetAsync(p.vmap, 0xFF, (size_t)Gr * ISL_SLOTS * sizeof(uint32_t), e->stream));
+    ISL_CUDA(e, cudaMemsetAsync(p.err, 0, sizeof(uint32_t), e->stream));
+    if (n_victims) {
+        ISL_CUDA(e, cudaMemcpyAsync(p.victims, victims, (size_t)n_victims * sizeof(isl_victim), cudaMemcpyHostToDevice, e->stream));
+        k_victim_map<<<ceil_div(n_victims, 256), 256, 0, e->stream>>>(n_victims, p.victims, e->d_occ, e->G, e->lo, e->hi, e->prof.flip, p.vmap, p.err);
+        if (int rc = check_launch(e, "k_victim_map")) return rc;
+        uint32_t err = 0;
+        ISL_CUDA(e, cudaMemcpyAsync(&err, p.err, sizeof err, cudaMemcpyDeviceToHost, e->stream));
+        ISL_CUDA(e, cudaStreamSynchronize(e->stream));
+        if (err) return ISL_EINVAL;                         // a malformed, free or overlapping victim: nothing else runs
+    }
+    PreemptArgs a{};
+    a.in = e->d_req; a.prio = p.stage + kMaskBytes; a.victims = p.victims; a.vmap = p.vmap; a.occ = e->d_occ; a.gtab = e->d_gtab;
+    a.masks = p.stage; a.out = e->d_res; a.evict = p.evict; a.keys = p.keys;
+    a.n = n; a.lo = e->lo; a.Gr = Gr; a.per_cta = per_cta;
+    void* params[] = {&a, &e->prof};
+    const cudaError_t err = cudaLaunchCooperativeKernel((const void*)k_preempt, dim3(grid), dim3(kPreThreads), params, smem, e->stream);
+    if (err != cudaSuccess) { cudaGetLastError(); snprintf(e->cuda_err, sizeof(e->cuda_err), "k_preempt: %s", cudaGetErrorString(err)); return ISL_ECUDA; }
+    ++e->st.kernel_launches;
+    ISL_CUDA(e, cudaMemcpyAsync(out, e->d_res, (size_t)n * sizeof(isl_result), cudaMemcpyDeviceToHost, e->stream));
+    ISL_CUDA(e, cudaMemcpyAsync(evict, p.evict, (size_t)n * ISL_SLOTS * sizeof(uint32_t), cudaMemcpyDeviceToHost, e->stream));
     ISL_CUDA(e, cudaStreamSynchronize(e->stream));
     return ISL_OK;
 }

@@ -36,8 +36,9 @@ RESULT_DTYPE = np.dtype([("gpu", "<u4"), ("start", "u1"), ("size", "u1"), ("stat
 SPAN_DTYPE = np.dtype([("gpu", "<u4"), ("start", "u1"), ("size", "u1"), ("pad", "<u2")])
 PROFILE_DTYPE = np.dtype([("size", "u1"), ("n_starts", "u1"), ("starts", "u1", (8,)), ("pad", "u1", (2,)),
                           ("gi", "<i4"), ("ci", "<i4"), ("cieng", "<i4")])
+VICTIM_DTYPE = np.dtype([("gpu", "<u4"), ("start", "u1"), ("size", "u1"), ("priority", "u1"), ("pad", "u1")])
 assert REQUEST_DTYPE.itemsize == 8 and RESULT_DTYPE.itemsize == 8 and SPAN_DTYPE.itemsize == 8
-assert PROFILE_DTYPE.itemsize == 24
+assert PROFILE_DTYPE.itemsize == 24 and VICTIM_DTYPE.itemsize == 8
 
 
 class Config(C.Structure):
@@ -114,7 +115,14 @@ SIGNATURES = {
     "isl_capacity": (C.c_int, [_P, _P]),
     "isl_what_if": (C.c_int, [_P, C.c_uint32, _P, _P, _P, _P]),
 }
-EXPORTED_SYMBOLS = list(SIGNATURES)
+# isl_preempt is bound from a table of its own: the return code of every entry point above in every engine state is classified by the
+# test suite's per-state contract, which also probes each of them; isl_preempt's codes in the same states (created, profiles only,
+# inventory only, ready, empty partition, the three sub-states of an open stream, ISL_FLAG_ALL_NODES) are pinned by
+# tests/test_gpu_preempt.py::test_return_code_in_every_engine_state
+PREEMPT_SIGNATURES = {
+    "isl_preempt": (C.c_int, [_P, C.c_uint32, _P, _P, C.c_uint32, _P, _P, _P]),
+}
+EXPORTED_SYMBOLS = list(SIGNATURES) + list(PREEMPT_SIGNATURES)
 
 _lib = None
 
@@ -127,7 +135,7 @@ def load_library(path: str = LIB_PATH):
     if not os.path.exists(path):
         raise ImportError(f"{path} not built: run __graft_entry__.build() (nvcc, sm_90a). There is no CPU fallback.")
     lib = C.CDLL(path)
-    for name, (res, args) in SIGNATURES.items():
+    for name, (res, args) in {**SIGNATURES, **PREEMPT_SIGNATURES}.items():
         try:
             fn = getattr(lib, name)
         except AttributeError:
@@ -336,6 +344,21 @@ class Engine:
         out = np.empty(len(requests), dtype=RESULT_DTYPE)
         self._check(self._lib.isl_place_gangs(self._h, len(gang_off) - 1, _ptr(gang_off), _ptr(requests), _ptr(out)), "isl_place_gangs")
         return out
+
+    def preempt(self, requests: np.ndarray, priority, victims: np.ndarray):
+        """Priority preemption query (isl_preempt): for each ALLOC in ``requests`` at ``priority[i]`` (uint8, higher = more important),
+        the GPU and start it would take once the lower-priority ``victims`` (VICTIM_DTYPE) listed in ``evict[i]`` are gone.  Returns
+        ``(results, evict)``, ``evict`` an [n, 8] uint32 array of victim indices padded with GPU_NONE.  Changes no engine state."""
+        requests = np.ascontiguousarray(requests, dtype=REQUEST_DTYPE)
+        priority = np.ascontiguousarray(priority, dtype=np.uint8)
+        victims = np.ascontiguousarray(victims, dtype=VICTIM_DTYPE)
+        if len(priority) != len(requests):
+            raise ValueError("one priority per request")
+        out = np.empty(len(requests), dtype=RESULT_DTYPE)
+        evict = np.empty((len(requests), 8), dtype=np.uint32)
+        self._check(self._lib.isl_preempt(self._h, len(requests), _ptr(requests), _ptr(priority), len(victims), _ptr(victims), _ptr(out),
+                                          _ptr(evict)), "isl_preempt")
+        return out, evict
 
     # -- open streams (the causal feed)
     def stream_open(self, max_batches: int):

@@ -1,6 +1,8 @@
 // instaslice_host.cpp — see instaslice_host.hpp.  Builds into instaslice_b200/libislhost.so (links libislplace.so).
 #include "instaslice_host.hpp"
 
+#include <algorithm>
+#include <set>
 #include <stdexcept>
 
 namespace instaslice {
@@ -248,6 +250,61 @@ std::vector<GangOutcome> InstasliceReconciler::PlaceGangs(InstasliceList& list, 
         }
         for (uint32_t i = off[g]; i < off[g + 1]; ++i) list.Items[gpuNode_[res[i].gpu]].Spec.Allocations[gangs[g][i - off[g]].pod.UID] = o.allocs[i - off[g]];
         o.verdict = Verdict::Placed;
+    }
+    return out;
+}
+
+std::vector<PreemptOutcome> InstasliceReconciler::PreemptPending(const InstasliceList& list, const std::vector<PreemptPod>& pods,
+                                                                 const std::map<std::string, int32_t>& podPriority) {
+    std::vector<PreemptOutcome> out(pods.size());
+    if (pods.empty()) return out;
+    std::set<int32_t> values;
+    for (const PreemptPod& p : pods) values.insert(p.Priority);
+    for (const auto& kv : podPriority) values.insert(kv.second);
+    if (values.size() > 255) throw std::runtime_error("more than 255 distinct priority values");
+    std::map<int32_t, uint8_t> rank;
+    for (int32_t v : values) rank.emplace(v, (uint8_t)rank.size());
+    auto span = [](uint32_t start, uint32_t size) { return ((1u << size) - 1u) << start; };
+    std::vector<isl_victim> victims;
+    std::vector<std::string> uids;
+    for (uint32_t g = 0; g < gpuUUID_.size(); ++g) {            // victims in (GPU, start) order
+        const InstasliceSpec& spec = list.Items[gpuNode_[g]].Spec;
+        const std::string& uuid = gpuUUID_[g];
+        std::vector<uint32_t> masks;                            // every entry that marks slices of this GPU busy (:306-328)
+        for (const auto& kv : spec.Prepared)
+            if (kv.second.Parent == uuid && kv.second.PodUUID.empty()) masks.push_back(span(kv.second.Start, kv.second.Size));
+        std::vector<std::pair<uint32_t, std::string>> allocs;
+        for (const auto& kv : spec.Allocations)
+            if (kv.second.GPUUUID == uuid) { masks.push_back(span(kv.second.Start, kv.second.Size)); allocs.push_back({kv.second.Start, kv.first}); }
+        std::sort(allocs.begin(), allocs.end());
+        for (const auto& [start, uid] : allocs) {
+            const AllocationDetails& a = spec.Allocations.at(uid);
+            const auto pr = podPriority.find(uid);
+            if (pr == podPriority.end() || a.Allocationstatus == "deleted") continue;
+            const uint32_t m = span(a.Start, a.Size);
+            int overlapping = 0;                                // itself once; anything more would keep its slices busy
+            for (uint32_t x : masks) overlapping += (x & m) != 0;
+            if (overlapping > 1) continue;
+            victims.push_back({g, (uint8_t)a.Start, (uint8_t)a.Size, rank.at(pr->second), 0});
+            uids.push_back(uid);
+        }
+    }
+    std::vector<std::string> names;
+    std::vector<uint8_t> prio;
+    for (const PreemptPod& p : pods) { names.push_back(p.ProfileName); prio.push_back(rank.at(p.Priority)); }
+    const std::vector<isl_request> req = requests(names);
+    std::vector<isl_result> res(pods.size());
+    std::vector<uint32_t> evict(pods.size() * 8);
+    check(isl_preempt(h_, (uint32_t)pods.size(), req.data(), prio.data(), (uint32_t)victims.size(), victims.data(), res.data(), evict.data()),
+          h_, "isl_preempt");
+    for (size_t i = 0; i < pods.size(); ++i) {
+        if (res[i].status != ISL_ST_PLACED) continue;
+        PreemptOutcome& o = out[i];
+        o.Nodename = list.Items[gpuNode_[res[i].gpu]].Name;
+        o.GPUUUID = gpuUUID_[res[i].gpu];
+        o.Start = res[i].start; o.Size = res[i].size;
+        for (size_t k = 0; k < 8; ++k) if (evict[i * 8 + k] != ISL_GPU_NONE) o.Victims.push_back(uids[evict[i * 8 + k]]);
+        o.verdict = o.Victims.empty() ? PreemptVerdict::Fits : PreemptVerdict::Preempt;
     }
     return out;
 }

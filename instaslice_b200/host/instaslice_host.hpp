@@ -71,6 +71,15 @@ struct RightToLeftPolicy : LeftToRightPolicy {}; // :464-469
 enum class Verdict { Placed, None, Veto };       // allocation written / "failed to find allocatable gpu" everywhere / :198-203 requeue
 struct PendingPod { Pod pod; std::string ProfileName; };
 struct Outcome { Verdict verdict = Verdict::None; AllocationDetails alloc; };
+// Priority preemption (extension: isl_preempt): a pending pod with the int32 value of its PriorityClass; the answer for it.
+struct PreemptPod { Pod pod; std::string ProfileName; int32_t Priority = 0; };
+enum class PreemptVerdict { Fits, Preempt, None };     // fits as things are / fits once Victims are gone / no GPU even with evictions
+struct PreemptOutcome {
+    PreemptVerdict verdict = PreemptVerdict::None;
+    std::string Nodename, GPUUUID;                    // where the pod would go (Fits and Preempt)
+    uint32_t Start = 0, Size = 0;
+    std::vector<std::string> Victims;                 // pod UIDs to delete first (Preempt)
+};
 struct GangOutcome { Verdict verdict = Verdict::None; std::vector<AllocationDetails> allocs; };   // allocs: one per pod when Placed
 
 extern const char* const kErrNoGpu;              // "failed to find allocatable gpu" (:261)
@@ -101,6 +110,13 @@ public:
     // only then are its allocations written into `list`.  None: a pod found no GPU, nothing of the gang was committed.  Veto: the
     // Prepared exact-match check (:198-203) fired on a pod, every span of the gang was released again.  Empty gangs throw.
     std::vector<GangOutcome> PlaceGangs(InstasliceList& list, AllocationPolicy& policy, const std::vector<std::vector<PendingPod>>& gangs);
+    // Which lower-priority allocations each pending pod should evict, in order, ONE engine call (isl_preempt).  podPriority maps the UID
+    // of each running pod to its PriorityClass value; values become dense ranks (more than 255 distinct values throw).  An allocation
+    // may be evicted only when its pod's priority is known, its status is not "deleted" and no other entry that marks slices busy
+    // overlaps it; every other busy slice is pinned.  Writes nothing into `list`: the caller deletes the Victims, and once their
+    // allocations are gone a later PlacePending places the pod there.
+    std::vector<PreemptOutcome> PreemptPending(const InstasliceList& list, const std::vector<PreemptPod>& pods,
+                                               const std::map<std::string, int32_t>& podPriority);
     // The daemonset removed Allocations[podUID] (instaslice_daemonset.go:261-263).
     bool Release(InstasliceList& list, const std::string& podUID);
 

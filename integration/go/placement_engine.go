@@ -591,3 +591,128 @@ func (e *PlacementEngine) WhatIf(plan func() error) error {
 	}
 	return err
 }
+
+// PreemptTarget is the answer of PreemptPending for one pod.  Victims empty and Placed: the pod fits as things are.  Not Placed: no GPU
+// even with evictions.
+type PreemptTarget struct {
+	Placed   bool
+	Nodename string
+	GPUUUID  string
+	Start    uint32
+	Size     uint32
+	Victims  []string // pod UIDs to delete before the pod is placed
+}
+
+// PreemptPending is priority preemption for the gated pods (ONE engine call, isl_preempt): for each pod, in order, the GPU and start it
+// would take and the lower-priority pods that must leave first.  priority[i] is the PriorityClass value of pods[i]; podPriority maps the
+// UID of each running pod to its value.  Values become dense order-preserving ranks (more than 255 distinct values is an error).  An
+// Allocations entry is a victim only when its pod's priority is known, its status is not "deleted" and no other entry that marks slices
+// busy (a dangling Prepared slice or another allocation) overlaps it; everything else is pinned.  Nothing is written to the custom
+// resources: the caller deletes the victims, and once the daemonset has removed their allocations a later PlacePending places the pod.
+func (r *InstasliceReconciler) PreemptPending(e *PlacementEngine, list *inferencev1alpha1.InstasliceList, pods []PendingPod,
+	priority []int32, podPriority map[string]int32) ([]PreemptTarget, error) {
+	out := make([]PreemptTarget, len(pods))
+	if len(pods) == 0 {
+		return out, nil
+	}
+	seen := map[int32]bool{}
+	for _, v := range priority {
+		seen[v] = true
+	}
+	for _, v := range podPriority {
+		seen[v] = true
+	}
+	if len(seen) > 255 {
+		return nil, fmt.Errorf("more than 255 distinct priority values")
+	}
+	values := make([]int32, 0, len(seen))
+	for v := range seen {
+		values = append(values, v)
+	}
+	sort.Slice(values, func(i, j int) bool { return values[i] < values[j] })
+	rank := map[int32]uint8{}
+	for i, v := range values {
+		rank[v] = uint8(i)
+	}
+	span := func(start, size uint32) uint32 { return ((1 << size) - 1) << start }
+	var victims []C.isl_victim
+	var uids []string
+	for g, uuid := range e.gpuUUID { // victims in (GPU, start) order
+		spec := &list.Items[e.gpuNode[g]].Spec
+		var masks []uint32 // every entry that marks slices of this GPU busy (:306-328)
+		for _, p := range spec.Prepared {
+			if p.Parent == uuid && p.PodUUID == "" {
+				masks = append(masks, span(uint32(p.Start), uint32(p.Size)))
+			}
+		}
+		var mine []string
+		for uid, a := range spec.Allocations {
+			if a.GPUUUID == uuid {
+				masks = append(masks, span(uint32(a.Start), uint32(a.Size)))
+				mine = append(mine, uid)
+			}
+		}
+		sort.Slice(mine, func(i, j int) bool {
+			ai, aj := spec.Allocations[mine[i]], spec.Allocations[mine[j]]
+			return ai.Start < aj.Start || (ai.Start == aj.Start && mine[i] < mine[j])
+		})
+		for _, uid := range mine {
+			a := spec.Allocations[uid]
+			v, known := podPriority[uid]
+			if !known || a.Allocationstatus == "deleted" {
+				continue
+			}
+			m, overlapping := span(uint32(a.Start), uint32(a.Size)), 0
+			for _, x := range masks {
+				if x&m != 0 {
+					overlapping++ // itself once; anything more would keep its slices busy
+				}
+			}
+			if overlapping > 1 {
+				continue
+			}
+			victims = append(victims, C.isl_victim{gpu: C.uint32_t(g), start: C.uint8_t(a.Start), size: C.uint8_t(a.Size), priority: C.uint8_t(rank[v])})
+			uids = append(uids, uid)
+		}
+	}
+	n := len(pods)
+	reqP, resP := C.malloc(C.size_t(n)*C.sizeof_isl_request), C.malloc(C.size_t(n)*C.sizeof_isl_result)
+	prioP, evictP := C.malloc(C.size_t(n)), C.malloc(C.size_t(n)*8*4)
+	vicP := C.malloc(C.size_t(len(victims)+1) * C.sizeof_isl_victim)
+	defer C.free(reqP)
+	defer C.free(resP)
+	defer C.free(prioP)
+	defer C.free(evictP)
+	defer C.free(vicP)
+	if reqP == nil || resP == nil || prioP == nil || evictP == nil || vicP == nil {
+		return nil, fmt.Errorf("out of memory")
+	}
+	req := (*[1 << 28]C.isl_request)(reqP)[:n:n]
+	res := (*[1 << 28]C.isl_result)(resP)[:n:n]
+	prio := (*[1 << 28]C.uint8_t)(prioP)[:n:n]
+	evict := (*[1 << 28]C.uint32_t)(evictP)[: 8*n : 8*n]
+	vic := (*[1 << 28]C.isl_victim)(vicP)[: len(victims)+1 : len(victims)+1]
+	copy(vic, victims)
+	e.fillRequests(req, pods, 0)
+	for i := range pods {
+		prio[i] = C.uint8_t(rank[priority[i]])
+	}
+	if rc := C.isl_preempt(e.h, C.uint32_t(n), &req[0], &prio[0], C.uint32_t(len(victims)), &vic[0], &res[0], &evict[0]); rc != C.ISL_OK {
+		return nil, fmt.Errorf("isl_preempt: %s (%s)", C.GoString(C.isl_strerror(rc)), C.GoString(C.isl_last_cuda_error(e.h)))
+	}
+	for i := range pods {
+		if res[i].status != C.ISL_ST_PLACED {
+			continue
+		}
+		g := int(res[i].gpu)
+		t := PreemptTarget{Placed: true, Nodename: list.Items[e.gpuNode[g]].Name, GPUUUID: e.gpuUUID[g],
+			Start: uint32(res[i].start), Size: uint32(res[i].size)}
+		for k := 0; k < 8; k++ {
+			if idx := uint32(evict[8*i+k]); idx != C.ISL_GPU_NONE {
+				t.Victims = append(t.Victims, uids[idx])
+			}
+		}
+		out[i] = t
+	}
+	return out, nil
+}
