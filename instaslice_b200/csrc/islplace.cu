@@ -11,6 +11,7 @@
 #include <cmath>
 #include <mutex>
 #include <new>
+#include <optional>
 #include <type_traits>
 #include <utility>
 #include <vector>
@@ -216,6 +217,32 @@ struct DeviceGuard {
     int prev = -1;
     explicit DeviceGuard(int dev) { cudaGetDevice(&prev); if (prev != dev) cudaSetDevice(dev); else prev = -1; }
     ~DeviceGuard() { if (prev >= 0) cudaSetDevice(prev); }
+};
+
+// What an entry point needs of the engine: the engine states of include/islplace.h, or an open stream (isl_stream_submit / _close).
+enum class Needs { nothing, profiles, inventory, ready, open_stream };
+
+// The prologue of every entry point that takes an engine, except the lock-free isl_stream_wait, destroy and the pure getters: the engine
+// lock, the state checks, then the engine's device.  rc is ISL_ESTATE while an open stream owns the engine (its resident kernel would keep
+// any work enqueued behind the call waiting until isl_stream_close, and the state it runs on must not change under it), or, for the
+// stream calls, while none is open; ISL_ESTATE when the tables or the inventory that `needs` names are missing; ISL_ERANGE when a batch of
+// n requests exceeds max_batch (Needs::ready).  The state is tested under the lock, so no call can slip in after another thread's
+// isl_stream_open.  The device is made current only when rc is ISL_OK; the lock is declared first, so the device is restored before the
+// unlock.
+struct Entry {
+    std::unique_lock<std::mutex> lock;
+    std::optional<DeviceGuard> device;
+    int rc = ISL_ESTATE;
+    Entry(isl_engine* e, Needs needs, uint64_t n = 0) : lock(e->mu) {
+        const bool have = needs == Needs::profiles    ? e->have_profiles
+                          : needs == Needs::inventory ? e->have_inventory
+                          : needs == Needs::ready     ? e->have_profiles && e->have_inventory
+                                                      : true;
+        if (e->open.active != (needs == Needs::open_stream) || !have) return;
+        if (needs == Needs::ready && n > e->cfg.max_batch) { rc = ISL_ERANGE; return; }
+        device.emplace(e->device);
+        rc = ISL_OK;
+    }
 };
 
 inline uint32_t ceil_div(uint32_t a, uint32_t b) { return (a + b - 1) / b; }
@@ -796,21 +823,6 @@ int run_stream(isl_engine* e, uint32_t n_batches, const uint32_t* sizes, const u
     return ISL_OK;
 }
 
-// The engine lock of every entry point except the stream calls and the pure getters, refused while an open stream owns the engine: its
-// resident kernel would keep any work enqueued behind it waiting until isl_stream_close, and the state it runs on must not change under
-// it.  The test runs under the lock, so no call can slip in after another thread's isl_stream_open.
-int lock_idle(isl_engine* e, std::unique_lock<std::mutex>& lk) {
-    lk = std::unique_lock<std::mutex>(e->mu);
-    return e->open.active ? ISL_ESTATE : ISL_OK;
-}
-
-// under lock_idle
-int validate_ready(isl_engine* e, uint32_t n) {
-    if (!e->have_profiles || !e->have_inventory) return ISL_ESTATE;
-    if (n > e->cfg.max_batch) return ISL_ERANGE;
-    return ISL_OK;
-}
-
 // Default row of every name (its size is what an unplaced ALLOC reports): the row of the first node, in canonical order, whose table has
 // the name; without a node map (isl_set_node_tables) every node uses table 0.
 void derive_default_rows(isl_engine* e) {
@@ -849,7 +861,7 @@ void spec_disconnect(isl_engine* e) {
 }
 
 // The argument checks of the stream entry points: 1..4096 batches that fit max_batch, buffers for a non-empty stream.  The engine's
-// readiness is checked under the lock (lock_idle, validate_ready).
+// readiness is checked under the lock (Entry).
 int stream_entry(isl_engine* e, uint32_t n_batches, const uint32_t* sizes, bool have_buffers, uint64_t* total) {
     if (!e || !sizes || n_batches == 0 || n_batches > 4096) return ISL_EINVAL;
     *total = 0;
@@ -1001,9 +1013,8 @@ int isl_destroy(isl_engine* e) {
 
 int isl_set_stream(isl_engine* e, void* cuda_stream) {
     if (!e) return ISL_EINVAL;
-    std::unique_lock<std::mutex> lk;
-    if (int rc = lock_idle(e, lk)) return rc;
-    DeviceGuard guard(e->device);
+    Entry guard(e, Needs::nothing);
+    if (guard.rc) return guard.rc;
     if (e->stream) ISL_CUDA(e, cudaStreamSynchronize(e->stream));
     if (cuda_stream) e->stream.borrow(static_cast<cudaStream_t>(cuda_stream));
     else ISL_CUDA(e, cudaStreamCreateWithFlags(e->stream.out(), cudaStreamNonBlocking));
@@ -1012,15 +1023,14 @@ int isl_set_stream(isl_engine* e, void* cuda_stream) {
 
 int isl_synchronize(isl_engine* e) {
     if (!e) return ISL_EINVAL;
-    std::unique_lock<std::mutex> lk;
-    if (int rc = lock_idle(e, lk)) return rc;
-    DeviceGuard guard(e->device);
+    Entry guard(e, Needs::nothing);
+    if (guard.rc) return guard.rc;
     ISL_CUDA(e, cudaStreamSynchronize(e->stream));
     return ISL_OK;
 }
 
-// shared by isl_load_profiles (one table, every row must have placements) and isl_load_profile_tables
-static int load_tables(isl_engine* e, uint32_t n_tables, uint32_t n, const isl_profile* rows, bool allow_absent) {
+// The argument checks of isl_load_profiles (one table, every row must have placements) and isl_load_profile_tables, before the lock
+static int check_tables(const isl_engine* e, uint32_t n_tables, uint32_t n, const isl_profile* rows, bool allow_absent) {
     if (!e || !rows || n == 0 || n > ISL_MAX_PROFILES || n_tables == 0 || n_tables > ISL_MAX_TABLES) return ISL_EINVAL;
     // Validate what would make the reference panic (SURVEY Q7): empty Placements (:334), start >= 8 (:345).
     uint32_t total_cand = 0;
@@ -1034,9 +1044,11 @@ static int load_tables(isl_engine* e, uint32_t n_tables, uint32_t n, const isl_p
         }
     }
     if (total_cand > kMaxCand) return ISL_EINVAL;          // more (table, profile, start) candidates than the chain's 4 x 32 lane slots
-    std::unique_lock<std::mutex> lk;
-    if (int rc = lock_idle(e, lk)) return rc;
-    DeviceGuard guard(e->device);
+    return ISL_OK;
+}
+
+// The tables of both calls, under their Entry
+static int load_tables(isl_engine* e, uint32_t n_tables, uint32_t n, const isl_profile* rows) {
     e->n_tables = n_tables;
     memset(e->rows_all, 0, sizeof(e->rows_all));
     for (uint32_t t = 0; t < n_tables; ++t) memcpy(e->rows_all[t], rows + (size_t)t * n, n * sizeof(isl_profile));
@@ -1107,20 +1119,26 @@ static int load_tables(isl_engine* e, uint32_t n_tables, uint32_t n, const isl_p
     return ISL_OK;
 }
 
-int isl_load_profiles(isl_engine* e, uint32_t n, const isl_profile* rows) { return load_tables(e, 1, n, rows, false); }
+int isl_load_profiles(isl_engine* e, uint32_t n, const isl_profile* rows) {
+    if (int rc = check_tables(e, 1, n, rows, false)) return rc;
+    Entry guard(e, Needs::nothing);
+    if (guard.rc) return guard.rc;
+    return load_tables(e, 1, n, rows);
+}
 
 int isl_load_profile_tables(isl_engine* e, uint32_t n_tables, uint32_t n_profiles, const isl_profile* rows) {
-    return load_tables(e, n_tables, n_profiles, rows, true);
+    if (int rc = check_tables(e, n_tables, n_profiles, rows, true)) return rc;
+    Entry guard(e, Needs::nothing);
+    if (guard.rc) return guard.rc;
+    return load_tables(e, n_tables, n_profiles, rows);
 }
 
 int isl_set_node_tables(isl_engine* e, uint32_t n_nodes, const uint8_t* table_of_node) {
     if (!e || !table_of_node) return ISL_EINVAL;
-    std::unique_lock<std::mutex> lk;
-    if (int rc = lock_idle(e, lk)) return rc;
-    if (!e->have_inventory || !e->have_profiles) return ISL_ESTATE;
+    Entry guard(e, Needs::ready);
+    if (guard.rc) return guard.rc;
     if (n_nodes + 1 != e->node_off.size()) return ISL_EINVAL;
     for (uint32_t n = 0; n < n_nodes; ++n) if (table_of_node[n] >= e->n_tables) return ISL_EINVAL;
-    DeviceGuard guard(e->device);
     e->node_table.assign(table_of_node, table_of_node + n_nodes);
     std::vector<uint8_t> gtab(e->G);
     for (uint32_t n = 0; n < n_nodes; ++n)
@@ -1138,9 +1156,8 @@ int isl_load_inventory(isl_engine* e, uint32_t n_nodes, const uint32_t* node_off
     const uint32_t G = node_off[n_nodes];
     if (G == 0 || !occ) return ISL_EINVAL;
     if (G > e->cfg.max_gpus) return ISL_ERANGE;
-    std::unique_lock<std::mutex> lk;
-    if (int rc = lock_idle(e, lk)) return rc;
-    DeviceGuard guard(e->device);
+    Entry guard(e, Needs::nothing);
+    if (guard.rc) return guard.rc;
     e->node_off.assign(node_off, node_off + n_nodes + 1);
     e->G = G; e->lo = 0; e->hi = G;
     e->prof.flip = reversed(e) ? G : 0u;      // ISL_POLICY_RIGHT_TO_LEFT: the inventory is stored in reverse canonical order
@@ -1157,10 +1174,8 @@ int isl_load_inventory(isl_engine* e, uint32_t n_nodes, const uint32_t* node_off
 
 int isl_read_occupancy(isl_engine* e, uint8_t* out) {
     if (!e || !out) return ISL_EINVAL;
-    std::unique_lock<std::mutex> lk;
-    if (int rc = lock_idle(e, lk)) return rc;
-    if (!e->have_inventory) return ISL_ESTATE;
-    DeviceGuard guard(e->device);
+    Entry guard(e, Needs::inventory);
+    if (guard.rc) return guard.rc;
     ISL_CUDA(e, cudaMemcpyAsync(out, e->d_occ, e->G, cudaMemcpyDeviceToHost, e->stream));
     ISL_CUDA(e, cudaStreamSynchronize(e->stream));
     if (e->prof.flip) std::reverse(out, out + e->G);       // canonical order at the boundary
@@ -1169,12 +1184,10 @@ int isl_read_occupancy(isl_engine* e, uint8_t* out) {
 
 int isl_write_occupancy(isl_engine* e, uint32_t first_gpu, uint32_t n, const uint8_t* occ) {
     if (!e || (n && !occ)) return ISL_EINVAL;
-    std::unique_lock<std::mutex> lk;
-    if (int rc = lock_idle(e, lk)) return rc;
-    if (!e->have_inventory) return ISL_ESTATE;
+    Entry guard(e, Needs::inventory);
+    if (guard.rc) return guard.rc;
     if ((uint64_t)first_gpu + n > e->G) return ISL_ERANGE;
     if (n == 0) return ISL_OK;
-    DeviceGuard guard(e->device);
     std::vector<uint8_t> rev;
     if (e->prof.flip) { rev.assign(occ, occ + n); std::reverse(rev.begin(), rev.end()); occ = rev.data(); first_gpu = e->G - first_gpu - n; }
     ISL_CUDA(e, cudaMemcpyAsync(e->d_occ + first_gpu, occ, n, cudaMemcpyHostToDevice, e->stream));
@@ -1184,10 +1197,8 @@ int isl_write_occupancy(isl_engine* e, uint32_t first_gpu, uint32_t n, const uin
 
 int isl_snapshot_occupancy(isl_engine* e) {
     if (!e) return ISL_EINVAL;
-    std::unique_lock<std::mutex> lk;
-    if (int rc = lock_idle(e, lk)) return rc;
-    if (!e->have_inventory) return ISL_ESTATE;
-    DeviceGuard guard(e->device);
+    Entry guard(e, Needs::inventory);
+    if (guard.rc) return guard.rc;
     if (int rc = snapshot_occ(e)) return rc;
     e->snap_G = e->G;
     return ISL_OK;
@@ -1195,10 +1206,9 @@ int isl_snapshot_occupancy(isl_engine* e) {
 
 int isl_restore_occupancy(isl_engine* e) {
     if (!e) return ISL_EINVAL;
-    std::unique_lock<std::mutex> lk;
-    if (int rc = lock_idle(e, lk)) return rc;
-    if (!e->have_inventory || !e->d_occ_snap || e->snap_G != e->G) return ISL_ESTATE;     // a snapshot belongs to the inventory it was taken from
-    DeviceGuard guard(e->device);
+    Entry guard(e, Needs::inventory);
+    if (guard.rc) return guard.rc;
+    if (!e->d_occ_snap || e->snap_G != e->G) return ISL_ESTATE;     // a snapshot belongs to the inventory it was taken from
     ISL_CUDA(e, cudaMemcpyAsync(e->d_occ, e->d_occ_snap, e->occ_bytes, cudaMemcpyDeviceToDevice, e->stream));
     return ISL_OK;
 }
@@ -1215,22 +1225,18 @@ static int place_batch_locked(isl_engine* e, uint32_t n, const isl_request* in, 
 
 int isl_place_batch(isl_engine* e, uint32_t n, const isl_request* in, isl_result* out) {
     if (!e || (n && (!in || !out))) return ISL_EINVAL;
-    std::unique_lock<std::mutex> lk;
-    if (int rc = lock_idle(e, lk)) return rc;
-    if (int rc = validate_ready(e, n)) return rc;
+    Entry guard(e, Needs::ready, n);
+    if (guard.rc) return guard.rc;
     if (n == 0) return ISL_OK;
-    DeviceGuard guard(e->device);
     return place_batch_locked(e, n, in, out);
 }
 
 int isl_place_batch_range(isl_engine* e, uint32_t lo, uint32_t hi, uint32_t n, const isl_request* in, isl_result* out) {
     if (!e || (n && (!in || !out))) return ISL_EINVAL;
-    std::unique_lock<std::mutex> lk;                // restriction, placement and restore under ONE lock: two callers cannot interleave
-    if (int rc = lock_idle(e, lk)) return rc;
-    if (int rc = validate_ready(e, n)) return rc;
+    Entry guard(e, Needs::ready, n);                // restriction, placement and restore under ONE lock: two callers cannot interleave
+    if (guard.rc) return guard.rc;
     if (lo > hi || hi > e->G) return ISL_EINVAL;
     if (n == 0) return ISL_OK;
-    DeviceGuard guard(e->device);
     const uint32_t lo0 = e->lo, hi0 = e->hi;
     if (e->prof.flip) { e->lo = e->G - hi; e->hi = e->G - lo; } else { e->lo = lo; e->hi = hi; }
     const int rc = place_batch_locked(e, n, in, out);
@@ -1246,11 +1252,9 @@ int isl_place_gangs(isl_engine* e, uint32_t n_gangs, const uint32_t* gang_off, c
     if (n && (!in || !out)) return ISL_EINVAL;
     if (e->cfg.flags & ISL_FLAG_ALL_NODES) return ISL_EINVAL;      // one pod on every node with capacity: no all-or-nothing meaning
     if (n > e->cfg.max_batch) return ISL_ERANGE;
-    std::unique_lock<std::mutex> lk;
-    if (int rc = lock_idle(e, lk)) return rc;
-    if (int rc = validate_ready(e, n)) return rc;
+    Entry guard(e, Needs::ready, n);
+    if (guard.rc) return guard.rc;
     if (n == 0) return ISL_OK;
-    DeviceGuard guard(e->device);
     if (e->hi == e->lo || e->hi - e->lo > kBfMaxGpus) return ISL_ERANGE;          // the class bitmaps of k_bestfit
     ISL_CUDA(e, e->d_scratch.reserve(((size_t)n_gangs + 1) * sizeof(uint32_t)));
     uint32_t* d_gang_off = reinterpret_cast<uint32_t*>(e->d_scratch.get());
@@ -1268,13 +1272,11 @@ int isl_preempt(isl_engine* e, uint32_t n, const isl_request* in, const uint8_t*
     if (e->cfg.flags & ISL_FLAG_ALL_NODES) return ISL_EINVAL;      // one pod on every node with capacity: no single GPU to evict on
     for (uint32_t i = 0; i < n; ++i) if (in[i].op == ISL_OP_FREE) return ISL_EINVAL;      // releases are expressed by the victim list
     if (n > e->cfg.max_batch || (uint64_t)n_victims > (uint64_t)ISL_SLOTS * e->cfg.max_gpus) return ISL_ERANGE;
-    std::unique_lock<std::mutex> lk;
-    if (int rc = lock_idle(e, lk)) return rc;
-    if (int rc = validate_ready(e, n)) return rc;
+    Entry guard(e, Needs::ready, n);
+    if (guard.rc) return guard.rc;
     if (n == 0) return ISL_OK;
     const uint32_t Gr = e->hi - e->lo;
     if (Gr == 0 || Gr > kPreMaxGpus) return ISL_ERANGE;
-    DeviceGuard guard(e->device);
     // one CTA per SM at most (the grid-wide exchange per preemptor is cheaper with fewer CTAs), at least one thread per GPU below that
     int sms = 0, per_sm = 0;
     ISL_CUDA(e, cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, e->device));
@@ -1384,11 +1386,9 @@ static int place_batch_plain(isl_engine* e, uint32_t n, const isl_request* in, i
 int isl_place_stream(isl_engine* e, uint32_t n_batches, const uint32_t* sizes, const isl_request* in, isl_result* out) {
     uint64_t total;
     if (int rc = stream_entry(e, n_batches, sizes, in && out, &total)) return rc;
-    std::unique_lock<std::mutex> lk;
-    if (int rc = lock_idle(e, lk)) return rc;
-    if (int rc = validate_ready(e, (uint32_t)total)) return rc;
+    Entry guard(e, Needs::ready, total);
+    if (guard.rc) return guard.rc;
     if (total == 0) return ISL_OK;
-    DeviceGuard guard(e->device);
     if (int rc = run_stream(e, n_batches, sizes, e->d_req, e->d_res, nullptr, nullptr, 0, reinterpret_cast<const uint2*>(in), reinterpret_cast<uint2*>(out))) {
         if (e->feed_stream) cudaStreamSynchronize(e->feed_stream);
         return rc;
@@ -1402,18 +1402,15 @@ int isl_place_stream_device(isl_engine* e, uint32_t n_batches, const uint32_t* s
     if (!d_in || !d_out) return ISL_EINVAL;
     uint64_t total;
     if (int rc = stream_entry(e, n_batches, sizes, true, &total)) return rc;
-    std::unique_lock<std::mutex> lk;
-    if (int rc = lock_idle(e, lk)) return rc;
-    if (int rc = validate_ready(e, (uint32_t)total)) return rc;
-    DeviceGuard guard(e->device);
+    Entry guard(e, Needs::ready, total);
+    if (guard.rc) return guard.rc;
     return run_stream(e, n_batches, sizes, static_cast<const uint2*>(d_in), static_cast<uint2*>(d_out), nullptr, nullptr);
 }
 
 int isl_ipc_inbox_handle(isl_engine* e, void* handle64) {
     if (!e || !handle64) return ISL_EINVAL;
-    std::unique_lock<std::mutex> lk;
-    if (int rc = lock_idle(e, lk)) return rc;
-    DeviceGuard guard(e->device);
+    Entry guard(e, Needs::nothing);
+    if (guard.rc) return guard.rc;
     bool fresh;
     ISL_CUDA(e, e->d_inbox.reserve(kMaxStreamChunks, Growth::exact, &fresh));
     if (fresh) ISL_CUDA(e, cudaMemset(e->d_inbox, 0, e->d_inbox.bytes()));
@@ -1422,9 +1419,8 @@ int isl_ipc_inbox_handle(isl_engine* e, void* handle64) {
 
 int isl_ipc_connect(isl_engine* e, const void* next_handle64, int has_prev) {
     if (!e) return ISL_EINVAL;
-    std::unique_lock<std::mutex> lk;
-    if (int rc = lock_idle(e, lk)) return rc;
-    DeviceGuard guard(e->device);
+    Entry guard(e, Needs::nothing);
+    if (guard.rc) return guard.rc;
     e->d_outbox.reset();
     if (next_handle64) if (int rc = ipc_open(e, next_handle64, e->d_outbox.out())) return rc;
     e->has_prev = has_prev != 0;
@@ -1434,8 +1430,8 @@ int isl_ipc_connect(isl_engine* e, const void* next_handle64, int has_prev) {
 
 int isl_connect_local(isl_engine* e, isl_engine* next, int has_prev) {
     if (!e) return ISL_EINVAL;
-    std::unique_lock<std::mutex> lk;
-    if (int rc = lock_idle(e, lk)) return rc;
+    Entry guard(e, Needs::nothing);
+    if (guard.rc) return guard.rc;
     e->d_outbox.reset();
     if (next) {
         if (!next->d_inbox) return ISL_ESTATE;
@@ -1449,9 +1445,8 @@ int isl_connect_local(isl_engine* e, isl_engine* next, int has_prev) {
 // ---- speculative rounds over a partitioned inventory: every rank's record memory mapped into every other rank ------------------------
 int isl_ipc_spec_handle(isl_engine* e, void* handle64) {
     if (!e || !handle64) return ISL_EINVAL;
-    std::unique_lock<std::mutex> lk;
-    if (int rc = lock_idle(e, lk)) return rc;
-    DeviceGuard guard(e->device);
+    Entry guard(e, Needs::nothing);
+    if (guard.rc) return guard.rc;
     if (int rc = spec_shared_alloc(e)) return rc;
     return ipc_export(e, e->d_spec, handle64);
 }
@@ -1460,9 +1455,8 @@ int isl_ipc_spec_handle(isl_engine* e, void* handle64) {
 // [bounds[r], bounds[r + 1]).  world = 0 disconnects.
 int isl_ipc_connect_spec(isl_engine* e, uint32_t world, uint32_t rank, const void* handles, const uint32_t* bounds) {
     if (!e) return ISL_EINVAL;
-    std::unique_lock<std::mutex> lk;
-    if (int rc = lock_idle(e, lk)) return rc;
-    DeviceGuard guard(e->device);
+    Entry guard(e, Needs::nothing);
+    if (guard.rc) return guard.rc;
     spec_disconnect(e);
     if (world == 0) return ISL_OK;
     if (world < 2 || world > 8 || rank >= world || !handles || !bounds) return ISL_EINVAL;
@@ -1479,9 +1473,8 @@ int isl_ipc_connect_spec(isl_engine* e, uint32_t world, uint32_t rank, const voi
 // same-process engines (tests: several ranks on one GPU)
 int isl_connect_spec_local(isl_engine* e, uint32_t world, uint32_t rank, isl_engine* const* engines, const uint32_t* bounds) {
     if (!e) return ISL_EINVAL;
-    std::unique_lock<std::mutex> lk;
-    if (int rc = lock_idle(e, lk)) return rc;
-    DeviceGuard guard(e->device);
+    Entry guard(e, Needs::nothing);
+    if (guard.rc) return guard.rc;
     spec_disconnect(e);
     if (world == 0) return ISL_OK;
     if (world < 2 || world > 8 || rank >= world || !engines || !bounds) return ISL_EINVAL;
@@ -1499,37 +1492,30 @@ int isl_place_stream_partitioned(isl_engine* e, uint32_t n_batches, const uint32
     if (!d_in || !d_out || stream_id == 0) return ISL_EINVAL;
     uint64_t total;
     if (int rc = stream_entry(e, n_batches, sizes, true, &total)) return rc;
-    std::unique_lock<std::mutex> lk;
-    if (int rc = lock_idle(e, lk)) return rc;
-    if (int rc = validate_ready(e, (uint32_t)total)) return rc;
-    DeviceGuard guard(e->device);
+    Entry guard(e, Needs::ready, total);
+    if (guard.rc) return guard.rc;
     return run_stream(e, n_batches, sizes, static_cast<const uint2*>(d_in), static_cast<uint2*>(d_out), nullptr, nullptr, stream_id);
 }
 
 int isl_place_batch_device(isl_engine* e, uint32_t n, const void* d_in, void* d_out) {
     if (!e || (n && (!d_in || !d_out))) return ISL_EINVAL;
-    std::unique_lock<std::mutex> lk;
-    if (int rc = lock_idle(e, lk)) return rc;
-    if (int rc = validate_ready(e, n)) return rc;
-    DeviceGuard guard(e->device);
+    Entry guard(e, Needs::ready, n);
+    if (guard.rc) return guard.rc;
     return run_stream(e, 1, &n, static_cast<const uint2*>(d_in), static_cast<uint2*>(d_out), nullptr, nullptr);
 }
 
 int isl_place_batch_partitioned(isl_engine* e, uint32_t n, const void* d_in, void* d_out, const void* d_heads_in, void* d_heads_out) {
     if (!e || (n && (!d_in || !d_out)) || !d_heads_out) return ISL_EINVAL;
-    std::unique_lock<std::mutex> lk;
-    if (int rc = lock_idle(e, lk)) return rc;
-    if (int rc = validate_ready(e, n)) return rc;
-    DeviceGuard guard(e->device);
+    Entry guard(e, Needs::ready, n);
+    if (guard.rc) return guard.rc;
     return run_stream(e, 1, &n, static_cast<const uint2*>(d_in), static_cast<uint2*>(d_out), static_cast<const uint32_t*>(d_heads_in),
                       static_cast<uint32_t*>(d_heads_out));
 }
 
 int isl_set_partition(isl_engine* e, uint32_t lo, uint32_t hi) {
     if (!e) return ISL_EINVAL;
-    std::unique_lock<std::mutex> lk;
-    if (int rc = lock_idle(e, lk)) return rc;
-    if (!e->have_inventory) return ISL_ESTATE;
+    Entry guard(e, Needs::inventory);
+    if (guard.rc) return guard.rc;
     if (lo > hi || hi > e->G) return ISL_EINVAL;
     if (e->prof.flip) { e->lo = e->G - hi; e->hi = e->G - lo; } else { e->lo = lo; e->hi = hi; }
     return ISL_OK;
@@ -1539,11 +1525,9 @@ void* isl_device_occupancy(isl_engine* e) { return e ? e->d_occ.get() : nullptr;
 
 int isl_free_batch(isl_engine* e, uint32_t n, const isl_span* spans) {
     if (!e || (n && !spans)) return ISL_EINVAL;
-    std::unique_lock<std::mutex> lk;
-    if (int rc = lock_idle(e, lk)) return rc;
-    if (!e->have_inventory) return ISL_ESTATE;
+    Entry guard(e, Needs::inventory);
+    if (guard.rc) return guard.rc;
     if (n == 0) return ISL_OK;
-    DeviceGuard guard(e->device);
     ISL_CUDA(e, e->d_scratch.reserve((size_t)n * sizeof(isl_span)));
     ISL_CUDA(e, cudaMemcpyAsync(e->d_scratch, spans, (size_t)n * sizeof(isl_span), cudaMemcpyHostToDevice, e->stream));
     k_free_spans<<<ceil_div(n, 256), 256, 0, e->stream>>>(n, reinterpret_cast<const isl_span*>(e->d_scratch.get()), reinterpret_cast<uint32_t*>(e->d_occ.get()),
@@ -1555,14 +1539,12 @@ int isl_free_batch(isl_engine* e, uint32_t n, const isl_span* spans) {
 
 int isl_eval_starts(isl_engine* e, uint32_t profile, uint32_t n, const uint8_t* occ, uint8_t* out) {
     if (!e || (n && (!occ || !out))) return ISL_EINVAL;
-    std::unique_lock<std::mutex> lk;
-    if (int rc = lock_idle(e, lk)) return rc;
-    if (!e->have_profiles) return ISL_ESTATE;
+    Entry guard(e, Needs::profiles);
+    if (guard.rc) return guard.rc;
     const uint32_t table = profile >> 8;
     profile &= 0xFFu;
     if (profile >= e->prof.n || table >= e->n_tables) return ISL_EINVAL;
     if (n == 0) return ISL_OK;
-    DeviceGuard guard(e->device);
     ISL_CUDA(e, e->d_scratch.reserve((size_t)n * 2));
     ISL_CUDA(e, cudaMemcpyAsync(e->d_scratch, occ, n, cudaMemcpyHostToDevice, e->stream));
     k_eval_starts<<<std::min(ceil_div(n, 256), 1184u), 256, 0, e->stream>>>(e->d_lut + (size_t)table * ISL_MAX_PROFILES * 256, profile, n, e->d_scratch, e->d_scratch + n);
@@ -1574,9 +1556,8 @@ int isl_eval_starts(isl_engine* e, uint32_t profile, uint32_t n, const uint8_t* 
 
 int isl_read_trace(isl_engine* e, uint64_t* out, uint32_t max_words, uint32_t* n_chunks, uint32_t* n_seg) {
     if (!e || !n_chunks || !n_seg) return ISL_EINVAL;
-    std::unique_lock<std::mutex> lk;
-    if (int rc = lock_idle(e, lk)) return rc;
-    DeviceGuard guard(e->device);
+    Entry guard(e, Needs::nothing);
+    if (guard.rc) return guard.rc;
     *n_chunks = e->trace_chunks; *n_seg = e->trace_seg;
     const size_t words = (size_t)e->trace_chunks * e->trace_seg * kTraceWords;
     if (!out || words == 0) return ISL_OK;
@@ -1588,9 +1569,8 @@ int isl_read_trace(isl_engine* e, uint64_t* out, uint32_t max_words, uint32_t* n
 
 int isl_get_stats(isl_engine* e, isl_stats* out) {
     if (!e || !out) return ISL_EINVAL;
-    std::unique_lock<std::mutex> lk;
-    if (int rc = lock_idle(e, lk)) return rc;
-    DeviceGuard guard(e->device);
+    Entry guard(e, Needs::nothing);
+    if (guard.rc) return guard.rc;
     Ctrl c;
     ISL_CUDA(e, cudaMemcpyAsync(&c, e->d_ctrl, sizeof(Ctrl), cudaMemcpyDeviceToHost, e->stream));
     ISL_CUDA(e, cudaStreamSynchronize(e->stream));
@@ -1602,9 +1582,8 @@ int isl_get_stats(isl_engine* e, isl_stats* out) {
 
 int isl_reset_stats(isl_engine* e) {
     if (!e) return ISL_EINVAL;
-    std::unique_lock<std::mutex> lk;
-    if (int rc = lock_idle(e, lk)) return rc;
-    DeviceGuard guard(e->device);
+    Entry guard(e, Needs::nothing);
+    if (guard.rc) return guard.rc;
     const uint64_t launches = e->st.kernel_launches;
     e->st = isl_stats{};
     e->st.kernel_launches = launches;      // launches are counted since creation
@@ -1629,19 +1608,15 @@ static int capacity_locked(isl_engine* e, uint64_t* cap) {
 
 int isl_capacity(isl_engine* e, uint64_t* cap) {
     if (!e || !cap) return ISL_EINVAL;
-    std::unique_lock<std::mutex> lk;
-    if (int rc = lock_idle(e, lk)) return rc;
-    if (int rc = validate_ready(e, 0)) return rc;
-    DeviceGuard guard(e->device);
+    Entry guard(e, Needs::ready);
+    if (guard.rc) return guard.rc;
     return capacity_locked(e, cap);
 }
 
 int isl_what_if(isl_engine* e, uint32_t n, const isl_request* plan, isl_result* out, uint64_t* cap_before, uint64_t* cap_after) {
     if (!e || (n && (!plan || !out))) return ISL_EINVAL;
-    std::unique_lock<std::mutex> lk;                // snapshot, plan, measurement and restore under ONE lock: nobody sees the hypothetical state
-    if (int rc = lock_idle(e, lk)) return rc;
-    if (int rc = validate_ready(e, n)) return rc;
-    DeviceGuard guard(e->device);
+    Entry guard(e, Needs::ready, n);                // snapshot, plan, measurement and restore under ONE lock: nobody sees the hypothetical state
+    if (guard.rc) return guard.rc;
     if (int rc = snapshot_occ(e)) return rc;
     int rc = ISL_OK;
     if (cap_before) rc = capacity_locked(e, cap_before);
@@ -1658,8 +1633,8 @@ int isl_what_if(isl_engine* e, uint32_t n, const isl_request* plan, isl_result* 
 // ---- causal window / pinned buffers / owner-gathered results --------------------------------------------------------------
 int isl_set_causal_window(isl_engine* e, uint32_t window) {
     if (!e) return ISL_EINVAL;
-    std::unique_lock<std::mutex> lk;
-    if (int rc = lock_idle(e, lk)) return rc;
+    Entry guard(e, Needs::nothing);
+    if (guard.rc) return guard.rc;
     e->window = window;
     return ISL_OK;
 }
@@ -1667,9 +1642,8 @@ int isl_set_causal_window(isl_engine* e, uint32_t window) {
 // debugging aid (not part of the boundary): the per-round stamps recorded under ISL_SPEC_DBG=chunk,stage; out: kSpecRounds x 8 uint64
 int isl_debug_spec_rounds(isl_engine* e, uint64_t* out, uint32_t max_words) {
     if (!e || !out || !e->d_specdbg) return ISL_EINVAL;
-    std::unique_lock<std::mutex> lk;
-    if (int rc = lock_idle(e, lk)) return rc;
-    DeviceGuard guard(e->device);
+    Entry guard(e, Needs::nothing);
+    if (guard.rc) return guard.rc;
     ISL_CUDA(e, cudaStreamSynchronize(e->stream));
     ISL_CUDA(e, cudaMemcpy(out, e->d_specdbg, std::min<size_t>(max_words, kSpecRounds * 8) * sizeof(uint64_t), cudaMemcpyDeviceToHost));
     return ISL_OK;
@@ -1677,16 +1651,16 @@ int isl_debug_spec_rounds(isl_engine* e, uint64_t* out, uint32_t max_words) {
 
 int isl_set_speculation(isl_engine* e, uint32_t mode) {
     if (!e || mode > ISL_SPEC_ON) return ISL_EINVAL;
-    std::unique_lock<std::mutex> lk;
-    if (int rc = lock_idle(e, lk)) return rc;
+    Entry guard(e, Needs::nothing);
+    if (guard.rc) return guard.rc;
     e->spec_mode = mode;
     return ISL_OK;
 }
 
 int isl_set_ring_world(isl_engine* e, uint32_t world) {
     if (!e) return ISL_EINVAL;
-    std::unique_lock<std::mutex> lk;
-    if (int rc = lock_idle(e, lk)) return rc;
+    Entry guard(e, Needs::nothing);
+    if (guard.rc) return guard.rc;
     e->ring_world = world;
     return ISL_OK;
 }
@@ -1703,17 +1677,15 @@ void* isl_device_results(isl_engine* e) { return e ? e->d_res.get() : nullptr; }
 
 int isl_ipc_results_handle(isl_engine* e, void* handle64) {
     if (!e || !handle64) return ISL_EINVAL;
-    std::unique_lock<std::mutex> lk;
-    if (int rc = lock_idle(e, lk)) return rc;
-    DeviceGuard guard(e->device);
+    Entry guard(e, Needs::nothing);
+    if (guard.rc) return guard.rc;
     return ipc_export(e, e->d_res, handle64);
 }
 
 int isl_ipc_connect_owner(isl_engine* e, const void* owner_handle64) {
     if (!e) return ISL_EINVAL;
-    std::unique_lock<std::mutex> lk;
-    if (int rc = lock_idle(e, lk)) return rc;
-    DeviceGuard guard(e->device);
+    Entry guard(e, Needs::nothing);
+    if (guard.rc) return guard.rc;
     e->d_owner_out.reset();
     if (owner_handle64) return ipc_open(e, owner_handle64, e->d_owner_out.out());
     return ISL_OK;
@@ -1721,8 +1693,8 @@ int isl_ipc_connect_owner(isl_engine* e, const void* owner_handle64) {
 
 int isl_connect_owner_local(isl_engine* e, isl_engine* owner) {
     if (!e) return ISL_EINVAL;
-    std::unique_lock<std::mutex> lk;
-    if (int rc = lock_idle(e, lk)) return rc;
+    Entry guard(e, Needs::nothing);
+    if (guard.rc) return guard.rc;
     e->d_owner_out.borrow(owner ? owner->d_res.get() : nullptr);
     return ISL_OK;
 }
@@ -1733,9 +1705,8 @@ int isl_connect_owner_local(isl_engine* e, isl_engine* owner) {
 // isl_stream_wait returns as soon as that word is up — the caller composes batch b+1 (or b+k) from results it has already seen.
 int isl_stream_open(isl_engine* e, uint32_t max_batches) {
     if (!e || max_batches == 0 || max_batches > kMaxStreamChunks) return ISL_EINVAL;
-    std::unique_lock<std::mutex> lk;
-    if (int rc = lock_idle(e, lk)) return rc;
-    if (int rc = validate_ready(e, 0)) return rc;
+    Entry guard(e, Needs::ready);
+    if (guard.rc) return guard.rc;
     if (bestfit_family(e->cfg.policy)) return ISL_EINVAL;
     // a tool that serialises kernels would starve a resident kernel that waits for kernels launched after it: refuse instead of hanging
     // until the device-side trap (callers fall back to isl_place_batch per batch)
@@ -1743,7 +1714,6 @@ int isl_stream_open(isl_engine* e, uint32_t max_batches) {
         snprintf(e->cuda_err, sizeof(e->cuda_err), "isl_stream_open: kernel-serialising tool or ISL_NO_FEED set; open streams need concurrent kernels");
         return ISL_ESTATE;
     }
-    DeviceGuard guard(e->device);
     auto& o = e->open;
     const uint32_t pc = e->pipe_chunk;
     if ((uint64_t)max_batches * pc > e->cfg.max_batch) return ISL_ERANGE;       // every batch owns a slot of the staging buffers
@@ -1776,9 +1746,8 @@ int isl_stream_open(isl_engine* e, uint32_t max_batches) {
 
 int isl_stream_submit(isl_engine* e, uint32_t n, const isl_request* in, isl_result* out, uint32_t* ticket) {
     if (!e || n == 0 || !in || !out) return ISL_EINVAL;
-    std::lock_guard<std::mutex> lk(e->mu);
-    if (!e->open.active) return ISL_ESTATE;
-    DeviceGuard guard(e->device);
+    Entry guard(e, Needs::open_stream);
+    if (guard.rc) return guard.rc;
     auto& o = e->open;
     if (o.submitted >= o.max_batches || n > e->pipe_chunk) return ISL_ERANGE;
     // the results are written by the running kernel: the destination must be mapped pinned host memory (isl_host_alloc, cudaHostAlloc,
@@ -1841,9 +1810,8 @@ int isl_stream_wait(isl_engine* e, uint32_t ticket) {
 
 int isl_stream_close(isl_engine* e) {
     if (!e) return ISL_EINVAL;
-    std::lock_guard<std::mutex> lk(e->mu);
-    if (!e->open.active) return ISL_ESTATE;
-    DeviceGuard guard(e->device);
+    Entry guard(e, Needs::open_stream);
+    if (guard.rc) return guard.rc;
     auto& o = e->open;
     int rc = ISL_OK;
     if (o.launched) {

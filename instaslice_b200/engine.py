@@ -96,6 +96,7 @@ SIGNATURES = {
     "isl_abi_version": (C.c_uint32, []),
     "isl_place_batch_range": (C.c_int, [_P, C.c_uint32, C.c_uint32, C.c_uint32, _P, _P]),
     "isl_place_gangs": (C.c_int, [_P, C.c_uint32, _P, _P, _P]),
+    "isl_preempt": (C.c_int, [_P, C.c_uint32, _P, _P, C.c_uint32, _P, _P, _P]),
     "isl_stream_open": (C.c_int, [_P, C.c_uint32]),
     "isl_stream_submit": (C.c_int, [_P, C.c_uint32, _P, _P, C.POINTER(C.c_uint32)]),
     "isl_stream_wait": (C.c_int, [_P, C.c_uint32]),
@@ -115,14 +116,6 @@ SIGNATURES = {
     "isl_capacity": (C.c_int, [_P, _P]),
     "isl_what_if": (C.c_int, [_P, C.c_uint32, _P, _P, _P, _P]),
 }
-# isl_preempt is bound from a table of its own: the return code of every entry point above in every engine state is classified by the
-# test suite's per-state contract, which also probes each of them; isl_preempt's codes in the same states (created, profiles only,
-# inventory only, ready, empty partition, the three sub-states of an open stream, ISL_FLAG_ALL_NODES) are pinned by
-# tests/test_gpu_preempt.py::test_return_code_in_every_engine_state
-PREEMPT_SIGNATURES = {
-    "isl_preempt": (C.c_int, [_P, C.c_uint32, _P, _P, C.c_uint32, _P, _P, _P]),
-}
-EXPORTED_SYMBOLS = list(SIGNATURES) + list(PREEMPT_SIGNATURES)
 
 _lib = None
 
@@ -135,7 +128,7 @@ def load_library(path: str = LIB_PATH):
     if not os.path.exists(path):
         raise ImportError(f"{path} not built: run __graft_entry__.build() (nvcc, sm_90a). There is no CPU fallback.")
     lib = C.CDLL(path)
-    for name, (res, args) in {**SIGNATURES, **PREEMPT_SIGNATURES}.items():
+    for name, (res, args) in SIGNATURES.items():
         try:
             fn = getattr(lib, name)
         except AttributeError:

@@ -62,10 +62,12 @@ _INV = _row(_ES, _ES, _OK, _OK)                       # needs an inventory
 _READY = _row(_ES, _ES, _ES, _OK)                     # needs profiles and an inventory
 
 
-def _gangs(state):
+def _one_pass_in_partition(state):
+    """isl_place_gangs and isl_preempt: a call over the partition, refused on an empty one; a pod on every node (ISL_FLAG_ALL_NODES)
+    has no all-or-nothing or eviction meaning."""
     def code(c):
         if c.flags & E.FLAG_ALL_NODES:
-            return E.EINVAL                          # checked before the state: no all-or-nothing meaning on every node
+            return E.EINVAL                          # checked before the state
         if state != "ready":
             return _ES
         return E.ERANGE if c.empty_partition else _OK
@@ -92,7 +94,8 @@ CODES = {
     "isl_place_stream": _READY,
     "isl_place_stream_device": _READY,
     "isl_place_batch_range": _READY,
-    "isl_place_gangs": {s: _gangs(s) for s in ALL_STATES},
+    "isl_place_gangs": {s: _one_pass_in_partition(s) for s in ALL_STATES},
+    "isl_preempt": {s: _one_pass_in_partition(s) for s in ALL_STATES},
     "isl_free_batch": _INV,
     "isl_eval_starts": _row(_ES, _OK, _ES, _OK),
     "isl_set_partition": _INV,

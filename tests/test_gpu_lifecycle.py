@@ -79,6 +79,7 @@ class Probe:
         self.d_heads = torch.zeros(16 * 4, dtype=torch.uint8, device="cuda")
         self.sizes = np.array([self.N], dtype=np.uint32)
         self.gang_off = np.array([0, self.N], dtype=np.uint32)
+        self.prio, self.evict = np.full(self.N, 3, dtype=np.uint8), np.zeros((self.N, 8), dtype=np.uint32)
         self.cap = np.zeros(E.MAX_PROFILES, dtype=np.uint64)
         self.cap2 = np.zeros(E.MAX_PROFILES, dtype=np.uint64)
         self.h64 = C.create_string_buffer(64)
@@ -127,6 +128,7 @@ class Probe:
             "isl_place_stream_device": lambda: L.isl_place_stream_device(h, 1, p(self.sizes), d_in, d_out),
             "isl_place_batch_range": lambda: L.isl_place_batch_range(h, 0, m.G, self.N, p(self.req), p(self.out)),
             "isl_place_gangs": lambda: L.isl_place_gangs(h, 1, p(self.gang_off), p(self.req), p(self.out)),
+            "isl_preempt": lambda: L.isl_preempt(h, self.N, p(self.req), p(self.prio), 0, None, p(self.out), p(self.evict)),
             "isl_free_batch": lambda: L.isl_free_batch(h, 1, p(self.span)),
             "isl_eval_starts": lambda: L.isl_eval_starts(h, 0, 4, p(self.bytes), p(np.zeros(4, dtype=np.uint8))),
             "isl_set_partition": lambda: L.isl_set_partition(h, 0, m.G),

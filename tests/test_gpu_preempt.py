@@ -1,7 +1,6 @@
 """Priority preemption (isl_preempt) on the H100: k_victim_map + k_preempt against the brute-force restatement of tests/preempt_fast.cpp,
 records and evict rows byte-identical; the known answers; the query leaves every piece of engine state as it found it; every error code
 of rules 2, 3 and 6; and the preempt -> release -> place flow through the controller."""
-import ctypes as C
 import random
 
 import numpy as np
@@ -287,67 +286,3 @@ def test_host_mirror_preempt_selftest(tmp_path):
                     "-L" + pkg, "-l:libislhost.so", "-l:libislplace.so", "-Wl,-rpath," + pkg], check=True)
     out = subprocess.run([exe], capture_output=True, text=True)
     assert out.returncode == 0 and "PASS" in out.stdout, out.stdout + out.stderr
-
-
-def preempt_code(eng):
-    """isl_preempt's return code for a well-formed call of 8 ALLOCs."""
-    req = np.zeros(8, dtype=E.REQUEST_DTYPE)
-    p = lambda a: a.ctypes.data_as(C.c_void_p)                               # noqa: E731
-    prio, out, ev = np.full(8, 3, np.uint8), np.zeros(8, dtype=E.RESULT_DTYPE), np.zeros((8, 8), dtype=np.uint32)
-    return eng._lib.isl_preempt(eng._h, 8, p(req), p(prio), 0, None, p(out), p(ev))
-
-
-@pytest.mark.parametrize("policy,flags", [(E.POLICY_FIRST_FIT, 0), (E.POLICY_RIGHT_TO_LEFT, 0), (E.POLICY_BEST_FIT, 0),
-                                          (E.POLICY_FIRST_FIT, E.FLAG_ALL_NODES)])
-def test_return_code_in_every_engine_state(policy, flags):
-    """Created, profiles only, inventory only: ESTATE; ready: OK; an empty partition: ERANGE; each sub-state of an open stream (opened,
-    partly fed, fully fed): ESTATE; an engine created with ISL_FLAG_ALL_NODES: EINVAL in every state.  A refused call changes nothing."""
-    G = 300
-    node_off = np.array([0, 100, 180, 300], dtype=np.uint32)
-    rng = np.random.default_rng(policy + flags)
-    occ = (rng.integers(0, 256, G) & rng.integers(0, 256, G) & 0x7F).astype(np.uint8)
-    rows = E.make_profiles(tables.H100_80GB)
-    refused = E.EINVAL if flags & E.FLAG_ALL_NODES else E.ESTATE
-
-    def fresh(profiles, inventory):
-        eng = E.Engine(max_gpus=4096, max_batch=3 * 65536, policy=policy, flags=flags)
-        if profiles:
-            eng.load_profiles(rows)
-        if inventory:
-            eng.load_inventory(node_off, occ)
-        return eng
-
-    for profiles, inventory in ((False, False), (True, False), (False, True)):
-        eng = fresh(profiles, inventory)
-        assert preempt_code(eng) == refused, (profiles, inventory)
-        if inventory:
-            assert np.array_equal(eng.read_occupancy(), occ)
-        eng.close()
-    eng = fresh(True, True)
-    assert preempt_code(eng) == (E.EINVAL if flags & E.FLAG_ALL_NODES else E.OK)
-    eng.set_partition(120, 120)
-    assert preempt_code(eng) == (E.EINVAL if flags & E.FLAG_ALL_NODES else E.ERANGE)
-    eng.set_partition(0, G)
-    assert np.array_equal(eng.read_occupancy(), occ)
-    if policy == E.POLICY_BEST_FIT:                      # the best-fit family opens no streams
-        eng.close()
-        return
-    # open stream: opened (nothing submitted), partly fed, fully fed and drained
-    n, mb = 200, 3
-    h_in, h_out = E.PinnedArray(mb * n, E.REQUEST_DTYPE), E.PinnedArray(mb * n, E.RESULT_DTYPE)
-    h_in.array[:] = np.zeros(mb * n, dtype=E.REQUEST_DTYPE)
-    h_in.array["profile"] = rng.integers(0, len(rows), mb * n)
-    eng.stream_open(mb)
-    try:
-        assert preempt_code(eng) == refused, "opened"
-        for b in range(mb):
-            t = eng.stream_submit_ptr(n, h_in.ptr + 8 * b * n, h_out.ptr + 8 * b * n)
-            eng.stream_wait(t)
-            assert preempt_code(eng) == refused, ("fed", b)
-    finally:
-        eng.stream_close()
-    after_stream = eng.read_occupancy()
-    assert preempt_code(eng) == (E.EINVAL if flags & E.FLAG_ALL_NODES else E.OK)
-    assert np.array_equal(eng.read_occupancy(), after_stream)
-    h_in.free(); h_out.free()
-    eng.close()
