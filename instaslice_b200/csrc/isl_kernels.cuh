@@ -73,7 +73,6 @@ struct Ctrl {                   // device-resident control block, rewritten per 
     uint32_t qcnt[ISL_MAX_PROFILES];       // requests of profile p in this chunk
     uint32_t active;                       // profiles with requests in this chunk AND >= 1 valid candidate
     uint32_t n_cand;                       // candidate GPUs found by the sweep
-    uint32_t heads_out[ISL_MAX_PROFILES];  // queue heads after the chain (token for the next rank)
     uint32_t n_log;                        // decisions logged by the chain of this chunk
     unsigned long long placed, freed, bad, steps, visited, allocs, jumps, scanned;
     unsigned long long spec_sims, spec_rounds, spec_cells;   // speculative rounds: segment simulations run (all stages), rounds until the last stage was certified summed over chunks, chunks
@@ -934,8 +933,6 @@ struct PipeArgs {
     uint2* out;
     const uint16_t* feas;
     Ctrl* stats;
-    const uint32_t* heads_in;       // [chunk][16] token entering the first segment (nullptr = zeros)
-    uint32_t* heads_out;            // [chunk][16] token leaving the last segment (may be nullptr)
     // partitioned inventory: the token crosses GPUs through peer-mapped memory (NVLink), one relaxed system-scope store per head word
     const uint32_t* inbox;          // local [chunk][kTokStride] of tagged head words, written by the previous rank's last segment (nullptr = first rank); cleared by the reader
     uint32_t* outbox;               // the next rank's inbox, peer-mapped (nullptr = last rank)
@@ -1127,14 +1124,12 @@ __device__ __forceinline__ uint32_t token_tag(const PipeArgs& a) { return a.epoc
 __device__ __forceinline__ uint32_t xtoken_tag(const PipeArgs& a) { return a.xepoch % 32767u + 1u; }
 __device__ __forceinline__ uint32_t tag_word(uint32_t tag, uint32_t h) { return (tag << 17) | h; }
 
-// Lane p < 16: head h of profile p leaves stage seg for chunk c — the word the next stage polls and, behind the last stage, the heads
-// for the caller and the word in the next rank's inbox
+// Lane p < 16: head h of profile p leaves stage seg for chunk c — the word the next stage polls and, behind the last stage, the word in
+// the next rank's inbox
 __device__ __forceinline__ void publish_token(const PipeArgs& a, uint32_t c, uint32_t seg, uint32_t lane, uint32_t h) {
-    const bool last = seg == a.n_seg - 1;
     uint32_t* tok = a.tokens + ((size_t)c * (a.n_seg + 1) + seg) * kTokStride;
-    uint32_t* peer = last && a.outbox ? a.outbox + (size_t)c * kTokStride : nullptr;
+    uint32_t* peer = seg == a.n_seg - 1 && a.outbox ? a.outbox + (size_t)c * kTokStride : nullptr;
     st_relaxed_gpu(tok + lane, tag_word(token_tag(a), h));
-    if (last && a.heads_out) a.heads_out[(size_t)c * ISL_MAX_PROFILES + lane] = h;
     if (peer) st_relaxed_sys(peer + lane, tag_word(xtoken_tag(a), h));
 }
 
@@ -1503,8 +1498,7 @@ __device__ __forceinline__ void predict_entry(const PipeArgs& a, const Stage& st
         }
         rr = __reduce_add_sync(0xFFFFFFFFu, rr);
         const uint32_t Q = min(__shfl_sync(0xFFFFFFFFu, incl, 31), totb), R = min(rr, tots);
-        uint32_t hg = lane < ISL_MAX_PROFILES && gseg == 0 && a.heads_in ? a.heads_in[(size_t)c * ISL_MAX_PROFILES + lane] : 0u;
-        if (gseg > 0) hg = shift_groups(hg, s, ss, (int)Q, (int)R, lane);
+        const uint32_t hg = gseg > 0 ? shift_groups(0u, s, ss, (int)Q, (int)R, lane) : 0u;
         if (lane < ISL_MAX_PROFILES) ss.specH[lane] = hg;
     }
     __syncthreads();
@@ -1554,7 +1548,7 @@ __device__ __forceinline__ bool read_entry(const PipeArgs& a, const Stage& st, P
                 return __all_sync(0xFFFFFFFFu, ok);
             }, a.wait_ns, 0);
             if (tid < ISL_MAX_PROFILES) st_relaxed_sys(slot, 0u);
-        } else if (tid < ISL_MAX_PROFILES) h = a.heads_in ? a.heads_in[(size_t)c * ISL_MAX_PROFILES + tid] : 0u;
+        }
         stamp_if(tr && tid == 0, tr + 1);
         const bool all_done = sb == 0 && __all_sync(0xFFFFFFFFu, from_done || tid >= ISL_MAX_PROFILES);
         if (tid < ISL_MAX_PROFILES) {
@@ -1846,10 +1840,7 @@ __device__ __forceinline__ bool exchange_round(const PipeArgs& a, uint32_t seg, 
     store_if(dbg && tid == 0, dbg + rnd * 8 + 7, s.nlog | ((unsigned long long)r.need_sim << 32));
     if (gseg > 0 && tid == 192) spec_pub_nb(a, seg, r.sm.ack + gseg, ((unsigned long long)r.tage << 32) | (certified ? 0xFFFFu : rnd), true);
     if (certified) {    // every entry up to mine was the true token one round ago and has not moved since
-        if (tid < ISL_MAX_PROFILES) {
-            spec_pub_nb(a, seg, r.sm.xf + (size_t)gseg * 16 + tid, r.tagF | (rnd << 24) | ss.specX[tid], false);
-            if (gseg == r.gtot - 1 && a.heads_out) a.heads_out[(size_t)c * ISL_MAX_PROFILES + tid] = ss.specX[tid];
-        }
+        if (tid < ISL_MAX_PROFILES) spec_pub_nb(a, seg, r.sm.xf + (size_t)gseg * 16 + tid, r.tagF | (rnd << 24) | ss.specX[tid], false);
         if (tid == 16) spec_pub_down(a, r.sm.df + gseg, r.tagF | (rnd << 24) | (ss.dqr[0] << 13) | ss.dqr[1]);
         if (tid == 0) {
             n.steps += n.spec_steps; n.visited += n.spec_visited;

@@ -12,6 +12,7 @@
 #include <mutex>
 #include <new>
 #include <optional>
+#include <tuple>
 #include <type_traits>
 #include <utility>
 #include <vector>
@@ -173,7 +174,6 @@ struct isl_engine {
         DevMem<uint8_t> stage;
         DevMem<unsigned long long> keys;
     } pre;
-    bool delivered = false;          // the last run_stream call already put the results into the caller's host buffer
     unsigned long long wait_ns = 20000000000ull;   // a starved device-side wait traps after this long (ISL_WAIT_SECONDS overrides the 20 s)
     uint32_t window = 0;             // causal window of stream calls (isl_set_causal_window): chunk c starts after chunk c - window is committed
     uint32_t spec_mode = ISL_SPEC_AUTO;     // speculative rounds (isl_set_speculation); ISL_SPEC=0|1 in the environment overrides
@@ -203,6 +203,15 @@ namespace {
 
 inline bool bestfit_family(uint32_t policy) { return policy == ISL_POLICY_BEST_FIT || policy == ISL_POLICY_MIN_FRAG; }
 inline bool reversed(const isl_engine* e) { return e->cfg.policy == ISL_POLICY_RIGHT_TO_LEFT; }
+
+// A canonical GPU range [lo, hi) in storage order (ISL_POLICY_RIGHT_TO_LEFT stores the inventory reversed), or back: its own inverse
+std::pair<uint32_t, uint32_t> storage_range(const isl_engine* e, uint32_t lo, uint32_t hi) { return e->prof.flip ? std::make_pair(e->G - hi, e->G - lo) : std::make_pair(lo, hi); }
+// Restricts e to canonical ranges (set) for one call, isl_place_batch_range or ISL_FLAG_ALL_NODES; {lo, hi} come back however it returns
+struct RangeRestriction {
+    isl_engine* e; const uint32_t lo, hi;
+    ~RangeRestriction() { e->lo = lo; e->hi = hi; }
+    void set(uint32_t a, uint32_t b) { std::tie(e->lo, e->hi) = storage_range(e, a, b); }
+};
 
 #define ISL_CUDA(e, call)                                                                    \
     do {                                                                                     \
@@ -288,22 +297,8 @@ void finish_batch(isl_engine* e, uint32_t n, bool with_prepare) {
     ++e->st.batches; e->st.requests += n;
 }
 
-template <int K>
-int launch_chain(isl_engine* e, uint2* d_out_chunk, const uint32_t* d_heads_in, uint32_t* d_heads_out) {
-    const size_t smem = (size_t)kQCap * sizeof(uint16_t);      // opted in per device by isl_create
-    k_chain<K><<<1, kChainThreads, smem, e->stream>>>(e->tab, e->d_ctrl, e->d_q, e->d_cand_o16, e->d_feas, e->d_log, d_heads_in, d_heads_out);
-    if (int rc = check_launch(e, "k_chain")) return rc;
-    k_commit<<<kChunk / 256, 256, 0, e->stream>>>(e->d_ctrl, e->d_log, e->d_cand, reinterpret_cast<uint32_t*>(e->d_occ.get()), d_out_chunk, e->prof.flip);
-    return check_launch(e, "k_commit");
-}
-
-// Resolve n requests that already sit in device memory.  Enqueues only; the caller synchronises.
-// The latency path: one launch of one CTA resolves a batch of <= 1024 requests (k_small).
-bool small_eligible(const isl_engine* e, uint32_t n) {
-    return n > 0 && n <= kSmallMax && !bestfit_family(e->cfg.policy) && !(e->cfg.flags & (ISL_FLAG_NO_SMALL | ISL_FLAG_FORCE_PIPELINE)) &&
-           e->hi > e->lo && e->hi - e->lo <= (1u << 18);
-}
-
+// The executors of route()'s paths.  Each enqueues only; the caller synchronises.
+// k_small: one launch of one CTA resolves a batch, from device memory or inline requests.
 int run_small(isl_engine* e, uint32_t n, const uint2* d_in, const SmallReqs* inl, uint2* d_out) {
     static const SmallReqs zero{};
     const SmallReqs& params = inl ? *inl : zero;
@@ -318,10 +313,7 @@ int run_small(isl_engine* e, uint32_t n, const uint2* d_in, const SmallReqs* inl
     return ISL_OK;
 }
 
-// The shortest path: <= kFewMax requests against <= kFewGpus GPUs (k_few).  Requests as kernel parameters, results into mapped pinned memory.
-bool few_eligible(const isl_engine* e, uint32_t n) {
-    return n <= kFewMax && small_eligible(e, n) && e->hi - (e->lo & ~15u) <= kFewGpus && !getenv("ISL_NO_FEW");
-}
+// k_few: the shortest path, requests as kernel parameters.
 int run_few(isl_engine* e, uint32_t n, const SmallReqs& inl, uint2* d_out) {
     const bool timing = e->cfg.flags & ISL_FLAG_TIMING;
     if (timing) cudaEventRecord(e->ev[0], e->stream);
@@ -382,9 +374,10 @@ int run_gangs(isl_engine* e, uint32_t n_gangs, const uint32_t* d_gang_off, uint3
     return ISL_OK;
 }
 
-int run_batch(isl_engine* e, uint32_t n, const uint2* d_in, uint2* d_out, const uint32_t* d_heads_in, uint32_t* d_heads_out) {
+// The chunk path: k_prepare, then per chunk of kChunk requests k_partition, the two sweeps, k_chain and k_commit.  d_heads_in / d_heads_out
+// (isl_place_batch_partitioned): the queue-head token per chunk, carried by the caller from the engine of the previous GPU range.
+int run_chunks(isl_engine* e, uint32_t n, const uint2* d_in, uint2* d_out, const uint32_t* d_heads_in, uint32_t* d_heads_out) {
     if (n == 0) return ISL_OK;
-    if (bestfit_family(e->cfg.policy)) return run_bestfit(e, n, d_in, d_out);
     const bool timing = e->cfg.flags & ISL_FLAG_TIMING;
     const uint32_t tiles = ceil_div(n, kTile);
     if (timing) cudaEventRecord(e->ev[0], e->stream);
@@ -403,7 +396,6 @@ int run_batch(isl_engine* e, uint32_t n, const uint2* d_in, uint2* d_out, const 
                                                              n_tiles, e->cand_profiles, e->d_q, e->d_ctrl, nullptr, 0, 0);
         if (int rc = check_launch(e, "k_partition")) return rc;
         if (timing) cudaEventRecord(e->ev[3], e->stream);
-        // the heads token of a chunk: first chunk of a partitioned call chains from the previous rank
         const uint32_t* h_in = d_heads_in ? d_heads_in + (size_t)(c0 / kChunk) * ISL_MAX_PROFILES : nullptr;
         uint32_t* h_out = d_heads_out ? d_heads_out + (size_t)(c0 / kChunk) * ISL_MAX_PROFILES : nullptr;
         if (h_out) {
@@ -420,7 +412,13 @@ int run_batch(isl_engine* e, uint32_t n, const uint2* d_in, uint2* d_out, const 
             if (int rc = check_launch(e, "k_sweep_scatter")) return rc;
         }
         if (timing) cudaEventRecord(e->ev[4], e->stream);
-        if (int rc = with_cand_slots(e, [&](auto k) { return launch_chain<decltype(k)::value>(e, d_out + c0, h_in, h_out); })) return rc;
+        with_cand_slots(e, [&](auto k) {      // dynamic shared memory opted in per device by isl_create
+            k_chain<decltype(k)::value><<<1, kChainThreads, (size_t)kQCap * sizeof(uint16_t), e->stream>>>(e->tab, e->d_ctrl, e->d_q, e->d_cand_o16, e->d_feas,
+                                                                                                    e->d_log, h_in, h_out);
+        });
+        if (int rc = check_launch(e, "k_chain")) return rc;
+        k_commit<<<kChunk / 256, 256, 0, e->stream>>>(e->d_ctrl, e->d_log, e->d_cand, reinterpret_cast<uint32_t*>(e->d_occ.get()), d_out + c0, e->prof.flip);
+        if (int rc = check_launch(e, "k_commit")) return rc;
         if (timing) {
             cudaEventRecord(e->ev[5], e->stream);
             cudaEventSynchronize(e->ev[5]);
@@ -442,12 +440,15 @@ int run_batch(isl_engine* e, uint32_t n, const uint2* d_in, uint2* d_out, const 
 }
 
 
-// One cooperative launch of k_pipeline<K, P15, Spec>.  P15: profile index 15 is in use, the pop test needs the slower, INF-safe form.
-template <int K>
-int launch_pipeline(isl_engine* e, PipeArgs& args) {
+// One cooperative launch of k_pipeline<K, P15, Spec> for the loaded tables.  P15: profile index 15 is in use, the pop test needs the
+// slower, INF-safe form.
+int start_pipeline(isl_engine* e, PipeArgs& args) {
     const bool p15 = e->prof.n == ISL_MAX_PROFILES;
-    void* kernel = p15 ? (args.spec ? (void*)k_pipeline<K, true, true> : (void*)k_pipeline<K, true, false>)
-                       : (args.spec ? (void*)k_pipeline<K, false, true> : (void*)k_pipeline<K, false, false>);
+    void* kernel = with_cand_slots(e, [&](auto k) {
+        constexpr int K = decltype(k)::value;
+        return p15 ? (args.spec ? (void*)k_pipeline<K, true, true> : (void*)k_pipeline<K, true, false>)
+                   : (args.spec ? (void*)k_pipeline<K, false, true> : (void*)k_pipeline<K, false, false>);
+    });
     void* params[] = {&e->tab, &args};
     const cudaError_t err = cudaLaunchCooperativeKernel(kernel, dim3(args.n_seg + (args.copier ? 1u : 0u)), dim3(kPipeThreads), params, kPipeSmem, e->stream);
     if (err == cudaErrorCooperativeLaunchTooLarge || err == cudaErrorLaunchOutOfResources) {   // e.g. the GPU is shared: not all CTAs can be co-resident
@@ -457,11 +458,6 @@ int launch_pipeline(isl_engine* e, PipeArgs& args) {
     if (err != cudaSuccess) { snprintf(e->cuda_err, sizeof(e->cuda_err), "cudaLaunchCooperativeKernel: %s", cudaGetErrorString(err)); return ISL_ECUDA; }
     ++e->st.kernel_launches;
     return ISL_OK;
-}
-
-// k_pipeline for the loaded tables
-int start_pipeline(isl_engine* e, PipeArgs& args) {
-    return with_cand_slots(e, [&](auto k) { return launch_pipeline<decltype(k)::value>(e, args); });
 }
 
 int query_coresident(isl_engine* e) {
@@ -629,88 +625,89 @@ PipeArgs pipe_args(const isl_engine* e, const PipePlan& plan, uint32_t n_chunks,
     return args;
 }
 
-// Resolve a stream of batches (semantics: one batch after the other).  Enqueues only.
-// h_in / h_out (isl_place_stream): the caller's host buffers.  With the segment pipeline the batches are copied and pre-passed one
-// by one on a second stream while the pipeline already runs (it waits per batch on a device flag), and an extra CTA copies every
-// finished chunk's results straight into h_out when that is mapped pinned memory (e->delivered) — H2D and D2H hide behind the kernel.
-int run_stream(isl_engine* e, uint32_t n_batches, const uint32_t* sizes, const uint2* d_in, uint2* d_out,
-               const uint32_t* d_heads_in, uint32_t* d_heads_out, uint32_t xepoch = 0, const uint2* h_in = nullptr, uint2* h_out = nullptr,
-               bool mixed_single_chunk = false) {
-    e->delivered = false;
-    const uint32_t pc = e->pipe_chunk;
-    uint64_t total = 0;
-    uint32_t n_chunks = 0, n_tiles_total = 0;
-    for (uint32_t b = 0; b < n_batches; ++b) {       // pipe_chunk is a whole number of tiles: a batch has as many tiles as its chunks
-        total += sizes[b]; n_chunks += ceil_div(sizes[b], pc); n_tiles_total += ceil_div(sizes[b], kTile);
-    }
-    if (total == 0) return ISL_OK;
-    if (total > e->cfg.max_batch) return ISL_ERANGE;
-    const uint32_t range = e->hi - e->lo;
-    const bool ring = xepoch != 0;      // partitioned inventory: tokens cross ranks through peer memory, pipeline mandatory
+// A placement call: n_batches batches, resolved one after the other.  Host calls stage through d_req / d_res and end with the results in
+// the caller's host buffer; src inline_host: <= kSmallInline host records, which can travel as kernel parameters.
+enum class Src { inline_host, host, device };
+struct Call {
+    uint32_t n_batches; const uint32_t* sizes;
+    Src src; const void* in; void* out;     // host or device memory, as src says
+    uint32_t xepoch = 0;                    // stream id of a partitioned inventory (isl_place_stream_partitioned; 0: none)
+    bool mixed = false;                     // one host batch of >= 4096 requests that mixes placeable profiles
+};
+
+enum class Path { few, small, chunks, bestfit, pipeline };
+struct Route {
+    Path path = Path::chunks;
+    PipePlan plan; bool feed = false; uint32_t window = 0;      // Path::pipeline: its plan, feed mode, causal window
+};
+
+// Which path a call of total (> 0) requests in n_chunks pipeline chunks takes (DESIGN.md 4.3), into a default Route.  Launches nothing.
+// ISL_ERANGE: a ring that cannot run as one pipeline; ISL_ECUDA: the co-residency query failed.
+int route(isl_engine* e, const Call& c, uint64_t total, uint32_t n_chunks, Route* r) {
+    const uint32_t flags = e->cfg.flags, range = e->hi - e->lo, n = c.sizes[0];
+    const bool ring = c.xepoch != 0;        // partitioned inventory: tokens cross ranks through peer memory, pipeline mandatory
     if (ring && n_chunks > kMaxStreamChunks) return ISL_ERANGE;
-    auto copy_in_whole = [&]() -> int {       // paths that do not feed batch by batch: one H2D copy up front
-        if (h_in) ISL_CUDA(e, cudaMemcpyAsync(const_cast<uint2*>(d_in), h_in, (size_t)total * sizeof(uint2), cudaMemcpyHostToDevice, e->stream));
+    // latency paths: one batch of <= kSmallMax requests in one CTA (k_small); <= kFewMax inline requests on <= kFewGpus GPUs (k_few)
+    if (c.n_batches == 1 && !ring && n <= kSmallMax && !bestfit_family(e->cfg.policy) && !(flags & (ISL_FLAG_NO_SMALL | ISL_FLAG_FORCE_PIPELINE)) &&
+        range > 0 && range <= (1u << 18)) {
+        const bool few = c.src == Src::inline_host && n <= kFewMax && e->hi - (e->lo & ~15u) <= kFewGpus && !getenv("ISL_NO_FEW");
+        r->path = few ? Path::few : Path::small;
         return ISL_OK;
-    };
-    auto batch_by_batch = [&]() -> int {      // one batch after the other through the single-chain path
-        uint64_t off = 0;
-        uint32_t hoff = 0;
-        for (uint32_t b = 0; b < n_batches; ++b) {
-            if (int rc = run_batch(e, sizes[b], d_in + off, d_out + off, d_heads_in ? d_heads_in + hoff : nullptr, d_heads_out ? d_heads_out + hoff : nullptr)) return rc;
-            off += sizes[b]; hoff += ceil_div(sizes[b], kChunk) * ISL_MAX_PROFILES;
-        }
-        return ISL_OK;
-    };
-    if (n_batches == 1 && !d_heads_in && !d_heads_out && !xepoch && small_eligible(e, sizes[0])) {
-        if (int rc = copy_in_whole()) return rc;
-        return run_small(e, sizes[0], d_in, nullptr, d_out);
     }
-    if ((bestfit_family(e->cfg.policy) || reversed(e)) && (d_heads_in || d_heads_out || xepoch)) return ISL_EINVAL;   // best-fit / right-to-left do not partition
-    const bool legacy_token = d_heads_in || d_heads_out || bestfit_family(e->cfg.policy);   // isl_place_batch_partitioned: host-carried token, kChunk layout
-    bool pipeline = ring || (!legacy_token && !(e->cfg.flags & ISL_FLAG_NO_PIPELINE) && range > 0 && (n_chunks >= 2 || mixed_single_chunk || (e->cfg.flags & ISL_FLAG_FORCE_PIPELINE)));
-    // the stream path keeps one free-mask byte per GPU and batch: very long streams over large inventories go batch by batch
-    if (pipeline && (uint64_t)n_batches * e->occ_bytes > (256ull << 20)) { if (ring) return ISL_ERANGE; pipeline = false; }
-    // feed mode (below): host buffers, more than one batch, no timing / tracing of the phases, no kernel-serialising tool around
-    // (ISL_NO_FEED=1 switches feeding off by hand)
-    const bool want_feed = h_in && h_out && n_batches >= 2 && !(e->cfg.flags & (ISL_FLAG_TIMING | ISL_FLAG_TRACE)) && !ring && !getenv("ISL_NO_FEED") &&
+    if (bestfit_family(e->cfg.policy)) { r->path = Path::bestfit; return ISL_OK; }
+    const bool pipeline = ring || (!(flags & ISL_FLAG_NO_PIPELINE) && range > 0 && (n_chunks >= 2 || c.mixed || (flags & ISL_FLAG_FORCE_PIPELINE)));
+    if (!pipeline) return ISL_OK;
+    // the pipeline keeps one free-mask byte per GPU and batch: very long streams over large inventories go batch by batch
+    if ((uint64_t)c.n_batches * e->occ_bytes > (256ull << 20)) return ring ? ISL_ERANGE : ISL_OK;
+    // feed mode: host buffers, >= 2 batches, no phase timing / tracing, no kernel-serialising tool around, no ISL_NO_FEED=1 (by hand)
+    const bool want_feed = c.src == Src::host && c.n_batches >= 2 && !(flags & (ISL_FLAG_TIMING | ISL_FLAG_TRACE)) && !ring && !getenv("ISL_NO_FEED") &&
                            !kernels_serialised();
-    // causal window (device-side): chunk c waits for chunk c - window on every segment (of every rank: a ring counts ranks on the owner)
-    const uint32_t window = (ring && e->ring_world == 0) ? 0u : e->window;
-    PipePlan plan;
-    if (pipeline) {     // speculative rounds by default for a single batch or a window of 1..3
-        const int rc = plan_pipeline(e, n_chunks, (double)total / n_chunks, want_feed, ring, n_batches == 1 || (window >= 1 && window <= 3), true, false, &plan);
-        if (rc == ISL_ECUDA) return rc;
-        if (rc != ISL_OK) { if (ring) return ISL_ERANGE; pipeline = false; }
-    }
-    if (!pipeline) {
-        if (int rc = copy_in_whole()) return rc;
-        return batch_by_batch();
-    }
-    const bool timing = e->cfg.flags & ISL_FLAG_TIMING;
-    e->h_chunks.resize(n_chunks); e->h_tiles.resize(n_tiles_total);
-    {
-        uint32_t off = 0, chunk = 0, tile = 0;
-        for (uint32_t b = 0; b < n_batches; ++b) { describe_batch(b, off, sizes[b], pc, e->h_chunks.data(), chunk, e->h_tiles.data(), tile); off += sizes[b]; }
-    }
-    const uint32_t q_stride = pc + kQPad * ISL_MAX_PROFILES;
-    const uint32_t free_stride = (uint32_t)e->occ_bytes;           // bytes per batch
+    r->window = (ring && e->ring_world == 0) ? 0u : e->window;      // a ring counts the ranks of a window on the owner
+    const bool auto_spec = c.n_batches == 1 || (r->window >= 1 && r->window <= 3);        // speculative rounds by default
+    const int rc = plan_pipeline(e, n_chunks, (double)total / n_chunks, want_feed, ring, auto_spec, true, false, &r->plan);
+    if (rc == ISL_ECUDA) return rc;
+    if (rc) return ring ? ISL_ERANGE : ISL_OK;
+    r->path = Path::pipeline;
     // feeding also needs room for the copier CTA plus the reserve: the pre-pass could starve behind a full house of pipeline CTAs
-    const bool feed = want_feed && plan.n_seg + 1 + kFeedReserve <= (uint32_t)e->max_coresident;
+    r->feed = want_feed && r->plan.n_seg + 1 + kFeedReserve <= (uint32_t)e->max_coresident;
+    return ISL_OK;
+}
+
+// Path::chunks / Path::bestfit: one batch after the other
+int run_batches(isl_engine* e, const Call& c, const uint2* d_in, uint2* d_out, bool bestfit) {
+    uint64_t off = 0;
+    for (uint32_t b = 0; b < c.n_batches; off += c.sizes[b++])
+        if (int rc = bestfit ? run_bestfit(e, c.sizes[b], d_in + off, d_out + off) : run_chunks(e, c.sizes[b], d_in + off, d_out + off, nullptr, nullptr)) return rc;
+    return ISL_OK;
+}
+
+// Path::pipeline: the pre-pass of every batch, then ONE cooperative k_pipeline.  With r.feed the batches are copied and pre-passed one by
+// one on the feed stream while the pipeline runs (it waits per batch on a device flag), and an extra CTA copies every finished chunk's
+// results into the caller's buffer when that is mapped pinned memory (*delivered).  A refused launch falls back to the chunk path.
+int run_pipeline(isl_engine* e, const Call& c, const Route& r, const uint2* d_in, uint2* d_out, uint64_t total, uint32_t n_chunks, bool* delivered) {
+    const uint32_t pc = e->pipe_chunk, n_batches = c.n_batches, *sizes = c.sizes, xepoch = c.xepoch, window = r.window;
+    const uint2* h_in = static_cast<const uint2*>(c.in);          // feed: the caller's host buffer
+    const PipePlan& plan = r.plan;
+    const bool ring = xepoch != 0, feed = r.feed, timing = e->cfg.flags & ISL_FLAG_TIMING;
+    uint32_t n_tiles_total = 0;         // pipe_chunk is a whole number of tiles: no tile spans two chunks
+    for (uint32_t b = 0; b < n_batches; ++b) n_tiles_total += ceil_div(sizes[b], kTile);
+    e->h_chunks.resize(n_chunks); e->h_tiles.resize(n_tiles_total);
+    for (uint32_t b = 0, off = 0, chunk = 0, tile = 0; b < n_batches; off += sizes[b++])
+        describe_batch(b, off, sizes[b], pc, e->h_chunks.data(), chunk, e->h_tiles.data(), tile);
+    const uint32_t q_stride = pc + kQPad * ISL_MAX_PROFILES, free_stride = (uint32_t)e->occ_bytes;      // free_stride: bytes per batch
     const bool need_done = feed || window;
     if (int rc = grow_stream_buffers(e, n_chunks, q_stride, n_tiles_total, n_batches, plan.n_seg, feed ? n_batches + 1 : 0, need_done ? n_chunks : 0)) return rc;
     if (n_tiles_total > ceil_div(e->cfg.max_batch, kTile) + 4096) return ISL_ERANGE;
     uint2* h_out_dev = nullptr;
-    if (feed) {
+    if (feed) {     // the feed stream starts behind whatever the engine's stream still holds (earlier calls, load_inventory)
         cudaPointerAttributes pa{};
-        if (cudaPointerGetAttributes(&pa, h_out) == cudaSuccess && pa.type == cudaMemoryTypeHost && pa.devicePointer) h_out_dev = static_cast<uint2*>(pa.devicePointer);
+        if (cudaPointerGetAttributes(&pa, c.out) == cudaSuccess && pa.type == cudaMemoryTypeHost && pa.devicePointer) h_out_dev = static_cast<uint2*>(pa.devicePointer);
         cudaGetLastError();
         if (int rc = ensure_feed_stream(e)) return rc;
-    }
-    const cudaStream_t pre = feed ? e->feed_stream : e->stream;     // the stream the tables and the pre-pass go to
-    if (feed) {     // the feed stream starts behind whatever the engine's stream still holds (earlier calls, load_inventory)
         ISL_CUDA(e, cudaEventRecord(e->ev_feed, e->stream));
         ISL_CUDA(e, cudaStreamWaitEvent(e->feed_stream, e->ev_feed, 0));
-    } else if (int rc = copy_in_whole()) return rc;
+    }
+    const cudaStream_t pre = feed ? e->feed_stream : e->stream;     // the stream the tables and the pre-pass go to
     if (need_done) ISL_CUDA(e, cudaMemsetAsync(e->d_done_cnt, 0, (size_t)n_chunks * sizeof(uint32_t), pre));
     ISL_CUDA(e, cudaMemcpyAsync(e->d_chunks, e->h_chunks.data(), n_chunks * sizeof(ChunkDesc), cudaMemcpyHostToDevice, pre));
     ISL_CUDA(e, cudaMemcpyAsync(e->d_tiles, e->h_tiles.data(), n_tiles_total * sizeof(TileDesc), cudaMemcpyHostToDevice, pre));
@@ -766,14 +763,13 @@ int run_stream(isl_engine* e, uint32_t n_batches, const uint32_t* sizes, const u
     args.ready = feed ? e->d_ready.get() : nullptr; args.done_cnt = (h_out_dev || window) ? e->d_done_cnt.get() : nullptr; args.host_out = h_out_dev;
     args.copier = h_out_dev ? 1u : 0u; args.window = window; args.owner_out = ring ? e->d_owner_out.get() : nullptr;
     if (ring_done) { args.ring_done = ring_done; args.world = e->ring_world; }
-    args.heads_in = d_heads_in; args.heads_out = d_heads_out;
     args.trace = trace ? e->d_trace.get() : nullptr;
     args.inbox = ring && e->has_prev ? e->d_inbox.get() : nullptr; args.outbox = ring ? e->d_outbox.get() : nullptr; args.xepoch = xepoch;
     if (plan.spec) {
         if (ring) {         // no token ring: the records themselves cross the ranks
             args.inbox = nullptr; args.outbox = nullptr;
             args.spec_world = e->spec_world; args.spec_rank = e->spec_rank; args.spec_base = e->lo / plan.seg; args.spec_total = ceil_div(e->G, plan.seg);
-            for (uint32_t r = 0; r < e->spec_world; ++r) args.spec_peer[r] = e->spec_peer[r];
+            for (uint32_t k = 0; k < e->spec_world; ++k) args.spec_peer[k] = e->spec_peer[k];
         }
         if (const char* v = getenv("ISL_SPEC_DBG")) {       // per-round stamps of one (chunk, stage) cell: tools/spec_trace.py
             unsigned cchunk = 0, cstage = 0;
@@ -791,9 +787,9 @@ int run_stream(isl_engine* e, uint32_t n_batches, const uint32_t* sizes, const u
         if (feed) {                 // only batch 0 was fed: bring the whole stream in behind it
             ISL_CUDA(e, cudaEventRecord(e->ev_feed_done, pre));
             ISL_CUDA(e, cudaStreamWaitEvent(e->stream, e->ev_feed_done, 0));
-            if (int rc2 = copy_in_whole()) return rc2;
+            ISL_CUDA(e, cudaMemcpyAsync(const_cast<uint2*>(d_in), h_in, (size_t)total * sizeof(uint2), cudaMemcpyHostToDevice, e->stream));
         }
-        return batch_by_batch();
+        return run_batches(e, c, d_in, d_out, false);
     }
     if (rc) return rc;
     if (feed) {     // the remaining batches, while the pipeline works on the first ones
@@ -807,7 +803,7 @@ int run_stream(isl_engine* e, uint32_t n_batches, const uint32_t* sizes, const u
             }
         ISL_CUDA(e, cudaEventRecord(e->ev_feed_done, pre));
         ISL_CUDA(e, cudaStreamWaitEvent(e->stream, e->ev_feed_done, 0));
-        e->delivered = h_out_dev != nullptr;
+        *delivered = h_out_dev != nullptr;
     }
     if (timing) {
         cudaEventRecord(e->ev[3], e->stream);
@@ -821,6 +817,77 @@ int run_stream(isl_engine* e, uint32_t n_batches, const uint32_t* sizes, const u
     e->st.batches += n_batches;
     e->st.requests += total;
     return ISL_OK;
+}
+
+// One placement call: route(), then the executor of its path.  A device call only enqueues; a host call ends with its results delivered.
+int run_stream(isl_engine* e, const Call& c) {
+    uint64_t total = 0;
+    uint32_t n_chunks = 0;
+    for (uint32_t b = 0; b < c.n_batches; ++b) { total += c.sizes[b]; n_chunks += ceil_div(c.sizes[b], e->pipe_chunk); }
+    if (total == 0) return ISL_OK;      // (every caller's Entry has checked total <= max_batch)
+    Route r;
+    if (int rc = route(e, c, total, n_chunks, &r)) return rc;
+    const uint32_t n = c.sizes[0];
+    if (c.src == Src::inline_host && (r.path == Path::few || r.path == Path::small)) {
+        SmallReqs inl{};        // requests as kernel parameters, results into mapped pinned memory: 1 launch + 1 sync
+        memcpy(inl.r, c.in, (size_t)n * sizeof(isl_request));
+        if (int rc = r.path == Path::few ? run_few(e, n, inl, e->h_small_out.dev()) : run_small(e, n, nullptr, &inl, e->h_small_out.dev())) return rc;
+        ISL_CUDA(e, cudaStreamSynchronize(e->stream));
+        memcpy(c.out, e->h_small_out, (size_t)n * sizeof(isl_result));
+        return ISL_OK;
+    }
+    const bool host = c.src != Src::device;
+    const uint2* d_in = host ? e->d_req.get() : static_cast<const uint2*>(c.in);
+    uint2* d_out = host ? e->d_res.get() : static_cast<uint2*>(c.out);
+    if (host && !r.feed)        // one H2D copy up front; a fed stream copies batch by batch
+        ISL_CUDA(e, cudaMemcpyAsync(e->d_req, c.in, (size_t)total * sizeof(isl_request), cudaMemcpyHostToDevice, e->stream));
+    bool delivered = false;
+    const int rc = r.path == Path::pipeline ? run_pipeline(e, c, r, d_in, d_out, total, n_chunks, &delivered)
+                   : r.path == Path::small  ? run_small(e, n, d_in, nullptr, d_out)
+                                            : run_batches(e, c, d_in, d_out, r.path == Path::bestfit);
+    if (rc || !host) return rc;
+    if (!delivered) ISL_CUDA(e, cudaMemcpyAsync(c.out, d_out, (size_t)total * sizeof(isl_result), cudaMemcpyDeviceToHost, e->stream));
+    ISL_CUDA(e, cudaStreamSynchronize(e->stream));
+    return ISL_OK;
+}
+
+int place_batch_plain(isl_engine* e, uint32_t n, const isl_request* in, isl_result* out) {
+    // One large batch that mixes profiles: the segment pipeline's decision loop (one launch for the chain of all segments, a shorter
+    // loop per decision) beats the chunk path although nothing overlaps inside one chunk; a single placeable profile stays on the
+    // chunk path, whose scan mode commits it without any chain.  A look at the profile bytes in host memory costs microseconds.
+    bool mixed = false;
+    if (n >= 4096) {
+        uint32_t seen = 0;
+        for (uint32_t i = 0; i < n && !mixed; ++i)
+            if (in[i].op == ISL_OP_ALLOC && in[i].profile < ISL_MAX_PROFILES) { seen |= (1u << in[i].profile) & e->cand_profiles; mixed = (seen & (seen - 1)) != 0; }
+    }
+    return run_stream(e, Call{1, &n, n <= kSmallInline ? Src::inline_host : Src::host, in, out, 0, mixed});
+}
+
+// ISL_FLAG_ALL_NODES — the reference's literal multi-node behaviour (SURVEY Q5): Reconcile's node loop (:190-227) has no `break` after a
+// successful node, so a pod is allocated on EVERY node that has capacity.  Nodes do not interact (an allocation on one node never
+// changes what another node can take), so "every pod over all nodes" equals "every node over all pods": one restricted pass per node,
+// each consuming capacity on its node; the record reported for a pod is the first node's (what the oracle's all_nodes switch reports).
+// A compatibility mode for parity studies, one engine call per node — not a fast path.
+int place_batch_locked(isl_engine* e, uint32_t n, const isl_request* in, isl_result* out) {
+    if (!(e->cfg.flags & ISL_FLAG_ALL_NODES)) return place_batch_plain(e, n, in, out);
+    const uint32_t n_nodes = (uint32_t)e->node_off.size() - 1;
+    const auto [clo, chi] = storage_range(e, e->lo, e->hi);         // the caller's range, canonical
+    RangeRestriction range{e, e->lo, e->hi};
+    std::vector<isl_result> tmp(n);
+    bool first = true;
+    for (uint32_t k = 0; k < n_nodes; ++k) {
+        const uint32_t node = e->prof.flip ? n_nodes - 1 - k : k;                  // nodes in policy order
+        const uint32_t a = std::max(clo, e->node_off[node]), b = std::min(chi, e->node_off[node + 1]);
+        if (a >= b) continue;
+        range.set(a, b);
+        if (int rc = place_batch_plain(e, n, in, first ? out : tmp.data())) return rc;
+        if (!first)
+            for (uint32_t i = 0; i < n; ++i)
+                if (in[i].op == ISL_OP_ALLOC && out[i].status != ISL_ST_PLACED && tmp[i].status == ISL_ST_PLACED) out[i] = tmp[i];
+        first = false;
+    }
+    return first ? place_batch_plain(e, n, in, out) : ISL_OK;      // empty range: defaults only
 }
 
 // Default row of every name (its size is what an unplaced ALLOC reports): the row of the first node, in canonical order, whose table has
@@ -1221,8 +1288,6 @@ uint32_t isl_gpu_to_node(const isl_engine* e, uint32_t gpu) {
     return (uint32_t)(it - e->node_off.begin()) - 1;
 }
 
-static int place_batch_locked(isl_engine* e, uint32_t n, const isl_request* in, isl_result* out);
-
 int isl_place_batch(isl_engine* e, uint32_t n, const isl_request* in, isl_result* out) {
     if (!e || (n && (!in || !out))) return ISL_EINVAL;
     Entry guard(e, Needs::ready, n);
@@ -1237,11 +1302,9 @@ int isl_place_batch_range(isl_engine* e, uint32_t lo, uint32_t hi, uint32_t n, c
     if (guard.rc) return guard.rc;
     if (lo > hi || hi > e->G) return ISL_EINVAL;
     if (n == 0) return ISL_OK;
-    const uint32_t lo0 = e->lo, hi0 = e->hi;
-    if (e->prof.flip) { e->lo = e->G - hi; e->hi = e->G - lo; } else { e->lo = lo; e->hi = hi; }
-    const int rc = place_batch_locked(e, n, in, out);
-    e->lo = lo0; e->hi = hi0;
-    return rc;
+    RangeRestriction range{e, e->lo, e->hi};
+    range.set(lo, hi);
+    return place_batch_locked(e, n, in, out);
 }
 
 int isl_place_gangs(isl_engine* e, uint32_t n_gangs, const uint32_t* gang_off, const isl_request* in, isl_result* out) {
@@ -1327,75 +1390,14 @@ int isl_preempt(isl_engine* e, uint32_t n, const isl_request* in, const uint8_t*
     return ISL_OK;
 }
 
-static int place_batch_plain(isl_engine* e, uint32_t n, const isl_request* in, isl_result* out);
-
-// ISL_FLAG_ALL_NODES — the reference's literal multi-node behaviour (SURVEY Q5): Reconcile's node loop (:190-227) has no `break` after a
-// successful node, so a pod is allocated on EVERY node that has capacity.  Nodes do not interact (an allocation on one node never
-// changes what another node can take), so "every pod over all nodes" equals "every node over all pods": one restricted pass per node,
-// each consuming capacity on its node; the record reported for a pod is the first node's (what the oracle's all_nodes switch reports).
-// A compatibility mode for parity studies, one engine call per node — not a fast path.
-static int place_batch_locked(isl_engine* e, uint32_t n, const isl_request* in, isl_result* out) {
-    if (!(e->cfg.flags & ISL_FLAG_ALL_NODES)) return place_batch_plain(e, n, in, out);
-    const uint32_t lo0 = e->lo, hi0 = e->hi, n_nodes = (uint32_t)e->node_off.size() - 1;
-    const uint32_t clo = e->prof.flip ? e->G - hi0 : lo0, chi = e->prof.flip ? e->G - lo0 : hi0;     // the caller's range, canonical
-    std::vector<isl_result> tmp(n);
-    bool first = true;
-    int rc = ISL_OK;
-    for (uint32_t k = 0; k < n_nodes && !rc; ++k) {
-        const uint32_t node = e->prof.flip ? n_nodes - 1 - k : k;                  // nodes in policy order
-        const uint32_t a = std::max(clo, e->node_off[node]), b = std::min(chi, e->node_off[node + 1]);
-        if (a >= b) continue;
-        if (e->prof.flip) { e->lo = e->G - b; e->hi = e->G - a; } else { e->lo = a; e->hi = b; }
-        rc = place_batch_plain(e, n, in, first ? out : tmp.data());
-        if (!rc && !first)
-            for (uint32_t i = 0; i < n; ++i)
-                if (in[i].op == ISL_OP_ALLOC && out[i].status != ISL_ST_PLACED && tmp[i].status == ISL_ST_PLACED) out[i] = tmp[i];
-        first = false;
-    }
-    e->lo = lo0; e->hi = hi0;
-    if (!rc && first) rc = place_batch_plain(e, n, in, out);       // empty range: defaults only
-    return rc;
-}
-
-static int place_batch_plain(isl_engine* e, uint32_t n, const isl_request* in, isl_result* out) {
-    if (n <= kSmallInline && small_eligible(e, n)) {        // requests as kernel parameters, results into mapped pinned memory: 1 launch + 1 sync
-        SmallReqs inl{};
-        memcpy(inl.r, in, (size_t)n * sizeof(isl_request));
-        if (int rc = few_eligible(e, n) ? run_few(e, n, inl, e->h_small_out.dev()) : run_small(e, n, nullptr, &inl, e->h_small_out.dev())) return rc;
-        ISL_CUDA(e, cudaStreamSynchronize(e->stream));
-        memcpy(out, e->h_small_out, (size_t)n * sizeof(isl_result));
-        return ISL_OK;
-    }
-    ISL_CUDA(e, cudaMemcpyAsync(e->d_req, in, (size_t)n * sizeof(isl_request), cudaMemcpyHostToDevice, e->stream));
-    // One large batch that mixes profiles: the segment pipeline's decision loop (one launch for the chain of all segments, a shorter
-    // loop per decision) beats the single-chain path although nothing overlaps inside one chunk.  A batch with a single placeable
-    // profile stays on the single-chain path, whose scan mode commits it without any chain.  (The buffer is on the host: a look at
-    // the profile bytes costs microseconds.)
-    bool mixed = false;
-    if (n >= 4096) {
-        uint32_t seen = 0;
-        for (uint32_t i = 0; i < n && !mixed; ++i)
-            if (in[i].op == ISL_OP_ALLOC && in[i].profile < ISL_MAX_PROFILES) { seen |= (1u << in[i].profile) & e->cand_profiles; mixed = (seen & (seen - 1)) != 0; }
-    }
-    if (int rc = run_stream(e, 1, &n, e->d_req, e->d_res, nullptr, nullptr, 0, nullptr, nullptr, mixed)) return rc;
-    ISL_CUDA(e, cudaMemcpyAsync(out, e->d_res, (size_t)n * sizeof(isl_result), cudaMemcpyDeviceToHost, e->stream));
-    ISL_CUDA(e, cudaStreamSynchronize(e->stream));
-    return ISL_OK;
-}
-
 int isl_place_stream(isl_engine* e, uint32_t n_batches, const uint32_t* sizes, const isl_request* in, isl_result* out) {
     uint64_t total;
     if (int rc = stream_entry(e, n_batches, sizes, in && out, &total)) return rc;
     Entry guard(e, Needs::ready, total);
     if (guard.rc) return guard.rc;
-    if (total == 0) return ISL_OK;
-    if (int rc = run_stream(e, n_batches, sizes, e->d_req, e->d_res, nullptr, nullptr, 0, reinterpret_cast<const uint2*>(in), reinterpret_cast<uint2*>(out))) {
-        if (e->feed_stream) cudaStreamSynchronize(e->feed_stream);
-        return rc;
-    }
-    if (!e->delivered) ISL_CUDA(e, cudaMemcpyAsync(out, e->d_res, (size_t)total * sizeof(isl_result), cudaMemcpyDeviceToHost, e->stream));
-    ISL_CUDA(e, cudaStreamSynchronize(e->stream));
-    return ISL_OK;
+    const int rc = run_stream(e, Call{n_batches, sizes, Src::host, in, out});
+    if (rc && e->feed_stream) cudaStreamSynchronize(e->feed_stream);
+    return rc;
 }
 
 int isl_place_stream_device(isl_engine* e, uint32_t n_batches, const uint32_t* sizes, const void* d_in, void* d_out) {
@@ -1404,7 +1406,7 @@ int isl_place_stream_device(isl_engine* e, uint32_t n_batches, const uint32_t* s
     if (int rc = stream_entry(e, n_batches, sizes, true, &total)) return rc;
     Entry guard(e, Needs::ready, total);
     if (guard.rc) return guard.rc;
-    return run_stream(e, n_batches, sizes, static_cast<const uint2*>(d_in), static_cast<uint2*>(d_out), nullptr, nullptr);
+    return run_stream(e, Call{n_batches, sizes, Src::device, d_in, d_out});
 }
 
 int isl_ipc_inbox_handle(isl_engine* e, void* handle64) {
@@ -1494,21 +1496,25 @@ int isl_place_stream_partitioned(isl_engine* e, uint32_t n_batches, const uint32
     if (int rc = stream_entry(e, n_batches, sizes, true, &total)) return rc;
     Entry guard(e, Needs::ready, total);
     if (guard.rc) return guard.rc;
-    return run_stream(e, n_batches, sizes, static_cast<const uint2*>(d_in), static_cast<uint2*>(d_out), nullptr, nullptr, stream_id);
+    if (total == 0) return ISL_OK;
+    if (bestfit_family(e->cfg.policy) || reversed(e)) return ISL_EINVAL;        // best-fit / right-to-left do not partition
+    return run_stream(e, Call{n_batches, sizes, Src::device, d_in, d_out, stream_id});
 }
 
 int isl_place_batch_device(isl_engine* e, uint32_t n, const void* d_in, void* d_out) {
     if (!e || (n && (!d_in || !d_out))) return ISL_EINVAL;
     Entry guard(e, Needs::ready, n);
     if (guard.rc) return guard.rc;
-    return run_stream(e, 1, &n, static_cast<const uint2*>(d_in), static_cast<uint2*>(d_out), nullptr, nullptr);
+    return run_stream(e, Call{1, &n, Src::device, d_in, d_out});
 }
 
 int isl_place_batch_partitioned(isl_engine* e, uint32_t n, const void* d_in, void* d_out, const void* d_heads_in, void* d_heads_out) {
     if (!e || (n && (!d_in || !d_out)) || !d_heads_out) return ISL_EINVAL;
     Entry guard(e, Needs::ready, n);
     if (guard.rc) return guard.rc;
-    return run_stream(e, 1, &n, static_cast<const uint2*>(d_in), static_cast<uint2*>(d_out), static_cast<const uint32_t*>(d_heads_in),
+    if (n == 0) return ISL_OK;
+    if (bestfit_family(e->cfg.policy) || reversed(e)) return ISL_EINVAL;        // best-fit / right-to-left do not partition
+    return run_chunks(e, n, static_cast<const uint2*>(d_in), static_cast<uint2*>(d_out), static_cast<const uint32_t*>(d_heads_in),
                       static_cast<uint32_t*>(d_heads_out));
 }
 
@@ -1517,7 +1523,7 @@ int isl_set_partition(isl_engine* e, uint32_t lo, uint32_t hi) {
     Entry guard(e, Needs::inventory);
     if (guard.rc) return guard.rc;
     if (lo > hi || hi > e->G) return ISL_EINVAL;
-    if (e->prof.flip) { e->lo = e->G - hi; e->hi = e->G - lo; } else { e->lo = lo; e->hi = hi; }
+    std::tie(e->lo, e->hi) = storage_range(e, lo, hi);
     return ISL_OK;
 }
 

@@ -1,7 +1,11 @@
 """Every C-ABI entry point of islplace.cu that takes an engine opens with one Entry, the guard that takes the engine lock, checks the
 engine state and makes the engine's device current; the state it asks for (Needs) is the one its row in tests/engine_contract.py
 refuses without.  These checks read the source; they need no GPU."""
+import ctypes as C
 import re
+
+import numpy as np
+import pytest
 
 import engine_contract as K
 from instaslice_b200 import engine as E
@@ -44,3 +48,23 @@ def test_lock_and_readiness_only_in_the_guard():
         assert flag in guard
         uses = re.findall(r"\b%s\b(\s*=(?!=))?" % flag, rest)
         assert uses and all(uses), flag           # declared and set, never read
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize("policy", [E.POLICY_BEST_FIT, E.POLICY_RIGHT_TO_LEFT])
+def test_empty_partitioned_call_returns_ok_before_the_policy_check(policy):
+    """Best-fit and right-to-left engines do not partition (ISL_EINVAL), but an empty partitioned call has nothing to place and returns
+    ISL_OK first.  Needs an H100."""
+    import torch
+    from instaslice_b200 import tables
+    eng = E.Engine(max_gpus=64, max_batch=64, policy=policy)
+    eng.load_profiles(E.make_profiles(tables.H100_80GB))
+    eng.load_inventory(np.array([0, 8], dtype=np.uint32), np.zeros(8, dtype=np.uint8))
+    buf = torch.zeros(64 * 8, dtype=torch.uint8, device="cuda")
+    torch.cuda.synchronize()
+    L, h, p = eng._lib, eng._h, C.c_void_p(buf.data_ptr())
+    for n, want in ((0, E.OK), (8, E.EINVAL)):
+        sizes = np.array([n], dtype=np.uint32)
+        assert L.isl_place_batch_partitioned(h, n, p, p, None, p) == want, n
+        assert L.isl_place_stream_partitioned(h, 1, sizes.ctypes.data_as(C.c_void_p), p, p, 1) == want, n
+    eng.close()

@@ -342,7 +342,8 @@ def check_every_path(rng, eng, chunk_eng, bf_eng, model, bf_model, what):
     """k_few, k_small, the chunk path and its scan mode, the plain pipeline, speculative rounds, k_bestfit, capacity, eval_starts and
     what_if against the model; each path's launch count says it ran."""
     G = model.G
-    for shape, n in (("few", 8), ("small", 700), ("scan", 5000), ("plain", 6000), ("spec", 6000), ("chunks", 6000)):
+    for shape, n in (("few", 8), ("small", 700), ("scan", 5000), ("plain", 6000), ("spec", 6000), ("chunks", 6000), ("mixed", 3000)):
+        # "mixed": a host batch that mixes profiles but is too short for the pipeline takes the chunk path
         req = mixed_requests(rng, model.occ, 0, G, model.n_names, n, profile=0 if shape == "scan" else None)
         e = chunk_eng if shape == "chunks" else eng
         if shape == "chunks":
@@ -352,7 +353,7 @@ def check_every_path(rng, eng, chunk_eng, bf_eng, model, bf_model, what):
         got = e.place_batch(req)
         want = model.place_batch(req)
         compare(got, want, e, model, (what, shape))
-        check_path(delta(e, before), {"few": "one", "small": "one"}.get(shape, shape), n, (what, shape), G, 0, G, model.n_tables)
+        check_path(delta(e, before), {"few": "one", "small": "one", "mixed": "chunks"}.get(shape, shape), n, (what, shape), G, 0, G, model.n_tables)
         if shape == "chunks":
             eng.write_occupancy(0, model.occ)
         if shape == "scan":

@@ -362,6 +362,17 @@ def test_device_resident_entry_point_matches_host_entry_point():
     assert np.array_equal(got, want)
     st = eng.stats()
     assert st["placed"] == int((want["status"] == E.ST_PLACED).sum()) * 2 and st["kernel_launches"] > 0
+    # one device-resident chunk: k_small up to 1024 requests, else the chunk path even when it mixes profiles (only a host batch is
+    # looked at for that)
+    for n, launches in ((700, 1), (5000, 6)):
+        eng.load_inventory(node_off, occ)
+        want = eng.place_batch(req[:n])
+        eng.load_inventory(node_off, occ)
+        before = eng.stats()["kernel_launches"]
+        eng.place_batch_device(n, d_in.data_ptr(), d_out.data_ptr())
+        eng.synchronize()
+        assert eng.stats()["kernel_launches"] - before == launches, (n, eng.stats())
+        assert np.array_equal(d_out[:n].cpu().numpy().view(E.RESULT_DTYPE), want), n
 
 
 # ---- partitioned inventory: token ring between engines (the N > 1 device path) on ONE GPU ---------------------------
