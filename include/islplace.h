@@ -75,6 +75,32 @@ extern "C" {
                                      right-to-left starts as well) */
 #define ISL_POLICY_MIN_FRAG  3u   /* extension (SURVEY 8a-ext "richer score"): among the feasible GPUs, the one where the placement makes the fewest
                                      (profile, start) pairs of the table infeasible; ties -> lowest canonical index */
+/* Node scoring: the kube-scheduler's NodeResourcesFit strategies, which never apply to gated MIG pods, over the NODES of the range.
+ * MOST_ALLOCATED packs pods onto the fullest nodes (so that the cluster autoscaler can drain the emptiest), LEAST_ALLOCATED (the
+ * scheduler's default) spreads them.  Batch semantics are unchanged: FREEs first, then the ALLOCs in array order, each seeing every
+ * earlier commit.  For one ALLOC of profile name p:
+ *   1. Candidate nodes: a node with at least one GPU inside the call's range (the partition, isl_place_batch_range) whose occupancy byte
+ *      has a start for p in the start search of its node's table (under the engine's quirk set).  GPUs outside the range do not exist for
+ *      the call, also on a node the range cuts.  An empty node is never a candidate.
+ *   2. Capacity and usage in MIG memory slices: width(t) = the largest start + size over the rows of table t (8 for the A100 / H100 /
+ *      B200 tables, 4 for A30); cap(N) = width(t_N) x the node's GPUs in range; busy(N) = the sum over those GPUs of
+ *      popcount(occ & ((1 << width) - 1)); req = the size of p's row in the node's table.
+ *   3. Score, NodeResourcesFit's integer formulas with one resource of weight 1 and MaxNodeScore 100:
+ *      MOST_ALLOCATED floor(100 x (busy + req) / cap), LEAST_ALLOCATED floor(100 x (cap - busy - req) / cap).  On a candidate
+ *      busy + req <= cap, and a table without rows (width 0) has no candidate.
+ *   4. The highest score wins, ties to the lowest canonical node index (the scheduler picks at random among ties; the engine is
+ *      deterministic).  Inside the node the reference's own search decides (findDeviceForASlice on one node, :240-262): the first GPU
+ *      in canonical order, within the range, whose byte admits p, and its first legal start in row order.
+ *   5. The usual records: PLACED (gpu, start, size); NO_CAPACITY with the default size when no node is a candidate; BAD_PROFILE;
+ *      FREED / BAD_SPAN / NOOP.  Stats count as for the best-fit family.
+ *   6. Accepted by isl_place_batch, _range, _device, isl_place_stream, _device (one batch after the other), isl_what_if, isl_capacity,
+ *      isl_free_batch, isl_eval_starts, isl_set_partition, per-node tables and isl_preempt (whose scan order is ascending canonical).
+ *   7. isl_create: ISL_EINVAL with ISL_FLAG_ALL_NODES (a pod placed on every node has no node to choose), ISL_ERANGE for
+ *      max_gpus > 2^20.  ISL_EINVAL from isl_place_batch_partitioned, isl_place_stream_partitioned, isl_stream_open and
+ *      isl_place_gangs.
+ * On an inventory of one node both give exactly ISL_POLICY_FIRST_FIT's records and occupancy. */
+#define ISL_POLICY_MOST_ALLOCATED  4u
+#define ISL_POLICY_LEAST_ALLOCATED 5u
 
 /* isl_config.quirks — bit set = reproduce the reference bug exactly */
 #define ISL_QUIRK_STRICT_BOUND 1u /* Q1: `value+size < 8` (:351,:360,:370) instead of <= 8 */
@@ -271,11 +297,11 @@ int  isl_place_batch_range(isl_engine* e, uint32_t lo, uint32_t hi, uint32_t n, 
  *      members after it are not tried, and every other ALLOC member of the gang reports ISL_ST_GANG_ABORTED with the unplaced default
  *      record (gpu ISL_GPU_NONE, start 9, the profile's size or 0 for an unknown profile).
  *   5. The occupancy after an aborted gang is exactly what it was before it: later gangs see no trace of it.
- *   6. Every policy, both quirk sets and per-node tables; inside the engine's partition (isl_set_partition).  Stats count committed
- *      placements only.
+ *   6. Every policy except node scoring (ISL_POLICY_MOST_ALLOCATED / _LEAST_ALLOCATED), both quirk sets and per-node tables; inside
+ *      the engine's partition (isl_set_partition).  Stats count committed placements only.
  * A call whose gangs all have one member equals isl_place_batch on the same requests, records and occupancy.  The gangs are resolved
  * request by request (the best-fit kernel's loop, DESIGN.md 4.6): first-fit gangs do not use the segment pipeline.
- * ISL_EINVAL: malformed offsets, NULL buffers, an engine created with ISL_FLAG_ALL_NODES.  ISL_ERANGE: n > max_batch, or a partition
+ * ISL_EINVAL: malformed offsets, NULL buffers, an engine created with ISL_FLAG_ALL_NODES or a node-scoring policy.  ISL_ERANGE: n > max_batch, or a partition
  * that is empty or holds more than 2^20 GPUs.  ISL_ESTATE: no profiles or inventory, or an open stream. */
 int  isl_place_gangs(isl_engine* e, uint32_t n_gangs, const uint32_t* gang_off, const isl_request* in, isl_result* out);
 
@@ -307,7 +333,7 @@ typedef struct isl_victim {
  *      also where it extends beyond the mask.
  *   5. The choice is the lexicographic minimum over all candidates of: the highest priority in V (an empty V below every priority),
  *      the sum of V's priorities, |V|, the GPU's position in the engine's scan order (ascending canonical index; descending under
- *      ISL_POLICY_RIGHT_TO_LEFT; ascending for the best-fit family), v's position in the row — the order of the kube-scheduler's
+ *      ISL_POLICY_RIGHT_TO_LEFT; ascending for the best-fit family and node scoring), v's position in the row — the order of the kube-scheduler's
  *      pickOneNodeForPreemption without its PodDisruptionBudget and start-time keys.  The record is PLACED (g, v, size) and
  *      evict[8i .. 8i+8) holds the indices into `victims` of V in ascending order, padded with ISL_GPU_NONE.  With no candidate the
  *      record is the usual unplaced one (NO_CAPACITY, gpu NONE, start 9, the default size); a record that is not PLACED has an

@@ -96,8 +96,12 @@ class InstasliceReconciler:
     GPUs by ascending UUID inside a node (the reference's orders are random, SURVEY Q6).
     """
 
-    def __init__(self, instaslices: list, quirks: int = E.QUIRKS_REF_EXACT, max_batch: int = 65536, engine: E.Engine | None = None):
+    def __init__(self, instaslices: list, quirks: int = E.QUIRKS_REF_EXACT, max_batch: int = 65536, engine: E.Engine | None = None,
+                 policy: int = E.POLICY_FIRST_FIT):
+        """``policy``: the engine policy of the engine this reconciler creates (``engine`` is None), e.g. ``E.POLICY_MOST_ALLOCATED`` to
+        pack MIG pods onto the fullest nodes or ``E.POLICY_LEAST_ALLOCATED`` to spread them (include/islplace.h)."""
         self.quirks = quirks
+        self.policy = policy
         self.items = instaslices
         self._engine = engine
         self._max_batch = max_batch
@@ -139,7 +143,7 @@ class InstasliceReconciler:
         self.node_off = np.asarray(node_off, dtype=np.uint32)
         self.gpu_index = {u: i for i, u in enumerate(self.gpu_uuid)}
         if self._engine is None:
-            self._engine = E.Engine(max_gpus=max(4096, len(self.gpu_uuid)), max_batch=self._max_batch, quirks=self.quirks)
+            self._engine = E.Engine(max_gpus=max(4096, len(self.gpu_uuid)), max_batch=self._max_batch, policy=self.policy, quirks=self.quirks)
         self._engine.load_profile_tables(self.rows)
         self._engine.load_inventory(self.node_off, np.asarray(occ, dtype=np.uint8))
         self._engine.set_node_tables(np.asarray(self.node_table, dtype=np.uint8))

@@ -2424,4 +2424,157 @@ __global__ void __launch_bounds__(kPreThreads, 1) k_preempt(PreemptArgs a, DevPr
     }
 }
 
+// ---------------------------------------------------------------------------------------------
+// k_nodefit: ISL_POLICY_MOST_ALLOCATED / ISL_POLICY_LEAST_ALLOCATED (DESIGN.md 4.8), the kube-scheduler's NodeResourcesFit scores over
+// the nodes of the range, in MIG memory slices.  Request-major like k_bestfit: one placement changes one node's score, and the very next
+// request sees it.  One CTA, one launch per batch behind k_prepare (frees and default records).
+//   build    one thread per node: cap = width(table) x GPUs in range, busy = popcount of the occupancy under the width, and per profile
+//            the GPUs that admit it; then per profile a 32-ary min-tree over the nodes, leaf key (100 - score) << 24 | local node index
+//            (INF where the profile fits on none of the node's GPUs), so the root is the winning node with ties to the lowest index
+//   request  every warp reads the root of the profile's tree.  INF: the default NO_CAPACITY record stands, the profile is dead for the
+//            rest of the batch (occupancy only grows).  Otherwise the chain warp takes the node's first admitting GPU (32 per ballot) and
+//            commits it; after a barrier warp q recounts profile q's fits on that node, rewrites its leaf and walks up (32 siblings and
+//            one redux.min per level, stopping where a parent keeps its value); a second barrier ends the request.
+// The trees live in shared memory up to kNfSmemNodes nodes and in global memory (L2) beyond.
+// ---------------------------------------------------------------------------------------------
+constexpr uint32_t kNfThreads = 32 * ISL_MAX_PROFILES;   // one warp per profile
+constexpr uint32_t kNfSmemNodes = 2048;                  // up to here the trees live in shared memory (16 x 2 176 words = 136 KiB)
+constexpr uint32_t kNfMaxLevels = 5;                     // 32^4 leaves >= kBfMaxGpus nodes
+
+struct NodeFitArgs {            // kernel parameter (by value)
+    const uint2* in;
+    uint2* out;
+    uint8_t* occ;
+    const uint8_t* gtab;        // table of every GPU's node
+    const uint8_t* lut;         // [table][profile][occ]
+    const uint8_t* sizes;       // [table][profile]
+    const uint32_t* node_off;   // the inventory's node offsets (n_nodes + 1)
+    uint32_t* tree;             // global trees ([profile][T] words), when they do not fit in shared memory
+    uint32_t* fit;              // [profile][Nr]: GPUs of the node that admit the profile
+    uint32_t* busy;             // [Nr]: busy slices under the width
+    uint32_t* meta;             // [Nr]: cap | table << 24
+    Ctrl* ctrl;
+    uint32_t n, lo, hi, nlo, Nr;        // requests; the range; its first node and node count
+    uint32_t most;                      // 1: MostAllocated, 0: LeastAllocated
+    uint32_t levels, T;                 // tree levels (the last holds the root) and words per profile
+    uint32_t lvl_off[kNfMaxLevels];     // first word of every level inside a profile's tree; level k has lvl_cnt[k] keys, padded to 32
+    uint32_t lvl_cnt[kNfMaxLevels];
+    uint8_t width[kMaxTables];          // largest start + size over the rows of every table
+};
+
+// The leaf key of a node for one profile: NodeResourcesFit's integer score with MaxNodeScore 100, smaller key = better node
+__device__ __forceinline__ uint32_t nodefit_leaf(uint32_t fit, uint32_t busy, uint32_t cap, uint32_t req, uint32_t most, uint32_t node) {
+    if (fit == 0) return kInf;
+    const uint32_t score = most ? 100u * (busy + req) / cap : 100u * (cap - busy - req) / cap;
+    return ((100u - score) << 24) | node;
+}
+
+__global__ void __launch_bounds__(kNfThreads, 1) k_nodefit(NodeFitArgs a, uint32_t n_profiles) {
+    extern __shared__ __align__(16) uint32_t s_tree[];
+    __shared__ uint8_t s_lut[kMaxTables * ISL_MAX_PROFILES * 256];
+    __shared__ uint8_t s_sizes[kMaxTables * ISL_MAX_PROFILES];
+    __shared__ uint32_t s_ev[2];                         // the committed GPU's occupancy byte before and after the request
+    const uint32_t tid = threadIdx.x, lane = tid & 31u, warp = tid >> 5;
+    uint32_t* tree = a.Nr <= kNfSmemNodes ? s_tree : a.tree;
+    for (uint32_t i = tid; i < sizeof(s_lut) / 4; i += kNfThreads) reinterpret_cast<uint32_t*>(s_lut)[i] = reinterpret_cast<const uint32_t*>(a.lut)[i];
+    if (tid < kMaxTables * ISL_MAX_PROFILES) s_sizes[tid] = a.sizes[tid];
+    __syncthreads();
+    auto admits = [&](uint32_t t, uint32_t q, uint32_t o) -> uint32_t { return s_lut[(t * ISL_MAX_PROFILES + q) * 256 + o] != ISL_START_NONE; };
+    // build: one thread per node
+    for (uint32_t v = tid; v < a.Nr; v += kNfThreads) {
+        const uint32_t g0 = max(a.lo, __ldg(a.node_off + a.nlo + v)), g1 = min(a.hi, __ldg(a.node_off + a.nlo + v + 1));
+        const uint32_t cnt = g1 > g0 ? g1 - g0 : 0u, t = cnt ? (uint32_t)(a.gtab[g0] & (kMaxTables - 1)) : 0u;
+        const uint32_t wm = (1u << a.width[t]) - 1u, cap = a.width[t] * cnt;
+        uint32_t busy = 0, fit[ISL_MAX_PROFILES] = {};
+        for (uint32_t g = g0; g < g1; ++g) {
+            const uint32_t o = a.occ[g];
+            busy += __popc(o & wm);
+#pragma unroll
+            for (uint32_t q = 0; q < ISL_MAX_PROFILES; ++q) fit[q] += admits(t, q, o);
+        }
+        a.busy[v] = busy; a.meta[v] = cap | (t << 24);
+#pragma unroll
+        for (uint32_t q = 0; q < ISL_MAX_PROFILES; ++q)
+            if (q < n_profiles) {
+                a.fit[(size_t)q * a.Nr + v] = fit[q];
+                tree[(size_t)q * a.T + v] = nodefit_leaf(fit[q], busy, cap, s_sizes[t * ISL_MAX_PROFILES + q], a.most, v);
+            }
+    }
+    for (uint32_t k = 0; k < a.levels; ++k) {            // level k from level k - 1 (leaves: only their padding), padding INF
+        __syncthreads();
+        const uint32_t cnt = a.lvl_cnt[k], padded = (cnt + 31u) & ~31u;
+        for (uint32_t i = tid; i < n_profiles * padded; i += kNfThreads) {
+            const uint32_t q = i / padded, j = i - q * padded;
+            uint32_t* lv = tree + (size_t)q * a.T + a.lvl_off[k];
+            if (j >= cnt) lv[j] = kInf;
+            else if (k > 0) {
+                const uint32_t* below = tree + (size_t)q * a.T + a.lvl_off[k - 1];
+                uint32_t m = kInf;
+                for (uint32_t c = 0; c < 32; ++c) m = min(m, below[j * 32 + c]);
+                lv[j] = m;
+            }
+        }
+    }
+    __syncthreads();
+    const uint32_t root = a.lvl_off[a.levels - 1];
+    uint32_t placed = 0, dead = 0;
+    uint2 ahead = lane < a.n ? a.in[lane] : make_uint2(0, (uint32_t)ISL_OP_NOOP << 8);
+    for (uint32_t base = 0; base < a.n; base += 32) {
+        const uint2 mine = ahead;                         // every warp walks the same requests and takes the same branches
+        ahead = base + 32 + lane < a.n ? a.in[base + 32 + lane] : make_uint2(0, (uint32_t)ISL_OP_NOOP << 8);
+        const uint32_t wp = mine.y & 0xFFu, wop = (mine.y >> 8) & 0xFFu;
+        uint32_t live = __ballot_sync(0xFFFFFFFFu, wop == ISL_OP_ALLOC && wp < n_profiles && !((dead >> wp) & 1u));
+        while (live) {
+            const uint32_t j = __ffs(live) - 1;
+            live &= live - 1;
+            const uint32_t p = __shfl_sync(0xFFFFFFFFu, mine.y, j) & 0xFFu;
+            if ((dead >> p) & 1u) continue;
+            const uint32_t key = tree[(size_t)p * a.T + root];
+            if (key == kInf) { dead |= 1u << p; continue; }
+            const uint32_t v = key & 0xFFFFFFu;
+            if (warp == 0) {                                 // the chain warp: the node's first GPU in range that admits p
+                const uint32_t g0 = max(a.lo, __ldg(a.node_off + a.nlo + v)), g1 = min(a.hi, __ldg(a.node_off + a.nlo + v + 1));
+                const uint32_t t = a.meta[v] >> 24;
+                for (uint32_t gb = g0; gb < g1; gb += 32) {
+                    const uint32_t g = gb + lane, o = g < g1 ? a.occ[g] : 0xFFu;
+                    const uint32_t hit = __ballot_sync(0xFFFFFFFFu, g < g1 && admits(t, p, o));
+                    if (!hit) continue;
+                    if (lane == __ffs(hit) - 1) {
+                        const uint32_t start = s_lut[(t * ISL_MAX_PROFILES + p) * 256 + o], size = s_sizes[t * ISL_MAX_PROFILES + p];
+                        const uint32_t o2 = o | ((((1u << size) - 1u) << start) & 0xFFu), wm = (1u << a.width[t]) - 1u;
+                        a.occ[g] = (uint8_t)o2;
+                        a.out[base + j] = pack_result(g, start, size, ISL_ST_PLACED);
+                        a.busy[v] += __popc(o2 & wm) - __popc(o & wm);
+                        s_ev[0] = o; s_ev[1] = o2;
+                    }
+                    ++placed;
+                    break;
+                }
+            }
+            __syncthreads();
+            if (warp < n_profiles) {                          // warp q: profile q's fit count on the node, its leaf, its path to the root
+                const uint32_t q = warp, o = s_ev[0], o2 = s_ev[1], meta = a.meta[v], t = meta >> 24;
+                uint32_t* fq = a.fit + (size_t)q * a.Nr + v;
+                const uint32_t f = *fq + admits(t, q, o2) - admits(t, q, o);
+                uint32_t* tq = tree + (size_t)q * a.T;
+                const uint32_t leaf = nodefit_leaf(f, a.busy[v], meta & 0xFFFFFFu, s_sizes[t * ISL_MAX_PROFILES + q], a.most, v);
+                __syncwarp();
+                if (lane == 0) { *fq = f; tq[v] = leaf; }
+                uint32_t idx = v;
+                for (uint32_t k = 0; k + 1 < a.levels; ++k) {
+                    __syncwarp();
+                    const uint32_t m = redux_min_u32(tq[a.lvl_off[k] + (idx & ~31u) + lane]);
+                    idx >>= 5;
+                    const uint32_t old = tq[a.lvl_off[k + 1] + idx];
+                    if (old == m) break;                      // the ancestors keep their values
+                    __syncwarp();
+                    if (lane == 0) tq[a.lvl_off[k + 1] + idx] = m;
+                }
+            }
+            __syncthreads();
+        }
+    }
+    if (tid == 0) { atomicAdd(&a.ctrl->placed, (unsigned long long)placed); atomicAdd(&a.ctrl->steps, (unsigned long long)placed); }
+}
+
 }  // namespace isl

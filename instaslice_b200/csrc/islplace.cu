@@ -174,6 +174,12 @@ struct isl_engine {
         DevMem<uint8_t> stage;
         DevMem<unsigned long long> keys;
     } pre;
+    // node scoring (k_nodefit): the inventory's node offsets (isl_load_inventory), the per-profile min-trees when they do not fit in shared
+    // memory, the per-(profile, node) fit counts and the per-node busy / cap words, grown to the partition; the width of every table
+    struct NodeFit {
+        DevMem<uint32_t> node_off, tree, fit, nodes;
+        uint8_t width[kMaxTables] = {};
+    } nf;
     unsigned long long wait_ns = 20000000000ull;   // a starved device-side wait traps after this long (ISL_WAIT_SECONDS overrides the 20 s)
     uint32_t window = 0;             // causal window of stream calls (isl_set_causal_window): chunk c starts after chunk c - window is committed
     uint32_t spec_mode = ISL_SPEC_AUTO;     // speculative rounds (isl_set_speculation); ISL_SPEC=0|1 in the environment overrides
@@ -202,6 +208,10 @@ struct isl_engine {
 namespace {
 
 inline bool bestfit_family(uint32_t policy) { return policy == ISL_POLICY_BEST_FIT || policy == ISL_POLICY_MIN_FRAG; }
+inline bool node_scoring(uint32_t policy) { return policy == ISL_POLICY_MOST_ALLOCATED || policy == ISL_POLICY_LEAST_ALLOCATED; }
+// The policies whose batches one CTA resolves request by request (k_bestfit, k_nodefit): no latency kernels, no segment pipeline, no
+// partitioned calls or open streams, at most kBfMaxGpus GPUs
+inline bool request_major(uint32_t policy) { return bestfit_family(policy) || node_scoring(policy); }
 inline bool reversed(const isl_engine* e) { return e->cfg.policy == ISL_POLICY_RIGHT_TO_LEFT; }
 
 // A canonical GPU range [lo, hi) in storage order (ISL_POLICY_RIGHT_TO_LEFT stores the inventory reversed), or back: its own inverse
@@ -323,6 +333,18 @@ int run_few(isl_engine* e, uint32_t n, const SmallReqs& inl, uint2* d_out) {
     return ISL_OK;
 }
 
+// k_prepare of one batch in front of a request-major kernel: the frees and the default records, bracketed by ev[0] .. ev[1] under
+// ISL_FLAG_TIMING.
+int prepare_batch(isl_engine* e, uint32_t n, const uint2* d_in, uint2* d_out) {
+    const bool timing = e->cfg.flags & ISL_FLAG_TIMING;
+    if (timing) cudaEventRecord(e->ev[0], e->stream);
+    k_prepare<<<ceil_div(n, kTile), kTileThreads, 0, e->stream>>>(n, d_in, d_out, reinterpret_cast<uint32_t*>(e->d_occ.get()), e->G, e->lo, e->hi,
+                                                                  e->prof, e->d_tile_counts, e->d_ctrl, nullptr, nullptr, 0, 0);
+    if (int rc = check_launch(e, "k_prepare")) return rc;
+    if (timing) cudaEventRecord(e->ev[1], e->stream);
+    return ISL_OK;
+}
+
 // What run_bestfit and run_gangs share in front of k_bestfit: the class bitmaps (shared memory up to kBfSmemGpus GPUs of one table, else
 // global memory zeroed here), then k_prepare (frees + default records).  *smem = the dynamic shared memory k_bestfit needs.  An empty
 // range has no class bitmaps: k_prepare's default records are the whole answer.
@@ -337,13 +359,7 @@ int prepare_bestfit(isl_engine* e, uint32_t n, const uint2* d_in, uint2* d_out, 
         ISL_CUDA(e, e->d_bf_bitmaps.reserve(words));
         ISL_CUDA(e, cudaMemsetAsync(e->d_bf_bitmaps, 0, words * sizeof(uint32_t), e->stream));
     }
-    const bool timing = e->cfg.flags & ISL_FLAG_TIMING;
-    if (timing) cudaEventRecord(e->ev[0], e->stream);
-    k_prepare<<<ceil_div(n, kTile), kTileThreads, 0, e->stream>>>(n, d_in, d_out, reinterpret_cast<uint32_t*>(e->d_occ.get()), e->G, e->lo, e->hi,
-                                                                  e->prof, e->d_tile_counts, e->d_ctrl, nullptr, nullptr, 0, 0);
-    if (int rc = check_launch(e, "k_prepare")) return rc;
-    if (timing) cudaEventRecord(e->ev[1], e->stream);
-    return ISL_OK;
+    return prepare_batch(e, n, d_in, d_out);
 }
 
 // ISL_POLICY_BEST_FIT: frees + defaults, then the request-major class-bitmap kernel (one CTA).
@@ -355,6 +371,36 @@ int run_bestfit(isl_engine* e, uint32_t n, const uint2* d_in, uint2* d_out) {
     if (e->n_tables == 1) k_bestfit<false><<<1, kBfThreads, smem, e->stream>>>(n, d_in, d_out, e->d_occ, e->lo, e->hi, e->d_lut, e->prof, e->d_bf_bitmaps, e->d_ctrl, e->d_score, e->d_gtab, e->d_sizes, 1);
     else k_bestfit<true><<<1, kBfThreads, 0, e->stream>>>(n, d_in, d_out, e->d_occ, e->lo, e->hi, e->d_lut, e->prof, e->d_bf_bitmaps, e->d_ctrl, e->d_score, e->d_gtab, e->d_sizes, e->n_tables);
     if (int rc = check_launch(e, "k_bestfit")) return rc;
+    finish_batch(e, n, true);
+    return ISL_OK;
+}
+
+// ISL_POLICY_MOST_ALLOCATED / _LEAST_ALLOCATED: frees + defaults, then k_nodefit (one CTA) over the nodes the range touches.
+int run_nodefit(isl_engine* e, uint32_t n, const uint2* d_in, uint2* d_out) {
+    if (n == 0) return ISL_OK;
+    if (int rc = prepare_batch(e, n, d_in, d_out)) return rc;
+    if (e->hi == e->lo) { finish_batch(e, n, true); return ISL_OK; }     // empty range: ALLOCs NO_CAPACITY, every FREE outside it
+    // the nodes that own a GPU of [lo, hi) (node scoring stores the inventory in canonical order)
+    const uint32_t nlo = (uint32_t)(std::upper_bound(e->node_off.begin(), e->node_off.end(), e->lo) - e->node_off.begin()) - 1;
+    const uint32_t nhi = (uint32_t)(std::upper_bound(e->node_off.begin(), e->node_off.end(), e->hi - 1) - e->node_off.begin());
+    NodeFitArgs a{};
+    a.Nr = nhi - nlo;
+    for (uint32_t cnt = a.Nr;; cnt = ceil_div(cnt, 32)) {       // level sizes down to the root, each padded to 32 keys
+        a.lvl_off[a.levels] = a.T; a.lvl_cnt[a.levels++] = cnt;
+        a.T += (cnt + 31u) & ~31u;
+        if (cnt == 1) break;
+    }
+    auto& nf = e->nf;
+    const bool in_smem = a.Nr <= kNfSmemNodes;
+    ISL_CUDA(e, nf.fit.reserve((size_t)e->prof.n * a.Nr));
+    ISL_CUDA(e, nf.nodes.reserve((size_t)2 * a.Nr));
+    if (!in_smem) ISL_CUDA(e, nf.tree.reserve((size_t)e->prof.n * a.T));
+    a.in = d_in; a.out = d_out; a.occ = e->d_occ; a.gtab = e->d_gtab; a.lut = e->d_lut; a.sizes = e->d_sizes; a.node_off = nf.node_off;
+    a.tree = nf.tree; a.fit = nf.fit; a.busy = nf.nodes; a.meta = nf.nodes + a.Nr; a.ctrl = e->d_ctrl;
+    a.n = n; a.lo = e->lo; a.hi = e->hi; a.nlo = nlo; a.most = e->cfg.policy == ISL_POLICY_MOST_ALLOCATED;
+    memcpy(a.width, nf.width, sizeof a.width);
+    k_nodefit<<<1, kNfThreads, in_smem ? (size_t)e->prof.n * a.T * sizeof(uint32_t) : 0, e->stream>>>(a, e->prof.n);
+    if (int rc = check_launch(e, "k_nodefit")) return rc;
     finish_batch(e, n, true);
     return ISL_OK;
 }
@@ -635,7 +681,7 @@ struct Call {
     bool mixed = false;                     // one host batch of >= 4096 requests that mixes placeable profiles
 };
 
-enum class Path { few, small, chunks, bestfit, pipeline };
+enum class Path { few, small, chunks, bestfit, nodefit, pipeline };
 struct Route {
     Path path = Path::chunks;
     PipePlan plan; bool feed = false; uint32_t window = 0;      // Path::pipeline: its plan, feed mode, causal window
@@ -648,13 +694,13 @@ int route(isl_engine* e, const Call& c, uint64_t total, uint32_t n_chunks, Route
     const bool ring = c.xepoch != 0;        // partitioned inventory: tokens cross ranks through peer memory, pipeline mandatory
     if (ring && n_chunks > kMaxStreamChunks) return ISL_ERANGE;
     // latency paths: one batch of <= kSmallMax requests in one CTA (k_small); <= kFewMax inline requests on <= kFewGpus GPUs (k_few)
-    if (c.n_batches == 1 && !ring && n <= kSmallMax && !bestfit_family(e->cfg.policy) && !(flags & (ISL_FLAG_NO_SMALL | ISL_FLAG_FORCE_PIPELINE)) &&
+    if (c.n_batches == 1 && !ring && n <= kSmallMax && !request_major(e->cfg.policy) && !(flags & (ISL_FLAG_NO_SMALL | ISL_FLAG_FORCE_PIPELINE)) &&
         range > 0 && range <= (1u << 18)) {
         const bool few = c.src == Src::inline_host && n <= kFewMax && e->hi - (e->lo & ~15u) <= kFewGpus && !getenv("ISL_NO_FEW");
         r->path = few ? Path::few : Path::small;
         return ISL_OK;
     }
-    if (bestfit_family(e->cfg.policy)) { r->path = Path::bestfit; return ISL_OK; }
+    if (request_major(e->cfg.policy)) { r->path = node_scoring(e->cfg.policy) ? Path::nodefit : Path::bestfit; return ISL_OK; }
     const bool pipeline = ring || (!(flags & ISL_FLAG_NO_PIPELINE) && range > 0 && (n_chunks >= 2 || c.mixed || (flags & ISL_FLAG_FORCE_PIPELINE)));
     if (!pipeline) return ISL_OK;
     // the pipeline keeps one free-mask byte per GPU and batch: very long streams over large inventories go batch by batch
@@ -673,11 +719,13 @@ int route(isl_engine* e, const Call& c, uint64_t total, uint32_t n_chunks, Route
     return ISL_OK;
 }
 
-// Path::chunks / Path::bestfit: one batch after the other
-int run_batches(isl_engine* e, const Call& c, const uint2* d_in, uint2* d_out, bool bestfit) {
+// Path::chunks / Path::bestfit / Path::nodefit: one batch after the other
+int run_batches(isl_engine* e, const Call& c, const uint2* d_in, uint2* d_out, Path path) {
     uint64_t off = 0;
     for (uint32_t b = 0; b < c.n_batches; off += c.sizes[b++])
-        if (int rc = bestfit ? run_bestfit(e, c.sizes[b], d_in + off, d_out + off) : run_chunks(e, c.sizes[b], d_in + off, d_out + off, nullptr, nullptr)) return rc;
+        if (int rc = path == Path::bestfit   ? run_bestfit(e, c.sizes[b], d_in + off, d_out + off)
+                     : path == Path::nodefit ? run_nodefit(e, c.sizes[b], d_in + off, d_out + off)
+                                             : run_chunks(e, c.sizes[b], d_in + off, d_out + off, nullptr, nullptr)) return rc;
     return ISL_OK;
 }
 
@@ -789,7 +837,7 @@ int run_pipeline(isl_engine* e, const Call& c, const Route& r, const uint2* d_in
             ISL_CUDA(e, cudaStreamWaitEvent(e->stream, e->ev_feed_done, 0));
             ISL_CUDA(e, cudaMemcpyAsync(const_cast<uint2*>(d_in), h_in, (size_t)total * sizeof(uint2), cudaMemcpyHostToDevice, e->stream));
         }
-        return run_batches(e, c, d_in, d_out, false);
+        return run_batches(e, c, d_in, d_out, Path::chunks);
     }
     if (rc) return rc;
     if (feed) {     // the remaining batches, while the pipeline works on the first ones
@@ -844,7 +892,7 @@ int run_stream(isl_engine* e, const Call& c) {
     bool delivered = false;
     const int rc = r.path == Path::pipeline ? run_pipeline(e, c, r, d_in, d_out, total, n_chunks, &delivered)
                    : r.path == Path::small  ? run_small(e, n, d_in, nullptr, d_out)
-                                            : run_batches(e, c, d_in, d_out, r.path == Path::bestfit);
+                                            : run_batches(e, c, d_in, d_out, r.path);
     if (rc || !host) return rc;
     if (!delivered) ISL_CUDA(e, cudaMemcpyAsync(c.out, d_out, (size_t)total * sizeof(isl_result), cudaMemcpyDeviceToHost, e->stream));
     ISL_CUDA(e, cudaStreamSynchronize(e->stream));
@@ -989,8 +1037,9 @@ int isl_create(const isl_config* cfg, isl_engine** out) {
     *out = nullptr;
     if (cfg->abi_version != ISL_ABI_VERSION) return ISL_EINVAL;
     if (cfg->max_gpus == 0 || cfg->max_gpus > ISL_MAX_GPUS || cfg->max_batch == 0) return ISL_EINVAL;
-    if (cfg->policy > ISL_POLICY_MIN_FRAG) return ISL_EINVAL;
-    if (bestfit_family(cfg->policy) && cfg->max_gpus > kBfMaxGpus) return ISL_ERANGE;
+    if (cfg->policy > ISL_POLICY_LEAST_ALLOCATED) return ISL_EINVAL;
+    if (node_scoring(cfg->policy) && (cfg->flags & ISL_FLAG_ALL_NODES)) return ISL_EINVAL;     // a pod on every node: no node to choose
+    if (request_major(cfg->policy) && cfg->max_gpus > kBfMaxGpus) return ISL_ERANGE;
     if (cfg->quirks & ~ISL_QUIRKS_REF_EXACT) return ISL_EINVAL;
     isl_engine* e = new (std::nothrow) isl_engine;
     if (!e) return ISL_ENOMEM;
@@ -1018,7 +1067,7 @@ int isl_create(const isl_config* cfg, isl_engine** out) {
         cudaFuncAttributes fa;
         const void* kernels[] = {(const void*)k_prepare, (const void*)k_partition, (const void*)k_set_flag, (const void*)k_few, (const void*)k_build_lut, (const void*)k_eval_starts,
                                  (const void*)k_free_spans, (const void*)k_capacity, (const void*)k_sweep_count, (const void*)k_sweep_scatter, (const void*)k_commit, (const void*)k_bestfit<false>, (const void*)k_bestfit<true>,
-                                 (const void*)k_bestfit<false, true>, (const void*)k_bestfit<true, true>, (const void*)k_victim_map, (const void*)k_preempt,
+                                 (const void*)k_bestfit<false, true>, (const void*)k_bestfit<true, true>, (const void*)k_victim_map, (const void*)k_preempt, (const void*)k_nodefit,
                                  (const void*)k_chain<1>, (const void*)k_chain<2>, (const void*)k_chain<4>, (const void*)k_small<1>, (const void*)k_small<2>, (const void*)k_small<4>};
         const void* pipes[] = {(const void*)k_pipeline<1, false, false>, (const void*)k_pipeline<1, true, false>, (const void*)k_pipeline<2, false, false>, (const void*)k_pipeline<2, true, false>,
                                (const void*)k_pipeline<4, false, false>, (const void*)k_pipeline<4, true, false>,
@@ -1033,6 +1082,8 @@ int isl_create(const isl_config* cfg, isl_engine** out) {
         for (const void* k : {(const void*)k_bestfit<false>, (const void*)k_bestfit<false, true>})
             ISL_TRY(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(256 * (kBfSmemGpus / 32 + kBfSmemGpus / 1024) * sizeof(uint32_t))));
         for (const void* k : pipes) ISL_TRY(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kPipeSmem));
+        ISL_TRY(cudaFuncSetAttribute((const void*)k_nodefit, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                     (int)(ISL_MAX_PROFILES * (kNfSmemNodes + 64 + 32 + 32) * sizeof(uint32_t))));
         int optin = 0;          // k_preempt's share of the partition: up to what the device lets one CTA have
         ISL_TRY(cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev));
         ISL_TRY(cudaFuncGetAttributes(&fa, k_preempt));
@@ -1140,6 +1191,12 @@ static int load_tables(isl_engine* e, uint32_t n_tables, uint32_t n, const isl_p
             }
         }
     e->n_cand_slots = c <= 32 ? 1 : (c <= 64 ? 2 : 4);
+    for (uint32_t t = 0; t < kMaxTables; ++t) {      // node scoring: a table's width in memory slices, the largest start + size of its rows
+        e->nf.width[t] = 0;
+        for (uint32_t p = 0; t < n_tables && p < n; ++p)
+            for (uint32_t k = 0; k < e->rows_all[t][p].n_starts; ++k)
+                e->nf.width[t] = std::max<uint8_t>(e->nf.width[t], e->rows_all[t][p].starts[k] + e->rows_all[t][p].size);
+    }
     ISL_CUDA(e, cudaMemsetAsync(e->d_feas, 0, ISL_MAX_TABLES * 256 * sizeof(uint16_t), e->stream));
     for (uint32_t t = 0; t < n_tables; ++t) {
         DevProfiles dp{};
@@ -1234,6 +1291,10 @@ int isl_load_inventory(isl_engine* e, uint32_t n_nodes, const uint32_t* node_off
     std::vector<uint8_t> rev;
     if (e->prof.flip) { rev.assign(occ, occ + G); std::reverse(rev.begin(), rev.end()); occ = rev.data(); }
     ISL_CUDA(e, cudaMemcpyAsync(e->d_occ, occ, G, cudaMemcpyHostToDevice, e->stream));
+    if (node_scoring(e->cfg.policy)) {      // k_nodefit finds the nodes of a range through them
+        ISL_CUDA(e, e->nf.node_off.replace((size_t)n_nodes + 1));
+        ISL_CUDA(e, cudaMemcpyAsync(e->nf.node_off, node_off, ((size_t)n_nodes + 1) * sizeof(uint32_t), cudaMemcpyHostToDevice, e->stream));
+    }
     ISL_CUDA(e, cudaStreamSynchronize(e->stream));
     e->have_inventory = true;
     return ISL_OK;
@@ -1314,6 +1375,7 @@ int isl_place_gangs(isl_engine* e, uint32_t n_gangs, const uint32_t* gang_off, c
     const uint32_t n = n_gangs ? gang_off[n_gangs] : 0;
     if (n && (!in || !out)) return ISL_EINVAL;
     if (e->cfg.flags & ISL_FLAG_ALL_NODES) return ISL_EINVAL;      // one pod on every node with capacity: no all-or-nothing meaning
+    if (node_scoring(e->cfg.policy)) return ISL_EINVAL;            // gangs under node scoring are not implemented
     if (n > e->cfg.max_batch) return ISL_ERANGE;
     Entry guard(e, Needs::ready, n);
     if (guard.rc) return guard.rc;
@@ -1497,7 +1559,7 @@ int isl_place_stream_partitioned(isl_engine* e, uint32_t n_batches, const uint32
     Entry guard(e, Needs::ready, total);
     if (guard.rc) return guard.rc;
     if (total == 0) return ISL_OK;
-    if (bestfit_family(e->cfg.policy) || reversed(e)) return ISL_EINVAL;        // best-fit / right-to-left do not partition
+    if (request_major(e->cfg.policy) || reversed(e)) return ISL_EINVAL;         // request-major / right-to-left policies do not partition
     return run_stream(e, Call{n_batches, sizes, Src::device, d_in, d_out, stream_id});
 }
 
@@ -1513,7 +1575,7 @@ int isl_place_batch_partitioned(isl_engine* e, uint32_t n, const void* d_in, voi
     Entry guard(e, Needs::ready, n);
     if (guard.rc) return guard.rc;
     if (n == 0) return ISL_OK;
-    if (bestfit_family(e->cfg.policy) || reversed(e)) return ISL_EINVAL;        // best-fit / right-to-left do not partition
+    if (request_major(e->cfg.policy) || reversed(e)) return ISL_EINVAL;         // request-major / right-to-left policies do not partition
     return run_chunks(e, n, static_cast<const uint2*>(d_in), static_cast<uint2*>(d_out), static_cast<const uint32_t*>(d_heads_in),
                       static_cast<uint32_t*>(d_heads_out));
 }
@@ -1713,7 +1775,7 @@ int isl_stream_open(isl_engine* e, uint32_t max_batches) {
     if (!e || max_batches == 0 || max_batches > kMaxStreamChunks) return ISL_EINVAL;
     Entry guard(e, Needs::ready);
     if (guard.rc) return guard.rc;
-    if (bestfit_family(e->cfg.policy)) return ISL_EINVAL;
+    if (request_major(e->cfg.policy)) return ISL_EINVAL;
     // a tool that serialises kernels would starve a resident kernel that waits for kernels launched after it: refuse instead of hanging
     // until the device-side trap (callers fall back to isl_place_batch per batch)
     if (getenv("ISL_NO_FEED") || kernels_serialised()) {

@@ -23,6 +23,7 @@ GPU_NONE = 0xFFFFFFFF
 PROFILE_UNKNOWN = 0xFF
 OK, EINVAL, ENOMEM, ECUDA, ESTATE, ERANGE = 0, -1, -2, -3, -4, -5
 POLICY_FIRST_FIT, POLICY_BEST_FIT, POLICY_RIGHT_TO_LEFT, POLICY_MIN_FRAG = 0, 1, 2, 3
+POLICY_MOST_ALLOCATED, POLICY_LEAST_ALLOCATED = 4, 5     # node scoring: the kube-scheduler's NodeResourcesFit strategies
 QUIRK_STRICT_BOUND, QUIRK_POW2_ONLY = 1, 2
 QUIRKS_REF_EXACT, QUIRKS_FIXED = 3, 0
 OP_ALLOC, OP_FREE, OP_NOOP = 0, 1, 2

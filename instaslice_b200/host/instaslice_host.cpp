@@ -22,9 +22,9 @@ AllocationDetails FirstFitPolicy::SetAllocationDetails(const std::string& profil
     return a;
 }
 
-InstasliceReconciler::InstasliceReconciler(uint32_t quirks, uint32_t max_gpus, uint32_t max_batch) {
+InstasliceReconciler::InstasliceReconciler(uint32_t quirks, uint32_t max_gpus, uint32_t max_batch, uint32_t policy) {
     isl_config cfg{};
-    cfg.abi_version = ISL_ABI_VERSION; cfg.policy = ISL_POLICY_FIRST_FIT; cfg.quirks = quirks; cfg.device = -1;
+    cfg.abi_version = ISL_ABI_VERSION; cfg.policy = policy; cfg.quirks = quirks; cfg.device = -1;
     cfg.max_gpus = max_gpus; cfg.max_batch = max_batch;
     check(isl_create(&cfg, &h_), nullptr, "isl_create");
 }

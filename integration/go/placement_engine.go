@@ -52,8 +52,24 @@ func hasOrphans(list *inferencev1alpha1.InstasliceList) bool {
 	return false
 }
 
+// Engine policies (isl_config.policy): which GPU, or which node, a pod goes to.  The AllocationPolicy hook still packs the answer.
+const (
+	PolicyFirstFit       = uint32(C.ISL_POLICY_FIRST_FIT)
+	PolicyBestFit        = uint32(C.ISL_POLICY_BEST_FIT)
+	PolicyRightToLeft    = uint32(C.ISL_POLICY_RIGHT_TO_LEFT)
+	PolicyMinFrag        = uint32(C.ISL_POLICY_MIN_FRAG)
+	PolicyMostAllocated  = uint32(C.ISL_POLICY_MOST_ALLOCATED)  // NodeResourcesFit MostAllocated: pack onto the fullest nodes
+	PolicyLeastAllocated = uint32(C.ISL_POLICY_LEAST_ALLOCATED) // NodeResourcesFit LeastAllocated: spread over the emptiest nodes
+)
+
 func NewPlacementEngine(maxGPUs, maxBatch uint32) (*PlacementEngine, error) {
-	cfg := C.isl_config{abi_version: C.ISL_ABI_VERSION, policy: C.ISL_POLICY_FIRST_FIT, quirks: C.ISL_QUIRKS_REF_EXACT,
+	return NewPlacementEngineWithPolicy(maxGPUs, maxBatch, PolicyFirstFit)
+}
+
+// NewPlacementEngineWithPolicy creates the engine with one of the Policy* values, e.g. PolicyMostAllocated so that the cluster
+// autoscaler can drain the nodes MIG pods leave empty, or PolicyLeastAllocated to spread inference replicas.
+func NewPlacementEngineWithPolicy(maxGPUs, maxBatch, policy uint32) (*PlacementEngine, error) {
+	cfg := C.isl_config{abi_version: C.ISL_ABI_VERSION, policy: C.uint32_t(policy), quirks: C.ISL_QUIRKS_REF_EXACT,
 		device: -1, max_gpus: C.uint32_t(maxGPUs), max_batch: C.uint32_t(maxBatch)}
 	var h *C.isl_engine
 	if rc := C.isl_create(&cfg, &h); rc != C.ISL_OK {
