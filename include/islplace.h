@@ -96,8 +96,9 @@ extern "C" {
  *   6. Accepted by isl_place_batch, _range, _device, isl_place_stream, _device (one batch after the other), isl_what_if, isl_capacity,
  *      isl_free_batch, isl_eval_starts, isl_set_partition, per-node tables and isl_preempt (whose scan order is ascending canonical).
  *   7. isl_create: ISL_EINVAL with ISL_FLAG_ALL_NODES (a pod placed on every node has no node to choose), ISL_ERANGE for
- *      max_gpus > 2^20.  ISL_EINVAL from isl_place_batch_partitioned, isl_place_stream_partitioned, isl_stream_open and
- *      isl_place_gangs.
+ *      max_gpus > 2^20.  isl_load_inventory: ISL_ERANGE for more than 2^20 nodes, empty nodes included (the nodes, not the GPUs,
+ *      are the leaves of the score trees); the previous inventory stays loaded.  ISL_EINVAL from isl_place_batch_partitioned,
+ *      isl_place_stream_partitioned, isl_stream_open and isl_place_gangs.
  * On an inventory of one node both give exactly ISL_POLICY_FIRST_FIT's records and occupancy. */
 #define ISL_POLICY_MOST_ALLOCATED  4u
 #define ISL_POLICY_LEAST_ALLOCATED 5u
@@ -235,7 +236,9 @@ int  isl_set_node_tables(isl_engine* e, uint32_t n_nodes, const uint8_t* table_o
 /* Replaces the occupancy rebuild (:306-328) for every GPU of every node.
  * node_off has n_nodes+1 entries (node i owns GPUs [node_off[i], node_off[i+1]));
  * occ has node_off[n_nodes] bytes.  This is also "resume": the CR is the checkpoint.
- * It resets the partition to [0, G), every node to table 0 (isl_set_node_tables) and drops a snapshot (isl_snapshot_occupancy). */
+ * It resets the partition to [0, G), every node to table 0 (isl_set_node_tables) and drops a snapshot (isl_snapshot_occupancy).
+ * ISL_ERANGE: node_off[n_nodes] > max_gpus, or more than 2^20 nodes (empty ones included) on a node-scoring engine; a refused
+ * call leaves the previous inventory, partition and snapshot in place. */
 int  isl_load_inventory(isl_engine* e, uint32_t n_nodes, const uint32_t* node_off, const uint8_t* occ);
 int  isl_read_occupancy(isl_engine* e, uint8_t* out /* G bytes */);
 /* Incremental sync: overwrite the occupancy bytes of canonical GPUs [first_gpu, first_gpu + n) — what the shim does

@@ -2439,7 +2439,9 @@ __global__ void __launch_bounds__(kPreThreads, 1) k_preempt(PreemptArgs a, DevPr
 // ---------------------------------------------------------------------------------------------
 constexpr uint32_t kNfThreads = 32 * ISL_MAX_PROFILES;   // one warp per profile
 constexpr uint32_t kNfSmemNodes = 2048;                  // up to here the trees live in shared memory (16 x 2 176 words = 136 KiB)
-constexpr uint32_t kNfMaxLevels = 5;                     // 32^4 leaves >= kBfMaxGpus nodes
+constexpr uint32_t kNfMaxNodes = 1u << 20;              // isl_load_inventory's limit for node scoring: empty nodes count, so not kBfMaxGpus
+constexpr uint32_t kNfMaxLevels = 5;                     // 32^4 leaves >= kNfMaxNodes nodes
+static_assert((1ull << (5 * (kNfMaxLevels - 1))) >= kNfMaxNodes, "a range of kNfMaxNodes nodes needs more tree levels");
 
 struct NodeFitArgs {            // kernel parameter (by value)
     const uint2* in;

@@ -1280,6 +1280,9 @@ int isl_load_inventory(isl_engine* e, uint32_t n_nodes, const uint32_t* node_off
     const uint32_t G = node_off[n_nodes];
     if (G == 0 || !occ) return ISL_EINVAL;
     if (G > e->cfg.max_gpus) return ISL_ERANGE;
+    // k_nodefit's min-trees have kNfMaxLevels levels over the nodes of a range, empty nodes included: refused here, before the guard,
+    // so that the previous inventory stays in place and an accepted inventory can always be placed on
+    if (node_scoring(e->cfg.policy) && n_nodes > kNfMaxNodes) return ISL_ERANGE;
     Entry guard(e, Needs::nothing);
     if (guard.rc) return guard.rc;
     e->node_off.assign(node_off, node_off + n_nodes + 1);

@@ -24,6 +24,7 @@ PROFILE_UNKNOWN = 0xFF
 OK, EINVAL, ENOMEM, ECUDA, ESTATE, ERANGE = 0, -1, -2, -3, -4, -5
 POLICY_FIRST_FIT, POLICY_BEST_FIT, POLICY_RIGHT_TO_LEFT, POLICY_MIN_FRAG = 0, 1, 2, 3
 POLICY_MOST_ALLOCATED, POLICY_LEAST_ALLOCATED = 4, 5     # node scoring: the kube-scheduler's NodeResourcesFit strategies
+NODE_SCORING_MAX_NODES = 1 << 20                         # isl_load_inventory on a node-scoring engine: ERANGE beyond
 QUIRK_STRICT_BOUND, QUIRK_POW2_ONLY = 1, 2
 QUIRKS_REF_EXACT, QUIRKS_FIXED = 3, 0
 OP_ALLOC, OP_FREE, OP_NOOP = 0, 1, 2
@@ -268,7 +269,9 @@ class Engine:
         self._check(self._lib.isl_set_node_tables(self._h, len(node_table), _ptr(node_table)), "isl_set_node_tables")
 
     def load_inventory(self, node_off, occ):
-        node_off = np.ascontiguousarray(node_off, dtype=np.uint32)
+        """Raises ``EngineError`` with code ``ERANGE`` for more GPUs than ``max_gpus``, and on a node-scoring engine for more than
+        ``NODE_SCORING_MAX_NODES`` nodes (empty ones count); the engine then keeps its previous inventory."""
+        node_off =np.ascontiguousarray(node_off, dtype=np.uint32)
         occ = np.ascontiguousarray(occ, dtype=np.uint8)
         assert len(occ) == int(node_off[-1])
         self._check(self._lib.isl_load_inventory(self._h, len(node_off) - 1, _ptr(node_off), _ptr(occ)), "isl_load_inventory")
