@@ -145,6 +145,7 @@ typedef struct isl_config {
                                        node that has capacity (state effect); the record reports the first node.  One restricted pass per node —
                                        a compatibility mode for parity studies, not a fast path.  isl_place_batch_range and isl_what_if
                                        follow it; the stream calls and isl_place_batch_device place each pod once, isl_place_gangs is EINVAL */
+#define ISL_FLAG_GANG_ONE_NODE 64u  /* isl_place_gangs puts every member of a gang on ONE node (see isl_place_gangs); every other call is unchanged */
 
 /* One Migplacement row (api/v1alpha1/instaslice_types.go:23-29).  `size` is
  * Placements[0].Size (:334); `starts` is [p.Start for p in Placements] in CRD
@@ -305,7 +306,25 @@ int  isl_place_batch_range(isl_engine* e, uint32_t lo, uint32_t hi, uint32_t n, 
  * A call whose gangs all have one member equals isl_place_batch on the same requests, records and occupancy.  The gangs are resolved
  * request by request (the best-fit kernel's loop, DESIGN.md 4.6): first-fit gangs do not use the segment pipeline.
  * ISL_EINVAL: malformed offsets, NULL buffers, an engine created with ISL_FLAG_ALL_NODES or a node-scoring policy.  ISL_ERANGE: n > max_batch, or a partition
- * that is empty or holds more than 2^20 GPUs.  ISL_ESTATE: no profiles or inventory, or an open stream. */
+ * that is empty or holds more than 2^20 GPUs.  ISL_ESTATE: no profiles or inventory, or an open stream.
+ *
+ * One-node gangs (ISL_FLAG_GANG_ONE_NODE): pods that talk to each other (a job's workers, a pipeline-parallel deployment) exchange data
+ * through host shared memory on one node and through the network across nodes; MIG instances have no peer-to-peer path.  On an engine
+ * created with the flag:
+ *   G1. Rules 1, 2 (FREEs first, NOOPs ignored, gangs in array order), 3 and 5 hold unchanged; rule 6 with the refusals of G5.
+ *   G2. A gang commits on the FIRST node, in the engine's scan order (ascending canonical; descending under ISL_POLICY_RIGHT_TO_LEFT), on
+ *       which all of its ALLOC members fit.  Inside that node the members are resolved in order by the engine's policy restricted to the
+ *       node's GPUs inside the partition: first-fit takes the first admitting GPU, right-to-left the last, best-fit and min-frag the
+ *       minimum of their score with ties to scan order.  A node the partition cuts offers only its GPUs inside the partition.
+ *   G3. Failure record (instead of rule 4): let D be the largest number of leading ALLOC members that any node can place on its own.  If
+ *       no node takes the whole gang, the ALLOC member at position D (counting ALLOC members from 0) gets its usual record (NO_CAPACITY,
+ *       or BAD_PROFILE for an unknown profile) and every other ALLOC member reports ISL_ST_GANG_ABORTED with the unplaced default
+ *       record.  On an inventory of one node this is rule 4.
+ *   G4. Consequences: on a one-node inventory, or a partition inside one node, a flagged call equals the unflagged one (records and
+ *       occupancy, every policy).  With gangs of one, a flagged ISL_POLICY_FIRST_FIT or _RIGHT_TO_LEFT engine equals isl_place_batch.
+ *   G5. isl_create: ISL_EINVAL for the flag with ISL_FLAG_ALL_NODES or a node-scoring policy.  isl_place_gangs keeps every code above,
+ *       the 2^20-GPU partition cap included.  Every other entry point returns exactly what it returns on an unflagged engine.
+ *   G6. The flag applies to every gang of the engine: choosing node locality per gang would need another entry point, and there is none. */
 int  isl_place_gangs(isl_engine* e, uint32_t n_gangs, const uint32_t* gang_off, const isl_request* in, isl_result* out);
 
 /* 8 bytes: one running allocation that MAY be evicted (isl_preempt). */

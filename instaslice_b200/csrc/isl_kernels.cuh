@@ -2579,4 +2579,173 @@ __global__ void __launch_bounds__(kNfThreads, 1) k_nodefit(NodeFitArgs a, uint32
     if (tid == 0) { atomicAdd(&a.ctrl->placed, (unsigned long long)placed); atomicAdd(&a.ctrl->steps, (unsigned long long)placed); }
 }
 
+// ---------------------------------------------------------------------------------------------
+// k_gangnode: isl_place_gangs on an engine created with ISL_FLAG_GANG_ONE_NODE (DESIGN.md 4.9): every gang commits on the first node, in
+// the engine's scan order (storage order: ascending canonical, descending under ISL_POLICY_RIGHT_TO_LEFT), that takes all of its ALLOC
+// members.  One cooperative launch per call behind k_prepare (frees and default records).  CTA c owns the partition's nodes
+// [cta_node[c], cta_node[c + 1]) (whole nodes, balanced by GPU count on the host) and keeps their occupancy bytes and a scratch copy in
+// shared memory (global memory when a share is too large for it).  Per gang:
+//   evaluate  one warp per node: copy the node's bytes to the scratch copy and count its free slices; a node with fewer free slices than
+//             the gang's members need on its table is skipped (pass 0 only).  Otherwise the warp resolves the members in order on the
+//             scratch copy, each one a warp min over the node's GPUs of score(t, p, o) << 24 | position (k_bestfit's lut and score tables; a
+//             zero score table is first-fit).  Key: the node index for a success, else bit 63 | (2^31 - 1 - depth) << 32 | node.
+//   reduce    warp, CTA, then grid (grid.sync, per-CTA minima double-buffered by round parity): the smallest key is the first node in scan
+//             order that takes the whole gang, or, with no such node, the deepest failure.  When the winner of pass 0 is a failure every
+//             node is evaluated again without the filter (pass 1), since the skipped nodes' depths are unknown.
+//   commit    the warp 0 of the CTA that owns the winning node resolves the members again on the live bytes and writes the PLACED records
+//             and the occupancy; a failure: CTA 0 reports every ALLOC member except the one at depth D GANG_ABORTED (that one keeps
+//             k_prepare's NO_CAPACITY or BAD_PROFILE record).
+// ---------------------------------------------------------------------------------------------
+constexpr uint32_t kGnThreads = 512;
+constexpr uint32_t kGnMaxCtas = 160;                    // CTAs of one launch (at most one per SM)
+constexpr unsigned long long kGnFail = 1ull << 63;
+
+struct GangNodeArgs {           // kernel parameter (by value)
+    const uint2* in;            // requests (isl_request)
+    uint2* out;                 // records: k_prepare's defaults, overwritten for the gang members
+    uint8_t* occ;               // live occupancy (storage order)
+    const uint8_t* gtab;        // table of every GPU's node (storage order)
+    const uint8_t* lut;         // [table][profile][occ]: first legal start or ISL_START_NONE
+    const uint8_t* score;       // [table][profile][occ]: what the policy minimises; zero for first-fit and right-to-left
+    const uint8_t* sizes;       // [table][profile]
+    const uint32_t* node_off;   // node offsets of the inventory in storage order
+    const uint32_t* gang_off;   // n_gangs + 1
+    uint8_t* scratch;           // Gr bytes: the scratch copies when the shares are in global memory
+    unsigned long long* keys;   // [2][gridDim.x] per-CTA minima
+    Ctrl* ctrl;
+    uint32_t n_gangs, n_tables, lo, hi, nlo;   // the partition [lo, hi) in storage order, its first node
+    uint32_t share;             // bytes of the largest share when the shares live in shared memory, 0 = global memory
+    uint32_t cta_node[kGnMaxCtas + 1];
+};
+
+// Warp-wide: resolve the ALLOC members of requests [r0, r1) in order on the `cnt` bytes `b` of one node of table t, the engine's policy
+// restricted to that node.  Returns how many leading ALLOC members were placed.  commit: b is the live share; the placements are also
+// written to the occupancy (storage index gbase + position) and reported PLACED.
+__device__ uint32_t gangnode_resolve(const GangNodeArgs& a, const DevProfiles& prof, uint8_t* b, uint32_t cnt, uint32_t gbase, uint32_t t,
+                                     uint32_t r0, uint32_t r1, bool commit, uint32_t lane) {
+    uint32_t depth = 0;
+    for (uint32_t base = r0; base < r1; base += 32) {
+        const uint2 q = base + lane < r1 ? a.in[base + lane] : make_uint2(0, (uint32_t)ISL_OP_NOOP << 8);
+        uint32_t live = __ballot_sync(0xFFFFFFFFu, ((q.y >> 8) & 0xFFu) == ISL_OP_ALLOC);
+        while (live) {
+            const uint32_t j = __ffs(live) - 1;
+            live &= live - 1;
+            const uint32_t p = __shfl_sync(0xFFFFFFFFu, q.y, j) & 0xFFu;
+            if (p >= prof.n) return depth;                  // an unknown profile fits nowhere
+            const uint32_t row = (t * ISL_MAX_PROFILES + p) * 256;
+            uint32_t key = kInf;
+            for (uint32_t g = lane; g < cnt; g += 32) {
+                const uint32_t o = b[g];
+                if (__ldg(a.lut + row + o) != ISL_START_NONE) key = min(key, ((uint32_t)__ldg(a.score + row + o) << 24) | g);
+            }
+            const uint32_t m = redux_min_u32(key);         // every lane has read its bytes: the owner may rewrite one below
+            if (m == kInf) return depth;
+            const uint32_t g = m & 0xFFFFFFu;
+            if ((g & 31u) == lane) {
+                const uint32_t o = b[g], start = __ldg(a.lut + row + o), size = __ldg(a.sizes + t * ISL_MAX_PROFILES + p);
+                const uint32_t o2 = o | ((((1u << size) - 1u) << start) & 0xFFu);
+                b[g] = (uint8_t)o2;
+                if (commit) {
+                    a.occ[gbase + g] = (uint8_t)o2;
+                    a.out[base + j] = pack_result(flip_gpu(gbase + g, prof.flip), start, size, ISL_ST_PLACED);
+                }
+            }
+            __syncwarp();
+            ++depth;
+        }
+    }
+    return depth;
+}
+
+__global__ void __launch_bounds__(kGnThreads, 1) k_gangnode(GangNodeArgs a, DevProfiles prof) {
+    extern __shared__ __align__(16) uint8_t gn_smem[];
+    __shared__ unsigned long long s_warp[kGnThreads / 32];
+    __shared__ unsigned long long s_win;
+    __shared__ uint32_t s_need[kMaxTables], s_allocs;
+    const uint32_t tid = threadIdx.x, lane = tid & 31u, warp = tid >> 5;
+    // node j of the partition owns the partition-local GPUs [nb(j), nb(j + 1)); a node the partition cuts keeps its GPUs inside it
+    auto nb = [&](uint32_t j) { return min(max(a.node_off[a.nlo + j], a.lo), a.hi) - a.lo; };
+    const uint32_t j0 = a.cta_node[blockIdx.x], j1 = a.cta_node[blockIdx.x + 1];
+    const uint32_t base = nb(j0), cnt = nb(j1) - base;
+    uint8_t* live = a.share ? gn_smem : a.occ + a.lo + base;             // committed bytes of the CTA's share
+    uint8_t* scr = a.share ? gn_smem + a.share : a.scratch + base;        // scratch copies of its nodes
+    if (a.share) for (uint32_t g = tid; g < cnt; g += kGnThreads) live[g] = a.occ[a.lo + base + g];
+    cooperative_groups::grid_group grid = cooperative_groups::this_grid();
+    uint32_t parity = 0, placed = 0;
+    for (uint32_t gi = 0; gi < a.n_gangs; ++gi) {
+        const uint32_t r0 = __ldg(a.gang_off + gi), r1 = __ldg(a.gang_off + gi + 1);
+        if (tid < kMaxTables) s_need[tid] = 0;
+        if (tid == 0) s_allocs = 0;
+        __syncthreads();                                    // also orders a commit of the previous gang before this gang's reads
+        uint32_t mine = 0;
+        for (uint32_t r = r0 + tid; r < r1; r += kGnThreads) {      // the slices the gang's ALLOCs take on a node of each table
+            const uint32_t y = a.in[r].y, p = y & 0xFFu;
+            if (((y >> 8) & 0xFFu) != ISL_OP_ALLOC) continue;
+            ++mine;
+            if (p < prof.n)
+                for (uint32_t t = 0; t < a.n_tables; ++t) atomicAdd(&s_need[t], (uint32_t)__ldg(a.sizes + t * ISL_MAX_PROFILES + p));
+        }
+        if (mine) atomicAdd(&s_allocs, mine);
+        __syncthreads();
+        const uint32_t allocs = s_allocs;
+        if (allocs == 0) continue;                          // FREEs and NOOPs only: k_prepare's records stand
+        unsigned long long win = ~0ull;
+        for (uint32_t pass = 0; pass < 2; ++pass) {
+            unsigned long long best = ~0ull;
+            for (uint32_t j = j0 + warp; j < j1; j += kGnThreads / 32) {
+                const uint32_t b0 = nb(j) - base, c = nb(j + 1) - base - b0;
+                if (c == 0) continue;                       // an empty node places nothing: depth 0, the floor of every failure
+                const uint32_t t = a.gtab[a.lo + base + b0] & (kMaxTables - 1);
+                uint32_t free_slices = 0;
+                for (uint32_t g = lane; g < c; g += 32) {
+                    const uint32_t o = live[b0 + g];
+                    scr[b0 + g] = (uint8_t)o;
+                    free_slices += 8u - __popc(o);
+                }
+                free_slices = __reduce_add_sync(0xFFFFFFFFu, free_slices);
+                if (pass == 0 && free_slices < s_need[t]) continue;
+                const uint32_t d = gangnode_resolve(a, prof, scr + b0, c, a.lo + base + b0, t, r0, r1, false, lane);
+                best = min(best, d == allocs ? (unsigned long long)j : kGnFail | ((unsigned long long)(0x7FFFFFFFu - d) << 32) | j);
+            }
+            best = warp_min_u64(best);
+            if (lane == 0) s_warp[warp] = best;
+            __syncthreads();
+            if (warp == 0) {
+                best = warp_min_u64(lane < kGnThreads / 32 ? s_warp[lane] : ~0ull);
+                if (lane == 0) a.keys[parity * gridDim.x + blockIdx.x] = best;
+            }
+            grid.sync();                                    // every CTA's minimum of this round is in keys[parity]
+            if (warp == 0) {
+                unsigned long long v = ~0ull;
+                for (uint32_t c = lane; c < gridDim.x; c += 32) v = min(v, __ldcg(a.keys + parity * gridDim.x + c));
+                v = warp_min_u64(v);
+                if (lane == 0) s_win = v;
+            }
+            __syncthreads();
+            win = s_win;
+            parity ^= 1u;
+            if (!(win & kGnFail)) break;                    // a node takes the whole gang: the skipped nodes could not have come first
+        }
+        if (!(win & kGnFail)) {
+            const uint32_t j = (uint32_t)win;
+            if (j >= j0 && j < j1 && warp == 0) {           // the owner commits on its live bytes
+                const uint32_t b0 = nb(j) - base, c = nb(j + 1) - base - b0;
+                gangnode_resolve(a, prof, live + b0, c, a.lo + base + b0, a.gtab[a.lo + base + b0] & (kMaxTables - 1), r0, r1, true, lane);
+                placed += allocs;
+            }
+        } else if (blockIdx.x == 0 && warp == 0) {          // ~0ull (no node evaluated) is depth 0 as well
+            const uint32_t D = 0x7FFFFFFFu - (uint32_t)((win >> 32) & 0x7FFFFFFFu);
+            uint32_t k = 0;                                 // ALLOC members before this block of 32
+            for (uint32_t r = r0; r < r1; r += 32) {
+                const uint32_t y = r + lane < r1 ? a.in[r + lane].y : (uint32_t)ISL_OP_NOOP << 8, p = y & 0xFFu;
+                const bool alloc = ((y >> 8) & 0xFFu) == ISL_OP_ALLOC;
+                const uint32_t ballot = __ballot_sync(0xFFFFFFFFu, alloc), rank = k + __popc(ballot & ((1u << lane) - 1u));
+                if (alloc && rank != D) a.out[r + lane] = pack_result(ISL_GPU_NONE, ISL_START_NONE, p < prof.n ? prof.rows[p].size : 0u, ISL_ST_GANG_ABORTED);
+                k += __popc(ballot);
+            }
+        }
+    }
+    if (tid == 0 && placed) { atomicAdd(&a.ctrl->placed, (unsigned long long)placed); atomicAdd(&a.ctrl->steps, (unsigned long long)placed); }
+}
+
 }  // namespace isl

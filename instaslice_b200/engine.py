@@ -30,6 +30,7 @@ QUIRKS_REF_EXACT, QUIRKS_FIXED = 3, 0
 OP_ALLOC, OP_FREE, OP_NOOP = 0, 1, 2
 ST_PLACED, ST_NO_CAPACITY, ST_BAD_PROFILE, ST_FREED, ST_BAD_SPAN, ST_NOOP, ST_GANG_ABORTED = 0, 1, 2, 3, 4, 5, 6
 FLAG_TIMING, FLAG_NO_PIPELINE, FLAG_FORCE_PIPELINE, FLAG_TRACE, FLAG_NO_SMALL, FLAG_ALL_NODES = 1, 2, 4, 8, 16, 32
+FLAG_GANG_ONE_NODE = 64     # isl_place_gangs puts every member of a gang on one node (include/islplace.h)
 SPEC_AUTO, SPEC_OFF, SPEC_ON = 0, 1, 2
 
 # ---- record layouts -------------------------------------------------------------------------
@@ -333,7 +334,9 @@ class Engine:
     def place_gangs(self, requests: np.ndarray, gang_off) -> np.ndarray:
         """All-or-nothing groups: gang i is ``requests[gang_off[i]:gang_off[i + 1]]`` (``gang_off[0] == 0``, no empty gang, the last
         offset is ``len(requests)``).  A gang commits only when every ALLOC member is placed; otherwise the first member that did not fit
-        keeps its record and every other ALLOC member reports ``ST_GANG_ABORTED`` (include/islplace.h)."""
+        keeps its record and every other ALLOC member reports ``ST_GANG_ABORTED`` (include/islplace.h).  On an engine created with
+        ``FLAG_GANG_ONE_NODE`` every gang lands on one node, the first in scan order that takes it whole, and the member at the depth no
+        node gets past keeps its record."""
         requests = np.ascontiguousarray(requests, dtype=REQUEST_DTYPE)
         gang_off = np.ascontiguousarray(gang_off, dtype=np.uint32)
         if len(gang_off) == 0 or int(gang_off[-1]) != len(requests):

@@ -22,10 +22,10 @@ AllocationDetails FirstFitPolicy::SetAllocationDetails(const std::string& profil
     return a;
 }
 
-InstasliceReconciler::InstasliceReconciler(uint32_t quirks, uint32_t max_gpus, uint32_t max_batch, uint32_t policy) {
+InstasliceReconciler::InstasliceReconciler(uint32_t quirks, uint32_t max_gpus, uint32_t max_batch, uint32_t policy, uint32_t flags) {
     isl_config cfg{};
     cfg.abi_version = ISL_ABI_VERSION; cfg.policy = policy; cfg.quirks = quirks; cfg.device = -1;
-    cfg.max_gpus = max_gpus; cfg.max_batch = max_batch;
+    cfg.max_gpus = max_gpus; cfg.max_batch = max_batch; cfg.flags = flags;
     check(isl_create(&cfg, &h_), nullptr, "isl_create");
 }
 InstasliceReconciler::~InstasliceReconciler() { if (h_) isl_destroy(h_); }

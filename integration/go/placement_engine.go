@@ -62,6 +62,11 @@ const (
 	PolicyLeastAllocated = uint32(C.ISL_POLICY_LEAST_ALLOCATED) // NodeResourcesFit LeastAllocated: spread over the emptiest nodes
 )
 
+// Engine flags (isl_config.flags) a controller may want.
+const (
+	FlagGangOneNode = uint32(C.ISL_FLAG_GANG_ONE_NODE) // PlaceGangs puts every gang on one node, the first in scan order that takes it
+)
+
 func NewPlacementEngine(maxGPUs, maxBatch uint32) (*PlacementEngine, error) {
 	return NewPlacementEngineWithPolicy(maxGPUs, maxBatch, PolicyFirstFit)
 }
@@ -69,8 +74,14 @@ func NewPlacementEngine(maxGPUs, maxBatch uint32) (*PlacementEngine, error) {
 // NewPlacementEngineWithPolicy creates the engine with one of the Policy* values, e.g. PolicyMostAllocated so that the cluster
 // autoscaler can drain the nodes MIG pods leave empty, or PolicyLeastAllocated to spread inference replicas.
 func NewPlacementEngineWithPolicy(maxGPUs, maxBatch, policy uint32) (*PlacementEngine, error) {
+	return NewPlacementEngineWithFlags(maxGPUs, maxBatch, policy, 0)
+}
+
+// NewPlacementEngineWithFlags also sets Flag* values, e.g. FlagGangOneNode so that the pods of a gang share a node (host shared memory
+// instead of the network).  isl_create refuses FlagGangOneNode with PolicyMostAllocated or PolicyLeastAllocated.
+func NewPlacementEngineWithFlags(maxGPUs, maxBatch, policy, flags uint32) (*PlacementEngine, error) {
 	cfg := C.isl_config{abi_version: C.ISL_ABI_VERSION, policy: C.uint32_t(policy), quirks: C.ISL_QUIRKS_REF_EXACT,
-		device: -1, max_gpus: C.uint32_t(maxGPUs), max_batch: C.uint32_t(maxBatch)}
+		device: -1, max_gpus: C.uint32_t(maxGPUs), max_batch: C.uint32_t(maxBatch), flags: C.uint32_t(flags)}
 	var h *C.isl_engine
 	if rc := C.isl_create(&cfg, &h); rc != C.ISL_OK {
 		return nil, fmt.Errorf("isl_create: %s", C.GoString(C.isl_strerror(rc)))
