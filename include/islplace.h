@@ -146,6 +146,8 @@ typedef struct isl_config {
                                        a compatibility mode for parity studies, not a fast path.  isl_place_batch_range and isl_what_if
                                        follow it; the stream calls and isl_place_batch_device place each pod once, isl_place_gangs is EINVAL */
 #define ISL_FLAG_GANG_ONE_NODE 64u  /* isl_place_gangs puts every member of a gang on ONE node (see isl_place_gangs); every other call is unchanged */
+#define ISL_FLAG_GANG_DISTINCT_NODES 128u  /* isl_place_gangs puts every member of a gang on a DIFFERENT node (see isl_place_gangs); every
+                                              other call is unchanged */
 
 /* One Migplacement row (api/v1alpha1/instaslice_types.go:23-29).  `size` is
  * Placements[0].Size (:334); `starts` is [p.Start for p in Placements] in CRD
@@ -324,7 +326,31 @@ int  isl_place_batch_range(isl_engine* e, uint32_t lo, uint32_t hi, uint32_t n, 
  *       occupancy, every policy).  With gangs of one, a flagged ISL_POLICY_FIRST_FIT or _RIGHT_TO_LEFT engine equals isl_place_batch.
  *   G5. isl_create: ISL_EINVAL for the flag with ISL_FLAG_ALL_NODES or a node-scoring policy.  isl_place_gangs keeps every code above,
  *       the 2^20-GPU partition cap included.  Every other entry point returns exactly what it returns on an unflagged engine.
- *   G6. The flag applies to every gang of the engine: choosing node locality per gang would need another entry point, and there is none. */
+ *   G6. The flag applies to every gang of the engine: choosing node locality per gang would need another entry point, and there is none.
+ *
+ * Distinct-node gangs (ISL_FLAG_GANG_DISTINCT_NODES): the replicas of a deployment on different nodes, so that one node or one GPU
+ * failing does not take down every replica (the kube-scheduler's required podAntiAffinity on kubernetes.io/hostname, which never applies
+ * to gated MIG pods).  On an engine created with the flag:
+ *   S1. Rules 1, 2 (FREEs first, NOOPs ignored, gangs in array order), 3 and 5 hold unchanged; rule 6 with the refusals of S6.
+ *   S2. Inside a gang the ALLOC members are resolved in order, each by the engine's policy restricted to the GPUs of the partition whose
+ *       node holds no earlier member of the SAME gang: first-fit takes the first admitting GPU in ascending canonical order,
+ *       right-to-left the last, best-fit and min-frag the minimum of their score with ties to scan order; the start inside the GPU is
+ *       the start search's.  A node the partition cuts counts as one node and offers only its GPUs inside the partition.  Nodes used by
+ *       earlier committed gangs are not excluded: the anti-affinity holds within one gang.
+ *   S3. Failure is rule 4 unchanged: the first member with no admitting GPU on an unused node gets its usual record (NO_CAPACITY, or
+ *       BAD_PROFILE for an unknown profile), the members after it are not tried, and every other ALLOC member reports
+ *       ISL_ST_GANG_ABORTED with the unplaced default record.  NO_CAPACITY may be reported while a node the gang already uses has room.
+ *   S4. The choice is greedy, member by member, not a matching (the kube-scheduler placing pods with required anti-affinity one at a
+ *       time): a gang can abort although some assignment to distinct nodes exists.  Node A admits 1g and 4g, node B only 1g: under
+ *       first-fit [1g, 4g] aborts (1g takes A) while [4g, 1g] places.  List the larger members of a gang first.
+ *   S5. Consequences: (a) with gangs of one, a flagged call equals isl_place_batch (records and occupancy, every policy); (b) the PLACED
+ *       members of a committed gang sit on pairwise distinct nodes (isl_gpu_to_node); (c) a gang with more ALLOC members than the
+ *       partition has non-empty nodes always aborts, so on a one-node inventory every gang of two or more ALLOC members aborts (when
+ *       member 0 places, member 1 reports NO_CAPACITY); (d) on an inventory of one-GPU nodes under ISL_QUIRKS_FIXED with gangs whose
+ *       profiles all take a whole GPU (size 8), a flagged call equals the unflagged one on every policy.
+ *   S6. isl_create: ISL_EINVAL for the flag with ISL_FLAG_GANG_ONE_NODE (they contradict each other), ISL_FLAG_ALL_NODES or a
+ *       node-scoring policy.  isl_place_gangs keeps every code above, the 2^20-GPU partition cap included.  Every other entry point
+ *       returns exactly what it returns on an unflagged engine.  The flag applies to every gang of the engine, as G6 says. */
 int  isl_place_gangs(isl_engine* e, uint32_t n_gangs, const uint32_t* gang_off, const isl_request* in, isl_result* out);
 
 /* 8 bytes: one running allocation that MAY be evicted (isl_preempt). */

@@ -2748,4 +2748,113 @@ __global__ void __launch_bounds__(kGnThreads, 1) k_gangnode(GangNodeArgs a, DevP
     if (tid == 0 && placed) { atomicAdd(&a.ctrl->placed, (unsigned long long)placed); atomicAdd(&a.ctrl->steps, (unsigned long long)placed); }
 }
 
+// ---------------------------------------------------------------------------------------------
+// k_gangspread: isl_place_gangs on an engine created with ISL_FLAG_GANG_DISTINCT_NODES (DESIGN.md 4.10): the ALLOC members of a gang are
+// resolved in order, each by the engine's policy restricted to the partition's GPUs whose node holds no earlier member of the same gang.
+// So no member ever sees another member's slices: a member's key on a GPU depends only on the committed bytes, and the kernel needs no
+// scratch copy and no rollback.  One cooperative launch per call behind k_prepare (frees and default records), with k_gangnode's layout:
+// CTA c owns the partition's nodes [cta_node[c], cta_node[c + 1]) and keeps their live bytes in shared memory, and its "node used" marks
+// next to them (both in global memory when a share is too large).  Per ALLOC member:
+//   choose    every CTA takes the minimum of score(t, p, o) << 24 | partition-local storage position over its GPUs not marked used
+//             (k_bestfit's lut and score tables; a zero score table is first-fit, and right-to-left is the ascending scan of its reversed
+//             storage); one grid.sync over the per-CTA minima (double-buffered by round parity) gives every CTA the member's GPU.
+//   mark      the CTA that owns that GPU marks its node's GPUs with the gang's tag and pushes (request, GPU) onto its stack of wins.
+// A member with no GPU ends the gang: it keeps k_prepare's record (NO_CAPACITY or BAD_PROFILE), CTA 0 reports every other ALLOC member
+// GANG_ABORTED, and no occupancy byte is written.  Otherwise every CTA writes the bytes and PLACED records of its stack.  A profile that
+// finds no GPU as a gang's first ALLOC member (no exclusion in force) is dead for the rest of the call: after the FREEs of k_prepare the
+// occupancy only grows.  Tags run 1..255 with the gang index; the marks are cleared once every 255 gangs.
+// ---------------------------------------------------------------------------------------------
+__global__ void __launch_bounds__(kGnThreads, 1) k_gangspread(GangNodeArgs a, DevProfiles prof, uint2* wins) {
+    extern __shared__ __align__(16) uint8_t gs_smem[];
+    __shared__ uint32_t s_warp[kGnThreads / 32];
+    __shared__ uint32_t s_win, s_nwins;
+    const uint32_t tid = threadIdx.x, lane = tid & 31u, warp = tid >> 5;
+    auto nb = [&](uint32_t j) { return min(max(a.node_off[a.nlo + j], a.lo), a.hi) - a.lo; };
+    const uint32_t j0 = a.cta_node[blockIdx.x], j1 = a.cta_node[blockIdx.x + 1];
+    const uint32_t base = nb(j0), cnt = nb(j1) - base;
+    uint8_t* live = a.share ? gs_smem : a.occ + a.lo + base;             // committed bytes of the CTA's share
+    uint8_t* mark = a.share ? gs_smem + a.share : a.scratch + base;       // tag of the gang whose member uses the GPU's node
+    if (a.share) for (uint32_t g = tid; g < cnt; g += kGnThreads) live[g] = a.occ[a.lo + base + g];
+    if (tid == 0) s_nwins = 0;
+    cooperative_groups::grid_group grid = cooperative_groups::this_grid();
+    uint32_t parity = 0, placed = 0, dead = 0;                            // dead: profiles no GPU of the partition admits any more
+    for (uint32_t gi = 0; gi < a.n_gangs; ++gi) {
+        const uint32_t r0 = __ldg(a.gang_off + gi), r1 = __ldg(a.gang_off + gi + 1), tag = 1u + gi % 255u;
+        if (tag == 1u) for (uint32_t g = tid; g < cnt; g += kGnThreads) mark[g] = 0;
+        __syncthreads();                                    // also orders the previous gang's commit before this gang's reads
+        uint32_t rank = 0, fail = kInf;                     // ALLOC members resolved so far; the rank of the one that found no GPU
+        for (uint32_t r = r0; r < r1; ++r) {
+            const uint32_t y = a.in[r].y, p = y & 0xFFu;
+            if (((y >> 8) & 0xFFu) != ISL_OP_ALLOC) continue;
+            uint32_t win = kInf;                            // an unknown or dead profile fails without a barrier: every CTA knows it
+            if (p < prof.n && !((dead >> p) & 1u)) {
+                uint32_t key = kInf;
+                for (uint32_t g = tid; g < cnt; g += kGnThreads) {
+                    if (mark[g] == tag) continue;
+                    const uint32_t o = live[g], t = a.n_tables > 1 ? a.gtab[a.lo + base + g] & (kMaxTables - 1) : 0u;
+                    const uint32_t row = (t * ISL_MAX_PROFILES + p) * 256;
+                    if (__ldg(a.lut + row + o) != ISL_START_NONE) key = min(key, ((uint32_t)__ldg(a.score + row + o) << 24) | (base + g));
+                }
+                key = redux_min_u32(key);
+                if (lane == 0) s_warp[warp] = key;
+                __syncthreads();
+                if (warp == 0) {
+                    key = redux_min_u32(lane < kGnThreads / 32 ? s_warp[lane] : kInf);
+                    if (lane == 0) a.keys[parity * gridDim.x + blockIdx.x] = key;
+                }
+                grid.sync();                                // every CTA's minimum of this member is in keys[parity]
+                if (warp == 0) {
+                    uint32_t v = kInf;
+                    for (uint32_t c = lane; c < gridDim.x; c += 32) v = min(v, (uint32_t)__ldcg(a.keys + parity * gridDim.x + c));
+                    v = redux_min_u32(v);
+                    if (lane == 0) s_win = v;
+                }
+                __syncthreads();
+                win = s_win;
+                parity ^= 1u;
+                if (win == kInf && rank == 0) dead |= 1u << p;
+            }
+            if (win == kInf) { fail = rank; break; }
+            const uint32_t pos = (win & 0xFFFFFFu) - base;
+            if (pos < cnt) {                                // this CTA owns the member's node: the node is used for the rest of the gang
+                uint32_t jl = j0, jh = j1;                  // nb(jl) <= base + pos < nb(jh): the last such jl is the non-empty node
+                while (jh - jl > 1) {
+                    const uint32_t mid = (jl + jh) / 2;
+                    if (nb(mid) - base <= pos) jl = mid; else jh = mid;
+                }
+                for (uint32_t g = nb(jl) - base + tid; g < nb(jl + 1) - base; g += kGnThreads) mark[g] = (uint8_t)tag;
+                if (tid == 0) wins[j0 + s_nwins++] = make_uint2(r, pos);  // one win per node of the CTA: the stack fits its nodes
+            }
+            __syncthreads();                                // the marks and the stack are in place before the next member's scan
+            ++rank;
+        }
+        if (fail == kInf) {                                 // commit: each CTA writes its members; their nodes, hence GPUs, differ
+            const uint32_t nw = s_nwins;
+            for (uint32_t k = tid; k < nw; k += kGnThreads) {
+                const uint2 w = wins[j0 + k];
+                const uint32_t g = w.y, p = a.in[w.x].y & 0xFFu, t = a.gtab[a.lo + base + g] & (kMaxTables - 1);
+                const uint32_t row = (t * ISL_MAX_PROFILES + p) * 256, o = live[g];
+                const uint32_t start = __ldg(a.lut + row + o), size = __ldg(a.sizes + t * ISL_MAX_PROFILES + p);
+                const uint32_t o2 = o | ((((1u << size) - 1u) << start) & 0xFFu);
+                live[g] = (uint8_t)o2;
+                a.occ[a.lo + base + g] = (uint8_t)o2;
+                a.out[w.x] = pack_result(flip_gpu(a.lo + base + g, prof.flip), start, size, ISL_ST_PLACED);
+            }
+            placed += nw;
+        } else if (blockIdx.x == 0 && warp == 0) {          // the member at rank `fail` keeps its record, every other ALLOC member aborts
+            uint32_t k = 0;                                 // ALLOC members before this block of 32
+            for (uint32_t r = r0; r < r1; r += 32) {
+                const uint32_t y = r + lane < r1 ? a.in[r + lane].y : (uint32_t)ISL_OP_NOOP << 8, p = y & 0xFFu;
+                const bool alloc = ((y >> 8) & 0xFFu) == ISL_OP_ALLOC;
+                const uint32_t ballot = __ballot_sync(0xFFFFFFFFu, alloc), rk = k + __popc(ballot & ((1u << lane) - 1u));
+                if (alloc && rk != fail) a.out[r + lane] = pack_result(ISL_GPU_NONE, ISL_START_NONE, p < prof.n ? prof.rows[p].size : 0u, ISL_ST_GANG_ABORTED);
+                k += __popc(ballot);
+            }
+        }
+        __syncthreads();                                    // every thread has read the stack's size
+        if (tid == 0) s_nwins = 0;
+    }
+    if (tid == 0 && placed) { atomicAdd(&a.ctrl->placed, (unsigned long long)placed); atomicAdd(&a.ctrl->steps, (unsigned long long)placed); }
+}
+
 }  // namespace isl

@@ -180,14 +180,16 @@ struct isl_engine {
         DevMem<uint32_t> node_off, tree, fit, nodes;
         uint8_t width[kMaxTables] = {};
     } nf;
-    // one-node gangs (ISL_FLAG_GANG_ONE_NODE, k_gangnode): the inventory's node offsets in storage order (host and device,
-    // isl_load_inventory), the scratch copies when the shares do not fit in shared memory, the per-CTA minima
+    // one-node and distinct-node gangs (ISL_FLAG_GANG_ONE_NODE, k_gangnode; ISL_FLAG_GANG_DISTINCT_NODES, k_gangspread): the inventory's
+    // node offsets in storage order (host and device, isl_load_inventory), the scratch copies (k_gangnode) or node-used marks
+    // (k_gangspread) when the shares do not fit in shared memory, the per-CTA minima, and k_gangspread's per-CTA stacks of wins
     struct GangNode {
         std::vector<uint32_t> off;
         DevMem<uint32_t> node_off;
         DevMem<uint8_t> scratch;
         DevMem<unsigned long long> keys;
-        int smem_optin = 0;          // dynamic shared memory one CTA of k_gangnode may have
+        DevMem<uint2> wins;
+        int smem_optin = 0;          // dynamic shared memory one CTA of k_gangnode or k_gangspread may have
     } gn;
     unsigned long long wait_ns = 20000000000ull;   // a starved device-side wait traps after this long (ISL_WAIT_SECONDS overrides the 20 s)
     uint32_t window = 0;             // causal window of stream calls (isl_set_causal_window): chunk c starts after chunk c - window is committed
@@ -429,10 +431,11 @@ int run_gangs(isl_engine* e, uint32_t n_gangs, const uint32_t* d_gang_off, uint3
     return ISL_OK;
 }
 
-// isl_place_gangs on an ISL_FLAG_GANG_ONE_NODE engine: frees + defaults, then one cooperative k_gangnode over the nodes the partition
-// touches.  Each CTA gets whole nodes, about Gr / grid GPUs (one CTA per SM at most, one per 512 GPUs below that, never more than nodes).
-int run_gangnode(isl_engine* e, uint32_t n_gangs, const uint32_t* d_gang_off, uint32_t n, const uint2* d_in, uint2* d_out) {
-    if (int rc = prepare_batch(e, n, d_in, d_out)) return rc;
+// The layout k_gangnode and k_gangspread share, over the nodes the partition touches: each CTA gets whole nodes, about Gr / grid GPUs
+// (one CTA per SM at most, one per 512 GPUs below that, never more than nodes), and 2 bytes per GPU of its share in shared memory when
+// they fit, else in global memory (gn.scratch).  Fills every field of `a`; *nodes = the nodes the partition touches.
+int gang_layout(isl_engine* e, const void* kernel, uint32_t n_gangs, const uint32_t* d_gang_off, const uint2* d_in, uint2* d_out,
+                GangNodeArgs& a, uint32_t* grid_out, size_t* smem_out, uint32_t* nodes) {
     auto& gn = e->gn;
     const uint32_t Gr = e->hi - e->lo;
     const uint32_t nlo = (uint32_t)(std::upper_bound(gn.off.begin(), gn.off.end(), e->lo) - gn.off.begin()) - 1;
@@ -440,7 +443,7 @@ int run_gangnode(isl_engine* e, uint32_t n_gangs, const uint32_t* d_gang_off, ui
     int sms = 0, per_sm = 0;
     ISL_CUDA(e, cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, e->device));
     const uint32_t grid = std::max(1u, std::min({(uint32_t)sms, kGnMaxCtas, ceil_div(Gr, 512), nhi - nlo}));
-    GangNodeArgs a{};
+    a = GangNodeArgs{};
     uint32_t share = 0;                                     // the largest share, in GPUs
     auto local = [&](uint32_t j) { return std::min(std::max(gn.off[nlo + j], e->lo), e->hi) - e->lo; };
     for (uint32_t c = 1; c <= grid; ++c) {
@@ -448,10 +451,10 @@ int run_gangnode(isl_engine* e, uint32_t n_gangs, const uint32_t* d_gang_off, ui
         a.cta_node[c] = c == grid ? nhi - nlo : (uint32_t)(std::lower_bound(gn.off.begin() + nlo, gn.off.begin() + nhi, target) - gn.off.begin()) - nlo;
         share = std::max(share, local(a.cta_node[c]) - local(a.cta_node[c - 1]));
     }
-    // the live bytes and the scratch copies of a share in shared memory when both fit, else in global memory
+    // the live bytes and the second byte per GPU (scratch copies or marks) of a share in shared memory when both fit, else in global memory
     size_t smem = ((size_t)share + 15) / 16 * 16 * 2;
     if (smem > (size_t)gn.smem_optin ||
-        cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_gangnode, kGnThreads, smem) != cudaSuccess || per_sm < 1) {
+        cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, kGnThreads, smem) != cudaSuccess || per_sm < 1) {
         cudaGetLastError();
         smem = 0;
         ISL_CUDA(e, gn.scratch.reserve(Gr));
@@ -460,12 +463,41 @@ int run_gangnode(isl_engine* e, uint32_t n_gangs, const uint32_t* d_gang_off, ui
     a.in = d_in; a.out = d_out; a.occ = e->d_occ; a.gtab = e->d_gtab; a.lut = e->d_lut; a.score = e->d_score; a.sizes = e->d_sizes;
     a.node_off = gn.node_off; a.gang_off = d_gang_off; a.scratch = gn.scratch; a.keys = gn.keys; a.ctrl = e->d_ctrl;
     a.n_gangs = n_gangs; a.n_tables = e->n_tables; a.lo = e->lo; a.hi = e->hi; a.nlo = nlo; a.share = (uint32_t)(smem / 2);
-    void* params[] = {&a, &e->prof};
-    const cudaError_t err = cudaLaunchCooperativeKernel((const void*)k_gangnode, dim3(grid), dim3(kGnThreads), params, smem, e->stream);
-    if (err != cudaSuccess) { cudaGetLastError(); snprintf(e->cuda_err, sizeof(e->cuda_err), "k_gangnode: %s", cudaGetErrorString(err)); return ISL_ECUDA; }
+    *grid_out = grid; *smem_out = smem; *nodes = nhi - nlo;
+    return ISL_OK;
+}
+
+int launch_gang_kernel(isl_engine* e, const void* kernel, const char* name, uint32_t grid, size_t smem, void** params, uint32_t n) {
+    const cudaError_t err = cudaLaunchCooperativeKernel(kernel, dim3(grid), dim3(kGnThreads), params, smem, e->stream);
+    if (err != cudaSuccess) { cudaGetLastError(); snprintf(e->cuda_err, sizeof(e->cuda_err), "%s: %s", name, cudaGetErrorString(err)); return ISL_ECUDA; }
     ++e->st.kernel_launches;
     finish_batch(e, n, true);
     return ISL_OK;
+}
+
+// isl_place_gangs on an ISL_FLAG_GANG_ONE_NODE engine: frees + defaults, then one cooperative k_gangnode (gang_layout).
+int run_gangnode(isl_engine* e, uint32_t n_gangs, const uint32_t* d_gang_off, uint32_t n, const uint2* d_in, uint2* d_out) {
+    if (int rc = prepare_batch(e, n, d_in, d_out)) return rc;
+    GangNodeArgs a;
+    uint32_t grid, nodes;
+    size_t smem;
+    if (int rc = gang_layout(e, (const void*)k_gangnode, n_gangs, d_gang_off, d_in, d_out, a, &grid, &smem, &nodes)) return rc;
+    void* params[] = {&a, &e->prof};
+    return launch_gang_kernel(e, (const void*)k_gangnode, "k_gangnode", grid, smem, params, n);
+}
+
+// isl_place_gangs on an ISL_FLAG_GANG_DISTINCT_NODES engine: frees + defaults, then one cooperative k_gangspread (gang_layout); CTA c
+// stacks its wins in gn.wins[cta_node[c] ..), at most one per node it owns.
+int run_gangspread(isl_engine* e, uint32_t n_gangs, const uint32_t* d_gang_off, uint32_t n, const uint2* d_in, uint2* d_out) {
+    if (int rc = prepare_batch(e, n, d_in, d_out)) return rc;
+    GangNodeArgs a;
+    uint32_t grid, nodes;
+    size_t smem;
+    if (int rc = gang_layout(e, (const void*)k_gangspread, n_gangs, d_gang_off, d_in, d_out, a, &grid, &smem, &nodes)) return rc;
+    ISL_CUDA(e, e->gn.wins.reserve(nodes));
+    uint2* wins = e->gn.wins;
+    void* params[] = {&a, &e->prof, &wins};
+    return launch_gang_kernel(e, (const void*)k_gangspread, "k_gangspread", grid, smem, params, n);
 }
 
 // The chunk path: k_prepare, then per chunk of kChunk requests k_partition, the two sweeps, k_chain and k_commit.  d_heads_in / d_heads_out
@@ -1089,6 +1121,9 @@ int isl_create(const isl_config* cfg, isl_engine** out) {
     if (node_scoring(cfg->policy) && (cfg->flags & ISL_FLAG_ALL_NODES)) return ISL_EINVAL;     // a pod on every node: no node to choose
     // one-node gangs choose the node by scan order: not with a pod on every node, nor with a policy that scores the nodes
     if ((cfg->flags & ISL_FLAG_GANG_ONE_NODE) && ((cfg->flags & ISL_FLAG_ALL_NODES) || node_scoring(cfg->policy))) return ISL_EINVAL;
+    // distinct-node gangs: the opposite of one-node gangs, and, like them, not with a pod on every node nor with node scoring
+    if ((cfg->flags & ISL_FLAG_GANG_DISTINCT_NODES) &&
+        ((cfg->flags & (ISL_FLAG_GANG_ONE_NODE | ISL_FLAG_ALL_NODES)) || node_scoring(cfg->policy))) return ISL_EINVAL;
     if (request_major(cfg->policy) && cfg->max_gpus > kBfMaxGpus) return ISL_ERANGE;
     if (cfg->quirks & ~ISL_QUIRKS_REF_EXACT) return ISL_EINVAL;
     isl_engine* e = new (std::nothrow) isl_engine;
@@ -1117,7 +1152,7 @@ int isl_create(const isl_config* cfg, isl_engine** out) {
         cudaFuncAttributes fa;
         const void* kernels[] = {(const void*)k_prepare, (const void*)k_partition, (const void*)k_set_flag, (const void*)k_few, (const void*)k_build_lut, (const void*)k_eval_starts,
                                  (const void*)k_free_spans, (const void*)k_capacity, (const void*)k_sweep_count, (const void*)k_sweep_scatter, (const void*)k_commit, (const void*)k_bestfit<false>, (const void*)k_bestfit<true>,
-                                 (const void*)k_bestfit<false, true>, (const void*)k_bestfit<true, true>, (const void*)k_victim_map, (const void*)k_preempt, (const void*)k_nodefit, (const void*)k_gangnode,
+                                 (const void*)k_bestfit<false, true>, (const void*)k_bestfit<true, true>, (const void*)k_victim_map, (const void*)k_preempt, (const void*)k_nodefit, (const void*)k_gangnode, (const void*)k_gangspread,
                                  (const void*)k_chain<1>, (const void*)k_chain<2>, (const void*)k_chain<4>, (const void*)k_small<1>, (const void*)k_small<2>, (const void*)k_small<4>};
         const void* pipes[] = {(const void*)k_pipeline<1, false, false>, (const void*)k_pipeline<1, true, false>, (const void*)k_pipeline<2, false, false>, (const void*)k_pipeline<2, true, false>,
                                (const void*)k_pipeline<4, false, false>, (const void*)k_pipeline<4, true, false>,
@@ -1139,8 +1174,11 @@ int isl_create(const isl_config* cfg, isl_engine** out) {
         ISL_TRY(cudaFuncGetAttributes(&fa, k_preempt));
         ISL_TRY(cudaFuncSetAttribute((const void*)k_preempt, cudaFuncAttributeMaxDynamicSharedMemorySize, optin - (int)fa.sharedSizeBytes));
         ISL_TRY(cudaFuncGetAttributes(&fa, k_gangnode));
-        e->gn.smem_optin = optin - (int)fa.sharedSizeBytes;
+        size_t gang_static = fa.sharedSizeBytes;            // the two gang-topology kernels share one sizing: the larger static share
+        ISL_TRY(cudaFuncGetAttributes(&fa, k_gangspread));
+        e->gn.smem_optin = optin - (int)std::max(gang_static, fa.sharedSizeBytes);
         ISL_TRY(cudaFuncSetAttribute((const void*)k_gangnode, cudaFuncAttributeMaxDynamicSharedMemorySize, e->gn.smem_optin));
+        ISL_TRY(cudaFuncSetAttribute((const void*)k_gangspread, cudaFuncAttributeMaxDynamicSharedMemorySize, e->gn.smem_optin));
     }
     e->occ_bytes = ((size_t)cfg->max_gpus + kSweepBlock - 1) / kSweepBlock * kSweepBlock;
     const uint32_t max_tiles = ceil_div(cfg->max_batch, kTile) + 4096;   // + one partial tile per batch of a stream
@@ -1351,7 +1389,8 @@ int isl_load_inventory(isl_engine* e, uint32_t n_nodes, const uint32_t* node_off
         ISL_CUDA(e, e->nf.node_off.replace((size_t)n_nodes + 1));
         ISL_CUDA(e, cudaMemcpyAsync(e->nf.node_off, node_off, ((size_t)n_nodes + 1) * sizeof(uint32_t), cudaMemcpyHostToDevice, e->stream));
     }
-    if (e->cfg.flags & ISL_FLAG_GANG_ONE_NODE) {      // k_gangnode walks the nodes in storage order (reversed under right-to-left)
+    if (e->cfg.flags & (ISL_FLAG_GANG_ONE_NODE | ISL_FLAG_GANG_DISTINCT_NODES)) {     // k_gangnode and k_gangspread walk the nodes in
+                                                                                      // storage order (reversed under right-to-left)
         auto& off = e->gn.off;
         off.assign(node_off, node_off + n_nodes + 1);
         if (e->prof.flip) { std::reverse(off.begin(), off.end()); for (auto& x : off) x = G - x; }
@@ -1448,8 +1487,9 @@ int isl_place_gangs(isl_engine* e, uint32_t n_gangs, const uint32_t* gang_off, c
     uint32_t* d_gang_off = reinterpret_cast<uint32_t*>(e->d_scratch.get());
     ISL_CUDA(e, cudaMemcpyAsync(d_gang_off, gang_off, ((size_t)n_gangs + 1) * sizeof(uint32_t), cudaMemcpyHostToDevice, e->stream));
     ISL_CUDA(e, cudaMemcpyAsync(e->d_req, in, (size_t)n * sizeof(isl_request), cudaMemcpyHostToDevice, e->stream));
-    if (int rc = (e->cfg.flags & ISL_FLAG_GANG_ONE_NODE) ? run_gangnode(e, n_gangs, d_gang_off, n, e->d_req, e->d_res)
-                                                         : run_gangs(e, n_gangs, d_gang_off, n, e->d_req, e->d_res)) return rc;
+    if (int rc = (e->cfg.flags & ISL_FLAG_GANG_ONE_NODE)        ? run_gangnode(e, n_gangs, d_gang_off, n, e->d_req, e->d_res)
+                 : (e->cfg.flags & ISL_FLAG_GANG_DISTINCT_NODES) ? run_gangspread(e, n_gangs, d_gang_off, n, e->d_req, e->d_res)
+                                                                 : run_gangs(e, n_gangs, d_gang_off, n, e->d_req, e->d_res)) return rc;
     ISL_CUDA(e, cudaMemcpyAsync(out, e->d_res, (size_t)n * sizeof(isl_result), cudaMemcpyDeviceToHost, e->stream));
     ISL_CUDA(e, cudaStreamSynchronize(e->stream));
     return ISL_OK;

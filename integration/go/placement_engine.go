@@ -65,6 +65,9 @@ const (
 // Engine flags (isl_config.flags) a controller may want.
 const (
 	FlagGangOneNode = uint32(C.ISL_FLAG_GANG_ONE_NODE) // PlaceGangs puts every gang on one node, the first in scan order that takes it
+	// PlaceGangs puts every member of a gang on a different node, member by member (greedy: list the larger pods first), so that
+	// one node failing does not take down every replica.  Not with FlagGangOneNode.
+	FlagGangDistinctNodes = uint32(C.ISL_FLAG_GANG_DISTINCT_NODES)
 )
 
 func NewPlacementEngine(maxGPUs, maxBatch uint32) (*PlacementEngine, error) {
@@ -78,7 +81,8 @@ func NewPlacementEngineWithPolicy(maxGPUs, maxBatch, policy uint32) (*PlacementE
 }
 
 // NewPlacementEngineWithFlags also sets Flag* values, e.g. FlagGangOneNode so that the pods of a gang share a node (host shared memory
-// instead of the network).  isl_create refuses FlagGangOneNode with PolicyMostAllocated or PolicyLeastAllocated.
+// instead of the network), or FlagGangDistinctNodes so that the replicas of a deployment land on different nodes.  isl_create refuses
+// either flag with PolicyMostAllocated or PolicyLeastAllocated, and the two together.
 func NewPlacementEngineWithFlags(maxGPUs, maxBatch, policy, flags uint32) (*PlacementEngine, error) {
 	cfg := C.isl_config{abi_version: C.ISL_ABI_VERSION, policy: C.uint32_t(policy), quirks: C.ISL_QUIRKS_REF_EXACT,
 		device: -1, max_gpus: C.uint32_t(maxGPUs), max_batch: C.uint32_t(maxBatch), flags: C.uint32_t(flags)}
