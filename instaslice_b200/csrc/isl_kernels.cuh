@@ -78,6 +78,15 @@ struct Ctrl {                   // device-resident control block, rewritten per 
     unsigned long long spec_sims, spec_rounds, spec_cells;   // speculative rounds: segment simulations run (all stages), rounds until the last stage was certified summed over chunks, chunks
 };
 
+// The batch counters of a kernel that commits its own placements, one decision step per placed request.
+__device__ __forceinline__ void count_placed(Ctrl* ctrl, uint32_t placed) {
+    atomicAdd(&ctrl->placed, (unsigned long long)placed);
+    atomicAdd(&ctrl->steps, (unsigned long long)placed);
+}
+
+// Slot mask of `size` slices from slice `start`, cut to the GPU's byte.
+__host__ __device__ inline uint32_t slice_span(uint32_t start, uint32_t size) { return (((1u << size) - 1u) << start) & 0xFFu; }
+
 // The one rule both the device table and the chain candidates come from: slot mask of placing a
 // `size`-slice profile at start v, or 0 when getStartIndexFromPreparedState can never return v
 //   size 1            -> only busy[v] is tested (:346-349)
@@ -90,7 +99,7 @@ __host__ __device__ inline uint32_t candidate_mask(uint32_t size, uint32_t v, ui
     if (pow2_only && !(size == 2 || size == 4 || size == 8)) return 0;
     const bool strict = quirks & ISL_QUIRK_STRICT_BOUND;
     if (strict ? !(v + size < ISL_SLOTS) : !(v + size <= ISL_SLOTS)) return 0;
-    return (((1u << size) - 1u) << v) & 0xFFu;
+    return slice_span(v, size);
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -150,7 +159,7 @@ __device__ __forceinline__ bool free_span(uint32_t gpu, uint32_t start, uint32_t
     span = 0;
     if (gpu >= G || size == 0 || start + size > ISL_SLOTS) return false;
     gi = flip_gpu(gpu, flip);
-    if (gi >= lo && gi < hi) span = (((1u << size) - 1u) << start) << ((gi & 3u) * 8u);
+    if (gi >= lo && gi < hi) span = slice_span(start, size) << ((gi & 3u) * 8u);      // start + size <= 8: the cut changes nothing
     return true;
 }
 
@@ -479,7 +488,7 @@ __global__ void __launch_bounds__(kSweepThreads) k_sweep_scatter(const uint4* __
                 for (uint32_t k = 0; k < cg && pos < n_p; ++k, ++pos) {
                     const uint32_t st = (starts >> (4 * k)) & 15u;
                     out_chunk[qp[pos]] = pack_result(flip_gpu(g, flip), st, size, ISL_ST_PLACED);
-                    o2 |= (((1u << size) - 1u) << st) & 0xFFu;
+                    o2 |= slice_span(st, size);
                 }
                 occ8[g] = (uint8_t)o2;
             }
@@ -847,7 +856,7 @@ __global__ void __launch_bounds__(kFewThreads, 1) k_few(DevProfiles prof, uint32
         if (g != kInf && g >= g0 && g < g0 + 16u) {             // the owner commits
             const uint32_t j = g - g0, sh = (j & 3u) * 8u, o = byte16(wv, j), t = byte16(twv, j) & (kMaxTables - 1);
             const uint32_t st = s_lut[(t * ISL_MAX_PROFILES + p) * 256 + o], size = s_sizes[t * ISL_MAX_PROFILES + p];
-            const uint32_t o2 = o | ((((1u << size) - 1u) << st) & 0xFFu);
+            const uint32_t o2 = o | slice_span(st, size);
             wv[j >> 2] = (wv[j >> 2] & ~(0xFFu << sh)) | (o2 << sh);
             occ[g] = (uint8_t)o2;
             out[r] = pack_result(flip_gpu(g, prof.flip), st, size, ISL_ST_PLACED);
@@ -2145,7 +2154,7 @@ __global__ void __launch_bounds__(kBfThreads, 1) k_bestfit(uint32_t n, const uin
                 undo &= undo - 1;
                 const uint32_t rx = __shfl_sync(0xFFFFFFFFu, rec.x, src), ry = __shfl_sync(0xFFFFFFFFu, rec.y, src);
                 const uint32_t p = __shfl_sync(0xFFFFFFFFu, q.y, src) & 0xFFu;
-                const uint32_t g = flip_gpu(rx, prof.flip) - lo, span = (((1u << ((ry >> 8) & 0xFFu)) - 1u) << (ry & 0xFFu)) & 0xFFu;
+                const uint32_t g = flip_gpu(rx, prof.flip) - lo, span = slice_span(ry & 0xFFu, (ry >> 8) & 0xFFu);
                 const uint32_t t = kMulti ? (uint32_t)(gtab[lo + g] & (kMaxTables - 1)) : 0u;
                 const uint32_t o2 = occ[lo + g], cw2 = (t << 8) | o2, cw = (t << 8) | (o2 & ~span);
                 uint32_t* c2 = bm + cw2 * stride;
@@ -2227,7 +2236,7 @@ __global__ void __launch_bounds__(kBfThreads, 1) k_bestfit(uint32_t n, const uin
             const uint32_t cw = __shfl_sync(0xFFFFFFFFu, kc, __ffs(__ballot_sync(0xFFFFFFFFu, key == m)) - 1);   // the class IS (table, occupancy byte)
             const uint32_t t = cw >> 8, o = cw & 255u;
             const uint32_t start = lut_at((t * ISL_MAX_PROFILES + p) * 256 + o), size = s_sizes[t * ISL_MAX_PROFILES + p];
-            const uint32_t o2 = o | ((((1u << size) - 1u) << start) & 0xFFu), cw2 = (t << 8) | o2;
+            const uint32_t o2 = o | slice_span(start, size), cw2 = (t << 8) | o2;
             uint32_t* c0 = bm + cw * stride;
             uint32_t* c1 = bm + cw2 * stride;
             __syncwarp();                                       // all lanes have read the class minima before they are rewritten
@@ -2246,7 +2255,7 @@ __global__ void __launch_bounds__(kBfThreads, 1) k_bestfit(uint32_t n, const uin
         }
     }
     if (kGang) close_gangs(n);
-    if (lane == 0) { atomicAdd(&ctrl->placed, (unsigned long long)placed); atomicAdd(&ctrl->steps, (unsigned long long)placed); }
+    if (lane == 0) count_placed(ctrl, placed);
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -2254,7 +2263,7 @@ __global__ void __launch_bounds__(kBfThreads, 1) k_bestfit(uint32_t n, const uin
 //   k_victim_map  one thread per victim: validates its span and claims its slices in the per-slice victim-index map (partition-local
 //                 GPU x 8 words, kVictimNone where no listed victim covers the slice); any violation raises a bit of *err
 //   k_preempt     one cooperative launch for the whole call: each CTA keeps its contiguous share of the partition in shared memory,
-//                 every preemptor is one 64-bit min over all (GPU, legal start) candidates, reduced per CTA and then grid-wide
+//                 every preemptor is one 64-bit min over all (GPU, legal start) candidates (grid_min)
 // ---------------------------------------------------------------------------------------------
 constexpr uint32_t kVictimNone = 0xFFFFFFFFu;
 constexpr uint32_t kPreThreads = 512;
@@ -2272,7 +2281,7 @@ __global__ void k_victim_map(uint32_t n, const isl_victim* __restrict__ victims,
     if (v.gpu >= G || v.size == 0 || v.start + v.size > ISL_SLOTS) { atomicOr(err, kVmErrSpan); return; }
     const uint32_t gi = flip_gpu(v.gpu, flip);
     if (gi < lo || gi >= hi) return;                    // outside the partition: ignored, as isl_free_batch ignores such spans
-    const uint32_t span = ((1u << v.size) - 1u) << v.start;
+    const uint32_t span = slice_span(v.start, v.size);   // start + size <= 8: the cut changes nothing
     if ((occ[gi] & span) != span) atomicOr(err, kVmErrFree);
     uint32_t* w = vmap + (size_t)(gi - lo) * ISL_SLOTS;
     for (uint32_t s = v.start; s < v.start + v.size; ++s)
@@ -2308,10 +2317,39 @@ __device__ __forceinline__ unsigned long long preempt_key(uint32_t m, uint32_t o
            ((unsigned long long)g << 3) | k;
 }
 
-__device__ __forceinline__ unsigned long long warp_min_u64(unsigned long long v) {
+__device__ __forceinline__ uint32_t warp_min(uint32_t v) { return redux_min_u32(v); }
+__device__ __forceinline__ unsigned long long warp_min(unsigned long long v) {
     const uint32_t hi = redux_min_u32((uint32_t)(v >> 32));
     const uint32_t lo = redux_min_u32((uint32_t)(v >> 32) == hi ? (uint32_t)v : kInf);
     return ((unsigned long long)hi << 32) | lo;
+}
+
+// The minimum of `v` over every thread of a cooperative launch of kThreads threads per CTA, returned to every thread (k_preempt,
+// k_gangnode, k_gangspread; DESIGN.md 4.7).  Every thread of every CTA must call it: it holds the grid barrier.  Each CTA reduces by warp,
+// then across the block, and writes its minimum to keys[parity * gridDim.x + blockIdx.x]; after grid.sync warp 0 reads every CTA's
+// minimum with __ldcg (other SMs wrote them; L1 is not coherent) and broadcasts the result through s_win.  The minima are double-buffered
+// by `parity`, which the call flips: a fast CTA may write round i + 1 before a slow one has read round i.
+template <uint32_t kThreads, typename T>
+__device__ __forceinline__ T grid_min(T v, unsigned long long* keys, uint32_t& parity, T* s_warp, T* s_win) {
+    const uint32_t lane = threadIdx.x & 31u, warp = threadIdx.x >> 5;
+    v = warp_min(v);
+    if (lane == 0) s_warp[warp] = v;
+    __syncthreads();
+    if (warp == 0) {
+        v = warp_min(lane < kThreads / 32 ? s_warp[lane] : ~T(0));
+        if (lane == 0) keys[parity * gridDim.x + blockIdx.x] = v;
+    }
+    cooperative_groups::grid_group grid = cooperative_groups::this_grid();
+    grid.sync();
+    if (warp == 0) {
+        v = ~T(0);
+        for (uint32_t c = lane; c < gridDim.x; c += 32) v = min(v, (T)__ldcg(keys + parity * gridDim.x + c));
+        v = warp_min(v);
+        if (lane == 0) *s_win = v;
+    }
+    __syncthreads();
+    parity ^= 1u;
+    return *s_win;
 }
 
 __global__ void __launch_bounds__(kPreThreads, 1) k_preempt(PreemptArgs a, DevProfiles prof) {
@@ -2319,7 +2357,7 @@ __global__ void __launch_bounds__(kPreThreads, 1) k_preempt(PreemptArgs a, DevPr
     __shared__ uint8_t s_masks[kMaxTables * ISL_MAX_PROFILES * ISL_MAX_STARTS];
     __shared__ unsigned long long s_warp[kPreThreads / 32];
     __shared__ unsigned long long s_win;
-    const uint32_t tid = threadIdx.x, lane = tid & 31u, warp = tid >> 5;
+    const uint32_t tid = threadIdx.x;
     const uint32_t base = blockIdx.x * a.per_cta, cnt = base < a.Gr ? min(a.per_cta, a.Gr - base) : 0u;
     unsigned long long* s_prio = reinterpret_cast<unsigned long long*>(pre_smem);      // byte s = priority of slice s, 255 = no victim
     uint8_t* s_occ = pre_smem + (size_t)a.per_cta * 8;
@@ -2342,17 +2380,18 @@ __global__ void __launch_bounds__(kPreThreads, 1) k_preempt(PreemptArgs a, DevPr
         s_occ[g] = a.occ[a.lo + base + g]; s_tab[g] = a.gtab[a.lo + base + g];
     }
     __syncthreads();
-    cooperative_groups::grid_group grid = cooperative_groups::this_grid();
+    auto unplaced = [&](uint32_t i, uint32_t size, uint32_t status) {
+        if (blockIdx.x == 0 && tid < ISL_SLOTS) {
+            if (tid == 0) a.out[i] = pack_result(ISL_GPU_NONE, ISL_START_NONE, size, status);
+            a.evict[(size_t)i * ISL_SLOTS + tid] = kVictimNone;
+        }
+    };
     uint32_t parity = 0;
     for (uint32_t i = 0; i < a.n; ++i) {
         const uint2 rq = a.in[i];
         const uint32_t profile = rq.y & 0xFFu, op = (rq.y >> 8) & 0xFFu;
         if (op != ISL_OP_ALLOC || profile >= prof.n) {      // the same for every CTA: no exchange
-            if (blockIdx.x == 0 && tid < ISL_SLOTS) {
-                if (tid == 0) a.out[i] = op == ISL_OP_ALLOC ? pack_result(ISL_GPU_NONE, ISL_START_NONE, 0, ISL_ST_BAD_PROFILE)
-                                                            : pack_result(ISL_GPU_NONE, ISL_START_NONE, 0, ISL_ST_NOOP);
-                a.evict[(size_t)i * ISL_SLOTS + tid] = kVictimNone;
-            }
+            unplaced(i, 0, op == ISL_OP_ALLOC ? ISL_ST_BAD_PROFILE : ISL_ST_NOOP);
             continue;
         }
         const uint32_t pi = a.prio[i];
@@ -2371,30 +2410,8 @@ __global__ void __launch_bounds__(kPreThreads, 1) k_preempt(PreemptArgs a, DevPr
                 if (m && !(m & blocked)) best = min(best, preempt_key(m, o, rs, pr, base + g, k));
             }
         }
-        best = warp_min_u64(best);
-        if (lane == 0) s_warp[warp] = best;
-        __syncthreads();
-        if (warp == 0) {
-            best = warp_min_u64(lane < kPreThreads / 32 ? s_warp[lane] : ~0ull);
-            if (lane == 0) a.keys[parity * gridDim.x + blockIdx.x] = best;
-        }
-        grid.sync();                                        // every CTA's minimum of preemptor i is in keys[parity]
-        if (warp == 0) {
-            unsigned long long v = ~0ull;
-            for (uint32_t c = lane; c < gridDim.x; c += 32) v = min(v, __ldcg(a.keys + parity * gridDim.x + c));
-            v = warp_min_u64(v);
-            if (lane == 0) s_win = v;
-        }
-        __syncthreads();
-        const unsigned long long win = s_win;
-        parity ^= 1u;
-        if (win == ~0ull) {                                 // no candidate anywhere: the usual unplaced record
-            if (blockIdx.x == 0 && tid < ISL_SLOTS) {
-                if (tid == 0) a.out[i] = pack_result(ISL_GPU_NONE, ISL_START_NONE, prof.rows[profile].size, ISL_ST_NO_CAPACITY);
-                a.evict[(size_t)i * ISL_SLOTS + tid] = kVictimNone;
-            }
-            continue;
-        }
+        const unsigned long long win = grid_min<kPreThreads>(best, a.keys, parity, s_warp, &s_win);
+        if (win == ~0ull) { unplaced(i, prof.rows[profile].size, ISL_ST_NO_CAPACITY); continue; }     // no candidate anywhere
         const uint32_t gw = (uint32_t)(win >> 3) & 0xFFFFFFu, k = (uint32_t)win & 7u;
         if (gw - base < cnt && tid == 0) {                  // the CTA that owns the GPU applies the eviction to its own state
             const uint32_t g = gw - base, o = s_occ[g], rs = s_rs[g];
@@ -2543,7 +2560,7 @@ __global__ void __launch_bounds__(kNfThreads, 1) k_nodefit(NodeFitArgs a, uint32
                     if (!hit) continue;
                     if (lane == __ffs(hit) - 1) {
                         const uint32_t start = s_lut[(t * ISL_MAX_PROFILES + p) * 256 + o], size = s_sizes[t * ISL_MAX_PROFILES + p];
-                        const uint32_t o2 = o | ((((1u << size) - 1u) << start) & 0xFFu), wm = (1u << a.width[t]) - 1u;
+                        const uint32_t o2 = o | slice_span(start, size), wm = (1u << a.width[t]) - 1u;
                         a.occ[g] = (uint8_t)o2;
                         a.out[base + j] = pack_result(g, start, size, ISL_ST_PLACED);
                         a.busy[v] += __popc(o2 & wm) - __popc(o & wm);
@@ -2576,7 +2593,7 @@ __global__ void __launch_bounds__(kNfThreads, 1) k_nodefit(NodeFitArgs a, uint32
             __syncthreads();
         }
     }
-    if (tid == 0) { atomicAdd(&a.ctrl->placed, (unsigned long long)placed); atomicAdd(&a.ctrl->steps, (unsigned long long)placed); }
+    if (tid == 0) count_placed(a.ctrl, placed);
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -2589,9 +2606,9 @@ __global__ void __launch_bounds__(kNfThreads, 1) k_nodefit(NodeFitArgs a, uint32
 //             the gang's members need on its table is skipped (pass 0 only).  Otherwise the warp resolves the members in order on the
 //             scratch copy, each one a warp min over the node's GPUs of score(t, p, o) << 24 | position (k_bestfit's lut and score tables; a
 //             zero score table is first-fit).  Key: the node index for a success, else bit 63 | (2^31 - 1 - depth) << 32 | node.
-//   reduce    warp, CTA, then grid (grid.sync, per-CTA minima double-buffered by round parity): the smallest key is the first node in scan
-//             order that takes the whole gang, or, with no such node, the deepest failure.  When the winner of pass 0 is a failure every
-//             node is evaluated again without the filter (pass 1), since the skipped nodes' depths are unknown.
+//   reduce    grid_min: the smallest key is the first node in scan order that takes the whole gang, or, with no such node, the deepest
+//             failure.  When the winner of pass 0 is a failure every node is evaluated again without the filter (pass 1), since the
+//             skipped nodes' depths are unknown.
 //   commit    the warp 0 of the CTA that owns the winning node resolves the members again on the live bytes and writes the PLACED records
 //             and the occupancy; a failure: CTA 0 reports every ALLOC member except the one at depth D GANG_ABORTED (that one keeps
 //             k_prepare's NO_CAPACITY or BAD_PROFILE record).
@@ -2610,7 +2627,7 @@ struct GangNodeArgs {           // kernel parameter (by value)
     const uint8_t* sizes;       // [table][profile]
     const uint32_t* node_off;   // node offsets of the inventory in storage order
     const uint32_t* gang_off;   // n_gangs + 1
-    uint8_t* scratch;           // Gr bytes: the scratch copies when the shares are in global memory
+    uint8_t* scratch;           // Gr bytes: NodeShare::aux when the shares are in global memory
     unsigned long long* keys;   // [2][gridDim.x] per-CTA minima
     Ctrl* ctrl;
     uint32_t n_gangs, n_tables, lo, hi, nlo;   // the partition [lo, hi) in storage order, its first node
@@ -2643,7 +2660,7 @@ __device__ uint32_t gangnode_resolve(const GangNodeArgs& a, const DevProfiles& p
             const uint32_t g = m & 0xFFFFFFu;
             if ((g & 31u) == lane) {
                 const uint32_t o = b[g], start = __ldg(a.lut + row + o), size = __ldg(a.sizes + t * ISL_MAX_PROFILES + p);
-                const uint32_t o2 = o | ((((1u << size) - 1u) << start) & 0xFFu);
+                const uint32_t o2 = o | slice_span(start, size);
                 b[g] = (uint8_t)o2;
                 if (commit) {
                     a.occ[gbase + g] = (uint8_t)o2;
@@ -2657,20 +2674,45 @@ __device__ uint32_t gangnode_resolve(const GangNodeArgs& a, const DevProfiles& p
     return depth;
 }
 
+// A CTA's share of the partition in k_gangnode and k_gangspread: the partition's nodes [j0, j1), which own its partition-local GPUs
+// [base, base + cnt).  `live` holds their committed bytes and `aux` a second byte per GPU (k_gangnode: scratch copies, k_gangspread:
+// node-used marks), both in shared memory, or in global memory when a share is too large for it (a.share == 0).  Every thread of the CTA
+// builds it: the constructor copies the committed bytes into shared memory.
+struct NodeShare {
+    const GangNodeArgs& a;
+    uint32_t j0, j1, base, cnt;
+    uint8_t *live, *aux;
+    __device__ __forceinline__ NodeShare(const GangNodeArgs& args, uint8_t* smem)
+        : a(args), j0(args.cta_node[blockIdx.x]), j1(args.cta_node[blockIdx.x + 1]), base(nb(j0)), cnt(nb(j1) - base),
+          live(args.share ? smem : args.occ + args.lo + base), aux(args.share ? smem + args.share : args.scratch + base) {
+        if (a.share) for (uint32_t g = threadIdx.x; g < cnt; g += kGnThreads) live[g] = a.occ[a.lo + base + g];
+    }
+    // node j of the partition owns the partition-local GPUs [nb(j), nb(j + 1)); a node the partition cuts keeps its GPUs inside it
+    __device__ __forceinline__ uint32_t nb(uint32_t j) const { return min(max(a.node_off[a.nlo + j], a.lo), a.hi) - a.lo; }
+};
+
+// Warp-wide: a gang of requests [r0, r1) failed.  Every ALLOC member except the one of rank keep_rank among them is reported
+// GANG_ABORTED; that one keeps k_prepare's NO_CAPACITY or BAD_PROFILE record.
+__device__ __forceinline__ void abort_gang_members(const uint2* in, uint2* out, const DevProfiles& prof, uint32_t r0, uint32_t r1,
+                                                   uint32_t keep_rank, uint32_t lane) {
+    uint32_t k = 0;                                         // ALLOC members before this block of 32
+    for (uint32_t r = r0; r < r1; r += 32) {
+        const uint32_t y = r + lane < r1 ? in[r + lane].y : (uint32_t)ISL_OP_NOOP << 8, p = y & 0xFFu;
+        const bool alloc = ((y >> 8) & 0xFFu) == ISL_OP_ALLOC;
+        const uint32_t ballot = __ballot_sync(0xFFFFFFFFu, alloc), rank = k + __popc(ballot & ((1u << lane) - 1u));
+        if (alloc && rank != keep_rank) out[r + lane] = pack_result(ISL_GPU_NONE, ISL_START_NONE, p < prof.n ? prof.rows[p].size : 0u, ISL_ST_GANG_ABORTED);
+        k += __popc(ballot);
+    }
+}
+
 __global__ void __launch_bounds__(kGnThreads, 1) k_gangnode(GangNodeArgs a, DevProfiles prof) {
     extern __shared__ __align__(16) uint8_t gn_smem[];
     __shared__ unsigned long long s_warp[kGnThreads / 32];
     __shared__ unsigned long long s_win;
     __shared__ uint32_t s_need[kMaxTables], s_allocs;
     const uint32_t tid = threadIdx.x, lane = tid & 31u, warp = tid >> 5;
-    // node j of the partition owns the partition-local GPUs [nb(j), nb(j + 1)); a node the partition cuts keeps its GPUs inside it
-    auto nb = [&](uint32_t j) { return min(max(a.node_off[a.nlo + j], a.lo), a.hi) - a.lo; };
-    const uint32_t j0 = a.cta_node[blockIdx.x], j1 = a.cta_node[blockIdx.x + 1];
-    const uint32_t base = nb(j0), cnt = nb(j1) - base;
-    uint8_t* live = a.share ? gn_smem : a.occ + a.lo + base;             // committed bytes of the CTA's share
-    uint8_t* scr = a.share ? gn_smem + a.share : a.scratch + base;        // scratch copies of its nodes
-    if (a.share) for (uint32_t g = tid; g < cnt; g += kGnThreads) live[g] = a.occ[a.lo + base + g];
-    cooperative_groups::grid_group grid = cooperative_groups::this_grid();
+    const NodeShare sh(a, gn_smem);
+    uint8_t* const scr = sh.aux;                            // scratch copies of the CTA's nodes
     uint32_t parity = 0, placed = 0;
     for (uint32_t gi = 0; gi < a.n_gangs; ++gi) {
         const uint32_t r0 = __ldg(a.gang_off + gi), r1 = __ldg(a.gang_off + gi + 1);
@@ -2692,60 +2734,36 @@ __global__ void __launch_bounds__(kGnThreads, 1) k_gangnode(GangNodeArgs a, DevP
         unsigned long long win = ~0ull;
         for (uint32_t pass = 0; pass < 2; ++pass) {
             unsigned long long best = ~0ull;
-            for (uint32_t j = j0 + warp; j < j1; j += kGnThreads / 32) {
-                const uint32_t b0 = nb(j) - base, c = nb(j + 1) - base - b0;
+            for (uint32_t j = sh.j0 + warp; j < sh.j1; j += kGnThreads / 32) {
+                const uint32_t b0 = sh.nb(j) - sh.base, c = sh.nb(j + 1) - sh.base - b0;
                 if (c == 0) continue;                       // an empty node places nothing: depth 0, the floor of every failure
-                const uint32_t t = a.gtab[a.lo + base + b0] & (kMaxTables - 1);
+                const uint32_t t = a.gtab[a.lo + sh.base + b0] & (kMaxTables - 1);
                 uint32_t free_slices = 0;
                 for (uint32_t g = lane; g < c; g += 32) {
-                    const uint32_t o = live[b0 + g];
+                    const uint32_t o = sh.live[b0 + g];
                     scr[b0 + g] = (uint8_t)o;
                     free_slices += 8u - __popc(o);
                 }
                 free_slices = __reduce_add_sync(0xFFFFFFFFu, free_slices);
                 if (pass == 0 && free_slices < s_need[t]) continue;
-                const uint32_t d = gangnode_resolve(a, prof, scr + b0, c, a.lo + base + b0, t, r0, r1, false, lane);
+                const uint32_t d = gangnode_resolve(a, prof, scr + b0, c, a.lo + sh.base + b0, t, r0, r1, false, lane);
                 best = min(best, d == allocs ? (unsigned long long)j : kGnFail | ((unsigned long long)(0x7FFFFFFFu - d) << 32) | j);
             }
-            best = warp_min_u64(best);
-            if (lane == 0) s_warp[warp] = best;
-            __syncthreads();
-            if (warp == 0) {
-                best = warp_min_u64(lane < kGnThreads / 32 ? s_warp[lane] : ~0ull);
-                if (lane == 0) a.keys[parity * gridDim.x + blockIdx.x] = best;
-            }
-            grid.sync();                                    // every CTA's minimum of this round is in keys[parity]
-            if (warp == 0) {
-                unsigned long long v = ~0ull;
-                for (uint32_t c = lane; c < gridDim.x; c += 32) v = min(v, __ldcg(a.keys + parity * gridDim.x + c));
-                v = warp_min_u64(v);
-                if (lane == 0) s_win = v;
-            }
-            __syncthreads();
-            win = s_win;
-            parity ^= 1u;
+            win = grid_min<kGnThreads>(best, a.keys, parity, s_warp, &s_win);
             if (!(win & kGnFail)) break;                    // a node takes the whole gang: the skipped nodes could not have come first
         }
         if (!(win & kGnFail)) {
             const uint32_t j = (uint32_t)win;
-            if (j >= j0 && j < j1 && warp == 0) {           // the owner commits on its live bytes
-                const uint32_t b0 = nb(j) - base, c = nb(j + 1) - base - b0;
-                gangnode_resolve(a, prof, live + b0, c, a.lo + base + b0, a.gtab[a.lo + base + b0] & (kMaxTables - 1), r0, r1, true, lane);
+            if (j >= sh.j0 && j < sh.j1 && warp == 0) {     // the owner commits on its live bytes
+                const uint32_t b0 = sh.nb(j) - sh.base, c = sh.nb(j + 1) - sh.base - b0;
+                gangnode_resolve(a, prof, sh.live + b0, c, a.lo + sh.base + b0, a.gtab[a.lo + sh.base + b0] & (kMaxTables - 1), r0, r1, true, lane);
                 placed += allocs;
             }
-        } else if (blockIdx.x == 0 && warp == 0) {          // ~0ull (no node evaluated) is depth 0 as well
-            const uint32_t D = 0x7FFFFFFFu - (uint32_t)((win >> 32) & 0x7FFFFFFFu);
-            uint32_t k = 0;                                 // ALLOC members before this block of 32
-            for (uint32_t r = r0; r < r1; r += 32) {
-                const uint32_t y = r + lane < r1 ? a.in[r + lane].y : (uint32_t)ISL_OP_NOOP << 8, p = y & 0xFFu;
-                const bool alloc = ((y >> 8) & 0xFFu) == ISL_OP_ALLOC;
-                const uint32_t ballot = __ballot_sync(0xFFFFFFFFu, alloc), rank = k + __popc(ballot & ((1u << lane) - 1u));
-                if (alloc && rank != D) a.out[r + lane] = pack_result(ISL_GPU_NONE, ISL_START_NONE, p < prof.n ? prof.rows[p].size : 0u, ISL_ST_GANG_ABORTED);
-                k += __popc(ballot);
-            }
+        } else if (blockIdx.x == 0 && warp == 0) {          // the deepest failure's depth; ~0ull (no node evaluated) is depth 0 as well
+            abort_gang_members(a.in, a.out, prof, r0, r1, 0x7FFFFFFFu - (uint32_t)((win >> 32) & 0x7FFFFFFFu), lane);
         }
     }
-    if (tid == 0 && placed) { atomicAdd(&a.ctrl->placed, (unsigned long long)placed); atomicAdd(&a.ctrl->steps, (unsigned long long)placed); }
+    if (tid == 0 && placed) count_placed(a.ctrl, placed);
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -2757,7 +2775,7 @@ __global__ void __launch_bounds__(kGnThreads, 1) k_gangnode(GangNodeArgs a, DevP
 // next to them (both in global memory when a share is too large).  Per ALLOC member:
 //   choose    every CTA takes the minimum of score(t, p, o) << 24 | partition-local storage position over its GPUs not marked used
 //             (k_bestfit's lut and score tables; a zero score table is first-fit, and right-to-left is the ascending scan of its reversed
-//             storage); one grid.sync over the per-CTA minima (double-buffered by round parity) gives every CTA the member's GPU.
+//             storage); grid_min over the CTAs' 32-bit minima gives every CTA the member's GPU.
 //   mark      the CTA that owns that GPU marks its node's GPUs with the gang's tag and pushes (request, GPU) onto its stack of wins.
 // A member with no GPU ends the gang: it keeps k_prepare's record (NO_CAPACITY or BAD_PROFILE), CTA 0 reports every other ALLOC member
 // GANG_ABORTED, and no occupancy byte is written.  Otherwise every CTA writes the bytes and PLACED records of its stack.  A profile that
@@ -2769,14 +2787,10 @@ __global__ void __launch_bounds__(kGnThreads, 1) k_gangspread(GangNodeArgs a, De
     __shared__ uint32_t s_warp[kGnThreads / 32];
     __shared__ uint32_t s_win, s_nwins;
     const uint32_t tid = threadIdx.x, lane = tid & 31u, warp = tid >> 5;
-    auto nb = [&](uint32_t j) { return min(max(a.node_off[a.nlo + j], a.lo), a.hi) - a.lo; };
-    const uint32_t j0 = a.cta_node[blockIdx.x], j1 = a.cta_node[blockIdx.x + 1];
-    const uint32_t base = nb(j0), cnt = nb(j1) - base;
-    uint8_t* live = a.share ? gs_smem : a.occ + a.lo + base;             // committed bytes of the CTA's share
-    uint8_t* mark = a.share ? gs_smem + a.share : a.scratch + base;       // tag of the gang whose member uses the GPU's node
-    if (a.share) for (uint32_t g = tid; g < cnt; g += kGnThreads) live[g] = a.occ[a.lo + base + g];
+    const NodeShare sh(a, gs_smem);
+    const uint32_t base = sh.base, cnt = sh.cnt;
+    uint8_t* const mark = sh.aux;                           // tag of the gang whose member uses the GPU's node
     if (tid == 0) s_nwins = 0;
-    cooperative_groups::grid_group grid = cooperative_groups::this_grid();
     uint32_t parity = 0, placed = 0, dead = 0;                            // dead: profiles no GPU of the partition admits any more
     for (uint32_t gi = 0; gi < a.n_gangs; ++gi) {
         const uint32_t r0 = __ldg(a.gang_off + gi), r1 = __ldg(a.gang_off + gi + 1), tag = 1u + gi % 255u;
@@ -2791,39 +2805,23 @@ __global__ void __launch_bounds__(kGnThreads, 1) k_gangspread(GangNodeArgs a, De
                 uint32_t key = kInf;
                 for (uint32_t g = tid; g < cnt; g += kGnThreads) {
                     if (mark[g] == tag) continue;
-                    const uint32_t o = live[g], t = a.n_tables > 1 ? a.gtab[a.lo + base + g] & (kMaxTables - 1) : 0u;
+                    const uint32_t o = sh.live[g], t = a.n_tables > 1 ? a.gtab[a.lo + base + g] & (kMaxTables - 1) : 0u;
                     const uint32_t row = (t * ISL_MAX_PROFILES + p) * 256;
                     if (__ldg(a.lut + row + o) != ISL_START_NONE) key = min(key, ((uint32_t)__ldg(a.score + row + o) << 24) | (base + g));
                 }
-                key = redux_min_u32(key);
-                if (lane == 0) s_warp[warp] = key;
-                __syncthreads();
-                if (warp == 0) {
-                    key = redux_min_u32(lane < kGnThreads / 32 ? s_warp[lane] : kInf);
-                    if (lane == 0) a.keys[parity * gridDim.x + blockIdx.x] = key;
-                }
-                grid.sync();                                // every CTA's minimum of this member is in keys[parity]
-                if (warp == 0) {
-                    uint32_t v = kInf;
-                    for (uint32_t c = lane; c < gridDim.x; c += 32) v = min(v, (uint32_t)__ldcg(a.keys + parity * gridDim.x + c));
-                    v = redux_min_u32(v);
-                    if (lane == 0) s_win = v;
-                }
-                __syncthreads();
-                win = s_win;
-                parity ^= 1u;
+                win = grid_min<kGnThreads>(key, a.keys, parity, s_warp, &s_win);
                 if (win == kInf && rank == 0) dead |= 1u << p;
             }
             if (win == kInf) { fail = rank; break; }
             const uint32_t pos = (win & 0xFFFFFFu) - base;
             if (pos < cnt) {                                // this CTA owns the member's node: the node is used for the rest of the gang
-                uint32_t jl = j0, jh = j1;                  // nb(jl) <= base + pos < nb(jh): the last such jl is the non-empty node
+                uint32_t jl = sh.j0, jh = sh.j1;            // nb(jl) <= base + pos < nb(jh): the last such jl is the non-empty node
                 while (jh - jl > 1) {
                     const uint32_t mid = (jl + jh) / 2;
-                    if (nb(mid) - base <= pos) jl = mid; else jh = mid;
+                    if (sh.nb(mid) - base <= pos) jl = mid; else jh = mid;
                 }
-                for (uint32_t g = nb(jl) - base + tid; g < nb(jl + 1) - base; g += kGnThreads) mark[g] = (uint8_t)tag;
-                if (tid == 0) wins[j0 + s_nwins++] = make_uint2(r, pos);  // one win per node of the CTA: the stack fits its nodes
+                for (uint32_t g = sh.nb(jl) - base + tid; g < sh.nb(jl + 1) - base; g += kGnThreads) mark[g] = (uint8_t)tag;
+                if (tid == 0) wins[sh.j0 + s_nwins++] = make_uint2(r, pos);     // one win per node of the CTA: the stack fits its nodes
             }
             __syncthreads();                                // the marks and the stack are in place before the next member's scan
             ++rank;
@@ -2831,30 +2829,23 @@ __global__ void __launch_bounds__(kGnThreads, 1) k_gangspread(GangNodeArgs a, De
         if (fail == kInf) {                                 // commit: each CTA writes its members; their nodes, hence GPUs, differ
             const uint32_t nw = s_nwins;
             for (uint32_t k = tid; k < nw; k += kGnThreads) {
-                const uint2 w = wins[j0 + k];
+                const uint2 w = wins[sh.j0 + k];
                 const uint32_t g = w.y, p = a.in[w.x].y & 0xFFu, t = a.gtab[a.lo + base + g] & (kMaxTables - 1);
-                const uint32_t row = (t * ISL_MAX_PROFILES + p) * 256, o = live[g];
+                const uint32_t row = (t * ISL_MAX_PROFILES + p) * 256, o = sh.live[g];
                 const uint32_t start = __ldg(a.lut + row + o), size = __ldg(a.sizes + t * ISL_MAX_PROFILES + p);
-                const uint32_t o2 = o | ((((1u << size) - 1u) << start) & 0xFFu);
-                live[g] = (uint8_t)o2;
+                const uint32_t o2 = o | slice_span(start, size);
+                sh.live[g] = (uint8_t)o2;
                 a.occ[a.lo + base + g] = (uint8_t)o2;
                 a.out[w.x] = pack_result(flip_gpu(a.lo + base + g, prof.flip), start, size, ISL_ST_PLACED);
             }
             placed += nw;
         } else if (blockIdx.x == 0 && warp == 0) {          // the member at rank `fail` keeps its record, every other ALLOC member aborts
-            uint32_t k = 0;                                 // ALLOC members before this block of 32
-            for (uint32_t r = r0; r < r1; r += 32) {
-                const uint32_t y = r + lane < r1 ? a.in[r + lane].y : (uint32_t)ISL_OP_NOOP << 8, p = y & 0xFFu;
-                const bool alloc = ((y >> 8) & 0xFFu) == ISL_OP_ALLOC;
-                const uint32_t ballot = __ballot_sync(0xFFFFFFFFu, alloc), rk = k + __popc(ballot & ((1u << lane) - 1u));
-                if (alloc && rk != fail) a.out[r + lane] = pack_result(ISL_GPU_NONE, ISL_START_NONE, p < prof.n ? prof.rows[p].size : 0u, ISL_ST_GANG_ABORTED);
-                k += __popc(ballot);
-            }
+            abort_gang_members(a.in, a.out, prof, r0, r1, fail, lane);
         }
         __syncthreads();                                    // every thread has read the stack's size
         if (tid == 0) s_nwins = 0;
     }
-    if (tid == 0 && placed) { atomicAdd(&a.ctrl->placed, (unsigned long long)placed); atomicAdd(&a.ctrl->steps, (unsigned long long)placed); }
+    if (tid == 0 && placed) count_placed(a.ctrl, placed);
 }
 
 }  // namespace isl

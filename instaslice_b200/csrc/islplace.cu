@@ -293,6 +293,20 @@ int check_launch(isl_engine* e, const char* what) {
     return ISL_OK;
 }
 
+// One cooperative launch (k_preempt, k_gangnode, k_gangspread): ISL_ECUDA, with the kernel's name, when it does not start.
+int launch_cooperative(isl_engine* e, const void* kernel, const char* name, uint32_t grid, uint32_t threads, size_t smem, void** params) {
+    const cudaError_t err = cudaLaunchCooperativeKernel(kernel, dim3(grid), dim3(threads), params, smem, e->stream);
+    if (err != cudaSuccess) { cudaGetLastError(); snprintf(e->cuda_err, sizeof(e->cuda_err), "%s: %s", name, cudaGetErrorString(err)); return ISL_ECUDA; }
+    ++e->st.kernel_launches;
+    return ISL_OK;
+}
+
+// The nodes [nlo, nhi) that own a GPU of [lo, hi), lo < hi, under the node offsets `off`.
+std::pair<uint32_t, uint32_t> node_span(const std::vector<uint32_t>& off, uint32_t lo, uint32_t hi) {
+    return {(uint32_t)(std::upper_bound(off.begin(), off.end(), lo) - off.begin()) - 1,
+            (uint32_t)(std::upper_bound(off.begin(), off.end(), hi - 1) - off.begin())};
+}
+
 // f(std::integral_constant<int, K>) with K = the candidate slots of the loaded tables (k_small<K>, k_chain<K>, k_pipeline<K, ..>)
 template <typename F>
 auto with_cand_slots(const isl_engine* e, F&& f) {
@@ -391,9 +405,8 @@ int run_nodefit(isl_engine* e, uint32_t n, const uint2* d_in, uint2* d_out) {
     if (n == 0) return ISL_OK;
     if (int rc = prepare_batch(e, n, d_in, d_out)) return rc;
     if (e->hi == e->lo) { finish_batch(e, n, true); return ISL_OK; }     // empty range: ALLOCs NO_CAPACITY, every FREE outside it
-    // the nodes that own a GPU of [lo, hi) (node scoring stores the inventory in canonical order)
-    const uint32_t nlo = (uint32_t)(std::upper_bound(e->node_off.begin(), e->node_off.end(), e->lo) - e->node_off.begin()) - 1;
-    const uint32_t nhi = (uint32_t)(std::upper_bound(e->node_off.begin(), e->node_off.end(), e->hi - 1) - e->node_off.begin());
+    uint32_t nlo, nhi;                                          // node scoring stores the inventory in canonical order
+    std::tie(nlo, nhi) = node_span(e->node_off, e->lo, e->hi);
     NodeFitArgs a{};
     a.Nr = nhi - nlo;
     for (uint32_t cnt = a.Nr;; cnt = ceil_div(cnt, 32)) {       // level sizes down to the root, each padded to 32 keys
@@ -438,8 +451,8 @@ int gang_layout(isl_engine* e, const void* kernel, uint32_t n_gangs, const uint3
                 GangNodeArgs& a, uint32_t* grid_out, size_t* smem_out, uint32_t* nodes) {
     auto& gn = e->gn;
     const uint32_t Gr = e->hi - e->lo;
-    const uint32_t nlo = (uint32_t)(std::upper_bound(gn.off.begin(), gn.off.end(), e->lo) - gn.off.begin()) - 1;
-    const uint32_t nhi = (uint32_t)(std::upper_bound(gn.off.begin(), gn.off.end(), e->hi - 1) - gn.off.begin());
+    uint32_t nlo, nhi;
+    std::tie(nlo, nhi) = node_span(gn.off, e->lo, e->hi);
     int sms = 0, per_sm = 0;
     ISL_CUDA(e, cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, e->device));
     const uint32_t grid = std::max(1u, std::min({(uint32_t)sms, kGnMaxCtas, ceil_div(Gr, 512), nhi - nlo}));
@@ -467,14 +480,6 @@ int gang_layout(isl_engine* e, const void* kernel, uint32_t n_gangs, const uint3
     return ISL_OK;
 }
 
-int launch_gang_kernel(isl_engine* e, const void* kernel, const char* name, uint32_t grid, size_t smem, void** params, uint32_t n) {
-    const cudaError_t err = cudaLaunchCooperativeKernel(kernel, dim3(grid), dim3(kGnThreads), params, smem, e->stream);
-    if (err != cudaSuccess) { cudaGetLastError(); snprintf(e->cuda_err, sizeof(e->cuda_err), "%s: %s", name, cudaGetErrorString(err)); return ISL_ECUDA; }
-    ++e->st.kernel_launches;
-    finish_batch(e, n, true);
-    return ISL_OK;
-}
-
 // isl_place_gangs on an ISL_FLAG_GANG_ONE_NODE engine: frees + defaults, then one cooperative k_gangnode (gang_layout).
 int run_gangnode(isl_engine* e, uint32_t n_gangs, const uint32_t* d_gang_off, uint32_t n, const uint2* d_in, uint2* d_out) {
     if (int rc = prepare_batch(e, n, d_in, d_out)) return rc;
@@ -483,7 +488,9 @@ int run_gangnode(isl_engine* e, uint32_t n_gangs, const uint32_t* d_gang_off, ui
     size_t smem;
     if (int rc = gang_layout(e, (const void*)k_gangnode, n_gangs, d_gang_off, d_in, d_out, a, &grid, &smem, &nodes)) return rc;
     void* params[] = {&a, &e->prof};
-    return launch_gang_kernel(e, (const void*)k_gangnode, "k_gangnode", grid, smem, params, n);
+    if (int rc = launch_cooperative(e, (const void*)k_gangnode, "k_gangnode", grid, kGnThreads, smem, params)) return rc;
+    finish_batch(e, n, true);
+    return ISL_OK;
 }
 
 // isl_place_gangs on an ISL_FLAG_GANG_DISTINCT_NODES engine: frees + defaults, then one cooperative k_gangspread (gang_layout); CTA c
@@ -497,7 +504,9 @@ int run_gangspread(isl_engine* e, uint32_t n_gangs, const uint32_t* d_gang_off, 
     ISL_CUDA(e, e->gn.wins.reserve(nodes));
     uint2* wins = e->gn.wins;
     void* params[] = {&a, &e->prof, &wins};
-    return launch_gang_kernel(e, (const void*)k_gangspread, "k_gangspread", grid, smem, params, n);
+    if (int rc = launch_cooperative(e, (const void*)k_gangspread, "k_gangspread", grid, kGnThreads, smem, params)) return rc;
+    finish_batch(e, n, true);
+    return ISL_OK;
 }
 
 // The chunk path: k_prepare, then per chunk of kChunk requests k_partition, the two sweeps, k_chain and k_commit.  d_heads_in / d_heads_out
@@ -1547,9 +1556,7 @@ int isl_preempt(isl_engine* e, uint32_t n, const isl_request* in, const uint8_t*
     a.masks = p.stage; a.out = e->d_res; a.evict = p.evict; a.keys = p.keys;
     a.n = n; a.lo = e->lo; a.Gr = Gr; a.per_cta = per_cta;
     void* params[] = {&a, &e->prof};
-    const cudaError_t err = cudaLaunchCooperativeKernel((const void*)k_preempt, dim3(grid), dim3(kPreThreads), params, smem, e->stream);
-    if (err != cudaSuccess) { cudaGetLastError(); snprintf(e->cuda_err, sizeof(e->cuda_err), "k_preempt: %s", cudaGetErrorString(err)); return ISL_ECUDA; }
-    ++e->st.kernel_launches;
+    if (int rc = launch_cooperative(e, (const void*)k_preempt, "k_preempt", grid, kPreThreads, smem, params)) return rc;
     ISL_CUDA(e, cudaMemcpyAsync(out, e->d_res, (size_t)n * sizeof(isl_result), cudaMemcpyDeviceToHost, e->stream));
     ISL_CUDA(e, cudaMemcpyAsync(evict, p.evict, (size_t)n * ISL_SLOTS * sizeof(uint32_t), cudaMemcpyDeviceToHost, e->stream));
     ISL_CUDA(e, cudaStreamSynchronize(e->stream));

@@ -125,11 +125,12 @@ def test_vs_brute_force(policy, quirks, n_tables):
     assert {E.ST_PLACED, E.ST_GANG_ABORTED, E.ST_NO_CAPACITY, E.ST_FREED, E.ST_NOOP} <= outcomes
 
 
-@pytest.mark.parametrize("shape", [(1, 1), (1, 4096), (3, 4096), (4096, 1), (1024, 8), (131072, 8), (1 << 20, 1)],
+@pytest.mark.parametrize("shape", [(1, 1), (1, 4096), (3, 4096), (4096, 1), (1024, 8), (131072, 8), (1 << 20, 1), (1, 1 << 20)],
                          ids=lambda s: "%dx%d" % s)
 @pytest.mark.parametrize("policy", [E.POLICY_FIRST_FIT, E.POLICY_BEST_FIT, E.POLICY_RIGHT_TO_LEFT])
 def test_scale(shape, policy):
-    """Inventories from one GPU to 2^20 GPUs (2^20 nodes of one), nodes of up to 4096 GPUs; gangs up to max_batch members."""
+    """Inventories from one GPU to 2^20 GPUs (2^20 nodes of one), nodes of up to 4096 GPUs, and one node of 2^20 GPUs, which one CTA
+    owns: its share does not fit in shared memory and lives in global memory; gangs up to max_batch members."""
     n_nodes, per = shape
     G = n_nodes * per
     rng = SplitMix64(G + policy)
@@ -141,6 +142,18 @@ def test_scale(shape, policy):
     check(node_off, rows, occ, None, req, off, policy, E.QUIRKS_REF_EXACT, max_batch=n)
     whole = np.array([0, n], dtype=np.uint32)           # one gang of max_batch members
     check(node_off, rows, occ, None, req, whole, policy, E.QUIRKS_REF_EXACT, max_batch=n)
+
+
+def test_share_in_global_memory_uneven():
+    """Three CTAs of which one owns a node of 2^20 - 8 GPUs and two own tiny nodes: the shares live in global memory."""
+    G = 1 << 20
+    rng = SplitMix64(4242)
+    rows = E.make_profiles(tables.H100_80GB)
+    node_off = np.array([0, 5, G - 3, G], dtype=np.uint32)
+    occ = ((rng.next(G) | rng.next(G)) & np.uint64(0x7F)).astype(np.uint8)
+    req, off = random_call(rng, G, len(rows), 48, 6)
+    for policy in POLICIES:
+        check(node_off, rows, occ, None, req, off, policy, E.QUIRKS_REF_EXACT, max_batch=48)
 
 
 @pytest.mark.parametrize("policy", POLICIES)
