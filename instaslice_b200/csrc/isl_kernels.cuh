@@ -1700,6 +1700,7 @@ __device__ __forceinline__ void decide(const PipeArgs& a, const Stage& st, PipeS
         if (!kDefer && la >= la_cap) { cut = true; break; }     // once per group of decisions, off the loop-carried path
         bool none = false;
         uint32_t m = 0, mmax = 0;
+        uint32_t lm[kUnroll], lc[kUnroll];     // kDefer: the group's log records, stored behind its last decision
 #pragma unroll
         for (int u = 0; u < kUnroll; ++u) {     // unrolled: one taken branch per kUnroll decisions
             m = redux_min_u32(key);
@@ -1712,10 +1713,8 @@ __device__ __forceinline__ void decide(const PipeArgs& a, const Stage& st, PipeS
             uint32_t ks;
             asm("shr.s32 %0, %1, 31;" : "=r"(ks) : "r"(m));                                            // all ones: landed on the next GPU
             asm("mad.lo.s32 %0, %1, -4, %0;" : "+r"(ca) : "r"(ks));                                     // ca += sel * 4
-            if (kDefer) {       // a pseudo-decision (m == INF: nothing fits here or on the next GPU, move on by one) leaves no log record
-                const bool real = m != kInf;
-                sts_v2_if(lane == 0 && real, la, m, ca);
-                la = add_if(real, la, 8u);
+            if (kDefer) {
+                lm[u] = m; lc[u] = ca;
                 mmax = max(mmax, m);
             } else {
                 sts_v2_if(lane == 0, la, m, ca);                // decision log: (key, address of the record two past the GPU it landed on)
@@ -1730,10 +1729,9 @@ __device__ __forceinline__ void decide(const PipeArgs& a, const Stage& st, PipeS
                 uint32_t zs, gn, kk;
                 asm("lop3.b32 %0, %1, %2, %3, 0xca;" : "=r"(zs) : "r"(ks), "r"(z1[k]), "r"(z0[k]));       // sel ? z1 : z0
                 asm("lop3.b32 %0, %1, %2, %3, 0xca;" : "=r"(gn) : "r"(ks), "r"(g2[k]), "r"(g1[k]));       // sel ? g2 : g1
-                asm("{ .reg .pred p; .reg .b32 t; lop3.b32 t, %1, %2, %3, 0xF8; setp.eq.u32 p, t, 0; selp.b32 %0, %4, %5, p; }"
-                    : "=r"(kk) : "r"(zs), "r"(m), "r"(cm8[k]), "r"(tn), "r"(tn | gn));
+                asm("{ .reg .pred p; lop3.b32 %1, %2, %3, %4, 0xF8; setp.eq.u32 p, %1, 0; selp.b32 %0, %5, %6, p; }"     // z0 = zs | winner's slices
+                    : "=r"(kk), "=r"(z0[k]) : "r"(zs), "r"(m), "r"(cm8[k]), "r"(tn), "r"(tn | gn));
                 key = min(key, kk);
-                z0[k] = zs | (m & cm8[k]);
                 g1[k] = gn;
                 asm("lop3.b32 %0, %1, %2, %3, 0xca;" : "=r"(z1[k]) : "r"(ks), "r"(z2[k]), "r"(z1[k]));    // sel ? z2 : z1
                 tcur[k] = tn;
@@ -1757,7 +1755,24 @@ __device__ __forceinline__ void decide(const PipeArgs& a, const Stage& st, PipeS
             // m == INF is a legitimate step of the recurrence ("neither this GPU nor the next takes anything: the next one becomes
             // current"; it pops only lanes whose window is exhausted, into their INF sentinels), so the loop body needs no exit
             // test per decision — one test per group: did ANY decision of the group find nothing?
-            if (__builtin_expect(mmax != kInf && la < la_cap, 1)) continue;     // (the cut-off test rides on the group's one branch)
+            // The group's log is written here, behind its last decision: a store between two reductions (with its predicate, and the
+            // address update that waits until the store has read its registers) would sit on the in-order issue path of every decision.
+            if (__builtin_expect(mmax != kInf, 1)) {
+                // every decision real: eight stores at fixed offsets, by all lanes (the same record; a lane predicate here is
+                // compiled into a branch around each store)
+#pragma unroll
+                for (int u = 0; u < kUnroll; ++u) sts_v2_if(true, la + 8u * u, lm[u], lc[u]);
+                la += 8u * kUnroll;
+                if (__builtin_expect(la < la_cap, 1)) continue;     // (the cut-off test rides on the group's one branch)
+                cut = true; break;
+            }
+            // a pseudo-decision (m == INF: nothing fits here or on the next GPU, move on by one) leaves no log record
+#pragma unroll
+            for (int u = 0; u < kUnroll; ++u) {
+                const bool real = lm[u] != kInf;
+                sts_v2_if(lane == 0 && real, la, lm[u], lc[u]);
+                la = add_if(real, la, 8u);
+            }
             if (la >= la_cap) { cut = true; break; }
             // exhausted lanes were popped past the end of their windows: back onto the sentinels (at most kUnroll pops since the last time)
 #pragma unroll

@@ -613,10 +613,11 @@ int segment_geometry(isl_engine* e, uint32_t n_chunks, double avg_chunk, bool wa
     const uint32_t range = e->hi - e->lo;
     // Segments aimed for.  A batch's decisions form ONE sequential chain over the inventory, only different chunks overlap, so a
     // stream of B chunks over S stages takes about (S + B - 1) x (D x t_dec / S + t_fix), D = decisions of a chunk.  tools/chain_cost.py
-    // on config 4, H100 SXM at 400 W: t_dec = 40.8 ns per decision, t_fix = 1.75 us per busy cell (token in -> loop start 1.58 us, loop
-    // end -> token out 0.17 us).  Minimum at S = sqrt((B - 1) x D x t_dec / t_fix); D is estimated by the smaller of the chunk size and
-    // ~3.5 placements per GPU.  ISL_PIPE_SEGMENTS overrides (experiments).
-    constexpr double kTdecUs = 0.0408, kTfixUs = 1.75;
+    // on config 4, H100 80GB HBM3 (SXM, 700 W power limit, SM clock 1980 MHz): t_dec = 32.6 ns per decision, t_fix = 1.57 us per busy
+    // cell (token in -> loop start 1.45 us, loop end -> token out 0.12 us; profiles/r03_chain_sm90.md).  Minimum at
+    // S = sqrt((B - 1) x D x t_dec / t_fix); D is estimated by the smaller of the chunk size and ~3.5 placements per GPU.
+    // ISL_PIPE_SEGMENTS overrides (experiments).
+    constexpr double kTdecUs = 0.0326, kTfixUs = 1.57;
     const uint32_t stages_max = (uint32_t)std::max(1, e->max_coresident);     // one CTA per SM: the SM count of the device
     uint32_t target = stages_max;
     {
