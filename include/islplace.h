@@ -410,7 +410,11 @@ int  isl_preempt(isl_engine* e, uint32_t n, const isl_request* in, const uint8_t
  * overlap on the device (segment pipeline).  While a stream is open (isl_stream_open until isl_stream_close, launched or not) every
  * call on the engine returns ISL_ESTATE and changes nothing, except: isl_stream_submit, _wait and _close, isl_destroy (closes the stream
  * first), and isl_num_gpus, isl_gpu_to_node, isl_device_occupancy, isl_device_results, isl_abi_version, isl_strerror,
- * isl_last_cuda_error, isl_host_alloc and isl_host_free.  The test is made under the engine lock. */
+ * isl_last_cuda_error, isl_host_alloc and isl_host_free.  The test is made under the engine lock.
+ * isl_stream_open returns ISL_ERANGE, and leaves no stream open, when max_batches x 65 536 > max_batch, or when the inventory does not
+ * fit one resident pipeline beside the feed kernels: the pipeline then has SMs - 4 stages of at most 8 x 512 GPUs, so on a 132-SM H100
+ * an inventory of more than 128 x 8 x 512 = 524 288 GPUs (fewer when the loaded tables cap the sub-segment below 512 GPUs) is refused.
+ * isl_place_stream takes the chunk-by-chunk path for such inventories instead. */
 int  isl_stream_open(isl_engine* e, uint32_t max_batches);
 int  isl_stream_submit(isl_engine* e, uint32_t n, const isl_request* in, isl_result* out, uint32_t* ticket);
 int  isl_stream_wait(isl_engine* e, uint32_t ticket);
