@@ -35,6 +35,7 @@ uint32_t first_mask(const isl_profile& row, uint32_t o, uint32_t quirks) {
 struct Ctx {
     uint32_t n_profiles, quirks, policy;
     const isl_profile* rows;
+    std::vector<int16_t> memo;              // [table][profile][byte]: a member's score, -1 until first asked; empty: no memo
 };
 
 // what the policy minimises on byte o for a placement of mask `mine` of profile p on a node of table t (first-fit family: nothing)
@@ -52,17 +53,28 @@ uint32_t score(const Ctx& c, uint32_t t, uint32_t o, uint32_t mine) {
     return lost;
 }
 
+// score() of profile p taking `mine`, its first legal start on byte o of a node of table t; with the memo on, each (table, profile, byte)
+// is walked once, the first time a member asks for it
+uint32_t member_score(Ctx& c, uint32_t t, uint32_t p, uint32_t o, uint32_t mine) {
+    if (c.memo.empty()) return score(c, t, o, mine);
+    int16_t& s = c.memo[((size_t)t * c.n_profiles + p) * 256 + o];
+    if (s < 0) s = (int16_t)score(c, t, o, mine);
+    return (uint32_t)s;
+}
+
 }  // namespace
 
 extern "C" {
 
 // rows[t * n_profiles + p]; node_off [n_nodes + 1] and node_table [n_nodes] in canonical order; occ: G bytes (canonical order), updated
-// in place; default_size[p]: the size an unplaced ALLOC reports; [lo, hi): the canonical range (the engine's partition).  out as
-// isl_place_gangs writes it.
+// in place; default_size[p]: the size an unplaced ALLOC reports; [lo, hi): the canonical range (the engine's partition); memo: remember
+// every score per (table, profile, byte).  out as isl_place_gangs writes it.
 void gnf_place_gangs(uint32_t n_nodes, const uint32_t* node_off, const uint8_t* node_table, uint32_t n_profiles, const isl_profile* rows,
                      const uint8_t* default_size, uint8_t* occ, uint32_t lo, uint32_t hi, uint32_t quirks, uint32_t policy,
-                     uint32_t n_gangs, const uint32_t* gang_off, const isl_request* in, isl_result* out) {
-    const Ctx c{n_profiles, quirks, policy, rows};
+                     uint32_t n_gangs, const uint32_t* gang_off, const isl_request* in, isl_result* out, uint32_t memo) {
+    Ctx c{n_profiles, quirks, policy, rows, {}};
+    if (memo && policy == ISL_POLICY_MIN_FRAG)
+        c.memo.assign((size_t)(*std::max_element(node_table, node_table + n_nodes) + 1) * n_profiles * 256, -1);
     const uint32_t G = node_off[n_nodes], n = gang_off[n_gangs];
     const bool descending = policy == ISL_POLICY_RIGHT_TO_LEFT;
     for (uint32_t i = 0; i < n; ++i) {                  // rule 1: every FREE first; default records for the rest
@@ -98,7 +110,7 @@ void gnf_place_gangs(uint32_t n_nodes, const uint32_t* node_off, const uint8_t* 
                     const uint32_t g = descending ? b - 1 - k : a + k;
                     const uint32_t m = first_mask(row, bytes[g - a], quirks);
                     if (!m) continue;
-                    const uint32_t sc = score(c, node_table[node], bytes[g - a], m);
+                    const uint32_t sc = member_score(c, node_table[node], p, bytes[g - a], m);
                     if (!found || sc < best_s) { found = true; best_g = g; best_m = m; best_s = sc; }
                 }
                 if (!found) break;

@@ -47,17 +47,30 @@ uint32_t score(uint32_t policy, uint32_t n_profiles, const isl_profile* rows, ui
     return lost;
 }
 
+// score() of profile p taking `mine`, its first legal start on byte o of a node of table t; with a memo ([table][profile][byte], -1 until
+// first asked), each (table, profile, byte) is walked once, the first time a member asks for it
+uint32_t member_score(std::vector<int16_t>& memo, uint32_t policy, uint32_t n_profiles, const isl_profile* rows, uint32_t quirks, uint32_t t,
+                      uint32_t p, uint32_t o, uint32_t mine) {
+    if (memo.empty()) return score(policy, n_profiles, rows, quirks, t, o, mine);
+    int16_t& s = memo[((size_t)t * n_profiles + p) * 256 + o];
+    if (s < 0) s = (int16_t)score(policy, n_profiles, rows, quirks, t, o, mine);
+    return (uint32_t)s;
+}
+
 }  // namespace
 
 extern "C" {
 
 // rows[t * n_profiles + p]; node_off [n_nodes + 1] and node_table [n_nodes] in canonical order; occ: G bytes (canonical order), updated
-// in place; default_size[p]: the size an unplaced ALLOC reports; [lo, hi): the canonical range (the engine's partition).  out as
-// isl_place_gangs writes it.
+// in place; default_size[p]: the size an unplaced ALLOC reports; [lo, hi): the canonical range (the engine's partition); memo: remember
+// every score per (table, profile, byte).  out as isl_place_gangs writes it.
 void gsf_place_gangs(uint32_t n_nodes, const uint32_t* node_off, const uint8_t* node_table, uint32_t n_profiles, const isl_profile* rows,
                      const uint8_t* default_size, uint8_t* occ, uint32_t lo, uint32_t hi, uint32_t quirks, uint32_t policy,
-                     uint32_t n_gangs, const uint32_t* gang_off, const isl_request* in, isl_result* out) {
+                     uint32_t n_gangs, const uint32_t* gang_off, const isl_request* in, isl_result* out, uint32_t memo) {
     const uint32_t G = node_off[n_nodes], n = gang_off[n_gangs];
+    std::vector<int16_t> scores;
+    if (memo && policy == ISL_POLICY_MIN_FRAG)
+        scores.assign((size_t)(*std::max_element(node_table, node_table + n_nodes) + 1) * n_profiles * 256, -1);
     const bool descending = policy == ISL_POLICY_RIGHT_TO_LEFT;
     for (uint32_t i = 0; i < n; ++i) {                  // rule 1: every FREE first; default records for the rest
         const isl_request& r = in[i];
@@ -89,7 +102,7 @@ void gsf_place_gangs(uint32_t n_nodes, const uint32_t* node_off, const uint8_t* 
                 const isl_profile& row = rows[(size_t)node_table[node_of[g]] * n_profiles + p];
                 const uint32_t m = first_mask(row, bytes[g - lo], quirks);
                 if (!m) continue;
-                const uint32_t sc = score(policy, n_profiles, rows, quirks, node_table[node_of[g]], bytes[g - lo], m);
+                const uint32_t sc = member_score(scores, policy, n_profiles, rows, quirks, node_table[node_of[g]], p, bytes[g - lo], m);
                 if (!found || sc < best_s) { found = true; best_g = g; best_m = m; best_s = sc; }
             }
             if (!found) break;

@@ -33,7 +33,7 @@ def lib():
         L = C.CDLL(so)
         p, u = C.c_void_p, C.c_uint32
         L.gsf_place_gangs.restype = None
-        L.gsf_place_gangs.argtypes = [u, p, p, u, p, p, p, u, u, u, u, u, p, p, p]
+        L.gsf_place_gangs.argtypes = [u, p, p, u, p, p, p, u, u, u, u, u, p, p, p, u]
         _lib = L
     return _lib
 
@@ -43,8 +43,9 @@ def _ptr(a):
 
 
 def place_gangs(node_off, rows, occ, requests, gang_off, quirks=E.QUIRKS_REF_EXACT, policy=E.POLICY_FIRST_FIT, node_table=None,
-                lo=0, hi=None):
-    """``rows``: [n_profiles] or [n_tables][n_profiles] with ``node_table`` [n_nodes]; [lo, hi): the engine's partition (canonical)."""
+                lo=0, hi=None, memo=True):
+    """``rows``: [n_profiles] or [n_tables][n_profiles] with ``node_table`` [n_nodes]; [lo, hi): the engine's partition (canonical);
+    ``memo``: ISL_POLICY_MIN_FRAG scores are walked once per (table, profile, byte) and remembered, which 2^20-GPU calls need."""
     node_off = np.ascontiguousarray(node_off, dtype=np.uint32)
     rows2 = np.ascontiguousarray(np.asarray(rows, dtype=E.PROFILE_DTYPE).reshape(-1, np.asarray(rows).shape[-1]))
     n_nodes = len(node_off) - 1
@@ -56,5 +57,5 @@ def place_gangs(node_off, rows, occ, requests, gang_off, quirks=E.QUIRKS_REF_EXA
     gang_off = np.ascontiguousarray(gang_off, dtype=np.uint32)
     out = np.zeros(len(requests), dtype=E.RESULT_DTYPE)
     lib().gsf_place_gangs(n_nodes, _ptr(node_off), _ptr(table), rows2.shape[1], _ptr(rows2), _ptr(dsize), _ptr(occ), lo, hi, quirks, policy,
-                          len(gang_off) - 1, _ptr(gang_off), _ptr(requests), _ptr(out))
+                          len(gang_off) - 1, _ptr(gang_off), _ptr(requests), _ptr(out), int(memo))
     return out, occ
