@@ -148,6 +148,8 @@ typedef struct isl_config {
 #define ISL_FLAG_GANG_ONE_NODE 64u  /* isl_place_gangs puts every member of a gang on ONE node (see isl_place_gangs); every other call is unchanged */
 #define ISL_FLAG_GANG_DISTINCT_NODES 128u  /* isl_place_gangs puts every member of a gang on a DIFFERENT node (see isl_place_gangs); every
                                               other call is unchanged */
+#define ISL_FLAG_GANG_FEW_NODES 256u  /* isl_place_gangs puts a gang on ONE node when one takes it, else on as FEW nodes as it greedily can
+                                         (see isl_place_gangs); every other call is unchanged */
 
 /* One Migplacement row (api/v1alpha1/instaslice_types.go:23-29).  `size` is
  * Placements[0].Size (:334); `starts` is [p.Start for p in Placements] in CRD
@@ -349,6 +351,36 @@ int  isl_place_batch_range(isl_engine* e, uint32_t lo, uint32_t hi, uint32_t n, 
  *       member 0 places, member 1 reports NO_CAPACITY); (d) on an inventory of one-GPU nodes under ISL_QUIRKS_FIXED with gangs whose
  *       profiles all take a whole GPU (size 8), a flagged call equals the unflagged one on every policy.
  *   S6. isl_create: ISL_EINVAL for the flag with ISL_FLAG_GANG_ONE_NODE (they contradict each other), ISL_FLAG_ALL_NODES or a
+ *       node-scoring policy.  isl_place_gangs keeps every code above, the 2^20-GPU partition cap included.  Every other entry point
+ *       returns exactly what it returns on an unflagged engine.  The flag applies to every gang of the engine, as G6 says.
+ *
+ * Few-node gangs (ISL_FLAG_GANG_FEW_NODES): a job's workers that should share a node but must still run when no single node has room for
+ * them (Kueue's preferred topology on kubernetes.io/hostname, which never applies to gated MIG pods).  On an engine created with the flag:
+ *   F1. Rules 1, 2 (FREEs first, NOOPs ignored, gangs in array order), 3 and 5 hold unchanged; rule 6 with the refusals of F6.
+ *   F2. Rounds.  Let m_0 .. m_{k-1} be the gang's ALLOC members and i = 0.  In each round d(node) is how many of the leading members
+ *       m_i, m_{i+1}, .. the node places, resolved in order by the engine's policy restricted to that node's GPUs inside the partition,
+ *       exactly as in G2, on the occupancy left by committed gangs and by this gang's earlier rounds (a node the partition cuts offers
+ *       only its GPUs inside the partition).  The node with the largest d takes m_i .. m_{i+d-1}, ties to the first node in scan order
+ *       (ascending canonical; descending under ISL_POLICY_RIGHT_TO_LEFT); then i += d.  The gang commits when i = k.  A node that takes
+ *       every remaining member has the largest possible d, so when some node takes them all, the first such node wins, as in G2.
+ *   F3. Failure: when the largest d of a round is 0, member m_i gets its usual record (NO_CAPACITY, or BAD_PROFILE for an unknown
+ *       profile) and every other ALLOC member reports ISL_ST_GANG_ABORTED with the unplaced default record.  The occupancy is what it was
+ *       before the gang (rule 5), the slices of its earlier rounds included.
+ *   F4. Consequences: (a) a gang that some single node takes whole gets exactly the records and occupancy of a GANG_ONE_NODE engine (round
+ *       1 is G2); (b) a gang that fails here fails on a GANG_ONE_NODE engine in the same state; (c) on a one-node inventory, or a partition
+ *       inside one node, a flagged call equals the unflagged one (records and occupancy, every policy): the second round on the same node
+ *       has d = 0 at the member that did not fit, which is rule 4; (d) with gangs of one, a flagged call equals a GANG_ONE_NODE call, and
+ *       under ISL_POLICY_FIRST_FIT and _RIGHT_TO_LEFT isl_place_batch; (e) two consecutive rounds never use the same node (the member that
+ *       ended round r does not fit on its node, so that node has d = 0 next), so the maximal runs of a committed gang's ALLOC members on
+ *       one node (isl_gpu_to_node) are exactly its rounds.  A node may come back in a later, non-adjacent round when a smaller member fits
+ *       where an earlier one did not: A100-40GB tables, reference-exact quirks, one-GPU nodes with bytes 0x01 and 0xF0, first-fit gang
+ *       [1g.5gb, 3g.20gb, 1g.5gb] commits on nodes 0, 1, 0 where a GANG_ONE_NODE engine aborts it.
+ *   F5. The choice is greedy, round by round (Kueue's largest domain first), not a minimum cover, and a tie goes to scan order even when
+ *       an earlier round already uses one of the tied nodes: the gang may use more nodes than it needs.  A100-40GB tables, reference-exact
+ *       quirks, first-fit, one-GPU nodes with bytes 0xF0, 0x0F and 0x80, gang [4g.20gb, 2g.10gb, 3g.20gb, 1g.5gb]: node 2 takes the
+ *       first two members (d = [1, 0, 2]), node 0 the 3g.20gb, and node 1 the last 1g.5gb (a tie with node 2): three nodes, where
+ *       node 2 could have taken the last member too.
+ *   F6. isl_create: ISL_EINVAL for the flag with ISL_FLAG_GANG_ONE_NODE, ISL_FLAG_GANG_DISTINCT_NODES, ISL_FLAG_ALL_NODES or a
  *       node-scoring policy.  isl_place_gangs keeps every code above, the 2^20-GPU partition cap included.  Every other entry point
  *       returns exactly what it returns on an unflagged engine.  The flag applies to every gang of the engine, as G6 says. */
 int  isl_place_gangs(isl_engine* e, uint32_t n_gangs, const uint32_t* gang_off, const isl_request* in, isl_result* out);

@@ -97,16 +97,19 @@ class InstasliceReconciler:
     """
 
     def __init__(self, instaslices: list, quirks: int = E.QUIRKS_REF_EXACT, max_batch: int = 65536, engine: E.Engine | None = None,
-                 policy: int = E.POLICY_FIRST_FIT, gang_one_node: bool = False, gang_distinct_nodes: bool = False):
+                 policy: int = E.POLICY_FIRST_FIT, gang_one_node: bool = False, gang_distinct_nodes: bool = False,
+                 gang_few_nodes: bool = False):
         """``policy``: the engine policy of the engine this reconciler creates (``engine`` is None), e.g. ``E.POLICY_MOST_ALLOCATED`` to
         pack MIG pods onto the fullest nodes or ``E.POLICY_LEAST_ALLOCATED`` to spread them (include/islplace.h).  ``gang_one_node``:
         that engine is created with ``E.FLAG_GANG_ONE_NODE``, so ``place_pending_gangs`` puts every gang on one node.
         ``gang_distinct_nodes``: with ``E.FLAG_GANG_DISTINCT_NODES``, so it puts every member of a gang on a different node (the engine
-        refuses both flags at once)."""
+        refuses both flags at once).  ``gang_few_nodes``: with ``E.FLAG_GANG_FEW_NODES``, so it puts a gang on one node when one takes
+        it, else on as few nodes as it greedily can (the engine refuses it with either of the other two)."""
         self.quirks = quirks
         self.policy = policy
         self.gang_one_node = gang_one_node
         self.gang_distinct_nodes = gang_distinct_nodes
+        self.gang_few_nodes = gang_few_nodes
         self.items = instaslices
         self._engine = engine
         self._max_batch = max_batch
@@ -150,7 +153,8 @@ class InstasliceReconciler:
         if self._engine is None:
             self._engine = E.Engine(max_gpus=max(4096, len(self.gpu_uuid)), max_batch=self._max_batch, policy=self.policy, quirks=self.quirks,
                                     flags=(E.FLAG_GANG_ONE_NODE if self.gang_one_node else 0) |
-                                          (E.FLAG_GANG_DISTINCT_NODES if self.gang_distinct_nodes else 0))
+                                          (E.FLAG_GANG_DISTINCT_NODES if self.gang_distinct_nodes else 0) |
+                                          (E.FLAG_GANG_FEW_NODES if self.gang_few_nodes else 0))
         self._engine.load_profile_tables(self.rows)
         self._engine.load_inventory(self.node_off, np.asarray(occ, dtype=np.uint8))
         self._engine.set_node_tables(np.asarray(self.node_table, dtype=np.uint8))

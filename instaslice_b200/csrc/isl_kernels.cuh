@@ -2627,6 +2627,12 @@ __global__ void __launch_bounds__(kNfThreads, 1) k_nodefit(NodeFitArgs a, uint32
 //   commit    the warp 0 of the CTA that owns the winning node resolves the members again on the live bytes and writes the PLACED records
 //             and the occupancy; a failure: CTA 0 reports every ALLOC member except the one at depth D GANG_ABORTED (that one keeps
 //             k_prepare's NO_CAPACITY or BAD_PROFILE record).
+// k_gangnode<true>: ISL_FLAG_GANG_FEW_NODES (DESIGN.md 4.11).  A gang is a loop of rounds over its remaining members, from request ri on;
+// each round is the evaluate and reduce steps above, and the winning key's depth d is how many members the round places (a success: all
+// that remain).  The owner commits those d on its live bytes as tentative PLACED records and every CTA advances ri past d ALLOC members.
+// d = 0 aborts the gang without an undo log: the spans of one gang are disjoint and were free before it, so each CTA clears the spans of
+// the tentative records on its own nodes (gangfew_undo) and reports those members GANG_ABORTED, while CTA 0 reports the members after
+// the one that found no node.  Every barrier depends only on the gang offsets and the winning keys, which every CTA sees alike.
 // ---------------------------------------------------------------------------------------------
 constexpr uint32_t kGnThreads = 512;
 constexpr uint32_t kGnMaxCtas = 160;                    // CTAs of one launch (at most one per SM)
@@ -2720,6 +2726,46 @@ __device__ __forceinline__ void abort_gang_members(const uint2* in, uint2* out, 
     }
 }
 
+// Warp-wide (k_gangnode<true>): the request just past the d-th ALLOC member at or after request r (d >= 1, and [r, r1) holds that many).
+__device__ __forceinline__ uint32_t skip_allocs(const uint2* in, uint32_t r, uint32_t r1, uint32_t d, uint32_t lane) {
+    for (;; r += 32) {
+        uint32_t ballot = __ballot_sync(0xFFFFFFFFu, r + lane < r1 && ((in[r + lane].y >> 8) & 0xFFu) == ISL_OP_ALLOC);
+        const uint32_t c = __popc(ballot);
+        if (d <= c) {
+            for (; d > 1; --d) ballot &= ballot - 1;
+            return r + __ffs(ballot);
+        }
+        d -= c;
+    }
+}
+
+// Warp-wide (k_gangnode<true>): a few-node gang aborted after earlier rounds committed its ALLOC members among requests [r0, r1) as
+// tentative PLACED records.  The CTA takes back those on its own nodes: the spans of one gang are disjoint and were free before it, so
+// clearing them restores its live bytes and the occupancy, and it reports those members GANG_ABORTED (it is their records' only writer).
+// The records may come from other CTAs, written before a grid barrier of a later round, so they are read from L2.  One lane at a time
+// writes, since two members may share a GPU.
+__device__ void gangfew_undo(const GangNodeArgs& a, const NodeShare& sh, const DevProfiles& prof, uint32_t r0, uint32_t r1, uint32_t lane) {
+    for (uint32_t r = r0; r < r1; r += 32) {
+        const uint32_t i = r + lane;
+        uint2 rec = make_uint2(ISL_GPU_NONE, (uint32_t)ISL_ST_GANG_ABORTED << 16);
+        if (i < r1 && ((a.in[i].y >> 8) & 0xFFu) == ISL_OP_ALLOC) rec = __ldcg(a.out + i);
+        const uint32_t pos = flip_gpu(rec.x, prof.flip) - a.lo - sh.base;     // inside this CTA's share when below sh.cnt
+        uint32_t hits = __ballot_sync(0xFFFFFFFFu, (rec.y >> 16) == ISL_ST_PLACED && pos < sh.cnt);
+        while (hits) {
+            const uint32_t src = __ffs(hits) - 1;
+            hits &= hits - 1;
+            if (lane == src) {
+                const uint32_t keep = ~slice_span(rec.y & 0xFFu, (rec.y >> 8) & 0xFFu), p = a.in[i].y & 0xFFu;
+                sh.live[pos] &= (uint8_t)keep;
+                a.occ[a.lo + sh.base + pos] &= (uint8_t)keep;
+                a.out[i] = pack_result(ISL_GPU_NONE, ISL_START_NONE, prof.rows[p].size, ISL_ST_GANG_ABORTED);
+            }
+            __syncwarp();
+        }
+    }
+}
+
+template <bool kFew>
 __global__ void __launch_bounds__(kGnThreads, 1) k_gangnode(GangNodeArgs a, DevProfiles prof) {
     extern __shared__ __align__(16) uint8_t gn_smem[];
     __shared__ unsigned long long s_warp[kGnThreads / 32];
@@ -2731,51 +2777,72 @@ __global__ void __launch_bounds__(kGnThreads, 1) k_gangnode(GangNodeArgs a, DevP
     uint32_t parity = 0, placed = 0;
     for (uint32_t gi = 0; gi < a.n_gangs; ++gi) {
         const uint32_t r0 = __ldg(a.gang_off + gi), r1 = __ldg(a.gang_off + gi + 1);
-        if (tid < kMaxTables) s_need[tid] = 0;
-        if (tid == 0) s_allocs = 0;
-        __syncthreads();                                    // also orders a commit of the previous gang before this gang's reads
-        uint32_t mine = 0;
-        for (uint32_t r = r0 + tid; r < r1; r += kGnThreads) {      // the slices the gang's ALLOCs take on a node of each table
-            const uint32_t y = a.in[r].y, p = y & 0xFFu;
-            if (((y >> 8) & 0xFFu) != ISL_OP_ALLOC) continue;
-            ++mine;
-            if (p < prof.n)
-                for (uint32_t t = 0; t < a.n_tables; ++t) atomicAdd(&s_need[t], (uint32_t)__ldg(a.sizes + t * ISL_MAX_PROFILES + p));
-        }
-        if (mine) atomicAdd(&s_allocs, mine);
-        __syncthreads();
-        const uint32_t allocs = s_allocs;
-        if (allocs == 0) continue;                          // FREEs and NOOPs only: k_prepare's records stand
-        unsigned long long win = ~0ull;
-        for (uint32_t pass = 0; pass < 2; ++pass) {
-            unsigned long long best = ~0ull;
-            for (uint32_t j = sh.j0 + warp; j < sh.j1; j += kGnThreads / 32) {
-                const uint32_t b0 = sh.nb(j) - sh.base, c = sh.nb(j + 1) - sh.base - b0;
-                if (c == 0) continue;                       // an empty node places nothing: depth 0, the floor of every failure
-                const uint32_t t = a.gtab[a.lo + sh.base + b0] & (kMaxTables - 1);
-                uint32_t free_slices = 0;
-                for (uint32_t g = lane; g < c; g += 32) {
-                    const uint32_t o = sh.live[b0 + g];
-                    scr[b0 + g] = (uint8_t)o;
-                    free_slices += 8u - __popc(o);
+        uint32_t ri = r0, held = 0;     // kFew: the round's first request; members this CTA committed tentatively in earlier rounds
+        for (;;) {                      // one round; without kFew every path leaves after the first
+            if (tid < kMaxTables) s_need[tid] = 0;
+            if (tid == 0) s_allocs = 0;
+            __syncthreads();                                    // also orders a commit of the previous gang or round before this one's reads
+            uint32_t mine = 0;
+            for (uint32_t r = ri + tid; r < r1; r += kGnThreads) {      // the slices the remaining ALLOCs take on a node of each table
+                const uint32_t y = a.in[r].y, p = y & 0xFFu;
+                if (((y >> 8) & 0xFFu) != ISL_OP_ALLOC) continue;
+                ++mine;
+                if (p < prof.n)
+                    for (uint32_t t = 0; t < a.n_tables; ++t) atomicAdd(&s_need[t], (uint32_t)__ldg(a.sizes + t * ISL_MAX_PROFILES + p));
+            }
+            if (mine) atomicAdd(&s_allocs, mine);
+            __syncthreads();
+            const uint32_t allocs = s_allocs;
+            if (allocs == 0) break;                             // FREEs and NOOPs only: k_prepare's records stand
+            unsigned long long win = ~0ull;
+            for (uint32_t pass = 0; pass < 2; ++pass) {
+                unsigned long long best = ~0ull;
+                for (uint32_t j = sh.j0 + warp; j < sh.j1; j += kGnThreads / 32) {
+                    const uint32_t b0 = sh.nb(j) - sh.base, c = sh.nb(j + 1) - sh.base - b0;
+                    if (c == 0) continue;                       // an empty node places nothing: depth 0, the floor of every failure
+                    const uint32_t t = a.gtab[a.lo + sh.base + b0] & (kMaxTables - 1);
+                    uint32_t free_slices = 0;
+                    for (uint32_t g = lane; g < c; g += 32) {
+                        const uint32_t o = sh.live[b0 + g];
+                        scr[b0 + g] = (uint8_t)o;
+                        free_slices += 8u - __popc(o);
+                    }
+                    free_slices = __reduce_add_sync(0xFFFFFFFFu, free_slices);
+                    if (pass == 0 && free_slices < s_need[t]) continue;
+                    const uint32_t d = gangnode_resolve(a, prof, scr + b0, c, a.lo + sh.base + b0, t, ri, r1, false, lane);
+                    best = min(best, d == allocs ? (unsigned long long)j : kGnFail | ((unsigned long long)(0x7FFFFFFFu - d) << 32) | j);
                 }
-                free_slices = __reduce_add_sync(0xFFFFFFFFu, free_slices);
-                if (pass == 0 && free_slices < s_need[t]) continue;
-                const uint32_t d = gangnode_resolve(a, prof, scr + b0, c, a.lo + sh.base + b0, t, r0, r1, false, lane);
-                best = min(best, d == allocs ? (unsigned long long)j : kGnFail | ((unsigned long long)(0x7FFFFFFFu - d) << 32) | j);
+                win = grid_min<kGnThreads>(best, a.keys, parity, s_warp, &s_win);
+                if (!(win & kGnFail)) break;                    // a node takes the whole gang: the skipped nodes could not have come first
             }
-            win = grid_min<kGnThreads>(best, a.keys, parity, s_warp, &s_win);
-            if (!(win & kGnFail)) break;                    // a node takes the whole gang: the skipped nodes could not have come first
-        }
-        if (!(win & kGnFail)) {
-            const uint32_t j = (uint32_t)win;
-            if (j >= sh.j0 && j < sh.j1 && warp == 0) {     // the owner commits on its live bytes
-                const uint32_t b0 = sh.nb(j) - sh.base, c = sh.nb(j + 1) - sh.base - b0;
-                gangnode_resolve(a, prof, sh.live + b0, c, a.lo + sh.base + b0, a.gtab[a.lo + sh.base + b0] & (kMaxTables - 1), r0, r1, true, lane);
-                placed += allocs;
+            if (!(win & kGnFail)) {
+                const uint32_t j = (uint32_t)win;
+                if (j >= sh.j0 && j < sh.j1 && warp == 0) {     // the owner commits on its live bytes
+                    const uint32_t b0 = sh.nb(j) - sh.base, c = sh.nb(j + 1) - sh.base - b0;
+                    gangnode_resolve(a, prof, sh.live + b0, c, a.lo + sh.base + b0, a.gtab[a.lo + sh.base + b0] & (kMaxTables - 1), ri, r1, true, lane);
+                    placed += allocs;
+                }
+                if (kFew) placed += held;                       // the gang commits: its tentative members count
+                break;
             }
-        } else if (blockIdx.x == 0 && warp == 0) {          // the deepest failure's depth; ~0ull (no node evaluated) is depth 0 as well
-            abort_gang_members(a.in, a.out, prof, r0, r1, 0x7FFFFFFFu - (uint32_t)((win >> 32) & 0x7FFFFFFFu), lane);
+            if constexpr (!kFew) {
+                if (blockIdx.x == 0 && warp == 0)               // the deepest failure's depth; ~0ull (no node evaluated) is depth 0 as well
+                    abort_gang_members(a.in, a.out, prof, r0, r1, 0x7FFFFFFFu - (uint32_t)((win >> 32) & 0x7FFFFFFFu), lane);
+                break;
+            } else {
+                const uint32_t d = 0x7FFFFFFFu - (uint32_t)((win >> 32) & 0x7FFFFFFFu), j = (uint32_t)win;  // members the round places
+                if (d == 0) {                                   // no node takes m_i: every CTA takes back its tentative members
+                    if (warp == 0) gangfew_undo(a, sh, prof, r0, ri, lane);
+                    if (blockIdx.x == 0 && warp == 0) abort_gang_members(a.in, a.out, prof, ri, r1, 0, lane);
+                    break;
+                }
+                if (j >= sh.j0 && j < sh.j1 && warp == 0) {     // the owner commits the round's d members on its live bytes
+                    const uint32_t b0 = sh.nb(j) - sh.base, c = sh.nb(j + 1) - sh.base - b0;
+                    gangnode_resolve(a, prof, sh.live + b0, c, a.lo + sh.base + b0, a.gtab[a.lo + sh.base + b0] & (kMaxTables - 1), ri, r1, true, lane);
+                    held += d;
+                }
+                ri = skip_allocs(a.in, ri, r1, d, lane);        // every CTA read the same key: all advance alike
+            }
         }
     }
     if (tid == 0 && placed) count_placed(a.ctrl, placed);

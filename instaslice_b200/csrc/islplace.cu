@@ -180,7 +180,8 @@ struct isl_engine {
         DevMem<uint32_t> node_off, tree, fit, nodes;
         uint8_t width[kMaxTables] = {};
     } nf;
-    // one-node and distinct-node gangs (ISL_FLAG_GANG_ONE_NODE, k_gangnode; ISL_FLAG_GANG_DISTINCT_NODES, k_gangspread): the inventory's
+    // one-node, few-node and distinct-node gangs (ISL_FLAG_GANG_ONE_NODE, k_gangnode<false>; ISL_FLAG_GANG_FEW_NODES, k_gangnode<true>;
+    // ISL_FLAG_GANG_DISTINCT_NODES, k_gangspread): the inventory's
     // node offsets in storage order (host and device, isl_load_inventory), the scratch copies (k_gangnode) or node-used marks
     // (k_gangspread) when the shares do not fit in shared memory, the per-CTA minima, and k_gangspread's per-CTA stacks of wins
     struct GangNode {
@@ -486,9 +487,23 @@ int run_gangnode(isl_engine* e, uint32_t n_gangs, const uint32_t* d_gang_off, ui
     GangNodeArgs a;
     uint32_t grid, nodes;
     size_t smem;
-    if (int rc = gang_layout(e, (const void*)k_gangnode, n_gangs, d_gang_off, d_in, d_out, a, &grid, &smem, &nodes)) return rc;
+    if (int rc = gang_layout(e, (const void*)k_gangnode<false>, n_gangs, d_gang_off, d_in, d_out, a, &grid, &smem, &nodes)) return rc;
     void* params[] = {&a, &e->prof};
-    if (int rc = launch_cooperative(e, (const void*)k_gangnode, "k_gangnode", grid, kGnThreads, smem, params)) return rc;
+    if (int rc = launch_cooperative(e, (const void*)k_gangnode<false>, "k_gangnode", grid, kGnThreads, smem, params)) return rc;
+    finish_batch(e, n, true);
+    return ISL_OK;
+}
+
+// isl_place_gangs on an ISL_FLAG_GANG_FEW_NODES engine: frees + defaults, then one cooperative k_gangnode<true> (gang_layout), which
+// places each gang in rounds, one node per round.
+int run_gangfew(isl_engine* e, uint32_t n_gangs, const uint32_t* d_gang_off, uint32_t n, const uint2* d_in, uint2* d_out) {
+    if (int rc = prepare_batch(e, n, d_in, d_out)) return rc;
+    GangNodeArgs a;
+    uint32_t grid, nodes;
+    size_t smem;
+    if (int rc = gang_layout(e, (const void*)k_gangnode<true>, n_gangs, d_gang_off, d_in, d_out, a, &grid, &smem, &nodes)) return rc;
+    void* params[] = {&a, &e->prof};
+    if (int rc = launch_cooperative(e, (const void*)k_gangnode<true>, "k_gangnode<true>", grid, kGnThreads, smem, params)) return rc;
     finish_batch(e, n, true);
     return ISL_OK;
 }
@@ -1134,6 +1149,9 @@ int isl_create(const isl_config* cfg, isl_engine** out) {
     // distinct-node gangs: the opposite of one-node gangs, and, like them, not with a pod on every node nor with node scoring
     if ((cfg->flags & ISL_FLAG_GANG_DISTINCT_NODES) &&
         ((cfg->flags & (ISL_FLAG_GANG_ONE_NODE | ISL_FLAG_ALL_NODES)) || node_scoring(cfg->policy))) return ISL_EINVAL;
+    // few-node gangs: a third locality mode, exclusive with the other two, and, like them, not with a pod on every node nor node scoring
+    if ((cfg->flags & ISL_FLAG_GANG_FEW_NODES) &&
+        ((cfg->flags & (ISL_FLAG_GANG_ONE_NODE | ISL_FLAG_GANG_DISTINCT_NODES | ISL_FLAG_ALL_NODES)) || node_scoring(cfg->policy))) return ISL_EINVAL;
     if (request_major(cfg->policy) && cfg->max_gpus > kBfMaxGpus) return ISL_ERANGE;
     if (cfg->quirks & ~ISL_QUIRKS_REF_EXACT) return ISL_EINVAL;
     isl_engine* e = new (std::nothrow) isl_engine;
@@ -1162,7 +1180,7 @@ int isl_create(const isl_config* cfg, isl_engine** out) {
         cudaFuncAttributes fa;
         const void* kernels[] = {(const void*)k_prepare, (const void*)k_partition, (const void*)k_set_flag, (const void*)k_few, (const void*)k_build_lut, (const void*)k_eval_starts,
                                  (const void*)k_free_spans, (const void*)k_capacity, (const void*)k_sweep_count, (const void*)k_sweep_scatter, (const void*)k_commit, (const void*)k_bestfit<false>, (const void*)k_bestfit<true>,
-                                 (const void*)k_bestfit<false, true>, (const void*)k_bestfit<true, true>, (const void*)k_victim_map, (const void*)k_preempt, (const void*)k_nodefit, (const void*)k_gangnode, (const void*)k_gangspread,
+                                 (const void*)k_bestfit<false, true>, (const void*)k_bestfit<true, true>, (const void*)k_victim_map, (const void*)k_preempt, (const void*)k_nodefit, (const void*)k_gangnode<false>, (const void*)k_gangnode<true>, (const void*)k_gangspread,
                                  (const void*)k_chain<1>, (const void*)k_chain<2>, (const void*)k_chain<4>, (const void*)k_small<1>, (const void*)k_small<2>, (const void*)k_small<4>};
         const void* pipes[] = {(const void*)k_pipeline<1, false, false>, (const void*)k_pipeline<1, true, false>, (const void*)k_pipeline<2, false, false>, (const void*)k_pipeline<2, true, false>,
                                (const void*)k_pipeline<4, false, false>, (const void*)k_pipeline<4, true, false>,
@@ -1183,12 +1201,12 @@ int isl_create(const isl_config* cfg, isl_engine** out) {
         ISL_TRY(cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev));
         ISL_TRY(cudaFuncGetAttributes(&fa, k_preempt));
         ISL_TRY(cudaFuncSetAttribute((const void*)k_preempt, cudaFuncAttributeMaxDynamicSharedMemorySize, optin - (int)fa.sharedSizeBytes));
-        ISL_TRY(cudaFuncGetAttributes(&fa, k_gangnode));
-        size_t gang_static = fa.sharedSizeBytes;            // the two gang-topology kernels share one sizing: the larger static share
-        ISL_TRY(cudaFuncGetAttributes(&fa, k_gangspread));
-        e->gn.smem_optin = optin - (int)std::max(gang_static, fa.sharedSizeBytes);
-        ISL_TRY(cudaFuncSetAttribute((const void*)k_gangnode, cudaFuncAttributeMaxDynamicSharedMemorySize, e->gn.smem_optin));
-        ISL_TRY(cudaFuncSetAttribute((const void*)k_gangspread, cudaFuncAttributeMaxDynamicSharedMemorySize, e->gn.smem_optin));
+        // the gang-topology kernels share one sizing: the largest static share
+        const void* gangs[] = {(const void*)k_gangnode<false>, (const void*)k_gangnode<true>, (const void*)k_gangspread};
+        size_t gang_static = 0;
+        for (const void* k : gangs) { ISL_TRY(cudaFuncGetAttributes(&fa, k)); gang_static = std::max(gang_static, fa.sharedSizeBytes); }
+        e->gn.smem_optin = optin - (int)gang_static;
+        for (const void* k : gangs) ISL_TRY(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, e->gn.smem_optin));
     }
     e->occ_bytes = ((size_t)cfg->max_gpus + kSweepBlock - 1) / kSweepBlock * kSweepBlock;
     const uint32_t max_tiles = ceil_div(cfg->max_batch, kTile) + 4096;   // + one partial tile per batch of a stream
@@ -1399,8 +1417,8 @@ int isl_load_inventory(isl_engine* e, uint32_t n_nodes, const uint32_t* node_off
         ISL_CUDA(e, e->nf.node_off.replace((size_t)n_nodes + 1));
         ISL_CUDA(e, cudaMemcpyAsync(e->nf.node_off, node_off, ((size_t)n_nodes + 1) * sizeof(uint32_t), cudaMemcpyHostToDevice, e->stream));
     }
-    if (e->cfg.flags & (ISL_FLAG_GANG_ONE_NODE | ISL_FLAG_GANG_DISTINCT_NODES)) {     // k_gangnode and k_gangspread walk the nodes in
-                                                                                      // storage order (reversed under right-to-left)
+    if (e->cfg.flags & (ISL_FLAG_GANG_ONE_NODE | ISL_FLAG_GANG_FEW_NODES | ISL_FLAG_GANG_DISTINCT_NODES)) {   // k_gangnode and
+                                                                    // k_gangspread walk the nodes in storage order (reversed under right-to-left)
         auto& off = e->gn.off;
         off.assign(node_off, node_off + n_nodes + 1);
         if (e->prof.flip) { std::reverse(off.begin(), off.end()); for (auto& x : off) x = G - x; }
@@ -1498,6 +1516,7 @@ int isl_place_gangs(isl_engine* e, uint32_t n_gangs, const uint32_t* gang_off, c
     ISL_CUDA(e, cudaMemcpyAsync(d_gang_off, gang_off, ((size_t)n_gangs + 1) * sizeof(uint32_t), cudaMemcpyHostToDevice, e->stream));
     ISL_CUDA(e, cudaMemcpyAsync(e->d_req, in, (size_t)n * sizeof(isl_request), cudaMemcpyHostToDevice, e->stream));
     if (int rc = (e->cfg.flags & ISL_FLAG_GANG_ONE_NODE)        ? run_gangnode(e, n_gangs, d_gang_off, n, e->d_req, e->d_res)
+                 : (e->cfg.flags & ISL_FLAG_GANG_FEW_NODES)      ? run_gangfew(e, n_gangs, d_gang_off, n, e->d_req, e->d_res)
                  : (e->cfg.flags & ISL_FLAG_GANG_DISTINCT_NODES) ? run_gangspread(e, n_gangs, d_gang_off, n, e->d_req, e->d_res)
                                                                  : run_gangs(e, n_gangs, d_gang_off, n, e->d_req, e->d_res)) return rc;
     ISL_CUDA(e, cudaMemcpyAsync(out, e->d_res, (size_t)n * sizeof(isl_result), cudaMemcpyDeviceToHost, e->stream));

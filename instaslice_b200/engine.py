@@ -32,6 +32,7 @@ ST_PLACED, ST_NO_CAPACITY, ST_BAD_PROFILE, ST_FREED, ST_BAD_SPAN, ST_NOOP, ST_GA
 FLAG_TIMING, FLAG_NO_PIPELINE, FLAG_FORCE_PIPELINE, FLAG_TRACE, FLAG_NO_SMALL, FLAG_ALL_NODES = 1, 2, 4, 8, 16, 32
 FLAG_GANG_ONE_NODE = 64     # isl_place_gangs puts every member of a gang on one node (include/islplace.h)
 FLAG_GANG_DISTINCT_NODES = 128  # isl_place_gangs puts every member of a gang on a different node (include/islplace.h)
+FLAG_GANG_FEW_NODES = 256  # isl_place_gangs puts a gang on one node when one takes it, else on as few nodes as it greedily can
 SPEC_AUTO, SPEC_OFF, SPEC_ON = 0, 1, 2
 
 # ---- record layouts -------------------------------------------------------------------------
@@ -338,7 +339,9 @@ class Engine:
         keeps its record and every other ALLOC member reports ``ST_GANG_ABORTED`` (include/islplace.h).  On an engine created with
         ``FLAG_GANG_ONE_NODE`` every gang lands on one node, the first in scan order that takes it whole, and the member at the depth no
         node gets past keeps its record.  On an engine created with ``FLAG_GANG_DISTINCT_NODES`` every member of a gang lands on a
-        different node, resolved greedily member by member, and the first member with no GPU on an unused node keeps its record."""
+        different node, resolved greedily member by member, and the first member with no GPU on an unused node keeps its record.  On an
+        engine created with ``FLAG_GANG_FEW_NODES`` a gang goes to one node when one takes it whole, else in rounds: each round the node
+        that places the most of the remaining members takes them; when no node places the next member, that member keeps its record."""
         requests = np.ascontiguousarray(requests, dtype=REQUEST_DTYPE)
         gang_off = np.ascontiguousarray(gang_off, dtype=np.uint32)
         if len(gang_off) == 0 or int(gang_off[-1]) != len(requests):

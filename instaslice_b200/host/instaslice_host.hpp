@@ -88,7 +88,8 @@ class InstasliceReconciler {
 public:
     // policy: the engine's isl_config.policy, e.g. ISL_POLICY_MOST_ALLOCATED to pack MIG pods onto the fullest nodes or
     // ISL_POLICY_LEAST_ALLOCATED to spread them (include/islplace.h).  flags: isl_config.flags, e.g. ISL_FLAG_GANG_ONE_NODE so that
-    // PlaceGangs puts every gang on one node, or ISL_FLAG_GANG_DISTINCT_NODES so that it puts every member of a gang on a different node
+    // PlaceGangs puts every gang on one node, ISL_FLAG_GANG_DISTINCT_NODES so that it puts every member of a gang on a different node,
+    // or ISL_FLAG_GANG_FEW_NODES so that it puts a gang on one node when one takes it and on as few nodes as it greedily can otherwise
     explicit InstasliceReconciler(uint32_t quirks = ISL_QUIRKS_REF_EXACT, uint32_t max_gpus = 1u << 16, uint32_t max_batch = 1u << 16,
                                   uint32_t policy = ISL_POLICY_FIRST_FIT, uint32_t flags = 0);
     ~InstasliceReconciler();

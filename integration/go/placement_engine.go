@@ -68,6 +68,9 @@ const (
 	// PlaceGangs puts every member of a gang on a different node, member by member (greedy: list the larger pods first), so that
 	// one node failing does not take down every replica.  Not with FlagGangOneNode.
 	FlagGangDistinctNodes = uint32(C.ISL_FLAG_GANG_DISTINCT_NODES)
+	// PlaceGangs puts a gang on one node when one takes it whole, else on as few nodes as it greedily can: each round the node that
+	// places the most of the remaining pods takes them.  Not with FlagGangOneNode or FlagGangDistinctNodes.
+	FlagGangFewNodes = uint32(C.ISL_FLAG_GANG_FEW_NODES)
 )
 
 func NewPlacementEngine(maxGPUs, maxBatch uint32) (*PlacementEngine, error) {
@@ -81,8 +84,9 @@ func NewPlacementEngineWithPolicy(maxGPUs, maxBatch, policy uint32) (*PlacementE
 }
 
 // NewPlacementEngineWithFlags also sets Flag* values, e.g. FlagGangOneNode so that the pods of a gang share a node (host shared memory
-// instead of the network), or FlagGangDistinctNodes so that the replicas of a deployment land on different nodes.  isl_create refuses
-// either flag with PolicyMostAllocated or PolicyLeastAllocated, and the two together.
+// instead of the network), FlagGangDistinctNodes so that the replicas of a deployment land on different nodes, or FlagGangFewNodes so
+// that a gang shares a node when one has room and still runs on a few nodes when none has.  isl_create refuses each of the three flags
+// with PolicyMostAllocated or PolicyLeastAllocated, and any two of them together.
 func NewPlacementEngineWithFlags(maxGPUs, maxBatch, policy, flags uint32) (*PlacementEngine, error) {
 	cfg := C.isl_config{abi_version: C.ISL_ABI_VERSION, policy: C.uint32_t(policy), quirks: C.ISL_QUIRKS_REF_EXACT,
 		device: -1, max_gpus: C.uint32_t(maxGPUs), max_batch: C.uint32_t(maxBatch), flags: C.uint32_t(flags)}
