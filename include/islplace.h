@@ -150,6 +150,13 @@ typedef struct isl_config {
                                               other call is unchanged */
 #define ISL_FLAG_GANG_FEW_NODES 256u  /* isl_place_gangs puts a gang on ONE node when one takes it, else on as FEW nodes as it greedily can
                                          (see isl_place_gangs); every other call is unchanged */
+#define ISL_FLAG_GANG_LOCALITY 512u  /* isl_place_gangs takes each gang's node locality from its ALLOC members' `start` byte, one of the
+                                        ISL_GANG_* values below (see isl_place_gangs); every other call is unchanged */
+/* Node locality of one gang on an ISL_FLAG_GANG_LOCALITY engine (isl_request.start of its ALLOC members, rules L1-L6) */
+#define ISL_GANG_ANY_NODES      0u  /* rules 2-4: members anywhere, as on an engine without a gang flag */
+#define ISL_GANG_ONE_NODE       1u  /* G2-G3: every member on one node */
+#define ISL_GANG_FEW_NODES      2u  /* F2-F3: one node when one takes the gang, else as few nodes as it greedily can */
+#define ISL_GANG_DISTINCT_NODES 3u  /* S2-S4: every member on a different node */
 
 /* One Migplacement row (api/v1alpha1/instaslice_types.go:23-29).  `size` is
  * Placements[0].Size (:334); `starts` is [p.Start for p in Placements] in CRD
@@ -328,7 +335,7 @@ int  isl_place_batch_range(isl_engine* e, uint32_t lo, uint32_t hi, uint32_t n, 
  *       occupancy, every policy).  With gangs of one, a flagged ISL_POLICY_FIRST_FIT or _RIGHT_TO_LEFT engine equals isl_place_batch.
  *   G5. isl_create: ISL_EINVAL for the flag with ISL_FLAG_ALL_NODES or a node-scoring policy.  isl_place_gangs keeps every code above,
  *       the 2^20-GPU partition cap included.  Every other entry point returns exactly what it returns on an unflagged engine.
- *   G6. The flag applies to every gang of the engine: choosing node locality per gang would need another entry point, and there is none.
+ *   G6. The flag applies to every gang of the engine.  To choose node locality gang by gang, use ISL_FLAG_GANG_LOCALITY (L1-L6).
  *
  * Distinct-node gangs (ISL_FLAG_GANG_DISTINCT_NODES): the replicas of a deployment on different nodes, so that one node or one GPU
  * failing does not take down every replica (the kube-scheduler's required podAntiAffinity on kubernetes.io/hostname, which never applies
@@ -382,7 +389,29 @@ int  isl_place_batch_range(isl_engine* e, uint32_t lo, uint32_t hi, uint32_t n, 
  *       node 2 could have taken the last member too.
  *   F6. isl_create: ISL_EINVAL for the flag with ISL_FLAG_GANG_ONE_NODE, ISL_FLAG_GANG_DISTINCT_NODES, ISL_FLAG_ALL_NODES or a
  *       node-scoring policy.  isl_place_gangs keeps every code above, the 2^20-GPU partition cap included.  Every other entry point
- *       returns exactly what it returns on an unflagged engine.  The flag applies to every gang of the engine, as G6 says. */
+ *       returns exactly what it returns on an unflagged engine.  The flag applies to every gang of the engine, as G6 says.
+ *
+ * Node locality per gang (ISL_FLAG_GANG_LOCALITY): one burst of pending pods that mixes a job needing one node, replicas that must sit on
+ * distinct nodes, a job that prefers few nodes and pods that go anywhere (Kueue's per-workload podset-required-topology and
+ * podset-preferred-topology), placed by one call on one occupancy.  On an engine created with the flag:
+ *   L1. An ALLOC member's `start` byte names its gang's locality: ISL_GANG_ANY_NODES (0), _ONE_NODE (1), _FEW_NODES (2) or
+ *       _DISTINCT_NODES (3).  A FREE's `start` stays its span; a NOOP's is ignored.  A gang with no ALLOC member has no locality.
+ *   L2. Rules 1, 3 and 5 hold unchanged.  Rule 2's order holds across localities: gangs go in array order, and each gang sees every
+ *       commit of every earlier gang, whatever that gang's locality.  Each gang is placed by the rules of its locality, on the
+ *       occupancy that the call's FREEs and the earlier gangs left: 0 by rules 2-4 (as on an engine without a gang flag), 1 by G2-G3,
+ *       2 by F2-F3, 3 by S2-S4.
+ *   L3. Consequences: (a) a call whose ALLOC members all carry locality k equals isl_place_gangs on an engine created with k's flag (no
+ *       gang flag for 0), with the same policy, quirks, node tables and partition: records, occupancy and stats.placed; (b) a call equals
+ *       its gangs run one at a time, each alone on the engine flagged for its locality, after the call's FREEs, with the occupancy handed
+ *       on from each gang to the next; (c) with every byte 0, under ISL_POLICY_FIRST_FIT or _RIGHT_TO_LEFT, gangs of one equal
+ *       isl_place_batch.
+ *   L4. ISL_EINVAL, and nothing changes, when an ALLOC's byte is greater than 3 or two ALLOC members of one gang name different
+ *       localities.  These checks run with the other argument checks, before the engine state is looked at.
+ *   L5. isl_create: ISL_EINVAL for the flag with ISL_FLAG_GANG_ONE_NODE, _DISTINCT_NODES, _FEW_NODES, ISL_FLAG_ALL_NODES or a
+ *       node-scoring policy.  isl_place_gangs keeps every code above, the 2^20-GPU partition cap included.  Every other entry point
+ *       returns exactly what it returns on an unflagged engine.
+ *   L6. Locality matters even for a gang of one: under best-fit a one-node gang of one takes the best GPU of the FIRST node in scan order
+ *       that admits it, not the best GPU of the whole partition. */
 int  isl_place_gangs(isl_engine* e, uint32_t n_gangs, const uint32_t* gang_off, const isl_request* in, isl_result* out);
 
 /* 8 bytes: one running allocation that MAY be evicted (isl_preempt). */

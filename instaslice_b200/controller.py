@@ -98,18 +98,20 @@ class InstasliceReconciler:
 
     def __init__(self, instaslices: list, quirks: int = E.QUIRKS_REF_EXACT, max_batch: int = 65536, engine: E.Engine | None = None,
                  policy: int = E.POLICY_FIRST_FIT, gang_one_node: bool = False, gang_distinct_nodes: bool = False,
-                 gang_few_nodes: bool = False):
+                 gang_few_nodes: bool = False, gang_locality: bool = False):
         """``policy``: the engine policy of the engine this reconciler creates (``engine`` is None), e.g. ``E.POLICY_MOST_ALLOCATED`` to
         pack MIG pods onto the fullest nodes or ``E.POLICY_LEAST_ALLOCATED`` to spread them (include/islplace.h).  ``gang_one_node``:
         that engine is created with ``E.FLAG_GANG_ONE_NODE``, so ``place_pending_gangs`` puts every gang on one node.
         ``gang_distinct_nodes``: with ``E.FLAG_GANG_DISTINCT_NODES``, so it puts every member of a gang on a different node (the engine
         refuses both flags at once).  ``gang_few_nodes``: with ``E.FLAG_GANG_FEW_NODES``, so it puts a gang on one node when one takes
-        it, else on as few nodes as it greedily can (the engine refuses it with either of the other two)."""
+        it, else on as few nodes as it greedily can (the engine refuses it with either of the other two).  ``gang_locality``: with
+        ``E.FLAG_GANG_LOCALITY``, so ``place_pending_gangs`` takes a locality per gang (the engine refuses it with the other three)."""
         self.quirks = quirks
         self.policy = policy
         self.gang_one_node = gang_one_node
         self.gang_distinct_nodes = gang_distinct_nodes
         self.gang_few_nodes = gang_few_nodes
+        self.gang_locality = gang_locality
         self.items = instaslices
         self._engine = engine
         self._max_batch = max_batch
@@ -154,7 +156,8 @@ class InstasliceReconciler:
             self._engine = E.Engine(max_gpus=max(4096, len(self.gpu_uuid)), max_batch=self._max_batch, policy=self.policy, quirks=self.quirks,
                                     flags=(E.FLAG_GANG_ONE_NODE if self.gang_one_node else 0) |
                                           (E.FLAG_GANG_DISTINCT_NODES if self.gang_distinct_nodes else 0) |
-                                          (E.FLAG_GANG_FEW_NODES if self.gang_few_nodes else 0))
+                                          (E.FLAG_GANG_FEW_NODES if self.gang_few_nodes else 0) |
+                                          (E.FLAG_GANG_LOCALITY if self.gang_locality else 0))
         self._engine.load_profile_tables(self.rows)
         self._engine.load_inventory(self.node_off, np.asarray(occ, dtype=np.uint8))
         self._engine.set_node_tables(np.asarray(self.node_table, dtype=np.uint8))
@@ -264,7 +267,7 @@ class InstasliceReconciler:
                 out.append(self._commit_or_veto(pod, pod["profile"], policy, res))
         return out
 
-    def place_pending_gangs(self, gangs: list, policy=None):
+    def place_pending_gangs(self, gangs: list, policy=None, locality=None):
         """All-or-nothing pod groups (the replicas of one deployment, the workers of one job): ``gangs`` is a list of non-empty pod
         lists shaped as ``place_pending_pods`` takes them, resolved in order with ONE engine call (isl_place_gangs).
 
@@ -272,16 +275,21 @@ class InstasliceReconciler:
         it gets a slice, and only then are its allocations written to the custom resources.  When the Prepared exact-match veto
         (:198-203) fires on any pod, the spans of the whole gang are released again.  With realised slices whose allocation is gone
         (the only state in which the veto can fire) the gangs are resolved one engine call each, as ``place_pending_pods`` does per pod.
+
+        ``locality``: one ``E.GANG_*`` value per gang (e.g. from Kueue's podset topology annotations, INTEGRATION.md), for a reconciler
+        created with ``gang_locality=True``: a training job on one node, replicas on distinct nodes, a job on few nodes and free pods in
+        one call on one occupancy.
         """
         policy = policy or FirstFitPolicy()
         if any(not g for g in gangs):
             raise ValueError("empty gang")
         if self._has_orphans and len(gangs) > 1:
-            return [self.place_pending_gangs([g], policy)[0] for g in gangs]
+            locs = [None] * len(gangs) if locality is None else [[loc] for loc in locality]
+            return [self.place_pending_gangs([g], policy, loc)[0] for g, loc in zip(gangs, locs)]
         if not gangs:
             return []
         off = np.cumsum([0] + [len(g) for g in gangs]).astype(np.uint32)
-        results = self._engine.place_gangs(self._requests([p["profile"] for g in gangs for p in g]), off)
+        results = self._engine.place_gangs(self._requests([p["profile"] for g in gangs for p in g]), off, locality)
         out = []
         for gang, a, b in zip(gangs, off[:-1], off[1:]):
             res = results[a:b]

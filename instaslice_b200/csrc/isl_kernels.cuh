@@ -2765,6 +2765,82 @@ __device__ void gangfew_undo(const GangNodeArgs& a, const NodeShare& sh, const D
     }
 }
 
+// One gang of requests [r0, r1) of k_gangnode<kFew> (and of k_ganglocal's localities 1 and 2), every thread of the CTA.  `scr`, the
+// scratch copies, is the share's aux byte.  The shared words are the kernel's: s_warp and s_win for grid_min, s_need and s_allocs.
+template <bool kFew>
+__device__ __forceinline__ void gangnode_gang(const GangNodeArgs& a, const DevProfiles& prof, const NodeShare& sh, uint32_t r0, uint32_t r1,
+                                              uint32_t& parity, uint32_t& placed, unsigned long long* s_warp, unsigned long long* s_win,
+                                              uint32_t* s_need, uint32_t* s_allocs, uint32_t tid, uint32_t lane, uint32_t warp) {
+    uint8_t* const scr = sh.aux;
+    uint32_t ri = r0, held = 0;     // kFew: the round's first request; members this CTA committed tentatively in earlier rounds
+    for (;;) {                      // one round; without kFew every path leaves after the first
+        if (tid < kMaxTables) s_need[tid] = 0;
+        if (tid == 0) *s_allocs = 0;
+        __syncthreads();                                    // also orders a commit of the previous gang or round before this one's reads
+        uint32_t mine = 0;
+        for (uint32_t r = ri + tid; r < r1; r += kGnThreads) {      // the slices the remaining ALLOCs take on a node of each table
+            const uint32_t y = a.in[r].y, p = y & 0xFFu;
+            if (((y >> 8) & 0xFFu) != ISL_OP_ALLOC) continue;
+            ++mine;
+            if (p < prof.n)
+                for (uint32_t t = 0; t < a.n_tables; ++t) atomicAdd(&s_need[t], (uint32_t)__ldg(a.sizes + t * ISL_MAX_PROFILES + p));
+        }
+        if (mine) atomicAdd(s_allocs, mine);
+        __syncthreads();
+        const uint32_t allocs = *s_allocs;
+        if (allocs == 0) break;                             // FREEs and NOOPs only: k_prepare's records stand
+        unsigned long long win = ~0ull;
+        for (uint32_t pass = 0; pass < 2; ++pass) {
+            unsigned long long best = ~0ull;
+            for (uint32_t j = sh.j0 + warp; j < sh.j1; j += kGnThreads / 32) {
+                const uint32_t b0 = sh.nb(j) - sh.base, c = sh.nb(j + 1) - sh.base - b0;
+                if (c == 0) continue;                       // an empty node places nothing: depth 0, the floor of every failure
+                const uint32_t t = a.gtab[a.lo + sh.base + b0] & (kMaxTables - 1);
+                uint32_t free_slices = 0;
+                for (uint32_t g = lane; g < c; g += 32) {
+                    const uint32_t o = sh.live[b0 + g];
+                    scr[b0 + g] = (uint8_t)o;
+                    free_slices += 8u - __popc(o);
+                }
+                free_slices = __reduce_add_sync(0xFFFFFFFFu, free_slices);
+                if (pass == 0 && free_slices < s_need[t]) continue;
+                const uint32_t d = gangnode_resolve(a, prof, scr + b0, c, a.lo + sh.base + b0, t, ri, r1, false, lane);
+                best = min(best, d == allocs ? (unsigned long long)j : kGnFail | ((unsigned long long)(0x7FFFFFFFu - d) << 32) | j);
+            }
+            win = grid_min<kGnThreads>(best, a.keys, parity, s_warp, s_win);
+            if (!(win & kGnFail)) break;                    // a node takes the whole gang: the skipped nodes could not have come first
+        }
+        if (!(win & kGnFail)) {
+            const uint32_t j = (uint32_t)win;
+            if (j >= sh.j0 && j < sh.j1 && warp == 0) {     // the owner commits on its live bytes
+                const uint32_t b0 = sh.nb(j) - sh.base, c = sh.nb(j + 1) - sh.base - b0;
+                gangnode_resolve(a, prof, sh.live + b0, c, a.lo + sh.base + b0, a.gtab[a.lo + sh.base + b0] & (kMaxTables - 1), ri, r1, true, lane);
+                placed += allocs;
+            }
+            if (kFew) placed += held;                       // the gang commits: its tentative members count
+            break;
+        }
+        if constexpr (!kFew) {
+            if (blockIdx.x == 0 && warp == 0)               // the deepest failure's depth; ~0ull (no node evaluated) is depth 0 as well
+                abort_gang_members(a.in, a.out, prof, r0, r1, 0x7FFFFFFFu - (uint32_t)((win >> 32) & 0x7FFFFFFFu), lane);
+            break;
+        } else {
+            const uint32_t d = 0x7FFFFFFFu - (uint32_t)((win >> 32) & 0x7FFFFFFFu), j = (uint32_t)win;  // members the round places
+            if (d == 0) {                                   // no node takes m_i: every CTA takes back its tentative members
+                if (warp == 0) gangfew_undo(a, sh, prof, r0, ri, lane);
+                if (blockIdx.x == 0 && warp == 0) abort_gang_members(a.in, a.out, prof, ri, r1, 0, lane);
+                break;
+            }
+            if (j >= sh.j0 && j < sh.j1 && warp == 0) {     // the owner commits the round's d members on its live bytes
+                const uint32_t b0 = sh.nb(j) - sh.base, c = sh.nb(j + 1) - sh.base - b0;
+                gangnode_resolve(a, prof, sh.live + b0, c, a.lo + sh.base + b0, a.gtab[a.lo + sh.base + b0] & (kMaxTables - 1), ri, r1, true, lane);
+                held += d;
+            }
+            ri = skip_allocs(a.in, ri, r1, d, lane);        // every CTA read the same key: all advance alike
+        }
+    }
+}
+
 template <bool kFew>
 __global__ void __launch_bounds__(kGnThreads, 1) k_gangnode(GangNodeArgs a, DevProfiles prof) {
     extern __shared__ __align__(16) uint8_t gn_smem[];
@@ -2773,78 +2849,10 @@ __global__ void __launch_bounds__(kGnThreads, 1) k_gangnode(GangNodeArgs a, DevP
     __shared__ uint32_t s_need[kMaxTables], s_allocs;
     const uint32_t tid = threadIdx.x, lane = tid & 31u, warp = tid >> 5;
     const NodeShare sh(a, gn_smem);
-    uint8_t* const scr = sh.aux;                            // scratch copies of the CTA's nodes
     uint32_t parity = 0, placed = 0;
-    for (uint32_t gi = 0; gi < a.n_gangs; ++gi) {
-        const uint32_t r0 = __ldg(a.gang_off + gi), r1 = __ldg(a.gang_off + gi + 1);
-        uint32_t ri = r0, held = 0;     // kFew: the round's first request; members this CTA committed tentatively in earlier rounds
-        for (;;) {                      // one round; without kFew every path leaves after the first
-            if (tid < kMaxTables) s_need[tid] = 0;
-            if (tid == 0) s_allocs = 0;
-            __syncthreads();                                    // also orders a commit of the previous gang or round before this one's reads
-            uint32_t mine = 0;
-            for (uint32_t r = ri + tid; r < r1; r += kGnThreads) {      // the slices the remaining ALLOCs take on a node of each table
-                const uint32_t y = a.in[r].y, p = y & 0xFFu;
-                if (((y >> 8) & 0xFFu) != ISL_OP_ALLOC) continue;
-                ++mine;
-                if (p < prof.n)
-                    for (uint32_t t = 0; t < a.n_tables; ++t) atomicAdd(&s_need[t], (uint32_t)__ldg(a.sizes + t * ISL_MAX_PROFILES + p));
-            }
-            if (mine) atomicAdd(&s_allocs, mine);
-            __syncthreads();
-            const uint32_t allocs = s_allocs;
-            if (allocs == 0) break;                             // FREEs and NOOPs only: k_prepare's records stand
-            unsigned long long win = ~0ull;
-            for (uint32_t pass = 0; pass < 2; ++pass) {
-                unsigned long long best = ~0ull;
-                for (uint32_t j = sh.j0 + warp; j < sh.j1; j += kGnThreads / 32) {
-                    const uint32_t b0 = sh.nb(j) - sh.base, c = sh.nb(j + 1) - sh.base - b0;
-                    if (c == 0) continue;                       // an empty node places nothing: depth 0, the floor of every failure
-                    const uint32_t t = a.gtab[a.lo + sh.base + b0] & (kMaxTables - 1);
-                    uint32_t free_slices = 0;
-                    for (uint32_t g = lane; g < c; g += 32) {
-                        const uint32_t o = sh.live[b0 + g];
-                        scr[b0 + g] = (uint8_t)o;
-                        free_slices += 8u - __popc(o);
-                    }
-                    free_slices = __reduce_add_sync(0xFFFFFFFFu, free_slices);
-                    if (pass == 0 && free_slices < s_need[t]) continue;
-                    const uint32_t d = gangnode_resolve(a, prof, scr + b0, c, a.lo + sh.base + b0, t, ri, r1, false, lane);
-                    best = min(best, d == allocs ? (unsigned long long)j : kGnFail | ((unsigned long long)(0x7FFFFFFFu - d) << 32) | j);
-                }
-                win = grid_min<kGnThreads>(best, a.keys, parity, s_warp, &s_win);
-                if (!(win & kGnFail)) break;                    // a node takes the whole gang: the skipped nodes could not have come first
-            }
-            if (!(win & kGnFail)) {
-                const uint32_t j = (uint32_t)win;
-                if (j >= sh.j0 && j < sh.j1 && warp == 0) {     // the owner commits on its live bytes
-                    const uint32_t b0 = sh.nb(j) - sh.base, c = sh.nb(j + 1) - sh.base - b0;
-                    gangnode_resolve(a, prof, sh.live + b0, c, a.lo + sh.base + b0, a.gtab[a.lo + sh.base + b0] & (kMaxTables - 1), ri, r1, true, lane);
-                    placed += allocs;
-                }
-                if (kFew) placed += held;                       // the gang commits: its tentative members count
-                break;
-            }
-            if constexpr (!kFew) {
-                if (blockIdx.x == 0 && warp == 0)               // the deepest failure's depth; ~0ull (no node evaluated) is depth 0 as well
-                    abort_gang_members(a.in, a.out, prof, r0, r1, 0x7FFFFFFFu - (uint32_t)((win >> 32) & 0x7FFFFFFFu), lane);
-                break;
-            } else {
-                const uint32_t d = 0x7FFFFFFFu - (uint32_t)((win >> 32) & 0x7FFFFFFFu), j = (uint32_t)win;  // members the round places
-                if (d == 0) {                                   // no node takes m_i: every CTA takes back its tentative members
-                    if (warp == 0) gangfew_undo(a, sh, prof, r0, ri, lane);
-                    if (blockIdx.x == 0 && warp == 0) abort_gang_members(a.in, a.out, prof, ri, r1, 0, lane);
-                    break;
-                }
-                if (j >= sh.j0 && j < sh.j1 && warp == 0) {     // the owner commits the round's d members on its live bytes
-                    const uint32_t b0 = sh.nb(j) - sh.base, c = sh.nb(j + 1) - sh.base - b0;
-                    gangnode_resolve(a, prof, sh.live + b0, c, a.lo + sh.base + b0, a.gtab[a.lo + sh.base + b0] & (kMaxTables - 1), ri, r1, true, lane);
-                    held += d;
-                }
-                ri = skip_allocs(a.in, ri, r1, d, lane);        // every CTA read the same key: all advance alike
-            }
-        }
-    }
+    for (uint32_t gi = 0; gi < a.n_gangs; ++gi)
+        gangnode_gang<kFew>(a, prof, sh, __ldg(a.gang_off + gi), __ldg(a.gang_off + gi + 1), parity, placed, s_warp, &s_win, s_need, &s_allocs,
+                            tid, lane, warp);
     if (tid == 0 && placed) count_placed(a.ctrl, placed);
 }
 
@@ -2864,68 +2872,161 @@ __global__ void __launch_bounds__(kGnThreads, 1) k_gangnode(GangNodeArgs a, DevP
 // finds no GPU as a gang's first ALLOC member (no exclusion in force) is dead for the rest of the call: after the FREEs of k_prepare the
 // occupancy only grows.  Tags run 1..255 with the gang index; the marks are cleared once every 255 gangs.
 // ---------------------------------------------------------------------------------------------
+// One gang of requests [r0, r1) of k_gangspread (and of k_ganglocal's locality 3), every thread of the CTA.  `tag` (1..255) marks the
+// nodes the gang uses in the share's aux byte; tag 1 clears the marks first, so a mark can only equal `tag` when this gang wrote it.
+// `dead`: profiles no GPU of the partition admits any more.  The shared words are the kernel's: s_warp and s_win for grid_min, and the
+// size of the CTA's stack of wins, which is 0 between gangs.
+__device__ __forceinline__ void gangspread_gang(const GangNodeArgs& a, const DevProfiles& prof, const NodeShare& sh, uint2* wins, uint32_t r0,
+                                                uint32_t r1, uint32_t tag, uint32_t& parity, uint32_t& placed, uint32_t& dead,
+                                                uint32_t* s_warp, uint32_t* s_win, uint32_t* s_nwins, uint32_t tid, uint32_t lane,
+                                                uint32_t warp) {
+    const uint32_t base = sh.base, cnt = sh.cnt;
+    uint8_t* const mark = sh.aux;                           // tag of the gang whose member uses the GPU's node
+    if (tag == 1u) for (uint32_t g = tid; g < cnt; g += kGnThreads) mark[g] = 0;
+    __syncthreads();                                        // also orders the previous gang's commit before this gang's reads
+    uint32_t rank = 0, fail = kInf;                         // ALLOC members resolved so far; the rank of the one that found no GPU
+    for (uint32_t r = r0; r < r1; ++r) {
+        const uint32_t y = a.in[r].y, p = y & 0xFFu;
+        if (((y >> 8) & 0xFFu) != ISL_OP_ALLOC) continue;
+        uint32_t win = kInf;                                // an unknown or dead profile fails without a barrier: every CTA knows it
+        if (p < prof.n && !((dead >> p) & 1u)) {
+            uint32_t key = kInf;
+            for (uint32_t g = tid; g < cnt; g += kGnThreads) {
+                if (mark[g] == tag) continue;
+                const uint32_t o = sh.live[g], t = a.n_tables > 1 ? a.gtab[a.lo + base + g] & (kMaxTables - 1) : 0u;
+                const uint32_t row = (t * ISL_MAX_PROFILES + p) * 256;
+                if (__ldg(a.lut + row + o) != ISL_START_NONE) key = min(key, ((uint32_t)__ldg(a.score + row + o) << 24) | (base + g));
+            }
+            win = grid_min<kGnThreads>(key, a.keys, parity, s_warp, s_win);
+            if (win == kInf && rank == 0) dead |= 1u << p;
+        }
+        if (win == kInf) { fail = rank; break; }
+        const uint32_t pos = (win & 0xFFFFFFu) - base;
+        if (pos < cnt) {                                    // this CTA owns the member's node: the node is used for the rest of the gang
+            uint32_t jl = sh.j0, jh = sh.j1;                // nb(jl) <= base + pos < nb(jh): the last such jl is the non-empty node
+            while (jh - jl > 1) {
+                const uint32_t mid = (jl + jh) / 2;
+                if (sh.nb(mid) - base <= pos) jl = mid; else jh = mid;
+            }
+            for (uint32_t g = sh.nb(jl) - base + tid; g < sh.nb(jl + 1) - base; g += kGnThreads) mark[g] = (uint8_t)tag;
+            if (tid == 0) wins[sh.j0 + (*s_nwins)++] = make_uint2(r, pos);     // one win per node of the CTA: the stack fits its nodes
+        }
+        __syncthreads();                                    // the marks and the stack are in place before the next member's scan
+        ++rank;
+    }
+    if (fail == kInf) {                                     // commit: each CTA writes its members; their nodes, hence GPUs, differ
+        const uint32_t nw = *s_nwins;
+        for (uint32_t k = tid; k < nw; k += kGnThreads) {
+            const uint2 w = wins[sh.j0 + k];
+            const uint32_t g = w.y, p = a.in[w.x].y & 0xFFu, t = a.gtab[a.lo + base + g] & (kMaxTables - 1);
+            const uint32_t row = (t * ISL_MAX_PROFILES + p) * 256, o = sh.live[g];
+            const uint32_t start = __ldg(a.lut + row + o), size = __ldg(a.sizes + t * ISL_MAX_PROFILES + p);
+            const uint32_t o2 = o | slice_span(start, size);
+            sh.live[g] = (uint8_t)o2;
+            a.occ[a.lo + base + g] = (uint8_t)o2;
+            a.out[w.x] = pack_result(flip_gpu(a.lo + base + g, prof.flip), start, size, ISL_ST_PLACED);
+        }
+        placed += nw;
+    } else if (blockIdx.x == 0 && warp == 0) {              // the member at rank `fail` keeps its record, every other ALLOC member aborts
+        abort_gang_members(a.in, a.out, prof, r0, r1, fail, lane);
+    }
+    __syncthreads();                                        // every thread has read the stack's size
+    if (tid == 0) *s_nwins = 0;
+}
+
 __global__ void __launch_bounds__(kGnThreads, 1) k_gangspread(GangNodeArgs a, DevProfiles prof, uint2* wins) {
     extern __shared__ __align__(16) uint8_t gs_smem[];
     __shared__ uint32_t s_warp[kGnThreads / 32];
     __shared__ uint32_t s_win, s_nwins;
     const uint32_t tid = threadIdx.x, lane = tid & 31u, warp = tid >> 5;
     const NodeShare sh(a, gs_smem);
-    const uint32_t base = sh.base, cnt = sh.cnt;
-    uint8_t* const mark = sh.aux;                           // tag of the gang whose member uses the GPU's node
     if (tid == 0) s_nwins = 0;
     uint32_t parity = 0, placed = 0, dead = 0;                            // dead: profiles no GPU of the partition admits any more
+    for (uint32_t gi = 0; gi < a.n_gangs; ++gi)                           // tags run 1..255 with the gang index
+        gangspread_gang(a, prof, sh, wins, __ldg(a.gang_off + gi), __ldg(a.gang_off + gi + 1), 1u + gi % 255u, parity, placed, dead,
+                        s_warp, &s_win, &s_nwins, tid, lane, warp);
+    if (tid == 0 && placed) count_placed(a.ctrl, placed);
+}
+
+// ---------------------------------------------------------------------------------------------
+// k_ganglocal: isl_place_gangs on an engine created with ISL_FLAG_GANG_LOCALITY (DESIGN.md 4.12): each gang names its own node locality
+// (locality[gi], one byte per gang, checked on the host), and the gangs run in array order, each on the occupancy the earlier ones left.
+// One cooperative launch per call behind k_prepare, with k_gangnode's layout.  The byte is the same for every CTA, so the branch is
+// grid-uniform, and every barrier depends only on the gang offsets, the locality bytes and the winning keys.
+//   1, 2      gangnode_gang<false> / <true>: k_gangnode's gang, one node or few nodes.  Its scratch copies overwrite the aux bytes.
+//   3         gangspread_gang: k_gangspread's gang.  Tags count locality-3 gangs and restart at 1, which clears the marks, after every
+//             locality-1 or -2 gang, whose scratch copies may equal any tag.
+//   0 (any)   ganglocal_any: rules 2-4, member by member over the whole share.
+// The dead-profile mask is shared by localities 0 and 3: a bit is set only when a gang's first ALLOC member finds no GPU, on a state
+// without tentative slices; after k_prepare's FREEs the occupancy only grows and an abort restores it exactly, so the bit stays valid.
+// ---------------------------------------------------------------------------------------------
+// One gang of locality 0: every CTA takes the minimum of score(t, p, o) << 24 | partition-local storage position over its live bytes
+// (k_gangspread's key with no GPU masked), grid_min gives every CTA the member's GPU, and the CTA that owns it commits the member
+// tentatively to its live share, the occupancy and a PLACED record.  A member with no GPU aborts the gang: every CTA takes back the
+// tentative members on its own nodes (gangfew_undo), and CTA 0 reports the members after the failing one GANG_ABORTED.  An unknown or
+// dead profile fails without a barrier: gangfew_undo only touches records on the CTA's own nodes, which that CTA wrote itself.
+__device__ __forceinline__ void ganglocal_any(const GangNodeArgs& a, const DevProfiles& prof, const NodeShare& sh, uint32_t r0, uint32_t r1,
+                                              uint32_t& parity, uint32_t& placed, uint32_t& dead, uint32_t* s_warp, uint32_t* s_win,
+                                              uint32_t tid, uint32_t lane, uint32_t warp) {
+    const uint32_t base = sh.base, cnt = sh.cnt;
+    __syncthreads();                                        // the previous gang's commits are in the live share before this gang's reads
+    uint32_t rank = 0;                                      // ALLOC members committed tentatively so far
+    for (uint32_t r = r0; r < r1; ++r) {
+        const uint32_t y = a.in[r].y, p = y & 0xFFu;
+        if (((y >> 8) & 0xFFu) != ISL_OP_ALLOC) continue;
+        uint32_t win = kInf;
+        if (p < prof.n && !((dead >> p) & 1u)) {
+            uint32_t key = kInf;
+            for (uint32_t g = tid; g < cnt; g += kGnThreads) {
+                const uint32_t o = sh.live[g], t = a.n_tables > 1 ? a.gtab[a.lo + base + g] & (kMaxTables - 1) : 0u;
+                const uint32_t row = (t * ISL_MAX_PROFILES + p) * 256;
+                if (__ldg(a.lut + row + o) != ISL_START_NONE) key = min(key, ((uint32_t)__ldg(a.score + row + o) << 24) | (base + g));
+            }
+            win = grid_min<kGnThreads>(key, a.keys, parity, s_warp, s_win);
+            if (win == kInf && rank == 0) dead |= 1u << p;  // no tentative slice of this gang is in the way
+        }
+        if (win == kInf) {
+            if (warp == 0) gangfew_undo(a, sh, prof, r0, r, lane);
+            if (blockIdx.x == 0 && warp == 0) abort_gang_members(a.in, a.out, prof, r, r1, 0, lane);
+            return;
+        }
+        const uint32_t pos = (win & 0xFFFFFFu) - base;
+        if (pos < cnt && tid == 0) {                        // the owner commits the member tentatively
+            const uint32_t t = a.gtab[a.lo + base + pos] & (kMaxTables - 1), row = (t * ISL_MAX_PROFILES + p) * 256, o = sh.live[pos];
+            const uint32_t start = __ldg(a.lut + row + o), size = __ldg(a.sizes + t * ISL_MAX_PROFILES + p);
+            const uint32_t o2 = o | slice_span(start, size);
+            sh.live[pos] = (uint8_t)o2;
+            a.occ[a.lo + base + pos] = (uint8_t)o2;
+            a.out[r] = pack_result(flip_gpu(a.lo + base + pos, prof.flip), start, size, ISL_ST_PLACED);
+        }
+        __syncthreads();                                    // the commit is in the live share before the next member's scan
+        ++rank;
+    }
+    if (blockIdx.x == 0) placed += rank;                    // the gang commits: CTA 0 counts its members once
+}
+
+__global__ void __launch_bounds__(kGnThreads, 1) k_ganglocal(GangNodeArgs a, DevProfiles prof, uint2* wins, const uint8_t* __restrict__ locality) {
+    extern __shared__ __align__(16) uint8_t gl_smem[];
+    __shared__ unsigned long long s_warp64[kGnThreads / 32];
+    __shared__ unsigned long long s_win64;
+    __shared__ uint32_t s_warp32[kGnThreads / 32];
+    __shared__ uint32_t s_win32, s_nwins, s_need[kMaxTables], s_allocs;
+    const uint32_t tid = threadIdx.x, lane = tid & 31u, warp = tid >> 5;
+    const NodeShare sh(a, gl_smem);
+    if (tid == 0) s_nwins = 0;
+    uint32_t parity = 0, placed = 0, dead = 0, spread = 0;  // spread: locality-3 gangs since the marks were last cleared
     for (uint32_t gi = 0; gi < a.n_gangs; ++gi) {
-        const uint32_t r0 = __ldg(a.gang_off + gi), r1 = __ldg(a.gang_off + gi + 1), tag = 1u + gi % 255u;
-        if (tag == 1u) for (uint32_t g = tid; g < cnt; g += kGnThreads) mark[g] = 0;
-        __syncthreads();                                    // also orders the previous gang's commit before this gang's reads
-        uint32_t rank = 0, fail = kInf;                     // ALLOC members resolved so far; the rank of the one that found no GPU
-        for (uint32_t r = r0; r < r1; ++r) {
-            const uint32_t y = a.in[r].y, p = y & 0xFFu;
-            if (((y >> 8) & 0xFFu) != ISL_OP_ALLOC) continue;
-            uint32_t win = kInf;                            // an unknown or dead profile fails without a barrier: every CTA knows it
-            if (p < prof.n && !((dead >> p) & 1u)) {
-                uint32_t key = kInf;
-                for (uint32_t g = tid; g < cnt; g += kGnThreads) {
-                    if (mark[g] == tag) continue;
-                    const uint32_t o = sh.live[g], t = a.n_tables > 1 ? a.gtab[a.lo + base + g] & (kMaxTables - 1) : 0u;
-                    const uint32_t row = (t * ISL_MAX_PROFILES + p) * 256;
-                    if (__ldg(a.lut + row + o) != ISL_START_NONE) key = min(key, ((uint32_t)__ldg(a.score + row + o) << 24) | (base + g));
-                }
-                win = grid_min<kGnThreads>(key, a.keys, parity, s_warp, &s_win);
-                if (win == kInf && rank == 0) dead |= 1u << p;
-            }
-            if (win == kInf) { fail = rank; break; }
-            const uint32_t pos = (win & 0xFFFFFFu) - base;
-            if (pos < cnt) {                                // this CTA owns the member's node: the node is used for the rest of the gang
-                uint32_t jl = sh.j0, jh = sh.j1;            // nb(jl) <= base + pos < nb(jh): the last such jl is the non-empty node
-                while (jh - jl > 1) {
-                    const uint32_t mid = (jl + jh) / 2;
-                    if (sh.nb(mid) - base <= pos) jl = mid; else jh = mid;
-                }
-                for (uint32_t g = sh.nb(jl) - base + tid; g < sh.nb(jl + 1) - base; g += kGnThreads) mark[g] = (uint8_t)tag;
-                if (tid == 0) wins[sh.j0 + s_nwins++] = make_uint2(r, pos);     // one win per node of the CTA: the stack fits its nodes
-            }
-            __syncthreads();                                // the marks and the stack are in place before the next member's scan
-            ++rank;
+        const uint32_t r0 = __ldg(a.gang_off + gi), r1 = __ldg(a.gang_off + gi + 1), loc = __ldg(locality + gi);
+        if (loc == ISL_GANG_ONE_NODE || loc == ISL_GANG_FEW_NODES) {
+            if (loc == ISL_GANG_ONE_NODE) gangnode_gang<false>(a, prof, sh, r0, r1, parity, placed, s_warp64, &s_win64, s_need, &s_allocs, tid, lane, warp);
+            else gangnode_gang<true>(a, prof, sh, r0, r1, parity, placed, s_warp64, &s_win64, s_need, &s_allocs, tid, lane, warp);
+            spread = 0;                                     // the scratch copies overwrote the marks
+        } else if (loc == ISL_GANG_DISTINCT_NODES) {
+            gangspread_gang(a, prof, sh, wins, r0, r1, 1u + spread % 255u, parity, placed, dead, s_warp32, &s_win32, &s_nwins, tid, lane, warp);
+            ++spread;
+        } else {
+            ganglocal_any(a, prof, sh, r0, r1, parity, placed, dead, s_warp32, &s_win32, tid, lane, warp);
         }
-        if (fail == kInf) {                                 // commit: each CTA writes its members; their nodes, hence GPUs, differ
-            const uint32_t nw = s_nwins;
-            for (uint32_t k = tid; k < nw; k += kGnThreads) {
-                const uint2 w = wins[sh.j0 + k];
-                const uint32_t g = w.y, p = a.in[w.x].y & 0xFFu, t = a.gtab[a.lo + base + g] & (kMaxTables - 1);
-                const uint32_t row = (t * ISL_MAX_PROFILES + p) * 256, o = sh.live[g];
-                const uint32_t start = __ldg(a.lut + row + o), size = __ldg(a.sizes + t * ISL_MAX_PROFILES + p);
-                const uint32_t o2 = o | slice_span(start, size);
-                sh.live[g] = (uint8_t)o2;
-                a.occ[a.lo + base + g] = (uint8_t)o2;
-                a.out[w.x] = pack_result(flip_gpu(a.lo + base + g, prof.flip), start, size, ISL_ST_PLACED);
-            }
-            placed += nw;
-        } else if (blockIdx.x == 0 && warp == 0) {          // the member at rank `fail` keeps its record, every other ALLOC member aborts
-            abort_gang_members(a.in, a.out, prof, r0, r1, fail, lane);
-        }
-        __syncthreads();                                    // every thread has read the stack's size
-        if (tid == 0) s_nwins = 0;
     }
     if (tid == 0 && placed) count_placed(a.ctrl, placed);
 }

@@ -180,8 +180,8 @@ struct isl_engine {
         DevMem<uint32_t> node_off, tree, fit, nodes;
         uint8_t width[kMaxTables] = {};
     } nf;
-    // one-node, few-node and distinct-node gangs (ISL_FLAG_GANG_ONE_NODE, k_gangnode<false>; ISL_FLAG_GANG_FEW_NODES, k_gangnode<true>;
-    // ISL_FLAG_GANG_DISTINCT_NODES, k_gangspread): the inventory's
+    // one-node, few-node and distinct-node gangs and per-gang locality (ISL_FLAG_GANG_ONE_NODE, k_gangnode<false>; ISL_FLAG_GANG_FEW_NODES,
+    // k_gangnode<true>; ISL_FLAG_GANG_DISTINCT_NODES, k_gangspread; ISL_FLAG_GANG_LOCALITY, k_ganglocal): the inventory's
     // node offsets in storage order (host and device, isl_load_inventory), the scratch copies (k_gangnode) or node-used marks
     // (k_gangspread) when the shares do not fit in shared memory, the per-CTA minima, and k_gangspread's per-CTA stacks of wins
     struct GangNode {
@@ -191,6 +191,7 @@ struct isl_engine {
         DevMem<unsigned long long> keys;
         DevMem<uint2> wins;
         int smem_optin = 0;          // dynamic shared memory one CTA of k_gangnode or k_gangspread may have
+        int local_optin = 0;         // the same for k_ganglocal, whose static shared memory is its own
     } gn;
     unsigned long long wait_ns = 20000000000ull;   // a starved device-side wait traps after this long (ISL_WAIT_SECONDS overrides the 20 s)
     uint32_t window = 0;             // causal window of stream calls (isl_set_causal_window): chunk c starts after chunk c - window is committed
@@ -445,10 +446,11 @@ int run_gangs(isl_engine* e, uint32_t n_gangs, const uint32_t* d_gang_off, uint3
     return ISL_OK;
 }
 
-// The layout k_gangnode and k_gangspread share, over the nodes the partition touches: each CTA gets whole nodes, about Gr / grid GPUs
-// (one CTA per SM at most, one per 512 GPUs below that, never more than nodes), and 2 bytes per GPU of its share in shared memory when
-// they fit, else in global memory (gn.scratch).  Fills every field of `a`; *nodes = the nodes the partition touches.
-int gang_layout(isl_engine* e, const void* kernel, uint32_t n_gangs, const uint32_t* d_gang_off, const uint2* d_in, uint2* d_out,
+// The layout k_gangnode, k_gangspread and k_ganglocal share, over the nodes the partition touches: each CTA gets whole nodes, about
+// Gr / grid GPUs (one CTA per SM at most, one per 512 GPUs below that, never more than nodes), and 2 bytes per GPU of its share in shared
+// memory when they fit in `smem_optin` (the kernel's dynamic shared memory opt-in), else in global memory (gn.scratch).  Fills every
+// field of `a`; *nodes = the nodes the partition touches.
+int gang_layout(isl_engine* e, const void* kernel, int smem_optin, uint32_t n_gangs, const uint32_t* d_gang_off, const uint2* d_in, uint2* d_out,
                 GangNodeArgs& a, uint32_t* grid_out, size_t* smem_out, uint32_t* nodes) {
     auto& gn = e->gn;
     const uint32_t Gr = e->hi - e->lo;
@@ -467,7 +469,7 @@ int gang_layout(isl_engine* e, const void* kernel, uint32_t n_gangs, const uint3
     }
     // the live bytes and the second byte per GPU (scratch copies or marks) of a share in shared memory when both fit, else in global memory
     size_t smem = ((size_t)share + 15) / 16 * 16 * 2;
-    if (smem > (size_t)gn.smem_optin ||
+    if (smem > (size_t)smem_optin ||
         cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, kGnThreads, smem) != cudaSuccess || per_sm < 1) {
         cudaGetLastError();
         smem = 0;
@@ -487,7 +489,7 @@ int run_gangnode(isl_engine* e, uint32_t n_gangs, const uint32_t* d_gang_off, ui
     GangNodeArgs a;
     uint32_t grid, nodes;
     size_t smem;
-    if (int rc = gang_layout(e, (const void*)k_gangnode<false>, n_gangs, d_gang_off, d_in, d_out, a, &grid, &smem, &nodes)) return rc;
+    if (int rc = gang_layout(e, (const void*)k_gangnode<false>, e->gn.smem_optin, n_gangs, d_gang_off, d_in, d_out, a, &grid, &smem, &nodes)) return rc;
     void* params[] = {&a, &e->prof};
     if (int rc = launch_cooperative(e, (const void*)k_gangnode<false>, "k_gangnode", grid, kGnThreads, smem, params)) return rc;
     finish_batch(e, n, true);
@@ -501,7 +503,7 @@ int run_gangfew(isl_engine* e, uint32_t n_gangs, const uint32_t* d_gang_off, uin
     GangNodeArgs a;
     uint32_t grid, nodes;
     size_t smem;
-    if (int rc = gang_layout(e, (const void*)k_gangnode<true>, n_gangs, d_gang_off, d_in, d_out, a, &grid, &smem, &nodes)) return rc;
+    if (int rc = gang_layout(e, (const void*)k_gangnode<true>, e->gn.smem_optin, n_gangs, d_gang_off, d_in, d_out, a, &grid, &smem, &nodes)) return rc;
     void* params[] = {&a, &e->prof};
     if (int rc = launch_cooperative(e, (const void*)k_gangnode<true>, "k_gangnode<true>", grid, kGnThreads, smem, params)) return rc;
     finish_batch(e, n, true);
@@ -515,11 +517,28 @@ int run_gangspread(isl_engine* e, uint32_t n_gangs, const uint32_t* d_gang_off, 
     GangNodeArgs a;
     uint32_t grid, nodes;
     size_t smem;
-    if (int rc = gang_layout(e, (const void*)k_gangspread, n_gangs, d_gang_off, d_in, d_out, a, &grid, &smem, &nodes)) return rc;
+    if (int rc = gang_layout(e, (const void*)k_gangspread, e->gn.smem_optin, n_gangs, d_gang_off, d_in, d_out, a, &grid, &smem, &nodes)) return rc;
     ISL_CUDA(e, e->gn.wins.reserve(nodes));
     uint2* wins = e->gn.wins;
     void* params[] = {&a, &e->prof, &wins};
     if (int rc = launch_cooperative(e, (const void*)k_gangspread, "k_gangspread", grid, kGnThreads, smem, params)) return rc;
+    finish_batch(e, n, true);
+    return ISL_OK;
+}
+
+// isl_place_gangs on an ISL_FLAG_GANG_LOCALITY engine: frees + defaults, then one cooperative k_ganglocal (gang_layout with its own
+// opt-in), which places each gang by the locality byte at d_locality[gang]; wins as in run_gangspread.
+int run_ganglocal(isl_engine* e, uint32_t n_gangs, const uint32_t* d_gang_off, const uint8_t* d_locality, uint32_t n, const uint2* d_in,
+                  uint2* d_out) {
+    if (int rc = prepare_batch(e, n, d_in, d_out)) return rc;
+    GangNodeArgs a;
+    uint32_t grid, nodes;
+    size_t smem;
+    if (int rc = gang_layout(e, (const void*)k_ganglocal, e->gn.local_optin, n_gangs, d_gang_off, d_in, d_out, a, &grid, &smem, &nodes)) return rc;
+    ISL_CUDA(e, e->gn.wins.reserve(nodes));
+    uint2* wins = e->gn.wins;
+    void* params[] = {&a, &e->prof, &wins, &d_locality};
+    if (int rc = launch_cooperative(e, (const void*)k_ganglocal, "k_ganglocal", grid, kGnThreads, smem, params)) return rc;
     finish_batch(e, n, true);
     return ISL_OK;
 }
@@ -1152,6 +1171,10 @@ int isl_create(const isl_config* cfg, isl_engine** out) {
     // few-node gangs: a third locality mode, exclusive with the other two, and, like them, not with a pod on every node nor node scoring
     if ((cfg->flags & ISL_FLAG_GANG_FEW_NODES) &&
         ((cfg->flags & (ISL_FLAG_GANG_ONE_NODE | ISL_FLAG_GANG_DISTINCT_NODES | ISL_FLAG_ALL_NODES)) || node_scoring(cfg->policy))) return ISL_EINVAL;
+    // per-gang locality: the gangs name the locality the other three flags fix for the engine; not with a pod on every node nor node scoring
+    if ((cfg->flags & ISL_FLAG_GANG_LOCALITY) &&
+        ((cfg->flags & (ISL_FLAG_GANG_ONE_NODE | ISL_FLAG_GANG_DISTINCT_NODES | ISL_FLAG_GANG_FEW_NODES | ISL_FLAG_ALL_NODES)) ||
+         node_scoring(cfg->policy))) return ISL_EINVAL;
     if (request_major(cfg->policy) && cfg->max_gpus > kBfMaxGpus) return ISL_ERANGE;
     if (cfg->quirks & ~ISL_QUIRKS_REF_EXACT) return ISL_EINVAL;
     isl_engine* e = new (std::nothrow) isl_engine;
@@ -1181,7 +1204,7 @@ int isl_create(const isl_config* cfg, isl_engine** out) {
         const void* kernels[] = {(const void*)k_prepare, (const void*)k_partition, (const void*)k_set_flag, (const void*)k_few, (const void*)k_build_lut, (const void*)k_eval_starts,
                                  (const void*)k_free_spans, (const void*)k_capacity, (const void*)k_sweep_count, (const void*)k_sweep_scatter, (const void*)k_commit, (const void*)k_bestfit<false>, (const void*)k_bestfit<true>,
                                  (const void*)k_bestfit<false, true>, (const void*)k_bestfit<true, true>, (const void*)k_victim_map, (const void*)k_preempt, (const void*)k_nodefit, (const void*)k_gangnode<false>, (const void*)k_gangnode<true>, (const void*)k_gangspread,
-                                 (const void*)k_chain<1>, (const void*)k_chain<2>, (const void*)k_chain<4>, (const void*)k_small<1>, (const void*)k_small<2>, (const void*)k_small<4>};
+                                 (const void*)k_ganglocal, (const void*)k_chain<1>, (const void*)k_chain<2>, (const void*)k_chain<4>, (const void*)k_small<1>, (const void*)k_small<2>, (const void*)k_small<4>};
         const void* pipes[] = {(const void*)k_pipeline<1, false, false>, (const void*)k_pipeline<1, true, false>, (const void*)k_pipeline<2, false, false>, (const void*)k_pipeline<2, true, false>,
                                (const void*)k_pipeline<4, false, false>, (const void*)k_pipeline<4, true, false>,
                                (const void*)k_pipeline<1, false, true>, (const void*)k_pipeline<1, true, true>, (const void*)k_pipeline<2, false, true>, (const void*)k_pipeline<2, true, true>,
@@ -1207,6 +1230,10 @@ int isl_create(const isl_config* cfg, isl_engine** out) {
         for (const void* k : gangs) { ISL_TRY(cudaFuncGetAttributes(&fa, k)); gang_static = std::max(gang_static, fa.sharedSizeBytes); }
         e->gn.smem_optin = optin - (int)gang_static;
         for (const void* k : gangs) ISL_TRY(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, e->gn.smem_optin));
+        // k_ganglocal sizes its shares by its own static shared memory, so the switch of the three above does not move with it
+        ISL_TRY(cudaFuncGetAttributes(&fa, k_ganglocal));
+        e->gn.local_optin = optin - (int)fa.sharedSizeBytes;
+        ISL_TRY(cudaFuncSetAttribute((const void*)k_ganglocal, cudaFuncAttributeMaxDynamicSharedMemorySize, e->gn.local_optin));
     }
     e->occ_bytes = ((size_t)cfg->max_gpus + kSweepBlock - 1) / kSweepBlock * kSweepBlock;
     const uint32_t max_tiles = ceil_div(cfg->max_batch, kTile) + 4096;   // + one partial tile per batch of a stream
@@ -1417,8 +1444,8 @@ int isl_load_inventory(isl_engine* e, uint32_t n_nodes, const uint32_t* node_off
         ISL_CUDA(e, e->nf.node_off.replace((size_t)n_nodes + 1));
         ISL_CUDA(e, cudaMemcpyAsync(e->nf.node_off, node_off, ((size_t)n_nodes + 1) * sizeof(uint32_t), cudaMemcpyHostToDevice, e->stream));
     }
-    if (e->cfg.flags & (ISL_FLAG_GANG_ONE_NODE | ISL_FLAG_GANG_FEW_NODES | ISL_FLAG_GANG_DISTINCT_NODES)) {   // k_gangnode and
-                                                                    // k_gangspread walk the nodes in storage order (reversed under right-to-left)
+    if (e->cfg.flags & (ISL_FLAG_GANG_ONE_NODE | ISL_FLAG_GANG_FEW_NODES | ISL_FLAG_GANG_DISTINCT_NODES | ISL_FLAG_GANG_LOCALITY)) {
+        // k_gangnode, k_gangspread and k_ganglocal walk the nodes in storage order (reversed under right-to-left)
         auto& off = e->gn.off;
         off.assign(node_off, node_off + n_nodes + 1);
         if (e->prof.flip) { std::reverse(off.begin(), off.end()); for (auto& x : off) x = G - x; }
@@ -1504,6 +1531,19 @@ int isl_place_gangs(isl_engine* e, uint32_t n_gangs, const uint32_t* gang_off, c
     for (uint32_t i = 0; i < n_gangs; ++i) if (gang_off[i + 1] <= gang_off[i]) return ISL_EINVAL;      // no empty gang
     const uint32_t n = n_gangs ? gang_off[n_gangs] : 0;
     if (n && (!in || !out)) return ISL_EINVAL;
+    std::vector<uint8_t> locality;                                  // ISL_FLAG_GANG_LOCALITY: each gang's byte (L1, L4), 0 without ALLOCs
+    if (e->cfg.flags & ISL_FLAG_GANG_LOCALITY) {
+        locality.assign(n_gangs, (uint8_t)ISL_GANG_ANY_NODES);
+        for (uint32_t i = 0; i < n_gangs; ++i) {
+            bool named = false;
+            for (uint32_t r = gang_off[i]; r < gang_off[i + 1]; ++r) {
+                if (in[r].op != ISL_OP_ALLOC) continue;
+                if (in[r].start > ISL_GANG_DISTINCT_NODES || (named && in[r].start != locality[i])) return ISL_EINVAL;
+                locality[i] = in[r].start;
+                named = true;
+            }
+        }
+    }
     if (e->cfg.flags & ISL_FLAG_ALL_NODES) return ISL_EINVAL;      // one pod on every node with capacity: no all-or-nothing meaning
     if (node_scoring(e->cfg.policy)) return ISL_EINVAL;            // gangs under node scoring are not implemented
     if (n > e->cfg.max_batch) return ISL_ERANGE;
@@ -1511,11 +1551,15 @@ int isl_place_gangs(isl_engine* e, uint32_t n_gangs, const uint32_t* gang_off, c
     if (guard.rc) return guard.rc;
     if (n == 0) return ISL_OK;
     if (e->hi == e->lo || e->hi - e->lo > kBfMaxGpus) return ISL_ERANGE;          // the class bitmaps of k_bestfit
-    ISL_CUDA(e, e->d_scratch.reserve(((size_t)n_gangs + 1) * sizeof(uint32_t)));
+    ISL_CUDA(e, e->d_scratch.reserve(((size_t)n_gangs + 1) * sizeof(uint32_t) + locality.size()));
     uint32_t* d_gang_off = reinterpret_cast<uint32_t*>(e->d_scratch.get());
+    const uint8_t* d_locality = reinterpret_cast<const uint8_t*>(d_gang_off + n_gangs + 1);      // the bytes right after the offsets
     ISL_CUDA(e, cudaMemcpyAsync(d_gang_off, gang_off, ((size_t)n_gangs + 1) * sizeof(uint32_t), cudaMemcpyHostToDevice, e->stream));
+    if (!locality.empty())
+        ISL_CUDA(e, cudaMemcpyAsync((void*)d_locality, locality.data(), locality.size(), cudaMemcpyHostToDevice, e->stream));
     ISL_CUDA(e, cudaMemcpyAsync(e->d_req, in, (size_t)n * sizeof(isl_request), cudaMemcpyHostToDevice, e->stream));
-    if (int rc = (e->cfg.flags & ISL_FLAG_GANG_ONE_NODE)        ? run_gangnode(e, n_gangs, d_gang_off, n, e->d_req, e->d_res)
+    if (int rc = (e->cfg.flags & ISL_FLAG_GANG_LOCALITY)        ? run_ganglocal(e, n_gangs, d_gang_off, d_locality, n, e->d_req, e->d_res)
+                 : (e->cfg.flags & ISL_FLAG_GANG_ONE_NODE)        ? run_gangnode(e, n_gangs, d_gang_off, n, e->d_req, e->d_res)
                  : (e->cfg.flags & ISL_FLAG_GANG_FEW_NODES)      ? run_gangfew(e, n_gangs, d_gang_off, n, e->d_req, e->d_res)
                  : (e->cfg.flags & ISL_FLAG_GANG_DISTINCT_NODES) ? run_gangspread(e, n_gangs, d_gang_off, n, e->d_req, e->d_res)
                                                                  : run_gangs(e, n_gangs, d_gang_off, n, e->d_req, e->d_res)) return rc;

@@ -33,6 +33,8 @@ FLAG_TIMING, FLAG_NO_PIPELINE, FLAG_FORCE_PIPELINE, FLAG_TRACE, FLAG_NO_SMALL, F
 FLAG_GANG_ONE_NODE = 64     # isl_place_gangs puts every member of a gang on one node (include/islplace.h)
 FLAG_GANG_DISTINCT_NODES = 128  # isl_place_gangs puts every member of a gang on a different node (include/islplace.h)
 FLAG_GANG_FEW_NODES = 256  # isl_place_gangs puts a gang on one node when one takes it, else on as few nodes as it greedily can
+FLAG_GANG_LOCALITY = 512  # isl_place_gangs takes each gang's node locality from its ALLOC members' start byte (GANG_*)
+GANG_ANY_NODES, GANG_ONE_NODE, GANG_FEW_NODES, GANG_DISTINCT_NODES = 0, 1, 2, 3     # node locality of one gang (include/islplace.h L1)
 SPEC_AUTO, SPEC_OFF, SPEC_ON = 0, 1, 2
 
 # ---- record layouts -------------------------------------------------------------------------
@@ -233,6 +235,7 @@ class Engine:
             raise EngineError(rc, "isl_create")
         self._h = h
         self.max_batch = max_batch
+        self.flags = cfg.flags
 
     # -- lifetime
     def close(self):
@@ -333,7 +336,7 @@ class Engine:
         self._check(self._lib.isl_place_batch_range(self._h, lo, hi, len(requests), _ptr(requests), _ptr(out)), "isl_place_batch_range")
         return out
 
-    def place_gangs(self, requests: np.ndarray, gang_off) -> np.ndarray:
+    def place_gangs(self, requests: np.ndarray, gang_off, locality=None) -> np.ndarray:
         """All-or-nothing groups: gang i is ``requests[gang_off[i]:gang_off[i + 1]]`` (``gang_off[0] == 0``, no empty gang, the last
         offset is ``len(requests)``).  A gang commits only when every ALLOC member is placed; otherwise the first member that did not fit
         keeps its record and every other ALLOC member reports ``ST_GANG_ABORTED`` (include/islplace.h).  On an engine created with
@@ -341,11 +344,25 @@ class Engine:
         node gets past keeps its record.  On an engine created with ``FLAG_GANG_DISTINCT_NODES`` every member of a gang lands on a
         different node, resolved greedily member by member, and the first member with no GPU on an unused node keeps its record.  On an
         engine created with ``FLAG_GANG_FEW_NODES`` a gang goes to one node when one takes it whole, else in rounds: each round the node
-        that places the most of the remaining members takes them; when no node places the next member, that member keeps its record."""
+        that places the most of the remaining members takes them; when no node places the next member, that member keeps its record.
+
+        On an engine created with ``FLAG_GANG_LOCALITY`` each gang is placed by its own locality, the ``start`` byte of its ALLOC members
+        (``GANG_ANY_NODES``, ``GANG_ONE_NODE``, ``GANG_FEW_NODES`` or ``GANG_DISTINCT_NODES``).  ``locality``: one such value per gang,
+        written into the ``start`` of the ALLOC members of a copy of ``requests``; it needs an engine created with the flag."""
         requests = np.ascontiguousarray(requests, dtype=REQUEST_DTYPE)
         gang_off = np.ascontiguousarray(gang_off, dtype=np.uint32)
         if len(gang_off) == 0 or int(gang_off[-1]) != len(requests):
             raise ValueError("gang_off must have n_gangs + 1 entries ending at len(requests)")
+        if locality is not None:
+            if not self.flags & FLAG_GANG_LOCALITY:
+                raise ValueError("a locality per gang needs an engine created with FLAG_GANG_LOCALITY")
+            locality = np.asarray(locality, dtype=np.int64)
+            if len(locality) != len(gang_off) - 1:
+                raise ValueError("one locality per gang")
+            requests = requests.copy()
+            per_request = np.repeat(locality, np.diff(gang_off.astype(np.int64)))
+            alloc = requests["op"] == OP_ALLOC
+            requests["start"][alloc] = per_request[alloc].astype(np.uint8)
         out = np.empty(len(requests), dtype=RESULT_DTYPE)
         self._check(self._lib.isl_place_gangs(self._h, len(gang_off) - 1, _ptr(gang_off), _ptr(requests), _ptr(out)), "isl_place_gangs")
         return out

@@ -217,10 +217,18 @@ Outcome InstasliceReconciler::commitOrVeto(InstasliceList& list, AllocationPolic
 }
 
 std::vector<GangOutcome> InstasliceReconciler::PlaceGangs(InstasliceList& list, AllocationPolicy& policy, const std::vector<std::vector<PendingPod>>& gangs) {
+    return PlaceGangs(list, policy, gangs, {});
+}
+
+// `locality` empty: every ALLOC keeps start 0, which an engine without ISL_FLAG_GANG_LOCALITY ignores
+std::vector<GangOutcome> InstasliceReconciler::PlaceGangs(InstasliceList& list, AllocationPolicy& policy, const std::vector<std::vector<PendingPod>>& gangs,
+                                                          const std::vector<uint8_t>& locality) {
     std::vector<GangOutcome> out(gangs.size());
+    if (!locality.empty() && locality.size() != gangs.size()) throw std::runtime_error("one locality per gang");
     if (gangs.empty()) return out;
     if (orphans_ && gangs.size() > 1) {         // the veto must see one gang at a time: a vetoed gang leaves no trace before the next
-        for (size_t g = 0; g < gangs.size(); ++g) out[g] = PlaceGangs(list, policy, {gangs[g]})[0];
+        for (size_t g = 0; g < gangs.size(); ++g)
+            out[g] = PlaceGangs(list, policy, {gangs[g]}, locality.empty() ? std::vector<uint8_t>{} : std::vector<uint8_t>{locality[g]})[0];
         return out;
     }
     std::vector<std::string> names;
@@ -230,7 +238,10 @@ std::vector<GangOutcome> InstasliceReconciler::PlaceGangs(InstasliceList& list, 
         for (const PendingPod& p : gang) names.push_back(p.ProfileName);
         off.push_back((uint32_t)names.size());
     }
-    const std::vector<isl_request> req = requests(names);
+    std::vector<isl_request> req = requests(names);
+    if (!locality.empty())
+        for (size_t g = 0; g < gangs.size(); ++g)
+            for (uint32_t i = off[g]; i < off[g + 1]; ++i) req[i].start = locality[g];
     std::vector<isl_result> res(names.size());
     check(isl_place_gangs(h_, (uint32_t)gangs.size(), off.data(), req.data(), res.data()), h_, "isl_place_gangs");
     for (size_t g = 0; g < gangs.size(); ++g) {

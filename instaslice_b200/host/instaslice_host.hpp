@@ -89,7 +89,8 @@ public:
     // policy: the engine's isl_config.policy, e.g. ISL_POLICY_MOST_ALLOCATED to pack MIG pods onto the fullest nodes or
     // ISL_POLICY_LEAST_ALLOCATED to spread them (include/islplace.h).  flags: isl_config.flags, e.g. ISL_FLAG_GANG_ONE_NODE so that
     // PlaceGangs puts every gang on one node, ISL_FLAG_GANG_DISTINCT_NODES so that it puts every member of a gang on a different node,
-    // or ISL_FLAG_GANG_FEW_NODES so that it puts a gang on one node when one takes it and on as few nodes as it greedily can otherwise
+    // ISL_FLAG_GANG_FEW_NODES so that it puts a gang on one node when one takes it and on as few nodes as it greedily can otherwise, or
+    // ISL_FLAG_GANG_LOCALITY so that PlaceGangs takes one of these localities per gang
     explicit InstasliceReconciler(uint32_t quirks = ISL_QUIRKS_REF_EXACT, uint32_t max_gpus = 1u << 16, uint32_t max_batch = 1u << 16,
                                   uint32_t policy = ISL_POLICY_FIRST_FIT, uint32_t flags = 0);
     ~InstasliceReconciler();
@@ -115,6 +116,10 @@ public:
     // only then are its allocations written into `list`.  None: a pod found no GPU, nothing of the gang was committed.  Veto: the
     // Prepared exact-match check (:198-203) fired on a pod, every span of the gang was released again.  Empty gangs throw.
     std::vector<GangOutcome> PlaceGangs(InstasliceList& list, AllocationPolicy& policy, const std::vector<std::vector<PendingPod>>& gangs);
+    // The same with one node locality per gang (ISL_GANG_ANY_NODES, _ONE_NODE, _FEW_NODES or _DISTINCT_NODES), for a reconciler created
+    // with ISL_FLAG_GANG_LOCALITY: one call places gangs of every locality on one occupancy.  Throws unless there is one per gang.
+    std::vector<GangOutcome> PlaceGangs(InstasliceList& list, AllocationPolicy& policy, const std::vector<std::vector<PendingPod>>& gangs,
+                                        const std::vector<uint8_t>& locality);
     // Which lower-priority allocations each pending pod should evict, in order, ONE engine call (isl_preempt).  podPriority maps the UID
     // of each running pod to its PriorityClass value; values become dense ranks (more than 255 distinct values throw).  An allocation
     // may be evicted only when its pod's priority is known, its status is not "deleted" and no other entry that marks slices busy

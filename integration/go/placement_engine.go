@@ -71,6 +71,17 @@ const (
 	// PlaceGangs puts a gang on one node when one takes it whole, else on as few nodes as it greedily can: each round the node that
 	// places the most of the remaining pods takes them.  Not with FlagGangOneNode or FlagGangDistinctNodes.
 	FlagGangFewNodes = uint32(C.ISL_FLAG_GANG_FEW_NODES)
+	// PlaceGangsWithLocality takes one of the Gang* localities per gang, so one call places every kind of gang on one occupancy.
+	// Not with the three flags above.
+	FlagGangLocality = uint32(C.ISL_FLAG_GANG_LOCALITY)
+)
+
+// Node locality of one gang for PlaceGangsWithLocality (an engine created with FlagGangLocality).
+const (
+	GangAnyNodes      = uint8(C.ISL_GANG_ANY_NODES)      // pods anywhere, as on an engine without a gang flag
+	GangOneNode       = uint8(C.ISL_GANG_ONE_NODE)       // every pod on one node (Kueue's required hostname topology)
+	GangFewNodes      = uint8(C.ISL_GANG_FEW_NODES)      // one node when one has room, else as few as it greedily can (preferred)
+	GangDistinctNodes = uint8(C.ISL_GANG_DISTINCT_NODES) // every pod on a different node
 )
 
 func NewPlacementEngine(maxGPUs, maxBatch uint32) (*PlacementEngine, error) {
@@ -379,7 +390,17 @@ func (r *InstasliceReconciler) PlacePending(e *PlacementEngine, list *inferencev
 // caller writes the returned allocations (r.Update).  Empty gangs are an error.
 func (r *InstasliceReconciler) PlaceGangs(e *PlacementEngine, list *inferencev1alpha1.InstasliceList, policy AllocationPolicy,
 	gangs [][]PendingPod) ([][]*inferencev1alpha1.AllocationDetails, error) {
+	return r.PlaceGangsWithLocality(e, list, policy, gangs, nil)
+}
+
+// PlaceGangsWithLocality is PlaceGangs with one Gang* locality per gang (nil: none), for an engine created with FlagGangLocality:
+// a training job on one node, replicas on distinct nodes, a job on few nodes and free pods in one call.
+func (r *InstasliceReconciler) PlaceGangsWithLocality(e *PlacementEngine, list *inferencev1alpha1.InstasliceList, policy AllocationPolicy,
+	gangs [][]PendingPod, locality []uint8) ([][]*inferencev1alpha1.AllocationDetails, error) {
 	out := make([][]*inferencev1alpha1.AllocationDetails, len(gangs))
+	if locality != nil && len(locality) != len(gangs) {
+		return nil, fmt.Errorf("one locality per gang")
+	}
 	if len(gangs) == 0 {
 		return out, nil
 	}
@@ -392,7 +413,11 @@ func (r *InstasliceReconciler) PlaceGangs(e *PlacementEngine, list *inferencev1a
 	}
 	if e.orphans && len(gangs) > 1 { // the exact-match veto (:198-203) must see one gang at a time
 		for g := range gangs {
-			one, err := r.PlaceGangs(e, list, policy, gangs[g:g+1])
+			var loc []uint8
+			if locality != nil {
+				loc = locality[g : g+1]
+			}
+			one, err := r.PlaceGangsWithLocality(e, list, policy, gangs[g:g+1], loc)
 			if err != nil {
 				return nil, err
 			}
@@ -418,6 +443,11 @@ func (r *InstasliceReconciler) PlaceGangs(e *PlacementEngine, list *inferencev1a
 	for g, pods := range gangs {
 		e.fillRequests(req, pods, int(off[g]))
 		off[g+1] = off[g] + C.uint32_t(len(pods))
+		if locality != nil {
+			for i := off[g]; i < off[g+1]; i++ {
+				req[i].start = C.uint8_t(locality[g])
+			}
+		}
 	}
 	if rc := C.isl_place_gangs(e.h, C.uint32_t(len(gangs)), &off[0], &req[0], &res[0]); rc != C.ISL_OK {
 		return nil, fmt.Errorf("isl_place_gangs: %s (%s)", C.GoString(C.isl_strerror(rc)), C.GoString(C.isl_last_cuda_error(e.h)))
