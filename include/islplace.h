@@ -524,7 +524,12 @@ int  isl_place_batch_partitioned(isl_engine* e, uint32_t n, const void* d_in, vo
  *   1. every rank:  isl_ipc_inbox_handle(e, h)             -> 64-byte handle, exchanged by the caller (e.g. all_gather)
  *   2. every rank:  isl_ipc_connect(e, next rank's handle or NULL for the last rank, has_prev)
  *   3. every rank:  isl_place_stream_partitioned(..., stream_id) with the same batches and the same non-zero,
- *      never repeated stream_id (it tags what crosses the ranks; the speculative rounds use its low 24 bits); only enqueues.  Results: element-wise MIN over ranks as for the batch variant. */
+ *      never repeated stream_id (it tags what crosses the ranks); only enqueues.  Results: element-wise MIN over ranks as for the batch variant.
+ *      The speculative rounds (isl_connect_spec_local / isl_ipc_connect_spec) tag their records with the low 24 bits of the id, and the
+ *      shared record memory is cleared only when it is allocated, so that ids s and s + 2^24 would share a tag: only a stream id below
+ *      2^24 speculates; a larger one takes the token ring (same records, all ranks decide alike).  An engine whose record memory is
+ *      shared (isl_ipc_spec_handle, isl_connect_spec_local, also after a disconnect) never speculates outside
+ *      isl_place_stream_partitioned: isl_place_stream, isl_place_batch and open streams on it keep the plain pipeline. */
 int  isl_ipc_inbox_handle(isl_engine* e, void* handle64);
 int  isl_ipc_connect(isl_engine* e, const void* next_handle64, int has_prev);
 /* Same wiring for two engines of ONE process (same device or peer-enabled devices): no IPC handle needed. */

@@ -22,6 +22,7 @@
 using namespace isl;
 
 static constexpr uint32_t kMaxStreamChunks = 4096;
+static constexpr uint32_t kSpecRingIds = 1u << 24;     // stream ids of isl_place_stream_partitioned that may speculate
 
 // What plan_pipeline decides for one k_pipeline launch: GPUs per stage (seg), stages, GPUs per sub-segment, speculative rounds.
 struct PipePlan {
@@ -834,7 +835,12 @@ int route(isl_engine* e, const Call& c, uint64_t total, uint32_t n_chunks, Route
                            !kernels_serialised();
     r->window = (ring && e->ring_world == 0) ? 0u : e->window;      // a ring counts the ranks of a window on the owner
     const bool auto_spec = c.n_batches == 1 || (r->window >= 1 && r->window <= 3);        // speculative rounds by default
-    const int rc = plan_pipeline(e, n_chunks, (double)total / n_chunks, want_feed, ring, auto_spec, true, false, &r->plan);
+    // Record words of the rounds carry 24 bits of their call's tag, and shared record memory (isl_ipc_spec_handle) is cleared only when
+    // it is allocated: a ring speculates only under a stream id below 2^24, so that no two calls share a tag (every rank sees the same
+    // id and takes the same path), and an engine whose record memory is shared speculates on the ring only, where the stream id tags
+    // the words, never on calls tagged with its own epoch.
+    const bool spec_allowed = ring ? c.xepoch < kSpecRingIds : !e->spec_shared;
+    const int rc = plan_pipeline(e, n_chunks, (double)total / n_chunks, want_feed, ring, auto_spec, spec_allowed, false, &r->plan);
     if (rc == ISL_ECUDA) return rc;
     if (rc) return ring ? ISL_ERANGE : ISL_OK;
     r->path = Path::pipeline;
@@ -1961,10 +1967,11 @@ int isl_stream_open(isl_engine* e, uint32_t max_batches) {
     const uint32_t pc = e->pipe_chunk;
     if ((uint64_t)max_batches * pc > e->cfg.max_batch) return ISL_ERANGE;       // every batch owns a slot of the staging buffers
     // speculative rounds: the caller says (isl_set_causal_window) that it keeps at most 1..3 batches in flight, or asks for them outright;
-    // their record memory stays within 1 GiB and their stages leave room for the copier CTA and the feed kernels
+    // their record memory stays within 1 GiB, is not shared with other ranks (route) and their stages leave room for the copier CTA and
+    // the feed kernels
     PipePlan plan;
     if (int rc = plan_pipeline(e, std::max(2u, max_batches), (double)pc, true, false, e->window >= 1 && e->window <= 3,
-                               (uint64_t)max_batches * kSpecWordsPerChunk * 8ull <= (1ull << 30), true, &plan)) return rc;
+                               !e->spec_shared && (uint64_t)max_batches * kSpecWordsPerChunk * 8ull <= (1ull << 30), true, &plan)) return rc;
     if (plan.n_seg + 1 + kFeedReserve > (uint32_t)e->max_coresident) return ISL_ERANGE;  // the feed kernels need SMs next to the resident pipeline
     o.plan = plan; o.max_batches = max_batches; o.submitted = 0; o.launched = false;
     o.q_stride = pc + kQPad * ISL_MAX_PROFILES; o.free_stride = (uint32_t)e->occ_bytes; o.tiles_per_batch = pc / kTile;

@@ -5,15 +5,25 @@
 // the one it was certified in, the exit heads live in two slots per stage (round parity) guarded by an ack word of the reader.  This model
 // runs the same protocol with a random scheduler that picks, step by step, any stage that can proceed, and checks soundness (a certified
 // entry is the true token), freedom from deadlock, termination — and that a reader never needs a record that has been overwritten.
+//
+// Record words are self-validating: a reader takes any word whose tag (24 bits of the call's tag, and the round) matches.  Two more
+// modes model what the record memory may hold when a call starts (argument 3):
+//   1  the records of an EARLIER call on other requests, over the same stages, carry this call's tag (stream ids s and s + 2^24 of a
+//      partitioned inventory, whose shared record memory is never cleared between calls): the device would take them as current
+//   2  this call's tag is 0 and the memory is cleared: only the round-0 mass words (tag 0, round 0) match a cleared word, so a stage may
+//      read 0 for the masses of stages in front that have not published yet; rounds >= 1 and final words never match a cleared word
 #define SPEC_MODEL_NO_MAIN
 #include "spec_rounds_model.cpp"
 
 struct DRec { bool valid = false; long dq = 0, dr = 0; bool c = false; };
-struct XSlot { int round = 0; Heads x; };
+struct XSlot { int round = 0; Heads x; bool cur = false; };      // cur: written by this call
 struct Final { bool valid = false; int rf = 0; Heads x; long dq = 0, dr = 0; };
 // fault injection (the tests check that the model notices): 1 = a final record stands for EVERY round, 2 = no flow control of the exit
 // slots, 3 = a final record is preferred over the round's own record
 static int fault = 0;
+static int stale = 0;
+// the records a call leaves behind (what a stale-tag call of mode 1 finds)
+static struct { uint32_t S = 0; std::vector<std::vector<DRec>> dhist; std::vector<XSlot> xslot; std::vector<Final> fin; } left;
 
 static int run_async(uint32_t G, uint32_t seg, uint32_t n_req, int table, bool bounded, uint32_t fill_mask, int bias) {
     World w;
@@ -47,7 +57,11 @@ static int run_async(uint32_t G, uint32_t seg, uint32_t n_req, int table, bool b
     long totb = 0, tots = 0; for (int p : big) totb += w.q[p].size(); for (int p : small) tots += (long)w.q[p].size() * w.prof[p].size;
     const int RMAX = (int)S + 8;
     std::vector<Heads> H(S, Heads(np, 0)), X(S, Heads(np, 0)), Hc(S, Heads(np, 0)), Xc(S, Heads(np, 0)), predA(S, Heads(np, 0)), predB(S, Heads(np, 0));
-    { long qs = 0, rs = 0; for (uint32_t s = 0; s < S; ++s) { if (s) { spread(w, H[s], big, std::min(qs, totb), false); spread(w, H[s], small, std::min(rs, tots), true); } rs += qs < totb ? Rw[s] : Ro[s]; qs += Q[s]; } }
+    for (uint32_t s = 1; s < S; ++s) {      // round 0: the masses of the stages in front (mode 2: each read as 0 by a reader that came early)
+        long qs = 0, rs = 0;
+        for (uint32_t j = 0; j < s; ++j) { const bool zero = stale == 2 && rnd() % 2; if (!zero) { rs += qs < totb ? Rw[j] : Ro[j]; qs += Q[j]; } }
+        spread(w, H[s], big, std::min(qs, totb), false); spread(w, H[s], small, std::min(rs, tots), true);
+    }
     std::vector<char> done(S, 0), cprev(S, 0), logvalid(S, 0), have(S, 0), known(S, 0), need(S, 1), phase(S, 0), havepred(S, 0);
     std::vector<int> round(S, 1);
     std::vector<uint64_t> maxdec(S, 0);
@@ -56,6 +70,10 @@ static int run_async(uint32_t G, uint32_t seg, uint32_t n_req, int table, bool b
     std::vector<XSlot> xslot(2 * S);
     std::vector<int> ack(S, 0);
     std::vector<Final> fin(S);
+    if (stale == 1 && left.S == S) {
+        dhist = left.dhist; xslot = left.xslot; fin = left.fin;
+        for (auto& x : xslot) x.cur = false;
+    }
     cprev[0] = 1; known[0] = 1;
     uint32_t n_done = 0;
     uint64_t steps = 0;
@@ -85,8 +103,8 @@ static int run_async(uint32_t G, uint32_t seg, uint32_t n_req, int table, bool b
                     Dq[s] = massq(X[s]) - massq(H[s]); Dr[s] = massr(X[s]) - massr(H[s]);
                 }
                 // overwriting a slot the successor has not read would lose a record it still needs
-                if (s + 1 < S && xslot[2 * s + (r & 1)].round != 0 && !done[s + 1] && ack[s + 1] < xslot[2 * s + (r & 1)].round) { printf("FAIL: exit slot overwritten before it was read\n"); return 1; }
-                xslot[2 * s + (r & 1)].round = r; xslot[2 * s + (r & 1)].x = X[s];
+                if (s + 1 < S && xslot[2 * s + (r & 1)].cur && !done[s + 1] && ack[s + 1] < xslot[2 * s + (r & 1)].round) { printf("FAIL: exit slot overwritten before it was read\n"); return 1; }
+                xslot[2 * s + (r & 1)] = XSlot{r, X[s], true};
                 dhist[r][s] = DRec{true, Dq[s], Dr[s], (bool)cprev[s]};
                 phase[s] = 1; progressed = true;
             } else {
@@ -104,7 +122,7 @@ static int run_async(uint32_t G, uint32_t seg, uint32_t n_req, int table, bool b
                 if (ready && s > 0) {
                     if (xslot[2 * (s - 1) + (r & 1)].round == r) xp = xslot[2 * (s - 1) + (r & 1)].x;
                     else if (fin[s - 1].valid && fin[s - 1].rf <= r) xp = fin[s - 1].x;
-                    else if (xslot[2 * (s - 1) + (r & 1)].round > r) { printf("FAIL: the exit of round %d was overwritten by round %d before stage %u read it\n", r, xslot[2 * (s - 1) + (r & 1)].round, s); return 1; }
+                    else if (xslot[2 * (s - 1) + (r & 1)].round > r && xslot[2 * (s - 1) + (r & 1)].cur) { printf("FAIL: the exit of round %d was overwritten by round %d before stage %u read it\n", r, xslot[2 * (s - 1) + (r & 1)].round, s); return 1; }
                     else ready = false;
                 }
                 if (!ready) continue;
@@ -135,12 +153,14 @@ static int run_async(uint32_t G, uint32_t seg, uint32_t n_req, int table, bool b
         }
         if (!progressed) { printf("FAIL: deadlock (%u of %u stages done)\n", n_done, S); return 1; }
     }
+    left.S = S; left.dhist = dhist; left.xslot = xslot; left.fin = fin;
     return 0;
 }
 
 int main(int argc, char** argv) {
     const int cases = argc > 1 ? atoi(argv[1]) : 60;
     fault = argc > 2 ? atoi(argv[2]) : 0;
+    const int mode = argc > 3 ? atoi(argv[3]) : 0;
     int bad = 0;
     for (int i = 0; i < cases && !bad; ++i) {
         const uint32_t seg = 16u << (rnd() % 4);
@@ -149,6 +169,12 @@ int main(int argc, char** argv) {
         const uint32_t n_req = 1 + (uint32_t)(rnd() % (6 * G));
         const uint32_t fills[] = {0x00, 0x7F, 0xFF, 0x15, 0x33};
         const int tbl = (int)(rnd() % 3); const uint32_t fm = fills[rnd() % 5];
+        if (mode == 1) {        // an earlier call on other requests over the same stages, then this one
+            stale = 0;
+            const uint32_t n0 = 1 + (uint32_t)(rnd() % (6 * G));
+            if (run_async(G, seg, n0, tbl, i % 2 == 1, fills[rnd() % 5], i % 4)) { printf("FAIL: the earlier call\n"); return 1; }
+        }
+        stale = mode;
         bad |= run_async(G, seg, n_req, tbl, i % 2 == 1, fm, i % 4);
         if (bad) printf("case %d: G %u seg %u requests %u table %d bounded %d fill %#x\n", i, G, seg, n_req, tbl, i % 2, fm);
     }
