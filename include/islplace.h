@@ -122,6 +122,7 @@ extern "C" {
 #define ISL_ST_BAD_SPAN    4u   /* FREE outside the inventory or start+size > 8 (the reference would panic, Q7) */
 #define ISL_ST_NOOP        5u
 #define ISL_ST_GANG_ABORTED 6u  /* placeable as far as it was tried, but another member of its gang was not: nothing of the gang was committed */
+#define ISL_ST_GANG_TRIMMED 7u  /* not placed: its elastic gang committed its leading members without it (ISL_FLAG_GANG_MIN_MEMBERS, M3) */
 
 typedef struct isl_engine isl_engine;
 
@@ -152,6 +153,8 @@ typedef struct isl_config {
                                          (see isl_place_gangs); every other call is unchanged */
 #define ISL_FLAG_GANG_LOCALITY 512u  /* isl_place_gangs takes each gang's node locality from its ALLOC members' `start` byte, one of the
                                         ISL_GANG_* values below (see isl_place_gangs); every other call is unchanged */
+#define ISL_FLAG_GANG_MIN_MEMBERS 1024u  /* elastic gangs: isl_place_gangs commits a gang's leading members once they reach the minimum its
+                                            ALLOC members name in their `size` byte (see isl_place_gangs, M1-M7); every other call is unchanged */
 /* Node locality of one gang on an ISL_FLAG_GANG_LOCALITY engine (isl_request.start of its ALLOC members, rules L1-L6) */
 #define ISL_GANG_ANY_NODES      0u  /* rules 2-4: members anywhere, as on an engine without a gang flag */
 #define ISL_GANG_ONE_NODE       1u  /* G2-G3: every member on one node */
@@ -412,6 +415,34 @@ int  isl_place_batch_range(isl_engine* e, uint32_t lo, uint32_t hi, uint32_t n, 
  *       returns exactly what it returns on an unflagged engine.
  *   L6. Locality matters even for a gang of one: under best-fit a one-node gang of one takes the best GPU of the FIRST node in scan order
  *       that admits it, not the best GPU of the whole partition. */
+/*
+ * Elastic gangs (ISL_FLAG_GANG_MIN_MEMBERS): a group of k pods that may run as soon as m <= k of them can (the coscheduling plugin's
+ * PodGroup minMember, Volcano's minAvailable, Kueue's partial admission; elastic training and inference replicas).  On an engine created
+ * with the flag, alone or with one of the four gang flags above:
+ *   M1. An ALLOC member's `size` byte names its gang's minimum m (0..255); every ALLOC member of one gang carries the same byte.  With k
+ *       the gang's ALLOC members, the effective minimum is m' = k when m = 0 or m >= k, else m' = m, so m' >= 1.  A FREE's `size` stays
+ *       its span and a NOOP's is ignored.  Under ISL_FLAG_GANG_LOCALITY the `start` byte still names the locality (L1).
+ *   M2. The gang is placed by the rules of its locality exactly as without the flag: rules 2-4 with no gang flag, G2-G3 one node, F2-F3
+ *       few nodes, S2-S4 distinct nodes, per gang under ISL_FLAG_GANG_LOCALITY.  A gang those rules commit is unchanged.
+ *   M3. Trimming.  When those rules fail at ALLOC member f (counted from 0; the member that keeps its usual record: rule 4, G3's D, F3's
+ *       m_i, S3) and f >= m', the gang commits its first f ALLOC members where the run put them (rules 2-4 and S: member by member; G:
+ *       on the first node in scan order that reaches depth D; F: the rounds so far), with PLACED records.  Member f keeps its usual
+ *       record (NO_CAPACITY or BAD_PROFILE); every ALLOC member after it reports ISL_ST_GANG_TRIMMED with the unplaced default record
+ *       (gpu ISL_GPU_NONE, start 9, the profile's size or 0 for an unknown profile).  stats.placed counts the f members.
+ *   M4. When f < m' the gang aborts exactly as without the flag (rule 4 / G3 / F3 / S3 and rule 5): f = 0 always aborts.
+ *   M5. Consequences: (a) with every byte 0, or every byte >= its gang's k, a flagged call equals the call on the engine without the
+ *       flag (records, occupancy, stats.placed) for every gang flag and none; (b) a gang trimmed at f gets exactly the records and
+ *       occupancy that the gang cut to its first f ALLOC members gets without the flag, and that cut gang commits; (c) under
+ *       ISL_FLAG_GANG_LOCALITY a call equals its gangs run one at a time, each on the engine flagged for its locality | MIN (L3 b);
+ *       (d) gangs of one ALLOC member are unaffected.
+ *   M6. isl_create: ISL_EINVAL for the flag with ISL_FLAG_ALL_NODES or a node-scoring policy (the four gang flags keep their own
+ *       refusals, so at most one of them comes with it).  isl_place_gangs: ISL_EINVAL, and nothing changes, when two ALLOC members of
+ *       one gang carry different bytes, checked with L4 before the engine state is looked at; every other code is unchanged, the
+ *       2^20-GPU partition cap included.  Every other entry point returns what it returns on an unflagged engine.
+ *   M7. The committed members are always a LEADING run, never the best subset: under first-fit a gang [4g, 1g, 1g] with m = 2 aborts
+ *       when the 4g fits nowhere, although both 1g would fit.  List the members the job needs first; for replicas of one profile the
+ *       leading run is as many members as the locality places.
+ */
 int  isl_place_gangs(isl_engine* e, uint32_t n_gangs, const uint32_t* gang_off, const isl_request* in, isl_result* out);
 
 /* 8 bytes: one running allocation that MAY be evicted (isl_preempt). */

@@ -98,20 +98,23 @@ class InstasliceReconciler:
 
     def __init__(self, instaslices: list, quirks: int = E.QUIRKS_REF_EXACT, max_batch: int = 65536, engine: E.Engine | None = None,
                  policy: int = E.POLICY_FIRST_FIT, gang_one_node: bool = False, gang_distinct_nodes: bool = False,
-                 gang_few_nodes: bool = False, gang_locality: bool = False):
+                 gang_few_nodes: bool = False, gang_locality: bool = False, gang_min_members: bool = False):
         """``policy``: the engine policy of the engine this reconciler creates (``engine`` is None), e.g. ``E.POLICY_MOST_ALLOCATED`` to
         pack MIG pods onto the fullest nodes or ``E.POLICY_LEAST_ALLOCATED`` to spread them (include/islplace.h).  ``gang_one_node``:
         that engine is created with ``E.FLAG_GANG_ONE_NODE``, so ``place_pending_gangs`` puts every gang on one node.
         ``gang_distinct_nodes``: with ``E.FLAG_GANG_DISTINCT_NODES``, so it puts every member of a gang on a different node (the engine
         refuses both flags at once).  ``gang_few_nodes``: with ``E.FLAG_GANG_FEW_NODES``, so it puts a gang on one node when one takes
         it, else on as few nodes as it greedily can (the engine refuses it with either of the other two).  ``gang_locality``: with
-        ``E.FLAG_GANG_LOCALITY``, so ``place_pending_gangs`` takes a locality per gang (the engine refuses it with the other three)."""
+        ``E.FLAG_GANG_LOCALITY``, so ``place_pending_gangs`` takes a locality per gang (the engine refuses it with the other three).
+        ``gang_min_members``: with ``E.FLAG_GANG_MIN_MEMBERS`` (alone or with one of the four), so ``place_pending_gangs`` takes a
+        minimum per gang and may place a gang's leading pods only."""
         self.quirks = quirks
         self.policy = policy
         self.gang_one_node = gang_one_node
         self.gang_distinct_nodes = gang_distinct_nodes
         self.gang_few_nodes = gang_few_nodes
         self.gang_locality = gang_locality
+        self.gang_min_members = gang_min_members
         self.items = instaslices
         self._engine = engine
         self._max_batch = max_batch
@@ -157,7 +160,8 @@ class InstasliceReconciler:
                                     flags=(E.FLAG_GANG_ONE_NODE if self.gang_one_node else 0) |
                                           (E.FLAG_GANG_DISTINCT_NODES if self.gang_distinct_nodes else 0) |
                                           (E.FLAG_GANG_FEW_NODES if self.gang_few_nodes else 0) |
-                                          (E.FLAG_GANG_LOCALITY if self.gang_locality else 0))
+                                          (E.FLAG_GANG_LOCALITY if self.gang_locality else 0) |
+                                          (E.FLAG_GANG_MIN_MEMBERS if self.gang_min_members else 0))
         self._engine.load_profile_tables(self.rows)
         self._engine.load_inventory(self.node_off, np.asarray(occ, dtype=np.uint8))
         self._engine.set_node_tables(np.asarray(self.node_table, dtype=np.uint8))
@@ -267,7 +271,7 @@ class InstasliceReconciler:
                 out.append(self._commit_or_veto(pod, pod["profile"], policy, res))
         return out
 
-    def place_pending_gangs(self, gangs: list, policy=None, locality=None):
+    def place_pending_gangs(self, gangs: list, policy=None, locality=None, min_members=None):
         """All-or-nothing pod groups (the replicas of one deployment, the workers of one job): ``gangs`` is a list of non-empty pod
         lists shaped as ``place_pending_pods`` takes them, resolved in order with ONE engine call (isl_place_gangs).
 
@@ -279,23 +283,30 @@ class InstasliceReconciler:
         ``locality``: one ``E.GANG_*`` value per gang (e.g. from Kueue's podset topology annotations, INTEGRATION.md), for a reconciler
         created with ``gang_locality=True``: a training job on one node, replicas on distinct nodes, a job on few nodes and free pods in
         one call on one occupancy.
+
+        ``min_members``: one minimum m (0..255) per gang (the PodGroup's minMember, Volcano's minAvailable or Kueue's PodSet minCount,
+        INTEGRATION.md), for a reconciler created with ``gang_min_members=True``.  A gang whose leading pods reach its minimum while a
+        later pod finds no slice is placed with those pods only: its allocation list is shorter than the gang, and only those pods'
+        allocations are written.  List the pods the job needs first: the placed pods are always a leading run.
         """
         policy = policy or FirstFitPolicy()
         if any(not g for g in gangs):
             raise ValueError("empty gang")
         if self._has_orphans and len(gangs) > 1:
             locs = [None] * len(gangs) if locality is None else [[loc] for loc in locality]
-            return [self.place_pending_gangs([g], policy, loc)[0] for g, loc in zip(gangs, locs)]
+            mins = [None] * len(gangs) if min_members is None else [[m] for m in min_members]
+            return [self.place_pending_gangs([g], policy, loc, m)[0] for g, loc, m in zip(gangs, locs, mins)]
         if not gangs:
             return []
         off = np.cumsum([0] + [len(g) for g in gangs]).astype(np.uint32)
-        results = self._engine.place_gangs(self._requests([p["profile"] for g in gangs for p in g]), off, locality)
+        results = self._engine.place_gangs(self._requests([p["profile"] for g in gangs for p in g]), off, locality, min_members)
         out = []
         for gang, a, b in zip(gangs, off[:-1], off[1:]):
-            res = results[a:b]
-            if (res["status"] != E.ST_PLACED).any():
+            placed = int((results["status"][a:b] == E.ST_PLACED).sum())    # a leading run: all, none, or an elastic gang's first pods
+            if placed == 0:
                 out.append(("none", None))
                 continue
+            gang, res = gang[:placed], results[a:a + placed]
             packed = [self._alloc_for(pod, pod["profile"], policy, r) for pod, r in zip(gang, res)]
             if any(self._vetoed(instaslice, alloc) for instaslice, alloc in packed):
                 spans = np.zeros(len(res), dtype=E.SPAN_DTYPE)

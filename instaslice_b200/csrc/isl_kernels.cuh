@@ -2713,7 +2713,9 @@ struct NodeShare {
 };
 
 // Warp-wide: a gang of requests [r0, r1) failed.  Every ALLOC member except the one of rank keep_rank among them is reported
-// GANG_ABORTED; that one keeps k_prepare's NO_CAPACITY or BAD_PROFILE record.
+// GANG_ABORTED; that one keeps k_prepare's NO_CAPACITY or BAD_PROFILE record.  kTrim (an elastic gang that commits its leading members,
+// M3): only the ALLOC members of rank above keep_rank are written, and they report GANG_TRIMMED.
+template <bool kTrim = false>
 __device__ __forceinline__ void abort_gang_members(const uint2* in, uint2* out, const DevProfiles& prof, uint32_t r0, uint32_t r1,
                                                    uint32_t keep_rank, uint32_t lane) {
     uint32_t k = 0;                                         // ALLOC members before this block of 32
@@ -2721,7 +2723,8 @@ __device__ __forceinline__ void abort_gang_members(const uint2* in, uint2* out, 
         const uint32_t y = r + lane < r1 ? in[r + lane].y : (uint32_t)ISL_OP_NOOP << 8, p = y & 0xFFu;
         const bool alloc = ((y >> 8) & 0xFFu) == ISL_OP_ALLOC;
         const uint32_t ballot = __ballot_sync(0xFFFFFFFFu, alloc), rank = k + __popc(ballot & ((1u << lane) - 1u));
-        if (alloc && rank != keep_rank) out[r + lane] = pack_result(ISL_GPU_NONE, ISL_START_NONE, p < prof.n ? prof.rows[p].size : 0u, ISL_ST_GANG_ABORTED);
+        if (alloc && (kTrim ? rank > keep_rank : rank != keep_rank))
+            out[r + lane] = pack_result(ISL_GPU_NONE, ISL_START_NONE, p < prof.n ? prof.rows[p].size : 0u, kTrim ? ISL_ST_GANG_TRIMMED : ISL_ST_GANG_ABORTED);
         k += __popc(ballot);
     }
 }
@@ -2767,12 +2770,17 @@ __device__ void gangfew_undo(const GangNodeArgs& a, const NodeShare& sh, const D
 
 // One gang of requests [r0, r1) of k_gangnode<kFew> (and of k_ganglocal's localities 1 and 2), every thread of the CTA.  `scr`, the
 // scratch copies, is the share's aux byte.  The shared words are the kernel's: s_warp and s_win for grid_min, s_need and s_allocs.
-template <bool kFew>
+// kMin (k_ganglocal<true>, M3): a gang that fails at ALLOC member f >= min_m commits its first f members instead of aborting.  One node:
+// f is the deepest failure's depth D, and the owner of the first node that reaches it replays the members on its live bytes, which stop
+// at D by themselves (the scratch copy started from the same bytes).  Few nodes: f is the members the earlier rounds placed.
+template <bool kFew, bool kMin = false>
 __device__ __forceinline__ void gangnode_gang(const GangNodeArgs& a, const DevProfiles& prof, const NodeShare& sh, uint32_t r0, uint32_t r1,
                                               uint32_t& parity, uint32_t& placed, unsigned long long* s_warp, unsigned long long* s_win,
-                                              uint32_t* s_need, uint32_t* s_allocs, uint32_t tid, uint32_t lane, uint32_t warp) {
+                                              uint32_t* s_need, uint32_t* s_allocs, uint32_t tid, uint32_t lane, uint32_t warp,
+                                              uint32_t min_m = 0) {
     uint8_t* const scr = sh.aux;
     uint32_t ri = r0, held = 0;     // kFew: the round's first request; members this CTA committed tentatively in earlier rounds
+    uint32_t done = 0;              // kFew && kMin: members the earlier rounds placed (grid-uniform: the sum of the winning depths)
     for (;;) {                      // one round; without kFew every path leaves after the first
         if (tid < kMaxTables) s_need[tid] = 0;
         if (tid == 0) *s_allocs = 0;
@@ -2821,11 +2829,28 @@ __device__ __forceinline__ void gangnode_gang(const GangNodeArgs& a, const DevPr
             break;
         }
         if constexpr (!kFew) {
+            if constexpr (kMin) {
+                const uint32_t d = 0x7FFFFFFFu - (uint32_t)((win >> 32) & 0x7FFFFFFFu), j = (uint32_t)win;
+                if (d >= min_m) {                           // min_m >= 1, so ~0ull (depth 0) never gets here
+                    if (j >= sh.j0 && j < sh.j1 && warp == 0) {
+                        const uint32_t b0 = sh.nb(j) - sh.base, c = sh.nb(j + 1) - sh.base - b0;
+                        gangnode_resolve(a, prof, sh.live + b0, c, a.lo + sh.base + b0, a.gtab[a.lo + sh.base + b0] & (kMaxTables - 1), ri, r1, true, lane);
+                        placed += d;
+                    }
+                    if (blockIdx.x == 0 && warp == 0) abort_gang_members<true>(a.in, a.out, prof, r0, r1, d, lane);
+                    break;
+                }
+            }
             if (blockIdx.x == 0 && warp == 0)               // the deepest failure's depth; ~0ull (no node evaluated) is depth 0 as well
                 abort_gang_members(a.in, a.out, prof, r0, r1, 0x7FFFFFFFu - (uint32_t)((win >> 32) & 0x7FFFFFFFu), lane);
             break;
         } else {
             const uint32_t d = 0x7FFFFFFFu - (uint32_t)((win >> 32) & 0x7FFFFFFFu), j = (uint32_t)win;  // members the round places
+            if (kMin && d == 0 && done >= min_m) {          // the earlier rounds' members commit, m_i keeps its record
+                placed += held;
+                if (blockIdx.x == 0 && warp == 0) abort_gang_members<true>(a.in, a.out, prof, ri, r1, 0, lane);
+                break;
+            }
             if (d == 0) {                                   // no node takes m_i: every CTA takes back its tentative members
                 if (warp == 0) gangfew_undo(a, sh, prof, r0, ri, lane);
                 if (blockIdx.x == 0 && warp == 0) abort_gang_members(a.in, a.out, prof, ri, r1, 0, lane);
@@ -2837,6 +2862,7 @@ __device__ __forceinline__ void gangnode_gang(const GangNodeArgs& a, const DevPr
                 held += d;
             }
             ri = skip_allocs(a.in, ri, r1, d, lane);        // every CTA read the same key: all advance alike
+            done += d;
         }
     }
 }
@@ -2875,11 +2901,13 @@ __global__ void __launch_bounds__(kGnThreads, 1) k_gangnode(GangNodeArgs a, DevP
 // One gang of requests [r0, r1) of k_gangspread (and of k_ganglocal's locality 3), every thread of the CTA.  `tag` (1..255) marks the
 // nodes the gang uses in the share's aux byte; tag 1 clears the marks first, so a mark can only equal `tag` when this gang wrote it.
 // `dead`: profiles no GPU of the partition admits any more.  The shared words are the kernel's: s_warp and s_win for grid_min, and the
-// size of the CTA's stack of wins, which is 0 between gangs.
+// size of the CTA's stack of wins, which is 0 between gangs.  kMin (k_ganglocal<true>, M3): a member that finds no GPU at rank
+// fail >= min_m commits the stack of wins, which holds the members before it, as a success does.
+template <bool kMin = false>
 __device__ __forceinline__ void gangspread_gang(const GangNodeArgs& a, const DevProfiles& prof, const NodeShare& sh, uint2* wins, uint32_t r0,
                                                 uint32_t r1, uint32_t tag, uint32_t& parity, uint32_t& placed, uint32_t& dead,
                                                 uint32_t* s_warp, uint32_t* s_win, uint32_t* s_nwins, uint32_t tid, uint32_t lane,
-                                                uint32_t warp) {
+                                                uint32_t warp, uint32_t min_m = 0) {
     const uint32_t base = sh.base, cnt = sh.cnt;
     uint8_t* const mark = sh.aux;                           // tag of the gang whose member uses the GPU's node
     if (tag == 1u) for (uint32_t g = tid; g < cnt; g += kGnThreads) mark[g] = 0;
@@ -2914,7 +2942,8 @@ __device__ __forceinline__ void gangspread_gang(const GangNodeArgs& a, const Dev
         __syncthreads();                                    // the marks and the stack are in place before the next member's scan
         ++rank;
     }
-    if (fail == kInf) {                                     // commit: each CTA writes its members; their nodes, hence GPUs, differ
+    const bool trim = kMin && fail != kInf && fail >= min_m;
+    if (fail == kInf || trim) {                             // commit: each CTA writes its members; their nodes, hence GPUs, differ
         const uint32_t nw = *s_nwins;
         for (uint32_t k = tid; k < nw; k += kGnThreads) {
             const uint2 w = wins[sh.j0 + k];
@@ -2927,6 +2956,7 @@ __device__ __forceinline__ void gangspread_gang(const GangNodeArgs& a, const Dev
             a.out[w.x] = pack_result(flip_gpu(a.lo + base + g, prof.flip), start, size, ISL_ST_PLACED);
         }
         placed += nw;
+        if (trim && blockIdx.x == 0 && warp == 0) abort_gang_members<true>(a.in, a.out, prof, r0, r1, fail, lane);
     } else if (blockIdx.x == 0 && warp == 0) {              // the member at rank `fail` keeps its record, every other ALLOC member aborts
         abort_gang_members(a.in, a.out, prof, r0, r1, fail, lane);
     }
@@ -2965,9 +2995,11 @@ __global__ void __launch_bounds__(kGnThreads, 1) k_gangspread(GangNodeArgs a, De
 // tentatively to its live share, the occupancy and a PLACED record.  A member with no GPU aborts the gang: every CTA takes back the
 // tentative members on its own nodes (gangfew_undo), and CTA 0 reports the members after the failing one GANG_ABORTED.  An unknown or
 // dead profile fails without a barrier: gangfew_undo only touches records on the CTA's own nodes, which that CTA wrote itself.
+// kMin (k_ganglocal<true>, M3): a member with no GPU at rank >= min_m keeps the tentative members, which then commit.
+template <bool kMin = false>
 __device__ __forceinline__ void ganglocal_any(const GangNodeArgs& a, const DevProfiles& prof, const NodeShare& sh, uint32_t r0, uint32_t r1,
                                               uint32_t& parity, uint32_t& placed, uint32_t& dead, uint32_t* s_warp, uint32_t* s_win,
-                                              uint32_t tid, uint32_t lane, uint32_t warp) {
+                                              uint32_t tid, uint32_t lane, uint32_t warp, uint32_t min_m = 0) {
     const uint32_t base = sh.base, cnt = sh.cnt;
     __syncthreads();                                        // the previous gang's commits are in the live share before this gang's reads
     uint32_t rank = 0;                                      // ALLOC members committed tentatively so far
@@ -2986,6 +3018,13 @@ __device__ __forceinline__ void ganglocal_any(const GangNodeArgs& a, const DevPr
             if (win == kInf && rank == 0) dead |= 1u << p;  // no tentative slice of this gang is in the way
         }
         if (win == kInf) {
+            if (kMin && rank >= min_m) {
+                if (blockIdx.x == 0) {
+                    placed += rank;
+                    if (warp == 0) abort_gang_members<true>(a.in, a.out, prof, r, r1, 0, lane);
+                }
+                return;
+            }
             if (warp == 0) gangfew_undo(a, sh, prof, r0, r, lane);
             if (blockIdx.x == 0 && warp == 0) abort_gang_members(a.in, a.out, prof, r, r1, 0, lane);
             return;
@@ -3005,6 +3044,10 @@ __device__ __forceinline__ void ganglocal_any(const GangNodeArgs& a, const DevPr
     if (blockIdx.x == 0) placed += rank;                    // the gang commits: CTA 0 counts its members once
 }
 
+// k_ganglocal<true>: every isl_place_gangs call on an ISL_FLAG_GANG_MIN_MEMBERS engine (DESIGN.md 4.13), whatever its locality flag: the
+// host writes the engine's locality into every gang's byte (or the gang's own under ISL_FLAG_GANG_LOCALITY), and each gang's effective
+// minimum m' (M1) as a uint32 right after the bytes, rounded up to 4.  Every CTA reads them alike, so the barriers stay grid-uniform.
+template <bool kMin>
 __global__ void __launch_bounds__(kGnThreads, 1) k_ganglocal(GangNodeArgs a, DevProfiles prof, uint2* wins, const uint8_t* __restrict__ locality) {
     extern __shared__ __align__(16) uint8_t gl_smem[];
     __shared__ unsigned long long s_warp64[kGnThreads / 32];
@@ -3017,15 +3060,18 @@ __global__ void __launch_bounds__(kGnThreads, 1) k_ganglocal(GangNodeArgs a, Dev
     uint32_t parity = 0, placed = 0, dead = 0, spread = 0;  // spread: locality-3 gangs since the marks were last cleared
     for (uint32_t gi = 0; gi < a.n_gangs; ++gi) {
         const uint32_t r0 = __ldg(a.gang_off + gi), r1 = __ldg(a.gang_off + gi + 1), loc = __ldg(locality + gi);
+        const uint32_t min_m = kMin ? __ldg(reinterpret_cast<const uint32_t*>(locality + ((a.n_gangs + 3u) & ~3u)) + gi) : 0u;
         if (loc == ISL_GANG_ONE_NODE || loc == ISL_GANG_FEW_NODES) {
-            if (loc == ISL_GANG_ONE_NODE) gangnode_gang<false>(a, prof, sh, r0, r1, parity, placed, s_warp64, &s_win64, s_need, &s_allocs, tid, lane, warp);
-            else gangnode_gang<true>(a, prof, sh, r0, r1, parity, placed, s_warp64, &s_win64, s_need, &s_allocs, tid, lane, warp);
+            if (loc == ISL_GANG_ONE_NODE)
+                gangnode_gang<false, kMin>(a, prof, sh, r0, r1, parity, placed, s_warp64, &s_win64, s_need, &s_allocs, tid, lane, warp, min_m);
+            else gangnode_gang<true, kMin>(a, prof, sh, r0, r1, parity, placed, s_warp64, &s_win64, s_need, &s_allocs, tid, lane, warp, min_m);
             spread = 0;                                     // the scratch copies overwrote the marks
         } else if (loc == ISL_GANG_DISTINCT_NODES) {
-            gangspread_gang(a, prof, sh, wins, r0, r1, 1u + spread % 255u, parity, placed, dead, s_warp32, &s_win32, &s_nwins, tid, lane, warp);
+            gangspread_gang<kMin>(a, prof, sh, wins, r0, r1, 1u + spread % 255u, parity, placed, dead, s_warp32, &s_win32, &s_nwins, tid, lane,
+                                  warp, min_m);
             ++spread;
         } else {
-            ganglocal_any(a, prof, sh, r0, r1, parity, placed, dead, s_warp32, &s_win32, tid, lane, warp);
+            ganglocal_any<kMin>(a, prof, sh, r0, r1, parity, placed, dead, s_warp32, &s_win32, tid, lane, warp, min_m);
         }
     }
     if (tid == 0 && placed) count_placed(a.ctrl, placed);

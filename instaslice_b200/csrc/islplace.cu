@@ -527,19 +527,21 @@ int run_gangspread(isl_engine* e, uint32_t n_gangs, const uint32_t* d_gang_off, 
     return ISL_OK;
 }
 
-// isl_place_gangs on an ISL_FLAG_GANG_LOCALITY engine: frees + defaults, then one cooperative k_ganglocal (gang_layout with its own
-// opt-in), which places each gang by the locality byte at d_locality[gang]; wins as in run_gangspread.
+// isl_place_gangs on an ISL_FLAG_GANG_LOCALITY or ISL_FLAG_GANG_MIN_MEMBERS engine: frees + defaults, then one cooperative k_ganglocal
+// (gang_layout with its own opt-in), which places each gang by the locality byte at d_locality[gang]; wins as in run_gangspread.
+// elastic: k_ganglocal<true>, which reads each gang's minimum m' from the uint32 words that follow the bytes (rounded up to 4).
 int run_ganglocal(isl_engine* e, uint32_t n_gangs, const uint32_t* d_gang_off, const uint8_t* d_locality, uint32_t n, const uint2* d_in,
-                  uint2* d_out) {
+                  uint2* d_out, bool elastic) {
     if (int rc = prepare_batch(e, n, d_in, d_out)) return rc;
+    const void* kernel = elastic ? (const void*)k_ganglocal<true> : (const void*)k_ganglocal<false>;
     GangNodeArgs a;
     uint32_t grid, nodes;
     size_t smem;
-    if (int rc = gang_layout(e, (const void*)k_ganglocal, e->gn.local_optin, n_gangs, d_gang_off, d_in, d_out, a, &grid, &smem, &nodes)) return rc;
+    if (int rc = gang_layout(e, kernel, e->gn.local_optin, n_gangs, d_gang_off, d_in, d_out, a, &grid, &smem, &nodes)) return rc;
     ISL_CUDA(e, e->gn.wins.reserve(nodes));
     uint2* wins = e->gn.wins;
     void* params[] = {&a, &e->prof, &wins, &d_locality};
-    if (int rc = launch_cooperative(e, (const void*)k_ganglocal, "k_ganglocal", grid, kGnThreads, smem, params)) return rc;
+    if (int rc = launch_cooperative(e, kernel, elastic ? "k_ganglocal<true>" : "k_ganglocal", grid, kGnThreads, smem, params)) return rc;
     finish_batch(e, n, true);
     return ISL_OK;
 }
@@ -1181,6 +1183,8 @@ int isl_create(const isl_config* cfg, isl_engine** out) {
     if ((cfg->flags & ISL_FLAG_GANG_LOCALITY) &&
         ((cfg->flags & (ISL_FLAG_GANG_ONE_NODE | ISL_FLAG_GANG_DISTINCT_NODES | ISL_FLAG_GANG_FEW_NODES | ISL_FLAG_ALL_NODES)) ||
          node_scoring(cfg->policy))) return ISL_EINVAL;
+    // elastic gangs (M6): with any one locality flag or none (their own checks refuse two), not with a pod on every node nor node scoring
+    if ((cfg->flags & ISL_FLAG_GANG_MIN_MEMBERS) && ((cfg->flags & ISL_FLAG_ALL_NODES) || node_scoring(cfg->policy))) return ISL_EINVAL;
     if (request_major(cfg->policy) && cfg->max_gpus > kBfMaxGpus) return ISL_ERANGE;
     if (cfg->quirks & ~ISL_QUIRKS_REF_EXACT) return ISL_EINVAL;
     isl_engine* e = new (std::nothrow) isl_engine;
@@ -1210,7 +1214,7 @@ int isl_create(const isl_config* cfg, isl_engine** out) {
         const void* kernels[] = {(const void*)k_prepare, (const void*)k_partition, (const void*)k_set_flag, (const void*)k_few, (const void*)k_build_lut, (const void*)k_eval_starts,
                                  (const void*)k_free_spans, (const void*)k_capacity, (const void*)k_sweep_count, (const void*)k_sweep_scatter, (const void*)k_commit, (const void*)k_bestfit<false>, (const void*)k_bestfit<true>,
                                  (const void*)k_bestfit<false, true>, (const void*)k_bestfit<true, true>, (const void*)k_victim_map, (const void*)k_preempt, (const void*)k_nodefit, (const void*)k_gangnode<false>, (const void*)k_gangnode<true>, (const void*)k_gangspread,
-                                 (const void*)k_ganglocal, (const void*)k_chain<1>, (const void*)k_chain<2>, (const void*)k_chain<4>, (const void*)k_small<1>, (const void*)k_small<2>, (const void*)k_small<4>};
+                                 (const void*)k_ganglocal<false>, (const void*)k_ganglocal<true>, (const void*)k_chain<1>, (const void*)k_chain<2>, (const void*)k_chain<4>, (const void*)k_small<1>, (const void*)k_small<2>, (const void*)k_small<4>};
         const void* pipes[] = {(const void*)k_pipeline<1, false, false>, (const void*)k_pipeline<1, true, false>, (const void*)k_pipeline<2, false, false>, (const void*)k_pipeline<2, true, false>,
                                (const void*)k_pipeline<4, false, false>, (const void*)k_pipeline<4, true, false>,
                                (const void*)k_pipeline<1, false, true>, (const void*)k_pipeline<1, true, true>, (const void*)k_pipeline<2, false, true>, (const void*)k_pipeline<2, true, true>,
@@ -1236,10 +1240,13 @@ int isl_create(const isl_config* cfg, isl_engine** out) {
         for (const void* k : gangs) { ISL_TRY(cudaFuncGetAttributes(&fa, k)); gang_static = std::max(gang_static, fa.sharedSizeBytes); }
         e->gn.smem_optin = optin - (int)gang_static;
         for (const void* k : gangs) ISL_TRY(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, e->gn.smem_optin));
-        // k_ganglocal sizes its shares by its own static shared memory, so the switch of the three above does not move with it
-        ISL_TRY(cudaFuncGetAttributes(&fa, k_ganglocal));
-        e->gn.local_optin = optin - (int)fa.sharedSizeBytes;
-        ISL_TRY(cudaFuncSetAttribute((const void*)k_ganglocal, cudaFuncAttributeMaxDynamicSharedMemorySize, e->gn.local_optin));
+        // k_ganglocal sizes its shares by its own static shared memory, so the switch of the three above does not move with it; both
+        // instantiations declare the same static words
+        const void* locals[] = {(const void*)k_ganglocal<false>, (const void*)k_ganglocal<true>};
+        size_t local_static = 0;
+        for (const void* k : locals) { ISL_TRY(cudaFuncGetAttributes(&fa, k)); local_static = std::max(local_static, fa.sharedSizeBytes); }
+        e->gn.local_optin = optin - (int)local_static;
+        for (const void* k : locals) ISL_TRY(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, e->gn.local_optin));
     }
     e->occ_bytes = ((size_t)cfg->max_gpus + kSweepBlock - 1) / kSweepBlock * kSweepBlock;
     const uint32_t max_tiles = ceil_div(cfg->max_batch, kTile) + 4096;   // + one partial tile per batch of a stream
@@ -1450,7 +1457,8 @@ int isl_load_inventory(isl_engine* e, uint32_t n_nodes, const uint32_t* node_off
         ISL_CUDA(e, e->nf.node_off.replace((size_t)n_nodes + 1));
         ISL_CUDA(e, cudaMemcpyAsync(e->nf.node_off, node_off, ((size_t)n_nodes + 1) * sizeof(uint32_t), cudaMemcpyHostToDevice, e->stream));
     }
-    if (e->cfg.flags & (ISL_FLAG_GANG_ONE_NODE | ISL_FLAG_GANG_FEW_NODES | ISL_FLAG_GANG_DISTINCT_NODES | ISL_FLAG_GANG_LOCALITY)) {
+    if (e->cfg.flags & (ISL_FLAG_GANG_ONE_NODE | ISL_FLAG_GANG_FEW_NODES | ISL_FLAG_GANG_DISTINCT_NODES | ISL_FLAG_GANG_LOCALITY |
+                        ISL_FLAG_GANG_MIN_MEMBERS)) {
         // k_gangnode, k_gangspread and k_ganglocal walk the nodes in storage order (reversed under right-to-left)
         auto& off = e->gn.off;
         off.assign(node_off, node_off + n_nodes + 1);
@@ -1550,6 +1558,26 @@ int isl_place_gangs(isl_engine* e, uint32_t n_gangs, const uint32_t* gang_off, c
             }
         }
     }
+    const bool elastic = e->cfg.flags & ISL_FLAG_GANG_MIN_MEMBERS;
+    std::vector<uint32_t> min_members;                              // ISL_FLAG_GANG_MIN_MEMBERS: each gang's m' (M1, M6), 0 without ALLOCs
+    if (elastic) {
+        const uint8_t loc = (e->cfg.flags & ISL_FLAG_GANG_ONE_NODE)         ? (uint8_t)ISL_GANG_ONE_NODE
+                            : (e->cfg.flags & ISL_FLAG_GANG_FEW_NODES)      ? (uint8_t)ISL_GANG_FEW_NODES
+                            : (e->cfg.flags & ISL_FLAG_GANG_DISTINCT_NODES) ? (uint8_t)ISL_GANG_DISTINCT_NODES
+                                                                            : (uint8_t)ISL_GANG_ANY_NODES;
+        if (locality.empty()) locality.assign(n_gangs, loc);       // the engine's locality for every gang
+        min_members.assign(n_gangs, 0);
+        for (uint32_t i = 0; i < n_gangs; ++i) {
+            uint32_t k = 0, m = 0;
+            for (uint32_t r = gang_off[i]; r < gang_off[i + 1]; ++r) {
+                if (in[r].op != ISL_OP_ALLOC) continue;
+                if (k && in[r].size != m) return ISL_EINVAL;
+                m = in[r].size;
+                ++k;
+            }
+            min_members[i] = (m == 0 || m >= k) ? k : m;
+        }
+    }
     if (e->cfg.flags & ISL_FLAG_ALL_NODES) return ISL_EINVAL;      // one pod on every node with capacity: no all-or-nothing meaning
     if (node_scoring(e->cfg.policy)) return ISL_EINVAL;            // gangs under node scoring are not implemented
     if (n > e->cfg.max_batch) return ISL_ERANGE;
@@ -1557,14 +1585,19 @@ int isl_place_gangs(isl_engine* e, uint32_t n_gangs, const uint32_t* gang_off, c
     if (guard.rc) return guard.rc;
     if (n == 0) return ISL_OK;
     if (e->hi == e->lo || e->hi - e->lo > kBfMaxGpus) return ISL_ERANGE;          // the class bitmaps of k_bestfit
-    ISL_CUDA(e, e->d_scratch.reserve(((size_t)n_gangs + 1) * sizeof(uint32_t) + locality.size()));
+    const size_t min_at = ((size_t)n_gangs + 1) * sizeof(uint32_t) + ((locality.size() + 3) & ~(size_t)3);     // m' after the bytes
+    ISL_CUDA(e, e->d_scratch.reserve(min_at + min_members.size() * sizeof(uint32_t)));
     uint32_t* d_gang_off = reinterpret_cast<uint32_t*>(e->d_scratch.get());
     const uint8_t* d_locality = reinterpret_cast<const uint8_t*>(d_gang_off + n_gangs + 1);      // the bytes right after the offsets
     ISL_CUDA(e, cudaMemcpyAsync(d_gang_off, gang_off, ((size_t)n_gangs + 1) * sizeof(uint32_t), cudaMemcpyHostToDevice, e->stream));
     if (!locality.empty())
         ISL_CUDA(e, cudaMemcpyAsync((void*)d_locality, locality.data(), locality.size(), cudaMemcpyHostToDevice, e->stream));
+    if (!min_members.empty())
+        ISL_CUDA(e, cudaMemcpyAsync((uint8_t*)e->d_scratch.get() + min_at, min_members.data(), min_members.size() * sizeof(uint32_t),
+                                    cudaMemcpyHostToDevice, e->stream));
     ISL_CUDA(e, cudaMemcpyAsync(e->d_req, in, (size_t)n * sizeof(isl_request), cudaMemcpyHostToDevice, e->stream));
-    if (int rc = (e->cfg.flags & ISL_FLAG_GANG_LOCALITY)        ? run_ganglocal(e, n_gangs, d_gang_off, d_locality, n, e->d_req, e->d_res)
+    if (int rc = (e->cfg.flags & (ISL_FLAG_GANG_LOCALITY | ISL_FLAG_GANG_MIN_MEMBERS))
+                                                                 ? run_ganglocal(e, n_gangs, d_gang_off, d_locality, n, e->d_req, e->d_res, elastic)
                  : (e->cfg.flags & ISL_FLAG_GANG_ONE_NODE)        ? run_gangnode(e, n_gangs, d_gang_off, n, e->d_req, e->d_res)
                  : (e->cfg.flags & ISL_FLAG_GANG_FEW_NODES)      ? run_gangfew(e, n_gangs, d_gang_off, n, e->d_req, e->d_res)
                  : (e->cfg.flags & ISL_FLAG_GANG_DISTINCT_NODES) ? run_gangspread(e, n_gangs, d_gang_off, n, e->d_req, e->d_res)

@@ -29,11 +29,13 @@ QUIRK_STRICT_BOUND, QUIRK_POW2_ONLY = 1, 2
 QUIRKS_REF_EXACT, QUIRKS_FIXED = 3, 0
 OP_ALLOC, OP_FREE, OP_NOOP = 0, 1, 2
 ST_PLACED, ST_NO_CAPACITY, ST_BAD_PROFILE, ST_FREED, ST_BAD_SPAN, ST_NOOP, ST_GANG_ABORTED = 0, 1, 2, 3, 4, 5, 6
+ST_GANG_TRIMMED = 7     # not placed: its elastic gang committed its leading members without it (include/islplace.h M3)
 FLAG_TIMING, FLAG_NO_PIPELINE, FLAG_FORCE_PIPELINE, FLAG_TRACE, FLAG_NO_SMALL, FLAG_ALL_NODES = 1, 2, 4, 8, 16, 32
 FLAG_GANG_ONE_NODE = 64     # isl_place_gangs puts every member of a gang on one node (include/islplace.h)
 FLAG_GANG_DISTINCT_NODES = 128  # isl_place_gangs puts every member of a gang on a different node (include/islplace.h)
 FLAG_GANG_FEW_NODES = 256  # isl_place_gangs puts a gang on one node when one takes it, else on as few nodes as it greedily can
 FLAG_GANG_LOCALITY = 512  # isl_place_gangs takes each gang's node locality from its ALLOC members' start byte (GANG_*)
+FLAG_GANG_MIN_MEMBERS = 1024  # elastic gangs: a gang commits its leading members once they reach its minimum (the ALLOC size byte)
 GANG_ANY_NODES, GANG_ONE_NODE, GANG_FEW_NODES, GANG_DISTINCT_NODES = 0, 1, 2, 3     # node locality of one gang (include/islplace.h L1)
 SPEC_AUTO, SPEC_OFF, SPEC_ON = 0, 1, 2
 
@@ -336,7 +338,7 @@ class Engine:
         self._check(self._lib.isl_place_batch_range(self._h, lo, hi, len(requests), _ptr(requests), _ptr(out)), "isl_place_batch_range")
         return out
 
-    def place_gangs(self, requests: np.ndarray, gang_off, locality=None) -> np.ndarray:
+    def place_gangs(self, requests: np.ndarray, gang_off, locality=None, min_members=None) -> np.ndarray:
         """All-or-nothing groups: gang i is ``requests[gang_off[i]:gang_off[i + 1]]`` (``gang_off[0] == 0``, no empty gang, the last
         offset is ``len(requests)``).  A gang commits only when every ALLOC member is placed; otherwise the first member that did not fit
         keeps its record and every other ALLOC member reports ``ST_GANG_ABORTED`` (include/islplace.h).  On an engine created with
@@ -348,7 +350,13 @@ class Engine:
 
         On an engine created with ``FLAG_GANG_LOCALITY`` each gang is placed by its own locality, the ``start`` byte of its ALLOC members
         (``GANG_ANY_NODES``, ``GANG_ONE_NODE``, ``GANG_FEW_NODES`` or ``GANG_DISTINCT_NODES``).  ``locality``: one such value per gang,
-        written into the ``start`` of the ALLOC members of a copy of ``requests``; it needs an engine created with the flag."""
+        written into the ``start`` of the ALLOC members of a copy of ``requests``; it needs an engine created with the flag.
+
+        On an engine created with ``FLAG_GANG_MIN_MEMBERS`` a gang may commit its leading members: when its locality's rules stop at
+        ALLOC member f and f reaches the gang's minimum m' (the ``size`` byte m of its ALLOC members; m' = m for 0 < m < k, else every
+        one of its k members), the first f members are placed, member f keeps its record and the members after it report
+        ``ST_GANG_TRIMMED`` (include/islplace.h M1-M7).  ``min_members``: one m in 0..255 per gang, written into the ``size`` of the
+        ALLOC members of a copy of ``requests``; it needs an engine created with the flag."""
         requests = np.ascontiguousarray(requests, dtype=REQUEST_DTYPE)
         gang_off = np.ascontiguousarray(gang_off, dtype=np.uint32)
         if len(gang_off) == 0 or int(gang_off[-1]) != len(requests):
@@ -363,6 +371,18 @@ class Engine:
             per_request = np.repeat(locality, np.diff(gang_off.astype(np.int64)))
             alloc = requests["op"] == OP_ALLOC
             requests["start"][alloc] = per_request[alloc].astype(np.uint8)
+        if min_members is not None:
+            if not self.flags & FLAG_GANG_MIN_MEMBERS:
+                raise ValueError("a minimum per gang needs an engine created with FLAG_GANG_MIN_MEMBERS")
+            min_members = np.asarray(min_members, dtype=np.int64).reshape(-1)
+            if len(min_members) != len(gang_off) - 1:
+                raise ValueError("one minimum per gang")
+            if len(min_members) and (min_members.min() < 0 or min_members.max() > 255):
+                raise ValueError("a gang's minimum is 0..255")
+            requests = requests.copy()
+            per_request = np.repeat(min_members, np.diff(gang_off.astype(np.int64)))
+            alloc = requests["op"] == OP_ALLOC
+            requests["size"][alloc] = per_request[alloc].astype(np.uint8)
         out = np.empty(len(requests), dtype=RESULT_DTYPE)
         self._check(self._lib.isl_place_gangs(self._h, len(gang_off) - 1, _ptr(gang_off), _ptr(requests), _ptr(out)), "isl_place_gangs")
         return out

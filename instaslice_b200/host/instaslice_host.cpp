@@ -223,12 +223,19 @@ std::vector<GangOutcome> InstasliceReconciler::PlaceGangs(InstasliceList& list, 
 // `locality` empty: every ALLOC keeps start 0, which an engine without ISL_FLAG_GANG_LOCALITY ignores
 std::vector<GangOutcome> InstasliceReconciler::PlaceGangs(InstasliceList& list, AllocationPolicy& policy, const std::vector<std::vector<PendingPod>>& gangs,
                                                           const std::vector<uint8_t>& locality) {
+    return PlaceGangs(list, policy, gangs, locality, {});
+}
+
+// `minMembers` empty: every ALLOC keeps size 0, which an engine without ISL_FLAG_GANG_MIN_MEMBERS ignores
+std::vector<GangOutcome> InstasliceReconciler::PlaceGangs(InstasliceList& list, AllocationPolicy& policy, const std::vector<std::vector<PendingPod>>& gangs,
+                                                          const std::vector<uint8_t>& locality, const std::vector<uint8_t>& minMembers) {
     std::vector<GangOutcome> out(gangs.size());
     if (!locality.empty() && locality.size() != gangs.size()) throw std::runtime_error("one locality per gang");
+    if (!minMembers.empty() && minMembers.size() != gangs.size()) throw std::runtime_error("one minimum per gang");
     if (gangs.empty()) return out;
     if (orphans_ && gangs.size() > 1) {         // the veto must see one gang at a time: a vetoed gang leaves no trace before the next
-        for (size_t g = 0; g < gangs.size(); ++g)
-            out[g] = PlaceGangs(list, policy, {gangs[g]}, locality.empty() ? std::vector<uint8_t>{} : std::vector<uint8_t>{locality[g]})[0];
+        auto one = [](const std::vector<uint8_t>& v, size_t g) { return v.empty() ? std::vector<uint8_t>{} : std::vector<uint8_t>{v[g]}; };
+        for (size_t g = 0; g < gangs.size(); ++g) out[g] = PlaceGangs(list, policy, {gangs[g]}, one(locality, g), one(minMembers, g))[0];
         return out;
     }
     std::vector<std::string> names;
@@ -242,24 +249,29 @@ std::vector<GangOutcome> InstasliceReconciler::PlaceGangs(InstasliceList& list, 
     if (!locality.empty())
         for (size_t g = 0; g < gangs.size(); ++g)
             for (uint32_t i = off[g]; i < off[g + 1]; ++i) req[i].start = locality[g];
+    if (!minMembers.empty())
+        for (size_t g = 0; g < gangs.size(); ++g)
+            for (uint32_t i = off[g]; i < off[g + 1]; ++i) req[i].size = minMembers[g];
     std::vector<isl_result> res(names.size());
     check(isl_place_gangs(h_, (uint32_t)gangs.size(), off.data(), req.data(), res.data()), h_, "isl_place_gangs");
     for (size_t g = 0; g < gangs.size(); ++g) {
-        bool placed = true, veto = false;
-        for (uint32_t i = off[g]; i < off[g + 1]; ++i) placed = placed && res[i].status == ISL_ST_PLACED;
-        if (!placed) continue;                  // nothing of the gang was committed
+        // the placed pods are a leading run: the whole gang, none, or an elastic gang's first pods
+        uint32_t end = off[g];
+        while (end < off[g + 1] && res[end].status == ISL_ST_PLACED) ++end;
+        if (end == off[g]) continue;            // nothing of the gang was committed
+        bool veto = false;
         GangOutcome& o = out[g];
-        for (uint32_t i = off[g]; i < off[g + 1]; ++i) {
+        for (uint32_t i = off[g]; i < end; ++i) {
             o.allocs.push_back(pack(list, policy, gangs[g][i - off[g]], res[i]));
             veto = veto || vetoed(list, res[i], o.allocs.back());
         }
         if (veto) {                             // one member vetoed: every span of the gang is released again
-            for (uint32_t i = off[g]; i < off[g + 1]; ++i) releaseSpan(res[i]);
+            for (uint32_t i = off[g]; i < end; ++i) releaseSpan(res[i]);
             o.allocs.clear();
             o.verdict = Verdict::Veto;
             continue;
         }
-        for (uint32_t i = off[g]; i < off[g + 1]; ++i) list.Items[gpuNode_[res[i].gpu]].Spec.Allocations[gangs[g][i - off[g]].pod.UID] = o.allocs[i - off[g]];
+        for (uint32_t i = off[g]; i < end; ++i) list.Items[gpuNode_[res[i].gpu]].Spec.Allocations[gangs[g][i - off[g]].pod.UID] = o.allocs[i - off[g]];
         o.verdict = Verdict::Placed;
     }
     return out;

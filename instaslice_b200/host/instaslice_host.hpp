@@ -90,7 +90,8 @@ public:
     // ISL_POLICY_LEAST_ALLOCATED to spread them (include/islplace.h).  flags: isl_config.flags, e.g. ISL_FLAG_GANG_ONE_NODE so that
     // PlaceGangs puts every gang on one node, ISL_FLAG_GANG_DISTINCT_NODES so that it puts every member of a gang on a different node,
     // ISL_FLAG_GANG_FEW_NODES so that it puts a gang on one node when one takes it and on as few nodes as it greedily can otherwise, or
-    // ISL_FLAG_GANG_LOCALITY so that PlaceGangs takes one of these localities per gang
+    // ISL_FLAG_GANG_LOCALITY so that PlaceGangs takes one of these localities per gang; ISL_FLAG_GANG_MIN_MEMBERS (alone or with one of
+    // the four) so that PlaceGangs takes a minimum per gang
     explicit InstasliceReconciler(uint32_t quirks = ISL_QUIRKS_REF_EXACT, uint32_t max_gpus = 1u << 16, uint32_t max_batch = 1u << 16,
                                   uint32_t policy = ISL_POLICY_FIRST_FIT, uint32_t flags = 0);
     ~InstasliceReconciler();
@@ -120,6 +121,12 @@ public:
     // with ISL_FLAG_GANG_LOCALITY: one call places gangs of every locality on one occupancy.  Throws unless there is one per gang.
     std::vector<GangOutcome> PlaceGangs(InstasliceList& list, AllocationPolicy& policy, const std::vector<std::vector<PendingPod>>& gangs,
                                         const std::vector<uint8_t>& locality);
+    // The same with one minimum m (0..255) per gang as well (empty: none), for a reconciler created with ISL_FLAG_GANG_MIN_MEMBERS
+    // (include/islplace.h M1-M7): a gang whose leading pods reach its minimum while a later pod finds no GPU is Placed with those pods
+    // only, so its allocs are a shorter, leading part of the gang, and only they are written into `list`.  `locality` may be empty
+    // on an engine without ISL_FLAG_GANG_LOCALITY.  Throws unless each non-empty list has one entry per gang.
+    std::vector<GangOutcome> PlaceGangs(InstasliceList& list, AllocationPolicy& policy, const std::vector<std::vector<PendingPod>>& gangs,
+                                        const std::vector<uint8_t>& locality, const std::vector<uint8_t>& minMembers);
     // Which lower-priority allocations each pending pod should evict, in order, ONE engine call (isl_preempt).  podPriority maps the UID
     // of each running pod to its PriorityClass value; values become dense ranks (more than 255 distinct values throw).  An allocation
     // may be evicted only when its pod's priority is known, its status is not "deleted" and no other entry that marks slices busy

@@ -74,7 +74,13 @@ const (
 	// PlaceGangsWithLocality takes one of the Gang* localities per gang, so one call places every kind of gang on one occupancy.
 	// Not with the three flags above.
 	FlagGangLocality = uint32(C.ISL_FLAG_GANG_LOCALITY)
+	// PlaceGangsElastic takes a minimum per gang: a gang whose leading pods reach it while a later pod finds no GPU is placed with
+	// those pods only.  Alone or with one of the four flags above.
+	FlagGangMinMembers = uint32(C.ISL_FLAG_GANG_MIN_MEMBERS)
 )
+
+// StGangTrimmed is the record status of a pod its elastic gang was placed without (isl_result.status, FlagGangMinMembers).
+const StGangTrimmed = uint16(C.ISL_ST_GANG_TRIMMED)
 
 // Node locality of one gang for PlaceGangsWithLocality (an engine created with FlagGangLocality).
 const (
@@ -397,9 +403,21 @@ func (r *InstasliceReconciler) PlaceGangs(e *PlacementEngine, list *inferencev1a
 // a training job on one node, replicas on distinct nodes, a job on few nodes and free pods in one call.
 func (r *InstasliceReconciler) PlaceGangsWithLocality(e *PlacementEngine, list *inferencev1alpha1.InstasliceList, policy AllocationPolicy,
 	gangs [][]PendingPod, locality []uint8) ([][]*inferencev1alpha1.AllocationDetails, error) {
+	return r.PlaceGangsElastic(e, list, policy, gangs, locality, nil)
+}
+
+// PlaceGangsElastic is PlaceGangsWithLocality with one minimum m (0..255) per gang as well (nil: none), for an engine created with
+// FlagGangMinMembers (a PodGroup's minMember, Volcano's minAvailable, Kueue's PodSet minCount).  locality may be nil on an engine
+// without FlagGangLocality.  A gang whose leading pods reach its minimum while a later pod finds no GPU gets the allocations of those
+// pods only, a shorter slice than the gang; list the pods the job needs first, since the placed pods are always a leading run.
+func (r *InstasliceReconciler) PlaceGangsElastic(e *PlacementEngine, list *inferencev1alpha1.InstasliceList, policy AllocationPolicy,
+	gangs [][]PendingPod, locality []uint8, minMembers []uint8) ([][]*inferencev1alpha1.AllocationDetails, error) {
 	out := make([][]*inferencev1alpha1.AllocationDetails, len(gangs))
 	if locality != nil && len(locality) != len(gangs) {
 		return nil, fmt.Errorf("one locality per gang")
+	}
+	if minMembers != nil && len(minMembers) != len(gangs) {
+		return nil, fmt.Errorf("one minimum per gang")
 	}
 	if len(gangs) == 0 {
 		return out, nil
@@ -413,11 +431,14 @@ func (r *InstasliceReconciler) PlaceGangsWithLocality(e *PlacementEngine, list *
 	}
 	if e.orphans && len(gangs) > 1 { // the exact-match veto (:198-203) must see one gang at a time
 		for g := range gangs {
-			var loc []uint8
+			var loc, mins []uint8
 			if locality != nil {
 				loc = locality[g : g+1]
 			}
-			one, err := r.PlaceGangsWithLocality(e, list, policy, gangs[g:g+1], loc)
+			if minMembers != nil {
+				mins = minMembers[g : g+1]
+			}
+			one, err := r.PlaceGangsElastic(e, list, policy, gangs[g:g+1], loc, mins)
 			if err != nil {
 				return nil, err
 			}
@@ -448,19 +469,25 @@ func (r *InstasliceReconciler) PlaceGangsWithLocality(e *PlacementEngine, list *
 				req[i].start = C.uint8_t(locality[g])
 			}
 		}
+		if minMembers != nil {
+			for i := off[g]; i < off[g+1]; i++ {
+				req[i].size = C.uint8_t(minMembers[g])
+			}
+		}
 	}
 	if rc := C.isl_place_gangs(e.h, C.uint32_t(len(gangs)), &off[0], &req[0], &res[0]); rc != C.ISL_OK {
 		return nil, fmt.Errorf("isl_place_gangs: %s (%s)", C.GoString(C.isl_strerror(rc)), C.GoString(C.isl_last_cuda_error(e.h)))
 	}
 	for g, pods := range gangs {
 		gres := res[off[g]:off[g+1]]
-		placed := true
-		for i := range gres {
-			placed = placed && gres[i].status == C.ISL_ST_PLACED
+		placed := 0 // a leading run: the whole gang, none, or an elastic gang's first pods
+		for placed < len(gres) && gres[placed].status == C.ISL_ST_PLACED {
+			placed++
 		}
-		if !placed {
+		if placed == 0 {
 			continue
 		}
+		pods, gres = pods[:placed], gres[:placed]
 		allocs := make([]*inferencev1alpha1.AllocationDetails, len(pods))
 		vetoed := false
 		for i, p := range pods {
