@@ -2340,7 +2340,7 @@ __device__ __forceinline__ unsigned long long warp_min(unsigned long long v) {
 }
 
 // The minimum of `v` over every thread of a cooperative launch of kThreads threads per CTA, returned to every thread (k_preempt,
-// k_gangnode, k_gangspread; DESIGN.md 4.7).  Every thread of every CTA must call it: it holds the grid barrier.  Each CTA reduces by warp,
+// k_ganglocal; DESIGN.md 4.7).  Every thread of every CTA must call it: it holds the grid barrier.  Each CTA reduces by warp,
 // then across the block, and writes its minimum to keys[parity * gridDim.x + blockIdx.x]; after grid.sync warp 0 reads every CTA's
 // minimum with __ldcg (other SMs wrote them; L1 is not coherent) and broadcasts the result through s_win.  The minima are double-buffered
 // by `parity`, which the call flips: a fast CTA may write round i + 1 before a slow one has read round i.
@@ -2612,31 +2612,16 @@ __global__ void __launch_bounds__(kNfThreads, 1) k_nodefit(NodeFitArgs a, uint32
 }
 
 // ---------------------------------------------------------------------------------------------
-// k_gangnode: isl_place_gangs on an engine created with ISL_FLAG_GANG_ONE_NODE (DESIGN.md 4.9): every gang commits on the first node, in
-// the engine's scan order (storage order: ascending canonical, descending under ISL_POLICY_RIGHT_TO_LEFT), that takes all of its ALLOC
-// members.  One cooperative launch per call behind k_prepare (frees and default records).  CTA c owns the partition's nodes
-// [cta_node[c], cta_node[c + 1]) (whole nodes, balanced by GPU count on the host) and keeps their occupancy bytes and a scratch copy in
-// shared memory (global memory when a share is too large for it).  Per gang:
-//   evaluate  one warp per node: copy the node's bytes to the scratch copy and count its free slices; a node with fewer free slices than
-//             the gang's members need on its table is skipped (pass 0 only).  Otherwise the warp resolves the members in order on the
-//             scratch copy, each one a warp min over the node's GPUs of score(t, p, o) << 24 | position (k_bestfit's lut and score tables; a
-//             zero score table is first-fit).  Key: the node index for a success, else bit 63 | (2^31 - 1 - depth) << 32 | node.
-//   reduce    grid_min: the smallest key is the first node in scan order that takes the whole gang, or, with no such node, the deepest
-//             failure.  When the winner of pass 0 is a failure every node is evaluated again without the filter (pass 1), since the
-//             skipped nodes' depths are unknown.
-//   commit    the warp 0 of the CTA that owns the winning node resolves the members again on the live bytes and writes the PLACED records
-//             and the occupancy; a failure: CTA 0 reports every ALLOC member except the one at depth D GANG_ABORTED (that one keeps
-//             k_prepare's NO_CAPACITY or BAD_PROFILE record).
-// k_gangnode<true>: ISL_FLAG_GANG_FEW_NODES (DESIGN.md 4.11).  A gang is a loop of rounds over its remaining members, from request ri on;
-// each round is the evaluate and reduce steps above, and the winning key's depth d is how many members the round places (a success: all
-// that remain).  The owner commits those d on its live bytes as tentative PLACED records and every CTA advances ri past d ALLOC members.
-// d = 0 aborts the gang without an undo log: the spans of one gang are disjoint and were free before it, so each CTA clears the spans of
-// the tentative records on its own nodes (gangfew_undo) and reports those members GANG_ABORTED, while CTA 0 reports the members after
-// the one that found no node.  Every barrier depends only on the gang offsets and the winning keys, which every CTA sees alike.
+// Gang topology: k_ganglocal (at the end of this file) and the per-gang bodies it runs (DESIGN.md 4.9-4.13).
 // ---------------------------------------------------------------------------------------------
 constexpr uint32_t kGnThreads = 512;
 constexpr uint32_t kGnMaxCtas = 160;                    // CTAs of one launch (at most one per SM)
 constexpr unsigned long long kGnFail = 1ull << 63;
+// A failed node's key in one- and few-node gangs: the deeper failure, then the lower node, is the smaller key
+__device__ __forceinline__ unsigned long long gn_fail_key(uint32_t depth, uint32_t j) {
+    return kGnFail | ((unsigned long long)(0x7FFFFFFFu - depth) << 32) | j;
+}
+__device__ __forceinline__ uint32_t gn_fail_depth(unsigned long long key) { return 0x7FFFFFFFu - (uint32_t)((key >> 32) & 0x7FFFFFFFu); }
 
 struct GangNodeArgs {           // kernel parameter (by value)
     const uint2* in;            // requests (isl_request)
@@ -2695,8 +2680,8 @@ __device__ uint32_t gangnode_resolve(const GangNodeArgs& a, const DevProfiles& p
     return depth;
 }
 
-// A CTA's share of the partition in k_gangnode and k_gangspread: the partition's nodes [j0, j1), which own its partition-local GPUs
-// [base, base + cnt).  `live` holds their committed bytes and `aux` a second byte per GPU (k_gangnode: scratch copies, k_gangspread:
+// A CTA's share of the partition in k_ganglocal: the partition's nodes [j0, j1), which own its partition-local GPUs [base, base + cnt).
+// `live` holds their committed bytes and `aux` a second byte per GPU (one- and few-node gangs: scratch copies, distinct-node gangs:
 // node-used marks), both in shared memory, or in global memory when a share is too large for it (a.share == 0).  Every thread of the CTA
 // builds it: the constructor copies the committed bytes into shared memory.
 struct NodeShare {
@@ -2711,6 +2696,26 @@ struct NodeShare {
     // node j of the partition owns the partition-local GPUs [nb(j), nb(j + 1)); a node the partition cuts keeps its GPUs inside it
     __device__ __forceinline__ uint32_t nb(uint32_t j) const { return min(max(a.node_off[a.nlo + j], a.lo), a.hi) - a.lo; }
 };
+
+// Warp-wide, on a warp of the CTA that owns node j: commit the ALLOC members of requests [r, r1) on the node's live bytes (they stop by
+// themselves where the evaluation on the scratch copy stopped).
+__device__ __forceinline__ void gangnode_commit(const GangNodeArgs& a, const DevProfiles& prof, const NodeShare& sh, uint32_t j, uint32_t r,
+                                                uint32_t r1, uint32_t lane) {
+    const uint32_t b0 = sh.nb(j) - sh.base, c = sh.nb(j + 1) - sh.base - b0;
+    gangnode_resolve(a, prof, sh.live + b0, c, a.lo + sh.base + b0, a.gtab[a.lo + sh.base + b0] & (kMaxTables - 1), r, r1, true, lane);
+}
+
+// One thread: request r, of profile p, takes its slices on the share's GPU g (partition-local sh.base + g) by the engine's policy: its
+// live byte, the occupancy and a PLACED record.
+__device__ __forceinline__ void commit_member(const GangNodeArgs& a, const DevProfiles& prof, const NodeShare& sh, uint32_t r, uint32_t p,
+                                              uint32_t g) {
+    const uint32_t t = a.gtab[a.lo + sh.base + g] & (kMaxTables - 1), row = (t * ISL_MAX_PROFILES + p) * 256, o = sh.live[g];
+    const uint32_t start = __ldg(a.lut + row + o), size = __ldg(a.sizes + t * ISL_MAX_PROFILES + p);
+    const uint32_t o2 = o | slice_span(start, size);
+    sh.live[g] = (uint8_t)o2;
+    a.occ[a.lo + sh.base + g] = (uint8_t)o2;
+    a.out[r] = pack_result(flip_gpu(a.lo + sh.base + g, prof.flip), start, size, ISL_ST_PLACED);
+}
 
 // Warp-wide: a gang of requests [r0, r1) failed.  Every ALLOC member except the one of rank keep_rank among them is reported
 // GANG_ABORTED; that one keeps k_prepare's NO_CAPACITY or BAD_PROFILE record.  kTrim (an elastic gang that commits its leading members,
@@ -2729,7 +2734,7 @@ __device__ __forceinline__ void abort_gang_members(const uint2* in, uint2* out, 
     }
 }
 
-// Warp-wide (k_gangnode<true>): the request just past the d-th ALLOC member at or after request r (d >= 1, and [r, r1) holds that many).
+// Warp-wide (few-node gangs): the request just past the d-th ALLOC member at or after request r (d >= 1, and [r, r1) holds that many).
 __device__ __forceinline__ uint32_t skip_allocs(const uint2* in, uint32_t r, uint32_t r1, uint32_t d, uint32_t lane) {
     for (;; r += 32) {
         uint32_t ballot = __ballot_sync(0xFFFFFFFFu, r + lane < r1 && ((in[r + lane].y >> 8) & 0xFFu) == ISL_OP_ALLOC);
@@ -2741,12 +2746,11 @@ __device__ __forceinline__ uint32_t skip_allocs(const uint2* in, uint32_t r, uin
         d -= c;
     }
 }
-
-// Warp-wide (k_gangnode<true>): a few-node gang aborted after earlier rounds committed its ALLOC members among requests [r0, r1) as
-// tentative PLACED records.  The CTA takes back those on its own nodes: the spans of one gang are disjoint and were free before it, so
-// clearing them restores its live bytes and the occupancy, and it reports those members GANG_ABORTED (it is their records' only writer).
-// The records may come from other CTAs, written before a grid barrier of a later round, so they are read from L2.  One lane at a time
-// writes, since two members may share a GPU.
+// Warp-wide (few-node and any-node gangs): a gang aborted after earlier rounds or members committed its ALLOC members among requests
+// [r0, r1) as tentative PLACED records.  The CTA takes back those on its own nodes: the spans of one gang are disjoint and were free
+// before it, so clearing them restores its live bytes and the occupancy, and it reports those members GANG_ABORTED (it is their records'
+// only writer).  The records may come from other CTAs, written before a grid barrier of a later round, so they are read from L2.  One
+// lane at a time writes, since two members may share a GPU.
 __device__ void gangfew_undo(const GangNodeArgs& a, const NodeShare& sh, const DevProfiles& prof, uint32_t r0, uint32_t r1, uint32_t lane) {
     for (uint32_t r = r0; r < r1; r += 32) {
         const uint32_t i = r + lane;
@@ -2768,11 +2772,28 @@ __device__ void gangfew_undo(const GangNodeArgs& a, const NodeShare& sh, const D
     }
 }
 
-// One gang of requests [r0, r1) of k_gangnode<kFew> (and of k_ganglocal's localities 1 and 2), every thread of the CTA.  `scr`, the
+// One gang of requests [r0, r1) of k_ganglocal of locality 1 (one node) or, kFew, 2 (few nodes), every thread of the CTA.  `scr`, the
 // scratch copies, is the share's aux byte.  The shared words are the kernel's: s_warp and s_win for grid_min, s_need and s_allocs.
-// kMin (k_ganglocal<true>, M3): a gang that fails at ALLOC member f >= min_m commits its first f members instead of aborting.  One node:
-// f is the deepest failure's depth D, and the owner of the first node that reaches it replays the members on its live bytes, which stop
-// at D by themselves (the scratch copy started from the same bytes).  Few nodes: f is the members the earlier rounds placed.
+// One node (DESIGN.md 4.9): the gang commits on the first node, in the engine's scan order (storage order: ascending canonical,
+// descending under ISL_POLICY_RIGHT_TO_LEFT), that takes all of its ALLOC members:
+//   evaluate  one warp per node: copy the node's bytes to the scratch copy and count its free slices; a node with fewer free slices than
+//             the gang's members need on its table is skipped (pass 0 only).  Otherwise the warp resolves the members in order on the
+//             scratch copy, each one a warp min over the node's GPUs of score(t, p, o) << 24 | position (k_bestfit's lut and score tables; a
+//             zero score table is first-fit).  Key: the node index for a success, else gn_fail_key(depth, node).
+//   reduce    grid_min: the smallest key is the first node in scan order that takes the whole gang, or, with no such node, the deepest
+//             failure.  When the winner of pass 0 is a failure every node is evaluated again without the filter (pass 1), since the
+//             skipped nodes' depths are unknown.
+//   commit    the warp 0 of the CTA that owns the winning node resolves the members again on the live bytes and writes the PLACED records
+//             and the occupancy; a failure: CTA 0 reports every ALLOC member except the one at depth D GANG_ABORTED (that one keeps
+//             k_prepare's NO_CAPACITY or BAD_PROFILE record).
+// Few nodes (4.11): a loop of rounds over the gang's remaining members, from request ri on; each round is the evaluate and reduce steps
+// above, and the winning key's depth d is how many members the round places (a success: all that remain).  The owner commits those d on
+// its live bytes as tentative PLACED records and every CTA advances ri past d ALLOC members.  d = 0 aborts the gang without an undo log:
+// each CTA takes back the tentative records on its own nodes (gangfew_undo), while CTA 0 reports the members after the one that found
+// no node.
+// kMin (k_ganglocal<kLocPerGang, true>, M3): a gang that fails at ALLOC member f >= min_m commits its first f members instead of aborting.
+// One node: f is the deepest failure's depth D, and the owner of the first node that reaches it replays the members on its live bytes,
+// which stop at D by themselves (the scratch copy started from the same bytes).  Few nodes: f is the members the earlier rounds placed.
 template <bool kFew, bool kMin = false>
 __device__ __forceinline__ void gangnode_gang(const GangNodeArgs& a, const DevProfiles& prof, const NodeShare& sh, uint32_t r0, uint32_t r1,
                                               uint32_t& parity, uint32_t& placed, unsigned long long* s_warp, unsigned long long* s_win,
@@ -2813,7 +2834,7 @@ __device__ __forceinline__ void gangnode_gang(const GangNodeArgs& a, const DevPr
                 free_slices = __reduce_add_sync(0xFFFFFFFFu, free_slices);
                 if (pass == 0 && free_slices < s_need[t]) continue;
                 const uint32_t d = gangnode_resolve(a, prof, scr + b0, c, a.lo + sh.base + b0, t, ri, r1, false, lane);
-                best = min(best, d == allocs ? (unsigned long long)j : kGnFail | ((unsigned long long)(0x7FFFFFFFu - d) << 32) | j);
+                best = min(best, d == allocs ? (unsigned long long)j : gn_fail_key(d, j));
             }
             win = grid_min<kGnThreads>(best, a.keys, parity, s_warp, s_win);
             if (!(win & kGnFail)) break;                    // a node takes the whole gang: the skipped nodes could not have come first
@@ -2821,8 +2842,7 @@ __device__ __forceinline__ void gangnode_gang(const GangNodeArgs& a, const DevPr
         if (!(win & kGnFail)) {
             const uint32_t j = (uint32_t)win;
             if (j >= sh.j0 && j < sh.j1 && warp == 0) {     // the owner commits on its live bytes
-                const uint32_t b0 = sh.nb(j) - sh.base, c = sh.nb(j + 1) - sh.base - b0;
-                gangnode_resolve(a, prof, sh.live + b0, c, a.lo + sh.base + b0, a.gtab[a.lo + sh.base + b0] & (kMaxTables - 1), ri, r1, true, lane);
+                gangnode_commit(a, prof, sh, j, ri, r1, lane);
                 placed += allocs;
             }
             if (kFew) placed += held;                       // the gang commits: its tentative members count
@@ -2830,11 +2850,10 @@ __device__ __forceinline__ void gangnode_gang(const GangNodeArgs& a, const DevPr
         }
         if constexpr (!kFew) {
             if constexpr (kMin) {
-                const uint32_t d = 0x7FFFFFFFu - (uint32_t)((win >> 32) & 0x7FFFFFFFu), j = (uint32_t)win;
+                const uint32_t d = gn_fail_depth(win), j = (uint32_t)win;
                 if (d >= min_m) {                           // min_m >= 1, so ~0ull (depth 0) never gets here
                     if (j >= sh.j0 && j < sh.j1 && warp == 0) {
-                        const uint32_t b0 = sh.nb(j) - sh.base, c = sh.nb(j + 1) - sh.base - b0;
-                        gangnode_resolve(a, prof, sh.live + b0, c, a.lo + sh.base + b0, a.gtab[a.lo + sh.base + b0] & (kMaxTables - 1), ri, r1, true, lane);
+                        gangnode_commit(a, prof, sh, j, ri, r1, lane);
                         placed += d;
                     }
                     if (blockIdx.x == 0 && warp == 0) abort_gang_members<true>(a.in, a.out, prof, r0, r1, d, lane);
@@ -2842,10 +2861,10 @@ __device__ __forceinline__ void gangnode_gang(const GangNodeArgs& a, const DevPr
                 }
             }
             if (blockIdx.x == 0 && warp == 0)               // the deepest failure's depth; ~0ull (no node evaluated) is depth 0 as well
-                abort_gang_members(a.in, a.out, prof, r0, r1, 0x7FFFFFFFu - (uint32_t)((win >> 32) & 0x7FFFFFFFu), lane);
+                abort_gang_members(a.in, a.out, prof, r0, r1, gn_fail_depth(win), lane);
             break;
         } else {
-            const uint32_t d = 0x7FFFFFFFu - (uint32_t)((win >> 32) & 0x7FFFFFFFu), j = (uint32_t)win;  // members the round places
+            const uint32_t d = gn_fail_depth(win), j = (uint32_t)win;      // members the round places
             if (kMin && d == 0 && done >= min_m) {          // the earlier rounds' members commit, m_i keeps its record
                 placed += held;
                 if (blockIdx.x == 0 && warp == 0) abort_gang_members<true>(a.in, a.out, prof, ri, r1, 0, lane);
@@ -2857,8 +2876,7 @@ __device__ __forceinline__ void gangnode_gang(const GangNodeArgs& a, const DevPr
                 break;
             }
             if (j >= sh.j0 && j < sh.j1 && warp == 0) {     // the owner commits the round's d members on its live bytes
-                const uint32_t b0 = sh.nb(j) - sh.base, c = sh.nb(j + 1) - sh.base - b0;
-                gangnode_resolve(a, prof, sh.live + b0, c, a.lo + sh.base + b0, a.gtab[a.lo + sh.base + b0] & (kMaxTables - 1), ri, r1, true, lane);
+                gangnode_commit(a, prof, sh, j, ri, r1, lane);
                 held += d;
             }
             ri = skip_allocs(a.in, ri, r1, d, lane);        // every CTA read the same key: all advance alike
@@ -2867,42 +2885,20 @@ __device__ __forceinline__ void gangnode_gang(const GangNodeArgs& a, const DevPr
     }
 }
 
-template <bool kFew>
-__global__ void __launch_bounds__(kGnThreads, 1) k_gangnode(GangNodeArgs a, DevProfiles prof) {
-    extern __shared__ __align__(16) uint8_t gn_smem[];
-    __shared__ unsigned long long s_warp[kGnThreads / 32];
-    __shared__ unsigned long long s_win;
-    __shared__ uint32_t s_need[kMaxTables], s_allocs;
-    const uint32_t tid = threadIdx.x, lane = tid & 31u, warp = tid >> 5;
-    const NodeShare sh(a, gn_smem);
-    uint32_t parity = 0, placed = 0;
-    for (uint32_t gi = 0; gi < a.n_gangs; ++gi)
-        gangnode_gang<kFew>(a, prof, sh, __ldg(a.gang_off + gi), __ldg(a.gang_off + gi + 1), parity, placed, s_warp, &s_win, s_need, &s_allocs,
-                            tid, lane, warp);
-    if (tid == 0 && placed) count_placed(a.ctrl, placed);
-}
-
-// ---------------------------------------------------------------------------------------------
-// k_gangspread: isl_place_gangs on an engine created with ISL_FLAG_GANG_DISTINCT_NODES (DESIGN.md 4.10): the ALLOC members of a gang are
-// resolved in order, each by the engine's policy restricted to the partition's GPUs whose node holds no earlier member of the same gang.
-// So no member ever sees another member's slices: a member's key on a GPU depends only on the committed bytes, and the kernel needs no
-// scratch copy and no rollback.  One cooperative launch per call behind k_prepare (frees and default records), with k_gangnode's layout:
-// CTA c owns the partition's nodes [cta_node[c], cta_node[c + 1]) and keeps their live bytes in shared memory, and its "node used" marks
-// next to them (both in global memory when a share is too large).  Per ALLOC member:
+// One gang of requests [r0, r1) of k_ganglocal of locality 3 (distinct nodes, DESIGN.md 4.10), every thread of the CTA: the ALLOC
+// members are resolved in order, each by the engine's policy restricted to the partition's GPUs whose node holds no earlier member of
+// the same gang.  So no member ever sees another member's slices: a member's key on a GPU depends only on the committed bytes, and the
+// gang needs no scratch copy and no rollback.  Per ALLOC member:
 //   choose    every CTA takes the minimum of score(t, p, o) << 24 | partition-local storage position over its GPUs not marked used
 //             (k_bestfit's lut and score tables; a zero score table is first-fit, and right-to-left is the ascending scan of its reversed
 //             storage); grid_min over the CTAs' 32-bit minima gives every CTA the member's GPU.
 //   mark      the CTA that owns that GPU marks its node's GPUs with the gang's tag and pushes (request, GPU) onto its stack of wins.
 // A member with no GPU ends the gang: it keeps k_prepare's record (NO_CAPACITY or BAD_PROFILE), CTA 0 reports every other ALLOC member
-// GANG_ABORTED, and no occupancy byte is written.  Otherwise every CTA writes the bytes and PLACED records of its stack.  A profile that
-// finds no GPU as a gang's first ALLOC member (no exclusion in force) is dead for the rest of the call: after the FREEs of k_prepare the
-// occupancy only grows.  Tags run 1..255 with the gang index; the marks are cleared once every 255 gangs.
-// ---------------------------------------------------------------------------------------------
-// One gang of requests [r0, r1) of k_gangspread (and of k_ganglocal's locality 3), every thread of the CTA.  `tag` (1..255) marks the
-// nodes the gang uses in the share's aux byte; tag 1 clears the marks first, so a mark can only equal `tag` when this gang wrote it.
-// `dead`: profiles no GPU of the partition admits any more.  The shared words are the kernel's: s_warp and s_win for grid_min, and the
-// size of the CTA's stack of wins, which is 0 between gangs.  kMin (k_ganglocal<true>, M3): a member that finds no GPU at rank
-// fail >= min_m commits the stack of wins, which holds the members before it, as a success does.
+// GANG_ABORTED, and no occupancy byte is written.  Otherwise every CTA writes the bytes and PLACED records of its stack.
+// `tag` (1..255) marks the nodes the gang uses in the share's aux byte; tag 1 clears the marks first, so a mark can only equal `tag` when
+// this gang wrote it.  `dead`: profiles no GPU of the partition admits any more.  The shared words are the kernel's: s_warp and s_win for
+// grid_min, and the size of the CTA's stack of wins, which is 0 between gangs.  kMin (k_ganglocal<kLocPerGang, true>, M3): a member that
+// finds no GPU at rank fail >= min_m commits the stack of wins, which holds the members before it, as a success does.
 template <bool kMin = false>
 __device__ __forceinline__ void gangspread_gang(const GangNodeArgs& a, const DevProfiles& prof, const NodeShare& sh, uint2* wins, uint32_t r0,
                                                 uint32_t r1, uint32_t tag, uint32_t& parity, uint32_t& placed, uint32_t& dead,
@@ -2947,13 +2943,7 @@ __device__ __forceinline__ void gangspread_gang(const GangNodeArgs& a, const Dev
         const uint32_t nw = *s_nwins;
         for (uint32_t k = tid; k < nw; k += kGnThreads) {
             const uint2 w = wins[sh.j0 + k];
-            const uint32_t g = w.y, p = a.in[w.x].y & 0xFFu, t = a.gtab[a.lo + base + g] & (kMaxTables - 1);
-            const uint32_t row = (t * ISL_MAX_PROFILES + p) * 256, o = sh.live[g];
-            const uint32_t start = __ldg(a.lut + row + o), size = __ldg(a.sizes + t * ISL_MAX_PROFILES + p);
-            const uint32_t o2 = o | slice_span(start, size);
-            sh.live[g] = (uint8_t)o2;
-            a.occ[a.lo + base + g] = (uint8_t)o2;
-            a.out[w.x] = pack_result(flip_gpu(a.lo + base + g, prof.flip), start, size, ISL_ST_PLACED);
+            commit_member(a, prof, sh, w.x, a.in[w.x].y & 0xFFu, w.y);
         }
         placed += nw;
         if (trim && blockIdx.x == 0 && warp == 0) abort_gang_members<true>(a.in, a.out, prof, r0, r1, fail, lane);
@@ -2964,38 +2954,12 @@ __device__ __forceinline__ void gangspread_gang(const GangNodeArgs& a, const Dev
     if (tid == 0) *s_nwins = 0;
 }
 
-__global__ void __launch_bounds__(kGnThreads, 1) k_gangspread(GangNodeArgs a, DevProfiles prof, uint2* wins) {
-    extern __shared__ __align__(16) uint8_t gs_smem[];
-    __shared__ uint32_t s_warp[kGnThreads / 32];
-    __shared__ uint32_t s_win, s_nwins;
-    const uint32_t tid = threadIdx.x, lane = tid & 31u, warp = tid >> 5;
-    const NodeShare sh(a, gs_smem);
-    if (tid == 0) s_nwins = 0;
-    uint32_t parity = 0, placed = 0, dead = 0;                            // dead: profiles no GPU of the partition admits any more
-    for (uint32_t gi = 0; gi < a.n_gangs; ++gi)                           // tags run 1..255 with the gang index
-        gangspread_gang(a, prof, sh, wins, __ldg(a.gang_off + gi), __ldg(a.gang_off + gi + 1), 1u + gi % 255u, parity, placed, dead,
-                        s_warp, &s_win, &s_nwins, tid, lane, warp);
-    if (tid == 0 && placed) count_placed(a.ctrl, placed);
-}
-
-// ---------------------------------------------------------------------------------------------
-// k_ganglocal: isl_place_gangs on an engine created with ISL_FLAG_GANG_LOCALITY (DESIGN.md 4.12): each gang names its own node locality
-// (locality[gi], one byte per gang, checked on the host), and the gangs run in array order, each on the occupancy the earlier ones left.
-// One cooperative launch per call behind k_prepare, with k_gangnode's layout.  The byte is the same for every CTA, so the branch is
-// grid-uniform, and every barrier depends only on the gang offsets, the locality bytes and the winning keys.
-//   1, 2      gangnode_gang<false> / <true>: k_gangnode's gang, one node or few nodes.  Its scratch copies overwrite the aux bytes.
-//   3         gangspread_gang: k_gangspread's gang.  Tags count locality-3 gangs and restart at 1, which clears the marks, after every
-//             locality-1 or -2 gang, whose scratch copies may equal any tag.
-//   0 (any)   ganglocal_any: rules 2-4, member by member over the whole share.
-// The dead-profile mask is shared by localities 0 and 3: a bit is set only when a gang's first ALLOC member finds no GPU, on a state
-// without tentative slices; after k_prepare's FREEs the occupancy only grows and an abort restores it exactly, so the bit stays valid.
-// ---------------------------------------------------------------------------------------------
 // One gang of locality 0: every CTA takes the minimum of score(t, p, o) << 24 | partition-local storage position over its live bytes
-// (k_gangspread's key with no GPU masked), grid_min gives every CTA the member's GPU, and the CTA that owns it commits the member
+// (locality 3's key with no GPU masked), grid_min gives every CTA the member's GPU, and the CTA that owns it commits the member
 // tentatively to its live share, the occupancy and a PLACED record.  A member with no GPU aborts the gang: every CTA takes back the
 // tentative members on its own nodes (gangfew_undo), and CTA 0 reports the members after the failing one GANG_ABORTED.  An unknown or
 // dead profile fails without a barrier: gangfew_undo only touches records on the CTA's own nodes, which that CTA wrote itself.
-// kMin (k_ganglocal<true>, M3): a member with no GPU at rank >= min_m keeps the tentative members, which then commit.
+// kMin (k_ganglocal<kLocPerGang, true>, M3): a member with no GPU at rank >= min_m keeps the tentative members, which then commit.
 template <bool kMin = false>
 __device__ __forceinline__ void ganglocal_any(const GangNodeArgs& a, const DevProfiles& prof, const NodeShare& sh, uint32_t r0, uint32_t r1,
                                               uint32_t& parity, uint32_t& placed, uint32_t& dead, uint32_t* s_warp, uint32_t* s_win,
@@ -3030,24 +2994,40 @@ __device__ __forceinline__ void ganglocal_any(const GangNodeArgs& a, const DevPr
             return;
         }
         const uint32_t pos = (win & 0xFFFFFFu) - base;
-        if (pos < cnt && tid == 0) {                        // the owner commits the member tentatively
-            const uint32_t t = a.gtab[a.lo + base + pos] & (kMaxTables - 1), row = (t * ISL_MAX_PROFILES + p) * 256, o = sh.live[pos];
-            const uint32_t start = __ldg(a.lut + row + o), size = __ldg(a.sizes + t * ISL_MAX_PROFILES + p);
-            const uint32_t o2 = o | slice_span(start, size);
-            sh.live[pos] = (uint8_t)o2;
-            a.occ[a.lo + base + pos] = (uint8_t)o2;
-            a.out[r] = pack_result(flip_gpu(a.lo + base + pos, prof.flip), start, size, ISL_ST_PLACED);
-        }
+        if (pos < cnt && tid == 0) commit_member(a, prof, sh, r, p, pos);     // the owner commits the member tentatively
         __syncthreads();                                    // the commit is in the live share before the next member's scan
         ++rank;
     }
     if (blockIdx.x == 0) placed += rank;                    // the gang commits: CTA 0 counts its members once
 }
 
-// k_ganglocal<true>: every isl_place_gangs call on an ISL_FLAG_GANG_MIN_MEMBERS engine (DESIGN.md 4.13), whatever its locality flag: the
-// host writes the engine's locality into every gang's byte (or the gang's own under ISL_FLAG_GANG_LOCALITY), and each gang's effective
-// minimum m' (M1) as a uint32 right after the bytes, rounded up to 4.  Every CTA reads them alike, so the barriers stay grid-uniform.
-template <bool kMin>
+// ---------------------------------------------------------------------------------------------
+// k_ganglocal: isl_place_gangs on an engine created with a gang-topology flag (DESIGN.md 4.9-4.13).  One cooperative launch per call
+// behind k_prepare (frees and default records).  CTA c owns the partition's nodes [cta_node[c], cta_node[c + 1]) (whole nodes, balanced
+// by GPU count on the host) and keeps their occupancy bytes and a second byte per GPU in shared memory, or in global memory when a share
+// is too large for it (NodeShare).  The gangs run in array order, each on the occupancy the earlier ones left.  kLoc is every gang's
+// locality, or kLocPerGang for each gang's own byte:
+//   ISL_GANG_ONE_NODE        gangnode_gang<false>   ISL_FLAG_GANG_ONE_NODE (4.9): every member on one node
+//   ISL_GANG_FEW_NODES       gangnode_gang<true>    ISL_FLAG_GANG_FEW_NODES (4.11): one node when one takes the gang, else few nodes
+//   ISL_GANG_DISTINCT_NODES  gangspread_gang        ISL_FLAG_GANG_DISTINCT_NODES (4.10): every member on a different node
+//   kLocPerGang              locality[gi]           ISL_FLAG_GANG_LOCALITY (4.12): the byte of gang gi (checked on the host) is 1, 2 or 3
+//                                                   as above or 0, ganglocal_any: rules 2-4, member by member over the whole share
+// kMin (kLocPerGang only): every call on an ISL_FLAG_GANG_MIN_MEMBERS engine (4.13), whatever its locality flag.  The host writes the
+// engine's locality into every gang's byte (or the gang's own under ISL_FLAG_GANG_LOCALITY), and each gang's effective minimum m' (M1)
+// as a uint32 right after the bytes, rounded up to 4; a gang that fails at ALLOC member f >= m' commits its first f members (M3).
+// With a constant kLoc the compiler drops the other branches and their shared words.
+// Every barrier depends only on the gang offsets, the locality bytes, the minima and the winning keys, which every CTA reads alike, so
+// every branch is grid-uniform.  The scratch copies of localities 1 and 2 overwrite the aux bytes, so the distinct-node tags count
+// locality-3 gangs and restart at 1, which clears the marks, after every locality-1 or -2 gang, whose scratch copies may equal any tag;
+// on their own the tags run 1..255 and the marks are cleared once every 255 gangs.  The dead-profile mask is shared by localities 0 and
+// 3: a bit is set only when a gang's first ALLOC member finds no GPU, on a state without tentative slices; after k_prepare's FREEs the
+// occupancy only grows and an abort restores it exactly, so the bit stays valid.  Every record has one writer: the CTA that owns a GPU
+// writes the PLACED records on it and rewrites its own tentative ones GANG_ABORTED when the gang aborts (gangfew_undo); CTA 0 writes
+// GANG_ABORTED or GANG_TRIMMED for the other members, except the one that stopped the gang, which keeps k_prepare's NO_CAPACITY or
+// BAD_PROFILE record.
+// ---------------------------------------------------------------------------------------------
+constexpr uint32_t kLocPerGang = 4;
+template <uint32_t kLoc, bool kMin = false>
 __global__ void __launch_bounds__(kGnThreads, 1) k_ganglocal(GangNodeArgs a, DevProfiles prof, uint2* wins, const uint8_t* __restrict__ locality) {
     extern __shared__ __align__(16) uint8_t gl_smem[];
     __shared__ unsigned long long s_warp64[kGnThreads / 32];
@@ -3059,7 +3039,7 @@ __global__ void __launch_bounds__(kGnThreads, 1) k_ganglocal(GangNodeArgs a, Dev
     if (tid == 0) s_nwins = 0;
     uint32_t parity = 0, placed = 0, dead = 0, spread = 0;  // spread: locality-3 gangs since the marks were last cleared
     for (uint32_t gi = 0; gi < a.n_gangs; ++gi) {
-        const uint32_t r0 = __ldg(a.gang_off + gi), r1 = __ldg(a.gang_off + gi + 1), loc = __ldg(locality + gi);
+        const uint32_t r0 = __ldg(a.gang_off + gi), r1 = __ldg(a.gang_off + gi + 1), loc = kLoc == kLocPerGang ? __ldg(locality + gi) : kLoc;
         const uint32_t min_m = kMin ? __ldg(reinterpret_cast<const uint32_t*>(locality + ((a.n_gangs + 3u) & ~3u)) + gi) : 0u;
         if (loc == ISL_GANG_ONE_NODE || loc == ISL_GANG_FEW_NODES) {
             if (loc == ISL_GANG_ONE_NODE)

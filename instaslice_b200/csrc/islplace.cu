@@ -24,6 +24,34 @@ using namespace isl;
 static constexpr uint32_t kMaxStreamChunks = 4096;
 static constexpr uint32_t kSpecRingIds = 1u << 24;     // stream ids of isl_place_stream_partitioned that may speculate
 
+// Engines created with one of these flags place gangs with k_ganglocal, the others with k_bestfit's gang loop.
+constexpr uint32_t kGangTopologyFlags = ISL_FLAG_GANG_ONE_NODE | ISL_FLAG_GANG_FEW_NODES | ISL_FLAG_GANG_DISTINCT_NODES |
+                                        ISL_FLAG_GANG_LOCALITY | ISL_FLAG_GANG_MIN_MEMBERS;
+
+// The instantiations of k_ganglocal, one per kind of gang-topology engine (gang_kind), with the name a launch error carries; wins:
+// distinct-node gangs may run, which stack their wins in GangNode::wins.
+struct GangKernel {
+    const void* fn;
+    const char* name;
+    bool wins;
+};
+constexpr uint32_t kGangKinds = 5;
+const GangKernel kGangKernels[kGangKinds] = {
+    {(const void*)k_ganglocal<ISL_GANG_ONE_NODE>, "k_ganglocal<one_node>", false},
+    {(const void*)k_ganglocal<ISL_GANG_FEW_NODES>, "k_ganglocal<few_nodes>", false},
+    {(const void*)k_ganglocal<ISL_GANG_DISTINCT_NODES>, "k_ganglocal<distinct_nodes>", true},
+    {(const void*)k_ganglocal<kLocPerGang, false>, "k_ganglocal<per_gang>", true},
+    {(const void*)k_ganglocal<kLocPerGang, true>, "k_ganglocal<per_gang, min_members>", true},
+};
+
+// The kGangKernels entry of an engine with a gang-topology flag: each gang's own byte under ISL_FLAG_GANG_LOCALITY, and under
+// ISL_FLAG_GANG_MIN_MEMBERS with its minimum as well, else the locality of the engine's flag for every gang.
+uint32_t gang_kind(uint32_t flags) {
+    if (flags & ISL_FLAG_GANG_MIN_MEMBERS) return 4;
+    if (flags & ISL_FLAG_GANG_LOCALITY) return 3;
+    return (flags & ISL_FLAG_GANG_ONE_NODE) ? 0 : (flags & ISL_FLAG_GANG_FEW_NODES) ? 1 : 2;
+}
+
 // What plan_pipeline decides for one k_pipeline launch: GPUs per stage (seg), stages, GPUs per sub-segment, speculative rounds.
 struct PipePlan {
     uint32_t seg = 0, n_seg = 0, sub = 0;
@@ -181,18 +209,16 @@ struct isl_engine {
         DevMem<uint32_t> node_off, tree, fit, nodes;
         uint8_t width[kMaxTables] = {};
     } nf;
-    // one-node, few-node and distinct-node gangs and per-gang locality (ISL_FLAG_GANG_ONE_NODE, k_gangnode<false>; ISL_FLAG_GANG_FEW_NODES,
-    // k_gangnode<true>; ISL_FLAG_GANG_DISTINCT_NODES, k_gangspread; ISL_FLAG_GANG_LOCALITY, k_ganglocal): the inventory's
-    // node offsets in storage order (host and device, isl_load_inventory), the scratch copies (k_gangnode) or node-used marks
-    // (k_gangspread) when the shares do not fit in shared memory, the per-CTA minima, and k_gangspread's per-CTA stacks of wins
+    // gang topology (kGangTopologyFlags, k_ganglocal): the inventory's node offsets in storage order (host and device,
+    // isl_load_inventory), the scratch copies or node-used marks when the shares do not fit in shared memory, the per-CTA minima, and
+    // the per-CTA stacks of wins of distinct-node gangs
     struct GangNode {
         std::vector<uint32_t> off;
         DevMem<uint32_t> node_off;
         DevMem<uint8_t> scratch;
         DevMem<unsigned long long> keys;
         DevMem<uint2> wins;
-        int smem_optin = 0;          // dynamic shared memory one CTA of k_gangnode or k_gangspread may have
-        int local_optin = 0;         // the same for k_ganglocal, whose static shared memory is its own
+        int optin[kGangKinds] = {};  // dynamic shared memory one CTA of each kGangKernels instantiation may have
     } gn;
     unsigned long long wait_ns = 20000000000ull;   // a starved device-side wait traps after this long (ISL_WAIT_SECONDS overrides the 20 s)
     uint32_t window = 0;             // causal window of stream calls (isl_set_causal_window): chunk c starts after chunk c - window is committed
@@ -296,7 +322,7 @@ int check_launch(isl_engine* e, const char* what) {
     return ISL_OK;
 }
 
-// One cooperative launch (k_preempt, k_gangnode, k_gangspread): ISL_ECUDA, with the kernel's name, when it does not start.
+// One cooperative launch (k_preempt, k_ganglocal): ISL_ECUDA, with the kernel's name, when it does not start.
 int launch_cooperative(isl_engine* e, const void* kernel, const char* name, uint32_t grid, uint32_t threads, size_t smem, void** params) {
     const cudaError_t err = cudaLaunchCooperativeKernel(kernel, dim3(grid), dim3(threads), params, smem, e->stream);
     if (err != cudaSuccess) { cudaGetLastError(); snprintf(e->cuda_err, sizeof(e->cuda_err), "%s: %s", name, cudaGetErrorString(err)); return ISL_ECUDA; }
@@ -447,10 +473,10 @@ int run_gangs(isl_engine* e, uint32_t n_gangs, const uint32_t* d_gang_off, uint3
     return ISL_OK;
 }
 
-// The layout k_gangnode, k_gangspread and k_ganglocal share, over the nodes the partition touches: each CTA gets whole nodes, about
-// Gr / grid GPUs (one CTA per SM at most, one per 512 GPUs below that, never more than nodes), and 2 bytes per GPU of its share in shared
-// memory when they fit in `smem_optin` (the kernel's dynamic shared memory opt-in), else in global memory (gn.scratch).  Fills every
-// field of `a`; *nodes = the nodes the partition touches.
+// The layout of k_ganglocal, over the nodes the partition touches: each CTA gets whole nodes, about Gr / grid GPUs (one CTA per SM at most,
+// one per 512 GPUs below that, never more than nodes), and 2 bytes per GPU of its share in shared memory when they fit in `smem_optin` (the
+// kernel's dynamic shared memory opt-in), else in global memory (gn.scratch).  Fills every field of `a`; *nodes = the nodes the partition
+// touches.
 int gang_layout(isl_engine* e, const void* kernel, int smem_optin, uint32_t n_gangs, const uint32_t* d_gang_off, const uint2* d_in, uint2* d_out,
                 GangNodeArgs& a, uint32_t* grid_out, size_t* smem_out, uint32_t* nodes) {
     auto& gn = e->gn;
@@ -484,64 +510,23 @@ int gang_layout(isl_engine* e, const void* kernel, int smem_optin, uint32_t n_ga
     return ISL_OK;
 }
 
-// isl_place_gangs on an ISL_FLAG_GANG_ONE_NODE engine: frees + defaults, then one cooperative k_gangnode (gang_layout).
-int run_gangnode(isl_engine* e, uint32_t n_gangs, const uint32_t* d_gang_off, uint32_t n, const uint2* d_in, uint2* d_out) {
+// isl_place_gangs on an engine with a gang-topology flag: frees + defaults, then one cooperative launch of kGangKernels[kind]
+// (gang_layout with the instantiation's own opt-in).  Under ISL_FLAG_GANG_LOCALITY or ISL_FLAG_GANG_MIN_MEMBERS it places each gang by
+// the byte at d_locality[gang], and under ISL_FLAG_GANG_MIN_MEMBERS it reads each gang's minimum m' from the uint32 words that follow
+// the bytes (rounded up to 4).  CTA c of an instantiation that runs distinct-node gangs stacks its wins in gn.wins[cta_node[c] ..), at
+// most one per node it owns.
+int run_ganglocal(isl_engine* e, uint32_t kind, uint32_t n_gangs, const uint32_t* d_gang_off, const uint8_t* d_locality, uint32_t n,
+                  const uint2* d_in, uint2* d_out) {
+    const GangKernel& k = kGangKernels[kind];
     if (int rc = prepare_batch(e, n, d_in, d_out)) return rc;
     GangNodeArgs a;
     uint32_t grid, nodes;
     size_t smem;
-    if (int rc = gang_layout(e, (const void*)k_gangnode<false>, e->gn.smem_optin, n_gangs, d_gang_off, d_in, d_out, a, &grid, &smem, &nodes)) return rc;
-    void* params[] = {&a, &e->prof};
-    if (int rc = launch_cooperative(e, (const void*)k_gangnode<false>, "k_gangnode", grid, kGnThreads, smem, params)) return rc;
-    finish_batch(e, n, true);
-    return ISL_OK;
-}
-
-// isl_place_gangs on an ISL_FLAG_GANG_FEW_NODES engine: frees + defaults, then one cooperative k_gangnode<true> (gang_layout), which
-// places each gang in rounds, one node per round.
-int run_gangfew(isl_engine* e, uint32_t n_gangs, const uint32_t* d_gang_off, uint32_t n, const uint2* d_in, uint2* d_out) {
-    if (int rc = prepare_batch(e, n, d_in, d_out)) return rc;
-    GangNodeArgs a;
-    uint32_t grid, nodes;
-    size_t smem;
-    if (int rc = gang_layout(e, (const void*)k_gangnode<true>, e->gn.smem_optin, n_gangs, d_gang_off, d_in, d_out, a, &grid, &smem, &nodes)) return rc;
-    void* params[] = {&a, &e->prof};
-    if (int rc = launch_cooperative(e, (const void*)k_gangnode<true>, "k_gangnode<true>", grid, kGnThreads, smem, params)) return rc;
-    finish_batch(e, n, true);
-    return ISL_OK;
-}
-
-// isl_place_gangs on an ISL_FLAG_GANG_DISTINCT_NODES engine: frees + defaults, then one cooperative k_gangspread (gang_layout); CTA c
-// stacks its wins in gn.wins[cta_node[c] ..), at most one per node it owns.
-int run_gangspread(isl_engine* e, uint32_t n_gangs, const uint32_t* d_gang_off, uint32_t n, const uint2* d_in, uint2* d_out) {
-    if (int rc = prepare_batch(e, n, d_in, d_out)) return rc;
-    GangNodeArgs a;
-    uint32_t grid, nodes;
-    size_t smem;
-    if (int rc = gang_layout(e, (const void*)k_gangspread, e->gn.smem_optin, n_gangs, d_gang_off, d_in, d_out, a, &grid, &smem, &nodes)) return rc;
-    ISL_CUDA(e, e->gn.wins.reserve(nodes));
-    uint2* wins = e->gn.wins;
-    void* params[] = {&a, &e->prof, &wins};
-    if (int rc = launch_cooperative(e, (const void*)k_gangspread, "k_gangspread", grid, kGnThreads, smem, params)) return rc;
-    finish_batch(e, n, true);
-    return ISL_OK;
-}
-
-// isl_place_gangs on an ISL_FLAG_GANG_LOCALITY or ISL_FLAG_GANG_MIN_MEMBERS engine: frees + defaults, then one cooperative k_ganglocal
-// (gang_layout with its own opt-in), which places each gang by the locality byte at d_locality[gang]; wins as in run_gangspread.
-// elastic: k_ganglocal<true>, which reads each gang's minimum m' from the uint32 words that follow the bytes (rounded up to 4).
-int run_ganglocal(isl_engine* e, uint32_t n_gangs, const uint32_t* d_gang_off, const uint8_t* d_locality, uint32_t n, const uint2* d_in,
-                  uint2* d_out, bool elastic) {
-    if (int rc = prepare_batch(e, n, d_in, d_out)) return rc;
-    const void* kernel = elastic ? (const void*)k_ganglocal<true> : (const void*)k_ganglocal<false>;
-    GangNodeArgs a;
-    uint32_t grid, nodes;
-    size_t smem;
-    if (int rc = gang_layout(e, kernel, e->gn.local_optin, n_gangs, d_gang_off, d_in, d_out, a, &grid, &smem, &nodes)) return rc;
-    ISL_CUDA(e, e->gn.wins.reserve(nodes));
+    if (int rc = gang_layout(e, k.fn, e->gn.optin[kind], n_gangs, d_gang_off, d_in, d_out, a, &grid, &smem, &nodes)) return rc;
+    if (k.wins) ISL_CUDA(e, e->gn.wins.reserve(nodes));
     uint2* wins = e->gn.wins;
     void* params[] = {&a, &e->prof, &wins, &d_locality};
-    if (int rc = launch_cooperative(e, kernel, elastic ? "k_ganglocal<true>" : "k_ganglocal", grid, kGnThreads, smem, params)) return rc;
+    if (int rc = launch_cooperative(e, k.fn, k.name, grid, kGnThreads, smem, params)) return rc;
     finish_batch(e, n, true);
     return ISL_OK;
 }
@@ -1213,8 +1198,8 @@ int isl_create(const isl_config* cfg, isl_engine** out) {
         cudaFuncAttributes fa;
         const void* kernels[] = {(const void*)k_prepare, (const void*)k_partition, (const void*)k_set_flag, (const void*)k_few, (const void*)k_build_lut, (const void*)k_eval_starts,
                                  (const void*)k_free_spans, (const void*)k_capacity, (const void*)k_sweep_count, (const void*)k_sweep_scatter, (const void*)k_commit, (const void*)k_bestfit<false>, (const void*)k_bestfit<true>,
-                                 (const void*)k_bestfit<false, true>, (const void*)k_bestfit<true, true>, (const void*)k_victim_map, (const void*)k_preempt, (const void*)k_nodefit, (const void*)k_gangnode<false>, (const void*)k_gangnode<true>, (const void*)k_gangspread,
-                                 (const void*)k_ganglocal<false>, (const void*)k_ganglocal<true>, (const void*)k_chain<1>, (const void*)k_chain<2>, (const void*)k_chain<4>, (const void*)k_small<1>, (const void*)k_small<2>, (const void*)k_small<4>};
+                                 (const void*)k_bestfit<false, true>, (const void*)k_bestfit<true, true>, (const void*)k_victim_map, (const void*)k_preempt, (const void*)k_nodefit,
+                                 (const void*)k_chain<1>, (const void*)k_chain<2>, (const void*)k_chain<4>, (const void*)k_small<1>, (const void*)k_small<2>, (const void*)k_small<4>};
         const void* pipes[] = {(const void*)k_pipeline<1, false, false>, (const void*)k_pipeline<1, true, false>, (const void*)k_pipeline<2, false, false>, (const void*)k_pipeline<2, true, false>,
                                (const void*)k_pipeline<4, false, false>, (const void*)k_pipeline<4, true, false>,
                                (const void*)k_pipeline<1, false, true>, (const void*)k_pipeline<1, true, true>, (const void*)k_pipeline<2, false, true>, (const void*)k_pipeline<2, true, true>,
@@ -1234,19 +1219,13 @@ int isl_create(const isl_config* cfg, isl_engine** out) {
         ISL_TRY(cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev));
         ISL_TRY(cudaFuncGetAttributes(&fa, k_preempt));
         ISL_TRY(cudaFuncSetAttribute((const void*)k_preempt, cudaFuncAttributeMaxDynamicSharedMemorySize, optin - (int)fa.sharedSizeBytes));
-        // the gang-topology kernels share one sizing: the largest static share
-        const void* gangs[] = {(const void*)k_gangnode<false>, (const void*)k_gangnode<true>, (const void*)k_gangspread};
-        size_t gang_static = 0;
-        for (const void* k : gangs) { ISL_TRY(cudaFuncGetAttributes(&fa, k)); gang_static = std::max(gang_static, fa.sharedSizeBytes); }
-        e->gn.smem_optin = optin - (int)gang_static;
-        for (const void* k : gangs) ISL_TRY(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, e->gn.smem_optin));
-        // k_ganglocal sizes its shares by its own static shared memory, so the switch of the three above does not move with it; both
-        // instantiations declare the same static words
-        const void* locals[] = {(const void*)k_ganglocal<false>, (const void*)k_ganglocal<true>};
-        size_t local_static = 0;
-        for (const void* k : locals) { ISL_TRY(cudaFuncGetAttributes(&fa, k)); local_static = std::max(local_static, fa.sharedSizeBytes); }
-        e->gn.local_optin = optin - (int)local_static;
-        for (const void* k : locals) ISL_TRY(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, e->gn.local_optin));
+        // each k_ganglocal instantiation (loaded here as well): its shares may have what the device lets one CTA have beside the
+        // instantiation's own static words
+        for (uint32_t i = 0; i < kGangKinds; ++i) {
+            ISL_TRY(cudaFuncGetAttributes(&fa, kGangKernels[i].fn));
+            e->gn.optin[i] = optin - (int)fa.sharedSizeBytes;
+            ISL_TRY(cudaFuncSetAttribute(kGangKernels[i].fn, cudaFuncAttributeMaxDynamicSharedMemorySize, e->gn.optin[i]));
+        }
     }
     e->occ_bytes = ((size_t)cfg->max_gpus + kSweepBlock - 1) / kSweepBlock * kSweepBlock;
     const uint32_t max_tiles = ceil_div(cfg->max_batch, kTile) + 4096;   // + one partial tile per batch of a stream
@@ -1457,9 +1436,8 @@ int isl_load_inventory(isl_engine* e, uint32_t n_nodes, const uint32_t* node_off
         ISL_CUDA(e, e->nf.node_off.replace((size_t)n_nodes + 1));
         ISL_CUDA(e, cudaMemcpyAsync(e->nf.node_off, node_off, ((size_t)n_nodes + 1) * sizeof(uint32_t), cudaMemcpyHostToDevice, e->stream));
     }
-    if (e->cfg.flags & (ISL_FLAG_GANG_ONE_NODE | ISL_FLAG_GANG_FEW_NODES | ISL_FLAG_GANG_DISTINCT_NODES | ISL_FLAG_GANG_LOCALITY |
-                        ISL_FLAG_GANG_MIN_MEMBERS)) {
-        // k_gangnode, k_gangspread and k_ganglocal walk the nodes in storage order (reversed under right-to-left)
+    if (e->cfg.flags & kGangTopologyFlags) {
+        // k_ganglocal walks the nodes in storage order (reversed under right-to-left)
         auto& off = e->gn.off;
         off.assign(node_off, node_off + n_nodes + 1);
         if (e->prof.flip) { std::reverse(off.begin(), off.end()); for (auto& x : off) x = G - x; }
@@ -1558,9 +1536,8 @@ int isl_place_gangs(isl_engine* e, uint32_t n_gangs, const uint32_t* gang_off, c
             }
         }
     }
-    const bool elastic = e->cfg.flags & ISL_FLAG_GANG_MIN_MEMBERS;
     std::vector<uint32_t> min_members;                              // ISL_FLAG_GANG_MIN_MEMBERS: each gang's m' (M1, M6), 0 without ALLOCs
-    if (elastic) {
+    if (e->cfg.flags & ISL_FLAG_GANG_MIN_MEMBERS) {
         const uint8_t loc = (e->cfg.flags & ISL_FLAG_GANG_ONE_NODE)         ? (uint8_t)ISL_GANG_ONE_NODE
                             : (e->cfg.flags & ISL_FLAG_GANG_FEW_NODES)      ? (uint8_t)ISL_GANG_FEW_NODES
                             : (e->cfg.flags & ISL_FLAG_GANG_DISTINCT_NODES) ? (uint8_t)ISL_GANG_DISTINCT_NODES
@@ -1596,12 +1573,9 @@ int isl_place_gangs(isl_engine* e, uint32_t n_gangs, const uint32_t* gang_off, c
         ISL_CUDA(e, cudaMemcpyAsync((uint8_t*)e->d_scratch.get() + min_at, min_members.data(), min_members.size() * sizeof(uint32_t),
                                     cudaMemcpyHostToDevice, e->stream));
     ISL_CUDA(e, cudaMemcpyAsync(e->d_req, in, (size_t)n * sizeof(isl_request), cudaMemcpyHostToDevice, e->stream));
-    if (int rc = (e->cfg.flags & (ISL_FLAG_GANG_LOCALITY | ISL_FLAG_GANG_MIN_MEMBERS))
-                                                                 ? run_ganglocal(e, n_gangs, d_gang_off, d_locality, n, e->d_req, e->d_res, elastic)
-                 : (e->cfg.flags & ISL_FLAG_GANG_ONE_NODE)        ? run_gangnode(e, n_gangs, d_gang_off, n, e->d_req, e->d_res)
-                 : (e->cfg.flags & ISL_FLAG_GANG_FEW_NODES)      ? run_gangfew(e, n_gangs, d_gang_off, n, e->d_req, e->d_res)
-                 : (e->cfg.flags & ISL_FLAG_GANG_DISTINCT_NODES) ? run_gangspread(e, n_gangs, d_gang_off, n, e->d_req, e->d_res)
-                                                                 : run_gangs(e, n_gangs, d_gang_off, n, e->d_req, e->d_res)) return rc;
+    if (int rc = (e->cfg.flags & kGangTopologyFlags)
+                     ? run_ganglocal(e, gang_kind(e->cfg.flags), n_gangs, d_gang_off, d_locality, n, e->d_req, e->d_res)
+                     : run_gangs(e, n_gangs, d_gang_off, n, e->d_req, e->d_res)) return rc;
     ISL_CUDA(e, cudaMemcpyAsync(out, e->d_res, (size_t)n * sizeof(isl_result), cudaMemcpyDeviceToHost, e->stream));
     ISL_CUDA(e, cudaStreamSynchronize(e->stream));
     return ISL_OK;

@@ -1,11 +1,11 @@
 // gang_few_fast.cpp — brute-force restatement of isl_place_gangs on an ISL_FLAG_GANG_FEW_NODES engine (include/islplace.h, rules F1-F6)
 // on flat occupancy bytes.
 //
-// TEST INFRASTRUCTURE: the large-scale checker of k_gangnode<true> and the single-core CPU baseline of tools/gang_few_time.py.  Every FREE
-// of the call is applied first; then, gang after gang, round after round, every node of the range is simulated in scan order on a copy of
-// its bytes, resolving the remaining ALLOC members one by one, each scoring every GPU of the node that admits it.  The node that places
-// the most leading members (the first in scan order on a tie) keeps its copy; a round in which no node places one aborts the gang and
-// drops every copy kept so far.  It shares nothing with the kernel but the rules.
+// TEST INFRASTRUCTURE: the large-scale checker of k_ganglocal<few_nodes> and the single-core CPU baseline of tools/gang_few_time.py.  Every
+// FREE of the call is applied first; then, gang after gang, round after round, every node of the range is simulated in scan order on a copy
+// of its bytes, resolving the remaining ALLOC members one by one, each scoring every GPU of the node that admits it.  The node that places
+// the most leading members (the first in scan order on a tie) keeps its copy; a round in which no node places one aborts the gang and drops
+// every copy kept so far.  It shares nothing with the kernel but the rules.
 #include <algorithm>
 #include <cstdint>
 #include <cstring>

@@ -1,11 +1,12 @@
 // gang_min_fast.cpp — brute-force restatement of isl_place_gangs on an ISL_FLAG_GANG_MIN_MEMBERS engine (include/islplace.h, rules
 // M1-M7) on flat occupancy bytes, for all four localities.
 //
-// TEST INFRASTRUCTURE: the large-scale checker of k_ganglocal<true> and the single-core CPU baseline of tools/gang_min_time.py.  Every FREE
-// of the call is applied first; then, gang after gang, the gang's locality is run on a copy of the occupancy until it commits or stops
-// at ALLOC member f: 0 member by member over every GPU of the range, 1 every node in scan order with the first deepest node kept, 2 rounds
-// of that, 3 member by member over the GPUs of nodes the gang does not use yet.  A gang that commits, or stops at f >= m', keeps the copy
-// and its first f records; any other gang drops it.  It shares nothing with the kernel or with the other brute forces but the rules.
+// TEST INFRASTRUCTURE: the large-scale checker of k_ganglocal<per_gang, min_members> and the single-core CPU baseline of
+// tools/gang_min_time.py.  Every FREE of the call is applied first; then, gang after gang, the gang's locality is run on a copy of the
+// occupancy until it commits or stops at ALLOC member f: 0 member by member over every GPU of the range, 1 every node in scan order with
+// the first deepest node kept, 2 rounds of that, 3 member by member over the GPUs of nodes the gang does not use yet.  A gang that commits,
+// or stops at f >= m', keeps the copy and its first f records; any other gang drops it.  It shares nothing with the kernel or with the
+// other brute forces but the rules.
 #include <algorithm>
 #include <cstdint>
 #include <cstring>

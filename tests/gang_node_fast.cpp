@@ -1,10 +1,10 @@
 // gang_node_fast.cpp — brute-force restatement of isl_place_gangs on an ISL_FLAG_GANG_ONE_NODE engine (include/islplace.h, rules G1-G6)
 // on flat occupancy bytes.
 //
-// TEST INFRASTRUCTURE: the large-scale checker of k_gangnode and the single-core CPU baseline of tools/gang_node_time.py.  Every FREE of
-// the call is applied first; then, gang after gang, every node of the range is tried in scan order by resolving the gang's ALLOC members
-// one by one on a copy of the node's bytes, each member scoring every GPU of the node that admits it.  The first node that takes every
-// member is committed; without one, the deepest failure decides the record.  It shares nothing with the kernel but the rules.
+// TEST INFRASTRUCTURE: the large-scale checker of k_ganglocal<one_node> and the single-core CPU baseline of tools/gang_node_time.py.  Every
+// FREE of the call is applied first; then, gang after gang, every node of the range is tried in scan order by resolving the gang's ALLOC
+// members one by one on a copy of the node's bytes, each member scoring every GPU of the node that admits it.  The first node that takes
+// every member is committed; without one, the deepest failure decides the record.  It shares nothing with the kernel but the rules.
 #include <algorithm>
 #include <cstdint>
 #include <cstring>

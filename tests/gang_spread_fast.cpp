@@ -1,10 +1,11 @@
 // gang_spread_fast.cpp — brute-force restatement of isl_place_gangs on an ISL_FLAG_GANG_DISTINCT_NODES engine (include/islplace.h, rules
 // S1-S6) on flat occupancy bytes.
 //
-// TEST INFRASTRUCTURE: the large-scale checker of k_gangspread and the single-core CPU baseline of tools/gang_spread_time.py.  Every FREE
-// of the call is applied first; then, gang after gang, the ALLOC members are resolved one by one: every GPU of the range, in scan order,
-// whose node holds no earlier member of the gang is scored, the best one is taken on a copy of the bytes, and its node is added to the
-// gang's used set.  A member with no GPU aborts the gang and the copy is dropped.  It shares nothing with the kernel but the rules.
+// TEST INFRASTRUCTURE: the large-scale checker of k_ganglocal<distinct_nodes> and the single-core CPU baseline of
+// tools/gang_spread_time.py.  Every FREE of the call is applied first; then, gang after gang, the ALLOC members are resolved one by one:
+// every GPU of the range, in scan order, whose node holds no earlier member of the gang is scored, the best one is taken on a copy of the
+// bytes, and its node is added to the gang's used set.  A member with no GPU aborts the gang and the copy is dropped.  It shares nothing
+// with the kernel but the rules.
 #include <algorithm>
 #include <cstdint>
 #include <cstring>

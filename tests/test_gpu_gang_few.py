@@ -1,6 +1,6 @@
-"""Few-node gangs (isl_place_gangs on an engine created with ISL_FLAG_GANG_FEW_NODES) on the H100: k_gangnode<true> against the brute
-force of tests/gang_few_fast.cpp, records and final occupancy byte-identical, plus the hand-worked vectors, the identities and refusals
-of include/islplace.h (F1-F6), the limits of the profile-table ABI and of the CTA layout, the reconciler flow and the C++ host mirror."""
+"""Few-node gangs (isl_place_gangs on an engine created with ISL_FLAG_GANG_FEW_NODES) on the H100: k_ganglocal<few_nodes> against the brute
+force of tests/gang_few_fast.cpp, records and final occupancy byte-identical, plus the hand-worked vectors, the identities and refusals of
+include/islplace.h (F1-F6), the limits of the profile-table ABI and of the CTA layout, the reconciler flow and the C++ host mirror."""
 import ctypes
 import os
 import subprocess

@@ -1,7 +1,7 @@
-"""Node locality per gang (isl_place_gangs on an engine created with ISL_FLAG_GANG_LOCALITY) on the H100: k_ganglocal against composition
-(i) of tests/gang_locality_oracle.py (each run of gangs on the brute force of its locality), records, final occupancy and stats.placed
-byte-identical, plus the hand-worked vectors, L3 (a) and (b) device against device, the marks and dead-profile hazards, the L4 / L5
-refusals, the isl_place_gangs codes in every engine state, the reconciler flow and the C++ host mirror."""
+"""Node locality per gang (isl_place_gangs on an engine created with ISL_FLAG_GANG_LOCALITY) on the H100: k_ganglocal<per_gang> against
+composition (i) of tests/gang_locality_oracle.py (each run of gangs on the brute force of its locality), records, final occupancy and
+stats.placed byte-identical, plus the hand-worked vectors, L3 (a) and (b) device against device, the marks and dead-profile hazards, the
+L4 / L5 refusals, the isl_place_gangs codes in every engine state, the reconciler flow and the C++ host mirror."""
 import ctypes
 import os
 import subprocess
@@ -180,8 +180,8 @@ def test_2_20_gpus(policy):
 
 @pytest.mark.parametrize("case", LAYOUT_CASES)
 def test_layout_edges(case):
-    """Every edge of the CTA layout built from this device's SM count and k_ganglocal's own shared-memory opt-in (its 256 B of static
-    shared memory), shares on both sides of the shared / global memory switch among them."""
+    """Every edge of the CTA layout built from this device's SM count and k_ganglocal<per_gang>'s own shared-memory opt-in (its 256 B of
+    static shared memory), shares on both sides of the shared / global memory switch among them."""
     sms, optin = device()
     node_off, lo, hi, edge = layout_cases(sms, optin)[case]
     assert edge(gang_plan(node_off, lo, hi, sms, optin - 256)), case

@@ -1,8 +1,8 @@
-"""Elastic gangs (isl_place_gangs on an engine created with ISL_FLAG_GANG_MIN_MEMBERS) on the H100: k_ganglocal<true> against the direct
-brute force tests/gang_min_fast.cpp, records, final occupancy and stats.placed byte-identical, under every policy, both quirk sets and
-every gang flag (none, one node, few nodes, distinct nodes, locality per gang); the hand-worked vectors; M5 (a), (b) and (d) device
-against device; the M6 refusals and the isl_place_gangs codes in every engine state; the table, inventory and layout limits; a gang of
-300 members trimmed past its 256th; the reconciler flow and the C++ host mirror."""
+"""Elastic gangs (isl_place_gangs on an engine created with ISL_FLAG_GANG_MIN_MEMBERS) on the H100: k_ganglocal<per_gang, min_members>
+against the direct brute force tests/gang_min_fast.cpp, records, final occupancy and stats.placed byte-identical, under every policy, both
+quirk sets and every gang flag (none, one node, few nodes, distinct nodes, locality per gang); the hand-worked vectors; M5 (a), (b) and (d)
+device against device; the M6 refusals and the isl_place_gangs codes in every engine state; the table, inventory and layout limits; a gang
+of 300 members trimmed past its 256th; the reconciler flow and the C++ host mirror."""
 import ctypes
 import os
 import subprocess
@@ -259,8 +259,8 @@ def test_2_20_gpus(policy):
 
 @pytest.mark.parametrize("case", LAYOUT_CASES)
 def test_layout_edges(case):
-    """Every edge of the CTA layout built from this device's SM count and k_ganglocal's shared-memory opt-in, shares on both sides of the
-    shared / global memory switch among them, on an engine without a locality flag (every gang through locality 0)."""
+    """Every edge of the CTA layout built from this device's SM count and k_ganglocal<per_gang, min_members>'s shared-memory opt-in, shares
+    on both sides of the shared / global memory switch among them, on an engine without a locality flag (every gang through locality 0)."""
     sms, optin = device()
     node_off, lo, hi, edge = layout_cases(sms, optin)[case]
     assert edge(gang_plan(node_off, lo, hi, sms, optin - 256)), case

@@ -1,5 +1,5 @@
-"""One-node gangs (isl_place_gangs on an engine created with ISL_FLAG_GANG_ONE_NODE) on the H100: k_gangnode against the brute force of
-tests/gang_node_fast.cpp, records and final occupancy byte-identical, plus the hand-worked vectors, the identities and refusals of
+"""One-node gangs (isl_place_gangs on an engine created with ISL_FLAG_GANG_ONE_NODE) on the H100: k_ganglocal<one_node> against the brute
+force of tests/gang_node_fast.cpp, records and final occupancy byte-identical, plus the hand-worked vectors, the identities and refusals of
 include/islplace.h (G1-G6), the reconciler flow and the C++ host mirror."""
 import ctypes
 import os

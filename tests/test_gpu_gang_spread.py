@@ -1,6 +1,6 @@
-"""Distinct-node gangs (isl_place_gangs on an engine created with ISL_FLAG_GANG_DISTINCT_NODES) on the H100: k_gangspread against the
-brute force of tests/gang_spread_fast.cpp, records and final occupancy byte-identical, plus the hand-worked vectors, the consequences and
-refusals of include/islplace.h (S1-S6), the reconciler flow and the C++ host mirror."""
+"""Distinct-node gangs (isl_place_gangs on an engine created with ISL_FLAG_GANG_DISTINCT_NODES) on the H100: k_ganglocal<distinct_nodes>
+against the brute force of tests/gang_spread_fast.cpp, records and final occupancy byte-identical, plus the hand-worked vectors, the
+consequences and refusals of include/islplace.h (S1-S6), the reconciler flow and the C++ host mirror."""
 import ctypes
 import os
 import subprocess

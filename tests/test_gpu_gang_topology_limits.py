@@ -1,12 +1,12 @@
-"""One-node gangs (k_gangnode) and distinct-node gangs (k_gangspread) at the limits of the profile-table ABI, of the inventory and of
-their shared layout (gang_layout), on the H100.  Every call is compared with its brute force (tests/gang_node_fast.cpp,
-tests/gang_spread_fast.cpp) — every record and the final occupancy — and its committed gangs are checked against the topology rule
-through isl_gpu_to_node: one node per gang, or pairwise distinct nodes.  The inputs come from ``test_oracle_gang_topology_limits.py``,
-which pins the checkers at these shapes and shows that every generator reaches its edge.
+"""One-node gangs (k_ganglocal<one_node>) and distinct-node gangs (k_ganglocal<distinct_nodes>) at the limits of the profile-table ABI, of
+the inventory and of their shared layout (gang_layout), on the H100.  Every call is compared with its brute force (tests/gang_node_fast.cpp,
+tests/gang_spread_fast.cpp) — every record and the final occupancy — and its committed gangs are checked against the topology rule through
+isl_gpu_to_node: one node per gang, or pairwise distinct nodes.  The inputs come from ``test_oracle_gang_topology_limits.py``, which pins
+the checkers at these shapes and shows that every generator reaches its edge.
 
   fixtures     T16x8, T16mix-1/2 under quirk sets 0-3, T8tab with node tables, T16top, T16straddle; every policy; 4 096 / 4 097 GPUs
                of eight-GPU nodes, whole bytes, every gang shape
-  calls        pass 0 of k_gangnode (perfect fits behind decoys, failures deepest on skipped nodes), profile 15 dead only after a failure
+  calls        one-node pass 0 (perfect fits behind decoys, failures deepest on skipped nodes), profile 15 dead only after a failure
                at rank 0, MIN_FRAG scores of 121 and on both sides of 64, more than 510 gangs (the node-used tags wrap)
   2^20 GPUs    T8tab with node tables, every policy, the lower half full but for what the call's FREEs release; under right-to-left also
                the top partition [2^20 - 4 109, 2^20), which cuts a node
@@ -96,7 +96,7 @@ def test_fixtures(kind, name, quirks, policy):
 @pytest.mark.parametrize("policy", POLICIES)
 @pytest.mark.parametrize("kind", list(KERNELS))
 def test_pass0_filter_calls(kind, policy):
-    """k_gangnode's pass 0 at its edges (free slices equal to the need, first and behind a decoy; the deepest failure on a skipped
+    """The one-node pass 0 at its edges (free slices equal to the need, first and behind a decoy; the deepest failure on a skipped
     node), T8tab with absent rows and tables 0..7; the same calls on the distinct-node engine."""
     rows = t8tab()
     rng = W.SplitMix64(600 + policy)
@@ -115,7 +115,7 @@ def test_pass0_filter_calls(kind, policy):
 @pytest.mark.parametrize("name,quirks", [("t16x8", E.QUIRKS_REF_EXACT), ("t8tab", E.QUIRKS_FIXED), ("t16top", E.QUIRKS_FIXED)])
 @pytest.mark.parametrize("kind", list(KERNELS))
 def test_profile_15_dead_only_after_rank_0(kind, name, quirks, policy):
-    """k_gangspread's dead mask: profile 15 failing behind the exclusion (rank >= 1) stays live, failing at rank 0 is dead."""
+    """The distinct-node dead mask: profile 15 failing behind the exclusion (rank >= 1) stays live, failing at rank 0 is dead."""
     rows = FIXTURES[name]()
     rng = W.SplitMix64(1500 + policy + len(name))
     node_off, node_table, occ, req, off, want = dead15_call(rng, rows, quirks)

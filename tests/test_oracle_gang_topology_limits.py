@@ -1,6 +1,6 @@
-"""One-node gangs (k_gangnode, ISL_FLAG_GANG_ONE_NODE) and distinct-node gangs (k_gangspread, ISL_FLAG_GANG_DISTINCT_NODES) at the
-limits of the ABI — the layout restatement, the generators, their self-checks and the pins of the checkers at these shapes (CPU only).
-``test_gpu_gang_topology_limits.py`` runs the same inputs through both kernels.
+"""One-node gangs (k_ganglocal<one_node>, ISL_FLAG_GANG_ONE_NODE) and distinct-node gangs (k_ganglocal<distinct_nodes>,
+ISL_FLAG_GANG_DISTINCT_NODES) at the limits of the ABI — the layout restatement, the generators, their self-checks and the pins of the
+checkers at these shapes (CPU only).  ``test_gpu_gang_topology_limits.py`` runs the same inputs through both kernels.
 
 The fixtures are those of ``test_oracle_table_limits.py`` (T16x8, T16mix-1/2, T8tab with its node tables, T16top) and one more:
   T16straddle  15 size-4 rows of 5 starts and a size-2 row (index 15): profile 15's ISL_POLICY_MIN_FRAG score is 76 on an empty GPU,
@@ -12,10 +12,10 @@ Built here:
   layout cases      a CTA that owns no node, as many nodes as the grid, a last CTA owning one one-GPU node, ceil(Gr / 512) limiting
                     the grid at 512 k and 512 k + 1 GPUs, a partition that cuts a node at both ends, one-node partitions on both sides
                     of the shared / global switch
-  pass0_call        (k_gangnode) the first node in scan order that takes a gang has exactly the free slices the gang needs; a node
+  pass0_call        (one node) the first node in scan order that takes a gang has exactly the free slices the gang needs; a node
                     before it has as many free slices but cannot take the gang
-  pass1_call        (k_gangnode) a gang's deepest failure is on a node that has fewer free slices than the gang needs
-  dead15_call       (k_gangspread) profile 15 fails at rank >= 1 behind the exclusion (and is placed by the next gang), then at rank 0
+  pass1_call        (one node) a gang's deepest failure is on a node that has fewer free slices than the gang needs
+  dead15_call       (distinct nodes) profile 15 fails at rank >= 1 behind the exclusion (and is placed by the next gang), then at rank 0
                     (and stays dead for the call)
   min_frag_call     T16top / T16straddle under ISL_POLICY_MIN_FRAG: profile 15 scores 121, or scores on both sides of 64
   wrap_call         more than 510 gangs (the node-used tags wrap twice) on nodes of 64 GPUs, profile 15 placed after each wrap

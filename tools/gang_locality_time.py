@@ -2,12 +2,12 @@
 pre-filled to about half of its slices by C3-mix pods of which every other one was released again), with 20 000 C3-mix pods cut into
 gangs of 2, 4 and 8 whose localities are drawn per gang from a seed.  Per (policy, gang size) one JSON line with:
 
-  flagged     one call on the flagged engine (k_ganglocal);
+  flagged     one call on the flagged engine (k_ganglocal<per_gang>);
   four_engines  what a caller does without the flag: four engines, one flagged for each locality (none for 0), one call per run of
               consecutive gangs of one locality, and the whole occupancy handed from each engine to the next between runs
               (isl_read_occupancy, isl_write_occupancy); host clock around the whole sequence;
-  homogeneous every gang at locality k, on the flagged engine and on k's own engine (k_bestfit's gang loop for 0, k_gangnode,
-              k_gangnode<true>, k_gangspread);
+  homogeneous every gang at locality k, on the flagged engine and on k's own engine (k_bestfit's gang loop for 0, k_ganglocal<one_node>,
+              <few_nodes>, <distinct_nodes>);
   brute force composition (i) of tests/gang_locality_oracle.py on one CPU core.
 
 Medians of --reps synchronous calls, the inventory reloaded before each.  Every line is printed only after the flagged call's records and

@@ -3,13 +3,14 @@ pre-filled to about half of its slices by C3-mix pods of which every other one w
 gangs of k = 4, 8 and 16 with minimum m = k / 2, under first-fit and best-fit, for every gang flag with MIN: none (any), one node, few
 nodes, distinct nodes and a locality per gang drawn from a seed.  Per (policy, mode, k) one JSON line with:
 
-  flagged      one call on the MIN engine (k_ganglocal<true>);
+  flagged      one call on the MIN engine (k_ganglocal<per_gang, min_members>);
   emulation    what a caller does without the flag, on the engine without MIN, host clock, run once: snapshot, place the rest of the
                call, and at the first gang that aborted at f >= m' restore, place the gangs before it and that gang cut to f in one call,
                then go on from the next gang (isl_snapshot_occupancy / isl_restore_occupancy); stopped after --emulation-s seconds, in
                which case the line holds the time so far as a lower bound;
   counts       trimmed and aborted gangs, pods placed;
-  m0           m = 0 on the MIN engine against the same call on the engine without MIN: the price of routing through k_ganglocal<true>;
+  m0           m = 0 on the MIN engine against the same call on the engine without MIN: the price of routing through
+               k_ganglocal<per_gang, min_members>;
   brute force  tests/gang_min_fast.cpp on one CPU core.
 
 Medians of --reps synchronous calls, the inventory reloaded before each.  Every line is printed only after the flagged call's records and

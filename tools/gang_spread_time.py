@@ -2,7 +2,7 @@
 to about half of its slices by C3-mix pods of which every other one was released again, as tools/gang_node_time.py does), with 20 000
 pods cut into gangs of 2, 4 and 8.  Two kinds of gang: "mix" (consecutive C3-mix pods) and "replicas" (k copies of one C3-mix profile).
 Next to it: the same call on an unflagged engine (k_bestfit, gangs packed as close as the policy puts them), on an ISL_FLAG_GANG_ONE_NODE
-engine (k_gangnode), and the brute force of tests/gang_spread_fast.cpp (one core, the CPU baseline).
+engine (k_ganglocal<one_node>), and the brute force of tests/gang_spread_fast.cpp (one core, the CPU baseline).
 
 Every line is printed only after the engine's records and final occupancy were found byte-identical to the brute force's.  One JSON
 line per (policy, kind, gang size); the card and its power limit are read in the same run.
