@@ -155,6 +155,8 @@ typedef struct isl_config {
                                         ISL_GANG_* values below (see isl_place_gangs); every other call is unchanged */
 #define ISL_FLAG_GANG_MIN_MEMBERS 1024u  /* elastic gangs: isl_place_gangs commits a gang's leading members once they reach the minimum its
                                             ALLOC members name in their `size` byte (see isl_place_gangs, M1-M7); every other call is unchanged */
+#define ISL_FLAG_GANG_PREEMPT 2048u  /* isl_preempt reads gangs from its requests (runs of equal `handle`) and picks the victims a whole gang
+                                        needs, or evicts nothing for it (see isl_preempt, P1-P8); every other call is unchanged */
 /* Node locality of one gang on an ISL_FLAG_GANG_LOCALITY engine (isl_request.start of its ALLOC members, rules L1-L6) */
 #define ISL_GANG_ANY_NODES      0u  /* rules 2-4: members anywhere, as on an engine without a gang flag */
 #define ISL_GANG_ONE_NODE       1u  /* G2-G3: every member on one node */
@@ -485,7 +487,48 @@ typedef struct isl_victim {
  *   6. Every policy, both quirk sets, per-node tables, inside isl_set_partition.  n == 0 does nothing.
  *      ISL_EINVAL: NULL buffers with n > 0 (or victims NULL with n_victims > 0), an engine created with ISL_FLAG_ALL_NODES.
  *      ISL_ERANGE: n > max_batch, n_victims > 8 x max_gpus, a partition that is empty or holds more than 2^20 GPUs.
- *      ISL_ESTATE: no profiles or inventory, or an open stream. */
+ *      ISL_ESTATE: no profiles or inventory, or an open stream.
+ *
+ * Gang preemption (ISL_FLAG_GANG_PREEMPT): a high-priority job whose pods must all run, or none of them (a gang of isl_place_gangs), asks
+ * for the victims of the whole gang in one query, so that no pod is deleted for a gang that still cannot run.  On an engine created with
+ * the flag, rules 1-6 hold except where these say otherwise:
+ *   P1. Gangs.  A gang is a maximal run of consecutive requests with equal `handle` (opaque otherwise, never echoed).  Its ALLOC members
+ *       carry the same `priority` byte, the gang's priority.  Its locality is the engine's: one node under ISL_FLAG_GANG_ONE_NODE,
+ *       distinct nodes under ISL_FLAG_GANG_DISTINCT_NODES, under ISL_FLAG_GANG_LOCALITY the ALLOC members' `start` byte as in L1 (0, 1
+ *       or 3), else any node.  ISL_EINVAL, nothing changed, when two ALLOC members of one gang carry different priority bytes, or under
+ *       ISL_FLAG_GANG_LOCALITY different locality bytes, or a locality byte of 2 (few nodes) or above 3; these checks run with the other
+ *       argument checks, before the engine state is looked at (as L4 and M6).  A FREE is still ISL_EINVAL (rule 3).  Other ops report
+ *       NOOP with an all-NONE evict row and do not count.
+ *   P2. Order.  Gangs go in array order.  Gang i sees the state the COMMITTED gangs before it left: their victims gone, their spans busy
+ *       and pinned.  An aborted gang leaves no trace.
+ *   P3. Choice.  Any node: the ALLOC members in order, each chosen by rules 4-5 over the partition, each seeing the gang's earlier
+ *       members (their victims gone, their spans pinned).  Distinct nodes: the same, restricted to the GPUs whose node holds no earlier
+ *       member of the gang (a node the partition cuts counts as one node, as in S2).  One node: for every node N of the partition the
+ *       members are resolved in order by rules 4-5 restricted to N's GPUs inside the partition; N can take the gang when every member
+ *       gets a candidate, and its cost is the lexicographic tuple (the highest priority among all the victims the members evict + 1, or
+ *       0 with none; the sum of their priorities; how many they are; N's position in the engine's scan order of rule 5).  The gang goes
+ *       to the node of least cost: pickOneNodeForPreemption with the gang treated as one pod.
+ *   P4. Commit.  Every ALLOC member gets a PLACED record (gpu, start, size), and its evict row the victims it evicts, ascending, padded
+ *       with ISL_GPU_NONE.  The union of a gang's rows is what the caller deletes.
+ *   P5. Failure.  Any node and distinct nodes: rule 4 of isl_place_gangs (the first member without a candidate keeps its NO_CAPACITY or
+ *       BAD_PROFILE record, every other ALLOC member reports ISL_ST_GANG_ABORTED).  One node: G3, with D the largest number of leading
+ *       ALLOC members that any node resolves with evictions.  Every evict row of an aborted gang is all ISL_GPU_NONE.
+ *   P6. Consequences.  (a) With all handles distinct (gangs of one) a flagged call equals the unflagged one under every policy, quirk
+ *       set, locality, node table and partition, records and evict rows (for one-node gangs of one because a node's GPUs are contiguous
+ *       in scan order).  (b) With no victim listed, or none below its gang's priority, a flagged FIRST_FIT or RIGHT_TO_LEFT call returns
+ *       the records isl_place_gangs returns on the same engine and requests, for localities 0, 1 and 3.  (c) The call is a query (rule 1).
+ *       (d) With the victims of a committed gang, and of every committed gang before it, removed, the gang's spans are free and pairwise
+ *       disjoint; a one-node gang's members share one node (isl_gpu_to_node), a distinct-node gang's members are on distinct nodes.
+ *       (e) Under any-node locality a call equals its gangs run one at a time through the unflagged isl_preempt, each gang's evictions
+ *       and spans applied when every member was placed and dropped otherwise.
+ *   P7. isl_create: ISL_EINVAL for the flag with ISL_FLAG_ALL_NODES, ISL_FLAG_GANG_FEW_NODES or ISL_FLAG_GANG_MIN_MEMBERS.  A
+ *       node-scoring engine takes it, with any-node gangs (its locality flags are refused already).  isl_preempt keeps every code of
+ *       rule 6, the 2^20-GPU partition cap included.  Every other entry point, isl_place_gangs included, returns exactly what it returns
+ *       without the flag.
+ *   P8. Greedy, member by member (as S4 and F5): a gang can abort although some choice of victims would fit it.  A100-40GB rows,
+ *       reference-exact quirks, first-fit, one GPU with byte 0x01 held by a victim of priority 0, a gang of priority 1: [1g.5gb, 4g.20gb]
+ *       aborts (the 1g takes the free start 1, since an empty V wins, and pins a slice the 4g needs), [4g.20gb, 1g.5gb] commits (the 4g
+ *       takes start 0 and evicts the victim, the 1g takes start 4).  List the larger members first. */
 int  isl_preempt(isl_engine* e, uint32_t n, const isl_request* in, const uint8_t* priority,
                  uint32_t n_victims, const isl_victim* victims, isl_result* out, uint32_t* evict);
 

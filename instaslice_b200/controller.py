@@ -98,7 +98,7 @@ class InstasliceReconciler:
 
     def __init__(self, instaslices: list, quirks: int = E.QUIRKS_REF_EXACT, max_batch: int = 65536, engine: E.Engine | None = None,
                  policy: int = E.POLICY_FIRST_FIT, gang_one_node: bool = False, gang_distinct_nodes: bool = False,
-                 gang_few_nodes: bool = False, gang_locality: bool = False, gang_min_members: bool = False):
+                 gang_few_nodes: bool = False, gang_locality: bool = False, gang_min_members: bool = False, gang_preempt: bool = False):
         """``policy``: the engine policy of the engine this reconciler creates (``engine`` is None), e.g. ``E.POLICY_MOST_ALLOCATED`` to
         pack MIG pods onto the fullest nodes or ``E.POLICY_LEAST_ALLOCATED`` to spread them (include/islplace.h).  ``gang_one_node``:
         that engine is created with ``E.FLAG_GANG_ONE_NODE``, so ``place_pending_gangs`` puts every gang on one node.
@@ -107,7 +107,8 @@ class InstasliceReconciler:
         it, else on as few nodes as it greedily can (the engine refuses it with either of the other two).  ``gang_locality``: with
         ``E.FLAG_GANG_LOCALITY``, so ``place_pending_gangs`` takes a locality per gang (the engine refuses it with the other three).
         ``gang_min_members``: with ``E.FLAG_GANG_MIN_MEMBERS`` (alone or with one of the four), so ``place_pending_gangs`` takes a
-        minimum per gang and may place a gang's leading pods only."""
+        minimum per gang and may place a gang's leading pods only.  ``gang_preempt``: with ``E.FLAG_GANG_PREEMPT`` (alone or with the
+        one-node, distinct-node or locality flag), so ``preempt_pending_gangs`` picks the victims of whole gangs."""
         self.quirks = quirks
         self.policy = policy
         self.gang_one_node = gang_one_node
@@ -115,6 +116,7 @@ class InstasliceReconciler:
         self.gang_few_nodes = gang_few_nodes
         self.gang_locality = gang_locality
         self.gang_min_members = gang_min_members
+        self.gang_preempt = gang_preempt
         self.items = instaslices
         self._engine = engine
         self._max_batch = max_batch
@@ -161,7 +163,8 @@ class InstasliceReconciler:
                                           (E.FLAG_GANG_DISTINCT_NODES if self.gang_distinct_nodes else 0) |
                                           (E.FLAG_GANG_FEW_NODES if self.gang_few_nodes else 0) |
                                           (E.FLAG_GANG_LOCALITY if self.gang_locality else 0) |
-                                          (E.FLAG_GANG_MIN_MEMBERS if self.gang_min_members else 0))
+                                          (E.FLAG_GANG_MIN_MEMBERS if self.gang_min_members else 0) |
+                                          (E.FLAG_GANG_PREEMPT if self.gang_preempt else 0))
         self._engine.load_profile_tables(self.rows)
         self._engine.load_inventory(self.node_off, np.asarray(occ, dtype=np.uint8))
         self._engine.set_node_tables(np.asarray(self.node_table, dtype=np.uint8))
@@ -333,6 +336,52 @@ class InstasliceReconciler:
         ("none", None, []).  Nothing is written to the custom resources: the caller deletes the victim pods, and once the daemonset
         has removed their allocations a later ``place_pending_pods`` places the pod on the reported slices (first-fit engine).
         """
+        rank, victims, uids = self._victims(pods, pod_priority)
+        res, evict = self._engine.preempt(self._requests([p["profile"] for p in pods]),
+                                          np.array([rank[int(p["priority"])] for p in pods], dtype=np.uint8), victims)
+        out = []
+        for r, row in zip(res, evict):
+            if r["status"] != E.ST_PLACED:
+                out.append(("none", None, []))
+                continue
+            gone = [uids[int(k)] for k in row if k != E.GPU_NONE]
+            out.append(("preempt", self._where(r), gone) if gone else ("fits", None, []))
+        return out
+
+    def preempt_pending_gangs(self, gangs: list, pod_priority: dict, locality=None):
+        """Gang preemption (ONE engine call, isl_preempt on an engine created with ``gang_preempt=True``): for each gang of pods that
+        must all run or none, the slices its pods would take and the running pods that must leave first, or nothing when the gang
+        cannot run even then.  ``gangs`` are lists of pods shaped as ``preempt_pending_pods`` takes them; the pods of one gang carry one
+        priority (else ``ValueError``).  The victims may be any ``Allocations`` entry ``preempt_pending_pods`` may evict.
+        ``locality``: one ``E.GANG_*`` value per gang (0, 1 or 3) for a reconciler created with ``gang_locality=True`` as well.
+
+        Returns per gang ("fits", None, []) | ("preempt", [{"nodename", "gpuUUID", "start", "size"} per pod], [victim pod UIDs]) |
+        ("none", None, []).  Nothing is written to the custom resources: the caller deletes the union of the victims, and once their
+        allocations are gone ``place_pending_gangs`` places the gang (include/islplace.h P6 (d): it fits where it was shown, though a
+        greedy placement may choose other slices).
+        """
+        if any(not g for g in gangs):
+            raise ValueError("empty gang")
+        if any(len({int(p["priority"]) for p in g}) > 1 for g in gangs):
+            raise ValueError("the pods of one gang have different priorities")
+        if not gangs:
+            return []
+        pods = [p for g in gangs for p in g]
+        rank, victims, uids = self._victims(pods, pod_priority)
+        off = np.cumsum([0] + [len(g) for g in gangs])
+        res, evict = self._engine.preempt(self._requests([p["profile"] for p in pods]),
+                                          np.array([rank[int(p["priority"])] for p in pods], dtype=np.uint8), victims, off, locality)
+        out = []
+        for a, b in zip(off[:-1], off[1:]):
+            if (res["status"][a:b] != E.ST_PLACED).any():
+                out.append(("none", None, []))
+                continue
+            gone = sorted({int(k) for row in evict[a:b] for k in row if k != E.GPU_NONE})
+            out.append(("preempt", [self._where(r) for r in res[a:b]], [uids[k] for k in gone]) if gone else ("fits", None, []))
+        return out
+
+    def _victims(self, pods, pod_priority):
+        """Dense priority ranks over every value seen, the victims (VICTIM_DTYPE) and their pod UIDs (preempt_pending_pods)."""
         values = sorted({int(p["priority"]) for p in pods} | {int(v) for v in pod_priority.values()})
         if len(values) > 255:
             raise ValueError("more than 255 distinct priority values")
@@ -352,20 +401,12 @@ class InstasliceReconciler:
                         continue
                     victims.append((g, int(a["start"]), int(a["size"]), rank[int(pod_priority[uid])], 0))
                     uids.append(uid)
-        res, evict = self._engine.preempt(self._requests([p["profile"] for p in pods]),
-                                          np.array([rank[int(p["priority"])] for p in pods], dtype=np.uint8),
-                                          np.array(victims, dtype=E.VICTIM_DTYPE))
-        out = []
-        for r, row in zip(res, evict):
-            if r["status"] != E.ST_PLACED:
-                out.append(("none", None, []))
-                continue
-            gone = [uids[int(k)] for k in row if k != E.GPU_NONE]
-            uuid = self.gpu_uuid[int(r["gpu"])]
-            where = {"nodename": self.items[self.node_of_uuid[uuid]]["metadata"]["name"], "gpuUUID": uuid,
-                     "start": int(r["start"]), "size": int(r["size"])}
-            out.append(("preempt", where, gone) if gone else ("fits", None, []))
-        return out
+        return rank, np.array(victims, dtype=E.VICTIM_DTYPE), uids
+
+    def _where(self, r):
+        uuid = self.gpu_uuid[int(r["gpu"])]
+        return {"nodename": self.items[self.node_of_uuid[uuid]]["metadata"]["name"], "gpuUUID": uuid, "start": int(r["start"]),
+                "size": int(r["size"])}
 
     def release(self, pod_uid: str):
         """The daemonset deleted ``Allocations[podUID]`` (instaslice_daemonset.go:261-263): free its span."""

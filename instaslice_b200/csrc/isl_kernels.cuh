@@ -3057,4 +3057,268 @@ __global__ void __launch_bounds__(kGnThreads, 1) k_ganglocal(GangNodeArgs a, Dev
     if (tid == 0 && placed) count_placed(a.ctrl, placed);
 }
 
+// ---------------------------------------------------------------------------------------------
+// Gang preemption: isl_preempt on an ISL_FLAG_GANG_PREEMPT engine (DESIGN.md 4.15), after k_victim_map.  One cooperative launch per call
+// on k_ganglocal's node-aligned shares: CTA c owns the partition's nodes [cta_node[c], cta_node[c + 1]) (NodeShare; only its node bounds
+// are used, since a query writes no occupancy byte).  Each GPU of a share keeps k_preempt's 11 bytes (priority of every slice's victim,
+// 255 = none; occupancy; run starts; table) and a scratch copy of the first 10, in shared memory when the share fits the opt-in, else in
+// global memory (kPgBytesPerGpu per GPU of the partition).  The gangs run in array order, each on the state the committed ones left:
+//   any node / distinct nodes  pg_members: per ALLOC member one grid_min of preempt_key over the share; the owner of the winning GPU logs
+//                              its prior state (one PgLog per member), applies the eviction and writes the record and evict row.
+//                              Distinct nodes also mark the winning node as used for the rest of the gang (in the scratch occupancy
+//                              byte).  A member with no candidate rolls the gang back from the log in reverse order.
+//   one node                   pg_one_node: one warp per node resolves the members on the scratch copy of its node, accumulating the
+//                              cost (max, sum, count of the victims); a two-word grid_min picks the node; its owner replays the gang on
+//                              its live state.
+// Records: every CTA writes the defaults of its slice of the requests (NOOP, BAD_PROFILE, NO_CAPACITY) before one grid barrier; the
+// host has set every evict row to ISL_GPU_NONE.  A PLACED record and its row have one writer, the CTA that owns the GPU; CTA 0 writes
+// GANG_ABORTED for the members after the one that stopped a gang.
+// ---------------------------------------------------------------------------------------------
+constexpr uint32_t kPgBytesPerGpu = 21;                 // 11 live bytes + 10 scratch bytes per GPU of a share
+
+struct PgLog {                  // a GPU's state before an any-node or distinct-node member took it (the rollback log, one per member)
+    unsigned long long prio;
+    uint32_t r, gw, o_rs, pad;  // the member's request, the partition-local GPU, occupancy | run starts << 8
+};
+
+struct PgState {                // one copy of the per-GPU state of a share, indexed by share position
+    unsigned long long* prio;
+    uint8_t *occ, *rs;
+};
+
+// The best candidate of one GPU for a preemptor of profile p at priority pi (k_preempt's scan of one GPU): ~0 when there is none.
+__device__ __forceinline__ unsigned long long pg_best(const uint8_t* s_masks, uint32_t tab, uint32_t p, uint32_t pi, unsigned long long pr,
+                                                      uint32_t o, uint32_t rs, uint32_t gw) {
+    uint32_t ev = 0;                                        // slices whose victim has a priority below the preemptor's
+#pragma unroll
+    for (uint32_t s = 0; s < ISL_SLOTS; ++s) ev |= (((uint32_t)(pr >> (8 * s)) & 0xFFu) < pi) << s;
+    const uint32_t blocked = o & ~ev;
+    const uint8_t* mk = s_masks + (tab * ISL_MAX_PROFILES + p) * ISL_MAX_STARTS;
+    unsigned long long best = ~0ull;
+#pragma unroll
+    for (uint32_t k = 0; k < ISL_MAX_STARTS; ++k) {
+        const uint32_t m = mk[k];
+        if (m && !(m & blocked)) best = min(best, preempt_key(m, o, rs, pr, gw, k));
+    }
+    return best;
+}
+
+// One thread: the preemptor of request r takes span m on share position g (partition-local GPU gw) of state st: its victims leave whole,
+// the span becomes busy and pinned.  rec: also write the PLACED record and the evict row (victim indices ascending).
+__device__ __forceinline__ void pg_take(const PreemptArgs& p, const DevProfiles& prof, const PgState& st, uint32_t g, uint32_t gw, uint32_t m,
+                                        uint32_t r, bool rec) {
+    const uint32_t o = st.occ[g], rs = st.rs[g];
+    const uint32_t heads = (rs & m) | (o & m & (m & (0u - m)));
+    const uint4* w4 = reinterpret_cast<const uint4*>(p.vmap + (size_t)gw * ISL_SLOTS);
+    const uint4 w0 = w4[0], w1 = w4[1];
+    const uint32_t w[ISL_SLOTS] = {w0.x, w0.y, w0.z, w0.w, w1.x, w1.y, w1.z, w1.w};
+    uint32_t idx[ISL_SLOTS], nv = 0, gone = 0;
+    for (uint32_t h = heads; h; h &= h - 1) {
+        const uint32_t v = w[__ffs(h) - 1];
+        uint32_t j = nv++;
+        for (; j > 0 && idx[j - 1] > v; --j) idx[j] = idx[j - 1];
+        idx[j] = v;
+#pragma unroll
+        for (uint32_t s = 0; s < ISL_SLOTS; ++s) gone |= (w[s] == v) << s;
+    }
+    const uint32_t touched = gone | m;
+    unsigned long long pr = st.prio[g];
+#pragma unroll
+    for (uint32_t s = 0; s < ISL_SLOTS; ++s) if ((touched >> s) & 1u) pr |= 0xFFull << (8 * s);
+    st.prio[g] = pr; st.rs[g] = (uint8_t)(rs & ~touched); st.occ[g] = (uint8_t)((o & ~gone) | m);
+    if (rec) {
+        p.out[r] = pack_result(flip_gpu(p.lo + gw, prof.flip), __ffs(m) - 1, __popc(m), ISL_ST_PLACED);
+        for (uint32_t j = 0; j < nv; ++j) p.evict[(size_t)r * ISL_SLOTS + j] = idx[j];
+    }
+}
+
+// Warp-wide: resolve the ALLOC members of requests [r0, r1) in order by rules 4-5 restricted to the c GPUs at share positions [b0, b0 + c)
+// of state st (one node).  Returns how many leading ALLOC members got a candidate; *all: every one did.  mx, sum, cnt: the highest
+// victim priority + 1, the sum of the priorities and the number of the victims they evict.  commit: also write records and evict rows.
+__device__ uint32_t pg_node_resolve(const PreemptArgs& p, const DevProfiles& prof, const PgState& st, const uint8_t* tab, const uint8_t* s_masks,
+                                    uint32_t b0, uint32_t c, uint32_t base, uint32_t r0, uint32_t r1, bool commit, uint32_t lane, bool* all,
+                                    uint32_t& mx, uint32_t& sum, uint32_t& cnt) {
+    uint32_t depth = 0;
+    mx = sum = cnt = 0;
+    *all = false;
+    for (uint32_t rb = r0; rb < r1; rb += 32) {
+        const uint2 q = rb + lane < r1 ? p.in[rb + lane] : make_uint2(0, (uint32_t)ISL_OP_NOOP << 8);
+        uint32_t live = __ballot_sync(0xFFFFFFFFu, ((q.y >> 8) & 0xFFu) == ISL_OP_ALLOC);
+        while (live) {
+            const uint32_t j = __ffs(live) - 1;
+            live &= live - 1;
+            const uint32_t prof_i = __shfl_sync(0xFFFFFFFFu, q.y, j) & 0xFFu;
+            if (prof_i >= prof.n) return depth;             // an unknown profile has no candidate
+            const uint32_t pi = p.prio[rb + j];
+            unsigned long long best = ~0ull;
+            for (uint32_t g = lane; g < c; g += 32)
+                best = min(best, pg_best(s_masks, tab[b0 + g], prof_i, pi, st.prio[b0 + g], st.occ[b0 + g], st.rs[b0 + g], base + b0 + g));
+            const unsigned long long win = warp_min(best);  // every lane has read its bytes: the owner may rewrite one below
+            if (win == ~0ull) return depth;
+            mx = max(mx, (uint32_t)(win >> 42));
+            sum += (uint32_t)(win >> 31) & 0x7FFu;
+            cnt += (uint32_t)(win >> 27) & 0xFu;
+            const uint32_t g = (uint32_t)(win >> 3) & 0xFFFFFFu;
+            if (((g - base - b0) & 31u) == lane) {
+                const uint32_t m = s_masks[((uint32_t)tab[g - base] * ISL_MAX_PROFILES + prof_i) * ISL_MAX_STARTS + ((uint32_t)win & 7u)];
+                pg_take(p, prof, st, g - base, g, m, rb + j, commit);
+            }
+            __syncwarp();
+            ++depth;
+        }
+    }
+    *all = true;
+    return depth;
+}
+
+// One gang of requests [r0, r1) of any-node or (distinct) distinct-node locality, every thread of the CTA (P3, P5: rule 4).  `rank`
+// counts the ALLOC members that took a GPU; the one that found none stops the gang, and every CTA puts back, in reverse order, the
+// logged GPUs of its share and reports their members GANG_ABORTED with an empty evict row.
+__device__ __forceinline__ void pg_members(const PreemptArgs& p, const DevProfiles& prof, const NodeShare& sh,
+                                           const PgState& live, const uint8_t* tab, uint8_t* mark, const uint8_t* s_masks, PgLog* log,
+                                           uint32_t r0, uint32_t r1, bool distinct, uint32_t& parity, unsigned long long* s_warp,
+                                           unsigned long long* s_win, uint32_t tid, uint32_t lane, uint32_t warp) {
+    const uint32_t base = sh.base, cnt = sh.cnt;
+    if (distinct) for (uint32_t g = tid; g < cnt; g += kGnThreads) mark[g] = 0;
+    __syncthreads();                                        // also orders the previous gang's commits before this gang's reads
+    uint32_t rank = 0;
+    for (uint32_t r = r0; r < r1; ++r) {
+        const uint32_t y = p.in[r].y, pq = y & 0xFFu;
+        if (((y >> 8) & 0xFFu) != ISL_OP_ALLOC) continue;
+        unsigned long long win = ~0ull;                     // an unknown profile fails without a barrier: every CTA knows it
+        if (pq < prof.n) {
+            const uint32_t pi = p.prio[r];
+            unsigned long long best = ~0ull;
+            for (uint32_t g = tid; g < cnt; g += kGnThreads)
+                if (!distinct || !mark[g]) best = min(best, pg_best(s_masks, tab[g], pq, pi, live.prio[g], live.occ[g], live.rs[g], base + g));
+            win = grid_min<kGnThreads>(best, p.keys, parity, s_warp, s_win);
+        }
+        if (win == ~0ull) {
+            cooperative_groups::this_grid().sync();         // every CTA's log entries of this gang are in L2
+            if (tid == 0) {
+                for (uint32_t k = rank; k-- > 0;) {
+                    const uint32_t gw = __ldcg(&log[k].gw), pos = gw - base;
+                    if (pos >= cnt) continue;
+                    const uint32_t o_rs = __ldcg(&log[k].o_rs), rr = __ldcg(&log[k].r);
+                    live.prio[pos] = __ldcg(&log[k].prio); live.occ[pos] = (uint8_t)o_rs; live.rs[pos] = (uint8_t)(o_rs >> 8);
+                    p.out[rr] = pack_result(ISL_GPU_NONE, ISL_START_NONE, prof.rows[p.in[rr].y & 0xFFu].size, ISL_ST_GANG_ABORTED);
+                    for (uint32_t j = 0; j < ISL_SLOTS; ++j) p.evict[(size_t)rr * ISL_SLOTS + j] = kVictimNone;
+                }
+            }
+            if (blockIdx.x == 0 && warp == 0) abort_gang_members(p.in, p.out, prof, r, r1, 0, lane);
+            return;
+        }
+        const uint32_t gw = (uint32_t)(win >> 3) & 0xFFFFFFu, pos = gw - base;
+        if (pos < cnt) {                                    // this CTA owns the GPU
+            if (tid == 0) {
+                const PgLog e{live.prio[pos], r, gw, (uint32_t)live.occ[pos] | (uint32_t)live.rs[pos] << 8, 0u};
+                log[rank] = e;
+                const uint32_t m = s_masks[((uint32_t)tab[pos] * ISL_MAX_PROFILES + pq) * ISL_MAX_STARTS + ((uint32_t)win & 7u)];
+                pg_take(p, prof, live, pos, gw, m, r, true);
+            }
+            if (distinct) {                                 // the member's node is used for the rest of the gang
+                uint32_t jl = sh.j0, jh = sh.j1;            // nb(jl) <= base + pos < nb(jh): the last such jl is the non-empty node
+                while (jh - jl > 1) {
+                    const uint32_t mid = (jl + jh) / 2;
+                    if (sh.nb(mid) - base <= pos) jl = mid; else jh = mid;
+                }
+                for (uint32_t g = sh.nb(jl) - base + tid; g < sh.nb(jl + 1) - base; g += kGnThreads) mark[g] = 1;
+            }
+        }
+        __syncthreads();                                    // the owner's state and marks are in place before the next member's scan
+        ++rank;
+    }
+}
+
+// One gang of requests [r0, r1) of one-node locality, every thread of the CTA (P3, P5: G3).  Each warp evaluates nodes of the share on
+// the scratch copy; a node's key is the two words (max + 1 << 31 | sum, count << 32 | node) for a node that takes the gang, else
+// (gn_fail_key(depth, node), 0).  The first grid_min takes the least first word, the second the least second word among the CTAs that
+// hold it.  The owner of the winning node replays the gang on its live state; a failure: CTA 0 reports every ALLOC member except the one
+// at the deepest depth D GANG_ABORTED.
+__device__ __forceinline__ void pg_one_node(const PreemptArgs& p, const DevProfiles& prof, const NodeShare& sh, const PgState& live,
+                                            const PgState& scr, const uint8_t* tab, const uint8_t* s_masks, uint32_t r0, uint32_t r1,
+                                            uint32_t& parity, unsigned long long* s_warp, unsigned long long* s_win, uint32_t lane,
+                                            uint32_t warp) {
+    __syncthreads();                                        // the previous gang's commits are in the live state before this gang's reads
+    unsigned long long hi = ~0ull, lo = ~0ull;              // the least key of this warp's nodes
+    for (uint32_t j = sh.j0 + warp; j < sh.j1; j += kGnThreads / 32) {
+        const uint32_t b0 = sh.nb(j) - sh.base, c = sh.nb(j + 1) - sh.base - b0;
+        if (c == 0) continue;                               // an empty node takes nothing: depth 0, the floor of every failure
+        for (uint32_t g = lane; g < c; g += 32) {
+            scr.prio[b0 + g] = live.prio[b0 + g]; scr.occ[b0 + g] = live.occ[b0 + g]; scr.rs[b0 + g] = live.rs[b0 + g];
+        }
+        __syncwarp();
+        bool all;
+        uint32_t mx, sum, cnt;
+        const uint32_t d = pg_node_resolve(p, prof, scr, tab, s_masks, b0, c, sh.base, r0, r1, false, lane, &all, mx, sum, cnt);
+        const unsigned long long kh = all ? ((unsigned long long)mx << 31) | sum : gn_fail_key(d, j);
+        const unsigned long long kl = all ? ((unsigned long long)cnt << 32) | j : 0ull;
+        if (kh < hi || (kh == hi && kl < lo)) { hi = kh; lo = kl; }
+    }
+    const unsigned long long win = grid_min<kGnThreads>(hi, p.keys, parity, s_warp, s_win);
+    if (!(win & kGnFail)) {
+        const uint32_t j = (uint32_t)grid_min<kGnThreads>(hi == win ? lo : ~0ull, p.keys, parity, s_warp, s_win);
+        if (j >= sh.j0 && j < sh.j1 && warp == 0) {         // the owner replays the gang on its live state
+            const uint32_t b0 = sh.nb(j) - sh.base, c = sh.nb(j + 1) - sh.base - b0;
+            bool all;
+            uint32_t mx, sum, cnt;
+            pg_node_resolve(p, prof, live, tab, s_masks, b0, c, sh.base, r0, r1, true, lane, &all, mx, sum, cnt);
+        }
+    } else if (blockIdx.x == 0 && warp == 0) {              // the deepest failure's depth; ~0ull (no node evaluated) is depth 0 as well
+        abort_gang_members(p.in, p.out, prof, r0, r1, gn_fail_depth(win), lane);
+    }
+}
+
+// kLoc: ISL_GANG_ANY_NODES, _ONE_NODE or _DISTINCT_NODES for every gang, or kLocPerGang for each gang's byte (0, 1 or 3, checked on the
+// host).  With a constant kLoc the compiler drops the other bodies.
+template <uint32_t kLoc>
+__global__ void __launch_bounds__(kGnThreads, 1) k_preempt_gangs(GangNodeArgs a, PreemptArgs p, DevProfiles prof, PgLog* log,
+                                                                const uint8_t* __restrict__ locality) {
+    extern __shared__ __align__(16) unsigned char pg_smem[];
+    __shared__ uint8_t s_masks[kMaxTables * ISL_MAX_PROFILES * ISL_MAX_STARTS];
+    __shared__ unsigned long long s_warp[kGnThreads / 32];
+    __shared__ unsigned long long s_win;
+    const uint32_t tid = threadIdx.x, lane = tid & 31u, warp = tid >> 5;
+    const NodeShare sh(a, pg_smem);                         // a.share == 0: it copies nothing
+    // p.per_cta: GPUs per array of a share in shared memory, 0 = every share's arrays in global memory, strided by the partition
+    const size_t S = p.per_cta ? p.per_cta : p.Gr, off = p.per_cta ? 0 : sh.base;
+    unsigned char* const mem = p.per_cta ? pg_smem : a.scratch;
+    const PgState live{reinterpret_cast<unsigned long long*>(mem) + off, mem + 16 * S + off, mem + 17 * S + off};
+    const PgState scr{reinterpret_cast<unsigned long long*>(mem) + S + off, mem + 19 * S + off, mem + 20 * S + off};
+    uint8_t* const tab = mem + 18 * S + off;
+    for (uint32_t i = tid; i < sizeof(s_masks); i += kGnThreads) s_masks[i] = p.masks[i];
+    for (uint32_t g = tid; g < sh.cnt; g += kGnThreads) {
+        const uint32_t gw = sh.base + g;
+        const uint4* w4 = reinterpret_cast<const uint4*>(p.vmap + (size_t)gw * ISL_SLOTS);
+        const uint4 w0 = w4[0], w1 = w4[1];
+        const uint32_t w[ISL_SLOTS] = {w0.x, w0.y, w0.z, w0.w, w1.x, w1.y, w1.z, w1.w};
+        unsigned long long pr = 0;
+        uint32_t rs = 0;
+#pragma unroll
+        for (uint32_t s = 0; s < ISL_SLOTS; ++s) {
+            const uint32_t v = w[s] == kVictimNone ? 0xFFu : p.victims[w[s]].priority;
+            pr |= (unsigned long long)v << (8 * s);
+            if (w[s] != kVictimNone && (s == 0 || w[s - 1] != w[s])) rs |= 1u << s;
+        }
+        live.prio[g] = pr; live.rs[g] = (uint8_t)rs;
+        live.occ[g] = p.occ[p.lo + gw]; tab[g] = p.gtab[p.lo + gw];
+    }
+    for (uint32_t i = blockIdx.x * kGnThreads + tid; i < p.n; i += gridDim.x * kGnThreads) {      // default records
+        const uint32_t y = p.in[i].y, q = y & 0xFFu;
+        p.out[i] = ((y >> 8) & 0xFFu) != ISL_OP_ALLOC ? pack_result(ISL_GPU_NONE, ISL_START_NONE, 0, ISL_ST_NOOP)
+                   : q >= prof.n                      ? pack_result(ISL_GPU_NONE, ISL_START_NONE, 0, ISL_ST_BAD_PROFILE)
+                                                      : pack_result(ISL_GPU_NONE, ISL_START_NONE, prof.rows[q].size, ISL_ST_NO_CAPACITY);
+    }
+    cooperative_groups::this_grid().sync();                 // the defaults are written before any owner or CTA 0 rewrites one
+    uint32_t parity = 0;
+    for (uint32_t gi = 0; gi < a.n_gangs; ++gi) {
+        const uint32_t r0 = __ldg(a.gang_off + gi), r1 = __ldg(a.gang_off + gi + 1), loc = kLoc == kLocPerGang ? __ldg(locality + gi) : kLoc;
+        if (loc == ISL_GANG_ONE_NODE)
+            pg_one_node(p, prof, sh, live, scr, tab, s_masks, r0, r1, parity, s_warp, &s_win, lane, warp);
+        else
+            pg_members(p, prof, sh, live, tab, scr.occ, s_masks, log, r0, r1, loc == ISL_GANG_DISTINCT_NODES, parity, s_warp, &s_win, tid, lane,
+                       warp);
+    }
+}
+
 }  // namespace isl

@@ -52,6 +52,19 @@ uint32_t gang_kind(uint32_t flags) {
     return (flags & ISL_FLAG_GANG_ONE_NODE) ? 0 : (flags & ISL_FLAG_GANG_FEW_NODES) ? 1 : 2;
 }
 
+// The instantiations of k_preempt_gangs, one per kind of ISL_FLAG_GANG_PREEMPT engine (preempt_gang_kind).
+constexpr uint32_t kPreemptGangKinds = 4;
+const GangKernel kPreemptGangKernels[kPreemptGangKinds] = {
+    {(const void*)k_preempt_gangs<ISL_GANG_ANY_NODES>, "k_preempt_gangs<any_node>", false},
+    {(const void*)k_preempt_gangs<ISL_GANG_ONE_NODE>, "k_preempt_gangs<one_node>", false},
+    {(const void*)k_preempt_gangs<ISL_GANG_DISTINCT_NODES>, "k_preempt_gangs<distinct_nodes>", false},
+    {(const void*)k_preempt_gangs<kLocPerGang>, "k_preempt_gangs<per_gang>", false},
+};
+uint32_t preempt_gang_kind(uint32_t flags) {
+    if (flags & ISL_FLAG_GANG_LOCALITY) return 3;
+    return (flags & ISL_FLAG_GANG_ONE_NODE) ? 1 : (flags & ISL_FLAG_GANG_DISTINCT_NODES) ? 2 : 0;
+}
+
 // What plan_pipeline decides for one k_pipeline launch: GPUs per stage (seg), stages, GPUs per sub-segment, speculative rounds.
 struct PipePlan {
     uint32_t seg = 0, n_seg = 0, sub = 0;
@@ -196,12 +209,16 @@ struct isl_engine {
     DevMem<uint32_t> d_done_cnt;     // [chunk] committed segments
     DevMem<uint8_t> d_occ_snap; uint32_t snap_G = 0;      // isl_snapshot_occupancy / isl_restore_occupancy
     // isl_preempt: the victim-index map (8 words per GPU of the partition), the victims, staging of [candidate masks | priorities], the
-    // evict rows, the per-CTA minima of k_preempt and k_victim_map's error word
+    // evict rows, the per-CTA minima of k_preempt and k_victim_map's error word.  ISL_FLAG_GANG_PREEMPT (k_preempt_gangs): the gang
+    // offsets followed by the locality bytes, the rollback log (one entry per request), the per-GPU state when the shares do not fit in
+    // shared memory, and the dynamic shared memory one CTA of each instantiation may have
     struct Preempt {
-        DevMem<uint32_t> vmap, evict, err;
+        DevMem<uint32_t> vmap, evict, err, gangs;
         DevMem<isl_victim> victims;
-        DevMem<uint8_t> stage;
+        DevMem<uint8_t> stage, state;
         DevMem<unsigned long long> keys;
+        DevMem<PgLog> log;
+        int optin[kPreemptGangKinds] = {};
     } pre;
     // node scoring (k_nodefit): the inventory's node offsets (isl_load_inventory), the per-profile min-trees when they do not fit in shared
     // memory, the per-(profile, node) fit counts and the per-node busy / cap words, grown to the partition; the width of every table
@@ -473,12 +490,12 @@ int run_gangs(isl_engine* e, uint32_t n_gangs, const uint32_t* d_gang_off, uint3
     return ISL_OK;
 }
 
-// The layout of k_ganglocal, over the nodes the partition touches: each CTA gets whole nodes, about Gr / grid GPUs (one CTA per SM at most,
-// one per 512 GPUs below that, never more than nodes), and 2 bytes per GPU of its share in shared memory when they fit in `smem_optin` (the
-// kernel's dynamic shared memory opt-in), else in global memory (gn.scratch).  Fills every field of `a`; *nodes = the nodes the partition
-// touches.
-int gang_layout(isl_engine* e, const void* kernel, int smem_optin, uint32_t n_gangs, const uint32_t* d_gang_off, const uint2* d_in, uint2* d_out,
-                GangNodeArgs& a, uint32_t* grid_out, size_t* smem_out, uint32_t* nodes) {
+// The layout of k_ganglocal and k_preempt_gangs, over the nodes the partition touches: each CTA gets whole nodes, about Gr / grid GPUs
+// (one CTA per SM at most, one per 512 GPUs below that, never more than nodes), and `per_gpu` bytes per GPU of its share (rounded up to 16
+// GPUs) in shared memory when they fit in `smem_optin` (the kernel's dynamic shared memory opt-in), else *smem_out = 0 and the caller
+// keeps them in global memory (a.scratch).  Fills every other field of `a`, a.share in GPUs; *nodes = the nodes the partition touches.
+int gang_layout(isl_engine* e, const void* kernel, int smem_optin, uint32_t per_gpu, uint32_t n_gangs, const uint32_t* d_gang_off,
+                const uint2* d_in, uint2* d_out, GangNodeArgs& a, uint32_t* grid_out, size_t* smem_out, uint32_t* nodes) {
     auto& gn = e->gn;
     const uint32_t Gr = e->hi - e->lo;
     uint32_t nlo, nhi;
@@ -494,18 +511,17 @@ int gang_layout(isl_engine* e, const void* kernel, int smem_optin, uint32_t n_ga
         a.cta_node[c] = c == grid ? nhi - nlo : (uint32_t)(std::lower_bound(gn.off.begin() + nlo, gn.off.begin() + nhi, target) - gn.off.begin()) - nlo;
         share = std::max(share, local(a.cta_node[c]) - local(a.cta_node[c - 1]));
     }
-    // the live bytes and the second byte per GPU (scratch copies or marks) of a share in shared memory when both fit, else in global memory
-    size_t smem = ((size_t)share + 15) / 16 * 16 * 2;
+    // the bytes of a share in shared memory when they fit, else in global memory
+    size_t smem = ((size_t)share + 15) / 16 * 16 * per_gpu;
     if (smem > (size_t)smem_optin ||
         cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, kGnThreads, smem) != cudaSuccess || per_sm < 1) {
         cudaGetLastError();
         smem = 0;
-        ISL_CUDA(e, gn.scratch.reserve(Gr));
     }
     ISL_CUDA(e, gn.keys.reserve((size_t)2 * grid));
     a.in = d_in; a.out = d_out; a.occ = e->d_occ; a.gtab = e->d_gtab; a.lut = e->d_lut; a.score = e->d_score; a.sizes = e->d_sizes;
-    a.node_off = gn.node_off; a.gang_off = d_gang_off; a.scratch = gn.scratch; a.keys = gn.keys; a.ctrl = e->d_ctrl;
-    a.n_gangs = n_gangs; a.n_tables = e->n_tables; a.lo = e->lo; a.hi = e->hi; a.nlo = nlo; a.share = (uint32_t)(smem / 2);
+    a.node_off = gn.node_off; a.gang_off = d_gang_off; a.keys = gn.keys; a.ctrl = e->d_ctrl;
+    a.n_gangs = n_gangs; a.n_tables = e->n_tables; a.lo = e->lo; a.hi = e->hi; a.nlo = nlo; a.share = (uint32_t)(smem / per_gpu);
     *grid_out = grid; *smem_out = smem; *nodes = nhi - nlo;
     return ISL_OK;
 }
@@ -522,7 +538,9 @@ int run_ganglocal(isl_engine* e, uint32_t kind, uint32_t n_gangs, const uint32_t
     GangNodeArgs a;
     uint32_t grid, nodes;
     size_t smem;
-    if (int rc = gang_layout(e, k.fn, e->gn.optin[kind], n_gangs, d_gang_off, d_in, d_out, a, &grid, &smem, &nodes)) return rc;
+    if (int rc = gang_layout(e, k.fn, e->gn.optin[kind], 2, n_gangs, d_gang_off, d_in, d_out, a, &grid, &smem, &nodes)) return rc;
+    if (!smem) ISL_CUDA(e, e->gn.scratch.reserve(e->hi - e->lo));     // the second byte per GPU; the live bytes are the occupancy
+    a.scratch = e->gn.scratch;
     if (k.wins) ISL_CUDA(e, e->gn.wins.reserve(nodes));
     uint2* wins = e->gn.wins;
     void* params[] = {&a, &e->prof, &wins, &d_locality};
@@ -1170,6 +1188,9 @@ int isl_create(const isl_config* cfg, isl_engine** out) {
          node_scoring(cfg->policy))) return ISL_EINVAL;
     // elastic gangs (M6): with any one locality flag or none (their own checks refuse two), not with a pod on every node nor node scoring
     if ((cfg->flags & ISL_FLAG_GANG_MIN_MEMBERS) && ((cfg->flags & ISL_FLAG_ALL_NODES) || node_scoring(cfg->policy))) return ISL_EINVAL;
+    // gang preemption (P7): few-node and elastic gangs have no preemption order, a pod on every node has no single GPU to evict on
+    if ((cfg->flags & ISL_FLAG_GANG_PREEMPT) &&
+        (cfg->flags & (ISL_FLAG_ALL_NODES | ISL_FLAG_GANG_FEW_NODES | ISL_FLAG_GANG_MIN_MEMBERS))) return ISL_EINVAL;
     if (request_major(cfg->policy) && cfg->max_gpus > kBfMaxGpus) return ISL_ERANGE;
     if (cfg->quirks & ~ISL_QUIRKS_REF_EXACT) return ISL_EINVAL;
     isl_engine* e = new (std::nothrow) isl_engine;
@@ -1225,6 +1246,11 @@ int isl_create(const isl_config* cfg, isl_engine** out) {
             ISL_TRY(cudaFuncGetAttributes(&fa, kGangKernels[i].fn));
             e->gn.optin[i] = optin - (int)fa.sharedSizeBytes;
             ISL_TRY(cudaFuncSetAttribute(kGangKernels[i].fn, cudaFuncAttributeMaxDynamicSharedMemorySize, e->gn.optin[i]));
+        }
+        for (uint32_t i = 0; i < kPreemptGangKinds; ++i) {     // and each k_preempt_gangs instantiation
+            ISL_TRY(cudaFuncGetAttributes(&fa, kPreemptGangKernels[i].fn));
+            e->pre.optin[i] = optin - (int)fa.sharedSizeBytes;
+            ISL_TRY(cudaFuncSetAttribute(kPreemptGangKernels[i].fn, cudaFuncAttributeMaxDynamicSharedMemorySize, e->pre.optin[i]));
         }
     }
     e->occ_bytes = ((size_t)cfg->max_gpus + kSweepBlock - 1) / kSweepBlock * kSweepBlock;
@@ -1436,8 +1462,8 @@ int isl_load_inventory(isl_engine* e, uint32_t n_nodes, const uint32_t* node_off
         ISL_CUDA(e, e->nf.node_off.replace((size_t)n_nodes + 1));
         ISL_CUDA(e, cudaMemcpyAsync(e->nf.node_off, node_off, ((size_t)n_nodes + 1) * sizeof(uint32_t), cudaMemcpyHostToDevice, e->stream));
     }
-    if (e->cfg.flags & kGangTopologyFlags) {
-        // k_ganglocal walks the nodes in storage order (reversed under right-to-left)
+    if (e->cfg.flags & (kGangTopologyFlags | ISL_FLAG_GANG_PREEMPT)) {
+        // k_ganglocal and k_preempt_gangs walk the nodes in storage order (reversed under right-to-left)
         auto& off = e->gn.off;
         off.assign(node_off, node_off + n_nodes + 1);
         if (e->prof.flip) { std::reverse(off.begin(), off.end()); for (auto& x : off) x = G - x; }
@@ -1581,11 +1607,71 @@ int isl_place_gangs(isl_engine* e, uint32_t n_gangs, const uint32_t* gang_off, c
     return ISL_OK;
 }
 
+// isl_preempt on an ISL_FLAG_GANG_PREEMPT engine, after k_victim_map: one cooperative launch of the engine's k_preempt_gangs
+// instantiation on gang_layout's shares (kPgBytesPerGpu per GPU, in p.state when they do not fit in shared memory).  The gang offsets
+// and the locality bytes go to p.gangs; every evict row starts as ISL_GPU_NONE.
+int run_preempt_gangs(isl_engine* e, const std::vector<uint32_t>& gang_off, const std::vector<uint8_t>& locality, uint32_t n,
+                      const uint8_t* d_prio, const uint8_t* d_masks) {
+    auto& p = e->pre;
+    const uint32_t kind = preempt_gang_kind(e->cfg.flags), n_gangs = (uint32_t)gang_off.size() - 1, Gr = e->hi - e->lo;
+    const GangKernel& k = kPreemptGangKernels[kind];
+    ISL_CUDA(e, p.gangs.reserve(gang_off.size() + (locality.size() + 3) / 4));
+    uint32_t* d_gang_off = p.gangs;
+    const uint8_t* d_locality = reinterpret_cast<const uint8_t*>(d_gang_off + gang_off.size());
+    ISL_CUDA(e, cudaMemcpyAsync(d_gang_off, gang_off.data(), gang_off.size() * sizeof(uint32_t), cudaMemcpyHostToDevice, e->stream));
+    if (!locality.empty())
+        ISL_CUDA(e, cudaMemcpyAsync((void*)d_locality, locality.data(), locality.size(), cudaMemcpyHostToDevice, e->stream));
+    ISL_CUDA(e, p.log.reserve(n));
+    GangNodeArgs a;
+    uint32_t grid, nodes;
+    size_t smem;
+    if (int rc = gang_layout(e, k.fn, p.optin[kind], kPgBytesPerGpu, n_gangs, d_gang_off, e->d_req, e->d_res, a, &grid, &smem, &nodes)) return rc;
+    if (!smem) ISL_CUDA(e, p.state.reserve((size_t)Gr * kPgBytesPerGpu));
+    a.scratch = p.state;
+    PreemptArgs pa{};
+    pa.in = e->d_req; pa.prio = d_prio; pa.victims = p.victims; pa.vmap = p.vmap; pa.occ = e->d_occ; pa.gtab = e->d_gtab; pa.masks = d_masks;
+    pa.out = e->d_res; pa.evict = p.evict;
+    pa.n = n; pa.lo = e->lo; pa.Gr = Gr; pa.per_cta = a.share;      // GPUs per array of a share in shared memory, 0 = global memory
+    a.share = 0;                                                    // NodeShare copies no occupancy byte: the kernel keeps its own state
+    ISL_CUDA(e, p.keys.reserve((size_t)2 * grid));
+    pa.keys = p.keys;
+    ISL_CUDA(e, cudaMemsetAsync(p.evict, 0xFF, (size_t)n * ISL_SLOTS * sizeof(uint32_t), e->stream));
+    PgLog* log = p.log;
+    void* params[] = {&a, &pa, &e->prof, &log, &d_locality};
+    return launch_cooperative(e, k.fn, k.name, grid, kGnThreads, smem, params);
+}
+
 int isl_preempt(isl_engine* e, uint32_t n, const isl_request* in, const uint8_t* priority,
                 uint32_t n_victims, const isl_victim* victims, isl_result* out, uint32_t* evict) {
     if (!e || (n && (!in || !priority || !out || !evict)) || (n_victims && !victims)) return ISL_EINVAL;
     if (e->cfg.flags & ISL_FLAG_ALL_NODES) return ISL_EINVAL;      // one pod on every node with capacity: no single GPU to evict on
     for (uint32_t i = 0; i < n; ++i) if (in[i].op == ISL_OP_FREE) return ISL_EINVAL;      // releases are expressed by the victim list
+    const bool gangs = e->cfg.flags & ISL_FLAG_GANG_PREEMPT;
+    std::vector<uint32_t> gang_off;                                 // P1: maximal runs of equal handles
+    std::vector<uint8_t> locality;                                  // under ISL_FLAG_GANG_LOCALITY: each gang's byte, 0 without ALLOCs
+    if (gangs) {
+        const bool per_gang = e->cfg.flags & ISL_FLAG_GANG_LOCALITY;
+        for (uint32_t i = 0; i < n; ++i) {
+            if (i == 0 || in[i].handle != in[i - 1].handle) {
+                gang_off.push_back(i);
+                if (per_gang) locality.push_back((uint8_t)ISL_GANG_ANY_NODES);
+            }
+        }
+        gang_off.push_back(n);
+        for (size_t g = 0; g + 1 < gang_off.size(); ++g) {
+            bool named = false;
+            uint8_t prio = 0;
+            for (uint32_t r = gang_off[g]; r < gang_off[g + 1]; ++r) {
+                if (in[r].op != ISL_OP_ALLOC) continue;
+                if (named && priority[r] != prio) return ISL_EINVAL;
+                if (per_gang && ((in[r].start != ISL_GANG_ANY_NODES && in[r].start != ISL_GANG_ONE_NODE &&
+                                  in[r].start != ISL_GANG_DISTINCT_NODES) || (named && in[r].start != locality[g]))) return ISL_EINVAL;
+                if (per_gang) locality[g] = in[r].start;
+                prio = priority[r];
+                named = true;
+            }
+        }
+    }
     if (n > e->cfg.max_batch || (uint64_t)n_victims > (uint64_t)ISL_SLOTS * e->cfg.max_gpus) return ISL_ERANGE;
     Entry guard(e, Needs::ready, n);
     if (guard.rc) return guard.rc;
@@ -1597,7 +1683,7 @@ int isl_preempt(isl_engine* e, uint32_t n, const isl_request* in, const uint8_t*
     ISL_CUDA(e, cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, e->device));
     const uint32_t grid = std::max(1u, std::min((uint32_t)sms, ceil_div(Gr, kPreThreads))), per_cta = ceil_div(Gr, grid);
     const size_t smem = (size_t)per_cta * kPreBytesPerGpu;
-    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_preempt, kPreThreads, smem) != cudaSuccess || per_sm < 1) {
+    if (!gangs && (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_preempt, kPreThreads, smem) != cudaSuccess || per_sm < 1)) {
         cudaGetLastError();
         return ISL_ERANGE;                                  // a share too large for one CTA's shared memory on this device
     }
@@ -1628,12 +1714,16 @@ int isl_preempt(isl_engine* e, uint32_t n, const isl_request* in, const uint8_t*
         ISL_CUDA(e, cudaStreamSynchronize(e->stream));
         if (err) return ISL_EINVAL;                         // a malformed, free or overlapping victim: nothing else runs
     }
-    PreemptArgs a{};
-    a.in = e->d_req; a.prio = p.stage + kMaskBytes; a.victims = p.victims; a.vmap = p.vmap; a.occ = e->d_occ; a.gtab = e->d_gtab;
-    a.masks = p.stage; a.out = e->d_res; a.evict = p.evict; a.keys = p.keys;
-    a.n = n; a.lo = e->lo; a.Gr = Gr; a.per_cta = per_cta;
-    void* params[] = {&a, &e->prof};
-    if (int rc = launch_cooperative(e, (const void*)k_preempt, "k_preempt", grid, kPreThreads, smem, params)) return rc;
+    if (gangs) {
+        if (int rc = run_preempt_gangs(e, gang_off, locality, n, p.stage + kMaskBytes, p.stage)) return rc;
+    } else {
+        PreemptArgs a{};
+        a.in = e->d_req; a.prio = p.stage + kMaskBytes; a.victims = p.victims; a.vmap = p.vmap; a.occ = e->d_occ; a.gtab = e->d_gtab;
+        a.masks = p.stage; a.out = e->d_res; a.evict = p.evict; a.keys = p.keys;
+        a.n = n; a.lo = e->lo; a.Gr = Gr; a.per_cta = per_cta;
+        void* params[] = {&a, &e->prof};
+        if (int rc = launch_cooperative(e, (const void*)k_preempt, "k_preempt", grid, kPreThreads, smem, params)) return rc;
+    }
     ISL_CUDA(e, cudaMemcpyAsync(out, e->d_res, (size_t)n * sizeof(isl_result), cudaMemcpyDeviceToHost, e->stream));
     ISL_CUDA(e, cudaMemcpyAsync(evict, p.evict, (size_t)n * ISL_SLOTS * sizeof(uint32_t), cudaMemcpyDeviceToHost, e->stream));
     ISL_CUDA(e, cudaStreamSynchronize(e->stream));

@@ -36,6 +36,7 @@ FLAG_GANG_DISTINCT_NODES = 128  # isl_place_gangs puts every member of a gang on
 FLAG_GANG_FEW_NODES = 256  # isl_place_gangs puts a gang on one node when one takes it, else on as few nodes as it greedily can
 FLAG_GANG_LOCALITY = 512  # isl_place_gangs takes each gang's node locality from its ALLOC members' start byte (GANG_*)
 FLAG_GANG_MIN_MEMBERS = 1024  # elastic gangs: a gang commits its leading members once they reach its minimum (the ALLOC size byte)
+FLAG_GANG_PREEMPT = 2048  # isl_preempt picks the victims a whole gang (a run of equal handles) needs, or evicts nothing for it
 GANG_ANY_NODES, GANG_ONE_NODE, GANG_FEW_NODES, GANG_DISTINCT_NODES = 0, 1, 2, 3     # node locality of one gang (include/islplace.h L1)
 SPEC_AUTO, SPEC_OFF, SPEC_ON = 0, 1, 2
 
@@ -387,15 +388,41 @@ class Engine:
         self._check(self._lib.isl_place_gangs(self._h, len(gang_off) - 1, _ptr(gang_off), _ptr(requests), _ptr(out)), "isl_place_gangs")
         return out
 
-    def preempt(self, requests: np.ndarray, priority, victims: np.ndarray):
+    def preempt(self, requests: np.ndarray, priority, victims: np.ndarray, gang_off=None, locality=None):
         """Priority preemption query (isl_preempt): for each ALLOC in ``requests`` at ``priority[i]`` (uint8, higher = more important),
         the GPU and start it would take once the lower-priority ``victims`` (VICTIM_DTYPE) listed in ``evict[i]`` are gone.  Returns
-        ``(results, evict)``, ``evict`` an [n, 8] uint32 array of victim indices padded with GPU_NONE.  Changes no engine state."""
+        ``(results, evict)``, ``evict`` an [n, 8] uint32 array of victim indices padded with GPU_NONE.  Changes no engine state.
+
+        On an engine created with ``FLAG_GANG_PREEMPT`` the runs of equal ``handle`` are gangs: a gang gets victims for every ALLOC
+        member or for none (include/islplace.h P1-P8), its members share one priority, and a one-node gang goes to the node whose
+        victims cost least.  ``gang_off``: gang i is ``requests[gang_off[i]:gang_off[i + 1]]``, written as gang indices into the
+        ``handle`` of a copy; ``locality``: one ``GANG_*`` value per gang (0, 1 or 3), written into the ``start`` of the ALLOC members of
+        the copy, which needs an engine created with ``FLAG_GANG_LOCALITY`` as well.  Both need an engine created with the flag."""
         requests = np.ascontiguousarray(requests, dtype=REQUEST_DTYPE)
         priority = np.ascontiguousarray(priority, dtype=np.uint8)
         victims = np.ascontiguousarray(victims, dtype=VICTIM_DTYPE)
         if len(priority) != len(requests):
             raise ValueError("one priority per request")
+        if gang_off is not None or locality is not None:
+            if not self.flags & FLAG_GANG_PREEMPT:
+                raise ValueError("gangs in isl_preempt need an engine created with FLAG_GANG_PREEMPT")
+            requests = requests.copy()
+        if gang_off is not None:
+            gang_off = np.asarray(gang_off, dtype=np.int64)
+            if len(gang_off) == 0 or gang_off[0] != 0 or int(gang_off[-1]) != len(requests) or (np.diff(gang_off) <= 0).any():
+                raise ValueError("gang_off must start at 0, rise strictly and end at len(requests)")
+            requests["handle"] = np.repeat(np.arange(len(gang_off) - 1), np.diff(gang_off)).astype(np.uint32)
+        if locality is not None:
+            if not self.flags & FLAG_GANG_LOCALITY:
+                raise ValueError("a locality per gang needs an engine created with FLAG_GANG_LOCALITY")
+            if gang_off is None:
+                raise ValueError("a locality per gang needs gang_off")
+            locality = np.asarray(locality, dtype=np.int64)
+            if len(locality) != len(gang_off) - 1:
+                raise ValueError("one locality per gang")
+            per_request = np.repeat(locality, np.diff(gang_off))
+            alloc = requests["op"] == OP_ALLOC
+            requests["start"][alloc] = per_request[alloc].astype(np.uint8)
         out = np.empty(len(requests), dtype=RESULT_DTYPE)
         evict = np.empty((len(requests), 8), dtype=np.uint32)
         self._check(self._lib.isl_preempt(self._h, len(requests), _ptr(requests), _ptr(priority), len(victims), _ptr(victims), _ptr(out),

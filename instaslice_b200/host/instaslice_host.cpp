@@ -277,19 +277,15 @@ std::vector<GangOutcome> InstasliceReconciler::PlaceGangs(InstasliceList& list, 
     return out;
 }
 
-std::vector<PreemptOutcome> InstasliceReconciler::PreemptPending(const InstasliceList& list, const std::vector<PreemptPod>& pods,
-                                                                 const std::map<std::string, int32_t>& podPriority) {
-    std::vector<PreemptOutcome> out(pods.size());
-    if (pods.empty()) return out;
-    std::set<int32_t> values;
-    for (const PreemptPod& p : pods) values.insert(p.Priority);
+// Dense ranks over the pending pods' values `own` and every value of podPriority, the victims in (GPU, start) order and their pod UIDs.
+void InstasliceReconciler::preemptVictims(const InstasliceList& list, const std::vector<int32_t>& own,
+                                          const std::map<std::string, int32_t>& podPriority, std::map<int32_t, uint8_t>& rank,
+                                          std::vector<isl_victim>& victims, std::vector<std::string>& uids) const {
+    std::set<int32_t> values(own.begin(), own.end());
     for (const auto& kv : podPriority) values.insert(kv.second);
     if (values.size() > 255) throw std::runtime_error("more than 255 distinct priority values");
-    std::map<int32_t, uint8_t> rank;
     for (int32_t v : values) rank.emplace(v, (uint8_t)rank.size());
     auto span = [](uint32_t start, uint32_t size) { return ((1u << size) - 1u) << start; };
-    std::vector<isl_victim> victims;
-    std::vector<std::string> uids;
     for (uint32_t g = 0; g < gpuUUID_.size(); ++g) {            // victims in (GPU, start) order
         const InstasliceSpec& spec = list.Items[gpuNode_[g]].Spec;
         const std::string& uuid = gpuUUID_[g];
@@ -312,6 +308,18 @@ std::vector<PreemptOutcome> InstasliceReconciler::PreemptPending(const Instaslic
             uids.push_back(uid);
         }
     }
+}
+
+std::vector<PreemptOutcome> InstasliceReconciler::PreemptPending(const InstasliceList& list, const std::vector<PreemptPod>& pods,
+                                                                 const std::map<std::string, int32_t>& podPriority) {
+    std::vector<PreemptOutcome> out(pods.size());
+    if (pods.empty()) return out;
+    std::vector<int32_t> own;
+    for (const PreemptPod& p : pods) own.push_back(p.Priority);
+    std::map<int32_t, uint8_t> rank;
+    std::vector<isl_victim> victims;
+    std::vector<std::string> uids;
+    preemptVictims(list, own, podPriority, rank, victims, uids);
     std::vector<std::string> names;
     std::vector<uint8_t> prio;
     for (const PreemptPod& p : pods) { names.push_back(p.ProfileName); prio.push_back(rank.at(p.Priority)); }
@@ -327,6 +335,59 @@ std::vector<PreemptOutcome> InstasliceReconciler::PreemptPending(const Instaslic
         o.GPUUUID = gpuUUID_[res[i].gpu];
         o.Start = res[i].start; o.Size = res[i].size;
         for (size_t k = 0; k < 8; ++k) if (evict[i * 8 + k] != ISL_GPU_NONE) o.Victims.push_back(uids[evict[i * 8 + k]]);
+        o.verdict = o.Victims.empty() ? PreemptVerdict::Fits : PreemptVerdict::Preempt;
+    }
+    return out;
+}
+
+std::vector<GangPreemptOutcome> InstasliceReconciler::PreemptPendingGangs(const InstasliceList& list,
+                                                                          const std::vector<std::vector<PreemptPod>>& gangs,
+                                                                          const std::map<std::string, int32_t>& podPriority,
+                                                                          const std::vector<uint8_t>& locality) {
+    std::vector<GangPreemptOutcome> out(gangs.size());
+    if (!locality.empty() && locality.size() != gangs.size()) throw std::runtime_error("one locality per gang");
+    std::vector<int32_t> own;
+    std::vector<std::string> names;
+    std::vector<uint32_t> gang_of;
+    for (size_t k = 0; k < gangs.size(); ++k) {
+        if (gangs[k].empty()) throw std::runtime_error("empty gang");
+        for (const PreemptPod& p : gangs[k]) {
+            if (p.Priority != gangs[k][0].Priority) throw std::runtime_error("the pods of one gang have different priorities");
+            own.push_back(p.Priority); names.push_back(p.ProfileName); gang_of.push_back((uint32_t)k);
+        }
+    }
+    if (names.empty()) return out;
+    std::map<int32_t, uint8_t> rank;
+    std::vector<isl_victim> victims;
+    std::vector<std::string> uids;
+    preemptVictims(list, own, podPriority, rank, victims, uids);
+    std::vector<isl_request> req = requests(names);
+    std::vector<uint8_t> prio;
+    for (size_t i = 0; i < req.size(); ++i) {
+        req[i].handle = gang_of[i];                                   // P1: a gang is a run of equal handles
+        if (!locality.empty() && req[i].op == ISL_OP_ALLOC) req[i].start = locality[gang_of[i]];
+        prio.push_back(rank.at(own[i]));
+    }
+    std::vector<isl_result> res(req.size());
+    std::vector<uint32_t> evict(req.size() * 8);
+    check(isl_preempt(h_, (uint32_t)req.size(), req.data(), prio.data(), (uint32_t)victims.size(), victims.data(), res.data(), evict.data()),
+          h_, "isl_preempt");
+    for (size_t i = 0, k = 0; k < gangs.size(); i += gangs[k].size(), ++k) {
+        GangPreemptOutcome& o = out[k];
+        bool all = true;
+        for (size_t j = i; j < i + gangs[k].size(); ++j) all &= res[j].status == ISL_ST_PLACED;
+        if (!all) continue;
+        std::set<uint32_t> gone;
+        for (size_t j = i; j < i + gangs[k].size(); ++j) {
+            PreemptOutcome w;
+            w.verdict = PreemptVerdict::Fits;
+            w.Nodename = list.Items[gpuNode_[res[j].gpu]].Name;
+            w.GPUUUID = gpuUUID_[res[j].gpu];
+            w.Start = res[j].start; w.Size = res[j].size;
+            o.pods.push_back(w);
+            for (size_t x = 0; x < 8; ++x) if (evict[j * 8 + x] != ISL_GPU_NONE) gone.insert(evict[j * 8 + x]);
+        }
+        for (uint32_t v : gone) o.Victims.push_back(uids[v]);
         o.verdict = o.Victims.empty() ? PreemptVerdict::Fits : PreemptVerdict::Preempt;
     }
     return out;

@@ -81,6 +81,13 @@ struct PreemptOutcome {
     std::vector<std::string> Victims;                 // pod UIDs to delete first (Preempt)
 };
 struct GangOutcome { Verdict verdict = Verdict::None; std::vector<AllocationDetails> allocs; };   // allocs: one per pod when Placed
+// One gang of PreemptPendingGangs: where each pod would go (Fits and Preempt, one entry per pod; their Victims are empty) and the union of
+// the pod UIDs to delete first (Preempt)
+struct GangPreemptOutcome {
+    PreemptVerdict verdict = PreemptVerdict::None;
+    std::vector<PreemptOutcome> pods;
+    std::vector<std::string> Victims;
+};
 
 extern const char* const kErrNoGpu;              // "failed to find allocatable gpu" (:261)
 
@@ -134,6 +141,12 @@ public:
     // allocations are gone a later PlacePending places the pod there.
     std::vector<PreemptOutcome> PreemptPending(const InstasliceList& list, const std::vector<PreemptPod>& pods,
                                                const std::map<std::string, int32_t>& podPriority);
+    // The same for gangs that must all run or none, ONE engine call on an engine created with ISL_FLAG_GANG_PREEMPT (include/islplace.h
+    // P1-P8): a gang gets victims for every pod or none.  The pods of one gang carry one priority (else it throws).  locality: empty, or
+    // one ISL_GANG_* value per gang (0, 1 or 3) on an engine created with ISL_FLAG_GANG_LOCALITY as well.
+    std::vector<GangPreemptOutcome> PreemptPendingGangs(const InstasliceList& list, const std::vector<std::vector<PreemptPod>>& gangs,
+                                                        const std::map<std::string, int32_t>& podPriority,
+                                                        const std::vector<uint8_t>& locality = {});
     // The daemonset removed Allocations[podUID] (instaslice_daemonset.go:261-263).
     bool Release(InstasliceList& list, const std::string& podUID);
 
@@ -147,6 +160,8 @@ private:
     std::map<std::string, uint8_t> profiles_;
     std::map<std::string, uint32_t> gpuIndex_;
     bool orphans_ = false;
+    void preemptVictims(const InstasliceList& list, const std::vector<int32_t>& own, const std::map<std::string, int32_t>& podPriority,
+                        std::map<int32_t, uint8_t>& rank, std::vector<isl_victim>& victims, std::vector<std::string>& uids) const;
     std::vector<isl_request> requests(const std::vector<std::string>& names) const;
     std::vector<isl_result> place(const std::vector<std::string>& names, uint32_t lo, uint32_t hi);
     void releaseSpan(const isl_result& r);

@@ -77,6 +77,9 @@ const (
 	// PlaceGangsElastic takes a minimum per gang: a gang whose leading pods reach it while a later pod finds no GPU is placed with
 	// those pods only.  Alone or with one of the four flags above.
 	FlagGangMinMembers = uint32(C.ISL_FLAG_GANG_MIN_MEMBERS)
+	// PreemptPendingGangs picks the victims of whole gangs, or none for a gang that still cannot run.  Alone or with FlagGangOneNode,
+	// FlagGangDistinctNodes or FlagGangLocality; not with FlagGangFewNodes or FlagGangMinMembers.
+	FlagGangPreempt = uint32(C.ISL_FLAG_GANG_PREEMPT)
 )
 
 // StGangTrimmed is the record status of a pod its elastic gang was placed without (isl_result.status, FlagGangMinMembers).
@@ -703,6 +706,77 @@ type PreemptTarget struct {
 // resources: the caller deletes the victims, and once the daemonset has removed their allocations a later PlacePending places the pod.
 func (r *InstasliceReconciler) PreemptPending(e *PlacementEngine, list *inferencev1alpha1.InstasliceList, pods []PendingPod,
 	priority []int32, podPriority map[string]int32) ([]PreemptTarget, error) {
+	return r.preempt(e, list, pods, priority, podPriority, nil, nil)
+}
+
+// GangPreemptTarget is the answer of PreemptPendingGangs for one gang: Placed when every pod of the gang got a GPU, with one target per
+// pod (their Victims empty) and the union of the pod UIDs to delete first.
+type GangPreemptTarget struct {
+	Placed  bool
+	Pods    []PreemptTarget
+	Victims []string
+}
+
+// PreemptPendingGangs is PreemptPending for gangs that must all run or none, ONE engine call on an engine created with FlagGangPreempt
+// (include/islplace.h P1-P8): a gang gets victims for every pod or for none, a one-node gang goes to the node whose victims cost least.
+// priority[k] is the PriorityClass value of every pod of gangs[k]; locality is nil, or one Gang* value per gang (any, one or distinct
+// nodes) on an engine created with FlagGangLocality as well.  The caller deletes the union of the victims, then PlaceGangs places the
+// gang once their allocations are gone; it fits there, though a greedy placement may choose other slices.
+func (r *InstasliceReconciler) PreemptPendingGangs(e *PlacementEngine, list *inferencev1alpha1.InstasliceList, gangs [][]PendingPod,
+	priority []int32, podPriority map[string]int32, locality []uint8) ([]GangPreemptTarget, error) {
+	if len(priority) != len(gangs) || (locality != nil && len(locality) != len(gangs)) {
+		return nil, fmt.Errorf("one priority (and locality) per gang")
+	}
+	var pods []PendingPod
+	var prio []int32
+	var gangOf []uint32
+	var loc []uint8
+	for k, g := range gangs {
+		if len(g) == 0 {
+			return nil, fmt.Errorf("empty gang")
+		}
+		for _, p := range g {
+			pods = append(pods, p)
+			prio = append(prio, priority[k])
+			gangOf = append(gangOf, uint32(k))
+			if locality != nil {
+				loc = append(loc, locality[k])
+			}
+		}
+	}
+	flat, err := r.preempt(e, list, pods, prio, podPriority, gangOf, loc)
+	if err != nil {
+		return nil, err
+	}
+	out := make([]GangPreemptTarget, len(gangs))
+	i := 0
+	for k, g := range gangs {
+		t := GangPreemptTarget{Placed: true}
+		seen := map[string]bool{}
+		for j := range g {
+			p := flat[i+j]
+			t.Placed = t.Placed && p.Placed
+			for _, v := range p.Victims {
+				if !seen[v] {
+					seen[v] = true
+					t.Victims = append(t.Victims, v)
+				}
+			}
+			p.Victims = nil
+			t.Pods = append(t.Pods, p)
+		}
+		if !t.Placed {
+			t = GangPreemptTarget{}
+		}
+		out[k] = t
+		i += len(g)
+	}
+	return out, nil
+}
+
+// preempt is PreemptPending with, for gangs, a gang index per pod written into the request's handle and a locality byte into its start.
+func (r *InstasliceReconciler) preempt(e *PlacementEngine, list *inferencev1alpha1.InstasliceList, pods []PendingPod, priority []int32,
+	podPriority map[string]int32, gangOf []uint32, locality []uint8) ([]PreemptTarget, error) {
 	out := make([]PreemptTarget, len(pods))
 	if len(pods) == 0 {
 		return out, nil
@@ -788,6 +862,12 @@ func (r *InstasliceReconciler) PreemptPending(e *PlacementEngine, list *inferenc
 	e.fillRequests(req, pods, 0)
 	for i := range pods {
 		prio[i] = C.uint8_t(rank[priority[i]])
+		if gangOf != nil {
+			req[i].handle = C.uint32_t(gangOf[i])
+		}
+		if locality != nil {
+			req[i].start = C.uint8_t(locality[i])
+		}
 	}
 	if rc := C.isl_preempt(e.h, C.uint32_t(n), &req[0], &prio[0], C.uint32_t(len(victims)), &vic[0], &res[0], &evict[0]); rc != C.ISL_OK {
 		return nil, fmt.Errorf("isl_preempt: %s (%s)", C.GoString(C.isl_strerror(rc)), C.GoString(C.isl_last_cuda_error(e.h)))
