@@ -98,7 +98,7 @@ extern "C" {
  *   7. isl_create: ISL_EINVAL with ISL_FLAG_ALL_NODES (a pod placed on every node has no node to choose), ISL_ERANGE for
  *      max_gpus > 2^20.  isl_load_inventory: ISL_ERANGE for more than 2^20 nodes, empty nodes included (the nodes, not the GPUs,
  *      are the leaves of the score trees); the previous inventory stays loaded.  ISL_EINVAL from isl_place_batch_partitioned,
- *      isl_place_stream_partitioned, isl_stream_open and isl_place_gangs.
+ *      isl_place_stream_partitioned, isl_stream_open, and isl_place_gangs without ISL_FLAG_GANG_NODE_SCORE (N1-N8).
  * On an inventory of one node both give exactly ISL_POLICY_FIRST_FIT's records and occupancy. */
 #define ISL_POLICY_MOST_ALLOCATED  4u
 #define ISL_POLICY_LEAST_ALLOCATED 5u
@@ -157,6 +157,8 @@ typedef struct isl_config {
                                             ALLOC members name in their `size` byte (see isl_place_gangs, M1-M7); every other call is unchanged */
 #define ISL_FLAG_GANG_PREEMPT 2048u  /* isl_preempt reads gangs from its requests (runs of equal `handle`) and picks the victims a whole gang
                                         needs, or evicts nothing for it (see isl_preempt, P1-P8); every other call is unchanged */
+#define ISL_FLAG_GANG_NODE_SCORE 4096u  /* on a node-scoring engine isl_place_gangs places gangs by MostAllocated or LeastAllocated (see
+                                           isl_place_gangs, N1-N8); every other call is unchanged */
 /* Node locality of one gang on an ISL_FLAG_GANG_LOCALITY engine (isl_request.start of its ALLOC members, rules L1-L6) */
 #define ISL_GANG_ANY_NODES      0u  /* rules 2-4: members anywhere, as on an engine without a gang flag */
 #define ISL_GANG_ONE_NODE       1u  /* G2-G3: every member on one node */
@@ -317,11 +319,12 @@ int  isl_place_batch_range(isl_engine* e, uint32_t lo, uint32_t hi, uint32_t n, 
  *      members after it are not tried, and every other ALLOC member of the gang reports ISL_ST_GANG_ABORTED with the unplaced default
  *      record (gpu ISL_GPU_NONE, start 9, the profile's size or 0 for an unknown profile).
  *   5. The occupancy after an aborted gang is exactly what it was before it: later gangs see no trace of it.
- *   6. Every policy except node scoring (ISL_POLICY_MOST_ALLOCATED / _LEAST_ALLOCATED), both quirk sets and per-node tables; inside
- *      the engine's partition (isl_set_partition).  Stats count committed placements only.
+ *   6. Every policy except node scoring (ISL_POLICY_MOST_ALLOCATED / _LEAST_ALLOCATED; see ISL_FLAG_GANG_NODE_SCORE, N1-N8), both
+ *      quirk sets and per-node tables; inside the engine's partition (isl_set_partition).  Stats count committed placements only.
  * A call whose gangs all have one member equals isl_place_batch on the same requests, records and occupancy.  The gangs are resolved
  * request by request (the best-fit kernel's loop, DESIGN.md 4.6): first-fit gangs do not use the segment pipeline.
- * ISL_EINVAL: malformed offsets, NULL buffers, an engine created with ISL_FLAG_ALL_NODES or a node-scoring policy.  ISL_ERANGE: n > max_batch, or a partition
+ * ISL_EINVAL: malformed offsets, NULL buffers, an engine created with ISL_FLAG_ALL_NODES, or with a node-scoring policy but without
+ * ISL_FLAG_GANG_NODE_SCORE.  ISL_ERANGE: n > max_batch, or a partition
  * that is empty or holds more than 2^20 GPUs.  ISL_ESTATE: no profiles or inventory, or an open stream.
  *
  * One-node gangs (ISL_FLAG_GANG_ONE_NODE): pods that talk to each other (a job's workers, a pipeline-parallel deployment) exchange data
@@ -444,6 +447,46 @@ int  isl_place_batch_range(isl_engine* e, uint32_t lo, uint32_t hi, uint32_t n, 
  *   M7. The committed members are always a LEADING run, never the best subset: under first-fit a gang [4g, 1g, 1g] with m = 2 aborts
  *       when the 4g fits nowhere, although both 1g would fit.  List the members the job needs first; for replicas of one profile the
  *       leading run is as many members as the locality places.
+ *
+ * Node-scored gangs (ISL_FLAG_GANG_NODE_SCORE): a cluster that packs its pods with MostAllocated (so that the autoscaler can drain the
+ * emptiest nodes) or spreads them with LeastAllocated places its jobs and replicas as gangs on the same engine, the same inventory and
+ * the same lock as its single pods, and a one-node gang goes to the fullest (emptiest) node that takes it, not the first.  On an engine
+ * created with the flag:
+ *   N1. isl_create: ISL_EINVAL for the flag without ISL_POLICY_MOST_ALLOCATED or _LEAST_ALLOCATED, or with ISL_FLAG_GANG_FEW_NODES or
+ *       ISL_FLAG_GANG_MIN_MEMBERS (ISL_FLAG_ALL_NODES is refused by node scoring already).  It may come with at most one of
+ *       ISL_FLAG_GANG_ONE_NODE, _DISTINCT_NODES and _LOCALITY (their mutual refusals are unchanged; only their refusal of node scoring is
+ *       lifted, and only with this bit), and with ISL_FLAG_GANG_PREEMPT (N7).  max_gpus > 2^20 and more than 2^20 nodes keep node
+ *       scoring's ISL_ERANGE.
+ *   N2. Rules 1, 2, 3 and 5 hold.  A gang's locality is the engine's flag, under ISL_FLAG_GANG_LOCALITY its ALLOC members' `start` byte
+ *       (L1), with neither any node.
+ *   N3. Any node: the ALLOC members in order, each placed by node-scoring rules 1-5 over the partition with req = its own row size, each
+ *       seeing every earlier commit, the gang's tentative members included (their slices count in busy).  Failure is rule 4.
+ *   N4. Distinct nodes: each member as in N3, restricted to the nodes that hold no earlier member of the same gang (a node the partition
+ *       cuts counts as one node, as in S2).  Failure is S3; the choice is greedy, member by member (S4).
+ *   N5. One node: node N can take the gang when its ALLOC members, resolved in order by the reference's search restricted to N's GPUs
+ *       inside the partition, all place.  Among those nodes the gang goes to the highest score for req = R(N), the sum of the members'
+ *       row sizes in N's table (the gang scored as one pod, as P3 does): MostAllocated floor(100 (busy + R) / cap), LeastAllocated
+ *       floor(100 (cap - busy - R) / cap); ties to the lowest canonical node index.  With no such node the failure record is G3 (same D).
+ *   N6. Both quirk sets, per-node tables (each node's score normalised by its own width), inside isl_set_partition; stats.placed counts
+ *       committed members only.  isl_place_gangs keeps every code above, the 2^20-GPU partition cap included.  Under
+ *       ISL_FLAG_GANG_LOCALITY a locality byte of 2 (few nodes) is ISL_EINVAL, checked with L4 before the engine state is looked at;
+ *       nothing changes.
+ *   N7. Every other entry point returns exactly what it returns on the same engine without the bit: isl_place_batch and every other
+ *       k_nodefit caller, isl_what_if, isl_capacity, isl_preempt.  With ISL_FLAG_GANG_PREEMPT, isl_preempt keeps P1-P8, whose scan
+ *       order is ascending canonical under node scoring (rule 5), so it returns what a FIRST_FIT engine with the same flags minus this
+ *       one returns.
+ *   N8. Consequences: (a) with gangs of one ALLOC member, a call of any locality (0, 1 or 3) equals isl_place_batch on the same engine:
+ *       records, occupancy and stats.placed; (b) under any-node locality a call equals its gangs run one at a time: a committed gang
+ *       equals isl_place_batch of its ALLOC members on the occupancy before it, an aborted gang changes nothing; (c) on a one-node
+ *       inventory, or a partition inside one node, a call equals isl_place_gangs on a FIRST_FIT engine with the same locality flags,
+ *       records and occupancy (on one node node scoring is first-fit); (d) a committed one-node gang's members share a node, a committed
+ *       distinct-node gang's members sit on pairwise distinct nodes (isl_gpu_to_node).
+ *   Example, H100-80GB rows (width 8), either quirk set: three one-GPU nodes with bytes 0x00, 0x3F and 0x0F, gang [1g.10gb, 1g.10gb].
+ *       one node        MOST: GPU 2 at starts 4, 5 (node 1 is fullest but start 7 is not legal, so it takes one member; R = 2 scores
+ *                       node 0 25 and node 2 75).  LEAST: GPU 0 at starts 0, 1 (75 against 25).  First-fit would take node 0.
+ *       any node        MOST: GPU 1 start 6 (87 against 12 and 62), then GPU 2 start 4 (node 1, now 0x7F, admits no 1g.10gb).
+ *                       LEAST: GPU 0 starts 0 then 1.
+ *       distinct nodes  MOST: as any node.  LEAST: GPU 0 start 0, then GPU 2 start 4 (node 0 is used; 37 against node 1's 12).
  */
 int  isl_place_gangs(isl_engine* e, uint32_t n_gangs, const uint32_t* gang_off, const isl_request* in, isl_result* out);
 

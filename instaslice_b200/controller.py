@@ -98,7 +98,8 @@ class InstasliceReconciler:
 
     def __init__(self, instaslices: list, quirks: int = E.QUIRKS_REF_EXACT, max_batch: int = 65536, engine: E.Engine | None = None,
                  policy: int = E.POLICY_FIRST_FIT, gang_one_node: bool = False, gang_distinct_nodes: bool = False,
-                 gang_few_nodes: bool = False, gang_locality: bool = False, gang_min_members: bool = False, gang_preempt: bool = False):
+                 gang_few_nodes: bool = False, gang_locality: bool = False, gang_min_members: bool = False, gang_preempt: bool = False,
+                 gang_node_score: bool = False):
         """``policy``: the engine policy of the engine this reconciler creates (``engine`` is None), e.g. ``E.POLICY_MOST_ALLOCATED`` to
         pack MIG pods onto the fullest nodes or ``E.POLICY_LEAST_ALLOCATED`` to spread them (include/islplace.h).  ``gang_one_node``:
         that engine is created with ``E.FLAG_GANG_ONE_NODE``, so ``place_pending_gangs`` puts every gang on one node.
@@ -108,7 +109,10 @@ class InstasliceReconciler:
         ``E.FLAG_GANG_LOCALITY``, so ``place_pending_gangs`` takes a locality per gang (the engine refuses it with the other three).
         ``gang_min_members``: with ``E.FLAG_GANG_MIN_MEMBERS`` (alone or with one of the four), so ``place_pending_gangs`` takes a
         minimum per gang and may place a gang's leading pods only.  ``gang_preempt``: with ``E.FLAG_GANG_PREEMPT`` (alone or with the
-        one-node, distinct-node or locality flag), so ``preempt_pending_gangs`` picks the victims of whole gangs."""
+        one-node, distinct-node or locality flag), so ``preempt_pending_gangs`` picks the victims of whole gangs.  ``gang_node_score``:
+        with ``E.FLAG_GANG_NODE_SCORE``, for a ``POLICY_MOST_ALLOCATED`` or ``POLICY_LEAST_ALLOCATED`` reconciler, so that
+        ``place_pending_gangs`` places gangs by the node score, alone (any node) or with the one-node, distinct-node or locality option
+        (the engine refuses it with any other policy, few-node gangs and elastic gangs)."""
         self.quirks = quirks
         self.policy = policy
         self.gang_one_node = gang_one_node
@@ -117,6 +121,7 @@ class InstasliceReconciler:
         self.gang_locality = gang_locality
         self.gang_min_members = gang_min_members
         self.gang_preempt = gang_preempt
+        self.gang_node_score = gang_node_score
         self.items = instaslices
         self._engine = engine
         self._max_batch = max_batch
@@ -164,7 +169,8 @@ class InstasliceReconciler:
                                           (E.FLAG_GANG_FEW_NODES if self.gang_few_nodes else 0) |
                                           (E.FLAG_GANG_LOCALITY if self.gang_locality else 0) |
                                           (E.FLAG_GANG_MIN_MEMBERS if self.gang_min_members else 0) |
-                                          (E.FLAG_GANG_PREEMPT if self.gang_preempt else 0))
+                                          (E.FLAG_GANG_PREEMPT if self.gang_preempt else 0) |
+                                          (E.FLAG_GANG_NODE_SCORE if self.gang_node_score else 0))
         self._engine.load_profile_tables(self.rows)
         self._engine.load_inventory(self.node_off, np.asarray(occ, dtype=np.uint8))
         self._engine.set_node_tables(np.asarray(self.node_table, dtype=np.uint8))

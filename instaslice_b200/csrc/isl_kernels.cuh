@@ -21,6 +21,8 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include <type_traits>
+
 #include "../../include/islplace.h"
 
 namespace isl {
@@ -2641,6 +2643,14 @@ struct GangNodeArgs {           // kernel parameter (by value)
     uint32_t cta_node[kGnMaxCtas + 1];
 };
 
+// k_ganglocal<.., kScore> on an ISL_FLAG_GANG_NODE_SCORE engine (DESIGN.md 4.16): what k_nodefit needs beside the gang arguments.  A
+// struct of its own, so that the parameter block of every other k_ganglocal and of k_preempt_gangs keeps its layout; the host fills one
+// for every launch, and the others read only its GangNodeArgs part, which comes first.
+struct GangScoreArgs : GangNodeArgs {
+    uint8_t width[kMaxTables];  // largest start + size over the rows of every table
+    uint32_t most;              // 1: MostAllocated, 0: LeastAllocated
+};
+
 // Warp-wide: resolve the ALLOC members of requests [r0, r1) in order on the `cnt` bytes `b` of one node of table t, the engine's policy
 // restricted to that node.  Returns how many leading ALLOC members were placed.  commit: b is the live share; the placements are also
 // written to the occupancy (storage index gbase + position) and reported PLACED.
@@ -2696,6 +2706,27 @@ struct NodeShare {
     // node j of the partition owns the partition-local GPUs [nb(j), nb(j + 1)); a node the partition cuts keeps its GPUs inside it
     __device__ __forceinline__ uint32_t nb(uint32_t j) const { return min(max(a.node_off[a.nlo + j], a.lo), a.hi) - a.lo; }
 };
+
+// Warp-wide (node-scored any-node and distinct-node members, DESIGN.md 4.16): node j's key for one member of profile p, nodefit_leaf over
+// the node's busy slices under its table's width on the live bytes, with the partition-local position of the node's first GPU that
+// admits p in place of the node.  One grid_min of these keys picks the highest score, then the lowest node, then that node's first
+// admitting GPU: node-scoring rules 4-5.  kInf for an empty node, a node that admits nothing, and under `mark` a node marked `tag`.
+__device__ __forceinline__ uint32_t gangscore_node(const GangScoreArgs& a, const NodeShare& sh, uint32_t j, uint32_t p, const uint8_t* mark,
+                                                   uint32_t tag, uint32_t lane) {
+    const uint32_t b0 = sh.nb(j) - sh.base, c = sh.nb(j + 1) - sh.base - b0;
+    if (c == 0 || (mark && mark[b0] == tag)) return kInf;  // a used node's GPUs are all marked
+    const uint32_t t = a.gtab[a.lo + sh.base + b0] & (kMaxTables - 1), row = (t * ISL_MAX_PROFILES + p) * 256;
+    const uint32_t wm = (1u << a.width[t]) - 1u;
+    uint32_t busy = 0, first = kInf;
+    for (uint32_t g = lane; g < c; g += 32) {
+        const uint32_t o = sh.live[b0 + g];
+        busy += __popc(o & wm);
+        if (__ldg(a.lut + row + o) != ISL_START_NONE) first = min(first, g);
+    }
+    busy = __reduce_add_sync(0xFFFFFFFFu, busy);
+    first = redux_min_u32(first);
+    return nodefit_leaf(first != kInf, busy, a.width[t] * c, __ldg(a.sizes + t * ISL_MAX_PROFILES + p), a.most, sh.base + b0 + first);
+}
 
 // Warp-wide, on a warp of the CTA that owns node j: commit the ALLOC members of requests [r, r1) on the node's live bytes (they stop by
 // themselves where the evaluation on the scratch copy stopped).
@@ -2794,8 +2825,12 @@ __device__ void gangfew_undo(const GangNodeArgs& a, const NodeShare& sh, const D
 // kMin (k_ganglocal<kLocPerGang, true>, M3): a gang that fails at ALLOC member f >= min_m commits its first f members instead of aborting.
 // One node: f is the deepest failure's depth D, and the owner of the first node that reaches it replays the members on its live bytes,
 // which stop at D by themselves (the scratch copy started from the same bytes).  Few nodes: f is the members the earlier rounds placed.
-template <bool kFew, bool kMin = false>
-__device__ __forceinline__ void gangnode_gang(const GangNodeArgs& a, const DevProfiles& prof, const NodeShare& sh, uint32_t r0, uint32_t r1,
+// kScore (one node on an ISL_FLAG_GANG_NODE_SCORE engine, 4.16, N5): a node that takes the gang also counts its busy slices under its
+// table's width (a second pass over its bytes), and its key is (100 - score(N, s_need[t])) << 32 | node, the gang scored as one pod;
+// bit 63 stays clear, so every success still sorts before every failure.  Pass 0's filter stays valid: a node it skips cannot take the
+// gang.
+template <bool kFew, bool kMin = false, bool kScore = false, class Args = GangNodeArgs>
+__device__ __forceinline__ void gangnode_gang(const Args& a, const DevProfiles& prof, const NodeShare& sh, uint32_t r0, uint32_t r1,
                                               uint32_t& parity, uint32_t& placed, unsigned long long* s_warp, unsigned long long* s_win,
                                               uint32_t* s_need, uint32_t* s_allocs, uint32_t tid, uint32_t lane, uint32_t warp,
                                               uint32_t min_m = 0) {
@@ -2834,7 +2869,15 @@ __device__ __forceinline__ void gangnode_gang(const GangNodeArgs& a, const DevPr
                 free_slices = __reduce_add_sync(0xFFFFFFFFu, free_slices);
                 if (pass == 0 && free_slices < s_need[t]) continue;
                 const uint32_t d = gangnode_resolve(a, prof, scr + b0, c, a.lo + sh.base + b0, t, ri, r1, false, lane);
-                best = min(best, d == allocs ? (unsigned long long)j : gn_fail_key(d, j));
+                if constexpr (kScore) {     // the node's busy slices under its width on the live bytes, before the gang
+                    uint32_t busy = 0;
+                    for (uint32_t g = lane; g < c; g += 32) busy += __popc(sh.live[b0 + g] & ((1u << a.width[t]) - 1u));
+                    busy = __reduce_add_sync(0xFFFFFFFFu, busy);
+                    const unsigned long long score = nodefit_leaf(1u, busy, a.width[t] * c, s_need[t], a.most, 0u) >> 24;     // 100 - score
+                    best = min(best, d == allocs ? score << 32 | j : gn_fail_key(d, j));
+                } else {
+                    best = min(best, d == allocs ? (unsigned long long)j : gn_fail_key(d, j));
+                }
             }
             win = grid_min<kGnThreads>(best, a.keys, parity, s_warp, s_win);
             if (!(win & kGnFail)) break;                    // a node takes the whole gang: the skipped nodes could not have come first
@@ -2899,8 +2942,9 @@ __device__ __forceinline__ void gangnode_gang(const GangNodeArgs& a, const DevPr
 // this gang wrote it.  `dead`: profiles no GPU of the partition admits any more.  The shared words are the kernel's: s_warp and s_win for
 // grid_min, and the size of the CTA's stack of wins, which is 0 between gangs.  kMin (k_ganglocal<kLocPerGang, true>, M3): a member that
 // finds no GPU at rank fail >= min_m commits the stack of wins, which holds the members before it, as a success does.
-template <bool kMin = false>
-__device__ __forceinline__ void gangspread_gang(const GangNodeArgs& a, const DevProfiles& prof, const NodeShare& sh, uint2* wins, uint32_t r0,
+// kScore (ISL_FLAG_GANG_NODE_SCORE, 4.16, N4): choose takes gangscore_node's key, one warp per unmarked node of the share.
+template <bool kMin = false, bool kScore = false, class Args = GangNodeArgs>
+__device__ __forceinline__ void gangspread_gang(const Args& a, const DevProfiles& prof, const NodeShare& sh, uint2* wins, uint32_t r0,
                                                 uint32_t r1, uint32_t tag, uint32_t& parity, uint32_t& placed, uint32_t& dead,
                                                 uint32_t* s_warp, uint32_t* s_win, uint32_t* s_nwins, uint32_t tid, uint32_t lane,
                                                 uint32_t warp, uint32_t min_m = 0) {
@@ -2915,11 +2959,15 @@ __device__ __forceinline__ void gangspread_gang(const GangNodeArgs& a, const Dev
         uint32_t win = kInf;                                // an unknown or dead profile fails without a barrier: every CTA knows it
         if (p < prof.n && !((dead >> p) & 1u)) {
             uint32_t key = kInf;
-            for (uint32_t g = tid; g < cnt; g += kGnThreads) {
-                if (mark[g] == tag) continue;
-                const uint32_t o = sh.live[g], t = a.n_tables > 1 ? a.gtab[a.lo + base + g] & (kMaxTables - 1) : 0u;
-                const uint32_t row = (t * ISL_MAX_PROFILES + p) * 256;
-                if (__ldg(a.lut + row + o) != ISL_START_NONE) key = min(key, ((uint32_t)__ldg(a.score + row + o) << 24) | (base + g));
+            if constexpr (kScore) {
+                for (uint32_t j = sh.j0 + warp; j < sh.j1; j += kGnThreads / 32) key = min(key, gangscore_node(a, sh, j, p, mark, tag, lane));
+            } else {
+                for (uint32_t g = tid; g < cnt; g += kGnThreads) {
+                    if (mark[g] == tag) continue;
+                    const uint32_t o = sh.live[g], t = a.n_tables > 1 ? a.gtab[a.lo + base + g] & (kMaxTables - 1) : 0u;
+                    const uint32_t row = (t * ISL_MAX_PROFILES + p) * 256;
+                    if (__ldg(a.lut + row + o) != ISL_START_NONE) key = min(key, ((uint32_t)__ldg(a.score + row + o) << 24) | (base + g));
+                }
             }
             win = grid_min<kGnThreads>(key, a.keys, parity, s_warp, s_win);
             if (win == kInf && rank == 0) dead |= 1u << p;
@@ -2960,8 +3008,10 @@ __device__ __forceinline__ void gangspread_gang(const GangNodeArgs& a, const Dev
 // tentative members on its own nodes (gangfew_undo), and CTA 0 reports the members after the failing one GANG_ABORTED.  An unknown or
 // dead profile fails without a barrier: gangfew_undo only touches records on the CTA's own nodes, which that CTA wrote itself.
 // kMin (k_ganglocal<kLocPerGang, true>, M3): a member with no GPU at rank >= min_m keeps the tentative members, which then commit.
-template <bool kMin = false>
-__device__ __forceinline__ void ganglocal_any(const GangNodeArgs& a, const DevProfiles& prof, const NodeShare& sh, uint32_t r0, uint32_t r1,
+// kScore (ISL_FLAG_GANG_NODE_SCORE, 4.16, N3): the key is gangscore_node's, one warp per node of the share, on the live bytes, so each
+// member sees the gang's tentative members in its nodes' busy slices.  No per-node state outlives a member, so gangfew_undo is unchanged.
+template <bool kMin = false, bool kScore = false, class Args = GangNodeArgs>
+__device__ __forceinline__ void ganglocal_any(const Args& a, const DevProfiles& prof, const NodeShare& sh, uint32_t r0, uint32_t r1,
                                               uint32_t& parity, uint32_t& placed, uint32_t& dead, uint32_t* s_warp, uint32_t* s_win,
                                               uint32_t tid, uint32_t lane, uint32_t warp, uint32_t min_m = 0) {
     const uint32_t base = sh.base, cnt = sh.cnt;
@@ -2973,10 +3023,14 @@ __device__ __forceinline__ void ganglocal_any(const GangNodeArgs& a, const DevPr
         uint32_t win = kInf;
         if (p < prof.n && !((dead >> p) & 1u)) {
             uint32_t key = kInf;
-            for (uint32_t g = tid; g < cnt; g += kGnThreads) {
-                const uint32_t o = sh.live[g], t = a.n_tables > 1 ? a.gtab[a.lo + base + g] & (kMaxTables - 1) : 0u;
-                const uint32_t row = (t * ISL_MAX_PROFILES + p) * 256;
-                if (__ldg(a.lut + row + o) != ISL_START_NONE) key = min(key, ((uint32_t)__ldg(a.score + row + o) << 24) | (base + g));
+            if constexpr (kScore) {
+                for (uint32_t j = sh.j0 + warp; j < sh.j1; j += kGnThreads / 32) key = min(key, gangscore_node(a, sh, j, p, nullptr, 0u, lane));
+            } else {
+                for (uint32_t g = tid; g < cnt; g += kGnThreads) {
+                    const uint32_t o = sh.live[g], t = a.n_tables > 1 ? a.gtab[a.lo + base + g] & (kMaxTables - 1) : 0u;
+                    const uint32_t row = (t * ISL_MAX_PROFILES + p) * 256;
+                    if (__ldg(a.lut + row + o) != ISL_START_NONE) key = min(key, ((uint32_t)__ldg(a.score + row + o) << 24) | (base + g));
+                }
             }
             win = grid_min<kGnThreads>(key, a.keys, parity, s_warp, s_win);
             if (win == kInf && rank == 0) dead |= 1u << p;  // no tentative slice of this gang is in the way
@@ -3025,10 +3079,15 @@ __device__ __forceinline__ void ganglocal_any(const GangNodeArgs& a, const DevPr
 // writes the PLACED records on it and rewrites its own tentative ones GANG_ABORTED when the gang aborts (gangfew_undo); CTA 0 writes
 // GANG_ABORTED or GANG_TRIMMED for the other members, except the one that stopped the gang, which keeps k_prepare's NO_CAPACITY or
 // BAD_PROFILE record.
+// kScore (an ISL_FLAG_GANG_NODE_SCORE engine, 4.16; kLoc ISL_GANG_ANY_NODES, _ONE_NODE, _DISTINCT_NODES or kLocPerGang, never with kMin):
+// the bodies put the node score in their keys, and `a` carries the widths and the policy (GangScoreArgs).  The host refuses a few-node
+// byte on such an engine, so its few-node branch is never taken.
 // ---------------------------------------------------------------------------------------------
 constexpr uint32_t kLocPerGang = 4;
-template <uint32_t kLoc, bool kMin = false>
-__global__ void __launch_bounds__(kGnThreads, 1) k_ganglocal(GangNodeArgs a, DevProfiles prof, uint2* wins, const uint8_t* __restrict__ locality) {
+template <uint32_t kLoc, bool kMin = false, bool kScore = false>
+__global__ void __launch_bounds__(kGnThreads, 1) k_ganglocal(std::conditional_t<kScore, GangScoreArgs, GangNodeArgs> a, DevProfiles prof, uint2* wins,
+                                                             const uint8_t* __restrict__ locality) {
+    static_assert(!(kScore && kMin), "elastic gangs are not node-scored");
     extern __shared__ __align__(16) uint8_t gl_smem[];
     __shared__ unsigned long long s_warp64[kGnThreads / 32];
     __shared__ unsigned long long s_win64;
@@ -3043,15 +3102,16 @@ __global__ void __launch_bounds__(kGnThreads, 1) k_ganglocal(GangNodeArgs a, Dev
         const uint32_t min_m = kMin ? __ldg(reinterpret_cast<const uint32_t*>(locality + ((a.n_gangs + 3u) & ~3u)) + gi) : 0u;
         if (loc == ISL_GANG_ONE_NODE || loc == ISL_GANG_FEW_NODES) {
             if (loc == ISL_GANG_ONE_NODE)
-                gangnode_gang<false, kMin>(a, prof, sh, r0, r1, parity, placed, s_warp64, &s_win64, s_need, &s_allocs, tid, lane, warp, min_m);
+                gangnode_gang<false, kMin, kScore>(a, prof, sh, r0, r1, parity, placed, s_warp64, &s_win64, s_need, &s_allocs, tid, lane, warp,
+                                                   min_m);
             else gangnode_gang<true, kMin>(a, prof, sh, r0, r1, parity, placed, s_warp64, &s_win64, s_need, &s_allocs, tid, lane, warp, min_m);
             spread = 0;                                     // the scratch copies overwrote the marks
         } else if (loc == ISL_GANG_DISTINCT_NODES) {
-            gangspread_gang<kMin>(a, prof, sh, wins, r0, r1, 1u + spread % 255u, parity, placed, dead, s_warp32, &s_win32, &s_nwins, tid, lane,
-                                  warp, min_m);
+            gangspread_gang<kMin, kScore>(a, prof, sh, wins, r0, r1, 1u + spread % 255u, parity, placed, dead, s_warp32, &s_win32, &s_nwins, tid,
+                                          lane, warp, min_m);
             ++spread;
         } else {
-            ganglocal_any<kMin>(a, prof, sh, r0, r1, parity, placed, dead, s_warp32, &s_win32, tid, lane, warp, min_m);
+            ganglocal_any<kMin, kScore>(a, prof, sh, r0, r1, parity, placed, dead, s_warp32, &s_win32, tid, lane, warp, min_m);
         }
     }
     if (tid == 0 && placed) count_placed(a.ctrl, placed);

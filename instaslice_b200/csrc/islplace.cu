@@ -26,7 +26,7 @@ static constexpr uint32_t kSpecRingIds = 1u << 24;     // stream ids of isl_plac
 
 // Engines created with one of these flags place gangs with k_ganglocal, the others with k_bestfit's gang loop.
 constexpr uint32_t kGangTopologyFlags = ISL_FLAG_GANG_ONE_NODE | ISL_FLAG_GANG_FEW_NODES | ISL_FLAG_GANG_DISTINCT_NODES |
-                                        ISL_FLAG_GANG_LOCALITY | ISL_FLAG_GANG_MIN_MEMBERS;
+                                        ISL_FLAG_GANG_LOCALITY | ISL_FLAG_GANG_MIN_MEMBERS | ISL_FLAG_GANG_NODE_SCORE;
 
 // The instantiations of k_ganglocal, one per kind of gang-topology engine (gang_kind), with the name a launch error carries; wins:
 // distinct-node gangs may run, which stack their wins in GangNode::wins.
@@ -35,18 +35,26 @@ struct GangKernel {
     const char* name;
     bool wins;
 };
-constexpr uint32_t kGangKinds = 5;
+constexpr uint32_t kGangKinds = 9;
 const GangKernel kGangKernels[kGangKinds] = {
     {(const void*)k_ganglocal<ISL_GANG_ONE_NODE>, "k_ganglocal<one_node>", false},
     {(const void*)k_ganglocal<ISL_GANG_FEW_NODES>, "k_ganglocal<few_nodes>", false},
     {(const void*)k_ganglocal<ISL_GANG_DISTINCT_NODES>, "k_ganglocal<distinct_nodes>", true},
     {(const void*)k_ganglocal<kLocPerGang, false>, "k_ganglocal<per_gang>", true},
     {(const void*)k_ganglocal<kLocPerGang, true>, "k_ganglocal<per_gang, min_members>", true},
+    {(const void*)k_ganglocal<ISL_GANG_ANY_NODES, false, true>, "k_ganglocal<any_node, node_score>", false},
+    {(const void*)k_ganglocal<ISL_GANG_ONE_NODE, false, true>, "k_ganglocal<one_node, node_score>", false},
+    {(const void*)k_ganglocal<ISL_GANG_DISTINCT_NODES, false, true>, "k_ganglocal<distinct_nodes, node_score>", true},
+    {(const void*)k_ganglocal<kLocPerGang, false, true>, "k_ganglocal<per_gang, node_score>", true},
 };
 
 // The kGangKernels entry of an engine with a gang-topology flag: each gang's own byte under ISL_FLAG_GANG_LOCALITY, and under
-// ISL_FLAG_GANG_MIN_MEMBERS with its minimum as well, else the locality of the engine's flag for every gang.
+// ISL_FLAG_GANG_MIN_MEMBERS with its minimum as well, else the locality of the engine's flag for every gang.  An
+// ISL_FLAG_GANG_NODE_SCORE engine (never with elastic or few-node gangs) takes the node-scored instantiation of its locality, any node
+// without a locality flag.
 uint32_t gang_kind(uint32_t flags) {
+    if (flags & ISL_FLAG_GANG_NODE_SCORE)
+        return (flags & ISL_FLAG_GANG_LOCALITY) ? 8 : (flags & ISL_FLAG_GANG_ONE_NODE) ? 6 : (flags & ISL_FLAG_GANG_DISTINCT_NODES) ? 7 : 5;
     if (flags & ISL_FLAG_GANG_MIN_MEMBERS) return 4;
     if (flags & ISL_FLAG_GANG_LOCALITY) return 3;
     return (flags & ISL_FLAG_GANG_ONE_NODE) ? 0 : (flags & ISL_FLAG_GANG_FEW_NODES) ? 1 : 2;
@@ -535,10 +543,12 @@ int run_ganglocal(isl_engine* e, uint32_t kind, uint32_t n_gangs, const uint32_t
                   const uint2* d_in, uint2* d_out) {
     const GangKernel& k = kGangKernels[kind];
     if (int rc = prepare_batch(e, n, d_in, d_out)) return rc;
-    GangNodeArgs a;
+    GangScoreArgs a;            // the node-scored instantiations read all of it, the others its GangNodeArgs part
     uint32_t grid, nodes;
     size_t smem;
     if (int rc = gang_layout(e, k.fn, e->gn.optin[kind], 2, n_gangs, d_gang_off, d_in, d_out, a, &grid, &smem, &nodes)) return rc;
+    memcpy(a.width, e->nf.width, sizeof a.width);
+    a.most = e->cfg.policy == ISL_POLICY_MOST_ALLOCATED;
     if (!smem) ISL_CUDA(e, e->gn.scratch.reserve(e->hi - e->lo));     // the second byte per GPU; the live bytes are the occupancy
     a.scratch = e->gn.scratch;
     if (k.wins) ISL_CUDA(e, e->gn.wins.reserve(nodes));
@@ -1174,18 +1184,25 @@ int isl_create(const isl_config* cfg, isl_engine** out) {
     if (cfg->max_gpus == 0 || cfg->max_gpus > ISL_MAX_GPUS || cfg->max_batch == 0) return ISL_EINVAL;
     if (cfg->policy > ISL_POLICY_LEAST_ALLOCATED) return ISL_EINVAL;
     if (node_scoring(cfg->policy) && (cfg->flags & ISL_FLAG_ALL_NODES)) return ISL_EINVAL;     // a pod on every node: no node to choose
-    // one-node gangs choose the node by scan order: not with a pod on every node, nor with a policy that scores the nodes
-    if ((cfg->flags & ISL_FLAG_GANG_ONE_NODE) && ((cfg->flags & ISL_FLAG_ALL_NODES) || node_scoring(cfg->policy))) return ISL_EINVAL;
-    // distinct-node gangs: the opposite of one-node gangs, and, like them, not with a pod on every node nor with node scoring
+    // node-scored gangs (N1): only under node scoring, not with few-node or elastic gangs; they lift the locality flags' refusal of node
+    // scoring below.  A pod on every node is refused by node scoring itself.
+    const bool gang_score = cfg->flags & ISL_FLAG_GANG_NODE_SCORE;
+    if (gang_score && (!node_scoring(cfg->policy) || (cfg->flags & (ISL_FLAG_GANG_FEW_NODES | ISL_FLAG_GANG_MIN_MEMBERS)))) return ISL_EINVAL;
+    const bool scored_gangs_refused = node_scoring(cfg->policy) && !gang_score;
+    // one-node gangs choose the node by scan order: not with a pod on every node, nor with a policy that scores the nodes unless the
+    // node score chooses it (N1)
+    if ((cfg->flags & ISL_FLAG_GANG_ONE_NODE) && ((cfg->flags & ISL_FLAG_ALL_NODES) || scored_gangs_refused)) return ISL_EINVAL;
+    // distinct-node gangs: the opposite of one-node gangs, and, like them, not with a pod on every node nor unscored under node scoring
     if ((cfg->flags & ISL_FLAG_GANG_DISTINCT_NODES) &&
-        ((cfg->flags & (ISL_FLAG_GANG_ONE_NODE | ISL_FLAG_ALL_NODES)) || node_scoring(cfg->policy))) return ISL_EINVAL;
+        ((cfg->flags & (ISL_FLAG_GANG_ONE_NODE | ISL_FLAG_ALL_NODES)) || scored_gangs_refused)) return ISL_EINVAL;
     // few-node gangs: a third locality mode, exclusive with the other two, and, like them, not with a pod on every node nor node scoring
     if ((cfg->flags & ISL_FLAG_GANG_FEW_NODES) &&
         ((cfg->flags & (ISL_FLAG_GANG_ONE_NODE | ISL_FLAG_GANG_DISTINCT_NODES | ISL_FLAG_ALL_NODES)) || node_scoring(cfg->policy))) return ISL_EINVAL;
-    // per-gang locality: the gangs name the locality the other three flags fix for the engine; not with a pod on every node nor node scoring
+    // per-gang locality: the gangs name the locality the other three flags fix for the engine; not with a pod on every node nor unscored
+    // under node scoring
     if ((cfg->flags & ISL_FLAG_GANG_LOCALITY) &&
         ((cfg->flags & (ISL_FLAG_GANG_ONE_NODE | ISL_FLAG_GANG_DISTINCT_NODES | ISL_FLAG_GANG_FEW_NODES | ISL_FLAG_ALL_NODES)) ||
-         node_scoring(cfg->policy))) return ISL_EINVAL;
+         scored_gangs_refused)) return ISL_EINVAL;
     // elastic gangs (M6): with any one locality flag or none (their own checks refuse two), not with a pod on every node nor node scoring
     if ((cfg->flags & ISL_FLAG_GANG_MIN_MEMBERS) && ((cfg->flags & ISL_FLAG_ALL_NODES) || node_scoring(cfg->policy))) return ISL_EINVAL;
     // gang preemption (P7): few-node and elastic gangs have no preemption order, a pod on every node has no single GPU to evict on
@@ -1557,6 +1574,8 @@ int isl_place_gangs(isl_engine* e, uint32_t n_gangs, const uint32_t* gang_off, c
             for (uint32_t r = gang_off[i]; r < gang_off[i + 1]; ++r) {
                 if (in[r].op != ISL_OP_ALLOC) continue;
                 if (in[r].start > ISL_GANG_DISTINCT_NODES || (named && in[r].start != locality[i])) return ISL_EINVAL;
+                // N6: few-node gangs are not node-scored
+                if ((e->cfg.flags & ISL_FLAG_GANG_NODE_SCORE) && in[r].start == ISL_GANG_FEW_NODES) return ISL_EINVAL;
                 locality[i] = in[r].start;
                 named = true;
             }
@@ -1582,7 +1601,8 @@ int isl_place_gangs(isl_engine* e, uint32_t n_gangs, const uint32_t* gang_off, c
         }
     }
     if (e->cfg.flags & ISL_FLAG_ALL_NODES) return ISL_EINVAL;      // one pod on every node with capacity: no all-or-nothing meaning
-    if (node_scoring(e->cfg.policy)) return ISL_EINVAL;            // gangs under node scoring are not implemented
+    // gangs under node scoring only on an ISL_FLAG_GANG_NODE_SCORE engine
+    if (node_scoring(e->cfg.policy) && !(e->cfg.flags & ISL_FLAG_GANG_NODE_SCORE)) return ISL_EINVAL;
     if (n > e->cfg.max_batch) return ISL_ERANGE;
     Entry guard(e, Needs::ready, n);
     if (guard.rc) return guard.rc;

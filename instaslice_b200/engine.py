@@ -37,6 +37,7 @@ FLAG_GANG_FEW_NODES = 256  # isl_place_gangs puts a gang on one node when one ta
 FLAG_GANG_LOCALITY = 512  # isl_place_gangs takes each gang's node locality from its ALLOC members' start byte (GANG_*)
 FLAG_GANG_MIN_MEMBERS = 1024  # elastic gangs: a gang commits its leading members once they reach its minimum (the ALLOC size byte)
 FLAG_GANG_PREEMPT = 2048  # isl_preempt picks the victims a whole gang (a run of equal handles) needs, or evicts nothing for it
+FLAG_GANG_NODE_SCORE = 4096  # on a node-scoring engine isl_place_gangs places gangs by MostAllocated / LeastAllocated (N1-N8)
 GANG_ANY_NODES, GANG_ONE_NODE, GANG_FEW_NODES, GANG_DISTINCT_NODES = 0, 1, 2, 3     # node locality of one gang (include/islplace.h L1)
 SPEC_AUTO, SPEC_OFF, SPEC_ON = 0, 1, 2
 
@@ -357,7 +358,13 @@ class Engine:
         ALLOC member f and f reaches the gang's minimum m' (the ``size`` byte m of its ALLOC members; m' = m for 0 < m < k, else every
         one of its k members), the first f members are placed, member f keeps its record and the members after it report
         ``ST_GANG_TRIMMED`` (include/islplace.h M1-M7).  ``min_members``: one m in 0..255 per gang, written into the ``size`` of the
-        ALLOC members of a copy of ``requests``; it needs an engine created with the flag."""
+        ALLOC members of a copy of ``requests``; it needs an engine created with the flag.
+
+        On a ``POLICY_MOST_ALLOCATED`` or ``POLICY_LEAST_ALLOCATED`` engine created with ``FLAG_GANG_NODE_SCORE`` the gangs are placed by
+        the node score (include/islplace.h N1-N8): any-node and distinct-node members one by one, each on the best-scored node that admits
+        it (ties to the lowest node) and there on its first admitting GPU; a one-node gang on the node that takes it whole with the best
+        score for the gang's slices taken as one pod.  Its locality is ``FLAG_GANG_ONE_NODE``, ``FLAG_GANG_DISTINCT_NODES``, each gang's
+        own under ``FLAG_GANG_LOCALITY`` (``GANG_FEW_NODES`` is refused), or any node."""
         requests = np.ascontiguousarray(requests, dtype=REQUEST_DTYPE)
         gang_off = np.ascontiguousarray(gang_off, dtype=np.uint32)
         if len(gang_off) == 0 or int(gang_off[-1]) != len(requests):
@@ -368,6 +375,8 @@ class Engine:
             locality = np.asarray(locality, dtype=np.int64)
             if len(locality) != len(gang_off) - 1:
                 raise ValueError("one locality per gang")
+            if self.flags & FLAG_GANG_NODE_SCORE and (locality == GANG_FEW_NODES).any():
+                raise ValueError("few-node gangs are not node-scored (FLAG_GANG_NODE_SCORE)")
             requests = requests.copy()
             per_request = np.repeat(locality, np.diff(gang_off.astype(np.int64)))
             alloc = requests["op"] == OP_ALLOC

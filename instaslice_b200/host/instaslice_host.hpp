@@ -98,7 +98,8 @@ public:
     // PlaceGangs puts every gang on one node, ISL_FLAG_GANG_DISTINCT_NODES so that it puts every member of a gang on a different node,
     // ISL_FLAG_GANG_FEW_NODES so that it puts a gang on one node when one takes it and on as few nodes as it greedily can otherwise, or
     // ISL_FLAG_GANG_LOCALITY so that PlaceGangs takes one of these localities per gang; ISL_FLAG_GANG_MIN_MEMBERS (alone or with one of
-    // the four) so that PlaceGangs takes a minimum per gang
+    // the four) so that PlaceGangs takes a minimum per gang; with a node-scoring policy, ISL_FLAG_GANG_NODE_SCORE (alone or with the
+    // one-node, distinct-node or locality flag) so that PlaceGangs places gangs by the node score
     explicit InstasliceReconciler(uint32_t quirks = ISL_QUIRKS_REF_EXACT, uint32_t max_gpus = 1u << 16, uint32_t max_batch = 1u << 16,
                                   uint32_t policy = ISL_POLICY_FIRST_FIT, uint32_t flags = 0);
     ~InstasliceReconciler();

@@ -80,6 +80,9 @@ const (
 	// PreemptPendingGangs picks the victims of whole gangs, or none for a gang that still cannot run.  Alone or with FlagGangOneNode,
 	// FlagGangDistinctNodes or FlagGangLocality; not with FlagGangFewNodes or FlagGangMinMembers.
 	FlagGangPreempt = uint32(C.ISL_FLAG_GANG_PREEMPT)
+	// On a PolicyMostAllocated or PolicyLeastAllocated engine, PlaceGangs places gangs by the node score: alone (any node) or with
+	// FlagGangOneNode, FlagGangDistinctNodes or FlagGangLocality (no few-node locality); not with FlagGangFewNodes or FlagGangMinMembers.
+	FlagGangNodeScore = uint32(C.ISL_FLAG_GANG_NODE_SCORE)
 )
 
 // StGangTrimmed is the record status of a pod its elastic gang was placed without (isl_result.status, FlagGangMinMembers).
