@@ -159,11 +159,14 @@ typedef struct isl_config {
                                         needs, or evicts nothing for it (see isl_preempt, P1-P8); every other call is unchanged */
 #define ISL_FLAG_GANG_NODE_SCORE 4096u  /* on a node-scoring engine isl_place_gangs places gangs by MostAllocated or LeastAllocated (see
                                            isl_place_gangs, N1-N8); every other call is unchanged */
+#define ISL_FLAG_GANG_BALANCED 8192u  /* with ISL_FLAG_GANG_LOCALITY: a locality byte of 4..255 spreads a gang's members over the nodes
+                                         within a maxSkew of byte - 3 (see isl_place_gangs, B1-B8); every other call is unchanged */
 /* Node locality of one gang on an ISL_FLAG_GANG_LOCALITY engine (isl_request.start of its ALLOC members, rules L1-L6) */
 #define ISL_GANG_ANY_NODES      0u  /* rules 2-4: members anywhere, as on an engine without a gang flag */
 #define ISL_GANG_ONE_NODE       1u  /* G2-G3: every member on one node */
 #define ISL_GANG_FEW_NODES      2u  /* F2-F3: one node when one takes the gang, else as few nodes as it greedily can */
 #define ISL_GANG_DISTINCT_NODES 3u  /* S2-S4: every member on a different node */
+#define ISL_GANG_BALANCED_NODES(max_skew) (3u + (max_skew))  /* B1-B8, ISL_FLAG_GANG_BALANCED: max_skew 1..252 */
 
 /* One Migplacement row (api/v1alpha1/instaslice_types.go:23-29).  `size` is
  * Placements[0].Size (:334); `starts` is [p.Start for p in Placements] in CRD
@@ -487,6 +490,48 @@ int  isl_place_batch_range(isl_engine* e, uint32_t lo, uint32_t hi, uint32_t n, 
  *       any node        MOST: GPU 1 start 6 (87 against 12 and 62), then GPU 2 start 4 (node 1, now 0x7F, admits no 1g.10gb).
  *                       LEAST: GPU 0 starts 0 then 1.
  *       distinct nodes  MOST: as any node.  LEAST: GPU 0 start 0, then GPU 2 start 4 (node 0 is used; 37 against node 1's 12).
+ *
+ * Balanced gangs (ISL_FLAG_GANG_BALANCED): the replicas of a deployment spread over the nodes for availability, but more of them than
+ * there are nodes (Kubernetes' topologySpreadConstraints with maxSkew k on kubernetes.io/hostname, which never applies to gated MIG
+ * pods).  Any-node gangs pack them onto the first GPU with room, and distinct-node gangs abort once every node holds one.  On an engine
+ * created with the flag:
+ *   B1. The flag is valid only with ISL_FLAG_GANG_LOCALITY.  An ALLOC member's `start` byte b of 4..255 makes its gang a balanced gang
+ *       with maxSkew k = b - 3 (1..252; ISL_GANG_BALANCED_NODES(k)).  Bytes 0..3 keep L1's meaning, and two ALLOC members of one gang
+ *       with different bytes are ISL_EINVAL (L4).  Without the flag L4 is unchanged: a byte above 3 is ISL_EINVAL.
+ *   B2. Rules 1, 3 and 5 hold, and so does L2's order across localities.  A balanced gang's ALLOC members are resolved in order, each
+ *       seeing the gang's earlier members as tentative slices (rules 2-4); two members may share a GPU.  For a member of profile p,
+ *       cnt(N) is the number of earlier ALLOC members of the same gang placed on node N, A is the set of the partition's nodes with a GPU
+ *       inside the partition whose current byte admits p under the start search of the node's table, and mu = the least cnt over A.  The
+ *       candidates are the admitting GPUs of the nodes N of A with cnt(N) <= mu + k - 1, and the engine's policy picks among them:
+ *       first-fit the first in ascending canonical order, right-to-left the last, best-fit and min-frag the minimum of their score with
+ *       ties to scan order.  The start is the start search's.  A node the partition cuts counts as one node and offers only its GPUs
+ *       inside the partition, as in S2.
+ *   B3. Failure is rule 4: the first member with no admitting GPU anywhere in the partition keeps its NO_CAPACITY or BAD_PROFILE record,
+ *       every other ALLOC member reports ISL_ST_GANG_ABORTED, and the occupancy is what it was before the gang.  The skew never causes a
+ *       failure: a node at mu always qualifies.
+ *   B4. Consequences: (a) a gang that commits whole with byte 3 gets the same records with byte 4 (k = 1): while an unused admitting node
+ *       exists, mu = 0 and the candidates are S2's; (b) byte 3 + k with k >= the gang's ALLOC members equals byte 0; (c) on a one-node
+ *       inventory, or a partition inside one node, every balanced byte equals byte 0; (d) gangs of one equal byte 0, and under FIRST_FIT
+ *       and RIGHT_TO_LEFT isl_place_batch; (e) L3 (b) extends: a call equals its gangs run one at a time; (f) with k = 1, on an inventory
+ *       where every node admits every member until the gang ends, the final per-node counts differ by at most 1.
+ *   B5. Elastic gangs: with ISL_FLAG_GANG_MIN_MEMBERS, M3 applies member by member, as for S: with f the rank of the first member with
+ *       no admitting GPU, the gang commits its leading f members when f >= m'.
+ *   B6. isl_create: ISL_EINVAL for the flag without ISL_FLAG_GANG_LOCALITY, with a node-scoring policy (hence with
+ *       ISL_FLAG_GANG_NODE_SCORE) or with ISL_FLAG_ALL_NODES.  ISL_FLAG_GANG_PREEMPT may come with it; isl_preempt keeps P1, which refuses
+ *       bytes above 3, so no balanced gang is preempted for.  isl_place_gangs keeps every other code, the 2^20-GPU partition cap
+ *       included.  Every other entry point returns exactly what it returns without the flag.
+ *   B7. The choice is greedy, member by member (as S4 and F5): list the larger members first.
+ *   B8. Deliberate difference from PodTopologySpread: mu is taken over the nodes that still admit the member, not over every node (a
+ *       full node would otherwise hold the minimum at its count, and DoNotSchedule would refuse every later member elsewhere); and the
+ *       counts are within the gang: replicas placed by earlier calls are not counted, as S2 ignores them.
+ *   Example, H100-80GB rows, either quirk set, two one-GPU nodes with bytes 0x00 and 0x00, a gang of four 1g.10gb, records (gpu, start):
+ *       byte 0        first-fit (0,0) (0,1) (0,2) (0,3)
+ *       byte 3        member 2 NO_CAPACITY, members 0, 1 and 3 GANG_ABORTED (they had reached (0,0) and (1,0))
+ *       byte 4 (k 1)  first-fit (0,0) (1,0) (0,1) (1,1); right-to-left (1,0) (0,0) (1,1) (0,1)
+ *       byte 5 (k 2)  first-fit (0,0) (0,1) (1,0) (0,2)
+ *       byte 7 (k 4)  equals byte 0
+ *   B8's case: three one-GPU nodes with bytes 0x00, 0x7F and 0x00, a gang of three 1g.10gb, byte 4, first-fit: (0,0) (2,0) (0,1).  Start
+ *       7 is not legal, so node 1 is not in A; a minimum over every node would stay at node 1's 0 and refuse member 2.
  */
 int  isl_place_gangs(isl_engine* e, uint32_t n_gangs, const uint32_t* gang_off, const isl_request* in, isl_result* out);
 

@@ -99,7 +99,7 @@ class InstasliceReconciler:
     def __init__(self, instaslices: list, quirks: int = E.QUIRKS_REF_EXACT, max_batch: int = 65536, engine: E.Engine | None = None,
                  policy: int = E.POLICY_FIRST_FIT, gang_one_node: bool = False, gang_distinct_nodes: bool = False,
                  gang_few_nodes: bool = False, gang_locality: bool = False, gang_min_members: bool = False, gang_preempt: bool = False,
-                 gang_node_score: bool = False):
+                 gang_node_score: bool = False, gang_balanced: bool = False):
         """``policy``: the engine policy of the engine this reconciler creates (``engine`` is None), e.g. ``E.POLICY_MOST_ALLOCATED`` to
         pack MIG pods onto the fullest nodes or ``E.POLICY_LEAST_ALLOCATED`` to spread them (include/islplace.h).  ``gang_one_node``:
         that engine is created with ``E.FLAG_GANG_ONE_NODE``, so ``place_pending_gangs`` puts every gang on one node.
@@ -112,7 +112,9 @@ class InstasliceReconciler:
         one-node, distinct-node or locality flag), so ``preempt_pending_gangs`` picks the victims of whole gangs.  ``gang_node_score``:
         with ``E.FLAG_GANG_NODE_SCORE``, for a ``POLICY_MOST_ALLOCATED`` or ``POLICY_LEAST_ALLOCATED`` reconciler, so that
         ``place_pending_gangs`` places gangs by the node score, alone (any node) or with the one-node, distinct-node or locality option
-        (the engine refuses it with any other policy, few-node gangs and elastic gangs)."""
+        (the engine refuses it with any other policy, few-node gangs and elastic gangs).  ``gang_balanced``: with
+        ``E.FLAG_GANG_BALANCED``, which needs ``gang_locality``, so that a gang's locality may be ``E.gang_balanced_nodes(k)``: its
+        replicas spread over the nodes within a maxSkew of k (the engine refuses it under node scoring)."""
         self.quirks = quirks
         self.policy = policy
         self.gang_one_node = gang_one_node
@@ -122,6 +124,7 @@ class InstasliceReconciler:
         self.gang_min_members = gang_min_members
         self.gang_preempt = gang_preempt
         self.gang_node_score = gang_node_score
+        self.gang_balanced = gang_balanced
         self.items = instaslices
         self._engine = engine
         self._max_batch = max_batch
@@ -170,7 +173,8 @@ class InstasliceReconciler:
                                           (E.FLAG_GANG_LOCALITY if self.gang_locality else 0) |
                                           (E.FLAG_GANG_MIN_MEMBERS if self.gang_min_members else 0) |
                                           (E.FLAG_GANG_PREEMPT if self.gang_preempt else 0) |
-                                          (E.FLAG_GANG_NODE_SCORE if self.gang_node_score else 0))
+                                          (E.FLAG_GANG_NODE_SCORE if self.gang_node_score else 0) |
+                                          (E.FLAG_GANG_BALANCED if self.gang_balanced else 0))
         self._engine.load_profile_tables(self.rows)
         self._engine.load_inventory(self.node_off, np.asarray(occ, dtype=np.uint8))
         self._engine.set_node_tables(np.asarray(self.node_table, dtype=np.uint8))
@@ -291,7 +295,9 @@ class InstasliceReconciler:
 
         ``locality``: one ``E.GANG_*`` value per gang (e.g. from Kueue's podset topology annotations, INTEGRATION.md), for a reconciler
         created with ``gang_locality=True``: a training job on one node, replicas on distinct nodes, a job on few nodes and free pods in
-        one call on one occupancy.
+        one call on one occupancy.  With ``gang_balanced=True`` as well, ``E.gang_balanced_nodes(k)`` spreads a Deployment's replicas
+        over the nodes within a maxSkew of k (``topologySpreadConstraints`` on ``kubernetes.io/hostname``), more replicas than nodes
+        included.
 
         ``min_members``: one minimum m (0..255) per gang (the PodGroup's minMember, Volcano's minAvailable or Kueue's PodSet minCount,
         INTEGRATION.md), for a reconciler created with ``gang_min_members=True``.  A gang whose leading pods reach its minimum while a

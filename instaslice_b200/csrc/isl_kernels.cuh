@@ -3055,6 +3055,99 @@ __device__ __forceinline__ void ganglocal_any(const Args& a, const DevProfiles& 
     if (blockIdx.x == 0) placed += rank;                    // the gang commits: CTA 0 counts its members once
 }
 
+// Balanced gangs (ISL_FLAG_GANG_BALANCED, DESIGN.md 4.17): node j of the partition holds wins[j] = (count, tag), the number of ALLOC
+// members of the running gang placed on it, valid only when `tag` is that gang's kBalTag | gang index.  k_ganglocal<.., kBal> clears the
+// words of its nodes once per launch; a distinct-node stack writes a share position, below 2^24, into the second word.  So no count
+// outlives its gang, and none is ever reset.
+constexpr uint32_t kBalTag = 1u << 31;
+__device__ __forceinline__ uint32_t gangbalance_count(const uint2* wins, uint32_t j, uint32_t tag) {
+    const uint2 w = wins[j];
+    return w.y == tag ? w.x : 0u;
+}
+
+// Warp-wide over the nodes of the share this warp visits, over the GPUs that admit p: with lim == kInf the least count << 32 | key, else
+// the least key alone over the nodes whose count is at most lim, where key is ganglocal_any's score << 24 | partition-local storage
+// position; ~0ull when there is none.  (A lane visits many nodes: with the count above a filtered key, its minimum would be the key of
+// its least-count node, not its least key.)
+__device__ __forceinline__ unsigned long long gangbalance_key(const GangNodeArgs& a, const NodeShare& sh, const uint2* wins, uint32_t p,
+                                                             uint32_t tag, uint32_t lim, uint32_t lane, uint32_t warp) {
+    unsigned long long key = ~0ull;
+    for (uint32_t j = sh.j0 + warp; j < sh.j1; j += kGnThreads / 32) {
+        const uint32_t b0 = sh.nb(j) - sh.base, c = sh.nb(j + 1) - sh.base - b0;
+        if (c == 0) continue;
+        const uint32_t n = gangbalance_count(wins, j, tag);
+        if (n > lim) continue;
+        const unsigned long long hi = lim == kInf ? (unsigned long long)n << 32 : 0ull;
+        const uint32_t t = a.n_tables > 1 ? a.gtab[a.lo + sh.base + b0] & (kMaxTables - 1) : 0u, row = (t * ISL_MAX_PROFILES + p) * 256;
+        for (uint32_t g = lane; g < c; g += 32) {
+            const uint32_t o = sh.live[b0 + g];
+            if (__ldg(a.lut + row + o) != ISL_START_NONE)
+                key = min(key, hi | ((uint32_t)__ldg(a.score + row + o) << 24) | (sh.base + b0 + g));
+        }
+    }
+    return key;
+}
+
+// One gang of a balanced locality byte (4..255, maxSkew skew = byte - 3; B2): ganglocal_any's member-by-member tentative commits, each
+// member restricted to the nodes whose count is at most mu + skew - 1, mu the least count over the nodes that admit it.  Per member:
+//   skew 1    one 64-bit grid_min of gangbalance_key: the least count first, then ganglocal_any's key among the nodes that have it;
+//   skew > 1  a 32-bit grid_min of the counts in those keys gives mu, a second one the least key over the nodes at most mu + skew - 1.
+// The CTA that owns the winning GPU commits the member (commit_member) and adds one to its node's count.  A node at mu always takes part,
+// so a member finds no GPU only where none admits it: the failure, the dead-profile mask and kMin's trim (B5) are ganglocal_any's.
+template <bool kMin = false>
+__device__ __forceinline__ void gangbalance_gang(const GangNodeArgs& a, const DevProfiles& prof, const NodeShare& sh, uint2* wins, uint32_t r0,
+                                                 uint32_t r1, uint32_t tag, uint32_t skew, uint32_t& parity, uint32_t& placed, uint32_t& dead,
+                                                 unsigned long long* s_warp64, unsigned long long* s_win64, uint32_t* s_warp32,
+                                                 uint32_t* s_win32, uint32_t tid, uint32_t lane, uint32_t warp, uint32_t min_m = 0) {
+    const uint32_t base = sh.base, cnt = sh.cnt;
+    __syncthreads();                                        // the previous gang's commits are in the live share before this gang's reads
+    uint32_t rank = 0;                                      // ALLOC members committed tentatively so far
+    for (uint32_t r = r0; r < r1; ++r) {
+        const uint32_t y = a.in[r].y, p = y & 0xFFu;
+        if (((y >> 8) & 0xFFu) != ISL_OP_ALLOC) continue;
+        uint32_t win = kInf;
+        if (p < prof.n && !((dead >> p) & 1u)) {
+            if (skew == 1) {
+                const unsigned long long w = grid_min<kGnThreads>(gangbalance_key(a, sh, wins, p, tag, kInf, lane, warp), a.keys, parity,
+                                                                  s_warp64, s_win64);
+                win = (uint32_t)w;                          // kInf when no GPU admits p
+            } else {
+                const uint32_t mu = grid_min<kGnThreads>((uint32_t)(gangbalance_key(a, sh, wins, p, tag, kInf, lane, warp) >> 32), a.keys,
+                                                         parity, s_warp32, s_win32);
+                if (mu != kInf)
+                    win = grid_min<kGnThreads>((uint32_t)gangbalance_key(a, sh, wins, p, tag, mu + skew - 1u, lane, warp), a.keys, parity,
+                                               s_warp32, s_win32);
+            }
+            if (win == kInf && rank == 0) dead |= 1u << p;  // no tentative slice of this gang is in the way
+        }
+        if (win == kInf) {
+            if (kMin && rank >= min_m) {
+                if (blockIdx.x == 0) {
+                    placed += rank;
+                    if (warp == 0) abort_gang_members<true>(a.in, a.out, prof, r, r1, 0, lane);
+                }
+                return;
+            }
+            if (warp == 0) gangfew_undo(a, sh, prof, r0, r, lane);
+            if (blockIdx.x == 0 && warp == 0) abort_gang_members(a.in, a.out, prof, r, r1, 0, lane);
+            return;
+        }
+        const uint32_t pos = (win & 0xFFFFFFu) - base;
+        if (pos < cnt && tid == 0) {                        // the owner commits the member tentatively and counts it on its node
+            commit_member(a, prof, sh, r, p, pos);
+            uint32_t jl = sh.j0, jh = sh.j1;                // nb(jl) <= base + pos < nb(jh): the last such jl is the non-empty node
+            while (jh - jl > 1) {
+                const uint32_t mid = (jl + jh) / 2;
+                if (sh.nb(mid) - base <= pos) jl = mid; else jh = mid;
+            }
+            wins[jl] = make_uint2(gangbalance_count(wins, jl, tag) + 1u, tag);
+        }
+        __syncthreads();                                    // the commit and the count are in place before the next member's scan
+        ++rank;
+    }
+    if (blockIdx.x == 0) placed += rank;                    // the gang commits: CTA 0 counts its members once
+}
+
 // ---------------------------------------------------------------------------------------------
 // k_ganglocal: isl_place_gangs on an engine created with a gang-topology flag (DESIGN.md 4.9-4.13).  One cooperative launch per call
 // behind k_prepare (frees and default records).  CTA c owns the partition's nodes [cta_node[c], cta_node[c + 1]) (whole nodes, balanced
@@ -3082,12 +3175,16 @@ __device__ __forceinline__ void ganglocal_any(const Args& a, const DevProfiles& 
 // kScore (an ISL_FLAG_GANG_NODE_SCORE engine, 4.16; kLoc ISL_GANG_ANY_NODES, _ONE_NODE, _DISTINCT_NODES or kLocPerGang, never with kMin):
 // the bodies put the node score in their keys, and `a` carries the widths and the policy (GangScoreArgs).  The host refuses a few-node
 // byte on such an engine, so its few-node branch is never taken.
+// kBal (kLocPerGang on an ISL_FLAG_GANG_BALANCED engine, 4.17, with or without kMin, never with kScore): a byte of 4..255 is a balanced
+// gang, gangbalance_gang with maxSkew byte - 3; its per-node counts are in `wins`, whose words of the CTA's nodes it clears first.  It
+// leaves the aux bytes alone, so the distinct-node tags run on across it.
 // ---------------------------------------------------------------------------------------------
 constexpr uint32_t kLocPerGang = 4;
-template <uint32_t kLoc, bool kMin = false, bool kScore = false>
+template <uint32_t kLoc, bool kMin = false, bool kScore = false, bool kBal = false>
 __global__ void __launch_bounds__(kGnThreads, 1) k_ganglocal(std::conditional_t<kScore, GangScoreArgs, GangNodeArgs> a, DevProfiles prof, uint2* wins,
                                                              const uint8_t* __restrict__ locality) {
     static_assert(!(kScore && kMin), "elastic gangs are not node-scored");
+    static_assert(!kBal || (kLoc == kLocPerGang && !kScore), "balanced gangs are per-gang bytes, not node-scored");
     extern __shared__ __align__(16) uint8_t gl_smem[];
     __shared__ unsigned long long s_warp64[kGnThreads / 32];
     __shared__ unsigned long long s_win64;
@@ -3096,6 +3193,7 @@ __global__ void __launch_bounds__(kGnThreads, 1) k_ganglocal(std::conditional_t<
     const uint32_t tid = threadIdx.x, lane = tid & 31u, warp = tid >> 5;
     const NodeShare sh(a, gl_smem);
     if (tid == 0) s_nwins = 0;
+    if constexpr (kBal) for (uint32_t j = sh.j0 + tid; j < sh.j1; j += kGnThreads) wins[j] = make_uint2(0u, 0u);
     uint32_t parity = 0, placed = 0, dead = 0, spread = 0;  // spread: locality-3 gangs since the marks were last cleared
     for (uint32_t gi = 0; gi < a.n_gangs; ++gi) {
         const uint32_t r0 = __ldg(a.gang_off + gi), r1 = __ldg(a.gang_off + gi + 1), loc = kLoc == kLocPerGang ? __ldg(locality + gi) : kLoc;
@@ -3110,6 +3208,9 @@ __global__ void __launch_bounds__(kGnThreads, 1) k_ganglocal(std::conditional_t<
             gangspread_gang<kMin, kScore>(a, prof, sh, wins, r0, r1, 1u + spread % 255u, parity, placed, dead, s_warp32, &s_win32, &s_nwins, tid,
                                           lane, warp, min_m);
             ++spread;
+        } else if (kBal && loc > ISL_GANG_DISTINCT_NODES) {
+            gangbalance_gang<kMin>(a, prof, sh, wins, r0, r1, kBalTag | gi, loc - ISL_GANG_DISTINCT_NODES, parity, placed, dead, s_warp64,
+                                   &s_win64, s_warp32, &s_win32, tid, lane, warp, min_m);
         } else {
             ganglocal_any<kMin, kScore>(a, prof, sh, r0, r1, parity, placed, dead, s_warp32, &s_win32, tid, lane, warp, min_m);
         }

@@ -26,16 +26,16 @@ static constexpr uint32_t kSpecRingIds = 1u << 24;     // stream ids of isl_plac
 
 // Engines created with one of these flags place gangs with k_ganglocal, the others with k_bestfit's gang loop.
 constexpr uint32_t kGangTopologyFlags = ISL_FLAG_GANG_ONE_NODE | ISL_FLAG_GANG_FEW_NODES | ISL_FLAG_GANG_DISTINCT_NODES |
-                                        ISL_FLAG_GANG_LOCALITY | ISL_FLAG_GANG_MIN_MEMBERS | ISL_FLAG_GANG_NODE_SCORE;
+                                        ISL_FLAG_GANG_LOCALITY | ISL_FLAG_GANG_MIN_MEMBERS | ISL_FLAG_GANG_NODE_SCORE | ISL_FLAG_GANG_BALANCED;
 
 // The instantiations of k_ganglocal, one per kind of gang-topology engine (gang_kind), with the name a launch error carries; wins:
-// distinct-node gangs may run, which stack their wins in GangNode::wins.
+// distinct-node gangs may run, which stack their wins in GangNode::wins, or balanced gangs, which keep their per-node counts there.
 struct GangKernel {
     const void* fn;
     const char* name;
     bool wins;
 };
-constexpr uint32_t kGangKinds = 9;
+constexpr uint32_t kGangKinds = 11;
 const GangKernel kGangKernels[kGangKinds] = {
     {(const void*)k_ganglocal<ISL_GANG_ONE_NODE>, "k_ganglocal<one_node>", false},
     {(const void*)k_ganglocal<ISL_GANG_FEW_NODES>, "k_ganglocal<few_nodes>", false},
@@ -46,13 +46,17 @@ const GangKernel kGangKernels[kGangKinds] = {
     {(const void*)k_ganglocal<ISL_GANG_ONE_NODE, false, true>, "k_ganglocal<one_node, node_score>", false},
     {(const void*)k_ganglocal<ISL_GANG_DISTINCT_NODES, false, true>, "k_ganglocal<distinct_nodes, node_score>", true},
     {(const void*)k_ganglocal<kLocPerGang, false, true>, "k_ganglocal<per_gang, node_score>", true},
+    {(const void*)k_ganglocal<kLocPerGang, false, false, true>, "k_ganglocal<per_gang, balanced>", true},
+    {(const void*)k_ganglocal<kLocPerGang, true, false, true>, "k_ganglocal<per_gang, min_members, balanced>", true},
 };
 
 // The kGangKernels entry of an engine with a gang-topology flag: each gang's own byte under ISL_FLAG_GANG_LOCALITY, and under
 // ISL_FLAG_GANG_MIN_MEMBERS with its minimum as well, else the locality of the engine's flag for every gang.  An
 // ISL_FLAG_GANG_NODE_SCORE engine (never with elastic or few-node gangs) takes the node-scored instantiation of its locality, any node
-// without a locality flag.
+// without a locality flag.  An ISL_FLAG_GANG_BALANCED engine (always with ISL_FLAG_GANG_LOCALITY, never node-scored) takes the balanced
+// per-gang instantiation, elastic or not.
 uint32_t gang_kind(uint32_t flags) {
+    if (flags & ISL_FLAG_GANG_BALANCED) return (flags & ISL_FLAG_GANG_MIN_MEMBERS) ? 10 : 9;
     if (flags & ISL_FLAG_GANG_NODE_SCORE)
         return (flags & ISL_FLAG_GANG_LOCALITY) ? 8 : (flags & ISL_FLAG_GANG_ONE_NODE) ? 6 : (flags & ISL_FLAG_GANG_DISTINCT_NODES) ? 7 : 5;
     if (flags & ISL_FLAG_GANG_MIN_MEMBERS) return 4;
@@ -538,7 +542,7 @@ int gang_layout(isl_engine* e, const void* kernel, int smem_optin, uint32_t per_
 // (gang_layout with the instantiation's own opt-in).  Under ISL_FLAG_GANG_LOCALITY or ISL_FLAG_GANG_MIN_MEMBERS it places each gang by
 // the byte at d_locality[gang], and under ISL_FLAG_GANG_MIN_MEMBERS it reads each gang's minimum m' from the uint32 words that follow
 // the bytes (rounded up to 4).  CTA c of an instantiation that runs distinct-node gangs stacks its wins in gn.wins[cta_node[c] ..), at
-// most one per node it owns.
+// most one per node it owns; a balanced instantiation keeps the count of node j in gn.wins[j] as well.
 int run_ganglocal(isl_engine* e, uint32_t kind, uint32_t n_gangs, const uint32_t* d_gang_off, const uint8_t* d_locality, uint32_t n,
                   const uint2* d_in, uint2* d_out) {
     const GangKernel& k = kGangKernels[kind];
@@ -1205,6 +1209,9 @@ int isl_create(const isl_config* cfg, isl_engine** out) {
          scored_gangs_refused)) return ISL_EINVAL;
     // elastic gangs (M6): with any one locality flag or none (their own checks refuse two), not with a pod on every node nor node scoring
     if ((cfg->flags & ISL_FLAG_GANG_MIN_MEMBERS) && ((cfg->flags & ISL_FLAG_ALL_NODES) || node_scoring(cfg->policy))) return ISL_EINVAL;
+    // balanced gangs (B6): a locality byte, so only with per-gang locality; not node-scored, not with a pod on every node
+    if ((cfg->flags & ISL_FLAG_GANG_BALANCED) &&
+        (!(cfg->flags & ISL_FLAG_GANG_LOCALITY) || node_scoring(cfg->policy) || (cfg->flags & ISL_FLAG_ALL_NODES))) return ISL_EINVAL;
     // gang preemption (P7): few-node and elastic gangs have no preemption order, a pod on every node has no single GPU to evict on
     if ((cfg->flags & ISL_FLAG_GANG_PREEMPT) &&
         (cfg->flags & (ISL_FLAG_ALL_NODES | ISL_FLAG_GANG_FEW_NODES | ISL_FLAG_GANG_MIN_MEMBERS))) return ISL_EINVAL;
@@ -1573,7 +1580,9 @@ int isl_place_gangs(isl_engine* e, uint32_t n_gangs, const uint32_t* gang_off, c
             bool named = false;
             for (uint32_t r = gang_off[i]; r < gang_off[i + 1]; ++r) {
                 if (in[r].op != ISL_OP_ALLOC) continue;
-                if (in[r].start > ISL_GANG_DISTINCT_NODES || (named && in[r].start != locality[i])) return ISL_EINVAL;
+                // B1: bytes 4..255 are balanced gangs on an ISL_FLAG_GANG_BALANCED engine
+                if ((in[r].start > ISL_GANG_DISTINCT_NODES && !(e->cfg.flags & ISL_FLAG_GANG_BALANCED)) ||
+                    (named && in[r].start != locality[i])) return ISL_EINVAL;
                 // N6: few-node gangs are not node-scored
                 if ((e->cfg.flags & ISL_FLAG_GANG_NODE_SCORE) && in[r].start == ISL_GANG_FEW_NODES) return ISL_EINVAL;
                 locality[i] = in[r].start;

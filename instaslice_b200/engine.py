@@ -38,6 +38,7 @@ FLAG_GANG_LOCALITY = 512  # isl_place_gangs takes each gang's node locality from
 FLAG_GANG_MIN_MEMBERS = 1024  # elastic gangs: a gang commits its leading members once they reach its minimum (the ALLOC size byte)
 FLAG_GANG_PREEMPT = 2048  # isl_preempt picks the victims a whole gang (a run of equal handles) needs, or evicts nothing for it
 FLAG_GANG_NODE_SCORE = 4096  # on a node-scoring engine isl_place_gangs places gangs by MostAllocated / LeastAllocated (N1-N8)
+FLAG_GANG_BALANCED = 8192  # with FLAG_GANG_LOCALITY: a locality of gang_balanced_nodes(k) spreads a gang over the nodes within maxSkew k
 GANG_ANY_NODES, GANG_ONE_NODE, GANG_FEW_NODES, GANG_DISTINCT_NODES = 0, 1, 2, 3     # node locality of one gang (include/islplace.h L1)
 SPEC_AUTO, SPEC_OFF, SPEC_ON = 0, 1, 2
 
@@ -155,6 +156,14 @@ class EngineError(RuntimeError):
     def __init__(self, code, what, detail=""):
         super().__init__(f"{what}: {load_library().isl_strerror(code).decode()} ({code}) {detail}".strip())
         self.code = code
+
+
+def gang_balanced_nodes(max_skew: int) -> int:
+    """The locality byte of a balanced gang with maxSkew ``max_skew`` (1..252) on a ``FLAG_GANG_BALANCED`` engine
+    (ISL_GANG_BALANCED_NODES, include/islplace.h B1): ``topologySpreadConstraints.maxSkew`` on ``kubernetes.io/hostname``."""
+    if isinstance(max_skew, bool) or int(max_skew) != max_skew or not 1 <= max_skew <= 252:
+        raise ValueError("maxSkew is 1..252")
+    return 3 + int(max_skew)
 
 
 def make_profiles(table, right_to_left: bool = False) -> np.ndarray:
@@ -364,7 +373,11 @@ class Engine:
         the node score (include/islplace.h N1-N8): any-node and distinct-node members one by one, each on the best-scored node that admits
         it (ties to the lowest node) and there on its first admitting GPU; a one-node gang on the node that takes it whole with the best
         score for the gang's slices taken as one pod.  Its locality is ``FLAG_GANG_ONE_NODE``, ``FLAG_GANG_DISTINCT_NODES``, each gang's
-        own under ``FLAG_GANG_LOCALITY`` (``GANG_FEW_NODES`` is refused), or any node."""
+        own under ``FLAG_GANG_LOCALITY`` (``GANG_FEW_NODES`` is refused), or any node.
+
+        On an engine created with ``FLAG_GANG_LOCALITY | FLAG_GANG_BALANCED`` a locality of ``gang_balanced_nodes(k)`` (4..255) spreads
+        the gang's members over the nodes: each member goes, by the engine's policy, to a node whose count of the gang's earlier members
+        is at most the least such count over the nodes that admit it plus k - 1 (include/islplace.h B1-B8)."""
         requests = np.ascontiguousarray(requests, dtype=REQUEST_DTYPE)
         gang_off = np.ascontiguousarray(gang_off, dtype=np.uint32)
         if len(gang_off) == 0 or int(gang_off[-1]) != len(requests):
@@ -377,6 +390,8 @@ class Engine:
                 raise ValueError("one locality per gang")
             if self.flags & FLAG_GANG_NODE_SCORE and (locality == GANG_FEW_NODES).any():
                 raise ValueError("few-node gangs are not node-scored (FLAG_GANG_NODE_SCORE)")
+            if self.flags & FLAG_GANG_BALANCED and len(locality) and (locality.min() < 0 or locality.max() > 255):
+                raise ValueError("a locality is 0..255 (gang_balanced_nodes(1..252) above GANG_DISTINCT_NODES)")
             requests = requests.copy()
             per_request = np.repeat(locality, np.diff(gang_off.astype(np.int64)))
             alloc = requests["op"] == OP_ALLOC

@@ -99,7 +99,8 @@ public:
     // ISL_FLAG_GANG_FEW_NODES so that it puts a gang on one node when one takes it and on as few nodes as it greedily can otherwise, or
     // ISL_FLAG_GANG_LOCALITY so that PlaceGangs takes one of these localities per gang; ISL_FLAG_GANG_MIN_MEMBERS (alone or with one of
     // the four) so that PlaceGangs takes a minimum per gang; with a node-scoring policy, ISL_FLAG_GANG_NODE_SCORE (alone or with the
-    // one-node, distinct-node or locality flag) so that PlaceGangs places gangs by the node score
+    // one-node, distinct-node or locality flag) so that PlaceGangs places gangs by the node score; with ISL_FLAG_GANG_LOCALITY,
+    // ISL_FLAG_GANG_BALANCED so that a locality of ISL_GANG_BALANCED_NODES(maxSkew) spreads a gang over the nodes
     explicit InstasliceReconciler(uint32_t quirks = ISL_QUIRKS_REF_EXACT, uint32_t max_gpus = 1u << 16, uint32_t max_batch = 1u << 16,
                                   uint32_t policy = ISL_POLICY_FIRST_FIT, uint32_t flags = 0);
     ~InstasliceReconciler();
@@ -126,7 +127,8 @@ public:
     // Prepared exact-match check (:198-203) fired on a pod, every span of the gang was released again.  Empty gangs throw.
     std::vector<GangOutcome> PlaceGangs(InstasliceList& list, AllocationPolicy& policy, const std::vector<std::vector<PendingPod>>& gangs);
     // The same with one node locality per gang (ISL_GANG_ANY_NODES, _ONE_NODE, _FEW_NODES or _DISTINCT_NODES), for a reconciler created
-    // with ISL_FLAG_GANG_LOCALITY: one call places gangs of every locality on one occupancy.  Throws unless there is one per gang.
+    // with ISL_FLAG_GANG_LOCALITY, or ISL_GANG_BALANCED_NODES(maxSkew) under ISL_FLAG_GANG_BALANCED as well: one call places gangs of
+    // every locality on one occupancy.  Throws unless there is one per gang.
     std::vector<GangOutcome> PlaceGangs(InstasliceList& list, AllocationPolicy& policy, const std::vector<std::vector<PendingPod>>& gangs,
                                         const std::vector<uint8_t>& locality);
     // The same with one minimum m (0..255) per gang as well (empty: none), for a reconciler created with ISL_FLAG_GANG_MIN_MEMBERS

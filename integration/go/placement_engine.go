@@ -83,6 +83,9 @@ const (
 	// On a PolicyMostAllocated or PolicyLeastAllocated engine, PlaceGangs places gangs by the node score: alone (any node) or with
 	// FlagGangOneNode, FlagGangDistinctNodes or FlagGangLocality (no few-node locality); not with FlagGangFewNodes or FlagGangMinMembers.
 	FlagGangNodeScore = uint32(C.ISL_FLAG_GANG_NODE_SCORE)
+	// With FlagGangLocality: a locality of GangBalancedNodes(maxSkew) spreads a gang's pods over the nodes within that maxSkew
+	// (topologySpreadConstraints on kubernetes.io/hostname).  Not under node scoring.
+	FlagGangBalanced = uint32(C.ISL_FLAG_GANG_BALANCED)
 )
 
 // StGangTrimmed is the record status of a pod its elastic gang was placed without (isl_result.status, FlagGangMinMembers).
@@ -95,6 +98,15 @@ const (
 	GangFewNodes      = uint8(C.ISL_GANG_FEW_NODES)      // one node when one has room, else as few as it greedily can (preferred)
 	GangDistinctNodes = uint8(C.ISL_GANG_DISTINCT_NODES) // every pod on a different node
 )
+
+// GangBalancedNodes is the locality of a gang whose pods spread over the nodes within maxSkew (1..252) of each other, on an engine
+// created with FlagGangLocality | FlagGangBalanced; ok is false outside 1..252.
+func GangBalancedNodes(maxSkew int) (locality uint8, ok bool) {
+	if maxSkew < 1 || maxSkew > 252 {
+		return 0, false
+	}
+	return uint8(3 + maxSkew), true
+}
 
 func NewPlacementEngine(maxGPUs, maxBatch uint32) (*PlacementEngine, error) {
 	return NewPlacementEngineWithPolicy(maxGPUs, maxBatch, PolicyFirstFit)
