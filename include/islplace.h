@@ -161,6 +161,8 @@ typedef struct isl_config {
                                            isl_place_gangs, N1-N8); every other call is unchanged */
 #define ISL_FLAG_GANG_BALANCED 8192u  /* with ISL_FLAG_GANG_LOCALITY: a locality byte of 4..255 spreads a gang's members over the nodes
                                          within a maxSkew of byte - 3 (see isl_place_gangs, B1-B8); every other call is unchanged */
+#define ISL_FLAG_GANG_NODE_SCORE_ALL 16384u  /* with ISL_FLAG_GANG_NODE_SCORE: few-node, elastic and balanced gangs are node-scored too
+                                                (see isl_place_gangs, C1-C8); every other call is unchanged */
 /* Node locality of one gang on an ISL_FLAG_GANG_LOCALITY engine (isl_request.start of its ALLOC members, rules L1-L6) */
 #define ISL_GANG_ANY_NODES      0u  /* rules 2-4: members anywhere, as on an engine without a gang flag */
 #define ISL_GANG_ONE_NODE       1u  /* G2-G3: every member on one node */
@@ -456,7 +458,8 @@ int  isl_place_batch_range(isl_engine* e, uint32_t lo, uint32_t hi, uint32_t n, 
  * the same lock as its single pods, and a one-node gang goes to the fullest (emptiest) node that takes it, not the first.  On an engine
  * created with the flag:
  *   N1. isl_create: ISL_EINVAL for the flag without ISL_POLICY_MOST_ALLOCATED or _LEAST_ALLOCATED, or with ISL_FLAG_GANG_FEW_NODES or
- *       ISL_FLAG_GANG_MIN_MEMBERS (ISL_FLAG_ALL_NODES is refused by node scoring already).  It may come with at most one of
+ *       ISL_FLAG_GANG_MIN_MEMBERS, unless ISL_FLAG_GANG_NODE_SCORE_ALL is set as well (C1; ISL_FLAG_ALL_NODES is refused by node
+ *       scoring already).  It may come with at most one of
  *       ISL_FLAG_GANG_ONE_NODE, _DISTINCT_NODES and _LOCALITY (their mutual refusals are unchanged; only their refusal of node scoring is
  *       lifted, and only with this bit), and with ISL_FLAG_GANG_PREEMPT (N7).  max_gpus > 2^20 and more than 2^20 nodes keep node
  *       scoring's ISL_ERANGE.
@@ -473,7 +476,7 @@ int  isl_place_batch_range(isl_engine* e, uint32_t lo, uint32_t hi, uint32_t n, 
  *   N6. Both quirk sets, per-node tables (each node's score normalised by its own width), inside isl_set_partition; stats.placed counts
  *       committed members only.  isl_place_gangs keeps every code above, the 2^20-GPU partition cap included.  Under
  *       ISL_FLAG_GANG_LOCALITY a locality byte of 2 (few nodes) is ISL_EINVAL, checked with L4 before the engine state is looked at;
- *       nothing changes.
+ *       nothing changes.  ISL_FLAG_GANG_NODE_SCORE_ALL lifts this (C2).
  *   N7. Every other entry point returns exactly what it returns on the same engine without the bit: isl_place_batch and every other
  *       k_nodefit caller, isl_what_if, isl_capacity, isl_preempt.  With ISL_FLAG_GANG_PREEMPT, isl_preempt keeps P1-P8, whose scan
  *       order is ascending canonical under node scoring (rule 5), so it returns what a FIRST_FIT engine with the same flags minus this
@@ -517,7 +520,7 @@ int  isl_place_batch_range(isl_engine* e, uint32_t lo, uint32_t hi, uint32_t n, 
  *   B5. Elastic gangs: with ISL_FLAG_GANG_MIN_MEMBERS, M3 applies member by member, as for S: with f the rank of the first member with
  *       no admitting GPU, the gang commits its leading f members when f >= m'.
  *   B6. isl_create: ISL_EINVAL for the flag without ISL_FLAG_GANG_LOCALITY, with a node-scoring policy (hence with
- *       ISL_FLAG_GANG_NODE_SCORE) or with ISL_FLAG_ALL_NODES.  ISL_FLAG_GANG_PREEMPT may come with it; isl_preempt keeps P1, which refuses
+ *       ISL_FLAG_GANG_NODE_SCORE) unless ISL_FLAG_GANG_NODE_SCORE_ALL is set (C1), or with ISL_FLAG_ALL_NODES.  ISL_FLAG_GANG_PREEMPT may come with it; isl_preempt keeps P1, which refuses
  *       bytes above 3, so no balanced gang is preempted for.  isl_place_gangs keeps every other code, the 2^20-GPU partition cap
  *       included.  Every other entry point returns exactly what it returns without the flag.
  *   B7. The choice is greedy, member by member (as S4 and F5): list the larger members first.
@@ -532,6 +535,50 @@ int  isl_place_batch_range(isl_engine* e, uint32_t lo, uint32_t hi, uint32_t n, 
  *       byte 7 (k 4)  equals byte 0
  *   B8's case: three one-GPU nodes with bytes 0x00, 0x7F and 0x00, a gang of three 1g.10gb, byte 4, first-fit: (0,0) (2,0) (0,1).  Start
  *       7 is not legal, so node 1 is not in A; a minimum over every node would stay at node 1's 0 and refuse member 2.
+ *
+ * Every gang kind node-scored (ISL_FLAG_GANG_NODE_SCORE_ALL): a cluster that packs with MostAllocated or spreads with LeastAllocated runs
+ * its elastic jobs, its jobs that prefer few nodes and its balanced replicas on the same engine as its pods.  Each kind keeps its own
+ * first criterion (a few-node round's largest d, an elastic one-node trim's depth D, a balanced member's candidate nodes); the node score
+ * breaks the ties below it where a first-fit engine takes scan order.  On an engine created with the flag:
+ *   C1. isl_create: ISL_EINVAL for the flag without ISL_FLAG_GANG_NODE_SCORE (hence without a node-scoring policy).  With both bits the
+ *       engine also accepts ISL_FLAG_GANG_FEW_NODES (N1's refusal is lifted; F6's refusal with ISL_FLAG_GANG_ONE_NODE, _DISTINCT_NODES and
+ *       _LOCALITY stays), ISL_FLAG_GANG_MIN_MEMBERS (the refusals of N1 and M6 are lifted) and ISL_FLAG_GANG_BALANCED with
+ *       ISL_FLAG_GANG_LOCALITY (B6's refusal of node scoring is lifted).  Every other refusal stays: ISL_FLAG_ALL_NODES,
+ *       ISL_FLAG_GANG_PREEMPT with few-node or elastic gangs (P7), BALANCED without LOCALITY, two locality flags, and node scoring's
+ *       ISL_ERANGE above 2^20 GPUs or nodes.  An engine without the bit keeps every code it returns.
+ *   C2. Under ISL_FLAG_GANG_LOCALITY a byte of 2 is accepted (N6 is lifted), and under ISL_FLAG_GANG_BALANCED so are 4..255.  Every other
+ *       check of L4 and M6 is unchanged and still runs before the engine state is looked at.
+ *   C3. score_N(R) is node-scoring rule 3 over N's GPUs inside the partition with N's table width: MostAllocated floor(100 (busy + R) /
+ *       cap), LeastAllocated floor(100 (cap - busy - R) / cap), busy counted on the occupancy the round or member sees (the call's FREEs,
+ *       the committed gangs and the gang's own tentative members).  Ties go to the lowest canonical node index; inside a node the
+ *       reference's first-fit search decides, as in N5.
+ *   C4. Few nodes (ISL_FLAG_GANG_FEW_NODES, or byte 2): F2's rounds and d(N) are unchanged; among the nodes with the largest d >= 1 the
+ *       round goes to the highest score_N(R_d(N)), R_d(N) the sum of the row sizes, in N's table, of the d members the node takes.  F3's
+ *       failure and rule 5 are unchanged.  Consequences: (a) a gang that some node takes whole gets exactly N5's records and occupancy;
+ *       (b) a gang that fails here fails on the one-node scored engine in the same state; (c) on a one-node inventory, or a partition
+ *       inside one node, a call equals a FIRST_FIT engine with the few-node flag; (d) with gangs of one a call equals isl_place_batch on
+ *       the same engine; (e) F4 (e) holds: two consecutive rounds never use the same node.
+ *   C5. Elastic gangs (ISL_FLAG_GANG_MIN_MEMBERS): M1-M7 hold with the scored rules as the rules of each locality: N3 any node, N4
+ *       distinct nodes, N5 one node, C4 few nodes, C6 balanced.  M3 trims member by member for any-node, distinct-node and balanced gangs
+ *       and after the rounds so far for few-node gangs; a one-node gang commits its first D members on the node that reaches depth D with
+ *       the highest score_N(R_D(N)).  M5 (a)-(d) hold: a gang trimmed at f equals the cut gang of f members placed without the flag.
+ *   C6. Balanced gangs (bytes 4..255): B2's A, cnt, mu and candidate nodes (cnt <= mu + k - 1) are unchanged; among the candidates the
+ *       member goes to the highest score_N(its row size).  B3, B5, B7 and B8 hold, and B4 (a)-(f) with N4 in place of S2 and N3 in place
+ *       of rules 2-4: byte 3 + k with k >= the gang's ALLOC members equals byte 0, which is N3.
+ *   C7. With the bit, a call whose gangs all have locality 0, 1 or 3, without ISL_FLAG_GANG_MIN_MEMBERS, returns exactly what the same
+ *       engine without the bit returns (records, occupancy, stats.placed).  Every other entry point returns what it returns without the
+ *       bit; isl_preempt keeps P1, so bytes 2 and above 3 are ISL_EINVAL there.
+ *   C8. The score never comes above the locality's own criterion: a round never takes fewer members for a better score and a trim never
+ *       keeps fewer members.  The choice stays greedy, as F5, S4, B7 and M7 say.
+ *   Examples, H100-80GB rows, either quirk set, one-GPU nodes, gangs of four 1g.10gb, records (gpu, start):
+ *       few nodes, bytes 0x0F 0xF8 0x3F   FIRST_FIT (F2): d = [3, 3, 1], node 0 takes (0,4) (0,5) (0,6); then d = [0, 1, 1]: (1,0).
+ *                                         MOST: round 1 scores node 0 87, node 1 100: (1,0) (1,1) (1,2); round 2 node 0 62, node 2 87:
+ *                                         (2,6).  LEAST: round 1 node 0 12, node 1 0: (0,4) (0,5) (0,6); round 2 node 1 25, node 2 12:
+ *                                         (1,0).
+ *       one node, m = 2, same nodes       D = 3, reached by nodes 0 and 1.  MOST (1,0) (1,1) (1,2); LEAST (0,4) (0,5) (0,6); member 3
+ *                                         NO_CAPACITY either way.
+ *       balanced, bytes 0x00 0x0F         byte 4: LEAST (0,0) (1,4) (0,1) (1,5), MOST (1,4) (0,0) (1,5) (0,1);
+ *                                         byte 5: LEAST (0,0) (0,1) (1,4) (0,2), MOST (1,4) (1,5) (0,0) (1,6).
  */
 int  isl_place_gangs(isl_engine* e, uint32_t n_gangs, const uint32_t* gang_off, const isl_request* in, isl_result* out);
 

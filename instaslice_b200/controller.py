@@ -99,7 +99,7 @@ class InstasliceReconciler:
     def __init__(self, instaslices: list, quirks: int = E.QUIRKS_REF_EXACT, max_batch: int = 65536, engine: E.Engine | None = None,
                  policy: int = E.POLICY_FIRST_FIT, gang_one_node: bool = False, gang_distinct_nodes: bool = False,
                  gang_few_nodes: bool = False, gang_locality: bool = False, gang_min_members: bool = False, gang_preempt: bool = False,
-                 gang_node_score: bool = False, gang_balanced: bool = False):
+                 gang_node_score: bool = False, gang_balanced: bool = False, gang_node_score_all: bool = False):
         """``policy``: the engine policy of the engine this reconciler creates (``engine`` is None), e.g. ``E.POLICY_MOST_ALLOCATED`` to
         pack MIG pods onto the fullest nodes or ``E.POLICY_LEAST_ALLOCATED`` to spread them (include/islplace.h).  ``gang_one_node``:
         that engine is created with ``E.FLAG_GANG_ONE_NODE``, so ``place_pending_gangs`` puts every gang on one node.
@@ -114,7 +114,10 @@ class InstasliceReconciler:
         ``place_pending_gangs`` places gangs by the node score, alone (any node) or with the one-node, distinct-node or locality option
         (the engine refuses it with any other policy, few-node gangs and elastic gangs).  ``gang_balanced``: with
         ``E.FLAG_GANG_BALANCED``, which needs ``gang_locality``, so that a gang's locality may be ``E.gang_balanced_nodes(k)``: its
-        replicas spread over the nodes within a maxSkew of k (the engine refuses it under node scoring)."""
+        replicas spread over the nodes within a maxSkew of k (the engine refuses it under node scoring unless ``gang_node_score_all``).
+        ``gang_node_score_all``: with ``E.FLAG_GANG_NODE_SCORE_ALL``, which needs ``gang_node_score``, so that the node score also places
+        few-node gangs (``gang_few_nodes`` or a ``GANG_FEW_NODES`` locality), elastic gangs (``gang_min_members``) and balanced gangs
+        (``gang_balanced``), all on the one packing or spreading engine."""
         self.quirks = quirks
         self.policy = policy
         self.gang_one_node = gang_one_node
@@ -125,6 +128,7 @@ class InstasliceReconciler:
         self.gang_preempt = gang_preempt
         self.gang_node_score = gang_node_score
         self.gang_balanced = gang_balanced
+        self.gang_node_score_all = gang_node_score_all
         self.items = instaslices
         self._engine = engine
         self._max_batch = max_batch
@@ -174,7 +178,8 @@ class InstasliceReconciler:
                                           (E.FLAG_GANG_MIN_MEMBERS if self.gang_min_members else 0) |
                                           (E.FLAG_GANG_PREEMPT if self.gang_preempt else 0) |
                                           (E.FLAG_GANG_NODE_SCORE if self.gang_node_score else 0) |
-                                          (E.FLAG_GANG_BALANCED if self.gang_balanced else 0))
+                                          (E.FLAG_GANG_BALANCED if self.gang_balanced else 0) |
+                                          (E.FLAG_GANG_NODE_SCORE_ALL if self.gang_node_score_all else 0))
         self._engine.load_profile_tables(self.rows)
         self._engine.load_inventory(self.node_off, np.asarray(occ, dtype=np.uint8))
         self._engine.set_node_tables(np.asarray(self.node_table, dtype=np.uint8))

@@ -2829,11 +2829,16 @@ __device__ void gangfew_undo(const GangNodeArgs& a, const NodeShare& sh, const D
 // table's width (a second pass over its bytes), and its key is (100 - score(N, s_need[t])) << 32 | node, the gang scored as one pod;
 // bit 63 stays clear, so every success still sorts before every failure.  Pass 0's filter stays valid: a node it skips cannot take the
 // gang.
+// kScore with kFew or kMin (ISL_FLAG_GANG_NODE_SCORE_ALL, 4.18, C4-C5): a failed node's key carries its score as well,
+// kGnFail | (0x7FFFFFFF - d) << 32 | (100 - score(N, R_d)) << 24 | j, so the deepest nodes sort by score, then by node (j < 2^24: a
+// node-scoring inventory has at most 2^20 nodes).  busy + R_d is the scratch copy's popcount under the width after the resolve, which
+// gives the success key's score too.  That one key decides a few-node round and a one-node trim; one node without kMin keeps N5's keys.
 template <bool kFew, bool kMin = false, bool kScore = false, class Args = GangNodeArgs>
 __device__ __forceinline__ void gangnode_gang(const Args& a, const DevProfiles& prof, const NodeShare& sh, uint32_t r0, uint32_t r1,
                                               uint32_t& parity, uint32_t& placed, unsigned long long* s_warp, unsigned long long* s_win,
                                               uint32_t* s_need, uint32_t* s_allocs, uint32_t tid, uint32_t lane, uint32_t warp,
                                               uint32_t min_m = 0) {
+    constexpr uint32_t kGnNodeMask = kScore ? 0xFFFFFFu : 0xFFFFFFFFu;    // the node in a failed key's low word
     uint8_t* const scr = sh.aux;
     uint32_t ri = r0, held = 0;     // kFew: the round's first request; members this CTA committed tentatively in earlier rounds
     uint32_t done = 0;              // kFew && kMin: members the earlier rounds placed (grid-uniform: the sum of the winning depths)
@@ -2869,7 +2874,13 @@ __device__ __forceinline__ void gangnode_gang(const Args& a, const DevProfiles& 
                 free_slices = __reduce_add_sync(0xFFFFFFFFu, free_slices);
                 if (pass == 0 && free_slices < s_need[t]) continue;
                 const uint32_t d = gangnode_resolve(a, prof, scr + b0, c, a.lo + sh.base + b0, t, ri, r1, false, lane);
-                if constexpr (kScore) {     // the node's busy slices under its width on the live bytes, before the gang
+                if constexpr (kScore && (kFew || kMin)) {   // busy + R_d: the scratch copy's slices under the width after the d members
+                    uint32_t busy = 0;
+                    for (uint32_t g = lane; g < c; g += 32) busy += __popc(scr[b0 + g] & ((1u << a.width[t]) - 1u));
+                    busy = __reduce_add_sync(0xFFFFFFFFu, busy);
+                    const unsigned long long score = nodefit_leaf(1u, busy, a.width[t] * c, 0u, a.most, 0u) >> 24;     // 100 - score
+                    best = min(best, d == allocs ? score << 32 | j : gn_fail_key(d, 0u) | score << 24 | j);
+                } else if constexpr (kScore) {     // the node's busy slices under its width on the live bytes, before the gang
                     uint32_t busy = 0;
                     for (uint32_t g = lane; g < c; g += 32) busy += __popc(sh.live[b0 + g] & ((1u << a.width[t]) - 1u));
                     busy = __reduce_add_sync(0xFFFFFFFFu, busy);
@@ -2893,7 +2904,7 @@ __device__ __forceinline__ void gangnode_gang(const Args& a, const DevProfiles& 
         }
         if constexpr (!kFew) {
             if constexpr (kMin) {
-                const uint32_t d = gn_fail_depth(win), j = (uint32_t)win;
+                const uint32_t d = gn_fail_depth(win), j = (uint32_t)win & kGnNodeMask;
                 if (d >= min_m) {                           // min_m >= 1, so ~0ull (depth 0) never gets here
                     if (j >= sh.j0 && j < sh.j1 && warp == 0) {
                         gangnode_commit(a, prof, sh, j, ri, r1, lane);
@@ -2907,7 +2918,7 @@ __device__ __forceinline__ void gangnode_gang(const Args& a, const DevProfiles& 
                 abort_gang_members(a.in, a.out, prof, r0, r1, gn_fail_depth(win), lane);
             break;
         } else {
-            const uint32_t d = gn_fail_depth(win), j = (uint32_t)win;      // members the round places
+            const uint32_t d = gn_fail_depth(win), j = (uint32_t)win & kGnNodeMask;      // members the round places
             if (kMin && d == 0 && done >= min_m) {          // the earlier rounds' members commit, m_i keeps its record
                 placed += held;
                 if (blockIdx.x == 0 && warp == 0) abort_gang_members<true>(a.in, a.out, prof, ri, r1, 0, lane);
@@ -3068,9 +3079,11 @@ __device__ __forceinline__ uint32_t gangbalance_count(const uint2* wins, uint32_
 // Warp-wide over the nodes of the share this warp visits, over the GPUs that admit p: with lim == kInf the least count << 32 | key, else
 // the least key alone over the nodes whose count is at most lim, where key is ganglocal_any's score << 24 | partition-local storage
 // position; ~0ull when there is none.  (A lane visits many nodes: with the count above a filtered key, its minimum would be the key of
-// its least-count node, not its least key.)
-__device__ __forceinline__ unsigned long long gangbalance_key(const GangNodeArgs& a, const NodeShare& sh, const uint2* wins, uint32_t p,
-                                                             uint32_t tag, uint32_t lim, uint32_t lane, uint32_t warp) {
+// its least-count node, not its least key.)  kScore (ISL_FLAG_GANG_NODE_SCORE_ALL, 4.18, C6): the key below the count is gangscore_node's,
+// so the nodes within the skew sort by score, then node, and the member takes its node's first admitting GPU.
+template <bool kScore = false, class Args = GangNodeArgs>
+__device__ __forceinline__ unsigned long long gangbalance_key(const Args& a, const NodeShare& sh, const uint2* wins, uint32_t p, uint32_t tag,
+                                                             uint32_t lim, uint32_t lane, uint32_t warp) {
     unsigned long long key = ~0ull;
     for (uint32_t j = sh.j0 + warp; j < sh.j1; j += kGnThreads / 32) {
         const uint32_t b0 = sh.nb(j) - sh.base, c = sh.nb(j + 1) - sh.base - b0;
@@ -3078,6 +3091,11 @@ __device__ __forceinline__ unsigned long long gangbalance_key(const GangNodeArgs
         const uint32_t n = gangbalance_count(wins, j, tag);
         if (n > lim) continue;
         const unsigned long long hi = lim == kInf ? (unsigned long long)n << 32 : 0ull;
+        if constexpr (kScore) {
+            const uint32_t s = gangscore_node(a, sh, j, p, nullptr, 0u, lane);
+            if (s != kInf) key = min(key, hi | s);
+            continue;
+        }
         const uint32_t t = a.n_tables > 1 ? a.gtab[a.lo + sh.base + b0] & (kMaxTables - 1) : 0u, row = (t * ISL_MAX_PROFILES + p) * 256;
         for (uint32_t g = lane; g < c; g += 32) {
             const uint32_t o = sh.live[b0 + g];
@@ -3094,8 +3112,9 @@ __device__ __forceinline__ unsigned long long gangbalance_key(const GangNodeArgs
 //   skew > 1  a 32-bit grid_min of the counts in those keys gives mu, a second one the least key over the nodes at most mu + skew - 1.
 // The CTA that owns the winning GPU commits the member (commit_member) and adds one to its node's count.  A node at mu always takes part,
 // so a member finds no GPU only where none admits it: the failure, the dead-profile mask and kMin's trim (B5) are ganglocal_any's.
-template <bool kMin = false>
-__device__ __forceinline__ void gangbalance_gang(const GangNodeArgs& a, const DevProfiles& prof, const NodeShare& sh, uint2* wins, uint32_t r0,
+// kScore (C6): the keys are gangbalance_key<true>'s, the node score among the nodes within the skew.
+template <bool kMin = false, bool kScore = false, class Args = GangNodeArgs>
+__device__ __forceinline__ void gangbalance_gang(const Args& a, const DevProfiles& prof, const NodeShare& sh, uint2* wins, uint32_t r0,
                                                  uint32_t r1, uint32_t tag, uint32_t skew, uint32_t& parity, uint32_t& placed, uint32_t& dead,
                                                  unsigned long long* s_warp64, unsigned long long* s_win64, uint32_t* s_warp32,
                                                  uint32_t* s_win32, uint32_t tid, uint32_t lane, uint32_t warp, uint32_t min_m = 0) {
@@ -3108,15 +3127,15 @@ __device__ __forceinline__ void gangbalance_gang(const GangNodeArgs& a, const De
         uint32_t win = kInf;
         if (p < prof.n && !((dead >> p) & 1u)) {
             if (skew == 1) {
-                const unsigned long long w = grid_min<kGnThreads>(gangbalance_key(a, sh, wins, p, tag, kInf, lane, warp), a.keys, parity,
-                                                                  s_warp64, s_win64);
+                const unsigned long long w = grid_min<kGnThreads>(gangbalance_key<kScore>(a, sh, wins, p, tag, kInf, lane, warp), a.keys,
+                                                                  parity, s_warp64, s_win64);
                 win = (uint32_t)w;                          // kInf when no GPU admits p
             } else {
-                const uint32_t mu = grid_min<kGnThreads>((uint32_t)(gangbalance_key(a, sh, wins, p, tag, kInf, lane, warp) >> 32), a.keys,
-                                                         parity, s_warp32, s_win32);
+                const uint32_t mu = grid_min<kGnThreads>((uint32_t)(gangbalance_key<kScore>(a, sh, wins, p, tag, kInf, lane, warp) >> 32),
+                                                         a.keys, parity, s_warp32, s_win32);
                 if (mu != kInf)
-                    win = grid_min<kGnThreads>((uint32_t)gangbalance_key(a, sh, wins, p, tag, mu + skew - 1u, lane, warp), a.keys, parity,
-                                               s_warp32, s_win32);
+                    win = grid_min<kGnThreads>((uint32_t)gangbalance_key<kScore>(a, sh, wins, p, tag, mu + skew - 1u, lane, warp), a.keys,
+                                               parity, s_warp32, s_win32);
             }
             if (win == kInf && rank == 0) dead |= 1u << p;  // no tentative slice of this gang is in the way
         }
@@ -3172,19 +3191,19 @@ __device__ __forceinline__ void gangbalance_gang(const GangNodeArgs& a, const De
 // writes the PLACED records on it and rewrites its own tentative ones GANG_ABORTED when the gang aborts (gangfew_undo); CTA 0 writes
 // GANG_ABORTED or GANG_TRIMMED for the other members, except the one that stopped the gang, which keeps k_prepare's NO_CAPACITY or
 // BAD_PROFILE record.
-// kScore (an ISL_FLAG_GANG_NODE_SCORE engine, 4.16; kLoc ISL_GANG_ANY_NODES, _ONE_NODE, _DISTINCT_NODES or kLocPerGang, never with kMin):
-// the bodies put the node score in their keys, and `a` carries the widths and the policy (GangScoreArgs).  The host refuses a few-node
-// byte on such an engine, so its few-node branch is never taken.
-// kBal (kLocPerGang on an ISL_FLAG_GANG_BALANCED engine, 4.17, with or without kMin, never with kScore): a byte of 4..255 is a balanced
-// gang, gangbalance_gang with maxSkew byte - 3; its per-node counts are in `wins`, whose words of the CTA's nodes it clears first.  It
-// leaves the aux bytes alone, so the distinct-node tags run on across it.
+// kScore (an ISL_FLAG_GANG_NODE_SCORE engine, 4.16): the bodies put the node score in their keys, and `a` carries the widths and the
+// policy (GangScoreArgs).  Without ISL_FLAG_GANG_NODE_SCORE_ALL (kLoc ISL_GANG_ANY_NODES, _ONE_NODE, _DISTINCT_NODES or kLocPerGang,
+// never with kMin) the host refuses a few-node byte, so the few-node branch is never taken; with it (4.18) kLoc may also be
+// ISL_GANG_FEW_NODES, and kMin and kBal may come with kScore.
+// kBal (kLocPerGang on an ISL_FLAG_GANG_BALANCED engine, 4.17, with or without kMin): a byte of 4..255 is a balanced gang,
+// gangbalance_gang with maxSkew byte - 3; its per-node counts are in `wins`, whose words of the CTA's nodes it clears first.  It leaves
+// the aux bytes alone, so the distinct-node tags run on across it.
 // ---------------------------------------------------------------------------------------------
 constexpr uint32_t kLocPerGang = 4;
 template <uint32_t kLoc, bool kMin = false, bool kScore = false, bool kBal = false>
 __global__ void __launch_bounds__(kGnThreads, 1) k_ganglocal(std::conditional_t<kScore, GangScoreArgs, GangNodeArgs> a, DevProfiles prof, uint2* wins,
                                                              const uint8_t* __restrict__ locality) {
-    static_assert(!(kScore && kMin), "elastic gangs are not node-scored");
-    static_assert(!kBal || (kLoc == kLocPerGang && !kScore), "balanced gangs are per-gang bytes, not node-scored");
+    static_assert(!kBal || kLoc == kLocPerGang, "balanced gangs are per-gang bytes");
     extern __shared__ __align__(16) uint8_t gl_smem[];
     __shared__ unsigned long long s_warp64[kGnThreads / 32];
     __shared__ unsigned long long s_win64;
@@ -3202,15 +3221,16 @@ __global__ void __launch_bounds__(kGnThreads, 1) k_ganglocal(std::conditional_t<
             if (loc == ISL_GANG_ONE_NODE)
                 gangnode_gang<false, kMin, kScore>(a, prof, sh, r0, r1, parity, placed, s_warp64, &s_win64, s_need, &s_allocs, tid, lane, warp,
                                                    min_m);
-            else gangnode_gang<true, kMin>(a, prof, sh, r0, r1, parity, placed, s_warp64, &s_win64, s_need, &s_allocs, tid, lane, warp, min_m);
+            else gangnode_gang<true, kMin, kScore>(a, prof, sh, r0, r1, parity, placed, s_warp64, &s_win64, s_need, &s_allocs, tid, lane, warp,
+                                                   min_m);
             spread = 0;                                     // the scratch copies overwrote the marks
         } else if (loc == ISL_GANG_DISTINCT_NODES) {
             gangspread_gang<kMin, kScore>(a, prof, sh, wins, r0, r1, 1u + spread % 255u, parity, placed, dead, s_warp32, &s_win32, &s_nwins, tid,
                                           lane, warp, min_m);
             ++spread;
         } else if (kBal && loc > ISL_GANG_DISTINCT_NODES) {
-            gangbalance_gang<kMin>(a, prof, sh, wins, r0, r1, kBalTag | gi, loc - ISL_GANG_DISTINCT_NODES, parity, placed, dead, s_warp64,
-                                   &s_win64, s_warp32, &s_win32, tid, lane, warp, min_m);
+            gangbalance_gang<kMin, kScore>(a, prof, sh, wins, r0, r1, kBalTag | gi, loc - ISL_GANG_DISTINCT_NODES, parity, placed, dead,
+                                           s_warp64, &s_win64, s_warp32, &s_win32, tid, lane, warp, min_m);
         } else {
             ganglocal_any<kMin, kScore>(a, prof, sh, r0, r1, parity, placed, dead, s_warp32, &s_win32, tid, lane, warp, min_m);
         }

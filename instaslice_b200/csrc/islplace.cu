@@ -35,7 +35,7 @@ struct GangKernel {
     const char* name;
     bool wins;
 };
-constexpr uint32_t kGangKinds = 11;
+constexpr uint32_t kGangKinds = 15;
 const GangKernel kGangKernels[kGangKinds] = {
     {(const void*)k_ganglocal<ISL_GANG_ONE_NODE>, "k_ganglocal<one_node>", false},
     {(const void*)k_ganglocal<ISL_GANG_FEW_NODES>, "k_ganglocal<few_nodes>", false},
@@ -48,17 +48,23 @@ const GangKernel kGangKernels[kGangKinds] = {
     {(const void*)k_ganglocal<kLocPerGang, false, true>, "k_ganglocal<per_gang, node_score>", true},
     {(const void*)k_ganglocal<kLocPerGang, false, false, true>, "k_ganglocal<per_gang, balanced>", true},
     {(const void*)k_ganglocal<kLocPerGang, true, false, true>, "k_ganglocal<per_gang, min_members, balanced>", true},
+    {(const void*)k_ganglocal<ISL_GANG_FEW_NODES, false, true>, "k_ganglocal<few_nodes, node_score>", false},
+    {(const void*)k_ganglocal<kLocPerGang, true, true>, "k_ganglocal<per_gang, min_members, node_score>", true},
+    {(const void*)k_ganglocal<kLocPerGang, false, true, true>, "k_ganglocal<per_gang, node_score, balanced>", true},
+    {(const void*)k_ganglocal<kLocPerGang, true, true, true>, "k_ganglocal<per_gang, min_members, node_score, balanced>", true},
 };
 
 // The kGangKernels entry of an engine with a gang-topology flag: each gang's own byte under ISL_FLAG_GANG_LOCALITY, and under
 // ISL_FLAG_GANG_MIN_MEMBERS with its minimum as well, else the locality of the engine's flag for every gang.  An
-// ISL_FLAG_GANG_NODE_SCORE engine (never with elastic or few-node gangs) takes the node-scored instantiation of its locality, any node
-// without a locality flag.  An ISL_FLAG_GANG_BALANCED engine (always with ISL_FLAG_GANG_LOCALITY, never node-scored) takes the balanced
-// per-gang instantiation, elastic or not.
+// ISL_FLAG_GANG_NODE_SCORE engine takes the node-scored instantiation of its locality, any node without a locality flag; elastic and
+// few-node gangs come only with ISL_FLAG_GANG_NODE_SCORE_ALL.  An ISL_FLAG_GANG_BALANCED engine (always with ISL_FLAG_GANG_LOCALITY,
+// node-scored only with ISL_FLAG_GANG_NODE_SCORE_ALL) takes the balanced per-gang instantiation, elastic or not, scored or not.
 uint32_t gang_kind(uint32_t flags) {
-    if (flags & ISL_FLAG_GANG_BALANCED) return (flags & ISL_FLAG_GANG_MIN_MEMBERS) ? 10 : 9;
+    const bool min = flags & ISL_FLAG_GANG_MIN_MEMBERS;
+    if (flags & ISL_FLAG_GANG_BALANCED) return (flags & ISL_FLAG_GANG_NODE_SCORE) ? (min ? 14 : 13) : (min ? 10 : 9);
     if (flags & ISL_FLAG_GANG_NODE_SCORE)
-        return (flags & ISL_FLAG_GANG_LOCALITY) ? 8 : (flags & ISL_FLAG_GANG_ONE_NODE) ? 6 : (flags & ISL_FLAG_GANG_DISTINCT_NODES) ? 7 : 5;
+        return min ? 12 : (flags & ISL_FLAG_GANG_LOCALITY) ? 8 : (flags & ISL_FLAG_GANG_ONE_NODE) ? 6 : (flags & ISL_FLAG_GANG_DISTINCT_NODES) ? 7
+                    : (flags & ISL_FLAG_GANG_FEW_NODES) ? 11 : 5;
     if (flags & ISL_FLAG_GANG_MIN_MEMBERS) return 4;
     if (flags & ISL_FLAG_GANG_LOCALITY) return 3;
     return (flags & ISL_FLAG_GANG_ONE_NODE) ? 0 : (flags & ISL_FLAG_GANG_FEW_NODES) ? 1 : 2;
@@ -1189,10 +1195,14 @@ int isl_create(const isl_config* cfg, isl_engine** out) {
     if (cfg->policy > ISL_POLICY_LEAST_ALLOCATED) return ISL_EINVAL;
     if (node_scoring(cfg->policy) && (cfg->flags & ISL_FLAG_ALL_NODES)) return ISL_EINVAL;     // a pod on every node: no node to choose
     // node-scored gangs (N1): only under node scoring, not with few-node or elastic gangs; they lift the locality flags' refusal of node
-    // scoring below.  A pod on every node is refused by node scoring itself.
-    const bool gang_score = cfg->flags & ISL_FLAG_GANG_NODE_SCORE;
-    if (gang_score && (!node_scoring(cfg->policy) || (cfg->flags & (ISL_FLAG_GANG_FEW_NODES | ISL_FLAG_GANG_MIN_MEMBERS)))) return ISL_EINVAL;
+    // scoring below.  A pod on every node is refused by node scoring itself.  Every gang kind (C1): only on a node-scored gang engine; it
+    // lifts the refusal of few-node, elastic and balanced gangs under node scoring.
+    const bool gang_score = cfg->flags & ISL_FLAG_GANG_NODE_SCORE, score_all = cfg->flags & ISL_FLAG_GANG_NODE_SCORE_ALL;
+    if (score_all && !gang_score) return ISL_EINVAL;
+    if (gang_score && (!node_scoring(cfg->policy) || (!score_all && (cfg->flags & (ISL_FLAG_GANG_FEW_NODES | ISL_FLAG_GANG_MIN_MEMBERS)))))
+        return ISL_EINVAL;
     const bool scored_gangs_refused = node_scoring(cfg->policy) && !gang_score;
+    const bool scored_kinds_refused = node_scoring(cfg->policy) && !score_all;      // few-node, elastic and balanced gangs
     // one-node gangs choose the node by scan order: not with a pod on every node, nor with a policy that scores the nodes unless the
     // node score chooses it (N1)
     if ((cfg->flags & ISL_FLAG_GANG_ONE_NODE) && ((cfg->flags & ISL_FLAG_ALL_NODES) || scored_gangs_refused)) return ISL_EINVAL;
@@ -1200,18 +1210,21 @@ int isl_create(const isl_config* cfg, isl_engine** out) {
     if ((cfg->flags & ISL_FLAG_GANG_DISTINCT_NODES) &&
         ((cfg->flags & (ISL_FLAG_GANG_ONE_NODE | ISL_FLAG_ALL_NODES)) || scored_gangs_refused)) return ISL_EINVAL;
     // few-node gangs: a third locality mode, exclusive with the other two, and, like them, not with a pod on every node nor node scoring
+    // unless every gang kind is scored (C1)
     if ((cfg->flags & ISL_FLAG_GANG_FEW_NODES) &&
-        ((cfg->flags & (ISL_FLAG_GANG_ONE_NODE | ISL_FLAG_GANG_DISTINCT_NODES | ISL_FLAG_ALL_NODES)) || node_scoring(cfg->policy))) return ISL_EINVAL;
+        ((cfg->flags & (ISL_FLAG_GANG_ONE_NODE | ISL_FLAG_GANG_DISTINCT_NODES | ISL_FLAG_ALL_NODES)) || scored_kinds_refused)) return ISL_EINVAL;
     // per-gang locality: the gangs name the locality the other three flags fix for the engine; not with a pod on every node nor unscored
     // under node scoring
     if ((cfg->flags & ISL_FLAG_GANG_LOCALITY) &&
         ((cfg->flags & (ISL_FLAG_GANG_ONE_NODE | ISL_FLAG_GANG_DISTINCT_NODES | ISL_FLAG_GANG_FEW_NODES | ISL_FLAG_ALL_NODES)) ||
          scored_gangs_refused)) return ISL_EINVAL;
     // elastic gangs (M6): with any one locality flag or none (their own checks refuse two), not with a pod on every node nor node scoring
-    if ((cfg->flags & ISL_FLAG_GANG_MIN_MEMBERS) && ((cfg->flags & ISL_FLAG_ALL_NODES) || node_scoring(cfg->policy))) return ISL_EINVAL;
-    // balanced gangs (B6): a locality byte, so only with per-gang locality; not node-scored, not with a pod on every node
+    // unless every gang kind is scored (C1)
+    if ((cfg->flags & ISL_FLAG_GANG_MIN_MEMBERS) && ((cfg->flags & ISL_FLAG_ALL_NODES) || scored_kinds_refused)) return ISL_EINVAL;
+    // balanced gangs (B6): a locality byte, so only with per-gang locality; not with a pod on every node, nor node-scored unless every gang
+    // kind is scored (C1)
     if ((cfg->flags & ISL_FLAG_GANG_BALANCED) &&
-        (!(cfg->flags & ISL_FLAG_GANG_LOCALITY) || node_scoring(cfg->policy) || (cfg->flags & ISL_FLAG_ALL_NODES))) return ISL_EINVAL;
+        (!(cfg->flags & ISL_FLAG_GANG_LOCALITY) || scored_kinds_refused || (cfg->flags & ISL_FLAG_ALL_NODES))) return ISL_EINVAL;
     // gang preemption (P7): few-node and elastic gangs have no preemption order, a pod on every node has no single GPU to evict on
     if ((cfg->flags & ISL_FLAG_GANG_PREEMPT) &&
         (cfg->flags & (ISL_FLAG_ALL_NODES | ISL_FLAG_GANG_FEW_NODES | ISL_FLAG_GANG_MIN_MEMBERS))) return ISL_EINVAL;
@@ -1583,8 +1596,9 @@ int isl_place_gangs(isl_engine* e, uint32_t n_gangs, const uint32_t* gang_off, c
                 // B1: bytes 4..255 are balanced gangs on an ISL_FLAG_GANG_BALANCED engine
                 if ((in[r].start > ISL_GANG_DISTINCT_NODES && !(e->cfg.flags & ISL_FLAG_GANG_BALANCED)) ||
                     (named && in[r].start != locality[i])) return ISL_EINVAL;
-                // N6: few-node gangs are not node-scored
-                if ((e->cfg.flags & ISL_FLAG_GANG_NODE_SCORE) && in[r].start == ISL_GANG_FEW_NODES) return ISL_EINVAL;
+                // N6: few-node gangs are not node-scored, unless the engine scores every gang kind (C2)
+                if ((e->cfg.flags & ISL_FLAG_GANG_NODE_SCORE) && !(e->cfg.flags & ISL_FLAG_GANG_NODE_SCORE_ALL) &&
+                    in[r].start == ISL_GANG_FEW_NODES) return ISL_EINVAL;
                 locality[i] = in[r].start;
                 named = true;
             }

@@ -39,6 +39,7 @@ FLAG_GANG_MIN_MEMBERS = 1024  # elastic gangs: a gang commits its leading member
 FLAG_GANG_PREEMPT = 2048  # isl_preempt picks the victims a whole gang (a run of equal handles) needs, or evicts nothing for it
 FLAG_GANG_NODE_SCORE = 4096  # on a node-scoring engine isl_place_gangs places gangs by MostAllocated / LeastAllocated (N1-N8)
 FLAG_GANG_BALANCED = 8192  # with FLAG_GANG_LOCALITY: a locality of gang_balanced_nodes(k) spreads a gang over the nodes within maxSkew k
+FLAG_GANG_NODE_SCORE_ALL = 16384  # with FLAG_GANG_NODE_SCORE: few-node, elastic and balanced gangs are node-scored too (C1-C8)
 GANG_ANY_NODES, GANG_ONE_NODE, GANG_FEW_NODES, GANG_DISTINCT_NODES = 0, 1, 2, 3     # node locality of one gang (include/islplace.h L1)
 SPEC_AUTO, SPEC_OFF, SPEC_ON = 0, 1, 2
 
@@ -375,6 +376,11 @@ class Engine:
         score for the gang's slices taken as one pod.  Its locality is ``FLAG_GANG_ONE_NODE``, ``FLAG_GANG_DISTINCT_NODES``, each gang's
         own under ``FLAG_GANG_LOCALITY`` (``GANG_FEW_NODES`` is refused), or any node.
 
+        With ``FLAG_GANG_NODE_SCORE_ALL`` as well such an engine places every gang kind (include/islplace.h C1-C8): ``FLAG_GANG_FEW_NODES``
+        or ``GANG_FEW_NODES``, ``FLAG_GANG_MIN_MEMBERS`` and ``FLAG_GANG_BALANCED``.  Each kind keeps its own first criterion (a few-node
+        round's depth, an elastic trim's depth, a balanced member's nodes within the skew); the node score breaks the ties below it, where
+        a first-fit engine takes scan order, and the lowest node breaks the ties of the score.
+
         On an engine created with ``FLAG_GANG_LOCALITY | FLAG_GANG_BALANCED`` a locality of ``gang_balanced_nodes(k)`` (4..255) spreads
         the gang's members over the nodes: each member goes, by the engine's policy, to a node whose count of the gang's earlier members
         is at most the least such count over the nodes that admit it plus k - 1 (include/islplace.h B1-B8)."""
@@ -388,7 +394,7 @@ class Engine:
             locality = np.asarray(locality, dtype=np.int64)
             if len(locality) != len(gang_off) - 1:
                 raise ValueError("one locality per gang")
-            if self.flags & FLAG_GANG_NODE_SCORE and (locality == GANG_FEW_NODES).any():
+            if self.flags & FLAG_GANG_NODE_SCORE and not self.flags & FLAG_GANG_NODE_SCORE_ALL and (locality == GANG_FEW_NODES).any():
                 raise ValueError("few-node gangs are not node-scored (FLAG_GANG_NODE_SCORE)")
             if self.flags & FLAG_GANG_BALANCED and len(locality) and (locality.min() < 0 or locality.max() > 255):
                 raise ValueError("a locality is 0..255 (gang_balanced_nodes(1..252) above GANG_DISTINCT_NODES)")

@@ -100,7 +100,8 @@ public:
     // ISL_FLAG_GANG_LOCALITY so that PlaceGangs takes one of these localities per gang; ISL_FLAG_GANG_MIN_MEMBERS (alone or with one of
     // the four) so that PlaceGangs takes a minimum per gang; with a node-scoring policy, ISL_FLAG_GANG_NODE_SCORE (alone or with the
     // one-node, distinct-node or locality flag) so that PlaceGangs places gangs by the node score; with ISL_FLAG_GANG_LOCALITY,
-    // ISL_FLAG_GANG_BALANCED so that a locality of ISL_GANG_BALANCED_NODES(maxSkew) spreads a gang over the nodes
+    // ISL_FLAG_GANG_BALANCED so that a locality of ISL_GANG_BALANCED_NODES(maxSkew) spreads a gang over the nodes; with
+    // ISL_FLAG_GANG_NODE_SCORE, ISL_FLAG_GANG_NODE_SCORE_ALL so that few-node, elastic and balanced gangs are node-scored as well
     explicit InstasliceReconciler(uint32_t quirks = ISL_QUIRKS_REF_EXACT, uint32_t max_gpus = 1u << 16, uint32_t max_batch = 1u << 16,
                                   uint32_t policy = ISL_POLICY_FIRST_FIT, uint32_t flags = 0);
     ~InstasliceReconciler();

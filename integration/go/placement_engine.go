@@ -81,11 +81,15 @@ const (
 	// FlagGangDistinctNodes or FlagGangLocality; not with FlagGangFewNodes or FlagGangMinMembers.
 	FlagGangPreempt = uint32(C.ISL_FLAG_GANG_PREEMPT)
 	// On a PolicyMostAllocated or PolicyLeastAllocated engine, PlaceGangs places gangs by the node score: alone (any node) or with
-	// FlagGangOneNode, FlagGangDistinctNodes or FlagGangLocality (no few-node locality); not with FlagGangFewNodes or FlagGangMinMembers.
+	// FlagGangOneNode, FlagGangDistinctNodes or FlagGangLocality (no few-node locality); not with FlagGangFewNodes or FlagGangMinMembers
+	// unless FlagGangNodeScoreAll is set as well.
 	FlagGangNodeScore = uint32(C.ISL_FLAG_GANG_NODE_SCORE)
 	// With FlagGangLocality: a locality of GangBalancedNodes(maxSkew) spreads a gang's pods over the nodes within that maxSkew
-	// (topologySpreadConstraints on kubernetes.io/hostname).  Not under node scoring.
+	// (topologySpreadConstraints on kubernetes.io/hostname).  Under node scoring only with FlagGangNodeScoreAll.
 	FlagGangBalanced = uint32(C.ISL_FLAG_GANG_BALANCED)
+	// With FlagGangNodeScore: few-node gangs (FlagGangFewNodes or GangFewNodes), elastic gangs (FlagGangMinMembers) and balanced
+	// gangs (FlagGangBalanced) are placed by the node score too, so a packing or spreading cluster needs no second engine for them.
+	FlagGangNodeScoreAll = uint32(C.ISL_FLAG_GANG_NODE_SCORE_ALL)
 )
 
 // StGangTrimmed is the record status of a pod its elastic gang was placed without (isl_result.status, FlagGangMinMembers).
