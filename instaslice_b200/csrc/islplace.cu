@@ -24,64 +24,45 @@ using namespace isl;
 static constexpr uint32_t kMaxStreamChunks = 4096;
 static constexpr uint32_t kSpecRingIds = 1u << 24;     // stream ids of isl_place_stream_partitioned that may speculate
 
-// Engines created with one of these flags place gangs with k_ganglocal, the others with k_bestfit's gang loop.
-constexpr uint32_t kGangTopologyFlags = ISL_FLAG_GANG_ONE_NODE | ISL_FLAG_GANG_FEW_NODES | ISL_FLAG_GANG_DISTINCT_NODES |
-                                        ISL_FLAG_GANG_LOCALITY | ISL_FLAG_GANG_MIN_MEMBERS | ISL_FLAG_GANG_NODE_SCORE | ISL_FLAG_GANG_BALANCED;
-
-// The instantiations of k_ganglocal, one per kind of gang-topology engine (gang_kind), with the name a launch error carries; wins:
-// distinct-node gangs may run, which stack their wins in GangNode::wins, or balanced gangs, which keep their per-node counts there.
+// One instantiation of k_ganglocal or k_preempt_gangs: the template arguments it was built with and the name a launch error carries.
 struct GangKernel {
     const void* fn;
     const char* name;
-    bool wins;
+    uint32_t loc;                    // kLoc: an ISL_GANG_* byte for every gang, or kLocPerGang
+    bool min, score, bal;            // kMin, kScore, kBal of k_ganglocal; false for k_preempt_gangs
 };
-constexpr uint32_t kGangKinds = 15;
-const GangKernel kGangKernels[kGangKinds] = {
-    {(const void*)k_ganglocal<ISL_GANG_ONE_NODE>, "k_ganglocal<one_node>", false},
-    {(const void*)k_ganglocal<ISL_GANG_FEW_NODES>, "k_ganglocal<few_nodes>", false},
-    {(const void*)k_ganglocal<ISL_GANG_DISTINCT_NODES>, "k_ganglocal<distinct_nodes>", true},
-    {(const void*)k_ganglocal<kLocPerGang, false>, "k_ganglocal<per_gang>", true},
-    {(const void*)k_ganglocal<kLocPerGang, true>, "k_ganglocal<per_gang, min_members>", true},
-    {(const void*)k_ganglocal<ISL_GANG_ANY_NODES, false, true>, "k_ganglocal<any_node, node_score>", false},
-    {(const void*)k_ganglocal<ISL_GANG_ONE_NODE, false, true>, "k_ganglocal<one_node, node_score>", false},
-    {(const void*)k_ganglocal<ISL_GANG_DISTINCT_NODES, false, true>, "k_ganglocal<distinct_nodes, node_score>", true},
-    {(const void*)k_ganglocal<kLocPerGang, false, true>, "k_ganglocal<per_gang, node_score>", true},
-    {(const void*)k_ganglocal<kLocPerGang, false, false, true>, "k_ganglocal<per_gang, balanced>", true},
-    {(const void*)k_ganglocal<kLocPerGang, true, false, true>, "k_ganglocal<per_gang, min_members, balanced>", true},
-    {(const void*)k_ganglocal<ISL_GANG_FEW_NODES, false, true>, "k_ganglocal<few_nodes, node_score>", false},
-    {(const void*)k_ganglocal<kLocPerGang, true, true>, "k_ganglocal<per_gang, min_members, node_score>", true},
-    {(const void*)k_ganglocal<kLocPerGang, false, true, true>, "k_ganglocal<per_gang, node_score, balanced>", true},
-    {(const void*)k_ganglocal<kLocPerGang, true, true, true>, "k_ganglocal<per_gang, min_members, node_score, balanced>", true},
+const GangKernel kGangKernels[] = {
+    {(const void*)k_ganglocal<ISL_GANG_ONE_NODE>, "k_ganglocal<one_node>", ISL_GANG_ONE_NODE, false, false, false},
+    {(const void*)k_ganglocal<ISL_GANG_FEW_NODES>, "k_ganglocal<few_nodes>", ISL_GANG_FEW_NODES, false, false, false},
+    {(const void*)k_ganglocal<ISL_GANG_DISTINCT_NODES>, "k_ganglocal<distinct_nodes>", ISL_GANG_DISTINCT_NODES, false, false, false},
+    {(const void*)k_ganglocal<kLocPerGang, false>, "k_ganglocal<per_gang>", kLocPerGang, false, false, false},
+    {(const void*)k_ganglocal<kLocPerGang, true>, "k_ganglocal<per_gang, min_members>", kLocPerGang, true, false, false},
+    {(const void*)k_ganglocal<ISL_GANG_ANY_NODES, false, true>, "k_ganglocal<any_node, node_score>", ISL_GANG_ANY_NODES, false, true, false},
+    {(const void*)k_ganglocal<ISL_GANG_ONE_NODE, false, true>, "k_ganglocal<one_node, node_score>", ISL_GANG_ONE_NODE, false, true, false},
+    {(const void*)k_ganglocal<ISL_GANG_DISTINCT_NODES, false, true>, "k_ganglocal<distinct_nodes, node_score>", ISL_GANG_DISTINCT_NODES, false, true, false},
+    {(const void*)k_ganglocal<kLocPerGang, false, true>, "k_ganglocal<per_gang, node_score>", kLocPerGang, false, true, false},
+    {(const void*)k_ganglocal<kLocPerGang, false, false, true>, "k_ganglocal<per_gang, balanced>", kLocPerGang, false, false, true},
+    {(const void*)k_ganglocal<kLocPerGang, true, false, true>, "k_ganglocal<per_gang, min_members, balanced>", kLocPerGang, true, false, true},
+    {(const void*)k_ganglocal<ISL_GANG_FEW_NODES, false, true>, "k_ganglocal<few_nodes, node_score>", ISL_GANG_FEW_NODES, false, true, false},
+    {(const void*)k_ganglocal<kLocPerGang, true, true>, "k_ganglocal<per_gang, min_members, node_score>", kLocPerGang, true, true, false},
+    {(const void*)k_ganglocal<kLocPerGang, false, true, true>, "k_ganglocal<per_gang, node_score, balanced>", kLocPerGang, false, true, true},
+    {(const void*)k_ganglocal<kLocPerGang, true, true, true>, "k_ganglocal<per_gang, min_members, node_score, balanced>", kLocPerGang, true, true, true},
+};
+const GangKernel kPreemptGangKernels[] = {
+    {(const void*)k_preempt_gangs<ISL_GANG_ANY_NODES>, "k_preempt_gangs<any_node>", ISL_GANG_ANY_NODES, false, false, false},
+    {(const void*)k_preempt_gangs<ISL_GANG_ONE_NODE>, "k_preempt_gangs<one_node>", ISL_GANG_ONE_NODE, false, false, false},
+    {(const void*)k_preempt_gangs<ISL_GANG_DISTINCT_NODES>, "k_preempt_gangs<distinct_nodes>", ISL_GANG_DISTINCT_NODES, false, false, false},
+    {(const void*)k_preempt_gangs<kLocPerGang>, "k_preempt_gangs<per_gang>", kLocPerGang, false, false, false},
 };
 
-// The kGangKernels entry of an engine with a gang-topology flag: each gang's own byte under ISL_FLAG_GANG_LOCALITY, and under
-// ISL_FLAG_GANG_MIN_MEMBERS with its minimum as well, else the locality of the engine's flag for every gang.  An
-// ISL_FLAG_GANG_NODE_SCORE engine takes the node-scored instantiation of its locality, any node without a locality flag; elastic and
-// few-node gangs come only with ISL_FLAG_GANG_NODE_SCORE_ALL.  An ISL_FLAG_GANG_BALANCED engine (always with ISL_FLAG_GANG_LOCALITY,
-// node-scored only with ISL_FLAG_GANG_NODE_SCORE_ALL) takes the balanced per-gang instantiation, elastic or not, scored or not.
-uint32_t gang_kind(uint32_t flags) {
-    const bool min = flags & ISL_FLAG_GANG_MIN_MEMBERS;
-    if (flags & ISL_FLAG_GANG_BALANCED) return (flags & ISL_FLAG_GANG_NODE_SCORE) ? (min ? 14 : 13) : (min ? 10 : 9);
-    if (flags & ISL_FLAG_GANG_NODE_SCORE)
-        return min ? 12 : (flags & ISL_FLAG_GANG_LOCALITY) ? 8 : (flags & ISL_FLAG_GANG_ONE_NODE) ? 6 : (flags & ISL_FLAG_GANG_DISTINCT_NODES) ? 7
-                    : (flags & ISL_FLAG_GANG_FEW_NODES) ? 11 : 5;
-    if (flags & ISL_FLAG_GANG_MIN_MEMBERS) return 4;
-    if (flags & ISL_FLAG_GANG_LOCALITY) return 3;
-    return (flags & ISL_FLAG_GANG_ONE_NODE) ? 0 : (flags & ISL_FLAG_GANG_FEW_NODES) ? 1 : 2;
-}
-
-// The instantiations of k_preempt_gangs, one per kind of ISL_FLAG_GANG_PREEMPT engine (preempt_gang_kind).
-constexpr uint32_t kPreemptGangKinds = 4;
-const GangKernel kPreemptGangKernels[kPreemptGangKinds] = {
-    {(const void*)k_preempt_gangs<ISL_GANG_ANY_NODES>, "k_preempt_gangs<any_node>", false},
-    {(const void*)k_preempt_gangs<ISL_GANG_ONE_NODE>, "k_preempt_gangs<one_node>", false},
-    {(const void*)k_preempt_gangs<ISL_GANG_DISTINCT_NODES>, "k_preempt_gangs<distinct_nodes>", false},
-    {(const void*)k_preempt_gangs<kLocPerGang>, "k_preempt_gangs<per_gang>", false},
+// What kind of gang engine a config makes, decoded once by isl_create from its flags and policy (gang_mode).
+struct GangMode {
+    uint32_t locality = ISL_GANG_ANY_NODES;      // an ISL_GANG_* byte for every gang, or kLocPerGang (ISL_FLAG_GANG_LOCALITY)
+    bool min_members = false, node_score = false, score_all = false, balanced = false;
+    bool gangs_refused = false;                  // isl_place_gangs refuses every call
+    const GangKernel* place = nullptr;           // the k_ganglocal isl_place_gangs launches; none: k_bestfit's gang loop
+    const GangKernel* preempt = nullptr;         // the k_preempt_gangs isl_preempt launches; none: k_preempt, gangs of one
 };
-uint32_t preempt_gang_kind(uint32_t flags) {
-    if (flags & ISL_FLAG_GANG_LOCALITY) return 3;
-    return (flags & ISL_FLAG_GANG_ONE_NODE) ? 1 : (flags & ISL_FLAG_GANG_DISTINCT_NODES) ? 2 : 0;
-}
 
 // What plan_pipeline decides for one k_pipeline launch: GPUs per stage (seg), stages, GPUs per sub-segment, speculative rounds.
 struct PipePlan {
@@ -229,14 +210,14 @@ struct isl_engine {
     // isl_preempt: the victim-index map (8 words per GPU of the partition), the victims, staging of [candidate masks | priorities], the
     // evict rows, the per-CTA minima of k_preempt and k_victim_map's error word.  ISL_FLAG_GANG_PREEMPT (k_preempt_gangs): the gang
     // offsets followed by the locality bytes, the rollback log (one entry per request), the per-GPU state when the shares do not fit in
-    // shared memory, and the dynamic shared memory one CTA of each instantiation may have
+    // shared memory, and the dynamic shared memory one CTA of the engine's instantiation may have
     struct Preempt {
         DevMem<uint32_t> vmap, evict, err, gangs;
         DevMem<isl_victim> victims;
         DevMem<uint8_t> stage, state;
         DevMem<unsigned long long> keys;
         DevMem<PgLog> log;
-        int optin[kPreemptGangKinds] = {};
+        int optin = 0;
     } pre;
     // node scoring (k_nodefit): the inventory's node offsets (isl_load_inventory), the per-profile min-trees when they do not fit in shared
     // memory, the per-(profile, node) fit counts and the per-node busy / cap words, grown to the partition; the width of every table
@@ -244,17 +225,18 @@ struct isl_engine {
         DevMem<uint32_t> node_off, tree, fit, nodes;
         uint8_t width[kMaxTables] = {};
     } nf;
-    // gang topology (kGangTopologyFlags, k_ganglocal): the inventory's node offsets in storage order (host and device,
-    // isl_load_inventory), the scratch copies or node-used marks when the shares do not fit in shared memory, the per-CTA minima, and
-    // the per-CTA stacks of wins of distinct-node gangs
+    // gang topology (gang.place, k_ganglocal): the inventory's node offsets in storage order (host and device, isl_load_inventory), the
+    // scratch copies or node-used marks when the shares do not fit in shared memory, the per-CTA minima, and the per-CTA stacks of wins
+    // of distinct-node gangs
     struct GangNode {
         std::vector<uint32_t> off;
         DevMem<uint32_t> node_off;
         DevMem<uint8_t> scratch;
         DevMem<unsigned long long> keys;
         DevMem<uint2> wins;
-        int optin[kGangKinds] = {};  // dynamic shared memory one CTA of each kGangKernels instantiation may have
+        int optin = 0;               // dynamic shared memory one CTA of gang.place may have
     } gn;
+    GangMode gang;
     unsigned long long wait_ns = 20000000000ull;   // a starved device-side wait traps after this long (ISL_WAIT_SECONDS overrides the 20 s)
     uint32_t window = 0;             // causal window of stream calls (isl_set_causal_window): chunk c starts after chunk c - window is committed
     uint32_t spec_mode = ISL_SPEC_AUTO;     // speculative rounds (isl_set_speculation); ISL_SPEC=0|1 in the environment overrides
@@ -288,6 +270,68 @@ inline bool node_scoring(uint32_t policy) { return policy == ISL_POLICY_MOST_ALL
 // partitioned calls or open streams, at most kBfMaxGpus GPUs
 inline bool request_major(uint32_t policy) { return bestfit_family(policy) || node_scoring(policy); }
 inline bool reversed(const isl_engine* e) { return e->cfg.policy == ISL_POLICY_RIGHT_TO_LEFT; }
+
+// The entry of `table` built with these template arguments, nullptr when none is
+template <size_t N>
+const GangKernel* find_gang_kernel(const GangKernel (&table)[N], uint32_t loc, bool min, bool score, bool bal) {
+    for (const GangKernel& k : table)
+        if (k.loc == loc && k.min == min && k.score == score && k.bal == bal) return &k;
+    return nullptr;
+}
+
+// The gang mode of a config with a valid policy, or ISL_EINVAL for a combination of gang flags and policy isl_create refuses: the
+// rules of G5, S6, F6, L5, M6, P7, N1, B6 and C1 in include/islplace.h.  Elastic gangs read each gang's byte, so they run the per-gang
+// k_ganglocal, whose bytes isl_place_gangs fills with the engine's locality when the gangs do not name it.
+int gang_mode(const isl_config* cfg, GangMode* m) {
+    const uint32_t f = cfg->flags;
+    const bool scoring = node_scoring(cfg->policy);
+    auto has = [f](uint32_t bits) { return (f & bits) != 0; };
+    const uint32_t localities = f & (ISL_FLAG_GANG_ONE_NODE | ISL_FLAG_GANG_DISTINCT_NODES | ISL_FLAG_GANG_FEW_NODES | ISL_FLAG_GANG_LOCALITY);
+    const uint32_t gang_flags = ISL_FLAG_GANG_ONE_NODE | ISL_FLAG_GANG_DISTINCT_NODES | ISL_FLAG_GANG_FEW_NODES | ISL_FLAG_GANG_LOCALITY |
+                                ISL_FLAG_GANG_MIN_MEMBERS | ISL_FLAG_GANG_PREEMPT | ISL_FLAG_GANG_NODE_SCORE | ISL_FLAG_GANG_BALANCED |
+                                ISL_FLAG_GANG_NODE_SCORE_ALL;
+    if (localities & (localities - 1)) return ISL_EINVAL;                       // at most one locality flag
+    if (has(ISL_FLAG_ALL_NODES) && has(gang_flags)) return ISL_EINVAL;           // a pod on every node: no gang kind applies
+    if (has(ISL_FLAG_GANG_NODE_SCORE_ALL) && !has(ISL_FLAG_GANG_NODE_SCORE)) return ISL_EINVAL;
+    if (has(ISL_FLAG_GANG_NODE_SCORE) && !scoring) return ISL_EINVAL;
+    // under node scoring a gang kind takes the node score, or is refused
+    if (scoring && has(ISL_FLAG_GANG_ONE_NODE | ISL_FLAG_GANG_DISTINCT_NODES | ISL_FLAG_GANG_LOCALITY) && !has(ISL_FLAG_GANG_NODE_SCORE))
+        return ISL_EINVAL;
+    if (scoring && has(ISL_FLAG_GANG_FEW_NODES | ISL_FLAG_GANG_MIN_MEMBERS | ISL_FLAG_GANG_BALANCED) && !has(ISL_FLAG_GANG_NODE_SCORE_ALL))
+        return ISL_EINVAL;
+    if (has(ISL_FLAG_GANG_BALANCED) && !has(ISL_FLAG_GANG_LOCALITY)) return ISL_EINVAL;        // the maxSkew is a locality byte
+    if (has(ISL_FLAG_GANG_PREEMPT) && has(ISL_FLAG_GANG_FEW_NODES | ISL_FLAG_GANG_MIN_MEMBERS)) return ISL_EINVAL;     // no preemption order
+    m->locality = has(ISL_FLAG_GANG_LOCALITY)        ? kLocPerGang
+                  : has(ISL_FLAG_GANG_ONE_NODE)      ? ISL_GANG_ONE_NODE
+                  : has(ISL_FLAG_GANG_FEW_NODES)     ? ISL_GANG_FEW_NODES
+                  : has(ISL_FLAG_GANG_DISTINCT_NODES) ? ISL_GANG_DISTINCT_NODES
+                                                      : ISL_GANG_ANY_NODES;
+    m->min_members = has(ISL_FLAG_GANG_MIN_MEMBERS);
+    m->node_score = has(ISL_FLAG_GANG_NODE_SCORE);
+    m->score_all = has(ISL_FLAG_GANG_NODE_SCORE_ALL);
+    m->balanced = has(ISL_FLAG_GANG_BALANCED);
+    m->gangs_refused = has(ISL_FLAG_ALL_NODES) || (scoring && !m->node_score);
+    // every mode the rules accept has its instantiations; one without would be refused here, never run on another kernel
+    if ((m->locality != ISL_GANG_ANY_NODES || m->min_members || m->node_score) &&
+        !(m->place = find_gang_kernel(kGangKernels, m->min_members ? kLocPerGang : m->locality, m->min_members, m->node_score, m->balanced)))
+        return ISL_EINVAL;
+    if (has(ISL_FLAG_GANG_PREEMPT) && !(m->preempt = find_gang_kernel(kPreemptGangKernels, m->locality, false, false, false))) return ISL_EINVAL;
+    return ISL_OK;
+}
+
+// The byte field(r) that every ALLOC request r of in[r0, r1) carries, in *v (left as it was when none is an ALLOC): the number of ALLOC
+// requests, or -1 when two of them differ.
+template <typename Field>
+int64_t alloc_shared(const isl_request* in, uint32_t r0, uint32_t r1, Field field, uint8_t* v) {
+    int64_t k = 0;
+    for (uint32_t r = r0; r < r1; ++r) {
+        if (in[r].op != ISL_OP_ALLOC) continue;
+        if (k && field(r) != *v) return -1;
+        *v = field(r);
+        ++k;
+    }
+    return k;
+}
 
 // A canonical GPU range [lo, hi) in storage order (ISL_POLICY_RIGHT_TO_LEFT stores the inventory reversed), or back: its own inverse
 std::pair<uint32_t, uint32_t> storage_range(const isl_engine* e, uint32_t lo, uint32_t hi) { return e->prof.flip ? std::make_pair(e->G - hi, e->G - lo) : std::make_pair(lo, hi); }
@@ -544,24 +588,24 @@ int gang_layout(isl_engine* e, const void* kernel, int smem_optin, uint32_t per_
     return ISL_OK;
 }
 
-// isl_place_gangs on an engine with a gang-topology flag: frees + defaults, then one cooperative launch of kGangKernels[kind]
-// (gang_layout with the instantiation's own opt-in).  Under ISL_FLAG_GANG_LOCALITY or ISL_FLAG_GANG_MIN_MEMBERS it places each gang by
-// the byte at d_locality[gang], and under ISL_FLAG_GANG_MIN_MEMBERS it reads each gang's minimum m' from the uint32 words that follow
-// the bytes (rounded up to 4).  CTA c of an instantiation that runs distinct-node gangs stacks its wins in gn.wins[cta_node[c] ..), at
-// most one per node it owns; a balanced instantiation keeps the count of node j in gn.wins[j] as well.
-int run_ganglocal(isl_engine* e, uint32_t kind, uint32_t n_gangs, const uint32_t* d_gang_off, const uint8_t* d_locality, uint32_t n,
+// isl_place_gangs on an engine with a k_ganglocal instantiation (gang.place): frees + defaults, then one cooperative launch of it
+// (gang_layout with its opt-in).  An instantiation of kLocPerGang places each gang by the byte at d_locality[gang], and one of kMin
+// reads each gang's minimum m' from the uint32 words that follow the bytes (rounded up to 4).  CTA c of an instantiation that runs
+// distinct-node gangs stacks its wins in gn.wins[cta_node[c] ..), at most one per node it owns; a balanced instantiation keeps the
+// count of node j in gn.wins[j] as well.
+int run_ganglocal(isl_engine* e, uint32_t n_gangs, const uint32_t* d_gang_off, const uint8_t* d_locality, uint32_t n,
                   const uint2* d_in, uint2* d_out) {
-    const GangKernel& k = kGangKernels[kind];
+    const GangKernel& k = *e->gang.place;
     if (int rc = prepare_batch(e, n, d_in, d_out)) return rc;
     GangScoreArgs a;            // the node-scored instantiations read all of it, the others its GangNodeArgs part
     uint32_t grid, nodes;
     size_t smem;
-    if (int rc = gang_layout(e, k.fn, e->gn.optin[kind], 2, n_gangs, d_gang_off, d_in, d_out, a, &grid, &smem, &nodes)) return rc;
+    if (int rc = gang_layout(e, k.fn, e->gn.optin, 2, n_gangs, d_gang_off, d_in, d_out, a, &grid, &smem, &nodes)) return rc;
     memcpy(a.width, e->nf.width, sizeof a.width);
     a.most = e->cfg.policy == ISL_POLICY_MOST_ALLOCATED;
     if (!smem) ISL_CUDA(e, e->gn.scratch.reserve(e->hi - e->lo));     // the second byte per GPU; the live bytes are the occupancy
     a.scratch = e->gn.scratch;
-    if (k.wins) ISL_CUDA(e, e->gn.wins.reserve(nodes));
+    if (k.loc == ISL_GANG_DISTINCT_NODES || k.loc == kLocPerGang) ISL_CUDA(e, e->gn.wins.reserve(nodes));
     uint2* wins = e->gn.wins;
     void* params[] = {&a, &e->prof, &wins, &d_locality};
     if (int rc = launch_cooperative(e, k.fn, k.name, grid, kGnThreads, smem, params)) return rc;
@@ -1194,45 +1238,14 @@ int isl_create(const isl_config* cfg, isl_engine** out) {
     if (cfg->max_gpus == 0 || cfg->max_gpus > ISL_MAX_GPUS || cfg->max_batch == 0) return ISL_EINVAL;
     if (cfg->policy > ISL_POLICY_LEAST_ALLOCATED) return ISL_EINVAL;
     if (node_scoring(cfg->policy) && (cfg->flags & ISL_FLAG_ALL_NODES)) return ISL_EINVAL;     // a pod on every node: no node to choose
-    // node-scored gangs (N1): only under node scoring, not with few-node or elastic gangs; they lift the locality flags' refusal of node
-    // scoring below.  A pod on every node is refused by node scoring itself.  Every gang kind (C1): only on a node-scored gang engine; it
-    // lifts the refusal of few-node, elastic and balanced gangs under node scoring.
-    const bool gang_score = cfg->flags & ISL_FLAG_GANG_NODE_SCORE, score_all = cfg->flags & ISL_FLAG_GANG_NODE_SCORE_ALL;
-    if (score_all && !gang_score) return ISL_EINVAL;
-    if (gang_score && (!node_scoring(cfg->policy) || (!score_all && (cfg->flags & (ISL_FLAG_GANG_FEW_NODES | ISL_FLAG_GANG_MIN_MEMBERS)))))
-        return ISL_EINVAL;
-    const bool scored_gangs_refused = node_scoring(cfg->policy) && !gang_score;
-    const bool scored_kinds_refused = node_scoring(cfg->policy) && !score_all;      // few-node, elastic and balanced gangs
-    // one-node gangs choose the node by scan order: not with a pod on every node, nor with a policy that scores the nodes unless the
-    // node score chooses it (N1)
-    if ((cfg->flags & ISL_FLAG_GANG_ONE_NODE) && ((cfg->flags & ISL_FLAG_ALL_NODES) || scored_gangs_refused)) return ISL_EINVAL;
-    // distinct-node gangs: the opposite of one-node gangs, and, like them, not with a pod on every node nor unscored under node scoring
-    if ((cfg->flags & ISL_FLAG_GANG_DISTINCT_NODES) &&
-        ((cfg->flags & (ISL_FLAG_GANG_ONE_NODE | ISL_FLAG_ALL_NODES)) || scored_gangs_refused)) return ISL_EINVAL;
-    // few-node gangs: a third locality mode, exclusive with the other two, and, like them, not with a pod on every node nor node scoring
-    // unless every gang kind is scored (C1)
-    if ((cfg->flags & ISL_FLAG_GANG_FEW_NODES) &&
-        ((cfg->flags & (ISL_FLAG_GANG_ONE_NODE | ISL_FLAG_GANG_DISTINCT_NODES | ISL_FLAG_ALL_NODES)) || scored_kinds_refused)) return ISL_EINVAL;
-    // per-gang locality: the gangs name the locality the other three flags fix for the engine; not with a pod on every node nor unscored
-    // under node scoring
-    if ((cfg->flags & ISL_FLAG_GANG_LOCALITY) &&
-        ((cfg->flags & (ISL_FLAG_GANG_ONE_NODE | ISL_FLAG_GANG_DISTINCT_NODES | ISL_FLAG_GANG_FEW_NODES | ISL_FLAG_ALL_NODES)) ||
-         scored_gangs_refused)) return ISL_EINVAL;
-    // elastic gangs (M6): with any one locality flag or none (their own checks refuse two), not with a pod on every node nor node scoring
-    // unless every gang kind is scored (C1)
-    if ((cfg->flags & ISL_FLAG_GANG_MIN_MEMBERS) && ((cfg->flags & ISL_FLAG_ALL_NODES) || scored_kinds_refused)) return ISL_EINVAL;
-    // balanced gangs (B6): a locality byte, so only with per-gang locality; not with a pod on every node, nor node-scored unless every gang
-    // kind is scored (C1)
-    if ((cfg->flags & ISL_FLAG_GANG_BALANCED) &&
-        (!(cfg->flags & ISL_FLAG_GANG_LOCALITY) || scored_kinds_refused || (cfg->flags & ISL_FLAG_ALL_NODES))) return ISL_EINVAL;
-    // gang preemption (P7): few-node and elastic gangs have no preemption order, a pod on every node has no single GPU to evict on
-    if ((cfg->flags & ISL_FLAG_GANG_PREEMPT) &&
-        (cfg->flags & (ISL_FLAG_ALL_NODES | ISL_FLAG_GANG_FEW_NODES | ISL_FLAG_GANG_MIN_MEMBERS))) return ISL_EINVAL;
+    GangMode gang;
+    if (int rc = gang_mode(cfg, &gang)) return rc;
     if (request_major(cfg->policy) && cfg->max_gpus > kBfMaxGpus) return ISL_ERANGE;
     if (cfg->quirks & ~ISL_QUIRKS_REF_EXACT) return ISL_EINVAL;
     isl_engine* e = new (std::nothrow) isl_engine;
     if (!e) return ISL_ENOMEM;
     e->cfg = *cfg;
+    e->gang = gang;
     {   // pipeline chunk size: ISL_PIPE_CHUNK (requests, rounded to tiles) overrides the default
         uint32_t pc = kChunk;
         if (const char* v = getenv("ISL_PIPE_CHUNK")) pc = (uint32_t)strtoul(v, nullptr, 10);
@@ -1278,16 +1291,16 @@ int isl_create(const isl_config* cfg, isl_engine** out) {
         ISL_TRY(cudaFuncGetAttributes(&fa, k_preempt));
         ISL_TRY(cudaFuncSetAttribute((const void*)k_preempt, cudaFuncAttributeMaxDynamicSharedMemorySize, optin - (int)fa.sharedSizeBytes));
         // each k_ganglocal instantiation (loaded here as well): its shares may have what the device lets one CTA have beside the
-        // instantiation's own static words
-        for (uint32_t i = 0; i < kGangKinds; ++i) {
-            ISL_TRY(cudaFuncGetAttributes(&fa, kGangKernels[i].fn));
-            e->gn.optin[i] = optin - (int)fa.sharedSizeBytes;
-            ISL_TRY(cudaFuncSetAttribute(kGangKernels[i].fn, cudaFuncAttributeMaxDynamicSharedMemorySize, e->gn.optin[i]));
+        // instantiation's own static words; the engine keeps the opt-in of the one it launches
+        for (const GangKernel& k : kGangKernels) {
+            ISL_TRY(cudaFuncGetAttributes(&fa, k.fn));
+            ISL_TRY(cudaFuncSetAttribute(k.fn, cudaFuncAttributeMaxDynamicSharedMemorySize, optin - (int)fa.sharedSizeBytes));
+            if (&k == e->gang.place) e->gn.optin = optin - (int)fa.sharedSizeBytes;
         }
-        for (uint32_t i = 0; i < kPreemptGangKinds; ++i) {     // and each k_preempt_gangs instantiation
-            ISL_TRY(cudaFuncGetAttributes(&fa, kPreemptGangKernels[i].fn));
-            e->pre.optin[i] = optin - (int)fa.sharedSizeBytes;
-            ISL_TRY(cudaFuncSetAttribute(kPreemptGangKernels[i].fn, cudaFuncAttributeMaxDynamicSharedMemorySize, e->pre.optin[i]));
+        for (const GangKernel& k : kPreemptGangKernels) {     // and each k_preempt_gangs instantiation
+            ISL_TRY(cudaFuncGetAttributes(&fa, k.fn));
+            ISL_TRY(cudaFuncSetAttribute(k.fn, cudaFuncAttributeMaxDynamicSharedMemorySize, optin - (int)fa.sharedSizeBytes));
+            if (&k == e->gang.preempt) e->pre.optin = optin - (int)fa.sharedSizeBytes;
         }
     }
     e->occ_bytes = ((size_t)cfg->max_gpus + kSweepBlock - 1) / kSweepBlock * kSweepBlock;
@@ -1499,7 +1512,7 @@ int isl_load_inventory(isl_engine* e, uint32_t n_nodes, const uint32_t* node_off
         ISL_CUDA(e, e->nf.node_off.replace((size_t)n_nodes + 1));
         ISL_CUDA(e, cudaMemcpyAsync(e->nf.node_off, node_off, ((size_t)n_nodes + 1) * sizeof(uint32_t), cudaMemcpyHostToDevice, e->stream));
     }
-    if (e->cfg.flags & (kGangTopologyFlags | ISL_FLAG_GANG_PREEMPT)) {
+    if (e->gang.place || e->gang.preempt) {
         // k_ganglocal and k_preempt_gangs walk the nodes in storage order (reversed under right-to-left)
         auto& off = e->gn.off;
         off.assign(node_off, node_off + n_nodes + 1);
@@ -1586,46 +1599,32 @@ int isl_place_gangs(isl_engine* e, uint32_t n_gangs, const uint32_t* gang_off, c
     for (uint32_t i = 0; i < n_gangs; ++i) if (gang_off[i + 1] <= gang_off[i]) return ISL_EINVAL;      // no empty gang
     const uint32_t n = n_gangs ? gang_off[n_gangs] : 0;
     if (n && (!in || !out)) return ISL_EINVAL;
-    std::vector<uint8_t> locality;                                  // ISL_FLAG_GANG_LOCALITY: each gang's byte (L1, L4), 0 without ALLOCs
-    if (e->cfg.flags & ISL_FLAG_GANG_LOCALITY) {
-        locality.assign(n_gangs, (uint8_t)ISL_GANG_ANY_NODES);
+    // one pod on every node with capacity has no all-or-nothing meaning; gangs under node scoring only on an ISL_FLAG_GANG_NODE_SCORE engine
+    const GangMode& m = e->gang;
+    if (m.gangs_refused) return ISL_EINVAL;
+    // per-gang bytes: each gang's locality (L1, L4), the engine's under ISL_FLAG_GANG_MIN_MEMBERS without ISL_FLAG_GANG_LOCALITY, and its
+    // m' (M1, M6); 0 for a gang without ALLOCs
+    const bool per_gang = m.locality == kLocPerGang;
+    std::vector<uint8_t> locality;
+    std::vector<uint32_t> min_members;
+    if (per_gang || m.min_members) {
+        locality.assign(n_gangs, (uint8_t)(per_gang ? ISL_GANG_ANY_NODES : m.locality));
+        min_members.assign(m.min_members ? n_gangs : 0, 0);
         for (uint32_t i = 0; i < n_gangs; ++i) {
-            bool named = false;
-            for (uint32_t r = gang_off[i]; r < gang_off[i + 1]; ++r) {
-                if (in[r].op != ISL_OP_ALLOC) continue;
-                // B1: bytes 4..255 are balanced gangs on an ISL_FLAG_GANG_BALANCED engine
-                if ((in[r].start > ISL_GANG_DISTINCT_NODES && !(e->cfg.flags & ISL_FLAG_GANG_BALANCED)) ||
-                    (named && in[r].start != locality[i])) return ISL_EINVAL;
-                // N6: few-node gangs are not node-scored, unless the engine scores every gang kind (C2)
-                if ((e->cfg.flags & ISL_FLAG_GANG_NODE_SCORE) && !(e->cfg.flags & ISL_FLAG_GANG_NODE_SCORE_ALL) &&
-                    in[r].start == ISL_GANG_FEW_NODES) return ISL_EINVAL;
-                locality[i] = in[r].start;
-                named = true;
+            const uint32_t r0 = gang_off[i], r1 = gang_off[i + 1];
+            // B1: bytes 4..255 are balanced gangs on an ISL_FLAG_GANG_BALANCED engine.  N6: few-node gangs are not node-scored, unless
+            // the engine scores every gang kind (C2)
+            if (per_gang && (alloc_shared(in, r0, r1, [&](uint32_t r) { return in[r].start; }, &locality[i]) < 0 ||
+                             (locality[i] > ISL_GANG_DISTINCT_NODES && !m.balanced) ||
+                             (locality[i] == ISL_GANG_FEW_NODES && m.node_score && !m.score_all))) return ISL_EINVAL;
+            if (m.min_members) {
+                uint8_t size = 0;
+                const int64_t k = alloc_shared(in, r0, r1, [&](uint32_t r) { return in[r].size; }, &size);
+                if (k < 0) return ISL_EINVAL;
+                min_members[i] = (size == 0 || size >= k) ? (uint32_t)k : size;
             }
         }
     }
-    std::vector<uint32_t> min_members;                              // ISL_FLAG_GANG_MIN_MEMBERS: each gang's m' (M1, M6), 0 without ALLOCs
-    if (e->cfg.flags & ISL_FLAG_GANG_MIN_MEMBERS) {
-        const uint8_t loc = (e->cfg.flags & ISL_FLAG_GANG_ONE_NODE)         ? (uint8_t)ISL_GANG_ONE_NODE
-                            : (e->cfg.flags & ISL_FLAG_GANG_FEW_NODES)      ? (uint8_t)ISL_GANG_FEW_NODES
-                            : (e->cfg.flags & ISL_FLAG_GANG_DISTINCT_NODES) ? (uint8_t)ISL_GANG_DISTINCT_NODES
-                                                                            : (uint8_t)ISL_GANG_ANY_NODES;
-        if (locality.empty()) locality.assign(n_gangs, loc);       // the engine's locality for every gang
-        min_members.assign(n_gangs, 0);
-        for (uint32_t i = 0; i < n_gangs; ++i) {
-            uint32_t k = 0, m = 0;
-            for (uint32_t r = gang_off[i]; r < gang_off[i + 1]; ++r) {
-                if (in[r].op != ISL_OP_ALLOC) continue;
-                if (k && in[r].size != m) return ISL_EINVAL;
-                m = in[r].size;
-                ++k;
-            }
-            min_members[i] = (m == 0 || m >= k) ? k : m;
-        }
-    }
-    if (e->cfg.flags & ISL_FLAG_ALL_NODES) return ISL_EINVAL;      // one pod on every node with capacity: no all-or-nothing meaning
-    // gangs under node scoring only on an ISL_FLAG_GANG_NODE_SCORE engine
-    if (node_scoring(e->cfg.policy) && !(e->cfg.flags & ISL_FLAG_GANG_NODE_SCORE)) return ISL_EINVAL;
     if (n > e->cfg.max_batch) return ISL_ERANGE;
     Entry guard(e, Needs::ready, n);
     if (guard.rc) return guard.rc;
@@ -1642,9 +1641,8 @@ int isl_place_gangs(isl_engine* e, uint32_t n_gangs, const uint32_t* gang_off, c
         ISL_CUDA(e, cudaMemcpyAsync((uint8_t*)e->d_scratch.get() + min_at, min_members.data(), min_members.size() * sizeof(uint32_t),
                                     cudaMemcpyHostToDevice, e->stream));
     ISL_CUDA(e, cudaMemcpyAsync(e->d_req, in, (size_t)n * sizeof(isl_request), cudaMemcpyHostToDevice, e->stream));
-    if (int rc = (e->cfg.flags & kGangTopologyFlags)
-                     ? run_ganglocal(e, gang_kind(e->cfg.flags), n_gangs, d_gang_off, d_locality, n, e->d_req, e->d_res)
-                     : run_gangs(e, n_gangs, d_gang_off, n, e->d_req, e->d_res)) return rc;
+    if (int rc = m.place ? run_ganglocal(e, n_gangs, d_gang_off, d_locality, n, e->d_req, e->d_res)
+                         : run_gangs(e, n_gangs, d_gang_off, n, e->d_req, e->d_res)) return rc;
     ISL_CUDA(e, cudaMemcpyAsync(out, e->d_res, (size_t)n * sizeof(isl_result), cudaMemcpyDeviceToHost, e->stream));
     ISL_CUDA(e, cudaStreamSynchronize(e->stream));
     return ISL_OK;
@@ -1656,8 +1654,8 @@ int isl_place_gangs(isl_engine* e, uint32_t n_gangs, const uint32_t* gang_off, c
 int run_preempt_gangs(isl_engine* e, const std::vector<uint32_t>& gang_off, const std::vector<uint8_t>& locality, uint32_t n,
                       const uint8_t* d_prio, const uint8_t* d_masks) {
     auto& p = e->pre;
-    const uint32_t kind = preempt_gang_kind(e->cfg.flags), n_gangs = (uint32_t)gang_off.size() - 1, Gr = e->hi - e->lo;
-    const GangKernel& k = kPreemptGangKernels[kind];
+    const uint32_t n_gangs = (uint32_t)gang_off.size() - 1, Gr = e->hi - e->lo;
+    const GangKernel& k = *e->gang.preempt;
     ISL_CUDA(e, p.gangs.reserve(gang_off.size() + (locality.size() + 3) / 4));
     uint32_t* d_gang_off = p.gangs;
     const uint8_t* d_locality = reinterpret_cast<const uint8_t*>(d_gang_off + gang_off.size());
@@ -1668,7 +1666,7 @@ int run_preempt_gangs(isl_engine* e, const std::vector<uint32_t>& gang_off, cons
     GangNodeArgs a;
     uint32_t grid, nodes;
     size_t smem;
-    if (int rc = gang_layout(e, k.fn, p.optin[kind], kPgBytesPerGpu, n_gangs, d_gang_off, e->d_req, e->d_res, a, &grid, &smem, &nodes)) return rc;
+    if (int rc = gang_layout(e, k.fn, p.optin, kPgBytesPerGpu, n_gangs, d_gang_off, e->d_req, e->d_res, a, &grid, &smem, &nodes)) return rc;
     if (!smem) ISL_CUDA(e, p.state.reserve((size_t)Gr * kPgBytesPerGpu));
     a.scratch = p.state;
     PreemptArgs pa{};
@@ -1689,30 +1687,23 @@ int isl_preempt(isl_engine* e, uint32_t n, const isl_request* in, const uint8_t*
     if (!e || (n && (!in || !priority || !out || !evict)) || (n_victims && !victims)) return ISL_EINVAL;
     if (e->cfg.flags & ISL_FLAG_ALL_NODES) return ISL_EINVAL;      // one pod on every node with capacity: no single GPU to evict on
     for (uint32_t i = 0; i < n; ++i) if (in[i].op == ISL_OP_FREE) return ISL_EINVAL;      // releases are expressed by the victim list
-    const bool gangs = e->cfg.flags & ISL_FLAG_GANG_PREEMPT;
+    const bool gangs = e->gang.preempt;
     std::vector<uint32_t> gang_off;                                 // P1: maximal runs of equal handles
     std::vector<uint8_t> locality;                                  // under ISL_FLAG_GANG_LOCALITY: each gang's byte, 0 without ALLOCs
     if (gangs) {
-        const bool per_gang = e->cfg.flags & ISL_FLAG_GANG_LOCALITY;
-        for (uint32_t i = 0; i < n; ++i) {
-            if (i == 0 || in[i].handle != in[i - 1].handle) {
-                gang_off.push_back(i);
-                if (per_gang) locality.push_back((uint8_t)ISL_GANG_ANY_NODES);
-            }
-        }
+        const bool per_gang = e->gang.locality == kLocPerGang;
+        for (uint32_t i = 0; i < n; ++i)
+            if (i == 0 || in[i].handle != in[i - 1].handle) gang_off.push_back(i);
         gang_off.push_back(n);
+        if (per_gang) locality.assign(gang_off.size() - 1, (uint8_t)ISL_GANG_ANY_NODES);
         for (size_t g = 0; g + 1 < gang_off.size(); ++g) {
-            bool named = false;
+            const uint32_t r0 = gang_off[g], r1 = gang_off[g + 1];
+            // P1: one priority byte per gang, and under ISL_FLAG_GANG_LOCALITY one locality byte, 0, 1 or 3
             uint8_t prio = 0;
-            for (uint32_t r = gang_off[g]; r < gang_off[g + 1]; ++r) {
-                if (in[r].op != ISL_OP_ALLOC) continue;
-                if (named && priority[r] != prio) return ISL_EINVAL;
-                if (per_gang && ((in[r].start != ISL_GANG_ANY_NODES && in[r].start != ISL_GANG_ONE_NODE &&
-                                  in[r].start != ISL_GANG_DISTINCT_NODES) || (named && in[r].start != locality[g]))) return ISL_EINVAL;
-                if (per_gang) locality[g] = in[r].start;
-                prio = priority[r];
-                named = true;
-            }
+            if (alloc_shared(in, r0, r1, [&](uint32_t r) { return priority[r]; }, &prio) < 0) return ISL_EINVAL;
+            if (per_gang && (alloc_shared(in, r0, r1, [&](uint32_t r) { return in[r].start; }, &locality[g]) < 0 ||
+                             (locality[g] != ISL_GANG_ANY_NODES && locality[g] != ISL_GANG_ONE_NODE &&
+                              locality[g] != ISL_GANG_DISTINCT_NODES))) return ISL_EINVAL;
         }
     }
     if (n > e->cfg.max_batch || (uint64_t)n_victims > (uint64_t)ISL_SLOTS * e->cfg.max_gpus) return ISL_ERANGE;
