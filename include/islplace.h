@@ -123,6 +123,7 @@ extern "C" {
 #define ISL_ST_NOOP        5u
 #define ISL_ST_GANG_ABORTED 6u  /* placeable as far as it was tried, but another member of its gang was not: nothing of the gang was committed */
 #define ISL_ST_GANG_TRIMMED 7u  /* not placed: its elastic gang committed its leading members without it (ISL_FLAG_GANG_MIN_MEMBERS, M3) */
+#define ISL_ST_ALT_SKIPPED  8u  /* not tried: an earlier alternative of its pod was placed (ISL_FLAG_FIRST_AVAILABLE, A3) */
 
 typedef struct isl_engine isl_engine;
 
@@ -163,6 +164,8 @@ typedef struct isl_config {
                                          within a maxSkew of byte - 3 (see isl_place_gangs, B1-B8); every other call is unchanged */
 #define ISL_FLAG_GANG_NODE_SCORE_ALL 16384u  /* with ISL_FLAG_GANG_NODE_SCORE: few-node, elastic and balanced gangs are node-scored too
                                                 (see isl_place_gangs, C1-C8); every other call is unchanged */
+#define ISL_FLAG_FIRST_AVAILABLE 32768u  /* a run of ALLOCs with equal `handle` is ONE pod listing alternative profiles in order of
+                                            preference: it gets the first that fits (see isl_place_batch_range, A1-A8) */
 /* Node locality of one gang on an ISL_FLAG_GANG_LOCALITY engine (isl_request.start of its ALLOC members, rules L1-L6) */
 #define ISL_GANG_ANY_NODES      0u  /* rules 2-4: members anywhere, as on an engine without a gang flag */
 #define ISL_GANG_ONE_NODE       1u  /* G2-G3: every member on one node */
@@ -313,6 +316,43 @@ int  isl_place_batch_device(isl_engine* e, uint32_t n, const void* d_in, void* d
  *     not that of the first node of the range;
  *   - an empty range (lo == hi) places nothing: ALLOCs NO_CAPACITY, FREEs FREED and not applied, on every policy. */
 int  isl_place_batch_range(isl_engine* e, uint32_t lo, uint32_t hi, uint32_t n, const isl_request* in, isl_result* out);
+/* Profile alternatives (ISL_FLAG_FIRST_AVAILABLE): a pod that can run on a smaller slice lists the profiles it accepts, most wanted
+ * first, and gets the first one that fits now — what the DRA prioritized list (`firstAvailable` subrequests) asks of an allocator, which
+ * gated MIG pods never reach.  On an engine created with the flag:
+ *   A1. Pods.  A pod is a maximal run of consecutive ISL_OP_ALLOC requests with equal `handle`; its members are its alternatives, in
+ *       order of preference.  Any other request (a FREE, a NOOP, an op treated as NOOP) ends the run; equal handles that are not adjacent
+ *       belong to different pods.  A run never crosses a batch boundary: in isl_place_stream each batch is its own.
+ *   A2. Order.  Batch semantics are unchanged: every FREE is applied first, then the pods go in array order, each seeing every earlier
+ *       commit.
+ *   A3. Choice.  A pod's alternatives are tried in order, each resolved exactly as one ALLOC of isl_place_batch on the same engine (the
+ *       engine's policy over the call's range or partition, node-scoring rules 1-5 under MOST_ / LEAST_ALLOCATED, per-node tables, both
+ *       quirk sets).  The first alternative that places gets its PLACED record; each one before it keeps its usual unplaced record
+ *       (NO_CAPACITY, or BAD_PROFILE for an unknown profile); each ALLOC after it reports ISL_ST_ALT_SKIPPED with the unplaced default
+ *       record isl_place_batch would write for it (gpu ISL_GPU_NONE, start 9, that request's default size, 0 for an unknown profile).
+ *       A pod none of whose alternatives places changes nothing.
+ *   A4. Pods of one.  With no two adjacent ALLOCs sharing a handle, a flagged call equals the same call on the unflagged engine: records,
+ *       occupancy and stats.placed, for every policy, quirk set, table set and partition.
+ *   A5. Consequences.  (a) The chosen alternative is the first one that some GPU of the range admits at that moment: under every policy
+ *       an ALLOC fails only when no GPU admits it.  (b) Keep only each pod's chosen alternative and turn every other alternative into a
+ *       NOOP: the unflagged engine then gives the same PLACED records and the same final occupancy.  (c) stats.placed counts placed pods,
+ *       stats.requests every request; stats.no_capacity counts, as ever, every ALLOC of a known profile that was not placed: each
+ *       alternative that was tried and failed, and each ALT_SKIPPED one.
+ *   A6. Entry points.  isl_place_batch, _range, _device, isl_place_stream, _device (one batch after the other) and isl_what_if follow
+ *       A1-A5.  A flagged engine is request-major for every policy and returns the codes a best-fit engine returns: ISL_EINVAL from
+ *       isl_stream_open, isl_place_batch_partitioned and isl_place_stream_partitioned, ISL_ERANGE for ranges of more than 2^20 GPUs.
+ *       isl_place_gangs (handles stay opaque there), isl_preempt, isl_capacity, isl_free_batch, isl_eval_starts and every other call
+ *       return exactly what they return without the flag.
+ *   A7. isl_create: ISL_EINVAL for the flag with ISL_FLAG_ALL_NODES, ISL_ERANGE for max_gpus > 2^20 (as node scoring).  The flag may
+ *       come with any policy and any gang flag; those only concern isl_place_gangs and isl_preempt.
+ *   A8. Greedy: a pod takes its first alternative that fits now and never looks ahead to later pods.  List the most wanted profile first.
+ * Worked example: H100-80GB rows, first-fit, two one-GPU nodes with occupancy bytes 0x0F and 0x3F, three pods:
+ *     pod                          ISL_QUIRKS_FIXED                                 ISL_QUIRKS_REF_EXACT
+ *     [3g.40gb, 2g.20gb]           (0,4) PLACED, ALT_SKIPPED                        NO_CAPACITY, (0,4) PLACED
+ *     [3g.40gb, 2g.20gb, 1g.10gb]  NO_CAPACITY, NO_CAPACITY, (1,6) PLACED           NO_CAPACITY, NO_CAPACITY, (0,6) PLACED
+ *     [2g.20gb, 1g.10gb]           NO_CAPACITY, NO_CAPACITY                         NO_CAPACITY, (1,6) PLACED
+ *     final bytes                  0xFF 0x7F                                        0x7F 0x7F
+ * ((gpu, start) of each PLACED record.)  Under ISL_QUIRKS_REF_EXACT 3g.40gb never takes start 4 because of the strict start + size < 8
+ * bound (Q1). */
 /* All-or-nothing pod groups (the replicas of a deployment, the workers of a job).  `in` / `out` hold n = gang_off[n_gangs] requests and
  * records (host buffers, as isl_place_batch); gang i is in[gang_off[i] .. gang_off[i + 1]), gang_off[0] == 0, no gang is empty.
  *   1. Every FREE of the call is applied first, wherever it is listed (FREED / BAD_SPAN); a FREE never aborts a gang.  NOOP members

@@ -99,7 +99,8 @@ class InstasliceReconciler:
     def __init__(self, instaslices: list, quirks: int = E.QUIRKS_REF_EXACT, max_batch: int = 65536, engine: E.Engine | None = None,
                  policy: int = E.POLICY_FIRST_FIT, gang_one_node: bool = False, gang_distinct_nodes: bool = False,
                  gang_few_nodes: bool = False, gang_locality: bool = False, gang_min_members: bool = False, gang_preempt: bool = False,
-                 gang_node_score: bool = False, gang_balanced: bool = False, gang_node_score_all: bool = False):
+                 gang_node_score: bool = False, gang_balanced: bool = False, gang_node_score_all: bool = False,
+                 first_available: bool = False):
         """``policy``: the engine policy of the engine this reconciler creates (``engine`` is None), e.g. ``E.POLICY_MOST_ALLOCATED`` to
         pack MIG pods onto the fullest nodes or ``E.POLICY_LEAST_ALLOCATED`` to spread them (include/islplace.h).  ``gang_one_node``:
         that engine is created with ``E.FLAG_GANG_ONE_NODE``, so ``place_pending_gangs`` puts every gang on one node.
@@ -117,7 +118,9 @@ class InstasliceReconciler:
         replicas spread over the nodes within a maxSkew of k (the engine refuses it under node scoring unless ``gang_node_score_all``).
         ``gang_node_score_all``: with ``E.FLAG_GANG_NODE_SCORE_ALL``, which needs ``gang_node_score``, so that the node score also places
         few-node gangs (``gang_few_nodes`` or a ``GANG_FEW_NODES`` locality), elastic gangs (``gang_min_members``) and balanced gangs
-        (``gang_balanced``), all on the one packing or spreading engine."""
+        (``gang_balanced``), all on the one packing or spreading engine.  ``first_available``: with ``E.FLAG_FIRST_AVAILABLE``, so that a
+        pod given to ``place_pending_pods`` may list ``"fallbacks"``, profiles it also accepts, and gets the first of its profiles that
+        fits (include/islplace.h A1-A8)."""
         self.quirks = quirks
         self.policy = policy
         self.gang_one_node = gang_one_node
@@ -129,6 +132,7 @@ class InstasliceReconciler:
         self.gang_node_score = gang_node_score
         self.gang_balanced = gang_balanced
         self.gang_node_score_all = gang_node_score_all
+        self.first_available = first_available
         self.items = instaslices
         self._engine = engine
         self._max_batch = max_batch
@@ -179,7 +183,8 @@ class InstasliceReconciler:
                                           (E.FLAG_GANG_PREEMPT if self.gang_preempt else 0) |
                                           (E.FLAG_GANG_NODE_SCORE if self.gang_node_score else 0) |
                                           (E.FLAG_GANG_BALANCED if self.gang_balanced else 0) |
-                                          (E.FLAG_GANG_NODE_SCORE_ALL if self.gang_node_score_all else 0))
+                                          (E.FLAG_GANG_NODE_SCORE_ALL if self.gang_node_score_all else 0) |
+                                          (E.FLAG_FIRST_AVAILABLE if self.first_available else 0))
         self._engine.load_profile_tables(self.rows)
         self._engine.load_inventory(self.node_off, np.asarray(occ, dtype=np.uint8))
         self._engine.set_node_tables(np.asarray(self.node_table, dtype=np.uint8))
@@ -276,18 +281,45 @@ class InstasliceReconciler:
         realised slices whose allocation is already gone (the only state in which the reference's exact-match veto
         can fire) the pods are resolved one engine call each, so that a vetoed pod leaves no trace before the next
         one is looked at — exactly the reference's sequence.
+
+        On a ``first_available`` reconciler a pod may carry ``"fallbacks": [names...]``, profiles it also accepts, in order of
+        preference after ``"profile"``.  The pod's names become one run of requests with the pod's index as handle, and the pod gets the
+        first of them that fits when its turn comes (include/islplace.h A1-A8).  Its AllocationDetails name the chosen profile: its
+        ``profile``, ``size`` and GI / CI ids come from ``extractGpuProfile`` of that name, so the daemonset creates that slice.  The
+        veto applies to the chosen span as to any other pod's.  A pod with fallbacks on any other reconciler raises ``ValueError``.
         """
         policy = policy or FirstFitPolicy()
+        names = [self._alternatives(p) for p in pods]
         if self._has_orphans:
-            return [self.reconcile_gated_pod(p, p["profile"], policy) for p in pods]
+            return [self._reconcile_alternatives(p, alts, policy) for p, alts in zip(pods, names)]
         out = []
-        results = self._place([p["profile"] for p in pods], 0, len(self.gpu_uuid))
-        for pod, res in zip(pods, results):
-            if res["status"] != E.ST_PLACED:
-                out.append(("none", None))
-            else:
-                out.append(self._commit_or_veto(pod, pod["profile"], policy, res))
+        handles = [i for i, alts in enumerate(names) for _ in alts]
+        results = self._place([n for alts in names for n in alts], 0, len(self.gpu_uuid), handles)
+        k = 0
+        for pod, alts in zip(pods, names):
+            out.append(self._chosen(pod, alts, results[k:k + len(alts)], policy))
+            k += len(alts)
         return out
+
+    def _alternatives(self, pod: dict) -> list:
+        """A pending pod's profile names in order of preference: its profile, then its fallbacks (``first_available`` only)."""
+        fallbacks = list(pod.get("fallbacks") or [])
+        if fallbacks and not self.first_available:
+            raise ValueError("a pod with fallbacks needs a reconciler created with first_available=True")
+        return [pod["profile"], *fallbacks]
+
+    def _chosen(self, pod, alts, res, policy):
+        """The outcome of one pod from the records of its alternatives: the PLACED one, if any, names the profile."""
+        for name, r in zip(alts, res):
+            if r["status"] == E.ST_PLACED:
+                return self._commit_or_veto(pod, name, policy, r)
+        return ("none", None)
+
+    def _reconcile_alternatives(self, pod, alts, policy):
+        """reconcile_gated_pod for a pod's whole run of alternatives: one engine call."""
+        if len(alts) == 1:
+            return self.reconcile_gated_pod(pod, alts[0], policy)
+        return self._chosen(pod, alts, self._place(alts, 0, len(self.gpu_uuid), [0] * len(alts)), policy)
 
     def place_pending_gangs(self, gangs: list, policy=None, locality=None, min_members=None):
         """All-or-nothing pod groups (the replicas of one deployment, the workers of one job): ``gangs`` is a list of non-empty pod
@@ -438,17 +470,17 @@ class InstasliceReconciler:
         return False
 
     # -- internals --------------------------------------------------------------------------------
-    def _requests(self, profile_names):
+    def _requests(self, profile_names, handles=None):
         req = np.zeros(len(profile_names), dtype=E.REQUEST_DTYPE)
-        req["handle"] = np.arange(len(profile_names), dtype=np.uint32)
+        req["handle"] = np.arange(len(profile_names), dtype=np.uint32) if handles is None else np.asarray(handles, dtype=np.uint32)
         req["profile"] = [self.profile_names.get(n, E.PROFILE_UNKNOWN) for n in profile_names]
         req["op"] = E.OP_ALLOC
         return req
 
-    def _place(self, profile_names, lo, hi):
+    def _place(self, profile_names, lo, hi, handles=None):
         # ONE locked call restricts, places and restores (isl_place_batch_range): two reconcile workers cannot interleave and
         # nothing leaks when the call fails
-        return self._engine.place_batch_range(lo, hi, self._requests(profile_names))
+        return self._engine.place_batch_range(lo, hi, self._requests(profile_names, handles))
 
     def _release(self, res):
         spans = np.zeros(1, dtype=E.SPAN_DTYPE)

@@ -2081,12 +2081,30 @@ __global__ void __launch_bounds__(256) k_capacity(const uint8_t* __restrict__ oc
 // classes in reverse order (a PLACED record holds gpu, start and size: `occupancy & ~span` is the byte it came from) and, like every
 // other ALLOC of the gang, reported GANG_ABORTED.  The `dead` profile mask assumes occupancy only grows: it is restored as well, except
 // for a profile that died before any member of its gang was placed (it died in the committed state).
+// kAlt (ISL_FLAG_FIRST_AVAILABLE, DESIGN.md 4.19): the requests come in pods, runs of consecutive ALLOCs with equal handles (A1), whose
+// members are alternatives in order of preference.  Each alternative is resolved as a plain ALLOC until one places; every later one of
+// its pod reports ALT_SKIPPED.  Nothing is undone, so the `dead` mask stays valid.  Pod edges come from the 32 requests of each block.
 // ---------------------------------------------------------------------------------------------
 constexpr uint32_t kBfThreads = 1024;
+
+// kAlt: bit l is set when request l of a block of 32 (lane = request) is an ALLOC that opens a pod: the request before it (`prev`, the
+// previous block's last one, for lane 0) is no ALLOC or carries another handle.  `prev` becomes this block's last request.
+__device__ __forceinline__ uint32_t pod_openings(uint2 mine, uint2& prev, uint32_t lane) {
+    const uint32_t bx = __shfl_up_sync(0xFFFFFFFFu, mine.x, 1), by = __shfl_up_sync(0xFFFFFFFFu, mine.y, 1);
+    const uint32_t px = lane ? bx : prev.x, pop = ((lane ? by : prev.y) >> 8) & 0xFFu;
+    const bool alloc = ((mine.y >> 8) & 0xFFu) == ISL_OP_ALLOC;
+    const uint32_t first = __ballot_sync(0xFFFFFFFFu, alloc && !(pop == ISL_OP_ALLOC && px == mine.x));
+    prev = make_uint2(__shfl_sync(0xFFFFFFFFu, mine.x, 31), __shfl_sync(0xFFFFFFFFu, mine.y, 31));
+    return first;
+}
+
+// kAlt: an alternative after its pod's placed one keeps k_prepare's default record (gpu NONE, start 9, the default size, 0 for an unknown
+// profile) with status ALT_SKIPPED
+__device__ __forceinline__ void skip_alternative(uint2* rec) { rec->y = (rec->y & 0xFFFFu) | ((uint32_t)ISL_ST_ALT_SKIPPED << 16); }
 constexpr uint32_t kBfMaxGpus = 1u << 20;           // class bitmaps: G / 32 words + G / 1024 summary words per (table, occupancy byte) class
 constexpr uint32_t kBfSmemGpus = 4096;              // up to here the class bitmaps live in shared memory (132 KiB)
 
-template <bool kMulti, bool kGang = false>
+template <bool kMulti, bool kGang = false, bool kAlt = false>
 __global__ void __launch_bounds__(kBfThreads, 1) k_bestfit(uint32_t n, const uint2* __restrict__ in, uint2* __restrict__ out, uint8_t* __restrict__ occ,
                                                            uint32_t lo, uint32_t hi, const uint8_t* __restrict__ lut, DevProfiles prof,
                                                            uint32_t* __restrict__ g_bitmaps, Ctrl* ctrl, const uint8_t* __restrict__ score,
@@ -2207,16 +2225,20 @@ __global__ void __launch_bounds__(kBfThreads, 1) k_bestfit(uint32_t n, const uin
             }
         }
     };
+    // kAlt: pod_done = the open pod has placed an alternative; prev = the request before the block
+    bool pod_done = false;
+    uint2 prev = make_uint2(0, (uint32_t)ISL_OP_NOOP << 8);
     uint2 ahead = lane < n ? in[lane] : make_uint2(0, (uint32_t)ISL_OP_NOOP << 8);
     for (uint32_t base = 0; base < n; base += 32) {
         const uint2 mine = ahead;                               // the next block's requests are fetched while this one is resolved
         ahead = base + 32 + lane < n ? in[base + 32 + lane] : make_uint2(0, (uint32_t)ISL_OP_NOOP << 8);
         // only the live ALLOCs of the block are looked at (frees, unknown or dead profiles: defaults were written by k_prepare); in a
-        // gang every ALLOC is looked at, since an unknown or dead profile fails its gang
-        uint32_t live;
+        // gang every ALLOC is looked at, since an unknown or dead profile fails its gang, and in a pod, since it may be skipped
+        uint32_t live, opens = 0;
         {
             const uint32_t wp = mine.y & 0xFFu, wop = (mine.y >> 8) & 0xFFu;
-            live = __ballot_sync(0xFFFFFFFFu, wop == ISL_OP_ALLOC && (kGang || (wp < prof.n && !((dead >> wp) & 1u))));
+            live = __ballot_sync(0xFFFFFFFFu, wop == ISL_OP_ALLOC && (kGang || kAlt || (wp < prof.n && !((dead >> wp) & 1u))));
+            if (kAlt) opens = pod_openings(mine, prev, lane);
         }
         while (live) {
             const uint32_t j = __ffs(live) - 1;
@@ -2229,6 +2251,13 @@ __global__ void __launch_bounds__(kBfThreads, 1) k_bestfit(uint32_t n, const uin
                     continue;
                 }
                 if (p >= prof.n || ((dead >> p) & 1u)) { g_fail = base + j; continue; }
+            } else if (kAlt) {
+                if ((opens >> j) & 1u) pod_done = false;
+                if (pod_done) {                                 // an earlier alternative of the pod placed
+                    if (lane == 0) skip_alternative(out + base + j);
+                    continue;
+                }
+                if (p >= prof.n || ((dead >> p) & 1u)) continue;    // keeps its record; the pod's next alternative is tried
             } else if ((dead >> p) & 1u) continue;              // died inside this block
             uint32_t key = kInf, kc = 0;
 #pragma unroll 8
@@ -2265,6 +2294,7 @@ __global__ void __launch_bounds__(kBfThreads, 1) k_bestfit(uint32_t n, const uin
                 ++placed;
             }
             if (kGang) ++g_placed;
+            if (kAlt) pod_done = true;
             __syncwarp();
             const uint32_t mn = min_after(c0, g);               // g was the class minimum
             if (lane == 0) s_min[cw] = mn;
@@ -2470,6 +2500,8 @@ __global__ void __launch_bounds__(kPreThreads, 1) k_preempt(PreemptArgs a, DevPr
 //            commits it; after a barrier warp q recounts profile q's fits on that node, rewrites its leaf and walks up (32 siblings and
 //            one redux.min per level, stopping where a parent keeps its value); a second barrier ends the request.
 // The trees live in shared memory up to kNfSmemNodes nodes and in global memory (L2) beyond.
+// kAlt (ISL_FLAG_FIRST_AVAILABLE): pods of alternatives as in k_bestfit; every warp walks the same requests and reads the same roots, so
+// the pod state is the same in every warp.
 // ---------------------------------------------------------------------------------------------
 constexpr uint32_t kNfThreads = 32 * ISL_MAX_PROFILES;   // one warp per profile
 constexpr uint32_t kNfSmemNodes = 2048;                  // up to here the trees live in shared memory (16 x 2 176 words = 136 KiB)
@@ -2505,6 +2537,7 @@ __device__ __forceinline__ uint32_t nodefit_leaf(uint32_t fit, uint32_t busy, ui
     return ((100u - score) << 24) | node;
 }
 
+template <bool kAlt = false>
 __global__ void __launch_bounds__(kNfThreads, 1) k_nodefit(NodeFitArgs a, uint32_t n_profiles) {
     extern __shared__ __align__(16) uint32_t s_tree[];
     __shared__ uint8_t s_lut[kMaxTables * ISL_MAX_PROFILES * 256];
@@ -2554,19 +2587,31 @@ __global__ void __launch_bounds__(kNfThreads, 1) k_nodefit(NodeFitArgs a, uint32
     __syncthreads();
     const uint32_t root = a.lvl_off[a.levels - 1];
     uint32_t placed = 0, dead = 0;
+    bool pod_done = false;                                // kAlt: the open pod has placed an alternative
+    uint2 prev = make_uint2(0, (uint32_t)ISL_OP_NOOP << 8);
     uint2 ahead = lane < a.n ? a.in[lane] : make_uint2(0, (uint32_t)ISL_OP_NOOP << 8);
     for (uint32_t base = 0; base < a.n; base += 32) {
         const uint2 mine = ahead;                         // every warp walks the same requests and takes the same branches
         ahead = base + 32 + lane < a.n ? a.in[base + 32 + lane] : make_uint2(0, (uint32_t)ISL_OP_NOOP << 8);
         const uint32_t wp = mine.y & 0xFFu, wop = (mine.y >> 8) & 0xFFu;
-        uint32_t live = __ballot_sync(0xFFFFFFFFu, wop == ISL_OP_ALLOC && wp < n_profiles && !((dead >> wp) & 1u));
+        uint32_t live = __ballot_sync(0xFFFFFFFFu, wop == ISL_OP_ALLOC && (kAlt || (wp < n_profiles && !((dead >> wp) & 1u))));
+        const uint32_t opens = kAlt ? pod_openings(mine, prev, lane) : 0u;
         while (live) {
             const uint32_t j = __ffs(live) - 1;
             live &= live - 1;
             const uint32_t p = __shfl_sync(0xFFFFFFFFu, mine.y, j) & 0xFFu;
+            if (kAlt) {
+                if ((opens >> j) & 1u) pod_done = false;
+                if (pod_done) {                           // an earlier alternative of the pod placed
+                    if (tid == 0) skip_alternative(a.out + base + j);
+                    continue;
+                }
+                if (p >= n_profiles) continue;            // BAD_PROFILE stands; the pod's next alternative is tried
+            }
             if ((dead >> p) & 1u) continue;
             const uint32_t key = tree[(size_t)p * a.T + root];
             if (key == kInf) { dead |= 1u << p; continue; }
+            if (kAlt) pod_done = true;                    // a node admits p: the chain warp places it
             const uint32_t v = key & 0xFFFFFFu;
             if (warp == 0) {                                 // the chain warp: the node's first GPU in range that admits p
                 const uint32_t g0 = max(a.lo, __ldg(a.node_off + a.nlo + v)), g1 = min(a.hi, __ldg(a.node_off + a.nlo + v + 1));

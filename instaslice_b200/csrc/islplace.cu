@@ -266,9 +266,13 @@ namespace {
 
 inline bool bestfit_family(uint32_t policy) { return policy == ISL_POLICY_BEST_FIT || policy == ISL_POLICY_MIN_FRAG; }
 inline bool node_scoring(uint32_t policy) { return policy == ISL_POLICY_MOST_ALLOCATED || policy == ISL_POLICY_LEAST_ALLOCATED; }
-// The policies whose batches one CTA resolves request by request (k_bestfit, k_nodefit): no latency kernels, no segment pipeline, no
-// partitioned calls or open streams, at most kBfMaxGpus GPUs
-inline bool request_major(uint32_t policy) { return bestfit_family(policy) || node_scoring(policy); }
+// The engines whose batches one CTA resolves request by request (k_bestfit, k_nodefit): the best-fit family, node scoring, and every
+// policy under ISL_FLAG_FIRST_AVAILABLE (a pod's fallback sees the occupancy its predecessors left).  No latency kernels, no segment
+// pipeline, no partitioned calls or open streams, at most kBfMaxGpus GPUs
+inline bool request_major(const isl_config& cfg) {
+    return bestfit_family(cfg.policy) || node_scoring(cfg.policy) || (cfg.flags & ISL_FLAG_FIRST_AVAILABLE);
+}
+inline bool first_available(const isl_engine* e) { return e->cfg.flags & ISL_FLAG_FIRST_AVAILABLE; }
 inline bool reversed(const isl_engine* e) { return e->cfg.policy == ISL_POLICY_RIGHT_TO_LEFT; }
 
 // The entry of `table` built with these template arguments, nullptr when none is
@@ -501,8 +505,11 @@ int run_bestfit(isl_engine* e, uint32_t n, const uint2* d_in, uint2* d_out) {
     size_t smem;
     if (int rc = prepare_bestfit(e, n, d_in, d_out, &smem)) return rc;
     if (e->hi == e->lo) { finish_batch(e, n, true); return ISL_OK; }     // empty range: ALLOCs NO_CAPACITY, every FREE outside it
-    if (e->n_tables == 1) k_bestfit<false><<<1, kBfThreads, smem, e->stream>>>(n, d_in, d_out, e->d_occ, e->lo, e->hi, e->d_lut, e->prof, e->d_bf_bitmaps, e->d_ctrl, e->d_score, e->d_gtab, e->d_sizes, 1);
-    else k_bestfit<true><<<1, kBfThreads, 0, e->stream>>>(n, d_in, d_out, e->d_occ, e->lo, e->hi, e->d_lut, e->prof, e->d_bf_bitmaps, e->d_ctrl, e->d_score, e->d_gtab, e->d_sizes, e->n_tables);
+    // ISL_FLAG_FIRST_AVAILABLE: the pods-of-alternatives loop (a zero score table makes it first-fit, prof.flip right-to-left)
+    const bool multi = e->n_tables != 1;
+    auto kernel = first_available(e) ? (multi ? k_bestfit<true, false, true> : k_bestfit<false, false, true>) : (multi ? k_bestfit<true> : k_bestfit<false>);
+    kernel<<<1, kBfThreads, multi ? 0 : smem, e->stream>>>(n, d_in, d_out, e->d_occ, e->lo, e->hi, e->d_lut, e->prof, e->d_bf_bitmaps, e->d_ctrl, e->d_score,
+                                                           e->d_gtab, e->d_sizes, e->n_tables, nullptr, 0);
     if (int rc = check_launch(e, "k_bestfit")) return rc;
     finish_batch(e, n, true);
     return ISL_OK;
@@ -531,7 +538,7 @@ int run_nodefit(isl_engine* e, uint32_t n, const uint2* d_in, uint2* d_out) {
     a.tree = nf.tree; a.fit = nf.fit; a.busy = nf.nodes; a.meta = nf.nodes + a.Nr; a.ctrl = e->d_ctrl;
     a.n = n; a.lo = e->lo; a.hi = e->hi; a.nlo = nlo; a.most = e->cfg.policy == ISL_POLICY_MOST_ALLOCATED;
     memcpy(a.width, nf.width, sizeof a.width);
-    k_nodefit<<<1, kNfThreads, in_smem ? (size_t)e->prof.n * a.T * sizeof(uint32_t) : 0, e->stream>>>(a, e->prof.n);
+    (first_available(e) ? k_nodefit<true> : k_nodefit<false>)<<<1, kNfThreads, in_smem ? (size_t)e->prof.n * a.T * sizeof(uint32_t) : 0, e->stream>>>(a, e->prof.n);
     if (int rc = check_launch(e, "k_nodefit")) return rc;
     finish_batch(e, n, true);
     return ISL_OK;
@@ -888,13 +895,13 @@ int route(isl_engine* e, const Call& c, uint64_t total, uint32_t n_chunks, Route
     const bool ring = c.xepoch != 0;        // partitioned inventory: tokens cross ranks through peer memory, pipeline mandatory
     if (ring && n_chunks > kMaxStreamChunks) return ISL_ERANGE;
     // latency paths: one batch of <= kSmallMax requests in one CTA (k_small); <= kFewMax inline requests on <= kFewGpus GPUs (k_few)
-    if (c.n_batches == 1 && !ring && n <= kSmallMax && !request_major(e->cfg.policy) && !(flags & (ISL_FLAG_NO_SMALL | ISL_FLAG_FORCE_PIPELINE)) &&
+    if (c.n_batches == 1 && !ring && n <= kSmallMax && !request_major(e->cfg) && !(flags & (ISL_FLAG_NO_SMALL | ISL_FLAG_FORCE_PIPELINE)) &&
         range > 0 && range <= (1u << 18)) {
         const bool few = c.src == Src::inline_host && n <= kFewMax && e->hi - (e->lo & ~15u) <= kFewGpus && !getenv("ISL_NO_FEW");
         r->path = few ? Path::few : Path::small;
         return ISL_OK;
     }
-    if (request_major(e->cfg.policy)) { r->path = node_scoring(e->cfg.policy) ? Path::nodefit : Path::bestfit; return ISL_OK; }
+    if (request_major(e->cfg)) { r->path = node_scoring(e->cfg.policy) ? Path::nodefit : Path::bestfit; return ISL_OK; }
     const bool pipeline = ring || (!(flags & ISL_FLAG_NO_PIPELINE) && range > 0 && (n_chunks >= 2 || c.mixed || (flags & ISL_FLAG_FORCE_PIPELINE)));
     if (!pipeline) return ISL_OK;
     // the pipeline keeps one free-mask byte per GPU and batch: very long streams over large inventories go batch by batch
@@ -1238,9 +1245,10 @@ int isl_create(const isl_config* cfg, isl_engine** out) {
     if (cfg->max_gpus == 0 || cfg->max_gpus > ISL_MAX_GPUS || cfg->max_batch == 0) return ISL_EINVAL;
     if (cfg->policy > ISL_POLICY_LEAST_ALLOCATED) return ISL_EINVAL;
     if (node_scoring(cfg->policy) && (cfg->flags & ISL_FLAG_ALL_NODES)) return ISL_EINVAL;     // a pod on every node: no node to choose
+    if ((cfg->flags & ISL_FLAG_FIRST_AVAILABLE) && (cfg->flags & ISL_FLAG_ALL_NODES)) return ISL_EINVAL;     // A7: one pod, every node
     GangMode gang;
     if (int rc = gang_mode(cfg, &gang)) return rc;
-    if (request_major(cfg->policy) && cfg->max_gpus > kBfMaxGpus) return ISL_ERANGE;
+    if (request_major(*cfg) && cfg->max_gpus > kBfMaxGpus) return ISL_ERANGE;
     if (cfg->quirks & ~ISL_QUIRKS_REF_EXACT) return ISL_EINVAL;
     isl_engine* e = new (std::nothrow) isl_engine;
     if (!e) return ISL_ENOMEM;
@@ -1269,7 +1277,8 @@ int isl_create(const isl_config* cfg, isl_engine** out) {
         cudaFuncAttributes fa;
         const void* kernels[] = {(const void*)k_prepare, (const void*)k_partition, (const void*)k_set_flag, (const void*)k_few, (const void*)k_build_lut, (const void*)k_eval_starts,
                                  (const void*)k_free_spans, (const void*)k_capacity, (const void*)k_sweep_count, (const void*)k_sweep_scatter, (const void*)k_commit, (const void*)k_bestfit<false>, (const void*)k_bestfit<true>,
-                                 (const void*)k_bestfit<false, true>, (const void*)k_bestfit<true, true>, (const void*)k_victim_map, (const void*)k_preempt, (const void*)k_nodefit,
+                                 (const void*)k_bestfit<false, true>, (const void*)k_bestfit<true, true>, (const void*)k_victim_map, (const void*)k_preempt, (const void*)k_nodefit<false>,
+                                 (const void*)k_bestfit<false, false, true>, (const void*)k_bestfit<true, false, true>, (const void*)k_nodefit<true>,
                                  (const void*)k_chain<1>, (const void*)k_chain<2>, (const void*)k_chain<4>, (const void*)k_small<1>, (const void*)k_small<2>, (const void*)k_small<4>};
         const void* pipes[] = {(const void*)k_pipeline<1, false, false>, (const void*)k_pipeline<1, true, false>, (const void*)k_pipeline<2, false, false>, (const void*)k_pipeline<2, true, false>,
                                (const void*)k_pipeline<4, false, false>, (const void*)k_pipeline<4, true, false>,
@@ -1281,11 +1290,11 @@ int isl_create(const isl_config* cfg, isl_engine** out) {
         // skip devices 8.. and race between threads)
         const void* chains[] = {(const void*)k_chain<1>, (const void*)k_chain<2>, (const void*)k_chain<4>};
         for (const void* k : chains) ISL_TRY(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(kQCap * sizeof(uint16_t))));
-        for (const void* k : {(const void*)k_bestfit<false>, (const void*)k_bestfit<false, true>})
+        for (const void* k : {(const void*)k_bestfit<false>, (const void*)k_bestfit<false, true>, (const void*)k_bestfit<false, false, true>})
             ISL_TRY(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(256 * (kBfSmemGpus / 32 + kBfSmemGpus / 1024) * sizeof(uint32_t))));
         for (const void* k : pipes) ISL_TRY(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kPipeSmem));
-        ISL_TRY(cudaFuncSetAttribute((const void*)k_nodefit, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                     (int)(ISL_MAX_PROFILES * (kNfSmemNodes + 64 + 32 + 32) * sizeof(uint32_t))));
+        for (const void* k : {(const void*)k_nodefit<false>, (const void*)k_nodefit<true>})
+            ISL_TRY(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(ISL_MAX_PROFILES * (kNfSmemNodes + 64 + 32 + 32) * sizeof(uint32_t))));
         int optin = 0;          // k_preempt's share of the partition: up to what the device lets one CTA have
         ISL_TRY(cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev));
         ISL_TRY(cudaFuncGetAttributes(&fa, k_preempt));
@@ -1871,7 +1880,7 @@ int isl_place_stream_partitioned(isl_engine* e, uint32_t n_batches, const uint32
     Entry guard(e, Needs::ready, total);
     if (guard.rc) return guard.rc;
     if (total == 0) return ISL_OK;
-    if (request_major(e->cfg.policy) || reversed(e)) return ISL_EINVAL;         // request-major / right-to-left policies do not partition
+    if (request_major(e->cfg) || reversed(e)) return ISL_EINVAL;         // request-major / right-to-left policies do not partition
     return run_stream(e, Call{n_batches, sizes, Src::device, d_in, d_out, stream_id});
 }
 
@@ -1887,7 +1896,7 @@ int isl_place_batch_partitioned(isl_engine* e, uint32_t n, const void* d_in, voi
     Entry guard(e, Needs::ready, n);
     if (guard.rc) return guard.rc;
     if (n == 0) return ISL_OK;
-    if (request_major(e->cfg.policy) || reversed(e)) return ISL_EINVAL;         // request-major / right-to-left policies do not partition
+    if (request_major(e->cfg) || reversed(e)) return ISL_EINVAL;         // request-major / right-to-left policies do not partition
     return run_chunks(e, n, static_cast<const uint2*>(d_in), static_cast<uint2*>(d_out), static_cast<const uint32_t*>(d_heads_in),
                       static_cast<uint32_t*>(d_heads_out));
 }
@@ -2087,7 +2096,7 @@ int isl_stream_open(isl_engine* e, uint32_t max_batches) {
     if (!e || max_batches == 0 || max_batches > kMaxStreamChunks) return ISL_EINVAL;
     Entry guard(e, Needs::ready);
     if (guard.rc) return guard.rc;
-    if (request_major(e->cfg.policy)) return ISL_EINVAL;
+    if (request_major(e->cfg)) return ISL_EINVAL;
     // a tool that serialises kernels would starve a resident kernel that waits for kernels launched after it: refuse instead of hanging
     // until the device-side trap (callers fall back to isl_place_batch per batch)
     if (getenv("ISL_NO_FEED") || kernels_serialised()) {

@@ -30,6 +30,7 @@ QUIRKS_REF_EXACT, QUIRKS_FIXED = 3, 0
 OP_ALLOC, OP_FREE, OP_NOOP = 0, 1, 2
 ST_PLACED, ST_NO_CAPACITY, ST_BAD_PROFILE, ST_FREED, ST_BAD_SPAN, ST_NOOP, ST_GANG_ABORTED = 0, 1, 2, 3, 4, 5, 6
 ST_GANG_TRIMMED = 7     # not placed: its elastic gang committed its leading members without it (include/islplace.h M3)
+ST_ALT_SKIPPED = 8      # not tried: an earlier alternative of its pod was placed (FLAG_FIRST_AVAILABLE, include/islplace.h A3)
 FLAG_TIMING, FLAG_NO_PIPELINE, FLAG_FORCE_PIPELINE, FLAG_TRACE, FLAG_NO_SMALL, FLAG_ALL_NODES = 1, 2, 4, 8, 16, 32
 FLAG_GANG_ONE_NODE = 64     # isl_place_gangs puts every member of a gang on one node (include/islplace.h)
 FLAG_GANG_DISTINCT_NODES = 128  # isl_place_gangs puts every member of a gang on a different node (include/islplace.h)
@@ -40,6 +41,7 @@ FLAG_GANG_PREEMPT = 2048  # isl_preempt picks the victims a whole gang (a run of
 FLAG_GANG_NODE_SCORE = 4096  # on a node-scoring engine isl_place_gangs places gangs by MostAllocated / LeastAllocated (N1-N8)
 FLAG_GANG_BALANCED = 8192  # with FLAG_GANG_LOCALITY: a locality of gang_balanced_nodes(k) spreads a gang over the nodes within maxSkew k
 FLAG_GANG_NODE_SCORE_ALL = 16384  # with FLAG_GANG_NODE_SCORE: few-node, elastic and balanced gangs are node-scored too (C1-C8)
+FLAG_FIRST_AVAILABLE = 32768  # a run of ALLOCs with equal handle is one pod listing alternative profiles; it gets the first that fits (A1-A8)
 GANG_ANY_NODES, GANG_ONE_NODE, GANG_FEW_NODES, GANG_DISTINCT_NODES = 0, 1, 2, 3     # node locality of one gang (include/islplace.h L1)
 SPEC_AUTO, SPEC_OFF, SPEC_ON = 0, 1, 2
 
@@ -314,7 +316,10 @@ class Engine:
 
     # -- hot path
     def place_batch(self, requests: np.ndarray, out: np.ndarray | None = None) -> np.ndarray:
-        """Host buffers in, host buffers out (the call the Go shim makes)."""
+        """Host buffers in, host buffers out (the call the Go shim makes).  On an engine created with ``FLAG_FIRST_AVAILABLE`` a run of
+        consecutive ALLOCs with equal ``handle`` is one pod whose profiles are alternatives in order of preference: the first that fits
+        is PLACED, the ones before it keep their unplaced records and the ones after it report ``ST_ALT_SKIPPED`` (include/islplace.h
+        A1-A8)."""
         requests = np.ascontiguousarray(requests, dtype=REQUEST_DTYPE)
         if out is None:
             out = np.empty(len(requests), dtype=RESULT_DTYPE)

@@ -27,6 +27,7 @@ InstasliceReconciler::InstasliceReconciler(uint32_t quirks, uint32_t max_gpus, u
     cfg.abi_version = ISL_ABI_VERSION; cfg.policy = policy; cfg.quirks = quirks; cfg.device = -1;
     cfg.max_gpus = max_gpus; cfg.max_batch = max_batch; cfg.flags = flags;
     check(isl_create(&cfg, &h_), nullptr, "isl_create");
+    flags_ = flags;
 }
 InstasliceReconciler::~InstasliceReconciler() { if (h_) isl_destroy(h_); }
 
@@ -152,17 +153,18 @@ uint32_t InstasliceReconciler::getStartIndexFromPreparedState(const Instaslice& 
     return start;
 }
 
-std::vector<isl_request> InstasliceReconciler::requests(const std::vector<std::string>& names) const {
+std::vector<isl_request> InstasliceReconciler::requests(const std::vector<std::string>& names, const std::vector<uint32_t>& handles) const {
     std::vector<isl_request> req(names.size());
     for (size_t i = 0; i < names.size(); ++i) {
         auto it = profiles_.find(names[i]);
-        req[i] = isl_request{(uint32_t)i, it == profiles_.end() ? (uint8_t)ISL_PROFILE_UNKNOWN : it->second, (uint8_t)ISL_OP_ALLOC, 0, 0};
+        req[i] = isl_request{handles.empty() ? (uint32_t)i : handles[i], it == profiles_.end() ? (uint8_t)ISL_PROFILE_UNKNOWN : it->second,
+                             (uint8_t)ISL_OP_ALLOC, 0, 0};
     }
     return req;
 }
 
-std::vector<isl_result> InstasliceReconciler::place(const std::vector<std::string>& names, uint32_t lo, uint32_t hi) {
-    std::vector<isl_request> req = requests(names);
+std::vector<isl_result> InstasliceReconciler::place(const std::vector<std::string>& names, uint32_t lo, uint32_t hi, const std::vector<uint32_t>& handles) {
+    std::vector<isl_request> req = requests(names, handles);
     std::vector<isl_result> res(names.size());
     // restriction, placement and restore under ONE engine lock: nothing leaks when the call throws, two callers cannot interleave
     check(isl_place_batch_range(h_, lo, hi, (uint32_t)req.size(), req.data(), res.data()), h_, "isl_place_batch_range");
@@ -396,15 +398,28 @@ std::vector<GangPreemptOutcome> InstasliceReconciler::PreemptPendingGangs(const 
 std::vector<Outcome> InstasliceReconciler::PlacePending(InstasliceList& list, AllocationPolicy& policy, const std::vector<PendingPod>& pods) {
     std::vector<Outcome> out(pods.size());
     if (pods.empty()) return out;
+    for (const PendingPod& p : pods)
+        if (!p.Fallbacks.empty() && !(flags_ & ISL_FLAG_FIRST_AVAILABLE))
+            throw std::invalid_argument("a pod with Fallbacks needs a reconciler created with ISL_FLAG_FIRST_AVAILABLE");
     if (orphans_ && pods.size() > 1) {          // the veto must see one pod at a time, exactly like the reference
         for (size_t i = 0; i < pods.size(); ++i) out[i] = PlacePending(list, policy, {pods[i]})[0];
         return out;
     }
+    // each pod's profile, then its fallbacks: one run of requests with the pod's index as handle
     std::vector<std::string> names;
-    for (const PendingPod& p : pods) names.push_back(p.ProfileName);
-    const std::vector<isl_result> res = place(names, 0, (uint32_t)gpuUUID_.size());
-    for (size_t i = 0; i < pods.size(); ++i)
-        if (res[i].status == ISL_ST_PLACED) out[i] = commitOrVeto(list, policy, pods[i], res[i]);
+    std::vector<uint32_t> handles;
+    for (size_t i = 0; i < pods.size(); ++i) {
+        names.push_back(pods[i].ProfileName);
+        names.insert(names.end(), pods[i].Fallbacks.begin(), pods[i].Fallbacks.end());
+        handles.resize(names.size(), (uint32_t)i);
+    }
+    const std::vector<isl_result> res = place(names, 0, (uint32_t)gpuUUID_.size(), handles);
+    for (size_t i = 0, k = 0; i < pods.size(); k += 1 + pods[i++].Fallbacks.size())
+        for (size_t a = 0; a <= pods[i].Fallbacks.size(); ++a)
+            if (res[k + a].status == ISL_ST_PLACED) {        // the pod's allocation names the chosen profile
+                out[i] = commitOrVeto(list, policy, PendingPod{pods[i].pod, names[k + a]}, res[k + a]);
+                break;
+            }
     return out;
 }
 

@@ -69,7 +69,9 @@ struct LeftToRightPolicy : AllocationPolicy {    // :456-461, a stub in the refe
 struct RightToLeftPolicy : LeftToRightPolicy {}; // :464-469
 
 enum class Verdict { Placed, None, Veto };       // allocation written / "failed to find allocatable gpu" everywhere / :198-203 requeue
-struct PendingPod { Pod pod; std::string ProfileName; };
+// Fallbacks: on a reconciler created with ISL_FLAG_FIRST_AVAILABLE, profiles the pod also accepts, in order of preference after
+// ProfileName (include/islplace.h A1-A8)
+struct PendingPod { Pod pod; std::string ProfileName; std::vector<std::string> Fallbacks{}; };
 struct Outcome { Verdict verdict = Verdict::None; AllocationDetails alloc; };
 // Priority preemption (extension: isl_preempt): a pending pod with the int32 value of its PriorityClass; the answer for it.
 struct PreemptPod { Pod pod; std::string ProfileName; int32_t Priority = 0; };
@@ -101,7 +103,8 @@ public:
     // the four) so that PlaceGangs takes a minimum per gang; with a node-scoring policy, ISL_FLAG_GANG_NODE_SCORE (alone or with the
     // one-node, distinct-node or locality flag) so that PlaceGangs places gangs by the node score; with ISL_FLAG_GANG_LOCALITY,
     // ISL_FLAG_GANG_BALANCED so that a locality of ISL_GANG_BALANCED_NODES(maxSkew) spreads a gang over the nodes; with
-    // ISL_FLAG_GANG_NODE_SCORE, ISL_FLAG_GANG_NODE_SCORE_ALL so that few-node, elastic and balanced gangs are node-scored as well
+    // ISL_FLAG_GANG_NODE_SCORE, ISL_FLAG_GANG_NODE_SCORE_ALL so that few-node, elastic and balanced gangs are node-scored as well;
+    // ISL_FLAG_FIRST_AVAILABLE so that PlacePending honours each pod's Fallbacks
     explicit InstasliceReconciler(uint32_t quirks = ISL_QUIRKS_REF_EXACT, uint32_t max_gpus = 1u << 16, uint32_t max_batch = 1u << 16,
                                   uint32_t policy = ISL_POLICY_FIRST_FIT, uint32_t flags = 0);
     ~InstasliceReconciler();
@@ -121,7 +124,10 @@ public:
     // does not record the allocation (the tentative engine commit is released again).
     bool findDeviceForASlice(const InstasliceList& list, size_t node, const std::string& profileName, AllocationPolicy& policy, const Pod& pod,
                              AllocationDetails* out, std::string* err);
-    // Reconcile's node loop for many gated pods in order, ONE engine call; allocations are written into `list`.
+    // Reconcile's node loop for many gated pods in order, ONE engine call; allocations are written into `list`.  On a reconciler created
+    // with ISL_FLAG_FIRST_AVAILABLE a pod's ProfileName and Fallbacks are one run of requests (handle = the pod's index) and the pod gets
+    // the first of them that fits; its AllocationDetails name that profile (Profile, Size and the GI / CI ids of extractGpuProfile).
+    // A pod with Fallbacks on any other reconciler throws std::invalid_argument.
     std::vector<Outcome> PlacePending(InstasliceList& list, AllocationPolicy& policy, const std::vector<PendingPod>& pods);
     // All-or-nothing pod groups in order, ONE engine call (isl_place_gangs): a gang is Placed only when every pod of it got a slice, and
     // only then are its allocations written into `list`.  None: a pod found no GPU, nothing of the gang was committed.  Veto: the
@@ -164,10 +170,12 @@ private:
     std::map<std::string, uint8_t> profiles_;
     std::map<std::string, uint32_t> gpuIndex_;
     bool orphans_ = false;
+    uint32_t flags_ = 0;
     void preemptVictims(const InstasliceList& list, const std::vector<int32_t>& own, const std::map<std::string, int32_t>& podPriority,
                         std::map<int32_t, uint8_t>& rank, std::vector<isl_victim>& victims, std::vector<std::string>& uids) const;
-    std::vector<isl_request> requests(const std::vector<std::string>& names) const;
-    std::vector<isl_result> place(const std::vector<std::string>& names, uint32_t lo, uint32_t hi);
+    // handles: one per name (empty: each request's index)
+    std::vector<isl_request> requests(const std::vector<std::string>& names, const std::vector<uint32_t>& handles = {}) const;
+    std::vector<isl_result> place(const std::vector<std::string>& names, uint32_t lo, uint32_t hi, const std::vector<uint32_t>& handles = {});
     void releaseSpan(const isl_result& r);
     AllocationDetails pack(const InstasliceList& list, AllocationPolicy& policy, const PendingPod& p, const isl_result& r);
     bool vetoed(const InstasliceList& list, const isl_result& r, const AllocationDetails& a) const;

@@ -36,6 +36,7 @@ type PlacementEngine struct {
 	orphans  bool              // a realised slice outlived its allocation: the :198-203 veto can fire
 	nodeOff  []C.uint32_t      // node index -> first canonical GPU index
 	nodeMig  [][]inferencev1alpha1.Mig // the Migplacement each node had at the last Sync (UpdateNode compares)
+	flags    uint32            // isl_config.flags the engine was created with
 }
 
 // hasOrphans: a Prepared entry that names a pod whose Allocations entry is gone — the only state in which the exact-match
@@ -90,10 +91,16 @@ const (
 	// With FlagGangNodeScore: few-node gangs (FlagGangFewNodes or GangFewNodes), elastic gangs (FlagGangMinMembers) and balanced
 	// gangs (FlagGangBalanced) are placed by the node score too, so a packing or spreading cluster needs no second engine for them.
 	FlagGangNodeScoreAll = uint32(C.ISL_FLAG_GANG_NODE_SCORE_ALL)
+	// PlacePending honours each pod's Fallbacks: a pod gets the first of its profiles that fits when its turn comes (the DRA
+	// prioritized list, firstAvailable).  With any policy and any gang flag; not with ISL_FLAG_ALL_NODES.
+	FlagFirstAvailable = uint32(C.ISL_FLAG_FIRST_AVAILABLE)
 )
 
 // StGangTrimmed is the record status of a pod its elastic gang was placed without (isl_result.status, FlagGangMinMembers).
 const StGangTrimmed = uint16(C.ISL_ST_GANG_TRIMMED)
+
+// StAltSkipped is the record status of a pod's alternative that was not tried because an earlier one was placed (FlagFirstAvailable).
+const StAltSkipped = uint16(C.ISL_ST_ALT_SKIPPED)
 
 // Node locality of one gang for PlaceGangsWithLocality (an engine created with FlagGangLocality).
 const (
@@ -133,7 +140,7 @@ func NewPlacementEngineWithFlags(maxGPUs, maxBatch, policy, flags uint32) (*Plac
 	if rc := C.isl_create(&cfg, &h); rc != C.ISL_OK {
 		return nil, fmt.Errorf("isl_create: %s", C.GoString(C.isl_strerror(rc)))
 	}
-	return &PlacementEngine{h: h}, nil
+	return &PlacementEngine{h: h, flags: flags}, nil
 }
 
 func (e *PlacementEngine) Close() { C.isl_destroy(e.h) }
@@ -294,6 +301,19 @@ func (e *PlacementEngine) UpdateNode(list *inferencev1alpha1.InstasliceList, n i
 type PendingPod struct {
 	Pod         *v1.Pod
 	ProfileName string // r.extractProfileName(limits), :154
+	// Profiles the pod also accepts, in order of preference after ProfileName.  Only PlacePending on an engine created with
+	// FlagFirstAvailable honours them; every other call returns an error for a pod that has them.
+	Fallbacks []string
+}
+
+// fallbacksRefused is the error of a call that does not take Fallbacks for pods that carry them (nil when none does).
+func fallbacksRefused(what string, pods []PendingPod) error {
+	for _, p := range pods {
+		if len(p.Fallbacks) > 0 {
+			return fmt.Errorf("%s: pod %s has fallbacks, which only PlacePending on a FlagFirstAvailable engine takes", what, p.Pod.Name)
+		}
+	}
+	return nil
 }
 
 const errNoGpu = "failed to find allocatable gpu" // :261
@@ -366,12 +386,22 @@ func (e *PlacementEngine) fillRequests(req []C.isl_request, pods []PendingPod, b
 
 // PlacePending resolves the pods in order with ONE engine call and packs the answers with the unchanged policy
 // hook.  result[i] == nil means "failed to find allocatable gpu" on every node (:261, :229-232: requeue) or a veto.
+// On an engine created with FlagFirstAvailable a pod's ProfileName and Fallbacks are one run of requests whose handle is the pod's
+// index: the pod gets the first of them that fits, and its AllocationDetails name that profile (Profile, Size and the GI / CI ids
+// of extractGpuProfile), so the daemonset creates that slice.  The veto applies to the chosen span.
 func (r *InstasliceReconciler) PlacePending(e *PlacementEngine, list *inferencev1alpha1.InstasliceList, policy AllocationPolicy,
 	pods []PendingPod) ([]*inferencev1alpha1.AllocationDetails, error) {
 	n := len(pods)
 	out := make([]*inferencev1alpha1.AllocationDetails, n)
 	if n == 0 {
 		return out, nil
+	}
+	alts := 0 // fallbacks over all pods
+	for _, p := range pods {
+		alts += len(p.Fallbacks)
+	}
+	if alts > 0 && e.flags&FlagFirstAvailable == 0 {
+		return nil, fallbacksRefused("PlacePending without FlagFirstAvailable", pods)
 	}
 	if e.orphans && n > 1 { // the exact-match veto (:198-203) must see one pod at a time
 		for i := range pods {
@@ -384,7 +414,8 @@ func (r *InstasliceReconciler) PlacePending(e *PlacementEngine, list *inferencev
 		return out, nil
 	}
 	// C-allocated request/result arrays: no Go pointer is retained by the engine after the call returns
-	reqP, resP := C.malloc(C.size_t(n)*C.sizeof_isl_request), C.malloc(C.size_t(n)*C.sizeof_isl_result)
+	m := n + alts
+	reqP, resP := C.malloc(C.size_t(m)*C.sizeof_isl_request), C.malloc(C.size_t(m)*C.sizeof_isl_result)
 	if reqP == nil || resP == nil {
 		C.free(reqP)
 		C.free(resP)
@@ -392,21 +423,41 @@ func (r *InstasliceReconciler) PlacePending(e *PlacementEngine, list *inferencev
 	}
 	defer C.free(reqP)
 	defer C.free(resP)
-	req := (*[1 << 28]C.isl_request)(reqP)[:n:n]
-	res := (*[1 << 28]C.isl_result)(resP)[:n:n]
-	e.fillRequests(req, pods, 0)
-	if rc := C.isl_place_batch(e.h, C.uint32_t(n), &req[0], &res[0]); rc != C.ISL_OK {
+	req := (*[1 << 28]C.isl_request)(reqP)[:m:m]
+	res := (*[1 << 28]C.isl_result)(resP)[:m:m]
+	if alts == 0 {
+		e.fillRequests(req, pods, 0)
+	} else {
+		k := 0
+		for i, p := range pods { // the pod's names, one run with the pod's index as handle
+			for _, name := range append([]string{p.ProfileName}, p.Fallbacks...) {
+				row, ok := e.profiles[name]
+				if !ok {
+					row = C.ISL_PROFILE_UNKNOWN
+				}
+				req[k] = C.isl_request{handle: C.uint32_t(i), profile: C.uint8_t(row), op: C.ISL_OP_ALLOC}
+				k++
+			}
+		}
+	}
+	if rc := C.isl_place_batch(e.h, C.uint32_t(m), &req[0], &res[0]); rc != C.ISL_OK {
 		return nil, fmt.Errorf("isl_place_batch: %s (%s)", C.GoString(C.isl_strerror(rc)), C.GoString(C.isl_last_cuda_error(e.h)))
 	}
+	k := 0
 	for i, p := range pods {
-		if res[i].status != C.ISL_ST_PLACED {
-			continue
+		names := append([]string{p.ProfileName}, p.Fallbacks...)
+		for a, name := range names {
+			if res[k+a].status != C.ISL_ST_PLACED {
+				continue
+			}
+			alloc, err := r.commitOrVeto(e, list, policy, PendingPod{Pod: p.Pod, ProfileName: name}, res[k+a])
+			if err != nil {
+				return nil, err
+			}
+			out[i] = alloc
+			break
 		}
-		a, err := r.commitOrVeto(e, list, policy, p, res[i])
-		if err != nil {
-			return nil, err
-		}
-		out[i] = a
+		k += len(names)
 	}
 	return out, nil
 }
@@ -446,6 +497,9 @@ func (r *InstasliceReconciler) PlaceGangsElastic(e *PlacementEngine, list *infer
 	}
 	n := 0
 	for _, g := range gangs {
+		if err := fallbacksRefused("PlaceGangs", g); err != nil {
+			return nil, err
+		}
 		if len(g) == 0 {
 			return nil, fmt.Errorf("empty gang")
 		}
@@ -569,6 +623,9 @@ func (r *InstasliceReconciler) PlaceBacklog(e *PlacementEngine, list *inferencev
 	total := 0
 	sizes := make([]C.uint32_t, len(batches))
 	for b, pods := range batches {
+		if err := fallbacksRefused("PlaceBacklog", pods); err != nil {
+			return nil, err
+		}
 		sizes[b] = C.uint32_t(len(pods))
 		total += len(pods)
 	}
@@ -642,6 +699,9 @@ func (e *PlacementEngine) OpenBacklogStream(maxBatches int, inFlight int) (*Back
 
 // Submit enqueues one batch and returns its ticket at once.
 func (s *BacklogStream) Submit(pods []PendingPod) (int, error) {
+	if err := fallbacksRefused("BacklogStream", pods); err != nil {
+		return -1, err
+	}
 	req, res, pinned, free, err := hostArrays(len(pods))
 	if err != nil {
 		return -1, err
@@ -796,6 +856,9 @@ func (r *InstasliceReconciler) PreemptPendingGangs(e *PlacementEngine, list *inf
 // preempt is PreemptPending with, for gangs, a gang index per pod written into the request's handle and a locality byte into its start.
 func (r *InstasliceReconciler) preempt(e *PlacementEngine, list *inferencev1alpha1.InstasliceList, pods []PendingPod, priority []int32,
 	podPriority map[string]int32, gangOf []uint32, locality []uint8) ([]PreemptTarget, error) {
+	if err := fallbacksRefused("PreemptPending", pods); err != nil {
+		return nil, err
+	}
 	out := make([]PreemptTarget, len(pods))
 	if len(pods) == 0 {
 		return out, nil
