@@ -41,6 +41,7 @@ struct Cluster {
     std::vector<uint32_t> node_of;  // node of every GPU
     std::vector<uint32_t> width;    // per table: the largest start + size over its rows
     std::vector<std::vector<uint32_t>> cand;    // per table: every (profile, start) mask the search can return
+    mutable std::vector<int32_t> memo;          // [table][profile][byte]: score << 8 | mask, -1 until first asked; empty: no memo
 
     const isl_profile& row(uint32_t g, uint32_t p) const { return rows[(size_t)node_table[node_of[g]] * n_profiles + p]; }
 
@@ -52,6 +53,16 @@ struct Cluster {
         uint32_t v = 0;
         for (uint32_t m : cand[node_table[node_of[g]]]) v += ((o & m) == 0) && (((o | mine) & m) != 0);
         return v;
+    }
+
+    // the best-fit family's (score, first legal mask) of profile p on GPU g as score << 8 | mask (mask 0: no legal start); with the memo
+    // on, each (table, profile, byte) is walked once, the first time a GPU asks for it
+    uint32_t scored(uint32_t g, uint32_t p) const {
+        int32_t* v = memo.empty() ? nullptr : &memo[((size_t)node_table[node_of[g]] * n_profiles + p) * 256 + occ[g]];
+        if (v && *v >= 0) return (uint32_t)*v;
+        const uint32_t m = first_mask(row(g, p), occ[g], quirks), r = m ? score(g, m) << 8 | m : 0u;
+        if (v) *v = (int32_t)r;
+        return r;
     }
 
     // one ALLOC of profile p as isl_place_batch resolves it: the GPU and the mask, or false
@@ -67,9 +78,9 @@ struct Cluster {
             bool found = false;
             uint32_t best = 0;
             for (uint32_t g = lo; g < hi; ++g) {
-                const uint32_t m = first_mask(row(g, p), occ[g], quirks);
+                const uint32_t sm = scored(g, p), m = sm & 0xFFu;
                 if (!m) continue;
-                const uint32_t s = score(g, m);
+                const uint32_t s = sm >> 8;
                 if (!found || s < best) { found = true; best = s; *gpu = g; *mask = m; }
             }
             return found;
@@ -105,16 +116,18 @@ extern "C" {
 
 // rows[t * n_profiles + p]; node_off: n_nodes + 1 offsets; node_table: the table of every node; default_size[p]: the size an unplaced
 // ALLOC reports; occ: G bytes, canonical order, updated in place; [lo, hi): the canonical range.  flagged: the rules of an
-// ISL_FLAG_FIRST_AVAILABLE engine (A1-A5), else those of isl_place_batch.  out: n records; returns the number of PLACED records.
+// ISL_FLAG_FIRST_AVAILABLE engine (A1-A5), else those of isl_place_batch.  memo: remember the best-fit family's score of every (table,
+// profile, byte).  out: n records; returns the number of PLACED records.
 uint32_t fa_place(uint32_t n_nodes, const uint32_t* node_off, uint32_t n_tables, uint32_t n_profiles, const isl_profile* rows,
                   const uint8_t* node_table, const uint8_t* default_size, uint8_t* occ, uint32_t lo, uint32_t hi, uint32_t quirks,
-                  uint32_t policy, uint32_t flagged, uint32_t n, const isl_request* in, isl_result* out) {
+                  uint32_t policy, uint32_t flagged, uint32_t n, const isl_request* in, isl_result* out, uint32_t memo) {
     Cluster c{node_off[n_nodes], n_nodes, n_profiles, quirks, policy, lo, hi, node_off, rows, node_table, occ, {}, {}, {}};
     c.node_of.resize(c.G);
     for (uint32_t v = 0; v < n_nodes; ++v)
         for (uint32_t g = node_off[v]; g < node_off[v + 1]; ++g) c.node_of[g] = v;
     c.width.assign(n_tables, 0);
     c.cand.assign(n_tables, {});
+    if (memo) c.memo.assign((size_t)n_tables * n_profiles * 256, -1);
     for (uint32_t t = 0; t < n_tables; ++t)
         for (uint32_t p = 0; p < n_profiles; ++p) {
             const isl_profile& r = rows[(size_t)t * n_profiles + p];

@@ -33,7 +33,7 @@ def lib():
         L = C.CDLL(so)
         p, u = C.c_void_p, C.c_uint32
         L.fa_place.restype = u
-        L.fa_place.argtypes = [u, p, u, u, p, p, p, p, u, u, u, u, u, u, p, p]
+        L.fa_place.argtypes = [u, p, u, u, p, p, p, p, u, u, u, u, u, u, p, p, u]
         _lib = L
     return _lib
 
@@ -43,9 +43,11 @@ def _ptr(a):
 
 
 def place(node_off, rows, occ, requests, policy=E.POLICY_FIRST_FIT, quirks=E.QUIRKS_REF_EXACT, node_table=None, lo=0, hi=None,
-          flagged=True):
+          flagged=True, memo=False):
     """One batch (isl_place_batch on the partition [lo, hi), or isl_place_batch_range(lo, hi)).  ``rows``: [n_profiles] or
-    [n_tables][n_profiles] with ``node_table`` [n_nodes]; ``flagged``: an ISL_FLAG_FIRST_AVAILABLE engine, else an unflagged one."""
+    [n_tables][n_profiles] with ``node_table`` [n_nodes]; ``flagged``: an ISL_FLAG_FIRST_AVAILABLE engine, else an unflagged one.
+    ``memo``: the best-fit family's score of every (table, profile, byte) is walked once and remembered, which 2^20-GPU
+    ISL_POLICY_MIN_FRAG calls need; off, every GPU is walked for every ALLOC (the one-core baseline of tools/first_available_time.py)."""
     node_off = np.ascontiguousarray(node_off, dtype=np.uint32)
     rows2 = np.ascontiguousarray(np.asarray(rows, dtype=E.PROFILE_DTYPE).reshape(-1, np.asarray(rows).shape[-1]))
     n_nodes = len(node_off) - 1
@@ -59,7 +61,7 @@ def place(node_off, rows, occ, requests, policy=E.POLICY_FIRST_FIT, quirks=E.QUI
     requests = np.ascontiguousarray(requests, dtype=E.REQUEST_DTYPE)
     out = np.zeros(len(requests), dtype=E.RESULT_DTYPE)
     placed = lib().fa_place(n_nodes, _ptr(node_off), rows2.shape[0], rows2.shape[1], _ptr(rows2), _ptr(table), _ptr(dsize), _ptr(occ),
-                            lo, hi, quirks, policy, int(flagged), len(requests), _ptr(requests), _ptr(out))
+                            lo, hi, quirks, policy, int(flagged), len(requests), _ptr(requests), _ptr(out), int(memo))
     return out, occ, int(placed)
 
 
